@@ -1,6 +1,6 @@
 # Plain-make entry points for integrators who do not want to go through Python (python -m hotstuff_b200.build does the same).
 NVCC ?= nvcc
-NVCCFLAGS ?= -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared -diag-suppress 550
+NVCCFLAGS ?= -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared -diag-suppress 550
 CSRC := hotstuff_b200/csrc
 
 .PHONY: all lib oracle hostemu test-cpu clean

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""bench.py — Ed25519 verifies/s on B200 for BASELINE.json's config[1]:
-   "1xB200 batch verify of 2^20 signatures, 512 B msgs" (per GPU; weak scaling across ranks).
+"""bench.py — Ed25519 verifies/s on H100 for BASELINE.json's config[1]:
+   "1xH100 batch verify of 2^20 signatures, 512 B msgs" (per GPU; weak scaling across ranks).
 
 A step = one pass of the hot path over one batch: for every record i,
     d_i = Digest(msg_i) = SHA-512(msg_i)[..32]                (mempool/src/processor.rs:30, messages.rs digests)
@@ -12,6 +12,8 @@ for N > 1 by the all-gather of the per-rank accept bitmaps.
   e2e   : the same metric through the host-pointer C-ABI call (pinned host buffers, H2D + D2H inside the timed region)
   --impl reference : the CPU path (oracle = restatement of the reference's dalek path; no Rust toolchain here) on all
                      host cores over a bounded sample of the same workload.
+  --dump-outputs DIR : after the timed steps, write what the last timed step returned to its caller as DIR/<name>.npy
+                     (float32; inputs are seeded, so two builds can be compared output for output).
 """
 import argparse
 import ctypes
@@ -34,6 +36,23 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 ALGO_BYTES_VERIFY = 128.125   # SURVEY §8(d): 64 B sig + 32 B pk + 32 B digest in, 1 bit out
 ALGO_BYTES_DIGEST = 512 + 32  # bytes hashed + digest out
+HBM_PEAK_GBS = 3350.0         # H100 SXM data sheet (700 W part); a denominator, not a measured rate
+DUMP_DIGEST_ROWS = 1 << 16    # digests written by --dump-outputs: a fixed, seeded sample of rows (8 MB as float32)
+
+
+def dump_outputs(out_dir, verdicts, digests=None, **extra):
+    """Write the arrays a caller of the timed path receives as float32 .npy files: one verdict per record (1 = accept) and,
+    for the Digest + verify path, the digests of a fixed seeded sample of DUMP_DIGEST_ROWS records (rows in digest_rows)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"verdicts": np.asarray(verdicts, dtype=np.float32)}
+    if digests is not None:
+        rows = np.arange(len(digests)) if len(digests) <= DUMP_DIGEST_ROWS else \
+            np.sort(np.random.default_rng(0).choice(len(digests), DUMP_DIGEST_ROWS, replace=False))
+        arrays["digest_rows"] = rows.astype(np.float64)
+        arrays["digests"] = np.asarray(digests)[rows].astype(np.float32)
+    arrays.update({k: np.asarray(v, dtype=np.float32) for k, v in extra.items()})
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------ input synthesis
@@ -178,6 +197,8 @@ def run_reference(args):
         dt, ok = cpu_reference_step(oracle, inp, 0, sample, cores)
         times.append(dt)
         assert int(ok.sum()) == sample - int(inp["corrupted"].sum())
+    if args.dump_outputs and args.steps:
+        dump_outputs(args.dump_outputs, ok)
     total = float(np.sum(times))
     v = sample * args.steps / total
     line = {
@@ -196,7 +217,7 @@ def workload_config(args, world):
     coll = "none (1 rank)" if world == 1 else ("fused peer-store all-gather in the finish kernel (NVLink P2P)" if args.collective == "peer" else "ncclAllGather")
     return {"collective": coll,"workload": "config[1]: 2^20 signatures per GPU, 512 B msgs: Digest(msg)=SHA-512[..32] on GPU then verify_strict over the digest",
             "records_per_gpu": args.n, "msg_len": args.msg_len, "distinct_keys": args.keys, "corrupted_frac": 0.01,
-            "key_mode": args.key_mode, "l2": "inputs (%.0f MB/GPU) larger than the 126 MB L2" % (args.n * (96 + args.msg_len) / 1e6),
+            "key_mode": args.key_mode, "l2": "inputs (%.0f MB/GPU) larger than the H100's 50 MB L2" % (args.n * (96 + args.msg_len) / 1e6),
             "parallelism": "records sharded across %d rank(s); all-gather of accept bitmaps" % world}
 
 
@@ -227,7 +248,7 @@ def make_qc_inputs(eng, n_val, n_qc, votes_per_qc, seed):
     return dict(pks=pks, pre=pre, digests=digests, vidx=vidx, midx=midx, sig=sig, corrupted=corrupted)
 
 
-def qc_leg(eng, torch, dist, dev, rank, world, committee, qcs, votes_per_qc, steps, warmup, collective):
+def qc_leg(eng, torch, dist, dev, rank, world, committee, qcs, votes_per_qc, steps, warmup, collective, dump_dir=None):
     """One QC-verification measurement: QC::digest for every certificate, the verify_batch condition per vote of THIS rank's
     shard, all-gather of the vote bitmaps (fused peer stores or ncclAllGather), per-QC AND over the gathered bitmap — every rank
     ends with every QC verdict.  STRONG scaling: the total number of votes is fixed.  Engine kernels only inside the timed region."""
@@ -293,11 +314,14 @@ def qc_leg(eng, torch, dist, dev, rank, world, committee, qcs, votes_per_qc, ste
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        step()
+        full = step()
     if deferred:
         eng.results_wait()
     e1.record()
     torch.cuda.synchronize()
+    if dump_dir and rank == 0 and steps:
+        dump_outputs(dump_dir, np.unpackbits(full.cpu().numpy().view(np.uint8), bitorder="little")[:n],
+                     qc_verdicts=np.unpackbits(d_qc.cpu().numpy().view(np.uint8), bitorder="little")[:qcs])
     if world > 1:
         dist.barrier()
     t = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
@@ -328,7 +352,8 @@ def run_qc(args):
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
-    r = qc_leg(eng, torch, dist, dev, rank, world, args.committee, args.qcs, args.votes_per_qc, args.steps, args.warmup, args.collective)
+    r = qc_leg(eng, torch, dist, dev, rank, world, args.committee, args.qcs, args.votes_per_qc, args.steps, args.warmup, args.collective,
+               dump_dir=args.dump_outputs)
     clocks = sampler.stop() if rank == 0 else None
     if rank == 0:
         print(json.dumps({
@@ -372,15 +397,17 @@ def main():
                     help="N > 1: how the per-rank accept bitmaps reach every rank.  peer: the verify finish kernel stores its words straight "
                          "into every rank's buffer over NVLink (fused all-gather, hs_peer_*).  nccl: ncclAllGather after the kernel (baseline)")
     ap.add_argument("--base-window", type=int, default=24,
-                    help="comb window of the base-point table in bits: 24 = the library default (11 windows, 8.9 GB).  26 (10 windows, 32 GB: one "
-                         "mixed addition fewer) was measured on B200 and buys nothing — 2.361 vs 2.371 ms for the main kernel — because the gathers "
-                         "from the 3.6x larger table miss L2/TLB more often (profiles/r02_bench_base_window_26.json)")
+                    help="comb window of the base-point table in bits: 24 = the library default (11 windows, 8.9 GB); 26 = 10 windows, 32 GB, "
+                         "one mixed addition fewer per verify")
     ap.add_argument("--key-window", type=int, default=0, help="force the per-key comb window (bits); 0 = widest that fits the table budget. "
                     "E.g. --base-window 20 --key-window 12 is the ~18 GB configuration for a shared GPU (DESIGN.md §5c)")
     ap.add_argument("--no-strong", action="store_true", help="skip the strong-scaling QC leg (BASELINE config[3]) reported next to the headline")
     ap.add_argument("--committee", type=int, default=1000)
     ap.add_argument("--qcs", type=int, default=10000)
     ap.add_argument("--votes-per-qc", type=int, default=100)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (per-record verdicts; digests of a seeded "
+                         "sample of records; per-QC verdicts for --workload qc) as DIR/<name>.npy in float32")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
@@ -485,6 +512,10 @@ def main():
         step_resident()
         ev[s_ + 1].record()
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0 and args.steps:
+        bm = ((pag.full if pag is not None else d_all) if world > 1 else d_bitmap).cpu().numpy().reshape(world, words)
+        dump_outputs(args.dump_outputs, np.unpackbits(bm.view(np.uint8), axis=1, bitorder="little")[:, :n].reshape(-1),
+                     digests=d_digest.cpu().numpy())
     if world > 1:
         dist.barrier()
     total_ms = ev[0].elapsed_time(ev[-1])
@@ -580,35 +611,17 @@ def main():
     # total, sharded across the ranks, every rank ends with every verdict).  Re-registers the committee (untimed, epoch set-up).
     strong = None
     if not args.no_strong:
-        strong = qc_leg(eng, torch, dist, dev, rank, world, 10000, 150, 6667, max(5, args.steps), args.warmup, args.collective)
+        strong = qc_leg(eng, torch, dist, dev, rank, world, 10000, 150, 6667, args.steps, args.warmup, args.collective)
     if rank == 0:
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = HBM_PEAK_GBS
         dom_ms = main_ms if main_ms and main_ms > 0 else kern_ms
         achieved = ALGO_BYTES_VERIFY * n / (dom_ms * 1e-3) / 1e9
-        # dram__bytes_read + dram__bytes_write and pipe utilisation of the kernels from THIS round's ncu --set full capture at the same
-        # 2^20 records per launch (tools/run_all_gpu.sh -> tools/ncu_traffic.py -> profiles/r02_traffic.json); not measured in this run
-        tr = {}
-        try:
-            tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        except Exception:
-            pass
-        traffic = (tr.get("k_verify_main_bytes_per_record", 0) * n) or None
         wa, wb = head_wa, head_wb
 
         def ndig(w):
             r = 253 % w
             return (253 + w - 1) // w + (1 if r in (0, w - 1) else 0)
         adds = (ndig(wa) if wa else 64) + ndig(wb)
-        # SASS counts of the hot loop (tools/sass_hist.py, profiles/r02_sass_mainloop.txt): per mixed addition 336 IMAD.WIDE.U32.X (carry-in form,
-        # measured issue rate 32 lanes/clk/SM) + 171 IMAD.WIDE.U32 (54 lanes/clk/SM) + 129 other FMA-pipe instructions (64 lanes/clk/SM)
-        fma_clk_per_add = 336 / 32.0 + 171 / 54.0 + 129 / 64.0          # SM-clocks of FMA-pipe time per mixed addition per lane-group
-        sm_clk = (clocks or {}).get("sm_mhz") or 1965.0
-        fma_floor_ms = adds * fma_clk_per_add * n / (148 * sm_clk * 1e6) * 1e3 if wa else None
         fe_muls = adds * 7 + 10 + (0 if wa else 252 * (3 + 4 * 0.7) + 64 * 8 + 254 * 0.7 + 20)
         line = {
             "metric": "Ed25519 verifies/s", "value": value, "unit": "verifies/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -617,26 +630,16 @@ def main():
             "e2e": e2e,
             "roofline": {"bound": "hbm", "kernel": "k_verify_main<committee>" if args.key_mode != "generic" else "k_verify_main<generic>", "cached_keys": head_cached,
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback 6650 GB/s", "traffic": traffic,
-                         "traffic_source": "profiles/r02_traffic.json: ncu --set full of this round at 2^20 records per launch (dram__bytes_read.sum + dram__bytes_write.sum); "
-                                           "table gathers, by design ~41x the algorithmic bytes" if traffic else None,
+                         "peak_source": "H100 SXM data sheet (3.35 TB/s HBM3), not a measured rate",
                          "kernel_ms": dom_ms, "kernel_ms_covers": "k_verify_main<committee> alone (CUDA events recorded by the engine on its launch stream)" if main_ms else
                                                                     "lookup + main + finish kernels of one verify pass",
                          "verify_pass_ms": kern_ms, "verify_pass_covers": "lookup + main + finish kernels over 2^20 resident records",
                          "digest_kernel_ms": dig_ms, "digest_algorithmic_GBps": ALGO_BYTES_DIGEST * n / (dig_ms * 1e-3) / 1e9,
-                         "digest_alu_pipe_pct_ncu": tr.get("k_digest32_fixed_alu_pipe_pct"),
                          "algorithmic_bytes_per_verify": ALGO_BYTES_VERIFY,
                          "note": "integer-ALU bound path: 128 B of compulsory I/O per ~30 k INT32 instructions; the HBM fraction is necessarily << 1 (SURVEY §0.7): "
                                  "see alu_roofline for the resource that binds"},
             "alu_roofline": {"bound": "integer-multiply (FMA-heavy / IMAD) pipe — the resource that actually binds k_verify_main",
-                             "fmaheavy_pipe_busy_pct_ncu": tr.get("k_verify_main_fmaheavy_pipe_pct"),
-                             "fmaheavy_source": "profiles/r02_traffic.json (sm__pipe_fmaheavy_cycles_active, this round's ncu capture at 2^20 records)",
-                             "issue_floor_ms": fma_floor_ms, "issue_floor_frac": (fma_floor_ms / dom_ms) if fma_floor_ms else None,
-                             "issue_floor_basis": "mixed additions x (336 IMAD.WIDE.X / 32 + 171 IMAD.WIDE / 54 + 129 other / 64 lanes per clk per SM): raw issue "
-                                                  "rates from profiles/r01_pipes.txt and r01_widex.txt, instruction counts from profiles/r02_sass_mainloop.txt",
-                             "field_muls_per_s": fe_muls * n / (dom_ms * 1e-3), "field_mul_microbench_peak": 1.138e11,
-                             "field_mul_frac": fe_muls * n / (dom_ms * 1e-3) / 1.138e11,
-                             "field_mul_peak_source": "best fe_mul rate of tools/microbench/febench.cu on this GPU (profiles/r01_febench.txt, 2,048 threads/SM)",
+                             "field_muls_per_s": fe_muls * n / (dom_ms * 1e-3),
                              "field_muls_per_verify": fe_muls, "mixed_additions_per_verify": adds, "window_bits": {"key": wa, "base": wb}},
             "cpu_baseline": cpu,
             "strong_scaling_config3": strong,

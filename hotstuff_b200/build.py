@@ -1,6 +1,6 @@
 """Build the native pieces in-tree (nvcc for the CUDA engine, gcc for the test-only oracle / host emulation).
 
-The product is `hotstuff_b200/libhs_crypto.so` (sm_100a only).  The oracle and the host-emulation library are test
+The product is `hotstuff_b200/libhs_crypto.so` (sm_90a only).  The oracle and the host-emulation library are test
 infrastructure: building them here is not using them.
 """
 import os
@@ -14,7 +14,7 @@ LIB = os.path.join(PKG, "libhs_crypto.so")
 ORACLE_LIB = os.path.join(ROOT, "oracle", "libhs_oracle.so")
 HOSTEMU_LIB = os.path.join(ROOT, "tests", "hostemu", "libhs_hostemu.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-shared", "-diag-suppress", "550"]
 
 

@@ -1,9 +1,9 @@
-// fe.cuh — GF(2^255-19) arithmetic for the sm_100a Ed25519 engine.
+// fe.cuh — GF(2^255-19) arithmetic for the sm_90a Ed25519 engine.
 //
 // Representation: 8 saturated 32-bit limbs, little-endian, value anywhere in [0, 2^256) and only
-// meaningful mod p = 2^255-19 (2^256 = 38 mod p).  This is NOT dalek's 5x51 / 10x25.5 layout: on B200 one
-// IMAD.WIDE.U32.X does a 32x32->64 multiply-accumulate with carry-in/out at ~52 lanes/clk/SM, so a
-// saturated-limb schoolbook product costs 64 of them and no separate carry handling (fe_asm.cuh), versus
+// meaningful mod p = 2^255-19 (2^256 = 38 mod p).  This is NOT dalek's 5x51 / 10x25.5 layout: one
+// IMAD.WIDE.U32.X does a 32x32->64 multiply-accumulate with carry-in/out,
+// so a saturated-limb schoolbook product costs 64 of them and no separate carry handling (fe_asm.cuh), versus
 // 100 for the 10-limb layout.  Replaces the field arithmetic that the reference reaches through
 // ed25519-dalek (crypto/Cargo.toml:10) on every Signature::verify (crypto/src/lib.rs:200-204).
 //

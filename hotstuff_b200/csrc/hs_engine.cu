@@ -1,7 +1,7 @@
-// hs_engine.cu — sm_100a kernels + the C ABI of include/hs_crypto.h.
+// hs_engine.cu — sm_90a kernels + the C ABI of include/hs_crypto.h.
 //
 // Hot path of asonnino/hotstuff's crypto crate (crypto/src/lib.rs:200-219 + the SHA-512 Digest call sites) rebuilt for
-// B200.  No CPU path: if CUDA fails the call returns an error and the caller must reject.
+// H100.  No CPU path: if CUDA fails the call returns an error and the caller must reject.
 //
 // Throughput pipeline of one verify call (any n):
 //   k_key_lookup      pk bytes -> committee index through a device hash table; misses -> compacted list
@@ -755,6 +755,7 @@ struct dev_buf {
 };
 struct hs_ctx {
   int device = 0;
+  unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
   cudaStream_t stream = nullptr, stream2 = nullptr, stream_side = nullptr;
   cudaEvent_t ev[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_side[2] = {nullptr, nullptr};
   ge_niels *d_btable = nullptr;
@@ -1066,7 +1067,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
       HS_CUDA(c, cudaEventRecord(c->ev_side[0], stream));
       HS_CUDA(c, cudaStreamWaitEvent(c->stream_side, c->ev_side[0], 0));
       unsigned grid = blocks_for(n, 32);
-      if (grid > 148u * 8u) grid = 148u * 8u;
+      if (grid > c->n_sms * 8u) grid = c->n_sms * 8u;
       k_verify_main<false><<<grid, 32, 0, c->stream_side>>>(L, 0, c->d_miss_count, (const uint32_t *)c->miss.p, c->d_btable, C, O, c->cp);
       c->launches++;
       HS_CUDA(c, cudaGetLastError());
@@ -1204,6 +1205,9 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
   if (!c) return HS_ERR_NOMEM;
   c->device = device;
   cudaError_t e = cudaSetDevice(device);
+  int sms = 0;
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  c->n_sms = (unsigned)sms;
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking);
   if (e == cudaSuccess) {
@@ -1361,8 +1365,8 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
   // host-side hash table (hashing only; first occurrence of a duplicated key wins)
   uint32_t cap = 16;
   std::vector<uint32_t> slots;
-  // widest per-key window whose tables fit in the budget: ~62 % of the device by default (B200: 16 bits up to ~2.2 k keys,
-  // 15 up to ~4.2 k, 14 up to ~7.6 k, 12 up to ~26 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device
+  // widest per-key window whose tables fit in the budget: ~62 % of the device by default (80 GB H100: 16 bits up to
+  // ~1 k keys, 15 up to ~1.8 k, 14 up to ~3.3 k, 13 up to ~6.3 k, 12 up to ~11 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device
   size_t free_b = 0, total_b = 0;
   HS_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
   size_t budget = total_b / 100 * 62;
@@ -1388,7 +1392,7 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
     if (!dup) slots[h] = (uint32_t)i;
   }
   int wa = 8;
-  for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8}) {  // 17 bits: 15 windows (94 MB per key: committees up to ~1,200 keys); 18 would still need 15
+  for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8}) {  // 17 bits: 15 windows (94 MB per key: committees up to ~500 keys on 80 GB); 18 would still need 15
     if (c->wa_forced && w != c->wa_forced) continue;
     wa = w;
     if (capk * comb_table_entries(w) * sizeof(ge_niels) <= budget) break;
@@ -1558,8 +1562,8 @@ int hs_verify_msgs_dev(hs_ctx *c, const void *d_sig, const void *d_pk, const voi
     return fail(c, HS_ERR_ARG, "hs_verify_msgs_dev: bad argument");
   if (n == 0) return HS_OK;
   HS_CUDA(c, cudaSetDevice(c->device));
-  // Digest(msg_i) in its own kernel: fusing it into k_verify_main was measured SLOWER on B200 (4.53 vs 4.13 ms per 2^20: the
-  // SHA phase then runs at the curve kernel's 128-register occupancy and the two phases do not overlap across pipes in practice).
+  // Digest(msg_i) in its own kernel: fused into k_verify_main, the SHA phase would run at the curve kernel's 128-register
+  // occupancy, and the two phases do not overlap across pipes in practice.
   HS_TRY(launch_digest_fixed(c, (const uint8_t *)d_msgs, msg_len, n, (uint32_t *)d_digests, (cudaStream_t)stream));
   in_layout L{(const uint8_t *)d_sig, 64, (const uint8_t *)d_pk, 32, (const uint32_t *)d_vidx, (const uint8_t *)d_digests, 32, nullptr, nullptr, 32, 0};
   return run_verify(c, L, n, mode, (uint32_t *)d_bitmap, (cudaStream_t)stream, d_vidx != nullptr);
@@ -2033,9 +2037,8 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  size_t CH = 1u << 17;  // records per chunk (multiple of 32).  Measured on B200 (512 B messages, 0.3 % unknown keys): 2^15 -> 2.9e7/s, 2^16 -> 4.5e7,
-                         // 2^17 -> 7.4e7, 2^18 -> 7.5e7 verifies/s end to end: every chunk with an unknown key waits ~0.84 ms for the generic pass,
-                         // so chunks must be long enough for the PCIe copy of the next chunk to cover it
+  size_t CH = 1u << 17;  // records per chunk (multiple of 32): every chunk with an unknown key waits for the single-warp latency of the
+                         // generic pass, so chunks must be long enough for the PCIe copy of the next chunk to cover it
   if (const char *e = getenv("HS_CHUNK_RECORDS")) {
     size_t v = strtoull(e, nullptr, 10);
     if (v >= 1024) CH = v & ~(size_t)31;

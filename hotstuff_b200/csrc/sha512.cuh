@@ -32,10 +32,9 @@ HS_HD uint64_t rotr64(uint64_t x, int n) { return (x >> n) | (x << (64 - n)); }
 // Ch / Maj one LOP3 per half, and the halves are packed with mov.b64 (free: a register pair) so that ptxas still sees 64-bit
 // adds and merges them into three-input IADD3 / IADD3.X pairs.  Per round: 24 SHF + 12 LOP3 + 12 add = 48 instructions
 // (r1 code, left to the compiler from uint64_t expressions: 67, with shifts split into IMAD.SHL + SHF + extra LOP3).
-// Experiment HS_SHA_FMA_ADD moves half of every 64-bit add to the FMA pipe (x + y = mad.wide(x_lo, 1, y) + (x_hi << 32)): Digest 1.52 vs
-// 0.99 ms.  Rotations on the FMA pipe (x * 2^(32-n) as IMAD.WIDE yields both shifted halves; 24 SHF -> 24 IMAD.WIDE + 8 LOP3 per round:
-// ALU instructions 46 -> 36 per round) were also measured SLOWER: 1.16 ms for the two big sigmas, 1.25 ms for all four
-// (profiles/r02_variants_sha_imad_rotations_NOT_KEPT.txt).  The kernel stays on the ALU pipe, at 94 % of its issue rate.
+// Experiment HS_SHA_FMA_ADD moves half of every 64-bit add to the FMA pipe (x + y = mad.wide(x_lo, 1, y) + (x_hi << 32)).
+// It and rotations on the FMA pipe (x * 2^(32-n) as IMAD.WIDE yields both shifted halves; 24 SHF -> 24 IMAD.WIDE + 8 LOP3 per round:
+// ALU instructions 46 -> 36 per round) were slower where they were measured; the kernel stays on the ALU pipe.
 #if defined(__CUDA_ARCH__)
 __device__ __forceinline__ uint64_t sha_pack(uint32_t lo, uint32_t hi) {
   uint64_t r;

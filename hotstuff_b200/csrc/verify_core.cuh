@@ -12,10 +12,10 @@
 //   small    = R or A is one of the 8 torsion points
 //   strict   = eq and not small
 //
-// Scalar multiplication layout (B200-first, not dalek's vartime NAF — see DESIGN.md):
+// Scalar multiplication layout (table gathers instead of doublings, not dalek's vartime NAF — see DESIGN.md):
 //   [S]B      : signed radix-2^w comb over a precomputed table of j * 2^(w i) * B, affine-Niels entries (96 B); no
-//               doublings.  w is chosen per context: 24 by default (11 windows, 8.8 GB of the 180 GB of HBM).
-//   [k](-A)   : committee key -> the same comb over that validator's own table (w = 16 / 14 / 12 by committee size);
+//               doublings.  w is chosen per context: 24 by default (11 windows, 8.9 GB of the H100's 80 GB of HBM).
+//   [k](-A)   : committee key -> the same comb over that validator's own table (w = 17 .. 8 by committee size);
 //               generic key   -> radix-2^4 signed fixed window, 8-entry per-thread table, 252 doublings + 64 additions.
 //   Every lane executes the same operation sequence (identity entry for digit 0), so warps never diverge.
 #pragma once
@@ -256,7 +256,7 @@ HS_HD void ge_scalarmult_window4(ge_ext &acc, const ge_ext &P, const uint32_t (&
   for (int i = 0; i < 64; i++) {
     if (i != 0) {
       // ONE copy of the doubling in the instruction stream (the 4x unrolled form made this loop body 5.2 k instructions and the
-      // kernel's top stall "no instruction": profiles/r02_ncu_generic_before.txt); T is only needed after the last of the four
+      // kernel's top stall "no instruction"); T is only needed after the last of the four
 #if defined(__CUDA_ARCH__)
 #pragma unroll 1
 #endif

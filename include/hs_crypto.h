@@ -1,5 +1,5 @@
 /*
- * hs_crypto.h — C ABI of the B200 batch Ed25519 verification / SHA-512 digest engine.
+ * hs_crypto.h — C ABI of the H100 batch Ed25519 verification / SHA-512 digest engine.
  *
  * This is the drop-in boundary for ONE path of asonnino/hotstuff: the `crypto` crate's verify / verify_batch /
  * Digest surface.  The reference has no FFI today (it calls ed25519-dalek directly, crypto/Cargo.toml:10); each

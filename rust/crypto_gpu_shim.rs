@@ -5,9 +5,9 @@
 //
 // What it adds over a bare FFI pass-through:
 //   * CPU/GPU cut-over (SURVEY §8f.2): a lone signature or a single large Digest stays on the reference's own dalek / sha2 path;
-//     the GPU takes every call with >= GPU_MIN_SIGS signatures and every multi-message digest.  Thresholds come from
-//     tools/replay_config5 on B200 (profiles/r02_replay_config5.json): 1 verify 72 us GPU vs ~62 us one CPU core; 3 votes
-//     72 us GPU vs ~185 us CPU; one 15 kB batch digest 327 us GPU vs ~40 us CPU.
+//     the GPU takes every call with >= GPU_MIN_SIGS signatures and every multi-message digest.  One verify costs the
+//     GPU about what one CPU core needs (a square-root chain in a lone warp), a few votes are already cheaper on the GPU, and one
+//     large digest is a sequential SHA-512 chain that a CPU core runs faster; tools/replay_config5 measures the three calls.
 //   * every status code is propagated: a failed registration or engine call is an Err / a rejected message, never an accept.
 //   * batch front ends for the consensus call sites: many QCs (view-change burst), TC votes, and whole bincode frames
 //     (ingest_frames + verify_ingested: the receiver path of consensus.rs:138 without building the message structs first).

@@ -27,11 +27,11 @@ def test_library_builds_and_exports_every_declared_symbol():
     _lib.load()
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     from hotstuff_b200 import build
     import subprocess
     out = subprocess.run(["cuobjdump", "--list-elf", build.build_engine()], capture_output=True, text=True).stdout
-    assert "sm_100a" in out and "sm_90" not in out and "sm_80" not in out
+    assert "sm_90a" in out and "sm_100" not in out and "sm_80" not in out
 
 
 def test_no_cpu_fallback_without_gpu():

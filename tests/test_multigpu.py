@@ -1,5 +1,5 @@
 """2-GPU check of the fused peer-store all-gather (include/hs_crypto.h hs_peer_*): each rank verifies its shard on its own
-B200 and the finish kernel writes the bitmap words into BOTH ranks' buffers over NVLink; both ranks must end up with the
+GPU and the finish kernel writes the bitmap words into BOTH ranks' buffers over NVLink; both ranks must end up with the
 oracle's full bitmap.  Skipped on boxes with fewer than 2 GPUs (the driver's single-GPU run); the ncclAllGather baseline and
 the sharding arithmetic are covered by tests/test_distributed.py on CPU (gloo)."""
 import os

@@ -1,11 +1,10 @@
 #!/usr/bin/env python3
-"""EXPERIMENT (measured, NOT kept — profiles/r02_latency_microbench.txt).  Generate tools/experiments/fe10.cuh: GF(2^255-19) multiply / square on TEN unsaturated limbs (26/25 bits alternating) — the
+"""EXPERIMENT (not kept: slower per dependent squaring than the saturated multiplier, tools/microbench/latency.cu).  Generate tools/experiments/fe10.cuh: GF(2^255-19) multiply / square on TEN unsaturated limbs (26/25 bits alternating) — the
 LATENCY representation used by the one-warp-per-signature path (k_verify_small).
 
 Why a second representation: the saturated 8 x 32 multiplier (fe_asm.cuh) is the throughput choice (72 wide multiplies instead of
-100) but every one of its instructions hangs on the carry flag of the previous one — measured on B200, ONE dependent fe_sqr takes
-369 cycles and fe_mul 519 (tools/microbench/latency.cu), so the 252-squaring square-root chain of a point decompression costs 56 us
-for a lone warp.  With 25.5-bit limbs the 100 (55) partial products are independent 64-bit multiply-accumulates (no carries until one
+100) but every one of its instructions hangs on the carry flag of the previous one, so ONE dependent fe_sqr takes hundreds of cycles
+(tools/microbench/latency.cu) and the 252-squaring square-root chain of a point decompression dominates the latency of a lone warp.  With 25.5-bit limbs the 100 (55) partial products are independent 64-bit multiply-accumulates (no carries until one
 short interleaved pass at the end), which a single warp can issue back to back.
 
 Every formula is generated from the rule  f_i g_j -> h_((i+j) mod 10), x19 if i+j >= 10, x2 if i and j are both odd,

@@ -1,12 +1,11 @@
 #!/usr/bin/env python3
-"""Generate the inline-PTX field multiplication / squaring for GF(2^255-19) on sm_100a.
+"""Generate the inline-PTX field multiplication / squaring for GF(2^255-19) on sm_90a.
 
 Representation: 8 saturated 32-bit limbs, value in [0, 2^256), congruent mod p = 2^255-19
 (2^256 = 38 mod p).  The schoolbook products are laid out as `mad.lo.cc.u32` / `madc.hi.cc.u32`
 pairs on two interleaved accumulator arrays (even / odd columns) so that ptxas fuses every pair into a
-single `IMAD.WIDE.U32.X Rd, Pc, Ra, Rb, Rd, Pc` (64-bit multiply-accumulate with carry-in/out) — measured
-on B200 at ~52 lane-ops/clk/SM, i.e. one SASS instruction per 32x32 partial product and no separate
-carry handling (tools/microbench/pipes.cu, profiles/r01_pipes.txt).
+single `IMAD.WIDE.U32.X Rd, Pc, Ra, Rb, Rd, Pc` (64-bit multiply-accumulate with carry-in/out), i.e. one
+SASS instruction per 32x32 partial product and no separate carry handling (issue rates: tools/microbench/pipes.cu).
 
 The generator builds an abstract instruction list, *simulates it in Python against big-integer
 arithmetic* (random + all-ones + edge inputs) and only then emits PTX, so a lost carry cannot reach the GPU.
@@ -583,7 +582,7 @@ def count(pr):
 
 if __name__ == "__main__":
     m, s = gen_mul(), gen_sqr(split=os.environ.get('HS_SQR_SPLIT', '1') == '1')
-    mk = gen_mul_karatsuba()   # experiment (measured slower on B200: profiles/r02_variants_karatsuba_NOT_KEPT.txt); emitted only on request
+    mk = gen_mul_karatsuba()   # experiment (the three short products triple the carry materialisations); emitted only on request
     check(mk, False)
     check(m, False)
     check(s, True)

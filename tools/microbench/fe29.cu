@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #include "../../hotstuff_b200/csrc/fe.cuh"
 #define ITERS 2048
 #define M29 0x1fffffffu
@@ -83,7 +84,7 @@ __global__ void __launch_bounds__(256) k(uint32_t *out, uint32_t seed) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = acc;
 }
 template <int KIND> void run(const char *name, int bps, double ops_per_iter) {
-  uint32_t *out; int blocks = 148 * bps, threads = 256;
+  uint32_t *out; int blocks = dev_sms() * bps, threads = 256;
   cudaMalloc(&out, blocks * threads * 4);
   k<KIND><<<blocks, threads>>>(out, 12345); cudaDeviceSynchronize();
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

@@ -5,10 +5,11 @@
 //   fold       V_j = col_j + 38 col_(j+8)   (2^256 = 38 mod p), three 32-bit words per lane
 //   carries    R_j = w0_j + w1_(j-1) + w2_(j-2) via shuffles (wrapping x38 at lane 0), then a shuffle ripple until no lane carries
 // Reports throughput (all SMs busy) and lone-warp latency for both designs, after checking the cooperative product against fe_mul.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/microbench/fe_warp tools/microbench/fe_warp.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/microbench/fe_warp tools/microbench/fe_warp.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #include "../../hotstuff_b200/csrc/fe.cuh"
 
 __device__ __forceinline__ uint32_t coop_mul(uint32_t a, uint32_t b) {
@@ -98,14 +99,14 @@ __global__ void k_check(uint32_t *bad, uint32_t seed) {
 }
 int main() {
   uint32_t *out, *bad; unsigned long long *cyc;
-  cudaMalloc(&out, 148 * 8 * 256 * 4); cudaMalloc(&bad, 4); cudaMalloc(&cyc, 8); cudaMemset(bad, 0, 4);
+  cudaMalloc(&out, (size_t)dev_sms() * 8 * 256 * 4); cudaMalloc(&bad, 4); cudaMalloc(&cyc, 8); cudaMemset(bad, 0, 4);
   k_check<<<64, 256>>>(bad, 12345u); k_check<<<64, 256>>>(bad, 777u);
   uint32_t hbad = 1; cudaMemcpy(&hbad, bad, 4, cudaMemcpyDeviceToHost);
   printf("cooperative product vs fe_mul: %u mismatching groups of %d\n", hbad, 2 * 64 * 256);
   const int iters = 2000;
   for (int kind = 0; kind < 2; kind++)
     for (int bps : {2, 4, 8}) {
-      const int blocks = 148 * bps;
+      const int blocks = dev_sms() * bps;
       cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
       if (kind == 0) k_tput<0><<<blocks, 256>>>(out, 10, 5); else k_tput<1><<<blocks, 256>>>(out, 10, 5);
       cudaDeviceSynchronize();

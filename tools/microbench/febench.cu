@@ -2,6 +2,7 @@
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #include "../../hotstuff_b200/csrc/fe.cuh"
 #define ITERS 2048
 template <int KIND>
@@ -24,15 +25,15 @@ __global__ void __launch_bounds__(256) k(uint32_t *out, unsigned long long *cyc,
   if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
 }
 template <int KIND> void run(const char *name, int threads, int bps) {
-  uint32_t *out; unsigned long long *cyc; int blocks = 148 * bps;
+  uint32_t *out; unsigned long long *cyc; int blocks = dev_sms() * bps;
   cudaMalloc(&out, blocks * threads * 4); cudaMalloc(&cyc, blocks * 8);
   k<KIND><<<blocks, threads>>>(out, cyc, 12345); cudaDeviceSynchronize();
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaEventRecord(e0); k<KIND><<<blocks, threads>>>(out, cyc, 12345); cudaEventRecord(e1); cudaDeviceSynchronize();
   float ms; cudaEventElapsedTime(&ms, e0, e1);
   double ops = (double)ITERS * 4.0 * threads * blocks;
-  printf("%-8s threads/SM=%4d  %.3f ms  %.3e ops/s  (%.1f clk/SM per lane-op @1.9GHz)\n", name, threads * bps, ms, ops / (ms * 1e-3),
-         1.9e9 * 148 / (ops / (ms * 1e-3)));
+  printf("%-8s threads/SM=%4d  %.3f ms  %.3e ops/s  (%.1f clk/SM per lane-op at the maximum SM clock)\n", name, threads * bps, ms, ops / (ms * 1e-3),
+         dev_clock_hz() * blocks / bps / (ops / (ms * 1e-3)));
   cudaFree(out); cudaFree(cyc);
 }
 int main() {

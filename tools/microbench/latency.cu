@@ -1,9 +1,10 @@
 // Single-warp LATENCY of the building blocks of the latency path (k_verify_small / k_digest32_long): cycles for one warp alone on
 // an SM.  Answers "where do the 70 us of a single verify go" and sizes the warp-cooperative alternatives.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/microbench/latency tools/microbench/latency.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/microbench/latency tools/microbench/latency.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #include "../../hotstuff_b200/csrc/verify_core.cuh"
 #include "../experiments/fe10.cuh"   // ten-limb latency experiment (not part of the product)
 
@@ -84,7 +85,7 @@ int main() {
                            "(convert)", "256 dependent fe10_sqr", "256 dependent fe10_mul", "pow (p-5)/8 on ten limbs"};
   for (int rep = 0; rep < 2; rep++) { k_lat<<<1, 32>>>(out, cyc, 77 + rep); cudaDeviceSynchronize(); }
   cudaMemcpy(h, cyc, 88, cudaMemcpyDeviceToHost);
-  for (int i = 0; i < 11; i++) printf("%-32s %8llu cycles  (%.2f us at 1.965 GHz)%s\n", names[i], h[i], h[i] / 1965.0, i < 2 ? "  [per op: /256]" : "");
+  for (int i = 0; i < 11; i++) printf("%-32s %8llu cycles  (%.2f us at the maximum SM clock)%s\n", names[i], h[i], h[i] / (dev_clock_hz() * 1e-6), i < 2 ? "  [per op: /256]" : "");
   for (int rep = 0; rep < 2; rep++) { k_sha_chain<<<1, 32>>>((uint64_t *)out, cyc, kw); cudaDeviceSynchronize(); }
   cudaMemcpy(h, cyc, 8, cudaMemcpyDeviceToHost);
   printf("%-32s %8llu cycles per block (%.1f per round)\n", "sha512 rounds from K+W table", h[0], h[0] / 80.0);

@@ -1,9 +1,10 @@
-// Instruction-pipe throughput microbenchmark for sm_100a (B200).
+// Instruction-pipe throughput microbenchmark for sm_90a (H100).
 // Measures lane-ops / clk / SM for the integer instructions the field arithmetic is built from,
 // so the limb representation is chosen from measurement, not folklore.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 
 #define ITERS 4096
 #define CK(x) do { cudaError_t e=(x); if(e!=cudaSuccess){printf("CUDA error %s at %d\n",cudaGetErrorString(e),__LINE__); return 1;} } while(0)
@@ -95,7 +96,7 @@ __global__ void __launch_bounds__(1024, 1) k(uint32_t *out, unsigned long long *
 template <int KIND>
 int run(const char *name, int threads) {
   uint32_t *out; unsigned long long *cyc;
-  int blocks = 148;
+  int blocks = dev_sms();
   CK(cudaMalloc(&out, blocks * 1024 * 4)); CK(cudaMalloc(&cyc, blocks * 8));
   k<KIND><<<blocks, threads>>>(out, cyc, 12345);  // warm-up
   CK(cudaDeviceSynchronize());
@@ -105,7 +106,7 @@ int run(const char *name, int threads) {
   cudaEventRecord(e1);
   CK(cudaDeviceSynchronize());
   float ms; cudaEventElapsedTime(&ms, e0, e1);
-  unsigned long long h[148]; CK(cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost));
+  unsigned long long h[1024]; CK(cudaMemcpy(h, cyc, blocks * sizeof(h[0]), cudaMemcpyDeviceToHost));
   double avg = 0; for (int i = 0; i < blocks; i++) avg += (double)h[i]; avg /= blocks;
   double ops = (double)ITERS * 8.0 * threads;  // PTX-level ops per SM (block)
   printf("%-34s threads=%4d  cycles=%9.0f  ptx-ops/clk/SM=%7.2f  ms=%.3f  (eff MHz=%.0f)\n", name, threads, avg, ops / avg, ms, avg / ms / 1e3);

@@ -3,6 +3,7 @@
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #define ITERS 4096
 template <int KIND>
 __global__ void __launch_bounds__(512, 1) k(uint32_t *out, uint32_t seed) {
@@ -32,13 +33,13 @@ __global__ void __launch_bounds__(512, 1) k(uint32_t *out, uint32_t seed) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = l0 ^ h0 ^ l1 ^ h1 ^ l2 ^ h2 ^ l3 ^ h3 ^ l4 ^ h4 ^ l5 ^ h5 ^ l6 ^ h6 ^ l7 ^ h7 ^ c0 ^ c1 ^ c2 ^ c3 ^ c4 ^ c5 ^ c6 ^ c7;
 }
 template <int KIND> void run(const char *name) {
-  uint32_t *out; int blocks = 148 * 2, threads = 512;
+  uint32_t *out; int blocks = dev_sms() * 2, threads = 512;
   cudaMalloc(&out, blocks * threads * 4);
   k<KIND><<<blocks, threads>>>(out, 12345); cudaDeviceSynchronize();
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaEventRecord(e0); k<KIND><<<blocks, threads>>>(out, 12345); cudaEventRecord(e1); cudaDeviceSynchronize();
   float ms; cudaEventElapsedTime(&ms, e0, e1);
-  printf("%-44s %.3f ms  wide-mads/clk/SM = %.2f (assuming 1.9 GHz)\n", name, ms, (double)ITERS * 8.0 * threads * 2 / (ms * 1e-3 * 1.9e9));
+  printf("%-44s %.3f ms  wide-mads/clk/SM = %.2f (at the maximum SM clock)\n", name, ms, (double)ITERS * 8.0 * threads * 2 / (ms * 1e-3 * dev_clock_hz()));
   cudaFree(out);
 }
 int main() { run<0>("carry-out wide mad + IADD3.X counter"); run<1>("plain wide mad"); run<2>(".X chains (4 long)"); }

@@ -2,6 +2,7 @@
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "device.cuh"
 #define ITERS 4096
 template <int KIND>
 __global__ void __launch_bounds__(512, 1) k(uint32_t *out, unsigned long long *cyc, uint32_t seed) {
@@ -54,15 +55,15 @@ __global__ void __launch_bounds__(512, 1) k(uint32_t *out, unsigned long long *c
   if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
 }
 template <int KIND> void run(const char *name, int bps) {
-  uint32_t *out; unsigned long long *cyc; int blocks = 148 * bps, threads = 512;
+  uint32_t *out; unsigned long long *cyc; int blocks = dev_sms() * bps, threads = 512;
   cudaMalloc(&out, blocks * threads * 4); cudaMalloc(&cyc, blocks * 8);
   k<KIND><<<blocks, threads>>>(out, cyc, 12345); cudaDeviceSynchronize();
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaEventRecord(e0); k<KIND><<<blocks, threads>>>(out, cyc, 12345); cudaEventRecord(e1); cudaDeviceSynchronize();
   float ms; cudaEventElapsedTime(&ms, e0, e1);
-  unsigned long long h[148]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
-  double avg = 0; for (int i = 0; i < 148; i++) avg += (double)h[i]; avg /= 148;
-  printf("%-36s %.3f ms  wide-mads/clk/SM = %.2f\n", name, ms, (double)ITERS * 8.0 * threads * bps / (ms * 1e-3 * 1.9e9) );
+  unsigned long long h[1024]; cudaMemcpy(h, cyc, dev_sms() * sizeof(h[0]), cudaMemcpyDeviceToHost);
+  double avg = 0; for (int i = 0; i < dev_sms(); i++) avg += (double)h[i]; avg /= dev_sms();
+  printf("%-36s %.3f ms  wide-mads/clk/SM = %.2f\n", name, ms, (double)ITERS * 8.0 * threads * bps / (ms * 1e-3 * dev_clock_hz()) );
   cudaFree(out); cudaFree(cyc);
 }
 int main() { run<0>("IMAD.WIDE.U32.X chains", 1); run<1>("IMAD.WIDE.U32 plain", 1); run<2>("plain + 2 IMAD per 8", 1); run<3>("plain + 8 IADD3.X per 8", 1);

@@ -5,7 +5,7 @@
     python tools/sass_hist.py lib.so k_digest32 --loops                        # also every loop body, innermost first
 
 Pipes (B300_MICROARCH.md "Pipe rates"): IMAD* / FFMA on the fma pipe, IADD3 / LOP3 / SHF / PRMT / ISETP / SEL on the alu pipe.
-Used for the before/after evidence under profiles/ (VERDICT r1 "Next round" #4).
+Used for before/after comparisons of the hot loop.
 """
 import collections
 import re

@@ -20,13 +20,17 @@
 // Front ends: QC / TC / Timeout / Block groups with on-GPU digests and per-certificate AND; load-generation keygen / signer.
 #include <cuda_runtime.h>
 #include <atomic>
+#include <condition_variable>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <mutex>
 #include <new>
 #include <string>
+#include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/hs_crypto.h"
@@ -271,13 +275,19 @@ __global__ void __launch_bounds__(HS_THREADS, COMMITTEE ? HS_MAIN_MINBLOCKS : HS
 // throughput kernels above would spend 5 launches and ~28 serial mixed additions + an inversion on it (r1: 155 us per
 // verify).  Here ONE launch of 64-thread blocks does a signature per block: warp 0 hashes, recodes, lets lane j fetch the table
 // entry of digit j and sums the lanes' points with a shuffle tree (5 levels); warp 1 decompresses R meanwhile; thread 0
-// compares projectively.  Inputs and verdicts live in mapped pinned host memory (no copy calls); the last block raises a
-// completion word the host polls.  Registered / cached keys only (the host resolves key bytes to indices first).
+// compares projectively.  Inputs and verdicts live in mapped pinned host memory (no copy calls).  Registered / cached keys
+// only (the host resolves key bytes to indices first).
+// One launch serves many REQUESTS (the verify queue coalesces concurrent small verifies): block b takes ring record
+// (base + b) & mask, the record names its request slot and the request's record count, and the block that finishes a
+// request's last record raises THAT request's completion word — a submitter sees its verdicts when its own records are
+// done, not when the launch is.  The synchronous latency path is the one-request case (slot 0, base 0).
 struct small_rec {
   uint8_t sig[64];
   uint8_t msg[32];
   uint32_t vidx;
-  uint32_t pad[7];
+  uint32_t req;    // request slot: index of the request's counter and completion word
+  uint32_t req_n;  // records of that request
+  uint32_t pad[5];
 };
 static_assert(sizeof(small_rec) == 128, "small_rec is 128 bytes");
 #define HS_SMALL_MAX 64
@@ -285,14 +295,15 @@ __device__ __forceinline__ void fe_shfl_down(fe &r, const fe &a, int delta) {
 #pragma unroll
   for (int i = 0; i < 8; i++) r.v[i] = __shfl_down_sync(0xffffffffu, a.v[i], delta);
 }
-__global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict__ in, uint32_t n, const ge_niels *__restrict__ btable,
-                                                      committee_tables C, const comb_params cp, uint8_t *out_flags, uint32_t *counter,
+__global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict__ ring, uint32_t base, uint32_t mask, const ge_niels *__restrict__ btable,
+                                                      committee_tables C, const comb_params cp, uint8_t *out_flags, uint32_t *counters,
                                                       volatile uint32_t *done, uint32_t seq) {
   __shared__ int32_t dig[HS_MAX_DIGITS];
   __shared__ fe sh_acc[3], sh_r[2];
   __shared__ uint32_t sh_meta[2];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const small_rec *rec = in + blockIdx.x;
+  const uint32_t slot = (base + blockIdx.x) & mask;
+  const small_rec *rec = ring + slot;
   uint32_t R[8], S[8];
   load32(R, rec->sig);
   load32(S, rec->sig + 32);
@@ -358,12 +369,13 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
     const uint32_t eq = sh_meta[0] & ge_proj_equals_affine(sh_acc[0], sh_acc[1], sh_acc[2], sh_r[0], sh_r[1]);
     if (eq) fl |= HS_F_EQ;
     if (eq && !(fl & HS_F_SMALL)) fl |= HS_F_STRICT;
-    out_flags[blockIdx.x] = (uint8_t)fl;
+    out_flags[slot] = (uint8_t)fl;
     __threadfence_system();
-    if (atomicAdd(counter, 1u) == n - 1) {
-      *counter = 0;
+    const uint32_t req = rec->req;
+    if (atomicAdd(counters + req, 1u) == rec->req_n - 1) {
+      counters[req] = 0;
       __threadfence_system();
-      *done = seq;
+      done[req] = seq;
     }
   }
 }
@@ -820,6 +832,8 @@ struct hs_ctx {
   std::mutex mu;
   std::mutex err_mu;                  // guards err only: fail() is also reached from argument checks taken before `mu`
   std::string err = "ok";
+  std::mutex queues_mu;               // guards queues only (hs_ctx_destroy tears them down without holding `mu`)
+  std::vector<hs_queue *> queues;     // verify queues attached to this context
 };
 
 static int fail(hs_ctx *c, int code, const char *what, cudaError_t e = cudaSuccess) {
@@ -1123,7 +1137,8 @@ static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
   return HS_NO_KEY;
 }
 static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->d_atables; }
-// c->h_small_in[0 .. n) is filled: one launch, then poll the completion word the last block writes to mapped host memory.
+// c->h_small_in[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
+// mapped host memory.
 static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, uint8_t *out_flags_or_null) {
   small_rec *d_in = nullptr;
   uint8_t *d_out = nullptr;
@@ -1131,10 +1146,14 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
   HS_CUDA(c, cudaHostGetDevicePointer(&d_in, c->h_small_in, 0));
   HS_CUDA(c, cudaHostGetDevicePointer(&d_out, c->h_small_out, 0));
   HS_CUDA(c, cudaHostGetDevicePointer(&d_done, c->h_small_done, 0));
+  for (size_t i = 0; i < n; i++) {
+    c->h_small_in[i].req = 0;
+    c->h_small_in[i].req_n = (uint32_t)n;
+  }
   const uint32_t seq = ++c->small_seq ? c->small_seq : ++c->small_seq;  // never 0
   committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
   if (c->ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_tables, 0));
-  k_verify_small<<<(unsigned)n, 64, 0, c->stream>>>(d_in, (uint32_t)n, c->d_btable, C, c->cp, d_out, c->d_small_counter, d_done, seq);
+  k_verify_small<<<(unsigned)n, 64, 0, c->stream>>>(d_in, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, d_out, c->d_small_counter, d_done, seq);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   volatile uint32_t *done = c->h_small_done;
@@ -1162,6 +1181,254 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
     if (fl & want) out_bitmap[i >> 5] |= 1u << (i & 31);
   }
   return HS_OK;
+}
+
+// ---- verify queue (hs_queue_*): continuous batching of concurrent small verifies onto k_verify_small
+// Ring positions grow without bound (slot = position & mask): [head, launched) is dispatched, [launched, tail) pending.  A
+// request's slot is the ring slot of its first record; it names the request's counter, completion word and bookkeeping.
+// The dispatcher thread is the only one that launches, watches completions, runs the slow path and advances `head`.
+#define HS_QUEUE_DEFAULT_RECORDS 4096u
+#define HS_QUEUE_MAX_RECORDS (1u << 20)
+#define HS_QUEUE_MAX_INFLIGHT 2
+struct hs_queue {
+  hs_ctx *c = nullptr;
+  uint32_t cap = 0, mask = 0;
+  small_rec *h_ring = nullptr, *d_ring = nullptr;  // mapped pinned: sig | msg | vidx | req | req_n per record
+  uint8_t *h_flags = nullptr, *d_flags = nullptr;  // mapped pinned: verdict flags per record
+  uint32_t *h_done = nullptr, *d_done = nullptr;   // mapped pinned: completion word per request slot (= launch sequence number)
+  uint32_t *d_counters = nullptr;                  // device: records finished per request slot
+  std::vector<uint8_t> pk;                         // key bytes per record (host only: resolved to a table index at dispatch)
+  cudaStream_t stream = nullptr;
+  cudaEvent_t ev_last = nullptr;                   // recorded after every launch: the ring is freed only after it
+  struct req {
+    size_t ticket;
+    uint32_t n, mode;
+    hs_queue_cb *cb;
+    void *user;
+    uint32_t seq;   // launch that verifies it (0: slow path)
+    bool finished;
+  };
+  std::vector<req> reqs;  // by request slot
+  struct result {
+    bool done;
+    int status;
+    uint32_t n;
+    uint32_t bits[(HS_SMALL_MAX + 31) / 32];
+  };
+  std::unordered_map<size_t, result> results;  // tickets without a callback, until poll / wait reads them
+  struct launch {
+    uint32_t seq;
+    uint64_t lo, hi;  // ring positions it covers
+  };
+  std::deque<launch> inflight;
+  uint64_t head = 0, launched = 0, tail = 0;
+  size_t next_ticket = 1;
+  uint32_t seq = 0;
+  uint64_t spins = 0;
+  bool stop = false;
+  std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
+  std::condition_variable cv_work, cv_done;
+  std::thread th;
+};
+
+struct queue_completion {
+  hs_queue_cb *cb;
+  void *user;
+  size_t ticket;
+  int status;
+  uint32_t bits[(HS_SMALL_MAX + 31) / 32];
+};
+// Releases the ring space of the finished requests at the head — but never inside the range of a launch still in flight: its
+// blocks may still read those records (slow-path requests between two device requests ride along in the launch).
+static void queue_release_locked(hs_queue *q) {
+  const uint64_t limit = q->inflight.empty() ? q->launched : q->inflight.front().lo;
+  while (q->head < limit && q->reqs[q->head & q->mask].finished) {
+    hs_queue::req &h = q->reqs[q->head & q->mask];
+    h.finished = false;
+    q->head += h.n;
+  }
+}
+// Marks the request at ring position p finished (under q->mu): a polled ticket's result is parked, a callback is returned to be
+// fired after the lock is released.
+static void queue_finish_locked(hs_queue *q, uint64_t p, int status, const uint32_t *bits, std::vector<queue_completion> &fire) {
+  hs_queue::req &r = q->reqs[p & q->mask];
+  r.finished = true;
+  if (r.cb) {
+    queue_completion f{r.cb, r.user, r.ticket, status, {0, 0}};
+    if (status == HS_OK) memcpy(f.bits, bits, sizeof(f.bits));
+    fire.push_back(f);
+  } else {
+    hs_queue::result &res = q->results[r.ticket];
+    res.done = true;
+    res.status = status;
+    memset(res.bits, 0, sizeof(res.bits));
+    if (status == HS_OK) memcpy(res.bits, bits, sizeof(res.bits));
+    q->cv_done.notify_all();
+  }
+  queue_release_locked(q);
+}
+static void queue_fire(std::vector<queue_completion> &fire) {
+  for (queue_completion &f : fire) f.cb(f.user, f.ticket, f.status, f.bits);
+  fire.clear();
+}
+
+// Dispatches the pending requests [lo, hi): under c->mu, keys are resolved through the host mirror of the key hash table and
+// ONE launch covers every request whose keys are all registered; the others then run through hs_verify_rec128 on this thread.
+static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
+  hs_ctx *c = q->c;
+  std::vector<uint64_t> slow;
+  std::vector<queue_completion> fire;
+  uint64_t dlo = hi, dhi = lo;  // ring positions of the first / past the last request on the device path
+  uint32_t seq = 0;
+  cudaError_t e = cudaSuccess;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables && c->small_enabled;
+    for (uint64_t p = lo; p < hi;) {
+      hs_queue::req &r = q->reqs[p & q->mask];
+      bool all = committee;
+      for (uint32_t i = 0; i < r.n; i++) {
+        small_rec &s = q->h_ring[(p + i) & q->mask];
+        s.vidx = all ? host_key_lookup(c, q->pk.data() + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
+        s.req = (uint32_t)(p & q->mask);
+        s.req_n = r.n;
+        if (s.vidx == HS_NO_KEY) all = false;
+      }
+      if (all) {
+        if (dlo == hi) dlo = p;
+        dhi = p + r.n;
+        r.seq = 1;  // the launch's number is set below
+      } else {
+        r.seq = 0;
+        slow.push_back(p);
+      }
+      p += r.n;
+    }
+    if (dlo < dhi) {  // slow-path requests between dlo and dhi ride along (rejected: no table index); their verdicts are ignored
+      seq = ++q->seq ? q->seq : ++q->seq;  // never 0
+      for (uint64_t p = dlo; p < dhi; p += q->reqs[p & q->mask].n)
+        if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = seq;
+      committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
+      k_verify_small<<<(unsigned)(dhi - dlo), 64, 0, q->stream>>>(q->d_ring, (uint32_t)(dlo & q->mask), q->mask, c->d_btable, C, c->cp, q->d_flags,
+                                                                   q->d_counters, q->d_done, seq);
+      c->launches++;
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaEventRecord(q->ev_last, q->stream);
+      if (e != cudaSuccess) fail(c, HS_ERR_CUDA, "verify queue launch", e);
+    }
+  }
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (dlo < dhi) {
+      if (e == cudaSuccess) {
+        q->inflight.push_back(hs_queue::launch{seq, dlo, dhi});
+      } else {
+        for (uint64_t p = dlo; p < dhi; p += q->reqs[p & q->mask].n)
+          if (q->reqs[p & q->mask].seq) queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
+      }
+    }
+  }
+  queue_fire(fire);
+  // the slow path: exactly the synchronous entry point (key cache, generic kernels), on this thread
+  std::vector<hs_rec128> recs;
+  for (uint64_t p : slow) {
+    const hs_queue::req &r = q->reqs[p & q->mask];
+    recs.resize(r.n);
+    for (uint32_t i = 0; i < r.n; i++) {
+      const uint32_t s = (uint32_t)((p + i) & q->mask);
+      memcpy(recs[i].sig, q->h_ring[s].sig, 64);
+      memcpy(recs[i].pk, q->pk.data() + 32 * (size_t)s, 32);
+      memcpy(recs[i].msg, q->h_ring[s].msg, 32);
+    }
+    uint32_t bits[(HS_SMALL_MAX + 31) / 32] = {0, 0};
+    const int rc = hs_verify_rec128(c, recs.data(), r.n, r.mode, bits);
+    {
+      std::lock_guard<std::mutex> g(q->mu);
+      queue_finish_locked(q, p, rc == HS_OK ? HS_OK : HS_ERR_CUDA, bits, fire);
+    }
+    queue_fire(fire);
+  }
+}
+
+// One pass over the launches in flight: a device request whose completion word carries its launch's number is finished with
+// its verdicts (the flags -> bits mapping of run_small).  A launch is retired once every request in its range — riders
+// included — has its word.  Every 4,096 passes the stream is queried: a CUDA error, or a drained stream with a word still
+// missing, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
+static void queue_watch(hs_queue *q) {
+  std::vector<queue_completion> fire;
+  cudaError_t qe = cudaErrorNotReady;
+  if ((++q->spins & 0xfff) == 0) qe = cudaStreamQuery(q->stream);  // queried BEFORE the words are read
+  if (qe != cudaSuccess && qe != cudaErrorNotReady) fail(q->c, HS_ERR_CUDA, "verify queue kernel", qe);
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    for (size_t k = 0; k < q->inflight.size(); k++) {
+      const hs_queue::launch L = q->inflight[k];
+      bool open = false;
+      for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n) {
+        hs_queue::req &r = q->reqs[p & q->mask];
+        const bool mine = r.seq == L.seq && !r.finished;
+        if (((volatile uint32_t *)q->h_done)[p & q->mask] == L.seq) {
+          if (!mine) continue;
+          std::atomic_thread_fence(std::memory_order_acquire);
+          uint32_t bits[(HS_SMALL_MAX + 31) / 32] = {0, 0};
+          const uint32_t want = (r.mode == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
+          for (uint32_t i = 0; i < r.n; i++)
+            if (((volatile uint8_t *)q->h_flags)[(p + i) & q->mask] & want) bits[i >> 5] |= 1u << (i & 31);
+          queue_finish_locked(q, p, HS_OK, bits, fire);
+        } else if (qe == cudaErrorNotReady) {
+          open = true;
+        } else if (mine) {
+          if (qe == cudaSuccess) fail(q->c, HS_ERR_CUDA, "verify queue: k_verify_small did not complete");
+          queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
+        }
+      }
+      if (!open) {
+        q->inflight.erase(q->inflight.begin() + (long)k--);
+        queue_release_locked(q);
+      }
+    }
+  }
+  queue_fire(fire);
+}
+
+static void queue_main(hs_queue *q) {
+  cudaSetDevice(q->c->device);
+  std::unique_lock<std::mutex> lk(q->mu);
+  for (;;) {
+    if (q->launched < q->tail && q->inflight.size() < HS_QUEUE_MAX_INFLIGHT) {
+      const uint64_t lo = q->launched, hi = q->tail;  // everything pending
+      q->launched = hi;
+      lk.unlock();
+      queue_dispatch(q, lo, hi);
+      lk.lock();
+    } else if (!q->inflight.empty()) {
+      lk.unlock();
+      queue_watch(q);
+      lk.lock();
+    } else if (q->stop) {
+      break;
+    } else {
+      q->cv_work.wait(lk);
+    }
+  }
+}
+
+static void queue_free(hs_queue *q) {
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    q->stop = true;
+  }
+  q->cv_work.notify_all();
+  if (q->th.joinable()) q->th.join();  // the thread finishes every request first
+  cudaSetDevice(q->c->device);
+  if (q->ev_last) cudaEventSynchronize(q->ev_last);  // the last launch's blocks have exited before the ring goes
+  if (q->ev_last) cudaEventDestroy(q->ev_last);
+  if (q->stream) cudaStreamDestroy(q->stream);
+  if (q->h_ring) cudaFreeHost(q->h_ring);
+  if (q->h_flags) cudaFreeHost(q->h_flags);
+  if (q->h_done) cudaFreeHost(q->h_done);
+  cudaFree(q->d_counters);
+  delete q;
 }
 
 // Digest of n fixed-size messages: staged/coalesced kernel when every message starts 16-byte aligned and has at least one
@@ -1254,6 +1521,12 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
 
 void hs_ctx_destroy(hs_ctx *c) {
   if (!c) return;
+  std::vector<hs_queue *> qs;
+  {
+    std::lock_guard<std::mutex> g(c->queues_mu);
+    qs.swap(c->queues);
+  }
+  for (hs_queue *q : qs) queue_free(q);  // completes their requests (callbacks fire) and joins their threads
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   cudaFree(c->d_btable);
@@ -1355,6 +1628,8 @@ void hs_host_free(void *p) {
 // ---- committee registration
 static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, uint32_t *out_valid_bitmap) {
   HS_CUDA(c, cudaSetDevice(c->device));
+  // Drains every stream of the device, the verify queues' included: a queue enqueues a launch only while it holds c->mu, so
+  // nothing launched against the old tables survives this line, and later dispatches resolve keys against the new mirror.
   HS_CUDA(c, cudaDeviceSynchronize());
   cache_release(c);
   c->learn_pending = false;
@@ -1449,7 +1724,7 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
   std::lock_guard<std::mutex> g(c->mu);
   if (!c->explicit_committee) return fail(c, HS_ERR_ARG, "hs_committee_update: no committee registered");
   HS_CUDA(c, cudaSetDevice(c->device));
-  HS_CUDA(c, cudaDeviceSynchronize());  // epoch boundary: nothing of the old set may be in flight
+  HS_CUDA(c, cudaDeviceSynchronize());  // epoch boundary: nothing of the old set may be in flight (verify queue launches included)
   for (size_t i = 0; i < n_remove; i++)
     if (remove_idx[i] >= c->n_keys) return fail(c, HS_ERR_ARG, "hs_committee_update: remove index out of range");
   for (size_t i = 0; i < n_remove; i++) {
@@ -2082,6 +2357,116 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
     lo += cnt;
   }
   return finish_bitmap(c, n, out_bitmap);
+}
+
+// ---- verify queue
+int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
+  if (!c || !out || ring_records > HS_QUEUE_MAX_RECORDS) return fail(c, HS_ERR_ARG, "hs_queue_create: bad argument");
+  *out = nullptr;
+  uint32_t cap = HS_SMALL_MAX;  // a request of 64 records must fit
+  while (cap < (ring_records ? ring_records : HS_QUEUE_DEFAULT_RECORDS)) cap <<= 1;
+  HS_CUDA(c, cudaSetDevice(c->device));
+  hs_queue *q = new (std::nothrow) hs_queue();
+  if (!q) return fail(c, HS_ERR_NOMEM, "hs_queue_create: out of host memory");
+  q->c = c;
+  q->cap = cap;
+  q->mask = cap - 1;
+  q->pk.assign((size_t)cap * 32, 0);
+  q->reqs.assign(cap, hs_queue::req{});
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->stream, cudaStreamNonBlocking, hi);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->ev_last, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_ring, (size_t)cap * sizeof(small_rec), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_flags, cap, cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_done, (size_t)cap * 4, cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_counters, (size_t)cap * 4);
+  if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_ring, q->h_ring, 0);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_flags, q->h_flags, 0);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_done, q->h_done, 0);
+  if (e != cudaSuccess) {
+    queue_free(q);
+    return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
+  }
+  memset(q->h_done, 0, (size_t)cap * 4);
+  try {
+    q->th = std::thread(queue_main, q);
+  } catch (...) {
+    queue_free(q);
+    return fail(c, HS_ERR_NOMEM, "hs_queue_create: cannot start the dispatcher thread");
+  }
+  {
+    std::lock_guard<std::mutex> g(c->queues_mu);
+    c->queues.push_back(q);
+  }
+  *out = q;
+  return HS_OK;
+}
+
+int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !recs || n == 0 || n > HS_SMALL_MAX || mode > 1) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit: bad argument");
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit: queue is being destroyed");
+    if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
+    for (size_t i = 0; i < n; i++) {
+      const uint32_t s = (uint32_t)((q->tail + i) & q->mask);
+      memcpy(q->h_ring[s].sig, recs[i].sig, 64);
+      memcpy(q->h_ring[s].msg, recs[i].msg, 32);
+      memcpy(q->pk.data() + 32 * (size_t)s, recs[i].pk, 32);
+    }
+    const size_t ticket = q->next_ticket++;
+    q->reqs[q->tail & q->mask] = hs_queue::req{ticket, (uint32_t)n, mode, cb, user, 0, false};
+    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {0, 0}};
+    q->tail += n;
+    if (out_ticket) *out_ticket = ticket;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+
+int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap) {
+  if (!q || !done || !out_bitmap) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_poll: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  auto it = q->results.find(ticket);
+  if (it == q->results.end()) return fail(q->c, HS_ERR_ARG, "hs_queue_poll: unknown ticket (already read, or consumed by its callback)");
+  *done = it->second.done ? 1 : 0;
+  if (!it->second.done) return HS_OK;
+  const hs_queue::result r = it->second;
+  q->results.erase(it);
+  memcpy(out_bitmap, r.bits, 4 * (size_t)((r.n + 31) / 32));
+  return r.status;
+}
+
+int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap) {
+  if (!q || !out_bitmap) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_wait: bad argument");
+  std::unique_lock<std::mutex> lk(q->mu);
+  for (;;) {
+    auto it = q->results.find(ticket);  // looked up again after every wake-up: submissions may rehash the map
+    if (it == q->results.end()) return fail(q->c, HS_ERR_ARG, "hs_queue_wait: unknown ticket (already read, or consumed by its callback)");
+    if (it->second.done) {
+      const hs_queue::result r = it->second;
+      q->results.erase(it);
+      memcpy(out_bitmap, r.bits, 4 * (size_t)((r.n + 31) / 32));
+      return r.status;
+    }
+    q->cv_done.wait(lk);
+  }
+}
+
+void hs_queue_destroy(hs_queue *q) {
+  if (!q) return;
+  {
+    std::lock_guard<std::mutex> g(q->c->queues_mu);
+    auto &v = q->c->queues;
+    for (size_t i = 0; i < v.size(); i++)
+      if (v[i] == q) {
+        v.erase(v.begin() + (long)i);
+        break;
+      }
+  }
+  queue_free(q);
 }
 
 }  // extern "C"

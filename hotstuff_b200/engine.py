@@ -4,6 +4,7 @@ Host-side mirror of the reference interface lives in crypto.py; this module is t
 sites would use (QC/TC vote sets, mempool batch digests) plus device-resident entry points for the benchmark.
 """
 import ctypes
+import threading
 
 import numpy as np
 
@@ -46,11 +47,18 @@ class Engine:
         self.h = h
         self.device = int(device)
         self.n_keys = 0
+        self._queues = []
 
     def close(self):
+        for q in list(getattr(self, "_queues", [])):
+            q.close()
         if getattr(self, "h", None):
             self.lib.hs_ctx_destroy(self.h)
             self.h = None
+
+    def queue(self, ring_records=0):
+        """A VerifyQueue on this context (hs_queue_create): concurrent small verifies share latency-path launches."""
+        return VerifyQueue(self, ring_records)
 
     def __del__(self):
         try:
@@ -292,3 +300,94 @@ class Engine:
 
     def digest32_dev(self, d_data, d_off, d_out, n):
         self._check(self.lib.hs_digest32_dev(self.h, d_data.data_ptr(), d_off.data_ptr(), n, d_out.data_ptr(), self._stream()), "hs_digest32_dev")
+
+
+class VerifyQueue:
+    """hs_queue_* (include/hs_crypto.h): submit 1..64 records without blocking; a dispatcher thread coalesces whatever is
+    pending into one latency-path launch.  Verdicts equal Engine.verify_rec128 on the same records.  A ticket is read once:
+    by poll() / wait(), or by the callback given to submit() (called on the queue's thread as callback(ticket, status, bools);
+    status != 0 means engine failure: reject every signature)."""
+
+    def __init__(self, engine, ring_records=0):
+        self.engine = engine
+        self.lib = engine.lib
+        h = ctypes.c_void_p()
+        engine._check(self.lib.hs_queue_create(engine.h, int(ring_records), ctypes.byref(h)), "hs_queue_create")
+        self.h = h
+        self._lock = threading.Lock()
+        self._n = {}          # ticket -> records, for tickets read by poll / wait
+        self._callbacks = {}  # user id -> (callback, records)
+        self._next_id = 1
+        self._trampoline = _lib.QUEUE_CB(self._on_done)  # one C callback for the queue's lifetime
+        engine._queues.append(self)
+
+    def _on_done(self, user, ticket, status, bitmap):
+        with self._lock:
+            fn, n = self._callbacks.pop(user)
+        words = np.ctypeslib.as_array(bitmap, shape=((n + 31) // 32,)).copy()
+        fn(int(ticket), int(status), bitmap_to_bools(words, n))
+
+    def submit(self, recs, mode=MODE_STRICT, callback=None):
+        """recs: (n,128) uint8 [sig64|pk32|msg32], 1 <= n <= 64.  Returns the ticket, or None when the ring is full (retry later)."""
+        recs = _u8(recs, 128).reshape(-1, 128)
+        n = recs.shape[0]
+        t = ctypes.c_size_t(0)
+        if callback is None:
+            with self._lock:  # registered first: poll / wait from another thread may race the return
+                rc = self.lib.hs_queue_submit(self.h, _ptr(recs), n, mode, None, None, ctypes.byref(t))
+                if rc == 0:
+                    self._n[t.value] = n
+        else:
+            with self._lock:
+                uid = self._next_id
+                self._next_id += 1
+                self._callbacks[uid] = (callback, n)
+            rc = self.lib.hs_queue_submit(self.h, _ptr(recs), n, mode, ctypes.cast(self._trampoline, ctypes.c_void_p), uid, ctypes.byref(t))
+            if rc != 0:
+                with self._lock:
+                    self._callbacks.pop(uid, None)
+        if rc == 3:  # HS_ERR_NOMEM: back-pressure
+            return None
+        self.engine._check(rc, "hs_queue_submit")
+        return t.value
+
+    def _take(self, ticket, rc, words):
+        with self._lock:
+            n = self._n.pop(ticket, None)
+        self.engine._check(rc, "hs_queue ticket %d" % ticket)
+        return bitmap_to_bools(words, n)
+
+    def poll(self, ticket):
+        """None while the request is in flight, else its verdicts (bool[n]); consumes the ticket."""
+        done = ctypes.c_int(0)
+        words = np.zeros(2, dtype=np.uint32)
+        rc = self.lib.hs_queue_poll(self.h, int(ticket), ctypes.byref(done), _ptr(words))
+        if rc == 0 and not done.value:
+            return None
+        return self._take(ticket, rc, words)
+
+    def wait(self, ticket):
+        """Blocks until the request is done; returns its verdicts (bool[n]) and consumes the ticket."""
+        words = np.zeros(2, dtype=np.uint32)
+        rc = self.lib.hs_queue_wait(self.h, int(ticket), _ptr(words))
+        return self._take(ticket, rc, words)
+
+    def close(self):
+        """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""
+        if getattr(self, "h", None):
+            self.lib.hs_queue_destroy(self.h)
+            self.h = None
+            if self in self.engine._queues:
+                self.engine._queues.remove(self)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

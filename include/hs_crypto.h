@@ -176,6 +176,40 @@ int hs_set_table_budget(hs_ctx *ctx, size_t bytes);
 int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_t *sig /* n x 64 */, const uint32_t *msg_idx,
                         const uint8_t *digests /* n_msgs x 32 */, size_t n_msgs, size_t n, uint32_t mode, uint32_t *out_bitmap);
 
+/* ---- verify queue: concurrent small verifies share latency-path launches ------------------------------------------------
+ * The leader's Vote::verify per incoming vote (consensus/src/core.rs handle_vote), Timeout::verify during a view change and the
+ * Block author check arrive as many independent 1..64-signature requests from different tasks at once.  A queue takes them
+ * without blocking and a dispatcher thread gathers EVERYTHING pending into one launch of the latency kernel whenever fewer than
+ * two of its launches are in flight (continuous batching: no timers, no knobs).  Each request completes when its own records
+ * are done.
+ *   - hs_queue_submit copies the records into the queue's ring and returns at once: HS_ERR_NOMEM when the ring has no room for
+ *     n records (retry after some requests complete), HS_ERR_ARG for n = 0, n > 64 or a bad mode.  One request = one message's
+ *     signatures (a Vote, a Timeout / Block author, a small QC); larger sets belong to the batch entry points.
+ *   - Verdicts equal hs_verify_rec128(ctx, recs, n, mode, ..) on the same records, bit for bit.
+ *   - Device path: only when a committee is registered (hs_committee_register) and every key of the request is in it.  Any
+ *     other request is run by the queue's thread through hs_verify_rec128 itself (key cache / generic kernels): correct, but
+ *     the slow path.
+ *   - Consumption: with a callback, it runs exactly once on the queue's thread (status HS_OK, or HS_ERR_CUDA = reject every
+ *     signature of the request; bitmap = n verdict bits, valid during the call) and the ticket is released when it returns.
+ *     Without one, the result is kept until ONE hs_queue_poll that reports done, or one hs_queue_wait; both return the
+ *     request's status.  Reading a ticket twice, or reading a callback ticket, is HS_ERR_ARG.
+ *   - hs_committee_register / hs_committee_update / hs_ctx_destroy drain the queue's launches before they touch the tables; a
+ *     request submitted after one of them returns is judged against the new committee.
+ *   - hs_queue_destroy completes every request in flight (callbacks fire) and joins the thread; hs_ctx_destroy destroys the
+ *     queues still attached to the context.  hs_kernel_launches counts the queue's launches. */
+typedef struct hs_queue hs_queue;
+/* Completion callback (a function type: parameters are `hs_queue_cb *`; the parentheses keep the name from reading as a function). */
+typedef void(hs_queue_cb)(void *user, size_t ticket, int status, const uint32_t *bitmap);
+/* ring_records: capacity of the record ring (0 = 4,096; rounded up to a power of two, at least 64). */
+int hs_queue_create(hs_ctx *ctx, size_t ring_records, hs_queue **out);
+/* n = 1..64 records, mode = HS_MODE_*; callback nullable; out_ticket nullable. */
+int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
+/* Non-blocking: *done = 0 (come back later) or 1 (out_bitmap holds the verdicts, ticket consumed, returns the request's status). */
+int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap);
+/* Blocks until the request is done; consumes the ticket and returns the request's status. */
+int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap);
+void hs_queue_destroy(hs_queue *q);
+
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */
 /* Replaces Sha512::digest(..)[..32] at mempool/src/processor.rs:30 and consensus/src/messages.rs:81,151,203,270,308. */
 int hs_digest32_batch(hs_ctx *ctx, const uint8_t *data, const uint64_t *off, size_t n, uint8_t *out /* n x 32 */);

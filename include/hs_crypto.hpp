@@ -8,7 +8,9 @@
 #include <array>
 #include <cstdint>
 #include <cstring>
+#include <future>
 #include <stdexcept>
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -40,6 +42,55 @@ class Engine {
 
  private:
   hs_ctx *ctx_ = nullptr;
+};
+
+// The verify queue's ring has no room for the request right now (HS_ERR_NOMEM): back-pressure, retry once requests complete.
+struct QueueFull : EngineError {
+  QueueFull() : EngineError("hs_queue_submit: the verify queue's ring is full") {}
+};
+
+// RAII handle on hs_queue_* (hs_crypto.h): many tasks submit small verifies (a Vote, a Timeout / Block author, a small QC) at
+// once and share latency-path launches.  Each future yields the request's verdicts, bit-identical to hs_verify_rec128, or throws
+// EngineError on an engine failure (reject every signature).  Destruction completes every request in flight.
+class VerifyQueue {
+ public:
+  explicit VerifyQueue(const Engine &e, size_t ring_records = 0) : e_(e) { e.check(hs_queue_create(e.raw(), ring_records, &q_), "hs_queue_create"); }
+  ~VerifyQueue() { hs_queue_destroy(q_); }
+  VerifyQueue(const VerifyQueue &) = delete;
+  VerifyQueue &operator=(const VerifyQueue &) = delete;
+
+  // 1..64 records, HS_MODE_*.  Throws QueueFull when the ring is full, EngineError on a bad argument.
+  std::future<std::vector<bool>> submit(const hs_rec128 *recs, size_t n, uint32_t mode = HS_MODE_STRICT) {
+    auto *p = new Pending{std::promise<std::vector<bool>>(), n};
+    std::future<std::vector<bool>> f = p->promise.get_future();
+    const int rc = hs_queue_submit(q_, recs, n, mode, &VerifyQueue::done, p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit");
+    }
+    return f;
+  }
+
+ private:
+  struct Pending {
+    std::promise<std::vector<bool>> promise;
+    size_t n;
+  };
+  // runs once per request on the queue's thread
+  static void done(void *user, size_t, int status, const uint32_t *bitmap) {
+    Pending *p = static_cast<Pending *>(user);
+    if (status == HS_OK) {
+      std::vector<bool> v(p->n);
+      for (size_t i = 0; i < p->n; i++) v[i] = (bitmap[i >> 5] >> (i & 31)) & 1u;
+      p->promise.set_value(std::move(v));
+    } else {
+      p->promise.set_exception(std::make_exception_ptr(EngineError("verify queue: engine failure (status " + std::to_string(status) + ")")));
+    }
+    delete p;
+  }
+  const Engine &e_;
+  hs_queue *q_ = nullptr;
 };
 
 struct Digest {  // crypto/src/lib.rs:22

@@ -14,6 +14,10 @@
 use std::os::raw::c_int;
 use std::sync::OnceLock;
 
+/// The verify queue (hs_queue_*): concurrent single-message verifies share latency-path launches (`queue::verify_queued`).
+#[path = "crypto_gpu_queue.rs"]
+pub mod queue;
+
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsVote   { pub pk: [u8; 32], pub sig: [u8; 64] }                     // QC.votes element, messages.rs:168

@@ -10,13 +10,21 @@
 // The CPU column times the oracle (the restatement of the reference's dalek path) on one core for the same calls:
 // it is the number the shim's CPU/GPU cut-over is chosen against.  This is a replay of the call pattern, NOT a fab run.
 //
-// build: g++ -O2 -std=c++17 tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
+// Leader vote burst (after the replay): the N - f Vote::verify calls of one round at the leader (N = 4, 100, 1,000), one
+// strict verify of a Digest over a 40-byte preimage per vote, 1 % of the votes corrupted, arriving at once from 16 native
+// threads (one per connection task).  Three arms: (a) the verify queue (hs_queue_submit + callback), (b) one synchronous
+// hs_verify_rec128(n = 1) per vote from the same 16 threads, (c) the CPU oracle verifying the votes serially on one core (what
+// Core does today).  Per-vote latency = burst start -> that vote's verdict; every verdict is checked against the oracle.
+//
+// build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
+#include <atomic>
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "hs_crypto.h"
@@ -40,6 +48,141 @@ struct series {
 static void emit(const char *name, series &g, series &c, bool last) {
   printf("\"%s\": {\"gpu_p50_us\": %.1f, \"gpu_p99_us\": %.1f, \"gpu_mean_us\": %.1f, \"cpu_oracle_1core_p50_us\": %.1f, \"calls\": %zu}%s", name, g.pct(0.5), g.pct(0.99),
          g.mean(), c.pct(0.5), g.v.size(), last ? "" : ", ");
+}
+
+// ---- leader vote burst
+struct burst_arm {
+  series total, vote;  // burst start -> last verdict; burst start -> each vote's verdict
+  uint64_t launches = 0;
+  int mismatches = 0;
+  void emit(const char *name, int bursts, bool last) {
+    printf("\"%s\": {\"burst_p50_us\": %.1f, \"burst_min_us\": %.1f, \"vote_p50_us\": %.1f, \"vote_p99_us\": %.1f, \"launches_per_burst\": %.1f, \"mismatches\": %d}%s", name,
+           total.pct(0.5), total.pct(0.0), vote.pct(0.5), vote.pct(0.99), (double)launches / bursts, mismatches, last ? "" : ", ");
+  }
+};
+struct burst_vote {
+  clk::time_point t0;
+  double *lat;
+  int *verdict;
+};
+static void on_vote(void *user, size_t, int status, const uint32_t *bitmap) {
+  burst_vote *v = (burst_vote *)user;
+  *v->lat = us_since(v->t0);
+  __atomic_store_n(v->verdict, status == HS_OK ? (int)(bitmap[0] & 1u) : -1, __ATOMIC_RELEASE);
+}
+// One committee size: `bursts` timed bursts (+3 warm-up) of N - f votes per arm.
+static int vote_burst(hs_ctx *ctx, int N, int bursts, bool last) {
+  const int f = (N - 1) / 3, nv = N - f, nth = 16;
+  std::vector<uint8_t> seeds((size_t)N * 32), pks((size_t)N * 32);
+  for (int i = 0; i < N; i++) {
+    for (int j = 0; j < 32; j++) seeds[(size_t)i * 32 + j] = (uint8_t)(29 * i + 5 * j + 7 + (i >> 8));
+    hso_keygen(&seeds[(size_t)i * 32], &pks[(size_t)i * 32]);
+  }
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, pks.data(), N, valid.data()) != HS_OK) return 1;
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 0, &q) != HS_OK) return 1;
+  burst_arm a, b, c;
+  std::vector<hs_rec128> recs(nv);
+  std::vector<int> want(nv), got(nv);
+  std::vector<double> lat(nv);
+  std::vector<burst_vote> bv(nv);
+  for (int r = 0; r < bursts + 3; r++) {
+    const bool timed = r >= 3;
+    uint8_t pre[40], d[32];  // Vote::digest = SHA-512(hash || round_le)[..32]
+    for (int j = 0; j < 32; j++) pre[j] = (uint8_t)(r * 13 + j);
+    const uint64_t round = 1000 + (uint64_t)r;
+    memcpy(pre + 32, &round, 8);
+    hso_digest32(pre, 40, d);
+    for (int i = 0; i < nv; i++) {
+      const int k = (i * 7 + r) % N;  // who voted varies per round
+      hso_sign(&seeds[(size_t)k * 32], d, 32, recs[i].sig);
+      memcpy(recs[i].pk, &pks[(size_t)k * 32], 32);
+      memcpy(recs[i].msg, d, 32);
+      if ((i * 37 + r * 11) % 100 == 0) recs[i].sig[(i + r) % 64] ^= 0x10;  // 1 % corrupted
+    }
+    // (c) CPU oracle, one core, serial: the reference verdicts
+    auto t0 = clk::now();
+    for (int i = 0; i < nv; i++) {
+      want[i] = hso_verify_strict(recs[i].sig, recs[i].pk, recs[i].msg, 32);
+      lat[i] = us_since(t0);
+    }
+    if (timed) {
+      c.total.v.push_back(us_since(t0));
+      c.vote.v.insert(c.vote.v.end(), lat.begin(), lat.end());
+    }
+    // (a) the queue: 16 threads submit their votes as one burst, verdicts arrive through the callback
+    std::atomic<int> go{0}, bad{0};
+    std::vector<std::thread> ts;
+    uint64_t l0 = hs_kernel_launches(ctx);
+    for (int t = 0; t < nth; t++)
+      ts.emplace_back([&, t] {
+        while (!go.load()) {
+        }
+        for (int i = t; i < nv; i += nth) {
+          bv[i] = burst_vote{t0, &lat[i], &got[i]};
+          int rc;
+          while ((rc = hs_queue_submit(q, &recs[i], 1, HS_MODE_STRICT, on_vote, &bv[i], nullptr)) == HS_ERR_NOMEM) std::this_thread::yield();
+          if (rc != HS_OK) bad++;
+        }
+      });
+    std::fill(got.begin(), got.end(), -2);
+    t0 = clk::now();  // the threads read it after `go`
+    go = 1;
+    for (auto &t : ts) t.join();
+    ts.clear();
+    for (int i = 0; i < nv; i++)
+      while (__atomic_load_n(&got[i], __ATOMIC_ACQUIRE) == -2) std::this_thread::yield();
+    const double ta = *std::max_element(lat.begin(), lat.end());
+    if (timed) {
+      a.total.v.push_back(ta);
+      a.vote.v.insert(a.vote.v.end(), lat.begin(), lat.end());
+      a.launches += hs_kernel_launches(ctx) - l0;
+      for (int i = 0; i < nv; i++) a.mismatches += got[i] != want[i];
+      a.mismatches += bad.load();
+    }
+    // (b) one synchronous hs_verify_rec128(n = 1) per vote from the same 16 threads
+    go = 0;
+    l0 = hs_kernel_launches(ctx);
+    for (int t = 0; t < nth; t++)
+      ts.emplace_back([&, t] {
+        while (!go.load()) {
+        }
+        for (int i = t; i < nv; i += nth) {
+          uint32_t bm = 0;
+          got[i] = hs_verify_rec128(ctx, &recs[i], 1, HS_MODE_STRICT, &bm) == HS_OK ? (int)(bm & 1u) : -1;
+          lat[i] = us_since(t0);
+        }
+      });
+    t0 = clk::now();
+    go = 1;
+    for (auto &t : ts) t.join();
+    if (timed) {
+      b.total.v.push_back(*std::max_element(lat.begin(), lat.end()));
+      b.vote.v.insert(b.vote.v.end(), lat.begin(), lat.end());
+      b.launches += hs_kernel_launches(ctx) - l0;
+      for (int i = 0; i < nv; i++) b.mismatches += got[i] != want[i];
+    }
+  }
+  hs_queue_destroy(q);
+  printf("\"committee_%d\": {\"votes\": %d, \"bursts\": %d, ", N, nv, bursts);
+  a.emit("queue", bursts, false);
+  b.emit("sync_verify_rec128_n1_16_threads", bursts, false);
+  c.emit("cpu_oracle_1core_serial", bursts, true);
+  printf("}%s", last ? "" : ", ");
+  return a.mismatches + b.mismatches;
+}
+static std::string gpu_identity() {  // name and enforced power limit, read in the same run
+  std::string s;
+  if (FILE *p = popen("nvidia-smi --query-gpu=name,power.limit --format=csv,noheader -i 0 2>/dev/null", "r")) {
+    char buf[256];
+    while (fgets(buf, sizeof(buf), p)) s += buf;
+    pclose(p);
+  }
+  while (!s.empty() && (s.back() == '\n' || s.back() == '\r')) s.pop_back();
+  for (char &ch : s)
+    if (ch == '"') ch = '\'';
+  return s.empty() ? "unknown" : s;
 }
 
 int main(int argc, char **argv) {
@@ -145,8 +288,13 @@ int main(int argc, char **argv) {
   emit("verify_batch_3", g_b3, c_b3, false);
   emit("verify_strict_3", g_v3, c_v3, true);
   printf("}, \"crypto_us_per_round_gpu\": %.1f, \"rounds_per_s_sustainable_single_caller_gpu\": %.0f, \"crypto_us_per_round_cpu_oracle_1core\": %.1f, "
-         "\"kernel_launches\": %llu}\n",
+         "\"kernel_launches\": %llu, ",
          per_round, 1e6 / per_round, per_round_cpu, (unsigned long long)hs_kernel_launches(ctx));
+  const int bursts = argc > 2 ? atoi(argv[2]) : 20;
+  printf("\"leader_vote_burst\": {\"gpu\": \"%s\", \"threads\": 16, ", gpu_identity().c_str());
+  int burst_bad = 0;
+  for (int N : {4, 100, 1000}) burst_bad += vote_burst(ctx, N, bursts, N == 1000);
+  printf("}}\n");
   hs_ctx_destroy(ctx);
-  return bad ? 9 : 0;
+  return (bad || burst_bad) ? 9 : 0;
 }

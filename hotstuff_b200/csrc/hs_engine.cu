@@ -1187,9 +1187,28 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
 // Ring positions grow without bound (slot = position & mask): [head, launched) is dispatched, [launched, tail) pending.  A
 // request's slot is the ring slot of its first record; it names the request's counter, completion word and bookkeeping.
 // The dispatcher thread is the only one that launches, watches completions, runs the slow path and advances `head`.
+// A request is either small (hs_queue_submit: 1..64 records, one mode) or a group (hs_queue_submit_group: one consensus
+// message's certificate, up to the ring's capacity, a mode per record); both take the same ring, launches and completion path.
 #define HS_QUEUE_DEFAULT_RECORDS 4096u
 #define HS_QUEUE_MAX_RECORDS (1u << 20)
 #define HS_QUEUE_MAX_INFLIGHT 2
+// A request's verdict bitmap: inline for <= 64 records (every small request), on the heap only for larger groups.
+struct queue_bits {
+  uint32_t inl[(HS_SMALL_MAX + 31) / 32] = {0, 0};
+  std::vector<uint32_t> big;
+  void set(uint32_t n, const uint32_t *src_or_null) {  // null: all zero (a failed request rejects every record)
+    const size_t w = (n + 31) / 32;
+    uint32_t *d = inl;
+    if (n > HS_SMALL_MAX) {
+      big.assign(w, 0);
+      d = big.data();
+    } else {
+      inl[0] = inl[1] = 0;
+    }
+    if (src_or_null) memcpy(d, src_or_null, 4 * w);
+  }
+  const uint32_t *data() const { return big.empty() ? inl : big.data(); }
+};
 struct hs_queue {
   hs_ctx *c = nullptr;
   uint32_t cap = 0, mask = 0;
@@ -1198,11 +1217,13 @@ struct hs_queue {
   uint32_t *h_done = nullptr, *d_done = nullptr;   // mapped pinned: completion word per request slot (= launch sequence number)
   uint32_t *d_counters = nullptr;                  // device: records finished per request slot
   std::vector<uint8_t> pk;                         // key bytes per record (host only: resolved to a table index at dispatch)
+  std::vector<uint8_t> modes;                      // HS_MODE_* per record (host only: picks the verdict flag of each record)
+  std::vector<uint32_t> wbits;                     // dispatcher thread only: verdict bitmap being assembled (cap bits)
   cudaStream_t stream = nullptr;
   cudaEvent_t ev_last = nullptr;                   // recorded after every launch: the ring is freed only after it
   struct req {
     size_t ticket;
-    uint32_t n, mode;
+    uint32_t n;
     hs_queue_cb *cb;
     void *user;
     uint32_t seq;   // launch that verifies it (0: slow path)
@@ -1213,7 +1234,7 @@ struct hs_queue {
     bool done;
     int status;
     uint32_t n;
-    uint32_t bits[(HS_SMALL_MAX + 31) / 32];
+    queue_bits bits;
   };
   std::unordered_map<size_t, result> results;  // tickets without a callback, until poll / wait reads them
   struct launch {
@@ -1236,7 +1257,7 @@ struct queue_completion {
   void *user;
   size_t ticket;
   int status;
-  uint32_t bits[(HS_SMALL_MAX + 31) / 32];
+  queue_bits bits;
 };
 // Releases the ring space of the finished requests at the head — but never inside the range of a launch still in flight: its
 // blocks may still read those records (slow-path requests between two device requests ride along in the launch).
@@ -1254,36 +1275,38 @@ static void queue_finish_locked(hs_queue *q, uint64_t p, int status, const uint3
   hs_queue::req &r = q->reqs[p & q->mask];
   r.finished = true;
   if (r.cb) {
-    queue_completion f{r.cb, r.user, r.ticket, status, {0, 0}};
-    if (status == HS_OK) memcpy(f.bits, bits, sizeof(f.bits));
-    fire.push_back(f);
+    fire.push_back(queue_completion{r.cb, r.user, r.ticket, status, {}});
+    fire.back().bits.set(r.n, status == HS_OK ? bits : nullptr);
   } else {
     hs_queue::result &res = q->results[r.ticket];
     res.done = true;
     res.status = status;
-    memset(res.bits, 0, sizeof(res.bits));
-    if (status == HS_OK) memcpy(res.bits, bits, sizeof(res.bits));
+    res.bits.set(r.n, status == HS_OK ? bits : nullptr);
     q->cv_done.notify_all();
   }
   queue_release_locked(q);
 }
 static void queue_fire(std::vector<queue_completion> &fire) {
-  for (queue_completion &f : fire) f.cb(f.user, f.ticket, f.status, f.bits);
+  for (queue_completion &f : fire) f.cb(f.user, f.ticket, f.status, f.bits.data());
   fire.clear();
 }
 
 // Dispatches the pending requests [lo, hi): under c->mu, keys are resolved through the host mirror of the key hash table and
-// ONE launch covers every request whose keys are all registered; the others then run through hs_verify_rec128 on this thread.
+// one launch covers every request whose keys are all registered; the others then run through hs_verify_rec128 on this thread.
+// A slow-path request of at most 64 records between two device requests rides along in the launch (its blocks find no table
+// index and reject; its verdicts are ignored).  A larger one would cost thousands of wasted blocks, so the launch is split
+// around it: one launch per run of device requests between such requests.
 static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   hs_ctx *c = q->c;
   std::vector<uint64_t> slow;
   std::vector<queue_completion> fire;
-  uint64_t dlo = hi, dhi = lo;  // ring positions of the first / past the last request on the device path
-  uint32_t seq = 0;
+  std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one
+  size_t n_ok = 0;                     // runs launched without a CUDA error (the first failure stops the rest)
   cudaError_t e = cudaSuccess;
   {
     std::lock_guard<std::mutex> g(c->mu);
     const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables && c->small_enabled;
+    uint64_t rlo = hi, rhi = lo;  // the run being gathered
     for (uint64_t p = lo; p < hi;) {
       hs_queue::req &r = q->reqs[p & q->mask];
       bool all = committee;
@@ -1295,56 +1318,81 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         if (s.vidx == HS_NO_KEY) all = false;
       }
       if (all) {
-        if (dlo == hi) dlo = p;
-        dhi = p + r.n;
+        if (rlo == hi) rlo = p;
+        rhi = p + r.n;
         r.seq = 1;  // the launch's number is set below
       } else {
         r.seq = 0;
         slow.push_back(p);
+        if (r.n > HS_SMALL_MAX && rlo < rhi) {  // no large riders: close the run before it
+          runs.push_back(hs_queue::launch{0, rlo, rhi});
+          rlo = hi;
+          rhi = lo;
+        }
       }
       p += r.n;
     }
-    if (dlo < dhi) {  // slow-path requests between dlo and dhi ride along (rejected: no table index); their verdicts are ignored
-      seq = ++q->seq ? q->seq : ++q->seq;  // never 0
-      for (uint64_t p = dlo; p < dhi; p += q->reqs[p & q->mask].n)
-        if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = seq;
-      committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
-      k_verify_small<<<(unsigned)(dhi - dlo), 64, 0, q->stream>>>(q->d_ring, (uint32_t)(dlo & q->mask), q->mask, c->d_btable, C, c->cp, q->d_flags,
-                                                                   q->d_counters, q->d_done, seq);
+    if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi});
+    committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
+    for (hs_queue::launch &L : runs) {
+      L.seq = ++q->seq ? q->seq : ++q->seq;  // never 0
+      for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
+        if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = L.seq;
+      k_verify_small<<<(unsigned)(L.hi - L.lo), 64, 0, q->stream>>>(q->d_ring, (uint32_t)(L.lo & q->mask), q->mask, c->d_btable, C, c->cp,
+                                                                     q->d_flags, q->d_counters, q->d_done, L.seq);
       c->launches++;
       e = cudaGetLastError();
       if (e == cudaSuccess) e = cudaEventRecord(q->ev_last, q->stream);
-      if (e != cudaSuccess) fail(c, HS_ERR_CUDA, "verify queue launch", e);
+      if (e != cudaSuccess) {
+        fail(c, HS_ERR_CUDA, "verify queue launch", e);
+        break;
+      }
+      n_ok++;
     }
   }
   {
     std::lock_guard<std::mutex> g(q->mu);
-    if (dlo < dhi) {
-      if (e == cudaSuccess) {
-        q->inflight.push_back(hs_queue::launch{seq, dlo, dhi});
+    for (size_t k = 0; k < runs.size(); k++) {
+      const hs_queue::launch &L = runs[k];
+      if (k < n_ok) {
+        q->inflight.push_back(L);
       } else {
-        for (uint64_t p = dlo; p < dhi; p += q->reqs[p & q->mask].n)
+        for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
           if (q->reqs[p & q->mask].seq) queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
       }
     }
   }
   queue_fire(fire);
-  // the slow path: exactly the synchronous entry point (key cache, generic kernels), on this thread
+  // the slow path: exactly the synchronous entry point (key cache, generic kernels), on this thread — one call per verdict mode
+  // present in the request (a small request has one mode; a Block group has a strict pass and a batch-eq pass)
   std::vector<hs_rec128> recs;
+  std::vector<uint32_t> idx, part;
   for (uint64_t p : slow) {
     const hs_queue::req &r = q->reqs[p & q->mask];
-    recs.resize(r.n);
-    for (uint32_t i = 0; i < r.n; i++) {
-      const uint32_t s = (uint32_t)((p + i) & q->mask);
-      memcpy(recs[i].sig, q->h_ring[s].sig, 64);
-      memcpy(recs[i].pk, q->pk.data() + 32 * (size_t)s, 32);
-      memcpy(recs[i].msg, q->h_ring[s].msg, 32);
+    std::fill(q->wbits.begin(), q->wbits.begin() + (r.n + 31) / 32, 0u);
+    int rc = HS_OK;
+    for (uint32_t mode = HS_MODE_STRICT; mode <= HS_MODE_BATCH_EQ && rc == HS_OK; mode++) {
+      recs.clear();
+      idx.clear();
+      for (uint32_t i = 0; i < r.n; i++) {
+        const uint32_t s = (uint32_t)((p + i) & q->mask);
+        if (q->modes[s] != mode) continue;
+        hs_rec128 x;
+        memcpy(x.sig, q->h_ring[s].sig, 64);
+        memcpy(x.pk, q->pk.data() + 32 * (size_t)s, 32);
+        memcpy(x.msg, q->h_ring[s].msg, 32);
+        recs.push_back(x);
+        idx.push_back(i);
+      }
+      if (recs.empty()) continue;
+      part.assign((recs.size() + 31) / 32, 0);
+      rc = hs_verify_rec128(c, recs.data(), recs.size(), mode, part.data());
+      for (size_t k = 0; k < idx.size(); k++)
+        if ((part[k >> 5] >> (k & 31)) & 1u) q->wbits[idx[k] >> 5] |= 1u << (idx[k] & 31);
     }
-    uint32_t bits[(HS_SMALL_MAX + 31) / 32] = {0, 0};
-    const int rc = hs_verify_rec128(c, recs.data(), r.n, r.mode, bits);
     {
       std::lock_guard<std::mutex> g(q->mu);
-      queue_finish_locked(q, p, rc == HS_OK ? HS_OK : HS_ERR_CUDA, bits, fire);
+      queue_finish_locked(q, p, rc == HS_OK ? HS_OK : HS_ERR_CUDA, q->wbits.data(), fire);
     }
     queue_fire(fire);
   }
@@ -1370,10 +1418,13 @@ static void queue_watch(hs_queue *q) {
         if (((volatile uint32_t *)q->h_done)[p & q->mask] == L.seq) {
           if (!mine) continue;
           std::atomic_thread_fence(std::memory_order_acquire);
-          uint32_t bits[(HS_SMALL_MAX + 31) / 32] = {0, 0};
-          const uint32_t want = (r.mode == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
-          for (uint32_t i = 0; i < r.n; i++)
-            if (((volatile uint8_t *)q->h_flags)[(p + i) & q->mask] & want) bits[i >> 5] |= 1u << (i & 31);
+          uint32_t *bits = q->wbits.data();
+          std::fill(bits, bits + (r.n + 31) / 32, 0u);
+          for (uint32_t i = 0; i < r.n; i++) {  // the kernel writes both flags: each record's mode picks its verdict
+            const uint32_t s = (uint32_t)((p + i) & q->mask);
+            const uint32_t want = (q->modes[s] == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
+            if (((volatile uint8_t *)q->h_flags)[s] & want) bits[i >> 5] |= 1u << (i & 31);
+          }
           queue_finish_locked(q, p, HS_OK, bits, fire);
         } else if (qe == cudaErrorNotReady) {
           open = true;
@@ -2372,6 +2423,8 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   q->cap = cap;
   q->mask = cap - 1;
   q->pk.assign((size_t)cap * 32, 0);
+  q->modes.assign(cap, 0);
+  q->wbits.assign(cap / 32, 0);
   q->reqs.assign(cap, hs_queue::req{});
   int lo = 0, hi = 0;
   cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -2404,26 +2457,41 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   return HS_OK;
 }
 
-int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb, void *user, size_t *out_ticket) {
-  if (!q || !recs || n == 0 || n > HS_SMALL_MAX || mode > 1) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit: bad argument");
+// Copies one request into the ring (arguments already checked): record i is judged by modes[i], or by `mode` when modes is null.
+static int queue_enqueue(hs_queue *q, const char *what, const hs_rec128 *recs, size_t n, uint32_t mode, const uint8_t *modes, hs_queue_cb *cb,
+                         void *user, size_t *out_ticket) {
   {
     std::lock_guard<std::mutex> g(q->mu);
-    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit: queue is being destroyed");
+    if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
     if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
     for (size_t i = 0; i < n; i++) {
       const uint32_t s = (uint32_t)((q->tail + i) & q->mask);
       memcpy(q->h_ring[s].sig, recs[i].sig, 64);
       memcpy(q->h_ring[s].msg, recs[i].msg, 32);
       memcpy(q->pk.data() + 32 * (size_t)s, recs[i].pk, 32);
+      q->modes[s] = modes ? modes[i] : (uint8_t)mode;
     }
     const size_t ticket = q->next_ticket++;
-    q->reqs[q->tail & q->mask] = hs_queue::req{ticket, (uint32_t)n, mode, cb, user, 0, false};
-    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {0, 0}};
+    q->reqs[q->tail & q->mask] = hs_queue::req{ticket, (uint32_t)n, cb, user, 0, false};
+    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
     q->tail += n;
     if (out_ticket) *out_ticket = ticket;
   }
   q->cv_work.notify_one();
   return HS_OK;
+}
+
+int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !recs || n == 0 || n > HS_SMALL_MAX || mode > 1) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit: bad argument");
+  return queue_enqueue(q, "hs_queue_submit", recs, n, mode, nullptr, cb, user, out_ticket);
+}
+
+int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const uint8_t *modes, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !recs || n == 0 || n > q->cap) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
+  if (modes)
+    for (size_t i = 0; i < n; i++)
+      if (modes[i] > HS_MODE_BATCH_EQ) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_group: bad mode byte");
+  return queue_enqueue(q, "hs_queue_submit_group", recs, n, HS_MODE_STRICT, modes, cb, user, out_ticket);
 }
 
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap) {
@@ -2433,10 +2501,10 @@ int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap) {
   if (it == q->results.end()) return fail(q->c, HS_ERR_ARG, "hs_queue_poll: unknown ticket (already read, or consumed by its callback)");
   *done = it->second.done ? 1 : 0;
   if (!it->second.done) return HS_OK;
-  const hs_queue::result r = it->second;
+  const int status = it->second.status;
+  memcpy(out_bitmap, it->second.bits.data(), 4 * (size_t)((it->second.n + 31) / 32));
   q->results.erase(it);
-  memcpy(out_bitmap, r.bits, 4 * (size_t)((r.n + 31) / 32));
-  return r.status;
+  return status;
 }
 
 int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap) {
@@ -2446,10 +2514,10 @@ int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap) {
     auto it = q->results.find(ticket);  // looked up again after every wake-up: submissions may rehash the map
     if (it == q->results.end()) return fail(q->c, HS_ERR_ARG, "hs_queue_wait: unknown ticket (already read, or consumed by its callback)");
     if (it->second.done) {
-      const hs_queue::result r = it->second;
+      const int status = it->second.status;
+      memcpy(out_bitmap, it->second.bits.data(), 4 * (size_t)((it->second.n + 31) / 32));
       q->results.erase(it);
-      memcpy(out_bitmap, r.bits, 4 * (size_t)((r.n + 31) / 32));
-      return r.status;
+      return status;
     }
     q->cv_done.wait(lk);
   }

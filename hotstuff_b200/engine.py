@@ -303,8 +303,9 @@ class Engine:
 
 
 class VerifyQueue:
-    """hs_queue_* (include/hs_crypto.h): submit 1..64 records without blocking; a dispatcher thread coalesces whatever is
-    pending into one latency-path launch.  Verdicts equal Engine.verify_rec128 on the same records.  A ticket is read once:
+    """hs_queue_* (include/hs_crypto.h): submit 1..64 records (submit) or a whole certificate (submit_group) without blocking;
+    a dispatcher thread coalesces whatever is pending into one latency-path launch.  Verdicts equal Engine.verify_rec128 on the
+    same records (per record and its mode for a group).  A ticket is read once:
     by poll() / wait(), or by the callback given to submit() (called on the queue's thread as callback(ticket, status, bools);
     status != 0 means engine failure: reject every signature)."""
 
@@ -329,12 +330,26 @@ class VerifyQueue:
 
     def submit(self, recs, mode=MODE_STRICT, callback=None):
         """recs: (n,128) uint8 [sig64|pk32|msg32], 1 <= n <= 64.  Returns the ticket, or None when the ring is full (retry later)."""
+        return self._submit(self.lib.hs_queue_submit, "hs_queue_submit", recs, mode, callback)
+
+    def submit_group(self, recs, modes=None, callback=None):
+        """One consensus message's whole certificate (a Block: author strict + QC votes batch-eq + TC votes strict; a Timeout with
+        its high_qc; a TC; a QC) as ONE request.  recs: (n,128) uint8, 1 <= n <= the ring's capacity; modes: uint8[n] of MODE_*
+        per record (None = all strict).  Returns the ticket, or None when the ring has no room now (verify synchronously)."""
+        recs = _u8(recs, 128).reshape(-1, 128)
+        if modes is not None:
+            modes = np.ascontiguousarray(modes, dtype=np.uint8).reshape(-1)
+            if modes.shape[0] != recs.shape[0]:
+                raise ValueError("submit_group: %d modes for %d records" % (modes.shape[0], recs.shape[0]))
+        return self._submit(self.lib.hs_queue_submit_group, "hs_queue_submit_group", recs, None if modes is None else _ptr(modes), callback)
+
+    def _submit(self, fn, name, recs, mode_arg, callback):
         recs = _u8(recs, 128).reshape(-1, 128)
         n = recs.shape[0]
         t = ctypes.c_size_t(0)
         if callback is None:
             with self._lock:  # registered first: poll / wait from another thread may race the return
-                rc = self.lib.hs_queue_submit(self.h, _ptr(recs), n, mode, None, None, ctypes.byref(t))
+                rc = fn(self.h, _ptr(recs), n, mode_arg, None, None, ctypes.byref(t))
                 if rc == 0:
                     self._n[t.value] = n
         else:
@@ -342,13 +357,13 @@ class VerifyQueue:
                 uid = self._next_id
                 self._next_id += 1
                 self._callbacks[uid] = (callback, n)
-            rc = self.lib.hs_queue_submit(self.h, _ptr(recs), n, mode, ctypes.cast(self._trampoline, ctypes.c_void_p), uid, ctypes.byref(t))
+            rc = fn(self.h, _ptr(recs), n, mode_arg, ctypes.cast(self._trampoline, ctypes.c_void_p), uid, ctypes.byref(t))
             if rc != 0:
                 with self._lock:
                     self._callbacks.pop(uid, None)
         if rc == 3:  # HS_ERR_NOMEM: back-pressure
             return None
-        self.engine._check(rc, "hs_queue_submit")
+        self.engine._check(rc, name)
         return t.value
 
     def _take(self, ticket, rc, words):
@@ -357,10 +372,16 @@ class VerifyQueue:
         self.engine._check(rc, "hs_queue ticket %d" % ticket)
         return bitmap_to_bools(words, n)
 
+    def _words(self, ticket):
+        """The verdict buffer of a ticket read by poll / wait: (n + 31) / 32 words (at least 2: an unknown ticket is an error)."""
+        with self._lock:
+            n = self._n.get(int(ticket), 64)
+        return np.zeros(max(2, (n + 31) // 32), dtype=np.uint32)
+
     def poll(self, ticket):
         """None while the request is in flight, else its verdicts (bool[n]); consumes the ticket."""
         done = ctypes.c_int(0)
-        words = np.zeros(2, dtype=np.uint32)
+        words = self._words(ticket)
         rc = self.lib.hs_queue_poll(self.h, int(ticket), ctypes.byref(done), _ptr(words))
         if rc == 0 and not done.value:
             return None
@@ -368,7 +389,7 @@ class VerifyQueue:
 
     def wait(self, ticket):
         """Blocks until the request is done; returns its verdicts (bool[n]) and consumes the ticket."""
-        words = np.zeros(2, dtype=np.uint32)
+        words = self._words(ticket)
         rc = self.lib.hs_queue_wait(self.h, int(ticket), _ptr(words))
         return self._take(ticket, rc, words)
 

@@ -184,11 +184,17 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  * are done.
  *   - hs_queue_submit copies the records into the queue's ring and returns at once: HS_ERR_NOMEM when the ring has no room for
  *     n records (retry after some requests complete), HS_ERR_ARG for n = 0, n > 64 or a bad mode.  One request = one message's
- *     signatures (a Vote, a Timeout / Block author, a small QC); larger sets belong to the batch entry points.
- *   - Verdicts equal hs_verify_rec128(ctx, recs, n, mode, ..) on the same records, bit for bit.
+ *     signatures (a Vote, a Timeout / Block author, a small QC).
+ *   - hs_queue_submit_group takes one consensus message's whole certificate as ONE request: a Block (author strict + QC votes
+ *     batch-eq + TC votes strict), a Timeout with its high_qc, a TC, a QC — up to the ring's capacity, with a verdict mode per
+ *     record.  It shares the ring, the dispatcher and the launches with small requests: a group whose keys are all registered
+ *     costs one launch when nothing else is pending.  HS_ERR_NOMEM here means "verify it through the synchronous entry points
+ *     now".
+ *   - Verdicts equal hs_verify_rec128(ctx, recs, n, mode, ..) on the same records, bit for bit (for a group: record i equals
+ *     hs_verify_rec128(ctx, &recs[i], 1, modes[i], ..)).
  *   - Device path: only when a committee is registered (hs_committee_register) and every key of the request is in it.  Any
- *     other request is run by the queue's thread through hs_verify_rec128 itself (key cache / generic kernels): correct, but
- *     the slow path.
+ *     other request is run by the queue's thread through hs_verify_rec128 itself (key cache / generic kernels; a group takes
+ *     at most one strict and one batch-eq call): correct, but the slow path.
  *   - Consumption: with a callback, it runs exactly once on the queue's thread (status HS_OK, or HS_ERR_CUDA = reject every
  *     signature of the request; bitmap = n verdict bits, valid during the call) and the ticket is released when it returns.
  *     Without one, the result is kept until ONE hs_queue_poll that reports done, or one hs_queue_wait; both return the
@@ -204,6 +210,12 @@ typedef void(hs_queue_cb)(void *user, size_t ticket, int status, const uint32_t 
 int hs_queue_create(hs_ctx *ctx, size_t ring_records, hs_queue **out);
 /* n = 1..64 records, mode = HS_MODE_*; callback nullable; out_ticket nullable. */
 int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
+/* One consensus message's signatures as ONE queue request: n = 1 .. ring capacity records; record i is judged by modes[i]
+ * (HS_MODE_*; NULL = all strict, as in hs_verify_groups).  HS_ERR_ARG: n = 0, n > ring capacity, a mode byte > 1.
+ * HS_ERR_NOMEM: no room right now (back-pressure).  Completion, tickets, poll / wait / callback exactly as hs_queue_submit; the
+ * bitmap holds n bits (poll / wait: (n + 31) / 32 words). */
+int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const uint8_t *modes_or_null, hs_queue_cb *cb_or_null, void *user,
+                          size_t *out_ticket);
 /* Non-blocking: *done = 0 (come back later) or 1 (out_bitmap holds the verdicts, ticket consumed, returns the request's status). */
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap);
 /* Blocks until the request is done; consumes the ticket and returns the request's status. */

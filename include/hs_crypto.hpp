@@ -72,6 +72,21 @@ class VerifyQueue {
     return f;
   }
 
+  // One consensus message's whole certificate as ONE request (hs_queue_submit_group): a Block (author strict + QC votes batch-eq
+  // + TC votes strict), a Timeout with its high_qc, a TC, a QC.  n = 1 .. ring capacity, modes[i] = HS_MODE_* of record i
+  // (nullptr = all strict).  Throws QueueFull when the ring has no room now (verify synchronously), EngineError on a bad argument.
+  std::future<std::vector<bool>> submit_group(const hs_rec128 *recs, size_t n, const uint8_t *modes = nullptr) {
+    auto *p = new Pending{std::promise<std::vector<bool>>(), n};
+    std::future<std::vector<bool>> f = p->promise.get_future();
+    const int rc = hs_queue_submit_group(q_, recs, n, modes, &VerifyQueue::done, p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit_group");
+    }
+    return f;
+  }
+
  private:
   struct Pending {
     std::promise<std::vector<bool>> promise;

@@ -31,8 +31,9 @@ unsafe impl Send for Queue {}
 unsafe impl Sync for Queue {}          // hs_queue_submit is thread-safe and never blocks
 static QUEUE: OnceLock<Option<Queue>> = OnceLock::new();
 
-/// The node-wide queue on the shim's context (default ring of 4,096 records); lives as long as the process.
-fn queue() -> Option<*mut HsQueue> {
+/// The node-wide queue on the shim's context (default ring of 4,096 records); lives as long as the process.  Shared with the
+/// certificate requests of `group_queue::verify_group_queued`.
+pub(crate) fn queue() -> Option<*mut HsQueue> {
     QUEUE.get_or_init(|| {
         let c = ctx()?;
         let mut q = std::ptr::null_mut();

@@ -17,6 +17,10 @@ use std::sync::OnceLock;
 /// The verify queue (hs_queue_*): concurrent single-message verifies share latency-path launches (`queue::verify_queued`).
 #[path = "crypto_gpu_queue.rs"]
 pub mod queue;
+/// Whole certificates through the same queue (hs_queue_submit_group): Block / Timeout / TC verifies at the connection tasks
+/// (`group_queue::verify_group_queued`).
+#[path = "crypto_gpu_group_queue.rs"]
+pub mod group_queue;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

@@ -16,6 +16,12 @@
 // hs_verify_rec128(n = 1) per vote from the same 16 threads, (c) the CPU oracle verifying the votes serially on one core (what
 // Core does today).  Per-vote latency = burst start -> that vote's verdict; every verdict is checked against the oracle.
 //
+// Replica block (after the burst): one Block::verify certificate = 1 strict author signature + N - f batch-eq QC votes, 1 % of
+// the records corrupted, N = 4 .. 10,000, on a 16,384-record ring.  Three arms per block: (a) one hs_queue_submit_group consumed by
+// hs_queue_wait, (b) the synchronous calls the shim makes today (a strict author verify + hs_verify_batch_shared_msg), (c) the CPU
+// oracle on one core.  Block during a burst: the 1,000-validator vote burst above with one 668-record Block certificate submitted
+// once half the votes are in, (a) through the same queue or (b) as the synchronous calls from another thread.
+//
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
 #include <atomic>
@@ -172,6 +178,248 @@ static int vote_burst(hs_ctx *ctx, int N, int bursts, bool last) {
   printf("}%s", last ? "" : ", ");
   return a.mismatches + b.mismatches;
 }
+// ---- replica Block::verify: one certificate = 1 strict author signature + N - f batch-eq QC votes (messages.rs:54-76, :180-208)
+struct cert {
+  std::vector<hs_rec128> recs;  // [0] author over the block digest, [1..] the QC's votes over the QC digest
+  std::vector<uint8_t> modes;
+  std::vector<hs_vote> votes;   // the same votes in the shape of hs_verify_batch_shared_msg
+  uint8_t qd[32];
+  std::vector<uint32_t> want;   // oracle verdict bitmap of recs in their modes
+};
+struct committee_keys {
+  int N = 0;
+  std::vector<uint8_t> seeds, pks;
+};
+static committee_keys make_keys(int N, int salt) {
+  committee_keys k;
+  k.N = N;
+  k.seeds.resize((size_t)N * 32);
+  k.pks.resize((size_t)N * 32);
+  for (int i = 0; i < N; i++)
+    for (int j = 0; j < 32; j++) k.seeds[(size_t)i * 32 + j] = (uint8_t)(29 * i + 5 * j + salt + (i >> 8) * 3 + (i >> 16));
+  hso_keygen_batch(k.seeds.data(), N, k.pks.data());
+  return k;
+}
+static int ncpu() { return std::max(1, (int)std::thread::hardware_concurrency()); }
+// Block of round r: author r % N signs the block digest, voters (i * 7 + r) % N sign the QC digest; 1 % of the records corrupted.
+static void make_cert(const committee_keys &k, int r, cert &c) {
+  const int N = k.N, f = (N - 1) / 3, nv = N - f, n = nv + 1;
+  uint8_t pre[40], bd[32];
+  for (int j = 0; j < 32; j++) pre[j] = (uint8_t)(r * 17 + j * 3 + 1);
+  const uint64_t round = 5000 + (uint64_t)r;
+  memcpy(pre + 32, &round, 8);
+  hso_digest32(pre, 40, c.qd);  // Vote / QC digest = SHA-512(block hash || round)
+  pre[0] ^= 0x55;
+  hso_digest32(pre, 40, bd);    // stands for Block::digest
+  std::vector<uint32_t> key(n);
+  std::vector<uint8_t> msgs((size_t)n * 32);
+  std::vector<uint64_t> off(n + 1);
+  for (int i = 0; i < n; i++) {
+    key[i] = (uint32_t)(i == 0 ? r % N : ((i - 1) * 7 + r) % N);
+    memcpy(&msgs[(size_t)i * 32], i == 0 ? bd : c.qd, 32);
+    off[i] = (uint64_t)i * 32;
+  }
+  off[n] = (uint64_t)n * 32;
+  std::vector<uint8_t> sigs((size_t)n * 64);
+  hso_sign_batch(k.seeds.data(), k.pks.data(), key.data(), msgs.data(), off.data(), n, ncpu(), sigs.data());
+  c.recs.resize(n);
+  c.modes.assign(n, (uint8_t)HS_MODE_BATCH_EQ);
+  c.modes[0] = (uint8_t)HS_MODE_STRICT;
+  c.votes.resize(nv);
+  for (int i = 0; i < n; i++) {
+    memcpy(c.recs[i].sig, &sigs[(size_t)i * 64], 64);
+    memcpy(c.recs[i].pk, &k.pks[(size_t)key[i] * 32], 32);
+    memcpy(c.recs[i].msg, &msgs[(size_t)i * 32], 32);
+    if ((i * 37 + r * 11) % 100 == 0) c.recs[i].sig[(i + r) % 64] ^= 0x10;  // 1 % corrupted
+    if (i) {
+      memcpy(c.votes[i - 1].pk, c.recs[i].pk, 32);
+      memcpy(c.votes[i - 1].sig, c.recs[i].sig, 64);
+    }
+  }
+  std::vector<uint32_t> s((n + 31) / 32), e((n + 31) / 32);
+  hso_verify_rec128_batch((const uint8_t *)c.recs.data(), n, 0, ncpu(), s.data());
+  hso_verify_rec128_batch((const uint8_t *)c.recs.data(), n, 1, ncpu(), e.data());
+  c.want.assign((n + 31) / 32, 0);
+  for (int i = 0; i < n; i++)
+    if ((((c.modes[i] ? e : s)[i >> 5]) >> (i & 31)) & 1u) c.want[i >> 5] |= 1u << (i & 31);
+}
+static bool bit(const std::vector<uint32_t> &b, int i) { return (b[i >> 5] >> (i & 31)) & 1u; }
+// The synchronous calls the shim makes for one Block today: a strict author verify + one verify_batch over the QC's votes.
+static int sync_block(hs_ctx *ctx, const cert &c, std::vector<uint32_t> &bits) {
+  const size_t nv = c.votes.size();
+  std::vector<uint32_t> vb((nv + 31) / 32);
+  uint32_t a = 0;
+  int all_ok = 0;
+  if (hs_verify_rec128(ctx, &c.recs[0], 1, HS_MODE_STRICT, &a) != HS_OK) return 1;
+  if (hs_verify_batch_shared_msg(ctx, c.qd, c.votes.data(), nv, &all_ok, vb.data()) != HS_OK) return 1;
+  bits.assign((nv + 1 + 31) / 32, 0);
+  bits[0] = a & 1u;
+  for (size_t i = 0; i < nv; i++)
+    if (bit(vb, (int)i)) bits[(i + 1) >> 5] |= 1u << ((i + 1) & 31);
+  return 0;
+}
+static int count_mismatch(const cert &c, const std::vector<uint32_t> &bits) {
+  int m = 0;
+  for (size_t i = 0; i < c.recs.size(); i++) m += bit(bits, (int)i) != bit(c.want, (int)i);
+  return m;
+}
+static int replica_block(hs_ctx *ctx, hs_queue *q, int N, int blocks, bool last) {
+  const committee_keys k = make_keys(N, 11);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  series qa, sb, cc;
+  uint64_t launches = 0;
+  int mism_a = 0, mism_b = 0, bad = 0;
+  cert c;
+  for (int r = 0; r < blocks + 3; r++) {
+    const bool timed = r >= 3;
+    make_cert(k, r, c);
+    const int n = (int)c.recs.size();
+    std::vector<uint32_t> bits((n + 31) / 32);
+    // (a) one hs_queue_submit_group, consumed by hs_queue_wait
+    uint64_t l0 = hs_kernel_launches(ctx);
+    auto t0 = clk::now();
+    size_t ticket = 0;
+    if (hs_queue_submit_group(q, c.recs.data(), n, c.modes.data(), nullptr, nullptr, &ticket) != HS_OK || hs_queue_wait(q, ticket, bits.data()) != HS_OK) bad++;
+    const double ta = us_since(t0);
+    if (timed) {
+      qa.v.push_back(ta);
+      launches += hs_kernel_launches(ctx) - l0;
+      mism_a += count_mismatch(c, bits);
+    }
+    // (b) the synchronous calls
+    t0 = clk::now();
+    bad += sync_block(ctx, c, bits);
+    const double tb = us_since(t0);
+    if (timed) {
+      sb.v.push_back(tb);
+      mism_b += count_mismatch(c, bits);
+    }
+    // (c) the CPU oracle on one core: strict author verify + verify_batch of the votes
+    std::vector<uint32_t> vb((n - 1 + 31) / 32);
+    t0 = clk::now();
+    const int au = hso_verify_strict(c.recs[0].sig, c.recs[0].pk, c.recs[0].msg, 32);
+    hso_verify_batch_shared_msg(c.qd, (const uint8_t *)c.votes.data(), n - 1, 1, vb.data());
+    if (timed) cc.v.push_back(us_since(t0));
+    bad += au != (int)bit(c.want, 0);
+  }
+  const int nv = N - (N - 1) / 3;
+  printf("\"committee_%d\": {\"records\": %d, \"blocks\": %d, \"queue_submit_group\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"launches_per_block\": %.2f, "
+         "\"mismatches\": %d}, \"sync_strict_author_plus_verify_batch_shared_msg\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"mismatches\": %d}, "
+         "\"cpu_oracle_1core\": {\"p50_us\": %.1f, \"p99_us\": %.1f}, \"errors\": %d}%s",
+         N, nv + 1, blocks, qa.pct(0.5), qa.pct(0.99), (double)launches / blocks, mism_a, sb.pct(0.5), sb.pct(0.99), mism_b, cc.pct(0.5), cc.pct(0.99), bad,
+         last ? "" : ", ");
+  return mism_a + mism_b + bad;
+}
+
+// ---- a Block certificate submitted in the middle of the leader's vote burst (N = 1,000: 667 votes + a 668-record Block)
+struct blk_done {
+  clk::time_point t0;
+  double lat;
+  std::vector<uint32_t> bits;
+  std::atomic<int> done{0};
+};
+static void on_block(void *user, size_t, int status, const uint32_t *bitmap) {
+  blk_done *b = (blk_done *)user;
+  b->lat = us_since(b->t0);
+  if (status == HS_OK) memcpy(b->bits.data(), bitmap, 4 * b->bits.size());
+  else std::fill(b->bits.begin(), b->bits.end(), 0u);
+  b->done.store(status == HS_OK ? 1 : -1, std::memory_order_release);
+}
+static int block_during_burst(hs_ctx *ctx, int bursts) {
+  const int N = 1000, f = (N - 1) / 3, nv = N - f, nth = 16;
+  const committee_keys k = make_keys(N, 23);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 0, &q) != HS_OK) return 1;
+  burst_arm arm[2];
+  series blk[2];
+  int blk_bad[2] = {0, 0};
+  std::vector<hs_rec128> votes(nv);
+  std::vector<int> want(nv), got(nv);
+  std::vector<double> lat(nv);
+  std::vector<burst_vote> bv(nv);
+  cert c;
+  for (int r = 0; r < bursts + 3; r++) {
+    const bool timed = r >= 3;
+    make_cert(k, 1000 + r, c);  // the replica's Block (another round's certificate)
+    uint8_t pre[40], d[32];
+    for (int j = 0; j < 32; j++) pre[j] = (uint8_t)(r * 13 + j);
+    const uint64_t round = 1000 + (uint64_t)r;
+    memcpy(pre + 32, &round, 8);
+    hso_digest32(pre, 40, d);
+    for (int i = 0; i < nv; i++) {
+      const int kk = (i * 7 + r) % N;
+      hso_sign(&k.seeds[(size_t)kk * 32], d, 32, votes[i].sig);
+      memcpy(votes[i].pk, &k.pks[(size_t)kk * 32], 32);
+      memcpy(votes[i].msg, d, 32);
+      if ((i * 37 + r * 11) % 100 == 0) votes[i].sig[(i + r) % 64] ^= 0x10;
+    }
+    std::vector<uint32_t> wb((nv + 31) / 32);
+    hso_verify_rec128_batch((const uint8_t *)votes.data(), nv, 0, ncpu(), wb.data());
+    for (int i = 0; i < nv; i++) want[i] = bit(wb, i);
+    for (int a = 0; a < 2; a++) {  // a = 0: the Block through the queue; a = 1: the Block as synchronous calls
+      std::atomic<int> go{0}, submitted{0}, bad{0};
+      blk_done bd;
+      bd.bits.assign((c.recs.size() + 31) / 32, 0);
+      std::vector<std::thread> ts;
+      std::fill(got.begin(), got.end(), -2);
+      clk::time_point t0;
+      const uint64_t l0 = hs_kernel_launches(ctx);
+      for (int t = 0; t < nth; t++)
+        ts.emplace_back([&, t] {
+          while (!go.load()) {
+          }
+          for (int i = t; i < nv; i += nth) {
+            bv[i] = burst_vote{t0, &lat[i], &got[i]};
+            int rc;
+            while ((rc = hs_queue_submit(q, &votes[i], 1, HS_MODE_STRICT, on_vote, &bv[i], nullptr)) == HS_ERR_NOMEM) std::this_thread::yield();
+            if (rc != HS_OK) bad++;
+            submitted++;
+          }
+        });
+      ts.emplace_back([&] {  // the replica's connection task: its Block arrives when half the votes are in
+        while (submitted.load() < nv / 2) {
+        }
+        bd.t0 = clk::now();
+        if (a == 0) {
+          if (hs_queue_submit_group(q, c.recs.data(), c.recs.size(), c.modes.data(), on_block, &bd, nullptr) != HS_OK) bd.done.store(-1);
+        } else {
+          std::vector<uint32_t> bits;
+          const int rc = sync_block(ctx, c, bits);
+          bd.lat = us_since(bd.t0);
+          if (rc == 0) bd.bits = bits;
+          bd.done.store(rc == 0 ? 1 : -1);
+        }
+      });
+      t0 = clk::now();
+      go = 1;
+      for (auto &t : ts) t.join();
+      for (int i = 0; i < nv; i++)
+        while (__atomic_load_n(&got[i], __ATOMIC_ACQUIRE) == -2) std::this_thread::yield();
+      while (bd.done.load(std::memory_order_acquire) == 0) std::this_thread::yield();
+      if (timed) {
+        arm[a].total.v.push_back(*std::max_element(lat.begin(), lat.end()));
+        arm[a].vote.v.insert(arm[a].vote.v.end(), lat.begin(), lat.end());
+        arm[a].launches += hs_kernel_launches(ctx) - l0;
+        for (int i = 0; i < nv; i++) arm[a].mismatches += got[i] != want[i];
+        arm[a].mismatches += bad.load();
+        blk[a].v.push_back(bd.lat);
+        blk_bad[a] += (bd.done.load() != 1) + count_mismatch(c, bd.bits);
+      }
+    }
+  }
+  hs_queue_destroy(q);
+  printf("\"votes\": %d, \"block_records\": %zu, \"bursts\": %d, ", nv, c.recs.size(), bursts);
+  const char *names[2] = {"block_via_queue_submit_group", "block_via_synchronous_calls_other_thread"};
+  for (int a = 0; a < 2; a++) {
+    printf("\"%s\": {\"block_p50_us\": %.1f, \"block_p99_us\": %.1f, \"block_mismatches\": %d, ", names[a], blk[a].pct(0.5), blk[a].pct(0.99), blk_bad[a]);
+    arm[a].emit("votes", bursts, true);
+    printf("}%s", a ? "" : ", ");
+  }
+  return arm[0].mismatches + arm[1].mismatches + blk_bad[0] + blk_bad[1];
+}
 static std::string gpu_identity() {  // name and enforced power limit, read in the same run
   std::string s;
   if (FILE *p = popen("nvidia-smi --query-gpu=name,power.limit --format=csv,noheader -i 0 2>/dev/null", "r")) {
@@ -294,6 +542,13 @@ int main(int argc, char **argv) {
   printf("\"leader_vote_burst\": {\"gpu\": \"%s\", \"threads\": 16, ", gpu_identity().c_str());
   int burst_bad = 0;
   for (int N : {4, 100, 1000}) burst_bad += vote_burst(ctx, N, bursts, N == 1000);
+  printf("}, \"replica_block\": {\"gpu\": \"%s\", \"ring_records\": 16384, ", gpu_identity().c_str());
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 16384, &q) != HS_OK) return 1;
+  for (int N : {4, 100, 250, 500, 750, 1000, 10000}) burst_bad += replica_block(ctx, q, N, bursts, N == 10000);
+  hs_queue_destroy(q);
+  printf("}, \"block_during_burst\": {\"gpu\": \"%s\", \"threads\": 16, ", gpu_identity().c_str());
+  burst_bad += block_during_burst(ctx, bursts);
   printf("}}\n");
   hs_ctx_destroy(ctx);
   return (bad || burst_bad) ? 9 : 0;

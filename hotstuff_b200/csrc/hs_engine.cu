@@ -15,6 +15,8 @@
 //                     epoch flags exchanged by the last block); optionally on the context's tail stream (deferred mode)
 // Latency pipeline (n <= 64, every key has a table): k_verify_small — ONE launch, a warp per signature sums the table entries
 //   with a shuffle tree while a second warp decompresses R; inputs / verdicts in mapped pinned memory.
+// Verify queue: small requests share k_verify_small launches; a large certificate gets k_verify_bulk (a thread per signature
+//   from the queue's ring, the block's Z's inverted together, verdicts written by the same launch).
 // Digest: k_digest32_fixed (staged coalesced loads, constant padding schedule), k_digest32 (any length), k_digest32_long
 //   (one warp per long message, schedules expanded across lanes).
 // Front ends: QC / TC / Timeout / Block groups with on-GPU digests and per-certificate AND; load-generation keygen / signer.
@@ -377,6 +379,102 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
       __threadfence_system();
       done[req] = seq;
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ bulk queue path (large groups)
+// A certificate of a large committee (thousands of votes) as ONE queue request: k_verify_small would spend a 64-thread block and a
+// square-root chain on every signature, several waves of them.  Here a THREAD verifies a signature as k_verify_main<true> does,
+// straight from the queue's mapped ring (logical record i = ring slot (base + i) & mask, so a group may wrap the ring's end), and
+// the block finishes its own records: the block's Z's share one batched inversion (Montgomery's trick through shared memory, warp 0
+// inverting the product of 4 threads' Z's per lane, as in k_verify_finish), then the affine comparison with R's encoding — no
+// decompression of R, no global scratch, no second launch.  Flags and completion as in k_verify_small: both HS_F_EQ and HS_F_STRICT
+// per record, one counter add per block, and the block that completes the request raises its completion word.  One launch carries
+// exactly one request (n records).
+// Sizing: 128 threads, at least 3 blocks per SM.  R and the request fields stay live across the comb, so the 4-block budget of
+// k_verify_main (128 registers) spilled; 3 blocks allow 168 (sm_90a: 142 registers, 0 spills, 36,864 bytes smem).  A 6,668-record
+// certificate is 53 blocks, one per SM, so occupancy does not bound this launch at committee sizes.
+#define HS_BULK_THREADS 128
+#define HS_BULK_MINBLOCKS 3
+__global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_bulk(const small_rec *__restrict__ ring, uint32_t base, uint32_t mask,
+                                                                                  uint32_t n, const ge_niels *__restrict__ btable, committee_tables C,
+                                                                                  const comb_params cp, uint8_t *out_flags, uint32_t *counters,
+                                                                                  volatile uint32_t *done, uint32_t seq) {
+  // one buffer, two lives: record staging while loading, then the signed digits [digit][thread] (conflict-free columns)
+  __shared__ __align__(16) unsigned char smem_raw[HS_MAX_DIGITS * HS_BULK_THREADS * 4];
+  static_assert(sizeof(smem_raw) >= (HS_BULK_THREADS / 32) * 256 * sizeof(uint4), "staging does not fit");
+  __shared__ fe tot[HS_BULK_THREADS];
+  const int lane = threadIdx.x & 31;
+  const uint32_t first = blockIdx.x * HS_BULK_THREADS, t = first + threadIdx.x;
+  const uint32_t cnt = (n - first < HS_BULK_THREADS) ? n - first : HS_BULK_THREADS;  // records of this block (the last one is partial)
+  // (threads past n compute on a zero record and store nothing: every thread reaches the barriers below)
+  uint4 q[8];
+  {  // a warp stages its 32 records (128 B each) with coalesced 16-byte loads, then each lane reads its own row back
+    uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
+    const uint32_t warp_first = first + (threadIdx.x & ~31u);
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+      const int c = j * 32 + lane, rec = c >> 3, part = c & 7;
+      uint4 v = make_uint4(0, 0, 0, 0);
+      if (warp_first + rec < n) v = __ldg(reinterpret_cast<const uint4 *>(ring + ((base + warp_first + rec) & mask)) + part);
+      sw[rec * 8 + (part ^ (rec & 7))] = v;
+    }
+    __syncwarp();
+#pragma unroll
+    for (int part = 0; part < 8; part++) q[part] = sw[lane * 8 + (part ^ (lane & 7))];
+  }
+  __syncthreads();  // the staging bytes become the digit slots
+  uint32_t R[8], S[8], A[8], h[16];
+  R[0] = q[0].x; R[1] = q[0].y; R[2] = q[0].z; R[3] = q[0].w; R[4] = q[1].x; R[5] = q[1].y; R[6] = q[1].z; R[7] = q[1].w;
+  S[0] = q[2].x; S[1] = q[2].y; S[2] = q[2].z; S[3] = q[2].w; S[4] = q[3].x; S[5] = q[3].y; S[6] = q[3].z; S[7] = q[3].w;
+  uint32_t v = q[6].x;  // small_rec: sig | msg | vidx | req | req_n
+  const uint32_t req = q[6].y, req_n = q[6].z;
+  const bool have_key = v < C.n_keys;  // HS_NO_KEY (cannot reach this path: kept as in k_verify_small) rejects the record
+  if (!have_key) v = 0;
+  {
+    uint32_t M[8];
+    M[0] = q[4].x; M[1] = q[4].y; M[2] = q[4].z; M[3] = q[4].w; M[4] = q[5].x; M[5] = q[5].y; M[6] = q[5].z; M[7] = q[5].w;
+    load32(A, C.pks + (size_t)v * 32);  // hash the registered key bytes, as k_verify_main<true>
+    sha512_ram32(h, R, A, M);
+  }
+  ge_ext acc;
+  uint32_t meta = verify_committee_main(acc, R, S, h, btable, C.atables + (size_t)v * C.table_entries, have_key ? C.key_flags[v] : 0u,
+                                        reinterpret_cast<int32_t *>(smem_raw) + threadIdx.x, HS_BULK_THREADS, cp);
+  if (!have_key) meta = 0;
+  if (fe_is_zero(acc.Z)) {  // cannot happen for curve points; keeps one bad record from poisoning the block's inversion
+    fe_set1(acc.Z);
+    meta &= ~HS_META_PARSE_OK;
+  }
+  tot[threadIdx.x] = acc.Z;
+  __syncthreads();
+  if (threadIdx.x < HS_BULK_THREADS / 4) {  // lane l: 1 / Z of threads 4l .. 4l+3 from one inversion
+    const int b = threadIdx.x * 4;
+    fe q0 = tot[b], q1, q2, q3, inv, u;
+    fe_mul(q1, q0, tot[b + 1]);
+    fe_mul(q2, q1, tot[b + 2]);
+    fe_mul(q3, q2, tot[b + 3]);
+    fe_invert(inv, q3);
+    fe_mul(u, inv, q2);
+    fe_mul(inv, inv, tot[b + 3]);
+    tot[b + 3] = u;
+    fe_mul(u, inv, q1);
+    fe_mul(inv, inv, tot[b + 2]);
+    tot[b + 2] = u;
+    fe_mul(u, inv, q0);
+    fe_mul(inv, inv, tot[b + 1]);
+    tot[b + 1] = u;
+    tot[b] = inv;
+  }
+  __syncthreads();
+  if (threadIdx.x < cnt) {
+    out_flags[(base + t) & mask] = (uint8_t)verify_flags_from(acc.X, acc.Y, tot[threadIdx.x], R, meta);
+    __threadfence_system();
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(counters + req, cnt) == req_n - cnt) {  // thread 0 holds a record of the request
+    counters[req] = 0;
+    __threadfence_system();
+    done[req] = seq;
   }
 }
 
@@ -1191,7 +1289,12 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
 // message's certificate, up to the ring's capacity, a mode per record); both take the same ring, launches and completion path.
 #define HS_QUEUE_DEFAULT_RECORDS 4096u
 #define HS_QUEUE_MAX_RECORDS (1u << 20)
-#define HS_QUEUE_MAX_INFLIGHT 2
+#define HS_QUEUE_MAX_INFLIGHT 2  // k_verify_small launches; bulk launches do not count against it
+// Device requests of at least this many records get their own k_verify_bulk launch on the queue's second stream: the smallest
+// measured Block certificate from which one thread per signature plus a block-level inversion was no slower than k_verify_small's
+// block per signature (1,002 records, N = 1,500: 345 vs 375 us p50; at 668 records 307 vs 298 us; DESIGN.md §5d).
+#define HS_QUEUE_BULK_MIN 1002
+static_assert(HS_QUEUE_BULK_MIN > HS_SMALL_MAX, "small requests never take the bulk path");
 // A request's verdict bitmap: inline for <= 64 records (every small request), on the heap only for larger groups.
 struct queue_bits {
   uint32_t inl[(HS_SMALL_MAX + 31) / 32] = {0, 0};
@@ -1219,8 +1322,11 @@ struct hs_queue {
   std::vector<uint8_t> pk;                         // key bytes per record (host only: resolved to a table index at dispatch)
   std::vector<uint8_t> modes;                      // HS_MODE_* per record (host only: picks the verdict flag of each record)
   std::vector<uint32_t> wbits;                     // dispatcher thread only: verdict bitmap being assembled (cap bits)
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev_last = nullptr;                   // recorded after every launch: the ring is freed only after it
+  cudaStream_t stream = nullptr;                   // k_verify_small launches: the device's highest priority
+  cudaStream_t bulk_stream = nullptr;              // k_verify_bulk launches: a lower priority, so votes never wait behind them
+  cudaEvent_t ev_last = nullptr;                   // recorded after every launch on `stream`: the ring is freed only after it
+  cudaEvent_t ev_bulk_last = nullptr;              // the same for `bulk_stream`
+  uint64_t stats[HS_QUEUE_STATS] = {};             // hs_queue_stats
   struct req {
     size_t ticket;
     uint32_t n;
@@ -1240,8 +1346,9 @@ struct hs_queue {
   struct launch {
     uint32_t seq;
     uint64_t lo, hi;  // ring positions it covers
+    bool bulk;        // k_verify_bulk on bulk_stream (one request), else k_verify_small on stream
   };
-  std::deque<launch> inflight;
+  std::deque<launch> inflight;  // in ring order
   uint64_t head = 0, launched = 0, tail = 0;
   size_t next_ticket = 1;
   uint32_t seq = 0;
@@ -1295,13 +1402,15 @@ static void queue_fire(std::vector<queue_completion> &fire) {
 // one launch covers every request whose keys are all registered; the others then run through hs_verify_rec128 on this thread.
 // A slow-path request of at most 64 records between two device requests rides along in the launch (its blocks find no table
 // index and reject; its verdicts are ignored).  A larger one would cost thousands of wasted blocks, so the launch is split
-// around it: one launch per run of device requests between such requests.
+// around it: one launch per run of device requests between such requests.  A device request of HS_QUEUE_BULK_MIN records or more
+// closes the run the same way and gets a k_verify_bulk launch of its own on the bulk stream; the small launches of the same
+// dispatch are enqueued first.
 static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   hs_ctx *c = q->c;
   std::vector<uint64_t> slow;
   std::vector<queue_completion> fire;
-  std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one
-  size_t n_ok = 0;                     // runs launched without a CUDA error (the first failure stops the rest)
+  std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one, in ring order
+  std::vector<char> ok;                // runs launched without a CUDA error (the first failure stops the rest)
   cudaError_t e = cudaSuccess;
   {
     std::lock_guard<std::mutex> g(c->mu);
@@ -1317,45 +1426,65 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         s.req_n = r.n;
         if (s.vidx == HS_NO_KEY) all = false;
       }
-      if (all) {
-        if (rlo == hi) rlo = p;
-        rhi = p + r.n;
-        r.seq = 1;  // the launch's number is set below
-      } else {
+      const bool bulk = all && r.n >= HS_QUEUE_BULK_MIN;
+      if (!all) {
         r.seq = 0;
         slow.push_back(p);
-        if (r.n > HS_SMALL_MAX && rlo < rhi) {  // no large riders: close the run before it
-          runs.push_back(hs_queue::launch{0, rlo, rhi});
-          rlo = hi;
-          rhi = lo;
-        }
+      } else {
+        r.seq = 1;  // the launch's number is set below
+      }
+      if ((bulk || (!all && r.n > HS_SMALL_MAX)) && rlo < rhi) {  // no large riders, and no small request in a bulk launch
+        runs.push_back(hs_queue::launch{0, rlo, rhi, false});
+        rlo = hi;
+        rhi = lo;
+      }
+      if (bulk) {
+        runs.push_back(hs_queue::launch{0, p, p + r.n, true});
+      } else if (all) {
+        if (rlo == hi) rlo = p;
+        rhi = p + r.n;
       }
       p += r.n;
     }
-    if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi});
+    if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi, false});
     committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
-    for (hs_queue::launch &L : runs) {
-      L.seq = ++q->seq ? q->seq : ++q->seq;  // never 0
-      for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
-        if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = L.seq;
-      k_verify_small<<<(unsigned)(L.hi - L.lo), 64, 0, q->stream>>>(q->d_ring, (uint32_t)(L.lo & q->mask), q->mask, c->d_btable, C, c->cp,
-                                                                     q->d_flags, q->d_counters, q->d_done, L.seq);
-      c->launches++;
-      e = cudaGetLastError();
-      if (e == cudaSuccess) e = cudaEventRecord(q->ev_last, q->stream);
-      if (e != cudaSuccess) {
-        fail(c, HS_ERR_CUDA, "verify queue launch", e);
-        break;
+    ok.assign(runs.size(), 0);
+    for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {  // pass 0: the small launches, pass 1: the bulk ones
+      for (size_t k = 0; k < runs.size(); k++) {
+        hs_queue::launch &L = runs[k];
+        if (L.bulk != (pass == 1)) continue;
+        L.seq = ++q->seq ? q->seq : ++q->seq;  // never 0
+        for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
+          if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = L.seq;
+        const uint32_t n = (uint32_t)(L.hi - L.lo), base = (uint32_t)(L.lo & q->mask);
+        if (L.bulk)
+          k_verify_bulk<<<(n + HS_BULK_THREADS - 1) / HS_BULK_THREADS, HS_BULK_THREADS, 0, q->bulk_stream>>>(
+              q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
+        else
+          k_verify_small<<<n, 64, 0, q->stream>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
+        c->launches++;
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = L.bulk ? cudaEventRecord(q->ev_bulk_last, q->bulk_stream) : cudaEventRecord(q->ev_last, q->stream);
+        if (e != cudaSuccess) {
+          fail(c, HS_ERR_CUDA, "verify queue launch", e);
+          break;
+        }
+        ok[k] = 1;
       }
-      n_ok++;
     }
   }
   {
     std::lock_guard<std::mutex> g(q->mu);
+    for (uint64_t p : slow) {
+      q->stats[4]++;
+      q->stats[5] += q->reqs[p & q->mask].n;
+    }
     for (size_t k = 0; k < runs.size(); k++) {
       const hs_queue::launch &L = runs[k];
-      if (k < n_ok) {
+      if (ok[k]) {
         q->inflight.push_back(L);
+        q->stats[L.bulk ? 2 : 0]++;
+        q->stats[L.bulk ? 3 : 1] += L.hi - L.lo;
       } else {
         for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
           if (q->reqs[p & q->mask].seq) queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
@@ -1400,17 +1529,22 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
 
 // One pass over the launches in flight: a device request whose completion word carries its launch's number is finished with
 // its verdicts (the flags -> bits mapping of run_small).  A launch is retired once every request in its range — riders
-// included — has its word.  Every 4,096 passes the stream is queried: a CUDA error, or a drained stream with a word still
-// missing, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
+// included — has its word.  Every 4,096 passes both streams are queried: a CUDA error, or a drained stream with a word still
+// missing in a launch it ran, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
 static void queue_watch(hs_queue *q) {
   std::vector<queue_completion> fire;
-  cudaError_t qe = cudaErrorNotReady;
-  if ((++q->spins & 0xfff) == 0) qe = cudaStreamQuery(q->stream);  // queried BEFORE the words are read
-  if (qe != cudaSuccess && qe != cudaErrorNotReady) fail(q->c, HS_ERR_CUDA, "verify queue kernel", qe);
+  cudaError_t qes[2] = {cudaErrorNotReady, cudaErrorNotReady};  // [0] stream, [1] bulk_stream: a launch is judged by its own
+  if ((++q->spins & 0xfff) == 0) {  // queried BEFORE the words are read
+    qes[0] = cudaStreamQuery(q->stream);
+    qes[1] = cudaStreamQuery(q->bulk_stream);
+  }
+  for (cudaError_t x : qes)
+    if (x != cudaSuccess && x != cudaErrorNotReady) fail(q->c, HS_ERR_CUDA, "verify queue kernel", x);
   {
     std::lock_guard<std::mutex> g(q->mu);
     for (size_t k = 0; k < q->inflight.size(); k++) {
       const hs_queue::launch L = q->inflight[k];
+      const cudaError_t qe = qes[L.bulk ? 1 : 0];
       bool open = false;
       for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n) {
         hs_queue::req &r = q->reqs[p & q->mask];
@@ -1429,7 +1563,8 @@ static void queue_watch(hs_queue *q) {
         } else if (qe == cudaErrorNotReady) {
           open = true;
         } else if (mine) {
-          if (qe == cudaSuccess) fail(q->c, HS_ERR_CUDA, "verify queue: k_verify_small did not complete");
+          if (qe == cudaSuccess)
+            fail(q->c, HS_ERR_CUDA, L.bulk ? "verify queue: k_verify_bulk did not complete" : "verify queue: k_verify_small did not complete");
           queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
         }
       }
@@ -1442,11 +1577,17 @@ static void queue_watch(hs_queue *q) {
   queue_fire(fire);
 }
 
+static size_t queue_small_inflight_locked(const hs_queue *q) {
+  size_t k = 0;
+  for (const hs_queue::launch &L : q->inflight) k += !L.bulk;
+  return k;
+}
+
 static void queue_main(hs_queue *q) {
   cudaSetDevice(q->c->device);
   std::unique_lock<std::mutex> lk(q->mu);
   for (;;) {
-    if (q->launched < q->tail && q->inflight.size() < HS_QUEUE_MAX_INFLIGHT) {
+    if (q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) {
       const uint64_t lo = q->launched, hi = q->tail;  // everything pending
       q->launched = hi;
       lk.unlock();
@@ -1472,9 +1613,13 @@ static void queue_free(hs_queue *q) {
   q->cv_work.notify_all();
   if (q->th.joinable()) q->th.join();  // the thread finishes every request first
   cudaSetDevice(q->c->device);
-  if (q->ev_last) cudaEventSynchronize(q->ev_last);  // the last launch's blocks have exited before the ring goes
-  if (q->ev_last) cudaEventDestroy(q->ev_last);
+  for (cudaEvent_t ev : {q->ev_last, q->ev_bulk_last}) {  // the last launches' blocks have exited before the ring goes
+    if (!ev) continue;
+    cudaEventSynchronize(ev);
+    cudaEventDestroy(ev);
+  }
   if (q->stream) cudaStreamDestroy(q->stream);
+  if (q->bulk_stream) cudaStreamDestroy(q->bulk_stream);
   if (q->h_ring) cudaFreeHost(q->h_ring);
   if (q->h_flags) cudaFreeHost(q->h_flags);
   if (q->h_done) cudaFreeHost(q->h_done);
@@ -2429,7 +2574,9 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   int lo = 0, hi = 0;
   cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
   if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->stream, cudaStreamNonBlocking, hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->bulk_stream, cudaStreamNonBlocking, lo);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->ev_last, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->ev_bulk_last, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_ring, (size_t)cap * sizeof(small_rec), cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_flags, cap, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_done, (size_t)cap * 4, cudaHostAllocMapped);
@@ -2521,6 +2668,13 @@ int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap) {
     }
     q->cv_done.wait(lk);
   }
+}
+
+int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, q->stats, sizeof(q->stats));
+  return HS_OK;
 }
 
 void hs_queue_destroy(hs_queue *q) {

@@ -393,6 +393,15 @@ class VerifyQueue:
         rc = self.lib.hs_queue_wait(self.h, int(ticket), _ptr(words))
         return self._take(ticket, rc, words)
 
+    STATS = ("small_launches", "small_records", "bulk_launches", "bulk_records", "slow_requests", "slow_records")
+
+    def stats(self):
+        """Counters since the queue was created (hs_queue_stats): k_verify_small launches and the records they carried (riders
+        included), k_verify_bulk launches and their records, slow-path requests and their records."""
+        out = (ctypes.c_uint64 * len(self.STATS))()
+        self.engine._check(self.lib.hs_queue_stats(self.h, out), "hs_queue_stats")
+        return dict(zip(self.STATS, (int(x) for x in out)))
+
     def close(self):
         """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""
         if getattr(self, "h", None):

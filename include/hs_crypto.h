@@ -194,7 +194,11 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *     hs_verify_rec128(ctx, &recs[i], 1, modes[i], ..)).
  *   - Device path: only when a committee is registered (hs_committee_register) and every key of the request is in it.  Any
  *     other request is run by the queue's thread through hs_verify_rec128 itself (key cache / generic kernels; a group takes
- *     at most one strict and one batch-eq call): correct, but the slow path.
+ *     at most one strict and one batch-eq call): correct, but the slow path.  The device path has two kernels: requests of
+ *     fewer than 1,002 records (every hs_queue_submit, and smaller groups) share k_verify_small launches, a block per
+ *     signature, on the queue's highest-priority stream; a group of 1,002 records or more (a committee of about 1,500 or
+ *     more) gets a k_verify_bulk launch of its own, a thread per signature, on a second, lower-priority stream, so a vote's
+ *     launch never waits behind it.  Bulk launches do not count against the two small launches in flight.
  *   - Consumption: with a callback, it runs exactly once on the queue's thread (status HS_OK, or HS_ERR_CUDA = reject every
  *     signature of the request; bitmap = n verdict bits, valid during the call) and the ticket is released when it returns.
  *     Without one, the result is kept until ONE hs_queue_poll that reports done, or one hs_queue_wait; both return the
@@ -202,7 +206,7 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *   - hs_committee_register / hs_committee_update / hs_ctx_destroy drain the queue's launches before they touch the tables; a
  *     request submitted after one of them returns is judged against the new committee.
  *   - hs_queue_destroy completes every request in flight (callbacks fire) and joins the thread; hs_ctx_destroy destroys the
- *     queues still attached to the context.  hs_kernel_launches counts the queue's launches. */
+ *     queues still attached to the context.  hs_kernel_launches counts the queue's launches; hs_queue_stats tells them apart. */
 typedef struct hs_queue hs_queue;
 /* Completion callback (a function type: parameters are `hs_queue_cb *`; the parentheses keep the name from reading as a function). */
 typedef void(hs_queue_cb)(void *user, size_t ticket, int status, const uint32_t *bitmap);
@@ -220,6 +224,10 @@ int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const ui
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap);
 /* Blocks until the request is done; consumes the ticket and returns the request's status. */
 int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap);
+/* Counters since hs_queue_create (each a uint64_t): [0] k_verify_small launches, [1] records they carried (riders included),
+ * [2] k_verify_bulk launches, [3] records they carried, [4] slow-path requests, [5] their records. */
+#define HS_QUEUE_STATS 6
+int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

@@ -87,6 +87,14 @@ class VerifyQueue {
     return f;
   }
 
+  // Counters since creation (hs_queue_stats): [0] k_verify_small launches, [1] their records, [2] k_verify_bulk launches,
+  // [3] their records, [4] slow-path requests, [5] their records.
+  std::array<uint64_t, HS_QUEUE_STATS> stats() const {
+    std::array<uint64_t, HS_QUEUE_STATS> s{};
+    e_.check(hs_queue_stats(q_, s.data()), "hs_queue_stats");
+    return s;
+  }
+
  private:
   struct Pending {
     std::promise<std::vector<bool>> promise;

@@ -17,10 +17,10 @@ use super::{HsRec128, HS_OK};
 
 /// Largest certificate sent through the queue: the largest measured size at which one queued request was no slower than the
 /// synchronous calls (strict author verify + verify_batch) — tools/replay_config5.cpp "replica_block", one H100 80GB HBM3 at a
-/// 400 W power limit, p50 over 20 blocks: 502 records (N = 750) 268 us queued vs 303 us synchronous; 668 records (N = 1,000)
-/// 331 us vs 322 us; 6,668 records (N = 10,000) 1,577 us vs 409 us.  Larger certificates use the synchronous batch front ends.
-/// The boundary is not monotone at the small end: 4 records (N = 4) took 162 us queued vs 150 us synchronous; they stay on the
-/// queue, which does not block a runtime worker while they verify.
+/// 400 W power limit, p50 over 20 blocks: 502 records (N = 750) 243 us queued vs 286 us synchronous; 668 records (N = 1,000)
+/// 304 us vs 297 us; 1,002 records (N = 1,500, the queue's bulk kernel) 327 us vs 316 us; 6,668 records (N = 10,000) 728 us
+/// vs 469 us.  Larger certificates use the synchronous batch front ends.  At 4 records (N = 4) the two took 141 us and 142 us;
+/// they stay on the queue, which does not block a runtime worker while they verify.
 pub const GROUP_MAX_SIGS: usize = 502;
 
 #[link(name = "hs_crypto")]

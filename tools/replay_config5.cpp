@@ -19,8 +19,9 @@
 // Replica block (after the burst): one Block::verify certificate = 1 strict author signature + N - f batch-eq QC votes, 1 % of
 // the records corrupted, N = 4 .. 10,000, on a 16,384-record ring.  Three arms per block: (a) one hs_queue_submit_group consumed by
 // hs_queue_wait, (b) the synchronous calls the shim makes today (a strict author verify + hs_verify_batch_shared_msg), (c) the CPU
-// oracle on one core.  Block during a burst: the 1,000-validator vote burst above with one 668-record Block certificate submitted
-// once half the votes are in, (a) through the same queue or (b) as the synchronous calls from another thread.
+// oracle on one core.  Block during a burst: the N-validator vote burst above (N = 1,000 and 10,000) with one Block certificate
+// (668 / 6,668 records) submitted once half the votes are in, (a) through the same queue or (b) as the synchronous calls from
+// another thread.  Every queue section prints the queue's counters (hs_queue_stats): which kernel carried how many records.
 //
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
@@ -244,6 +245,15 @@ static void make_cert(const committee_keys &k, int r, cert &c) {
     if ((((c.modes[i] ? e : s)[i >> 5]) >> (i & 31)) & 1u) c.want[i >> 5] |= 1u << (i & 31);
 }
 static bool bit(const std::vector<uint32_t> &b, int i) { return (b[i >> 5] >> (i & 31)) & 1u; }
+// the queue's counters since `since` (hs_queue_stats), as a JSON object
+static void emit_stats(hs_queue *q, const uint64_t (&since)[HS_QUEUE_STATS]) {
+  static const char *names[HS_QUEUE_STATS] = {"small_launches", "small_records", "bulk_launches", "bulk_records", "slow_requests", "slow_records"};
+  uint64_t s[HS_QUEUE_STATS] = {};
+  hs_queue_stats(q, s);
+  printf("\"queue_stats\": {");
+  for (int i = 0; i < HS_QUEUE_STATS; i++) printf("\"%s\": %llu%s", names[i], (unsigned long long)(s[i] - since[i]), i + 1 < HS_QUEUE_STATS ? ", " : "");
+  printf("}");
+}
 // The synchronous calls the shim makes for one Block today: a strict author verify + one verify_batch over the QC's votes.
 static int sync_block(hs_ctx *ctx, const cert &c, std::vector<uint32_t> &bits) {
   const size_t nv = c.votes.size();
@@ -268,9 +278,10 @@ static int replica_block(hs_ctx *ctx, hs_queue *q, int N, int blocks, bool last)
   std::vector<uint32_t> valid((N + 31) / 32);
   if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
   series qa, sb, cc;
-  uint64_t launches = 0;
+  uint64_t launches = 0, s0[HS_QUEUE_STATS] = {};
   int mism_a = 0, mism_b = 0, bad = 0;
   cert c;
+  hs_queue_stats(q, s0);
   for (int r = 0; r < blocks + 3; r++) {
     const bool timed = r >= 3;
     make_cert(k, r, c);
@@ -306,13 +317,15 @@ static int replica_block(hs_ctx *ctx, hs_queue *q, int N, int blocks, bool last)
   const int nv = N - (N - 1) / 3;
   printf("\"committee_%d\": {\"records\": %d, \"blocks\": %d, \"queue_submit_group\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"launches_per_block\": %.2f, "
          "\"mismatches\": %d}, \"sync_strict_author_plus_verify_batch_shared_msg\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"mismatches\": %d}, "
-         "\"cpu_oracle_1core\": {\"p50_us\": %.1f, \"p99_us\": %.1f}, \"errors\": %d}%s",
-         N, nv + 1, blocks, qa.pct(0.5), qa.pct(0.99), (double)launches / blocks, mism_a, sb.pct(0.5), sb.pct(0.99), mism_b, cc.pct(0.5), cc.pct(0.99), bad,
-         last ? "" : ", ");
+         "\"cpu_oracle_1core\": {\"p50_us\": %.1f, \"p99_us\": %.1f}, \"errors\": %d, ",
+         N, nv + 1, blocks, qa.pct(0.5), qa.pct(0.99), (double)launches / blocks, mism_a, sb.pct(0.5), sb.pct(0.99), mism_b, cc.pct(0.5), cc.pct(0.99), bad);
+  emit_stats(q, s0);  // warm-up blocks included
+  printf("}%s", last ? "" : ", ");
   return mism_a + mism_b + bad;
 }
 
-// ---- a Block certificate submitted in the middle of the leader's vote burst (N = 1,000: 667 votes + a 668-record Block)
+// ---- a Block certificate submitted in the middle of the leader's vote burst (N = 1,000: 667 votes + a 668-record Block;
+// N = 10,000: 6,667 votes + a 6,668-record Block, on a ring of `ring` records)
 struct blk_done {
   clk::time_point t0;
   double lat;
@@ -326,13 +339,13 @@ static void on_block(void *user, size_t, int status, const uint32_t *bitmap) {
   else std::fill(b->bits.begin(), b->bits.end(), 0u);
   b->done.store(status == HS_OK ? 1 : -1, std::memory_order_release);
 }
-static int block_during_burst(hs_ctx *ctx, int bursts) {
-  const int N = 1000, f = (N - 1) / 3, nv = N - f, nth = 16;
+static int block_during_burst(hs_ctx *ctx, int N, size_t ring, int bursts, bool last) {
+  const int f = (N - 1) / 3, nv = N - f, nth = 16;
   const committee_keys k = make_keys(N, 23);
   std::vector<uint32_t> valid((N + 31) / 32);
   if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
   hs_queue *q = nullptr;
-  if (hs_queue_create(ctx, 0, &q) != HS_OK) return 1;
+  if (hs_queue_create(ctx, ring, &q) != HS_OK) return 1;
   burst_arm arm[2];
   series blk[2];
   int blk_bad[2] = {0, 0};
@@ -410,14 +423,17 @@ static int block_during_burst(hs_ctx *ctx, int bursts) {
       }
     }
   }
-  hs_queue_destroy(q);
-  printf("\"votes\": %d, \"block_records\": %zu, \"bursts\": %d, ", nv, c.recs.size(), bursts);
+  printf("\"committee_%d\": {\"ring_records\": %zu, \"votes\": %d, \"block_records\": %zu, \"bursts\": %d, ", N, ring, nv, c.recs.size(), bursts);
   const char *names[2] = {"block_via_queue_submit_group", "block_via_synchronous_calls_other_thread"};
   for (int a = 0; a < 2; a++) {
     printf("\"%s\": {\"block_p50_us\": %.1f, \"block_p99_us\": %.1f, \"block_mismatches\": %d, ", names[a], blk[a].pct(0.5), blk[a].pct(0.99), blk_bad[a]);
     arm[a].emit("votes", bursts, true);
-    printf("}%s", a ? "" : ", ");
+    printf("}, ");
   }
+  const uint64_t zero[HS_QUEUE_STATS] = {};
+  emit_stats(q, zero);  // both arms' votes and the queued blocks, warm-up bursts included
+  printf("}%s", last ? "" : ", ");
+  hs_queue_destroy(q);
   return arm[0].mismatches + arm[1].mismatches + blk_bad[0] + blk_bad[1];
 }
 static std::string gpu_identity() {  // name and enforced power limit, read in the same run
@@ -545,10 +561,11 @@ int main(int argc, char **argv) {
   printf("}, \"replica_block\": {\"gpu\": \"%s\", \"ring_records\": 16384, ", gpu_identity().c_str());
   hs_queue *q = nullptr;
   if (hs_queue_create(ctx, 16384, &q) != HS_OK) return 1;
-  for (int N : {4, 100, 250, 500, 750, 1000, 10000}) burst_bad += replica_block(ctx, q, N, bursts, N == 10000);
+  for (int N : {4, 100, 250, 500, 750, 1000, 1500, 3000, 6000, 10000}) burst_bad += replica_block(ctx, q, N, bursts, N == 10000);
   hs_queue_destroy(q);
   printf("}, \"block_during_burst\": {\"gpu\": \"%s\", \"threads\": 16, ", gpu_identity().c_str());
-  burst_bad += block_during_burst(ctx, bursts);
+  burst_bad += block_during_burst(ctx, 1000, 0, bursts, false);
+  burst_bad += block_during_burst(ctx, 10000, 16384, bursts, true);
   printf("}}\n");
   hs_ctx_destroy(ctx);
   return (bad || burst_bad) ? 9 : 0;

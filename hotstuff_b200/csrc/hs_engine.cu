@@ -721,6 +721,55 @@ __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restri
   dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
 }
 
+// Verify queue requests that carry signed preimages instead of Digests (hs_queue_submit_msgs).  A request's region of the queue's
+// mapped arena is pre_off[m + 1] (u64, relative to the preimage bytes) | msg_idx[n] (u32) | the m preimages, each section 16-byte
+// aligned.  The host keeps only the preimages some record names, so each of the m is hashed once.
+struct qmsg_desc {
+  uint32_t off;        // arena offset of the request's region (16-byte aligned)
+  uint32_t m;          // preimages
+  uint32_t n;          // records
+  uint32_t base;       // ring slot of record 0: record i is slot (base + i) & mask
+  uint32_t pre_bytes;  // preimage bytes
+  uint32_t pad[3];
+};
+static_assert(sizeof(qmsg_desc) == 32, "qmsg_desc is 32 bytes");
+__host__ __device__ inline uint64_t qmsg_o_pre(uint64_t m, uint64_t n) { return (8 * (m + 1) + 4 * n + 15) & ~(uint64_t)15; }
+__host__ __device__ inline uint64_t qmsg_bytes(uint64_t m, uint64_t n, uint64_t pre_bytes) { return qmsg_o_pre(m, n) + ((pre_bytes + 15) & ~(uint64_t)15); }
+// One block per preimage request of the launch that follows on the same stream; its descriptor is list[(first + blockIdx.x) & mask].
+// The region crosses the bus once (coalesced 16-byte loads into `stage`, the arena's device mirror), each preimage is hashed once
+// into the request's digest slots (digs: 32 bytes per 8 arena bytes, so concurrent requests never share one), and every record's
+// 32-byte Digest is stored into the msg field of its ring record, where the verify kernel reads it.
+#define HS_QDIG_THREADS 256
+__global__ void __launch_bounds__(HS_QDIG_THREADS) k_queue_digests(const qmsg_desc *__restrict__ list, uint32_t first, uint32_t mask,
+                                                                    const uint8_t *__restrict__ arena, uint8_t *stage, uint32_t *digs, small_rec *ring) {
+  const qmsg_desc d = list[(first + blockIdx.x) & mask];
+  const uint32_t words = (uint32_t)(qmsg_bytes(d.m, d.n, d.pre_bytes) / 16);
+  const uint4 *src = reinterpret_cast<const uint4 *>(arena + d.off);
+  uint4 *dst = reinterpret_cast<uint4 *>(stage + d.off);
+  for (uint32_t k = threadIdx.x; k < words; k += HS_QDIG_THREADS) dst[k] = src[k];
+  __syncthreads();
+  const uint64_t *pre_off = reinterpret_cast<const uint64_t *>(stage + d.off);
+  const uint32_t *msg_idx = reinterpret_cast<const uint32_t *>(stage + d.off + 8 * ((size_t)d.m + 1));
+  const uint8_t *pre = stage + d.off + qmsg_o_pre(d.m, d.n);
+  uint32_t *dig = digs + (size_t)(d.off / 8) * 8;
+#pragma unroll 1
+  for (uint32_t j = threadIdx.x; j < d.m; j += HS_QDIG_THREADS) {
+    uint32_t h[16];
+    const uint64_t none[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    sha512_prefix_msg(h, none, 0, pre + pre_off[j], pre_off[j + 1] - pre_off[j]);
+    uint4 *o = reinterpret_cast<uint4 *>(dig + (size_t)j * 8);
+    o[0] = make_uint4(h[0], h[1], h[2], h[3]);
+    o[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  }
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < d.n; i += HS_QDIG_THREADS) {
+    const uint4 *s = reinterpret_cast<const uint4 *>(dig + (size_t)msg_idx[i] * 8);
+    uint4 *r = reinterpret_cast<uint4 *>(ring[(d.base + i) & mask].msg);
+    r[0] = s[0];
+    r[1] = s[1];
+  }
+}
+
 // Fixed-size, 16-byte aligned messages (the transaction / payload shape of BASELINE config[1]): every full 128-byte block is
 // fetched by the warp with coalesced 16-byte loads through shared memory (a per-thread 8-byte walk touches 32 sectors per
 // load instruction), and when the length is a multiple of 128 the padding-only last block runs without its message
@@ -1295,6 +1344,9 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
 // block per signature (1,002 records, N = 1,500: 345 vs 375 us p50; at 668 records 307 vs 298 us; DESIGN.md §5d).
 #define HS_QUEUE_BULK_MIN 1002
 static_assert(HS_QUEUE_BULK_MIN > HS_SMALL_MAX, "small requests never take the bulk path");
+// Preimage arena bytes per ring record: a full ring of 16-byte TC preimages with their offsets and indices (28 bytes a record), or
+// a Block preimage with about a thousand payload digests.
+#define HS_QUEUE_ARENA_PER_RECORD 64u
 // A request's verdict bitmap: inline for <= 64 records (every small request), on the heap only for larger groups.
 struct queue_bits {
   uint32_t inl[(HS_SMALL_MAX + 31) / 32] = {0, 0};
@@ -1327,6 +1379,16 @@ struct hs_queue {
   cudaEvent_t ev_last = nullptr;                   // recorded after every launch on `stream`: the ring is freed only after it
   cudaEvent_t ev_bulk_last = nullptr;              // the same for `bulk_stream`
   uint64_t stats[HS_QUEUE_STATS] = {};             // hs_queue_stats
+  // preimage requests (hs_queue_submit_msgs): a byte arena of HS_QUEUE_ARENA_PER_RECORD x cap bytes, positions growing without
+  // bound like the ring's ([a_head, a_tail) in use, offset = position & (acap - 1)); a request's region is contiguous (one that
+  // would cross the arena's end starts at its beginning) and is released with its ring slots
+  uint32_t acap = 0;
+  uint8_t *h_arena = nullptr, *d_arena = nullptr;  // mapped pinned: the requests' regions (layout: qmsg_desc)
+  uint8_t *d_stage = nullptr;                      // device: k_queue_digests' copy of the arena (same offsets)
+  uint32_t *d_digs = nullptr;                      // device: digest slots, 32 bytes per 8 arena bytes
+  qmsg_desc *h_mlist = nullptr, *d_mlist = nullptr;  // mapped pinned: a launch's descriptors at the ring slots of its range
+  uint64_t a_head = 0, a_tail = 0;
+  uint64_t dstats[HS_QUEUE_DIGEST_STATS] = {};     // hs_queue_digest_stats
   struct req {
     size_t ticket;
     uint32_t n;
@@ -1334,6 +1396,9 @@ struct hs_queue {
     void *user;
     uint32_t seq;   // launch that verifies it (0: slow path)
     bool finished;
+    bool msgs;           // a preimage request: its records' Digests are computed by k_queue_digests
+    uint32_t a_off, m, pre_bytes;  // its arena region: offset, preimages, preimage bytes
+    uint64_t a_end;      // arena position past its region (0: none)
   };
   std::vector<req> reqs;  // by request slot
   struct result {
@@ -1374,6 +1439,7 @@ static void queue_release_locked(hs_queue *q) {
     hs_queue::req &h = q->reqs[q->head & q->mask];
     h.finished = false;
     q->head += h.n;
+    q->a_head = std::max(q->a_head, h.a_end);
   }
 }
 // Marks the request at ring position p finished (under q->mu): a polled ticket's result is parked, a callback is returned to be
@@ -1411,6 +1477,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   std::vector<queue_completion> fire;
   std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one, in ring order
   std::vector<char> ok;                // runs launched without a CUDA error (the first failure stops the rest)
+  uint64_t dig_launched[3] = {0, 0, 0};  // k_queue_digests launches, their preimages and preimage bytes (hs_queue_digest_stats)
   cudaError_t e = cudaSuccess;
   {
     std::lock_guard<std::mutex> g(c->mu);
@@ -1454,16 +1521,38 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         hs_queue::launch &L = runs[k];
         if (L.bulk != (pass == 1)) continue;
         L.seq = ++q->seq ? q->seq : ++q->seq;  // never 0
-        for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n)
-          if (q->reqs[p & q->mask].seq) q->reqs[p & q->mask].seq = L.seq;
+        uint32_t n_msgs_req = 0;  // the run's device-path preimage requests (slow-path riders carry no digest)
+        uint64_t n_pre = 0, n_pre_bytes = 0;
+        for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n) {
+          hs_queue::req &r = q->reqs[p & q->mask];
+          if (!r.seq) continue;
+          r.seq = L.seq;
+          if (!r.msgs) continue;
+          q->h_mlist[(L.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
+          n_pre += r.m;
+          n_pre_bytes += r.pre_bytes;
+        }
         const uint32_t n = (uint32_t)(L.hi - L.lo), base = (uint32_t)(L.lo & q->mask);
-        if (L.bulk)
-          k_verify_bulk<<<(n + HS_BULK_THREADS - 1) / HS_BULK_THREADS, HS_BULK_THREADS, 0, q->bulk_stream>>>(
-              q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
-        else
-          k_verify_small<<<n, 64, 0, q->stream>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
-        c->launches++;
-        e = cudaGetLastError();
+        cudaStream_t s = L.bulk ? q->bulk_stream : q->stream;
+        if (n_msgs_req) {  // the Digests first, on the verify launch's stream
+          k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, s>>>(q->d_mlist, base, q->mask, q->d_arena, q->d_stage, q->d_digs, q->d_ring);
+          c->launches++;
+          e = cudaGetLastError();
+          if (e == cudaSuccess) {
+            dig_launched[0]++;
+            dig_launched[1] += n_pre;
+            dig_launched[2] += n_pre_bytes;
+          }
+        }
+        if (e == cudaSuccess) {
+          if (L.bulk)
+            k_verify_bulk<<<(n + HS_BULK_THREADS - 1) / HS_BULK_THREADS, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp,
+                                                                                                  q->d_flags, q->d_counters, q->d_done, L.seq);
+          else
+            k_verify_small<<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
+          c->launches++;
+          e = cudaGetLastError();
+        }
         if (e == cudaSuccess) e = L.bulk ? cudaEventRecord(q->ev_bulk_last, q->bulk_stream) : cudaEventRecord(q->ev_last, q->stream);
         if (e != cudaSuccess) {
           fail(c, HS_ERR_CUDA, "verify queue launch", e);
@@ -1479,6 +1568,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       q->stats[4]++;
       q->stats[5] += q->reqs[p & q->mask].n;
     }
+    for (int i = 0; i < 3; i++) q->dstats[i] += dig_launched[i];
     for (size_t k = 0; k < runs.size(); k++) {
       const hs_queue::launch &L = runs[k];
       if (ok[k]) {
@@ -1496,11 +1586,28 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   // present in the request (a small request has one mode; a Block group has a strict pass and a batch-eq pass)
   std::vector<hs_rec128> recs;
   std::vector<uint32_t> idx, part;
+  std::vector<uint8_t> msig, mpk, mmode;
   for (uint64_t p : slow) {
     const hs_queue::req &r = q->reqs[p & q->mask];
     std::fill(q->wbits.begin(), q->wbits.begin() + (r.n + 31) / 32, 0u);
     int rc = HS_OK;
-    for (uint32_t mode = HS_MODE_STRICT; mode <= HS_MODE_BATCH_EQ && rc == HS_OK; mode++) {
+    if (r.msgs) {  // a preimage request: one hs_verify_groups call, the request as one group with per-item modes
+      msig.resize((size_t)r.n * 64);
+      mpk.resize((size_t)r.n * 32);
+      mmode.resize(r.n);
+      idx.assign(r.n, 0);  // group_idx
+      for (uint32_t i = 0; i < r.n; i++) {
+        const uint32_t s = (uint32_t)((p + i) & q->mask);
+        memcpy(&msig[(size_t)i * 64], q->h_ring[s].sig, 64);
+        memcpy(&mpk[(size_t)i * 32], q->pk.data() + 32 * (size_t)s, 32);
+        mmode[i] = q->modes[s];
+      }
+      const uint8_t *a = q->h_arena + r.a_off;
+      uint32_t group_bit = 0;
+      rc = hs_verify_groups(c, a + qmsg_o_pre(r.m, r.n), reinterpret_cast<const uint64_t *>(a), r.m, msig.data(), mpk.data(), nullptr,
+                            reinterpret_cast<const uint32_t *>(a + 8 * ((size_t)r.m + 1)), idx.data(), mmode.data(), r.n, 1, q->wbits.data(), &group_bit);
+    }
+    for (uint32_t mode = HS_MODE_STRICT; mode <= HS_MODE_BATCH_EQ && rc == HS_OK && !r.msgs; mode++) {
       recs.clear();
       idx.clear();
       for (uint32_t i = 0; i < r.n; i++) {
@@ -1623,7 +1730,11 @@ static void queue_free(hs_queue *q) {
   if (q->h_ring) cudaFreeHost(q->h_ring);
   if (q->h_flags) cudaFreeHost(q->h_flags);
   if (q->h_done) cudaFreeHost(q->h_done);
+  if (q->h_arena) cudaFreeHost(q->h_arena);
+  if (q->h_mlist) cudaFreeHost(q->h_mlist);
   cudaFree(q->d_counters);
+  cudaFree(q->d_stage);
+  cudaFree(q->d_digs);
   delete q;
 }
 
@@ -2567,6 +2678,7 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   q->c = c;
   q->cap = cap;
   q->mask = cap - 1;
+  q->acap = cap * HS_QUEUE_ARENA_PER_RECORD;
   q->pk.assign((size_t)cap * 32, 0);
   q->modes.assign(cap, 0);
   q->wbits.assign(cap / 32, 0);
@@ -2582,9 +2694,15 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_done, (size_t)cap * 4, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaMalloc(&q->d_counters, (size_t)cap * 4);
   if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_arena, q->acap, cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_mlist, (size_t)cap * sizeof(qmsg_desc), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_stage, q->acap);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_digs, (size_t)q->acap * 4);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_ring, q->h_ring, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_flags, q->h_flags, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_done, q->h_done, 0);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_arena, q->h_arena, 0);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_mlist, q->h_mlist, 0);
   if (e != cudaSuccess) {
     queue_free(q);
     return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
@@ -2641,6 +2759,67 @@ int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const ui
   return queue_enqueue(q, "hs_queue_submit_group", recs, n, HS_MODE_STRICT, modes, cb, user, out_ticket);
 }
 
+int hs_queue_submit_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                         const uint32_t *msg_idx, const uint8_t *modes, size_t n, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !pre_off || !sig || !pk || !msg_idx || n == 0 || n > q->cap || n_msgs == 0)
+    return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_msgs: bad argument");
+  if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages)) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: bad preimage offsets");
+  for (size_t i = 0; i < n; i++)
+    if (msg_idx[i] >= n_msgs || (modes && modes[i] > HS_MODE_BATCH_EQ)) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: index or mode out of range");
+  // keep only the preimages some record names, in their order: remap[j] = new index of preimage j
+  std::vector<uint32_t> remap(n_msgs, HS_NO_KEY);
+  for (size_t i = 0; i < n; i++) remap[msg_idx[i]] = 0;
+  uint32_t m = 0;
+  uint64_t pre_bytes = 0;
+  for (size_t j = 0; j < n_msgs; j++)
+    if (remap[j] == 0) {
+      remap[j] = m++;
+      pre_bytes += pre_off[j + 1] - pre_off[j];
+    }
+  const uint64_t size = qmsg_bytes(m, n, pre_bytes);
+  if (size > q->acap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more preimage bytes than the queue's arena holds");
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: queue is being destroyed");
+    uint64_t start = q->a_tail;
+    if ((start & (q->acap - 1)) + size > q->acap) start += q->acap - (start & (q->acap - 1));  // would cross the end: start over
+    if (start + size - q->a_head > q->acap) {  // arena full
+      if (q->a_head != q->a_tail) return HS_ERR_NOMEM;
+      start = q->a_head = q->a_tail = start;  // empty: the skipped tail is free too
+    }
+    if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
+    uint8_t *a = q->h_arena + (start & (q->acap - 1));
+    uint64_t *off = reinterpret_cast<uint64_t *>(a);
+    uint32_t *idx = reinterpret_cast<uint32_t *>(a + 8 * ((size_t)m + 1));
+    uint8_t *pre = a + qmsg_o_pre(m, n);
+    off[0] = 0;
+    for (size_t j = 0, k = 0; j < n_msgs; j++)
+      if (remap[j] != HS_NO_KEY) {
+        const uint64_t len = pre_off[j + 1] - pre_off[j];
+        if (len) memcpy(pre + off[k], preimages + pre_off[j], len);
+        off[k + 1] = off[k] + len;
+        k++;
+      }
+    for (size_t i = 0; i < n; i++) {
+      const uint32_t s = (uint32_t)((q->tail + i) & q->mask);
+      memcpy(q->h_ring[s].sig, sig + 64 * i, 64);
+      memcpy(q->pk.data() + 32 * (size_t)s, pk + 32 * i, 32);
+      q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
+      idx[i] = remap[msg_idx[i]];
+    }
+    const size_t ticket = q->next_ticket++;
+    q->reqs[q->tail & q->mask] =
+        hs_queue::req{ticket, (uint32_t)n, cb, user, 0, false, true, (uint32_t)(start & (q->acap - 1)), m, (uint32_t)pre_bytes, start + size};
+    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
+    q->tail += n;
+    q->a_tail = start + size;
+    q->dstats[3]++;
+    if (out_ticket) *out_ticket = ticket;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap) {
   if (!q || !done || !out_bitmap) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_poll: bad argument");
   std::lock_guard<std::mutex> g(q->mu);
@@ -2674,6 +2853,13 @@ int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]) {
   if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_stats: bad argument");
   std::lock_guard<std::mutex> g(q->mu);
   memcpy(out, q->stats, sizeof(q->stats));
+  return HS_OK;
+}
+
+int hs_queue_digest_stats(hs_queue *q, uint64_t out[HS_QUEUE_DIGEST_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_digest_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, q->dstats, sizeof(q->dstats));
   return HS_OK;
 }
 

@@ -303,7 +303,8 @@ class Engine:
 
 
 class VerifyQueue:
-    """hs_queue_* (include/hs_crypto.h): submit 1..64 records (submit) or a whole certificate (submit_group) without blocking;
+    """hs_queue_* (include/hs_crypto.h): submit 1..64 records (submit) or a whole certificate (submit_group, or submit_msgs with the
+    signed preimages instead of their Digests) without blocking;
     a dispatcher thread coalesces whatever is pending into one latency-path launch.  Verdicts equal Engine.verify_rec128 on the
     same records (per record and its mode for a group).  A ticket is read once:
     by poll() / wait(), or by the callback given to submit() (called on the queue's thread as callback(ticket, status, bools);
@@ -343,13 +344,36 @@ class VerifyQueue:
                 raise ValueError("submit_group: %d modes for %d records" % (modes.shape[0], recs.shape[0]))
         return self._submit(self.lib.hs_queue_submit_group, "hs_queue_submit_group", recs, None if modes is None else _ptr(modes), callback)
 
+    def submit_msgs(self, preimages, pre_off, sig, pk, msg_idx, modes=None, callback=None):
+        """One consensus message's signatures as ONE request with the signed preimages instead of their Digests (hs_queue_submit_msgs):
+        record i is (sig[i], pk[i]) over SHA-512(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1]))[..32], hashed on the
+        GPU, judged by modes[i] (None = all strict) — the arrays wire.ingest_frames returns for one frame.  Returns the ticket, or None
+        when the ring or the preimage arena has no room now (verify synchronously)."""
+        pre = _u8(preimages)
+        off = np.ascontiguousarray(pre_off, dtype=np.uint64).reshape(-1)
+        sig = _u8(sig, 64).reshape(-1, 64)
+        pk = _u8(pk, 32).reshape(-1, 32)
+        mi = np.ascontiguousarray(msg_idx, dtype=np.uint32).reshape(-1)
+        n = sig.shape[0]
+        mo = None if modes is None else np.ascontiguousarray(modes, dtype=np.uint8).reshape(-1)
+        if pk.shape[0] != n or mi.shape[0] != n or (mo is not None and mo.shape[0] != n) or off.shape[0] < 1:
+            raise ValueError("submit_msgs: %d signatures, %d keys, %d message indices, %s modes, %d offsets"
+                             % (n, pk.shape[0], mi.shape[0], "no" if mo is None else mo.shape[0], off.shape[0]))
+        return self._enqueue("hs_queue_submit_msgs", n, callback, lambda cb, user, t: self.lib.hs_queue_submit_msgs(
+            self.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk) if n else None,
+            _ptr(mi) if n else None, _ptr(mo), n, cb, user, t))
+
     def _submit(self, fn, name, recs, mode_arg, callback):
         recs = _u8(recs, 128).reshape(-1, 128)
         n = recs.shape[0]
+        return self._enqueue(name, n, callback, lambda cb, user, t: fn(self.h, _ptr(recs), n, mode_arg, cb, user, t))
+
+    def _enqueue(self, name, n, callback, call):
+        """call(callback pointer or None, user id or None, ticket out-pointer) -> status."""
         t = ctypes.c_size_t(0)
         if callback is None:
             with self._lock:  # registered first: poll / wait from another thread may race the return
-                rc = fn(self.h, _ptr(recs), n, mode_arg, None, None, ctypes.byref(t))
+                rc = call(None, None, ctypes.byref(t))
                 if rc == 0:
                     self._n[t.value] = n
         else:
@@ -357,7 +381,7 @@ class VerifyQueue:
                 uid = self._next_id
                 self._next_id += 1
                 self._callbacks[uid] = (callback, n)
-            rc = fn(self.h, _ptr(recs), n, mode_arg, ctypes.cast(self._trampoline, ctypes.c_void_p), uid, ctypes.byref(t))
+            rc = call(ctypes.cast(self._trampoline, ctypes.c_void_p), uid, ctypes.byref(t))
             if rc != 0:
                 with self._lock:
                     self._callbacks.pop(uid, None)
@@ -401,6 +425,15 @@ class VerifyQueue:
         out = (ctypes.c_uint64 * len(self.STATS))()
         self.engine._check(self.lib.hs_queue_stats(self.h, out), "hs_queue_stats")
         return dict(zip(self.STATS, (int(x) for x in out)))
+
+    DIGEST_STATS = ("digest_launches", "preimages", "preimage_bytes", "msgs_requests")
+
+    def digest_stats(self):
+        """Counters since the queue was created (hs_queue_digest_stats): k_queue_digests launches, the preimages and preimage bytes
+        they hashed, and the submit_msgs requests."""
+        out = (ctypes.c_uint64 * len(self.DIGEST_STATS))()
+        self.engine._check(self.lib.hs_queue_digest_stats(self.h, out), "hs_queue_digest_stats")
+        return dict(zip(self.DIGEST_STATS, (int(x) for x in out)))
 
     def close(self):
         """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""

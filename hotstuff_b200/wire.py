@@ -51,6 +51,17 @@ def ingest_frames(frames):
     raise RuntimeError("ingest capacity retry failed")
 
 
+def submit_frame(queue, frame, callback=None):
+    """Ingests ONE frame and submits every signature in it to a VerifyQueue as one request (VerifyQueue.submit_msgs, preimages
+    hashed on the GPU).  Returns None when the frame carries no signature (a SyncRequest, a malformed frame: nothing is submitted),
+    else (info, ticket): info is the frame's FRAME_INFO, ticket None when the queue has no room now.  The verdicts are per item in
+    ingest order; the frame's certificates hold iff they all do.  The stake / duplicate pre-checks stay with the caller."""
+    g = ingest_frames([frame])
+    if len(g["sig"]) == 0:
+        return None
+    return g["info"][0], queue.submit_msgs(g["preimages"], g["pre_off"], g["sig"], g["pk"], g["msg_idx"], modes=g["mode"], callback=callback)
+
+
 def verify_frames(frames, committee, engine):
     """Ingest + the reference's pre-checks + ONE engine pass.  Returns a list: None (valid), "Malformed", or the ConsensusError name
     the reference would raise first (same order as messages.verify_blocks).  SyncRequest frames are None (nothing to verify)."""

@@ -190,6 +190,10 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *     record.  It shares the ring, the dispatcher and the launches with small requests: a group whose keys are all registered
  *     costs one launch when nothing else is pending.  HS_ERR_NOMEM here means "verify it through the synchronous entry points
  *     now".
+ *   - hs_queue_submit_msgs takes the same request with the signed preimages instead of their Digests (the arrays
+ *     hs_ingest_consensus_frames writes for one frame), so the caller hashes nothing: the preimages go into a mapped arena beside
+ *     the ring (64 bytes per ring record) and one k_queue_digests launch ahead of the verify launch, on the same stream, hashes each
+ *     distinct preimage once and writes every record's Digest into the ring.  A lone device-path request costs two launches.
  *   - Verdicts equal hs_verify_rec128(ctx, recs, n, mode, ..) on the same records, bit for bit (for a group: record i equals
  *     hs_verify_rec128(ctx, &recs[i], 1, modes[i], ..)).
  *   - Device path: only when a committee is registered (hs_committee_register) and every key of the request is in it.  Any
@@ -220,6 +224,15 @@ int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode,
  * bitmap holds n bits (poll / wait: (n + 31) / 32 words). */
 int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const uint8_t *modes_or_null, hs_queue_cb *cb_or_null, void *user,
                           size_t *out_ticket);
+/* One consensus message's signatures as ONE queue request, with the signed preimages instead of their Digests: record i is
+ * (sig[i], pk[i]) over Digest(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1])) = SHA-512(..)[..32], hashed ON THE GPU,
+ * judged by modes[i] (HS_MODE_*; NULL = all strict).  Exactly the arrays hs_ingest_consensus_frames writes for one frame.
+ * n = 1 .. ring capacity, n_msgs >= 1 (a preimage no record names is not hashed).  HS_ERR_ARG: bad sizes / offsets, msg_idx[i] >= n_msgs, a mode byte > 1, or more
+ * preimage bytes than the queue's preimage arena holds (64 bytes per ring record, offsets and indices included).  HS_ERR_NOMEM: no
+ * ring or arena room right now (back-pressure).  Completion, tickets, poll / wait / callback exactly as hs_queue_submit_group. */
+int hs_queue_submit_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off /* n_msgs + 1 */, size_t n_msgs,
+                         const uint8_t *sig /* n x 64 */, const uint8_t *pk /* n x 32 */, const uint32_t *msg_idx /* n */,
+                         const uint8_t *modes_or_null, size_t n, hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
 /* Non-blocking: *done = 0 (come back later) or 1 (out_bitmap holds the verdicts, ticket consumed, returns the request's status). */
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap);
 /* Blocks until the request is done; consumes the ticket and returns the request's status. */
@@ -228,6 +241,9 @@ int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap);
  * [2] k_verify_bulk launches, [3] records they carried, [4] slow-path requests, [5] their records. */
 #define HS_QUEUE_STATS 6
 int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]);
+/* [0] k_queue_digests launches, [1] preimages hashed, [2] preimage bytes hashed, [3] hs_queue_submit_msgs requests. */
+#define HS_QUEUE_DIGEST_STATS 4
+int hs_queue_digest_stats(hs_queue *q, uint64_t out[HS_QUEUE_DIGEST_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

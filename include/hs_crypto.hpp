@@ -87,11 +87,33 @@ class VerifyQueue {
     return f;
   }
 
+  // The same with the signed preimages instead of their Digests (hs_queue_submit_msgs): record i is (sig[i], pk[i]) over
+  // Digest(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1])), hashed on the GPU — the arrays hs_ingest_consensus_frames
+  // writes for one frame.  Throws QueueFull when the ring or the preimage arena has no room now, EngineError on a bad argument.
+  std::future<std::vector<bool>> submit_msgs(const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                                             const uint32_t *msg_idx, size_t n, const uint8_t *modes = nullptr) {
+    auto *p = new Pending{std::promise<std::vector<bool>>(), n};
+    std::future<std::vector<bool>> f = p->promise.get_future();
+    const int rc = hs_queue_submit_msgs(q_, preimages, pre_off, n_msgs, sig, pk, msg_idx, modes, n, &VerifyQueue::done, p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit_msgs");
+    }
+    return f;
+  }
+
   // Counters since creation (hs_queue_stats): [0] k_verify_small launches, [1] their records, [2] k_verify_bulk launches,
   // [3] their records, [4] slow-path requests, [5] their records.
   std::array<uint64_t, HS_QUEUE_STATS> stats() const {
     std::array<uint64_t, HS_QUEUE_STATS> s{};
     e_.check(hs_queue_stats(q_, s.data()), "hs_queue_stats");
+    return s;
+  }
+  // hs_queue_digest_stats: [0] k_queue_digests launches, [1] preimages hashed, [2] their bytes, [3] submit_msgs requests.
+  std::array<uint64_t, HS_QUEUE_DIGEST_STATS> digest_stats() const {
+    std::array<uint64_t, HS_QUEUE_DIGEST_STATS> s{};
+    e_.check(hs_queue_digest_stats(q_, s.data()), "hs_queue_digest_stats");
     return s;
   }
 

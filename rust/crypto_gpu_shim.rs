@@ -21,6 +21,10 @@ pub mod queue;
 /// (`group_queue::verify_group_queued`).
 #[path = "crypto_gpu_group_queue.rs"]
 pub mod group_queue;
+/// The same with the signed preimages instead of their Digests (hs_queue_submit_msgs): the GPU hashes them, so a TC's votes cost
+/// the connection task no SHA-512 calls (`msgs_queue::verify_msgs_queued`).
+#[path = "crypto_gpu_msgs_queue.rs"]
+pub mod msgs_queue;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

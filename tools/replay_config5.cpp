@@ -23,6 +23,10 @@
 // (668 / 6,668 records) submitted once half the votes are in, (a) through the same queue or (b) as the synchronous calls from
 // another thread.  Every queue section prints the queue's counters (hs_queue_stats): which kernel carried how many records.
 //
+// Certificate preimages (last; alone with argv[3] = certificate_preimages): a TC and a Block with a TC, N = 4 .. 750, verified
+// (a) by hashing the preimages on the caller's thread then hs_queue_submit_group, (b) by hs_queue_submit_msgs (the GPU hashes them),
+// (c) synchronously; latency and the caller thread's CPU time per certificate, plus hs_queue_digest_stats.
+//
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
 #include <atomic>
@@ -30,6 +34,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <ctime>
 #include <string>
 #include <thread>
 #include <vector>
@@ -436,6 +441,162 @@ static int block_during_burst(hs_ctx *ctx, int N, size_t ring, int bursts, bool 
   hs_queue_destroy(q);
   return arm[0].mismatches + arm[1].mismatches + blk_bad[0] + blk_bad[1];
 }
+// ---- certificate preimages: a TC (N - f strict votes, each over its own 16-byte preimage tc.round || high_qc_round) and a Block
+// with a TC (strict author over the Block preimage, N - f batch-eq QC votes over one 40-byte preimage, N - f strict TC votes), 1 %
+// of the signatures corrupted.  Three arms per certificate, timed from the start of the caller's work to the verdict:
+//   (a) the caller hashes every distinct preimage on its own thread (hso_digest32: the oracle's C restatement of SHA-512, not the
+//       reference's sha2 crate), packs hs_rec128 records and calls hs_queue_submit_group + hs_queue_wait (the queue path until now);
+//   (b) hs_queue_submit_msgs with the preimages + hs_queue_wait (the Digests are computed by k_queue_digests);
+//   (c) the synchronous hs_verify_tcs (TC) / hs_verify_groups (Block).
+// CPU time of the caller's thread per certificate: CLOCK_THREAD_CPUTIME_ID over a back-to-back pass of 400 certificates per arm.
+struct pre_cert {
+  std::vector<uint8_t> pre, sig, pk, modes;
+  std::vector<uint64_t> off, hq;  // hq: high_qc_round per TC vote (the TC shape only)
+  std::vector<uint32_t> midx, want;
+  uint64_t tc_round = 0;
+};
+static double thread_cpu_us() {
+  timespec ts;
+  clock_gettime(CLOCK_THREAD_CPUTIME_ID, &ts);
+  return ts.tv_sec * 1e6 + ts.tv_nsec / 1e3;
+}
+static void make_pre_cert(const committee_keys &k, int r, bool block, pre_cert &c) {
+  const int N = k.N, nv = N - (N - 1) / 3;
+  c = pre_cert{};
+  c.tc_round = 7000 + (uint64_t)r;
+  auto add_pre = [&](const uint8_t *p, size_t len) {
+    c.pre.insert(c.pre.end(), p, p + len);
+    c.off.push_back(c.pre.size());
+  };
+  c.off.push_back(0);
+  std::vector<uint32_t> key;
+  if (block) {
+    uint8_t bp[32 + 8 + 64 + 32], qp[40];  // Block::digest preimage (author, round, payload digests, qc hash), QC digest preimage
+    for (size_t j = 0; j < sizeof(bp); j++) bp[j] = (uint8_t)(r * 5 + j * 11 + 3);
+    for (size_t j = 0; j < sizeof(qp); j++) qp[j] = (uint8_t)(r * 7 + j * 13 + 1);
+    add_pre(bp, sizeof(bp));
+    add_pre(qp, sizeof(qp));
+    key.push_back((uint32_t)(r % N));
+    c.midx.push_back(0);
+    c.modes.push_back(HS_MODE_STRICT);
+    for (int i = 0; i < nv; i++) {
+      key.push_back((uint32_t)((i * 7 + r) % N));
+      c.midx.push_back(1);
+      c.modes.push_back(HS_MODE_BATCH_EQ);
+    }
+  }
+  for (int i = 0; i < nv; i++) {  // the TC's votes
+    const uint64_t hq = c.tc_round - 1 - (uint64_t)((i * 3 + r) % 5);
+    uint8_t tp[16];
+    memcpy(tp, &c.tc_round, 8);
+    memcpy(tp + 8, &hq, 8);
+    add_pre(tp, 16);
+    c.hq.push_back(hq);
+    key.push_back((uint32_t)((i * 5 + r + 1) % N));
+    c.midx.push_back((uint32_t)(c.off.size() - 2));
+    c.modes.push_back(HS_MODE_STRICT);
+  }
+  const size_t n = key.size(), n_msgs = c.off.size() - 1;
+  std::vector<uint8_t> dig(n_msgs * 32), msgs(n * 32);
+  for (size_t j = 0; j < n_msgs; j++) hso_digest32(&c.pre[c.off[j]], c.off[j + 1] - c.off[j], &dig[j * 32]);
+  std::vector<uint64_t> moff(n + 1);
+  for (size_t i = 0; i <= n; i++) moff[i] = 32 * i;
+  for (size_t i = 0; i < n; i++) memcpy(&msgs[i * 32], &dig[c.midx[i] * 32], 32);
+  c.sig.resize(n * 64);
+  c.pk.resize(n * 32);
+  hso_sign_batch(k.seeds.data(), k.pks.data(), key.data(), msgs.data(), moff.data(), n, ncpu(), c.sig.data());
+  std::vector<uint8_t> recs(n * 128);
+  for (size_t i = 0; i < n; i++) {
+    if ((i * 37 + r * 11) % 100 == 0) c.sig[i * 64 + (i + r) % 64] ^= 0x10;  // 1 % corrupted
+    memcpy(&c.pk[i * 32], &k.pks[(size_t)key[i] * 32], 32);
+    memcpy(&recs[i * 128], &c.sig[i * 64], 64);
+    memcpy(&recs[i * 128 + 64], &c.pk[i * 32], 32);
+    memcpy(&recs[i * 128 + 96], &msgs[i * 32], 32);
+  }
+  std::vector<uint32_t> s((n + 31) / 32), e((n + 31) / 32);
+  hso_verify_rec128_batch(recs.data(), n, 0, ncpu(), s.data());
+  hso_verify_rec128_batch(recs.data(), n, 1, ncpu(), e.data());
+  c.want.assign((n + 31) / 32, 0);
+  for (size_t i = 0; i < n; i++)
+    if ((((c.modes[i] ? e : s)[i >> 5]) >> (i & 31)) & 1u) c.want[i >> 5] |= 1u << (i & 31);
+}
+static int certificate_preimages(hs_ctx *ctx, hs_queue *q, int N, bool block, int certs, int cpu_reps, bool last) {
+  const committee_keys k = make_keys(N, 31);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  series lat[3], cpu[3];
+  int mism[3] = {0, 0, 0}, bad = 0;
+  uint64_t s0[HS_QUEUE_STATS] = {}, d0[HS_QUEUE_DIGEST_STATS] = {}, d1[HS_QUEUE_DIGEST_STATS] = {};
+  hs_queue_stats(q, s0);
+  hs_queue_digest_stats(q, d0);
+  pre_cert c;
+  std::vector<hs_rec128> recs;
+  std::vector<uint8_t> dig;
+  for (int r = 0; r < certs + 3; r++) {
+    const bool timed = r >= 3;
+    make_pre_cert(k, r, block, c);
+    const size_t n = c.midx.size(), n_msgs = c.off.size() - 1;
+    std::vector<uint32_t> bits((n + 31) / 32);
+    // one arm on certificate c; with `timed`, its latency and mismatches are recorded
+    auto run_arm = [&](int a, bool timed) {
+      std::fill(bits.begin(), bits.end(), 0u);
+      const auto t0 = clk::now();
+      int rc = HS_OK;
+      size_t ticket = 0;
+      if (a == 0) {  // (a) hash on the caller's thread, pack records, submit_group
+        dig.resize(n_msgs * 32);
+        for (size_t j = 0; j < n_msgs; j++) hso_digest32(&c.pre[c.off[j]], c.off[j + 1] - c.off[j], &dig[j * 32]);
+        recs.resize(n);
+        for (size_t i = 0; i < n; i++) {
+          memcpy(recs[i].sig, &c.sig[i * 64], 64);
+          memcpy(recs[i].pk, &c.pk[i * 32], 32);
+          memcpy(recs[i].msg, &dig[c.midx[i] * 32], 32);
+        }
+        rc = hs_queue_submit_group(q, recs.data(), n, c.modes.data(), nullptr, nullptr, &ticket);
+        if (rc == HS_OK) rc = hs_queue_wait(q, ticket, bits.data());
+      } else if (a == 1) {  // (b) the preimages, hashed on the GPU
+        rc = hs_queue_submit_msgs(q, c.pre.data(), c.off.data(), n_msgs, c.sig.data(), c.pk.data(), c.midx.data(), c.modes.data(), n, nullptr, nullptr,
+                                  &ticket);
+        if (rc == HS_OK) rc = hs_queue_wait(q, ticket, bits.data());
+      } else if (!block) {  // (c) synchronous: one TC
+        uint32_t tcb = 0;
+        rc = hs_verify_tcs(ctx, &c.tc_round, 1, c.pk.data(), nullptr, c.sig.data(), c.hq.data(), std::vector<uint32_t>(n, 0).data(), n, bits.data(), &tcb);
+      } else {  // (c) synchronous: one Block with its QC and TC
+        uint32_t gb = 0;
+        rc = hs_verify_groups(ctx, c.pre.data(), c.off.data(), n_msgs, c.sig.data(), c.pk.data(), nullptr, c.midx.data(), std::vector<uint32_t>(n, 0).data(),
+                              c.modes.data(), n, 1, bits.data(), &gb);
+      }
+      const double t = us_since(t0);
+      bad += rc != HS_OK;
+      if (timed) {
+        lat[a].v.push_back(t);
+        for (size_t i = 0; i < n; i++) mism[a] += bit(bits, (int)i) != bit(c.want, (int)i);
+      }
+    };
+    for (int a = 0; a < 3; a++) run_arm(a, timed);
+    if (r == certs + 2) {  // the caller thread's CPU time: a back-to-back pass per arm (the thread CPU clock may tick coarsely)
+      for (int a = 0; a < 3; a++) {
+        const double c0 = thread_cpu_us();
+        for (int rep = 0; rep < cpu_reps; rep++) run_arm(a, false);
+        cpu[a].v.push_back((thread_cpu_us() - c0) / cpu_reps);
+      }
+    }
+  }
+  hs_queue_digest_stats(q, d1);
+  const int nv = N - (N - 1) / 3;
+  printf("\"%s_committee_%d\": {\"records\": %d, \"preimages\": %d, \"certificates\": %d, \"cpu_pass_certificates\": %d, ", block ? "block_with_tc" : "tc", N,
+         block ? 1 + 2 * nv : nv, block ? 2 + nv : nv, certs, cpu_reps);
+  const char *names[3] = {"a_caller_hashes_then_submit_group", "b_submit_msgs", block ? "c_sync_verify_groups" : "c_sync_verify_tcs"};
+  for (int a = 0; a < 3; a++)
+    printf("\"%s\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"caller_cpu_us_per_cert\": %.1f, \"mismatches\": %d}, ", names[a], lat[a].pct(0.5), lat[a].pct(0.99),
+           cpu[a].mean(), mism[a]);
+  printf("\"errors\": %d, \"digest_stats\": {\"digest_launches\": %llu, \"preimages\": %llu, \"preimage_bytes\": %llu, \"msgs_requests\": %llu}, ", bad,
+         (unsigned long long)(d1[0] - d0[0]), (unsigned long long)(d1[1] - d0[1]), (unsigned long long)(d1[2] - d0[2]), (unsigned long long)(d1[3] - d0[3]));
+  emit_stats(q, s0);  // warm-up certificates included
+  printf("}%s", last ? "" : ", ");
+  return mism[0] + mism[1] + mism[2] + bad;
+}
+
 static std::string gpu_identity() {  // name and enforced power limit, read in the same run
   std::string s;
   if (FILE *p = popen("nvidia-smi --query-gpu=name,power.limit --format=csv,noheader -i 0 2>/dev/null", "r")) {
@@ -449,12 +610,36 @@ static std::string gpu_identity() {  // name and enforced power limit, read in t
   return s.empty() ? "unknown" : s;
 }
 
+// The certificate_preimages section alone (argv[3] == "certificate_preimages"), or after the others.
+static int run_certificate_preimages(hs_ctx *ctx, int certs) {
+  timespec res;
+  clock_getres(CLOCK_THREAD_CPUTIME_ID, &res);
+  printf("\"certificate_preimages\": {\"gpu\": \"%s\", \"ring_records\": 16384, \"caller_sha512\": \"oracle C restatement (hso_digest32), not the sha2 crate\", "
+         "\"thread_cpu_clock_res_ns\": %ld, ",
+         gpu_identity().c_str(), (long)(res.tv_sec * 1000000000L + res.tv_nsec));
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 16384, &q) != HS_OK) return 1;
+  int bad = 0;
+  for (int block = 0; block < 2; block++)
+    for (int N : {4, 100, 250, 500, 750}) bad += certificate_preimages(ctx, q, N, block == 1, certs, 400, block == 1 && N == 750);
+  hs_queue_destroy(q);
+  printf("}");
+  return bad;
+}
+
 int main(int argc, char **argv) {
   const int rounds = argc > 1 ? atoi(argv[1]) : 1000;
   hs_ctx *ctx = nullptr;
   if (hs_ctx_create(&ctx, 0, 0) != HS_OK) {
     fprintf(stderr, "hs_ctx_create failed (no GPU?)\n");
     return 1;
+  }
+  if (argc > 3 && strcmp(argv[3], "certificate_preimages") == 0) {
+    printf("{");
+    const int bad = run_certificate_preimages(ctx, argc > 2 ? atoi(argv[2]) : 20);
+    printf("}\n");
+    hs_ctx_destroy(ctx);
+    return bad ? 9 : 0;
   }
   uint8_t seeds[4][32], pks[4][32];
   for (int i = 0; i < 4; i++) {
@@ -566,7 +751,9 @@ int main(int argc, char **argv) {
   printf("}, \"block_during_burst\": {\"gpu\": \"%s\", \"threads\": 16, ", gpu_identity().c_str());
   burst_bad += block_during_burst(ctx, 1000, 0, bursts, false);
   burst_bad += block_during_burst(ctx, 10000, 16384, bursts, true);
-  printf("}}\n");
+  printf("}, ");
+  burst_bad += run_certificate_preimages(ctx, bursts);
+  printf("}\n");
   hs_ctx_destroy(ctx);
   return (bad || burst_bad) ? 9 : 0;
 }

@@ -28,9 +28,12 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <list>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
+#include <string_view>
 #include <thread>
 #include <unordered_map>
 #include <vector>
@@ -1364,6 +1367,43 @@ struct queue_bits {
   }
   const uint32_t *data() const { return big.empty() ? inl : big.data(); }
 };
+// Certificate cache (hs_queue_cert_cache).  A span is the batch-eq records of one request that sign the same message, at least two
+// of them: a QC's votes.  Its key is a kind byte ('P': a preimage of hs_queue_submit_msgs, 'D': a Digest of hs_queue_submit_group),
+// the message's length and bytes, then (pk | sig) of each record in request order; lookups go through a hash of the key and match
+// only on equal bytes.  A span that verified in full is kept (least recently used first out, up to max_bytes of keys) and answers 1
+// for every record of an identical span later.  An identical span still pending or in flight is joined: the later request puts
+// none of those records in the ring and takes the earlier request's bits and status for them.
+struct cert_key {
+  size_t h;
+  std::string_view k;
+  bool operator==(const cert_key &o) const { return h == o.h && k == o.k; }
+};
+struct cert_key_hash {
+  size_t operator()(const cert_key &x) const { return x.h; }
+};
+struct cert_span {
+  std::string key;
+  size_t h;
+  std::vector<uint32_t> idx;  // its records in the request, in request order
+  uint8_t role;               // CERT_NEW (its records enter the ring: this request is its primary), CERT_HIT or CERT_JOINED
+};
+enum { CERT_NEW, CERT_HIT, CERT_JOINED };
+// A request submitted with the cache on that has at least one span.  It completes when its ring part (the records that entered
+// the ring, if any) and every span it joined are done: `pending` counts them.
+struct cert_req {
+  size_t ticket;
+  hs_queue_cb *cb;
+  void *user;
+  uint32_t n;
+  std::vector<cert_span> spans;
+  std::vector<uint32_t> ring_idx;  // the request's record of each ring record of its ring part
+  uint32_t pending = 0;
+  int status = HS_OK;
+  std::vector<uint32_t> bits;  // n verdict bits
+};
+struct cert_flight {  // the identical spans waiting on a span its primary request is verifying
+  std::vector<std::pair<cert_req *, const cert_span *>> joiners;
+};
 struct hs_queue {
   hs_ctx *c = nullptr;
   uint32_t cap = 0, mask = 0;
@@ -1399,6 +1439,7 @@ struct hs_queue {
     bool msgs;           // a preimage request: its records' Digests are computed by k_queue_digests
     uint32_t a_off, m, pre_bytes;  // its arena region: offset, preimages, preimage bytes
     uint64_t a_end;      // arena position past its region (0: none)
+    cert_req *cr = nullptr;  // the ring part of a certificate-cache request: its verdicts go there (ticket and cb unused)
   };
   std::vector<req> reqs;  // by request slot
   struct result {
@@ -1419,6 +1460,14 @@ struct hs_queue {
   uint32_t seq = 0;
   uint64_t spins = 0;
   bool stop = false;
+  // certificate cache (hs_queue_cert_cache): off while cc_max is 0
+  std::atomic<size_t> cc_max{0};
+  size_t cc_bytes = 0;                                // key bytes held
+  std::list<std::pair<std::string, size_t>> cc_lru;  // verified span keys and their hashes, most recently used first
+  std::unordered_map<cert_key, std::list<std::pair<std::string, size_t>>::iterator, cert_key_hash> cc_map;
+  std::unordered_map<cert_key, cert_flight, cert_key_hash> cc_flights;  // keyed by the primary's span key
+  std::vector<cert_req *> cc_ready;  // answered entirely at submit: the queue's thread completes them
+  uint64_t cstats[HS_QUEUE_CERT_STATS] = {};  // hs_queue_cert_stats ([5] is cc_bytes)
   std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
   std::condition_variable cv_work, cv_done;
   std::thread th;
@@ -1442,12 +1491,71 @@ static void queue_release_locked(hs_queue *q) {
     q->a_head = std::max(q->a_head, h.a_end);
   }
 }
+// Completes a certificate-cache request whose parts are all done (under q->mu), exactly as queue_finish_locked completes a request.
+static void cert_complete_locked(hs_queue *q, cert_req *cr, std::vector<queue_completion> &fire) {
+  if (cr->cb) {
+    fire.push_back(queue_completion{cr->cb, cr->user, cr->ticket, cr->status, {}});
+    fire.back().bits.set(cr->n, cr->status == HS_OK ? cr->bits.data() : nullptr);
+  } else {
+    hs_queue::result &res = q->results[cr->ticket];
+    res.done = true;
+    res.status = cr->status;
+    res.bits.set(cr->n, cr->status == HS_OK ? cr->bits.data() : nullptr);
+    q->cv_done.notify_all();
+  }
+  delete cr;
+}
+static void cert_evict_locked(hs_queue *q, size_t limit) {  // least recently used first out, until at most `limit` bytes are held
+  while (q->cc_bytes > limit) {
+    const auto &b = q->cc_lru.back();
+    q->cc_map.erase(cert_key{b.second, b.first});
+    q->cc_bytes -= b.first.size();
+    q->cc_lru.pop_back();
+  }
+}
+static void cert_insert_locked(hs_queue *q, std::string &&key, size_t h) {
+  const size_t max = q->cc_max.load();
+  if (key.size() > max || q->cc_map.count(cert_key{h, key})) return;
+  cert_evict_locked(q, max - key.size());
+  q->cc_bytes += key.size();
+  q->cc_lru.emplace_front(std::move(key), h);
+  q->cc_map.emplace(cert_key{h, q->cc_lru.front().first}, q->cc_lru.begin());
+  q->cstats[4]++;
+}
+// The ring part of certificate-cache request cr is done (bits: its ring records' verdicts, null on error).  Each span it verified
+// hands its bits and status to the requests that joined it, and enters the cache if every one of its records verified.
+static void cert_part_done_locked(hs_queue *q, cert_req *cr, int status, const uint32_t *bits, std::vector<queue_completion> &fire) {
+  if (status != HS_OK) cr->status = status;
+  else
+    for (size_t k = 0; k < cr->ring_idx.size(); k++)
+      if ((bits[k >> 5] >> (k & 31)) & 1u) cr->bits[cr->ring_idx[k] >> 5] |= 1u << (cr->ring_idx[k] & 31);
+  for (cert_span &sp : cr->spans) {
+    if (sp.role != CERT_NEW) continue;
+    bool all = status == HS_OK;
+    for (uint32_t i : sp.idx) all = all && ((cr->bits[i >> 5] >> (i & 31)) & 1u);
+    auto it = q->cc_flights.find(cert_key{sp.h, sp.key});
+    for (auto &[jr, js] : it->second.joiners) {
+      if (status != HS_OK) jr->status = status;
+      else
+        for (size_t t = 0; t < sp.idx.size(); t++)
+          if ((cr->bits[sp.idx[t] >> 5] >> (sp.idx[t] & 31)) & 1u) jr->bits[js->idx[t] >> 5] |= 1u << (js->idx[t] & 31);
+      if (--jr->pending == 0) cert_complete_locked(q, jr, fire);
+    }
+    q->cc_flights.erase(it);
+    if (all) cert_insert_locked(q, std::move(sp.key), sp.h);
+  }
+  if (--cr->pending == 0) cert_complete_locked(q, cr, fire);
+}
+
 // Marks the request at ring position p finished (under q->mu): a polled ticket's result is parked, a callback is returned to be
 // fired after the lock is released.
 static void queue_finish_locked(hs_queue *q, uint64_t p, int status, const uint32_t *bits, std::vector<queue_completion> &fire) {
   hs_queue::req &r = q->reqs[p & q->mask];
   r.finished = true;
-  if (r.cb) {
+  if (r.cr) {
+    cert_part_done_locked(q, r.cr, status, status == HS_OK ? bits : nullptr, fire);
+    r.cr = nullptr;
+  } else if (r.cb) {
     fire.push_back(queue_completion{r.cb, r.user, r.ticket, status, {}});
     fire.back().bits.set(r.n, status == HS_OK ? bits : nullptr);
   } else {
@@ -1694,7 +1802,15 @@ static void queue_main(hs_queue *q) {
   cudaSetDevice(q->c->device);
   std::unique_lock<std::mutex> lk(q->mu);
   for (;;) {
-    if (q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) {
+    if (!q->cc_ready.empty()) {  // requests the certificate cache answered at submit
+      std::vector<cert_req *> ready;
+      ready.swap(q->cc_ready);
+      std::vector<queue_completion> fire;
+      for (cert_req *cr : ready) cert_complete_locked(q, cr, fire);
+      lk.unlock();
+      queue_fire(fire);
+      lk.lock();
+    } else if (q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) {
       const uint64_t lo = q->launched, hi = q->tail;  // everything pending
       q->launched = hi;
       lk.unlock();
@@ -2722,24 +2838,191 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   return HS_OK;
 }
 
+// The records of one request that enter the ring: record sel[k] of the caller's arrays (k itself when sel is null), k < n.
+struct queue_sel {
+  const uint32_t *sel;
+  size_t n;
+  size_t operator[](size_t k) const { return sel ? sel[k] : k; }
+};
+
+// Copies one request's selected records into the ring (under q->mu, arguments already checked) as ring request r: record i is
+// judged by modes[i], or by `mode` when modes is null.  HS_ERR_NOMEM when the ring has no room.
+static int queue_put_recs_locked(hs_queue *q, const char *what, const hs_rec128 *recs, queue_sel sel, uint32_t mode, const uint8_t *modes,
+                                 hs_queue::req r) {
+  if (sel.n > q->cap) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": more records than the ring holds").c_str());
+  if (q->tail - q->head + sel.n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
+  for (size_t k = 0; k < sel.n; k++) {
+    const size_t i = sel[k];
+    const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
+    memcpy(q->h_ring[s].sig, recs[i].sig, 64);
+    memcpy(q->h_ring[s].msg, recs[i].msg, 32);
+    memcpy(q->pk.data() + 32 * (size_t)s, recs[i].pk, 32);
+    q->modes[s] = modes ? modes[i] : (uint8_t)mode;
+  }
+  r.n = (uint32_t)sel.n;
+  q->reqs[q->tail & q->mask] = r;
+  q->tail += sel.n;
+  return HS_OK;
+}
+
+// The same for a preimage request: the selected records go into the ring and the preimages they name, in their order, into one
+// arena region.  HS_ERR_ARG when the region is larger than the arena, HS_ERR_NOMEM when the arena or the ring has no room.
+static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                                 const uint32_t *msg_idx, const uint8_t *modes, queue_sel sel, hs_queue::req r) {
+  const size_t n = sel.n;
+  if (n > q->cap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more records than the ring holds");
+  // keep only the preimages some record names, in their order: remap[j] = new index of preimage j
+  std::vector<uint32_t> remap(n_msgs, HS_NO_KEY);
+  for (size_t k = 0; k < n; k++) remap[msg_idx[sel[k]]] = 0;
+  uint32_t m = 0;
+  uint64_t pre_bytes = 0;
+  for (size_t j = 0; j < n_msgs; j++)
+    if (remap[j] == 0) {
+      remap[j] = m++;
+      pre_bytes += pre_off[j + 1] - pre_off[j];
+    }
+  const uint64_t size = qmsg_bytes(m, n, pre_bytes);
+  if (size > q->acap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more preimage bytes than the queue's arena holds");
+  uint64_t start = q->a_tail;
+  if ((start & (q->acap - 1)) + size > q->acap) start += q->acap - (start & (q->acap - 1));  // would cross the end: start over
+  if (start + size - q->a_head > q->acap) {  // arena full
+    if (q->a_head != q->a_tail) return HS_ERR_NOMEM;
+    start = q->a_head = q->a_tail = start;  // empty: the skipped tail is free too
+  }
+  if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
+  uint8_t *a = q->h_arena + (start & (q->acap - 1));
+  uint64_t *off = reinterpret_cast<uint64_t *>(a);
+  uint32_t *idx = reinterpret_cast<uint32_t *>(a + 8 * ((size_t)m + 1));
+  uint8_t *pre = a + qmsg_o_pre(m, n);
+  off[0] = 0;
+  for (size_t j = 0, k = 0; j < n_msgs; j++)
+    if (remap[j] != HS_NO_KEY) {
+      const uint64_t len = pre_off[j + 1] - pre_off[j];
+      if (len) memcpy(pre + off[k], preimages + pre_off[j], len);
+      off[k + 1] = off[k] + len;
+      k++;
+    }
+  for (size_t k = 0; k < n; k++) {
+    const size_t i = sel[k];
+    const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
+    memcpy(q->h_ring[s].sig, sig + 64 * i, 64);
+    memcpy(q->pk.data() + 32 * (size_t)s, pk + 32 * i, 32);
+    q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
+    idx[k] = remap[msg_idx[i]];
+  }
+  r.n = (uint32_t)n;
+  r.msgs = true;
+  r.a_off = (uint32_t)(start & (q->acap - 1));
+  r.m = m;
+  r.pre_bytes = (uint32_t)pre_bytes;
+  r.a_end = start + size;
+  q->reqs[q->tail & q->mask] = r;
+  q->tail += n;
+  q->a_tail = start + size;
+  q->dstats[3]++;
+  return HS_OK;
+}
+
+// A request's spans (see cert_key): record i signs msg(i) with key pk(i) (32 bytes) and signature sig(i) (64 bytes).  Null when
+// the request has no span; its records then all enter the ring exactly as with the cache off.
+extern "C++" {
+template <class Msg, class Pk, class Sig>
+static std::unique_ptr<cert_req> cert_spans(char kind, size_t n, const uint8_t *modes, hs_queue_cb *cb, void *user, Msg msg, Pk pk, Sig sig) {
+  if (!modes) return nullptr;  // all strict
+  std::unordered_map<std::string_view, size_t> by_msg;
+  std::vector<std::vector<uint32_t>> groups;
+  for (uint32_t i = 0; i < n; i++) {
+    if (modes[i] != HS_MODE_BATCH_EQ) continue;
+    auto it = by_msg.emplace(msg(i), groups.size()).first;
+    if (it->second == groups.size()) groups.emplace_back();
+    groups[it->second].push_back(i);
+  }
+  std::unique_ptr<cert_req> cr;
+  for (std::vector<uint32_t> &g : groups) {
+    if (g.size() < 2) continue;
+    if (!cr) cr.reset(new cert_req{0, cb, user, (uint32_t)n, {}, {}, 0, HS_OK, std::vector<uint32_t>((n + 31) / 32, 0u)});
+    const std::string_view m = msg(g[0]);
+    const uint64_t len = m.size();
+    std::string key;
+    key.reserve(1 + 8 + m.size() + 96 * g.size());
+    key.push_back(kind);
+    key.append(reinterpret_cast<const char *>(&len), 8);
+    key.append(m);
+    for (uint32_t i : g) {
+      key.append(reinterpret_cast<const char *>(pk(i)), 32);
+      key.append(reinterpret_cast<const char *>(sig(i)), 64);
+    }
+    const size_t h = std::hash<std::string_view>{}(key);
+    cr->spans.push_back(cert_span{std::move(key), h, std::move(g), CERT_NEW});
+  }
+  return cr;
+}
+
+// Submits a request that has spans, with the cache on.  Under q->mu each span is a hit, a join of an identical span pending or in
+// flight in an earlier request, or new; `put(sel, r)` enters the records of no hit or joined span into the ring as request r.  When
+// there are none the request is answered entirely here and the queue's thread completes it.  Nothing changes on an error.
+template <class Put>
+static int cert_submit(hs_queue *q, const char *what, std::unique_ptr<cert_req> cr, size_t *out_ticket, Put put) {
+  std::vector<int32_t> span_of(cr->n, -1);
+  for (size_t j = 0; j < cr->spans.size(); j++)
+    for (uint32_t i : cr->spans[j].idx) span_of[i] = (int32_t)j;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
+    for (cert_span &sp : cr->spans) {
+      const cert_key k{sp.h, sp.key};
+      sp.role = q->cc_map.count(k) ? CERT_HIT : q->cc_flights.count(k) ? CERT_JOINED : CERT_NEW;
+    }
+    std::vector<uint32_t> sel;
+    for (uint32_t i = 0; i < cr->n; i++)
+      if (span_of[i] < 0 || cr->spans[span_of[i]].role == CERT_NEW) sel.push_back(i);
+    if (!sel.empty()) {
+      hs_queue::req r{};
+      r.cr = cr.get();
+      const int rc = put(queue_sel{sel.data(), sel.size()}, r);
+      if (rc != HS_OK) return rc;
+      cr->pending++;
+    }
+    cr->ring_idx = std::move(sel);
+    cr->ticket = q->next_ticket++;
+    if (!cr->cb) q->results[cr->ticket] = hs_queue::result{false, HS_OK, cr->n, {}};
+    q->cstats[0] += cr->spans.size();
+    for (cert_span &sp : cr->spans) {
+      const cert_key k{sp.h, sp.key};
+      if (sp.role == CERT_HIT) {
+        auto it = q->cc_map.find(k);
+        q->cc_lru.splice(q->cc_lru.begin(), q->cc_lru, it->second);
+        for (uint32_t i : sp.idx) cr->bits[i >> 5] |= 1u << (i & 31);
+        q->cstats[1]++;
+      } else if (sp.role == CERT_JOINED) {
+        q->cc_flights.find(k)->second.joiners.emplace_back(cr.get(), &sp);
+        cr->pending++;
+        q->cstats[2]++;
+      } else {
+        q->cc_flights.emplace(k, cert_flight{});
+        continue;
+      }
+      q->cstats[3] += sp.idx.size();
+    }
+    if (out_ticket) *out_ticket = cr->ticket;
+    if (cr->pending == 0) q->cc_ready.push_back(cr.get());
+    cr.release();  // owned by the queue until it completes
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+}  // extern "C++"
+
 // Copies one request into the ring (arguments already checked): record i is judged by modes[i], or by `mode` when modes is null.
 static int queue_enqueue(hs_queue *q, const char *what, const hs_rec128 *recs, size_t n, uint32_t mode, const uint8_t *modes, hs_queue_cb *cb,
                          void *user, size_t *out_ticket) {
   {
     std::lock_guard<std::mutex> g(q->mu);
     if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
-    if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
-    for (size_t i = 0; i < n; i++) {
-      const uint32_t s = (uint32_t)((q->tail + i) & q->mask);
-      memcpy(q->h_ring[s].sig, recs[i].sig, 64);
-      memcpy(q->h_ring[s].msg, recs[i].msg, 32);
-      memcpy(q->pk.data() + 32 * (size_t)s, recs[i].pk, 32);
-      q->modes[s] = modes ? modes[i] : (uint8_t)mode;
-    }
+    const int rc = queue_put_recs_locked(q, what, recs, queue_sel{nullptr, n}, mode, modes, hs_queue::req{q->next_ticket, 0, cb, user, 0, false});
+    if (rc != HS_OK) return rc;
     const size_t ticket = q->next_ticket++;
-    q->reqs[q->tail & q->mask] = hs_queue::req{ticket, (uint32_t)n, cb, user, 0, false};
     if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
-    q->tail += n;
     if (out_ticket) *out_ticket = ticket;
   }
   q->cv_work.notify_one();
@@ -2751,69 +3034,55 @@ int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode,
   return queue_enqueue(q, "hs_queue_submit", recs, n, mode, nullptr, cb, user, out_ticket);
 }
 
+// With the certificate cache on, the ring capacity limits the records that enter the ring (checked under the lock), not n.
+#define HS_QUEUE_CERT_MAX_N ((size_t)UINT32_MAX)
+
 int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const uint8_t *modes, hs_queue_cb *cb, void *user, size_t *out_ticket) {
-  if (!q || !recs || n == 0 || n > q->cap) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
+  const bool cache = q && q->cc_max.load() > 0;
+  if (!q || !recs || n == 0 || n > (cache ? HS_QUEUE_CERT_MAX_N : q->cap)) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
   if (modes)
     for (size_t i = 0; i < n; i++)
       if (modes[i] > HS_MODE_BATCH_EQ) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_group: bad mode byte");
-  return queue_enqueue(q, "hs_queue_submit_group", recs, n, HS_MODE_STRICT, modes, cb, user, out_ticket);
+  std::unique_ptr<cert_req> cr;
+  if (cache)
+    cr = cert_spans('D', n, modes, cb, user, [&](size_t i) { return std::string_view(reinterpret_cast<const char *>(recs[i].msg), 32); },
+                    [&](size_t i) { return recs[i].pk; }, [&](size_t i) { return recs[i].sig; });
+  if (!cr) {
+    if (n > q->cap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
+    return queue_enqueue(q, "hs_queue_submit_group", recs, n, HS_MODE_STRICT, modes, cb, user, out_ticket);
+  }
+  return cert_submit(q, "hs_queue_submit_group", std::move(cr), out_ticket, [&](queue_sel sel, const hs_queue::req &r) {
+    return queue_put_recs_locked(q, "hs_queue_submit_group", recs, sel, HS_MODE_STRICT, modes, r);
+  });
 }
 
 int hs_queue_submit_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
                          const uint32_t *msg_idx, const uint8_t *modes, size_t n, hs_queue_cb *cb, void *user, size_t *out_ticket) {
-  if (!q || !pre_off || !sig || !pk || !msg_idx || n == 0 || n > q->cap || n_msgs == 0)
+  const bool cache = q && q->cc_max.load() > 0;
+  if (!q || !pre_off || !sig || !pk || !msg_idx || n == 0 || n > (cache ? HS_QUEUE_CERT_MAX_N : q->cap) || n_msgs == 0)
     return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_msgs: bad argument");
   if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages)) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: bad preimage offsets");
   for (size_t i = 0; i < n; i++)
     if (msg_idx[i] >= n_msgs || (modes && modes[i] > HS_MODE_BATCH_EQ)) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: index or mode out of range");
-  // keep only the preimages some record names, in their order: remap[j] = new index of preimage j
-  std::vector<uint32_t> remap(n_msgs, HS_NO_KEY);
-  for (size_t i = 0; i < n; i++) remap[msg_idx[i]] = 0;
-  uint32_t m = 0;
-  uint64_t pre_bytes = 0;
-  for (size_t j = 0; j < n_msgs; j++)
-    if (remap[j] == 0) {
-      remap[j] = m++;
-      pre_bytes += pre_off[j + 1] - pre_off[j];
-    }
-  const uint64_t size = qmsg_bytes(m, n, pre_bytes);
-  if (size > q->acap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more preimage bytes than the queue's arena holds");
+  std::unique_ptr<cert_req> cr;
+  if (cache)
+    cr = cert_spans('P', n, modes, cb, user,
+                    [&](size_t i) {
+                      const uint64_t lo = pre_off[msg_idx[i]], hi = pre_off[msg_idx[i] + 1];
+                      return hi > lo ? std::string_view(reinterpret_cast<const char *>(preimages + lo), hi - lo) : std::string_view();
+                    },
+                    [&](size_t i) { return pk + 32 * i; }, [&](size_t i) { return sig + 64 * i; });
+  const auto put = [&](queue_sel sel, const hs_queue::req &r) {
+    return queue_put_msgs_locked(q, preimages, pre_off, n_msgs, sig, pk, msg_idx, modes, sel, r);
+  };
+  if (cr) return cert_submit(q, "hs_queue_submit_msgs", std::move(cr), out_ticket, put);
   {
     std::lock_guard<std::mutex> g(q->mu);
     if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: queue is being destroyed");
-    uint64_t start = q->a_tail;
-    if ((start & (q->acap - 1)) + size > q->acap) start += q->acap - (start & (q->acap - 1));  // would cross the end: start over
-    if (start + size - q->a_head > q->acap) {  // arena full
-      if (q->a_head != q->a_tail) return HS_ERR_NOMEM;
-      start = q->a_head = q->a_tail = start;  // empty: the skipped tail is free too
-    }
-    if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
-    uint8_t *a = q->h_arena + (start & (q->acap - 1));
-    uint64_t *off = reinterpret_cast<uint64_t *>(a);
-    uint32_t *idx = reinterpret_cast<uint32_t *>(a + 8 * ((size_t)m + 1));
-    uint8_t *pre = a + qmsg_o_pre(m, n);
-    off[0] = 0;
-    for (size_t j = 0, k = 0; j < n_msgs; j++)
-      if (remap[j] != HS_NO_KEY) {
-        const uint64_t len = pre_off[j + 1] - pre_off[j];
-        if (len) memcpy(pre + off[k], preimages + pre_off[j], len);
-        off[k + 1] = off[k] + len;
-        k++;
-      }
-    for (size_t i = 0; i < n; i++) {
-      const uint32_t s = (uint32_t)((q->tail + i) & q->mask);
-      memcpy(q->h_ring[s].sig, sig + 64 * i, 64);
-      memcpy(q->pk.data() + 32 * (size_t)s, pk + 32 * i, 32);
-      q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
-      idx[i] = remap[msg_idx[i]];
-    }
+    const int rc = put(queue_sel{nullptr, n}, hs_queue::req{q->next_ticket, 0, cb, user, 0, false});
+    if (rc != HS_OK) return rc;
     const size_t ticket = q->next_ticket++;
-    q->reqs[q->tail & q->mask] =
-        hs_queue::req{ticket, (uint32_t)n, cb, user, 0, false, true, (uint32_t)(start & (q->acap - 1)), m, (uint32_t)pre_bytes, start + size};
     if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
-    q->tail += n;
-    q->a_tail = start + size;
-    q->dstats[3]++;
     if (out_ticket) *out_ticket = ticket;
   }
   q->cv_work.notify_one();
@@ -2860,6 +3129,22 @@ int hs_queue_digest_stats(hs_queue *q, uint64_t out[HS_QUEUE_DIGEST_STATS]) {
   if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_digest_stats: bad argument");
   std::lock_guard<std::mutex> g(q->mu);
   memcpy(out, q->dstats, sizeof(q->dstats));
+  return HS_OK;
+}
+
+int hs_queue_cert_cache(hs_queue *q, size_t max_bytes) {
+  if (!q) return fail(nullptr, HS_ERR_ARG, "hs_queue_cert_cache: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  q->cc_max = max_bytes;
+  cert_evict_locked(q, max_bytes);
+  return HS_OK;
+}
+
+int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_cert_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  q->cstats[5] = q->cc_bytes;
+  memcpy(out, q->cstats, sizeof(q->cstats));
   return HS_OK;
 }
 

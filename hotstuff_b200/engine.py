@@ -435,6 +435,21 @@ class VerifyQueue:
         self.engine._check(self.lib.hs_queue_digest_stats(self.h, out), "hs_queue_digest_stats")
         return dict(zip(self.DIGEST_STATS, (int(x) for x in out)))
 
+    def cert_cache(self, max_bytes):
+        """Turns the certificate cache on (hs_queue_cert_cache): keep up to max_bytes of verified certificates, so an identical QC in a
+        later submit_group / submit_msgs request is answered without verifying it again, and one still in flight is joined instead of
+        verified twice.  Verdicts do not change.  0 turns it off (the default)."""
+        self.engine._check(self.lib.hs_queue_cert_cache(self.h, int(max_bytes)), "hs_queue_cert_cache")
+
+    CERT_STATS = ("lookups", "hits", "joins", "records_answered", "inserted", "bytes_held")
+
+    def cert_stats(self):
+        """Counters of the certificate cache (hs_queue_cert_stats): spans looked up, cache hits, in-flight joins, records answered
+        without verifying them, spans inserted, and the bytes held now."""
+        out = (ctypes.c_uint64 * len(self.CERT_STATS))()
+        self.engine._check(self.lib.hs_queue_cert_stats(self.h, out), "hs_queue_cert_stats")
+        return dict(zip(self.CERT_STATS, (int(x) for x in out)))
+
     def close(self):
         """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""
         if getattr(self, "h", None):

@@ -209,6 +209,9 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *     request's status.  Reading a ticket twice, or reading a callback ticket, is HS_ERR_ARG.
  *   - hs_committee_register / hs_committee_update / hs_ctx_destroy drain the queue's launches before they touch the tables; a
  *     request submitted after one of them returns is judged against the new committee.
+ *   - hs_queue_cert_cache (off by default) lets the queue verify a certificate that many requests carry once: during a view
+ *     change every Timeout carries the same high_qc, and a copy that is in flight is joined and one that verified is a hit, so
+ *     each Timeout puts only its author's record in the ring.  Verdicts do not change.
  *   - hs_queue_destroy completes every request in flight (callbacks fire) and joins the thread; hs_ctx_destroy destroys the
  *     queues still attached to the context.  hs_kernel_launches counts the queue's launches; hs_queue_stats tells them apart. */
 typedef struct hs_queue hs_queue;
@@ -244,6 +247,22 @@ int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]);
 /* [0] k_queue_digests launches, [1] preimages hashed, [2] preimage bytes hashed, [3] hs_queue_submit_msgs requests. */
 #define HS_QUEUE_DIGEST_STATS 4
 int hs_queue_digest_stats(hs_queue *q, uint64_t out[HS_QUEUE_DIGEST_STATS]);
+/* Certificate cache of hs_queue_submit_group / hs_queue_submit_msgs.  A span is the HS_MODE_BATCH_EQ records of one request that
+ * sign the same message (the 32-byte Digest for submit_group, the preimage bytes for submit_msgs; the two never match), at least
+ * two of them: a QC's votes.  Strict records are never cached.  A span matches only a span with the same kind, message and
+ * (pk, sig) of every record in the same order, byte for byte.  A span whose records all verified is kept: a later identical span
+ * is a hit and answers 1 for each of its records.  An identical span still pending or in flight in an earlier request is joined:
+ * the later request takes that request's bits for it and its status (HS_ERR_CUDA propagates).  Hit and joined records take no
+ * ring slot and their preimages no arena bytes, so HS_ERR_NOMEM and the ring-capacity and arena-size HS_ERR_ARG apply to the
+ * records that enter the ring (a Timeout whose high_qc hits costs one record).  A request answered entirely from the cache still
+ * gets a ticket and completes on the queue's thread.  Verdicts are bit for bit those of the same request with the cache off.
+ * 0 = off (the default: every request behaves exactly as without this call). Otherwise keep up to max_bytes of verified certificates
+ * (the key bytes: 9 + message length + 96 per record), least recently used first out. */
+int hs_queue_cert_cache(hs_queue *q, size_t max_bytes);
+#define HS_QUEUE_CERT_STATS 6
+/* [0] spans looked up, [1] cache hits, [2] in-flight joins, [3] records answered without verifying them,
+ * [4] spans inserted, [5] bytes held now */
+int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

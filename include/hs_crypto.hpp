@@ -116,6 +116,15 @@ class VerifyQueue {
     e_.check(hs_queue_digest_stats(q_, s.data()), "hs_queue_digest_stats");
     return s;
   }
+  // hs_queue_cert_cache: keep up to max_bytes of verified certificates (0 = off, the default).  Verdicts do not change.
+  void cert_cache(size_t max_bytes) { e_.check(hs_queue_cert_cache(q_, max_bytes), "hs_queue_cert_cache"); }
+  // hs_queue_cert_stats: [0] spans looked up, [1] hits, [2] in-flight joins, [3] records answered without verifying them,
+  // [4] spans inserted, [5] bytes held now.
+  std::array<uint64_t, HS_QUEUE_CERT_STATS> cert_stats() const {
+    std::array<uint64_t, HS_QUEUE_CERT_STATS> s{};
+    e_.check(hs_queue_cert_stats(q_, s.data()), "hs_queue_cert_stats");
+    return s;
+  }
 
  private:
   struct Pending {

@@ -25,6 +25,10 @@ pub mod group_queue;
 /// the connection task no SHA-512 calls (`msgs_queue::verify_msgs_queued`).
 #[path = "crypto_gpu_msgs_queue.rs"]
 pub mod msgs_queue;
+/// The queue's certificate cache (hs_queue_cert_cache): a QC that several Timeouts carry is verified once
+/// (`msgs_queue::verify_timeout_queued`).
+#[path = "crypto_gpu_cert_cache.rs"]
+pub mod cert_cache;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

@@ -27,6 +27,10 @@
 // (a) by hashing the preimages on the caller's thread then hs_queue_submit_group, (b) by hs_queue_submit_msgs (the GPU hashes them),
 // (c) synchronously; latency and the caller thread's CPU time per certificate, plus hs_queue_digest_stats.
 //
+// View change (last; alone with argv[3] = view_change): N = 100, 1,000 and 4,000 Timeouts released at once to 16 threads, nearly all
+// carrying the same high_qc, through (a) the queue without its certificate cache (synchronous fallback as the Rust module), (b) the
+// queue with it, (c) the synchronous batched calls; burst time, signatures verified and hs_queue_cert_stats.
+//
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
 #include <atomic>
@@ -627,6 +631,308 @@ static int run_certificate_preimages(hs_ctx *ctx, int certs) {
   return bad;
 }
 
+// ---- view change: every validator's Timeout at once, nearly all carrying the same high_qc (consensus/src/core.rs local_timeout
+// -> handle_timeout).  One burst = N Timeout frames released together to 16 threads (one per connection task): record 0 the author's
+// strict signature over round || high_qc.round (16 bytes), records 1.. the high_qc's N - f batch-eq votes over hash || round (40
+// bytes).  1 % of the author signatures are corrupted.  Each burst has a new QC: cold = first seen in the burst; warm = the Block
+// carrying it went through the queue first, and a tenth of the Timeouts carry a copy of the QC with one bad vote (each must be
+// rejected, and that QC must never enter the cache).  Arms:
+//   (a) the queue without the cache, as the Rust module does today: a Timeout of more than GROUP_MAX_SIGS = 502 records, or one the
+//       queue refuses, is verified synchronously (a strict author verify + hs_verify_batch_shared_msg);
+//   (b) the queue with the certificate cache (hs_queue_submit_msgs, the same synchronous fallback on a refusal);
+//   (c) the synchronous batched calls of Core::verify_timeouts: one hs_verify_tcs for every author + one QC verify per distinct QC.
+// Burst time = release -> the last Timeout's verdict.  Signatures verified = the records the queue's launches and slow path carried
+// plus the synchronous ones.
+#define VC_THREADS 16
+#define VC_GROUP_MAX_SIGS 502
+struct vc_qc {
+  uint8_t pre[40], dig[32];
+  std::vector<uint8_t> sig, pk;  // nv x 64, nv x 32
+  std::vector<hs_vote> votes;
+  std::vector<uint32_t> want;    // oracle, batch-eq
+};
+struct vc_burst {
+  int N = 0, nv = 0;
+  uint64_t round = 0, hq = 0;
+  std::vector<uint8_t> a_sig, a_pk;  // N authors
+  std::vector<uint32_t> a_want;      // oracle, strict
+  vc_qc qc[2];                       // [1]: [0] with one bad vote
+  std::vector<uint8_t> bad;          // Timeout i carries qc[1]
+};
+static void vc_make(const committee_keys &k, int b, bool bad_qc, vc_burst &v) {
+  const int N = k.N, nv = N - (N - 1) / 3;
+  v.N = N;
+  v.nv = nv;
+  v.round = 90000 + (uint64_t)b * 3 + (bad_qc ? 1 : 0);
+  v.hq = v.round - 1;
+  uint8_t tp[16];
+  memcpy(tp, &v.round, 8);
+  memcpy(tp + 8, &v.hq, 8);
+  uint8_t td[32];
+  hso_digest32(tp, 16, td);
+  std::vector<uint32_t> key(N);
+  std::vector<uint8_t> msgs((size_t)N * 32);
+  std::vector<uint64_t> off(N + 1);
+  for (int i = 0; i < N; i++) {
+    key[i] = (uint32_t)i;
+    memcpy(&msgs[(size_t)i * 32], td, 32);
+  }
+  for (int i = 0; i <= N; i++) off[i] = (uint64_t)i * 32;
+  v.a_sig.resize((size_t)N * 64);
+  v.a_pk.assign(k.pks.begin(), k.pks.end());
+  hso_sign_batch(k.seeds.data(), k.pks.data(), key.data(), msgs.data(), off.data(), N, ncpu(), v.a_sig.data());
+  for (int i = 0; i < N; i++)
+    if ((i * 37 + b * 11) % 100 == 0) v.a_sig[(size_t)i * 64 + (i + b) % 64] ^= 0x10;  // 1 % of the authors corrupted
+  std::vector<uint8_t> recs((size_t)N * 128);
+  for (int i = 0; i < N; i++) {
+    memcpy(&recs[(size_t)i * 128], &v.a_sig[(size_t)i * 64], 64);
+    memcpy(&recs[(size_t)i * 128 + 64], &v.a_pk[(size_t)i * 32], 32);
+    memcpy(&recs[(size_t)i * 128 + 96], td, 32);
+  }
+  v.a_want.assign((N + 31) / 32, 0);
+  hso_verify_rec128_batch(recs.data(), N, 0, ncpu(), v.a_want.data());
+  vc_qc &q = v.qc[0];
+  for (int j = 0; j < 32; j++) q.pre[j] = (uint8_t)(b * 19 + j * 7 + (bad_qc ? 101 : 3));
+  memcpy(q.pre + 32, &v.hq, 8);
+  hso_digest32(q.pre, 40, q.dig);
+  for (int i = 0; i < nv; i++) {
+    key[i] = (uint32_t)((i * 7 + b) % N);
+    memcpy(&msgs[(size_t)i * 32], q.dig, 32);
+  }
+  q.sig.resize((size_t)nv * 64);
+  q.pk.resize((size_t)nv * 32);
+  hso_sign_batch(k.seeds.data(), k.pks.data(), key.data(), msgs.data(), off.data(), nv, ncpu(), q.sig.data());
+  for (int i = 0; i < nv; i++) memcpy(&q.pk[(size_t)i * 32], &k.pks[(size_t)key[i] * 32], 32);
+  v.qc[1] = q;
+  v.qc[1].sig[(size_t)(nv / 2) * 64 + 40] ^= 0x04;  // one bad vote
+  for (vc_qc &x : v.qc) {
+    x.votes.resize(nv);
+    recs.resize((size_t)nv * 128);
+    for (int i = 0; i < nv; i++) {
+      memcpy(x.votes[i].pk, &x.pk[(size_t)i * 32], 32);
+      memcpy(x.votes[i].sig, &x.sig[(size_t)i * 64], 64);
+      memcpy(&recs[(size_t)i * 128], &x.sig[(size_t)i * 64], 64);
+      memcpy(&recs[(size_t)i * 128 + 64], &x.pk[(size_t)i * 32], 32);
+      memcpy(&recs[(size_t)i * 128 + 96], x.dig, 32);
+    }
+    x.want.assign((nv + 31) / 32, 0);
+    hso_verify_rec128_batch(recs.data(), nv, 1, ncpu(), x.want.data());
+  }
+  v.bad.assign(N, 0);
+  if (bad_qc)
+    for (int i = 7; i < N; i += 10) v.bad[i] = 1;
+}
+struct vc_arm {
+  series t;
+  uint64_t sync_sigs = 0, fallbacks = 0;
+  int mismatches = 0, bad_accepted = 0, errors = 0;
+};
+// The synchronous Timeout::verify of the Rust module's fallback: a strict author verify + verify_batch over the QC's votes.
+static int vc_sync_timeout(hs_ctx *ctx, const vc_burst &v, int i, std::vector<uint32_t> &bits) {
+  const vc_qc &q = v.qc[v.bad[i]];
+  hs_rec128 a;
+  memcpy(a.sig, &v.a_sig[(size_t)i * 64], 64);
+  memcpy(a.pk, &v.a_pk[(size_t)i * 32], 32);
+  uint8_t tp[16];
+  memcpy(tp, &v.round, 8);
+  memcpy(tp + 8, &v.hq, 8);
+  hso_digest32(tp, 16, a.msg);
+  uint32_t ab = 0;
+  int ok = 0;
+  std::vector<uint32_t> vb((v.nv + 31) / 32);
+  if (hs_verify_rec128(ctx, &a, 1, HS_MODE_STRICT, &ab) != HS_OK) return 1;
+  if (hs_verify_batch_shared_msg(ctx, q.dig, q.votes.data(), v.nv, &ok, vb.data()) != HS_OK) return 1;
+  std::fill(bits.begin(), bits.end(), 0u);
+  bits[0] = ab & 1u;
+  for (int k = 0; k < v.nv; k++)
+    if (bit(vb, k)) bits[(k + 1) >> 5] |= 1u << ((k + 1) & 31);
+  return 0;
+}
+static void vc_check(const vc_burst &v, int i, const std::vector<uint32_t> &bits, std::atomic<int> &mism, std::atomic<int> &bad_acc) {
+  const vc_qc &q = v.qc[v.bad[i]];
+  int m = bit(bits, 0) != bit(v.a_want, i), all = bit(bits, 0);
+  for (int k = 0; k < v.nv; k++) {
+    m += bit(bits, k + 1) != bit(q.want, k);
+    all &= bit(bits, k + 1);
+  }
+  mism += m;
+  bad_acc += v.bad[i] && all;
+}
+// One burst through a queue (arms a and b): thread t takes Timeouts t, t + 16, ...; it submits each, then waits for each.
+static double vc_queue_burst(hs_ctx *ctx, hs_queue *q, bool cache, const vc_burst &v, vc_arm &arm) {
+  const int N = v.N, n = 1 + v.nv;
+  std::atomic<int> go{0}, mism{0}, bad_acc{0}, errs{0};
+  std::atomic<uint64_t> sync_sigs{0}, fallbacks{0};
+  uint8_t pre[56];
+  memcpy(pre, &v.round, 8);
+  memcpy(pre + 8, &v.hq, 8);
+  const uint64_t off[3] = {0, 16, 56};
+  std::vector<std::thread> th;
+  for (int t = 0; t < VC_THREADS; t++)
+    th.emplace_back([&, t] {
+      std::vector<uint8_t> sig((size_t)n * 64), pk((size_t)n * 32), modes(n, HS_MODE_BATCH_EQ), p(pre, pre + 56);
+      std::vector<uint32_t> midx(n, 1), bits((n + 31) / 32);
+      midx[0] = 0;
+      modes[0] = HS_MODE_STRICT;
+      std::vector<std::pair<int, size_t>> tickets;
+      while (!go.load()) {
+      }
+      for (int i = t; i < N; i += VC_THREADS) {
+        const vc_qc &qc = v.qc[v.bad[i]];
+        int rc = HS_ERR_ARG;
+        size_t ticket = 0;
+        if (cache || n <= VC_GROUP_MAX_SIGS) {
+          memcpy(p.data() + 16, qc.pre, 40);
+          memcpy(sig.data(), &v.a_sig[(size_t)i * 64], 64);
+          memcpy(pk.data(), &v.a_pk[(size_t)i * 32], 32);
+          memcpy(sig.data() + 64, qc.sig.data(), qc.sig.size());
+          memcpy(pk.data() + 32, qc.pk.data(), qc.pk.size());
+          rc = hs_queue_submit_msgs(q, p.data(), off, 2, sig.data(), pk.data(), midx.data(), modes.data(), n, nullptr, nullptr, &ticket);
+        }
+        if (rc == HS_OK) {
+          tickets.emplace_back(i, ticket);
+          continue;
+        }
+        if (rc != HS_ERR_NOMEM && rc != HS_ERR_ARG) errs++;
+        fallbacks += cache || n <= VC_GROUP_MAX_SIGS;
+        errs += vc_sync_timeout(ctx, v, i, bits);
+        sync_sigs += n;
+        vc_check(v, i, bits, mism, bad_acc);
+      }
+      for (auto &[i, ticket] : tickets) {
+        std::fill(bits.begin(), bits.end(), 0u);
+        errs += hs_queue_wait(q, ticket, bits.data()) != HS_OK;
+        vc_check(v, i, bits, mism, bad_acc);
+      }
+    });
+  const auto t0 = clk::now();
+  go = 1;
+  for (std::thread &x : th) x.join();
+  const double us = us_since(t0);
+  arm.mismatches += mism;
+  arm.bad_accepted += bad_acc;
+  arm.errors += errs;
+  arm.sync_sigs += sync_sigs;
+  arm.fallbacks += fallbacks;
+  return us;
+}
+// Arm (c): the Timeouts' authors in one hs_verify_tcs (one TC of N votes over round || high_qc.round), then each distinct QC once.
+static double vc_sync_burst(hs_ctx *ctx, const vc_burst &v, vc_arm &arm) {
+  const int N = v.N;
+  std::vector<uint32_t> ab((N + 31) / 32), vb[2], tcidx(N, 0);
+  std::vector<uint64_t> hq(N, v.hq);
+  const bool two = std::count(v.bad.begin(), v.bad.end(), 1) > 0;
+  const auto t0 = clk::now();
+  uint32_t tcb = 0;
+  arm.errors += hs_verify_tcs(ctx, &v.round, 1, v.a_pk.data(), nullptr, v.a_sig.data(), hq.data(), tcidx.data(), N, ab.data(), &tcb) != HS_OK;
+  for (int k = 0; k < 1 + two; k++) {
+    int ok = 0;
+    vb[k].assign((v.nv + 31) / 32, 0);
+    arm.errors += hs_verify_batch_shared_msg(ctx, v.qc[k].dig, v.qc[k].votes.data(), v.nv, &ok, vb[k].data()) != HS_OK;
+  }
+  const double us = us_since(t0);
+  arm.sync_sigs += N + (uint64_t)(1 + two) * v.nv;
+  std::atomic<int> mism{0}, bad_acc{0};
+  std::vector<uint32_t> bits((1 + v.nv + 31) / 32);
+  for (int i = 0; i < N; i++) {
+    std::fill(bits.begin(), bits.end(), 0u);
+    bits[0] = bit(ab, i);
+    for (int k = 0; k < v.nv; k++)
+      if (bit(vb[v.bad[i]], k)) bits[(k + 1) >> 5] |= 1u << ((k + 1) & 31);
+    vc_check(v, i, bits, mism, bad_acc);
+  }
+  arm.mismatches += mism;
+  arm.bad_accepted += bad_acc;
+  return us;
+}
+static uint64_t queue_sigs(hs_queue *q) {  // records the queue's launches and slow path carried
+  uint64_t s[HS_QUEUE_STATS] = {};
+  hs_queue_stats(q, s);
+  return s[1] + s[3] + s[5];
+}
+static int view_change(hs_ctx *ctx, int N, int bursts, bool warm, bool last) {
+  const committee_keys k = make_keys(N, 41);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  hs_queue *qa = nullptr, *qb = nullptr;
+  if (hs_queue_create(ctx, 0, &qa) != HS_OK || hs_queue_create(ctx, 0, &qb) != HS_OK) return 1;
+  hs_queue_cert_cache(qb, 64u << 20);
+  vc_arm arm[3];
+  uint64_t qsig[2] = {0, 0}, c0[HS_QUEUE_CERT_STATS] = {}, c1[HS_QUEUE_CERT_STATS] = {};
+  int bad = 0, inserted_in_bursts = 0;
+  vc_burst v;
+  for (int b = 0; b < bursts + 2; b++) {
+    const bool timed = b >= 2;
+    vc_make(k, b, warm, v);
+    if (warm) {  // the Block carrying the QC, through the cached queue first (not timed)
+      uint8_t bp[136 + 40];
+      for (int j = 0; j < 136; j++) bp[j] = (uint8_t)(b * 3 + j);
+      memcpy(bp + 136, v.qc[0].pre, 40);
+      const uint64_t off[3] = {0, 136, 176};
+      const int n = 1 + v.nv;
+      std::vector<uint8_t> sig((size_t)n * 64), pk((size_t)n * 32), modes(n, HS_MODE_BATCH_EQ);
+      std::vector<uint32_t> midx(n, 1), bits((n + 31) / 32);
+      midx[0] = 0;
+      modes[0] = HS_MODE_STRICT;
+      memcpy(sig.data() + 64, v.qc[0].sig.data(), v.qc[0].sig.size());
+      memcpy(pk.data() + 32, v.qc[0].pk.data(), v.qc[0].pk.size());
+      size_t ticket = 0;
+      bad += hs_queue_submit_msgs(qb, bp, off, 2, sig.data(), pk.data(), midx.data(), modes.data(), n, nullptr, nullptr, &ticket) != HS_OK;
+      hs_queue_wait(qb, ticket, bits.data());
+    }
+    uint64_t s0[2] = {queue_sigs(qa), queue_sigs(qb)};
+    uint64_t i0[HS_QUEUE_CERT_STATS] = {}, i1[HS_QUEUE_CERT_STATS] = {};
+    hs_queue_cert_stats(qb, i0);
+    if (timed && b == 2) memcpy(c0, i0, sizeof(c0));
+    vc_arm scratch[3];
+    vc_arm *use = timed ? arm : scratch;
+    const double ta = vc_queue_burst(ctx, qa, false, v, use[0]);
+    const double tb = vc_queue_burst(ctx, qb, true, v, use[1]);
+    const double tc = vc_sync_burst(ctx, v, use[2]);
+    hs_queue_cert_stats(qb, i1);
+    if (timed) {
+      arm[0].t.v.push_back(ta);
+      arm[1].t.v.push_back(tb);
+      arm[2].t.v.push_back(tc);
+      qsig[0] += queue_sigs(qa) - s0[0];
+      qsig[1] += queue_sigs(qb) - s0[1];
+      inserted_in_bursts += (int)(i1[4] - i0[4]);
+    }
+    for (vc_arm &a : scratch) bad += a.mismatches + a.bad_accepted + a.errors;
+  }
+  hs_queue_cert_stats(qb, c1);
+  const int f = (N - 1) / 3;
+  printf("\"%s_committee_%d\": {\"timeouts_per_burst\": %d, \"records_per_timeout\": %d, \"bad_qc_timeouts_per_burst\": %d, \"bursts\": %d, ", warm ? "warm" : "cold", N, N,
+         1 + N - f, warm ? (N + 2) / 10 : 0, bursts);
+  const char *names[3] = {"a_queue_no_cache_sync_fallback", "b_queue_cert_cache", "c_sync_verify_tcs_plus_qc"};
+  for (int a = 0; a < 3; a++) {
+    const uint64_t sigs = (a < 2 ? qsig[a] : 0) + arm[a].sync_sigs;
+    printf("\"%s\": {\"burst_p50_us\": %.1f, \"burst_p99_us\": %.1f, \"signatures_verified_per_burst\": %.0f, \"sync_fallbacks_per_burst\": %.1f, "
+           "\"mismatches\": %d, \"bad_qc_timeouts_accepted\": %d, \"errors\": %d}, ",
+           names[a], arm[a].t.pct(0.5), arm[a].t.pct(0.99), (double)sigs / bursts, (double)arm[a].fallbacks / bursts, arm[a].mismatches, arm[a].bad_accepted,
+           arm[a].errors);
+    bad += arm[a].mismatches + arm[a].bad_accepted + arm[a].errors;
+  }
+  static const char *cn[HS_QUEUE_CERT_STATS] = {"lookups", "hits", "joins", "records_answered", "inserted", "bytes_held"};
+  printf("\"cert_stats\": {");
+  for (int i = 0; i < HS_QUEUE_CERT_STATS; i++)
+    printf("\"%s\": %llu%s", cn[i], (unsigned long long)(i == 5 ? c1[i] : c1[i] - c0[i]), i + 1 < HS_QUEUE_CERT_STATS ? ", " : "");
+  printf("}, \"inserted_during_bursts\": %d}%s", inserted_in_bursts, last ? "" : ", ");
+  // every burst has a new QC: cold inserts it once per burst, warm inserted it before the burst and never inserts the bad copy
+  bad += inserted_in_bursts != (warm ? 0 : bursts);
+  hs_queue_destroy(qa);
+  hs_queue_destroy(qb);
+  return bad;
+}
+static int run_view_change(hs_ctx *ctx, int bursts) {
+  printf("\"view_change\": {\"gpu\": \"%s\", \"threads\": %d, \"ring_records\": 4096, \"cache_bytes\": %u, ", gpu_identity().c_str(), VC_THREADS, 64u << 20);
+  int bad = 0;
+  for (int warm = 0; warm < 2; warm++)
+    for (int N : {100, 1000, 4000}) bad += view_change(ctx, N, N == 100 ? 2 * bursts : bursts, warm == 1, warm == 1 && N == 4000);
+  printf("}");
+  return bad;
+}
+
 int main(int argc, char **argv) {
   const int rounds = argc > 1 ? atoi(argv[1]) : 1000;
   hs_ctx *ctx = nullptr;
@@ -637,6 +943,13 @@ int main(int argc, char **argv) {
   if (argc > 3 && strcmp(argv[3], "certificate_preimages") == 0) {
     printf("{");
     const int bad = run_certificate_preimages(ctx, argc > 2 ? atoi(argv[2]) : 20);
+    printf("}\n");
+    hs_ctx_destroy(ctx);
+    return bad ? 9 : 0;
+  }
+  if (argc > 3 && strcmp(argv[3], "view_change") == 0) {
+    printf("{");
+    const int bad = run_view_change(ctx, argc > 2 ? atoi(argv[2]) : 10);
     printf("}\n");
     hs_ctx_destroy(ctx);
     return bad ? 9 : 0;
@@ -753,6 +1066,8 @@ int main(int argc, char **argv) {
   burst_bad += block_during_burst(ctx, 10000, 16384, bursts, true);
   printf("}, ");
   burst_bad += run_certificate_preimages(ctx, bursts);
+  printf(", ");
+  burst_bad += run_view_change(ctx, bursts);
   printf("}\n");
   hs_ctx_destroy(ctx);
   return (bad || burst_bad) ? 9 : 0;

@@ -32,6 +32,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <random>
 #include <string>
 #include <string_view>
 #include <thread>
@@ -300,9 +301,172 @@ __device__ __forceinline__ void fe_shfl_down(fe &r, const fe &a, int delta) {
 #pragma unroll
   for (int i = 0; i < 8; i++) r.v[i] = __shfl_down_sync(0xffffffffu, a.v[i], delta);
 }
+
+// ------------------------------------------------------------------------------------------------ signature cache (hs_queue_sig_cache)
+// A queue's table in HBM of the records its kernels accepted under batch-eq: (sig[64] | pk[32] | msg[32]) -> the record's flag
+// byte.  The key bytes are the registered key's (C.pks), never its index: hs_committee_update reuses indices.  A record's flags
+// depend on these 128 bytes alone, so a hit (all 128 bytes equal) answers both verdict modes exactly and committee changes need
+// no flush.  Buckets of HS_SIG_WAYS entries; the bucket is a keyed mix of the 32 record words (a random key per queue, so records
+// cannot be aimed at one bucket from outside); a full bucket's victim comes from its round-robin counter.  Each entry is a seqlock:
+// seq 0 = never written, odd = being written, even = holds a record.  A writer claims with atomicCAS(seq, even, even + 1), writes,
+// fences and stores even + 2; a reader loads seq (acquire), the payload and flags (relaxed, so L1 is bypassed: the other queue
+// stream writes too), fences and re-reads seq: a hit needs both reads equal, even, non-zero, and every word equal.
+#define HS_SIG_WAYS 4
+struct sig_entry {
+  uint32_t w[32];  // sig | pk | msg
+  uint32_t seq;
+  uint32_t flags;
+  uint32_t pad[2];
+};
+static_assert(sizeof(sig_entry) == 144, "sig_entry is 144 bytes");
+struct sig_bucket {
+  sig_entry e[HS_SIG_WAYS];
+  uint32_t rr;  // round-robin victim counter
+  uint32_t pad[3];
+};
+// Counters of a request, summed per block into ctr[4 * slot ..] (slot = the request's ring slot) and moved to the mapped host array
+// by the block that completes the request, before its completion word: [0] records probed, [1] hits, [2] inserts, [3] inserts
+// that evicted a live entry.
+#define HS_SIG_CTRS 4
+struct sig_cache_dev {
+  sig_bucket *b;        // the table (nullptr when the launch runs without it)
+  const uint64_t *key;  // 32 words: the bucket mix's key
+  uint32_t bmask;       // buckets - 1
+  uint32_t *ctr;        // device: HS_SIG_CTRS per ring slot
+  uint32_t *hctr;       // mapped host: the same layout
+};
+#define HS_SIG_HIT 0x100u  // a probe's result: stored flags | HS_SIG_HIT (0 = miss)
+
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t *p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t *p) {
+  uint32_t v;
+  asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_relaxed_gpu(uint32_t *p, uint32_t v) {
+  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint64_t sig_mix(uint32_t w, uint64_t k) {  // splitmix64's finalizer of (word << 32) ^ key
+  uint64_t z = ((uint64_t)w << 32) ^ k;
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ uint32_t sig_bucket_of(const sig_cache_dev &sc, uint64_t h) { return (uint32_t)(h >> 32) & sc.bmask; }
+__device__ __forceinline__ uint32_t pick8(const uint32_t (&a)[8], int i) {  // a[i] without local memory
+  uint32_t r = a[0];
+#pragma unroll
+  for (int j = 1; j < 8; j++)
+    if (i == j) r = a[j];
+  return r;
+}
+// Warp-wide probe: lane l holds word l of the record.  Every lane must call it; the result is the same on every lane.
+__device__ __forceinline__ uint32_t sig_probe_warp(const sig_cache_dev &sc, uint32_t w, int lane, uint32_t &bucket) {
+  uint64_t h = sig_mix(w, __ldg(sc.key + lane));
+#pragma unroll
+  for (int d = 16; d; d >>= 1) h += __shfl_xor_sync(0xffffffffu, h, d);
+  bucket = sig_bucket_of(sc, h);
+  const sig_entry *x = sc.b[bucket].e;
+  uint32_t s0[HS_SIG_WAYS], m[HS_SIG_WAYS], f[HS_SIG_WAYS];
+#pragma unroll
+  for (int e = 0; e < HS_SIG_WAYS; e++) s0[e] = ld_acquire_gpu(&x[e].seq);
+#pragma unroll
+  for (int e = 0; e < HS_SIG_WAYS; e++) {
+    m[e] = ld_relaxed_gpu(x[e].w + lane);
+    f[e] = ld_relaxed_gpu(&x[e].flags);
+  }
+  __threadfence();
+#pragma unroll
+  for (int e = 0; e < HS_SIG_WAYS; e++) {
+    // each lane read its word between two equal reads of seq; the same even value on every lane makes them one version.  The
+    // shuffles stay outside any condition: every lane must reach them.
+    const uint32_t s1 = ld_relaxed_gpu(&x[e].seq), s_lane0 = __shfl_sync(0xffffffffu, s0[e], 0), fl = __shfl_sync(0xffffffffu, f[e], 0);
+    const bool ok = s0[e] != 0 && !(s0[e] & 1u) && s1 == s0[e] && s0[e] == s_lane0 && m[e] == w;
+    if (__all_sync(0xffffffffu, ok)) return fl | HS_SIG_HIT;
+  }
+  return 0;
+}
+// One thread's probe of its own record (k_verify_bulk): word(j) = word j of the record.
+template <class W>
+__device__ __forceinline__ uint32_t sig_probe_thread(const sig_cache_dev &sc, W word, uint32_t &bucket) {
+  uint64_t h = 0;
+#pragma unroll
+  for (int j = 0; j < 32; j++) h += sig_mix(word(j), __ldg(sc.key + j));
+  bucket = sig_bucket_of(sc, h);
+  const sig_entry *x = sc.b[bucket].e;
+#pragma unroll 1
+  for (int e = 0; e < HS_SIG_WAYS; e++) {
+    const uint32_t s0 = ld_acquire_gpu(&x[e].seq);
+    if (!s0 || (s0 & 1u) || ld_relaxed_gpu(x[e].w) != word(0)) continue;
+    bool eq = true;
+#pragma unroll
+    for (int j = 1; j < 32; j++) eq &= ld_relaxed_gpu(x[e].w + j) == word(j);
+    const uint32_t fl = ld_relaxed_gpu(&x[e].flags);
+    __threadfence();
+    if (eq && ld_relaxed_gpu(&x[e].seq) == s0) return fl | HS_SIG_HIT;
+  }
+  return 0;
+}
+// One thread inserts an accepted record into its bucket: a never-written entry if there is one, else the round-robin victim.  A
+// claim another writer won is retried, at most HS_SIG_WAYS times; then the record is simply not cached.  Returns 0: not inserted,
+// 1: inserted into a free entry, 2: inserted over a live entry.
+template <class W>
+__device__ __forceinline__ uint32_t sig_insert(const sig_cache_dev &sc, uint32_t bucket, W word, uint32_t flags) {
+  sig_bucket *b = sc.b + bucket;
+#pragma unroll 1
+  for (int attempt = 0; attempt < HS_SIG_WAYS; attempt++) {
+    int e = -1;
+    uint32_t old = 0;
+#pragma unroll 1
+    for (int i = 0; i < HS_SIG_WAYS && e < 0; i++)
+      if (ld_relaxed_gpu(&b->e[i].seq) == 0) e = i;
+    if (e < 0) {
+      e = (int)(atomicAdd(&b->rr, 1u) % HS_SIG_WAYS);
+      old = ld_relaxed_gpu(&b->e[e].seq);
+      if (old & 1u) continue;
+    }
+    sig_entry *x = b->e + e;
+    if (atomicCAS(&x->seq, old, old + 1) != old) continue;
+    __threadfence();
+#pragma unroll
+    for (int j = 0; j < 32; j++) st_relaxed_gpu(x->w + j, word(j));
+    st_relaxed_gpu(&x->flags, flags);
+    __threadfence();
+    st_relaxed_gpu(&x->seq, old + 2);
+    return old ? 2u : 1u;
+  }
+  return 0;
+}
+// A block's counts for request slot `req`, ordered before the block's completion add.
+__device__ __forceinline__ void sig_count(const sig_cache_dev &sc, uint32_t req, uint32_t probed, uint32_t hits, uint32_t ins, uint32_t ev) {
+  uint32_t *c = sc.ctr + HS_SIG_CTRS * (size_t)req;
+  if (probed) atomicAdd(c, probed);
+  if (hits) atomicAdd(c + 1, hits);
+  if (ins) atomicAdd(c + 2, ins);
+  if (ev) atomicAdd(c + 3, ev);
+  __threadfence();
+}
+// The block completing request slot `req` moves its counts to the host and clears them for the slot's next request.
+__device__ __forceinline__ void sig_publish(const sig_cache_dev &sc, uint32_t req) {
+#pragma unroll
+  for (int k = 0; k < HS_SIG_CTRS; k++) sc.hctr[HS_SIG_CTRS * (size_t)req + k] = atomicExch(sc.ctr + HS_SIG_CTRS * (size_t)req + k, 0u);
+}
+// Per-kernel shared scratch of the cache-on instantiations only (the cache-off kernels keep their shared-memory size).
+template <int N>
+__device__ __forceinline__ uint32_t *sig_smem() {
+  __shared__ __align__(16) uint32_t s[N];
+  return s;
+}
+
+// SIGC: probe and fill the signature cache.  The cache-off instantiation is the kernel without it, instruction for instruction.
+template <bool SIGC>
 __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict__ ring, uint32_t base, uint32_t mask, const ge_niels *__restrict__ btable,
                                                       committee_tables C, const comb_params cp, uint8_t *out_flags, uint32_t *counters,
-                                                      volatile uint32_t *done, uint32_t seq) {
+                                                      volatile uint32_t *done, uint32_t seq, sig_cache_dev sc) {
   __shared__ int32_t dig[HS_MAX_DIGITS];
   __shared__ fe sh_acc[3], sh_r[2];
   __shared__ uint32_t sh_meta[2];
@@ -316,6 +480,43 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
   const bool have_key = v < C.n_keys;
   if (!have_key) v = 0;
   const uint32_t a_flags = have_key ? C.key_flags[v] : 0u;
+  uint32_t *sk = nullptr;  // cache on: [0, 32) the record's words, [32] the probe's result, [33] its bucket
+  if constexpr (SIGC) {
+    sk = sig_smem<34>();
+    if (warp == 0) {
+      uint32_t hit = 0, bucket = 0;
+      if (have_key) {  // slow-path riders (HS_NO_KEY) neither probe nor insert
+        uint32_t A[8], M[8];
+        load32(A, C.pks + (size_t)v * 32);
+        load32(M, rec->msg);
+        const int j = lane & 7;
+        const uint32_t w = lane < 8 ? pick8(R, j) : lane < 16 ? pick8(S, j) : lane < 24 ? pick8(A, j) : pick8(M, j);
+        sk[lane] = w;
+        hit = sig_probe_warp(sc, w, lane, bucket);
+      }
+      if (lane == 0) {
+        sk[32] = hit;
+        sk[33] = bucket;
+      }
+    }
+    __syncthreads();
+    const uint32_t hit = sk[32];
+    if (hit) {  // the stored flags, then the counter and completion step; no hashing, no decompression
+      if (threadIdx.x == 0) {
+        out_flags[slot] = (uint8_t)hit;
+        const uint32_t req = rec->req;
+        sig_count(sc, req, 1, 1, 0, 0);
+        __threadfence_system();
+        if (atomicAdd(counters + req, 1u) == rec->req_n - 1) {
+          sig_publish(sc, req);
+          counters[req] = 0;
+          __threadfence_system();
+          done[req] = seq;
+        }
+      }
+      return;
+    }
+  }
   if (warp == 0) {
     uint32_t A[8], M[8], h[16], k[8];
     load32(A, C.pks + (size_t)v * 32);
@@ -375,9 +576,14 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
     if (eq) fl |= HS_F_EQ;
     if (eq && !(fl & HS_F_SMALL)) fl |= HS_F_STRICT;
     out_flags[slot] = (uint8_t)fl;
+    if constexpr (SIGC) {
+      const uint32_t ins = (have_key && (fl & HS_F_EQ)) ? sig_insert(sc, sk[33], [&](int j) { return sk[j]; }, fl) : 0u;
+      sig_count(sc, rec->req, have_key ? 1u : 0u, 0, ins != 0, ins == 2);
+    }
     __threadfence_system();
     const uint32_t req = rec->req;
     if (atomicAdd(counters + req, 1u) == rec->req_n - 1) {
+      if constexpr (SIGC) sig_publish(sc, req);
       counters[req] = 0;
       __threadfence_system();
       done[req] = seq;
@@ -397,12 +603,16 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
 // Sizing: 128 threads, at least 3 blocks per SM.  R and the request fields stay live across the comb, so the 4-block budget of
 // k_verify_main (128 registers) spilled; 3 blocks allow 168 (sm_90a: 142 registers, 0 spills, 36,864 bytes smem).  A 6,668-record
 // certificate is 53 blocks, one per SM, so occupancy does not bound this launch at committee sizes.
+// SIGC (signature cache on): each thread probes its own record first; a hit skips the hash and the comb but still takes part in
+// every barrier (Z = 1 in the block's inversion) and writes the stored flags; a miss that verifies under batch-eq is inserted.  S, A
+// and M wait for the insert in shared memory (12 KB more: 48 KB, the static limit), so they need not stay live across the comb.
 #define HS_BULK_THREADS 128
 #define HS_BULK_MINBLOCKS 3
+template <bool SIGC>
 __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_bulk(const small_rec *__restrict__ ring, uint32_t base, uint32_t mask,
                                                                                   uint32_t n, const ge_niels *__restrict__ btable, committee_tables C,
                                                                                   const comb_params cp, uint8_t *out_flags, uint32_t *counters,
-                                                                                  volatile uint32_t *done, uint32_t seq) {
+                                                                                  volatile uint32_t *done, uint32_t seq, sig_cache_dev sc) {
   // one buffer, two lives: record staging while loading, then the signed digits [digit][thread] (conflict-free columns)
   __shared__ __align__(16) unsigned char smem_raw[HS_MAX_DIGITS * HS_BULK_THREADS * 4];
   static_assert(sizeof(smem_raw) >= (HS_BULK_THREADS / 32) * 256 * sizeof(uint4), "staging does not fit");
@@ -434,15 +644,40 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
   const uint32_t req = q[6].y, req_n = q[6].z;
   const bool have_key = v < C.n_keys;  // HS_NO_KEY (cannot reach this path: kept as in k_verify_small) rejects the record
   if (!have_key) v = 0;
+  // cache on: record word j >= 8 of thread t (S, A, M) at keep[((j - 8) / 4 * HS_BULK_THREADS + t) * 4 + j % 4]; R stays in
+  // registers across the comb anyway (verify_flags_from reads it)
+  uint32_t *keep = nullptr;
+  uint32_t hit = 0, bucket = 0;
+  const bool probed = SIGC && have_key && threadIdx.x < cnt;
   {
     uint32_t M[8];
     M[0] = q[4].x; M[1] = q[4].y; M[2] = q[4].z; M[3] = q[4].w; M[4] = q[5].x; M[5] = q[5].y; M[6] = q[5].z; M[7] = q[5].w;
     load32(A, C.pks + (size_t)v * 32);  // hash the registered key bytes, as k_verify_main<true>
-    sha512_ram32(h, R, A, M);
+    if constexpr (SIGC) {
+      keep = sig_smem<24 * HS_BULK_THREADS>();
+      uint4 *k4 = reinterpret_cast<uint4 *>(keep) + threadIdx.x;
+      k4[0] = q[2];
+      k4[HS_BULK_THREADS] = q[3];
+      k4[2 * HS_BULK_THREADS] = make_uint4(A[0], A[1], A[2], A[3]);
+      k4[3 * HS_BULK_THREADS] = make_uint4(A[4], A[5], A[6], A[7]);
+      k4[4 * HS_BULK_THREADS] = q[4];
+      k4[5 * HS_BULK_THREADS] = q[5];
+      if (probed)
+        hit = sig_probe_thread(
+            sc, [&](int j) { return j < 8 ? R[j] : j < 16 ? S[j - 8] : j < 24 ? A[j - 16] : M[j - 24]; }, bucket);
+    }
+    if (!hit) sha512_ram32(h, R, A, M);
   }
   ge_ext acc;
-  uint32_t meta = verify_committee_main(acc, R, S, h, btable, C.atables + (size_t)v * C.table_entries, have_key ? C.key_flags[v] : 0u,
-                                        reinterpret_cast<int32_t *>(smem_raw) + threadIdx.x, HS_BULK_THREADS, cp);
+  uint32_t meta = 0;
+  if (!hit) {
+    meta = verify_committee_main(acc, R, S, h, btable, C.atables + (size_t)v * C.table_entries, have_key ? C.key_flags[v] : 0u,
+                                 reinterpret_cast<int32_t *>(smem_raw) + threadIdx.x, HS_BULK_THREADS, cp);
+  } else {
+    fe_set0(acc.X);
+    fe_set0(acc.Y);
+    fe_set1(acc.Z);
+  }
   if (!have_key) meta = 0;
   if (fe_is_zero(acc.Z)) {  // cannot happen for curve points; keeps one bad record from poisoning the block's inversion
     fe_set1(acc.Z);
@@ -468,13 +703,32 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
     tot[b + 1] = u;
     tot[b] = inv;
   }
-  __syncthreads();
-  if (threadIdx.x < cnt) {
-    out_flags[(base + t) & mask] = (uint8_t)verify_flags_from(acc.X, acc.Y, tot[threadIdx.x], R, meta);
-    __threadfence_system();
+  if constexpr (SIGC) {  // the digit slots are free now (every thread is past the comb): word 0 gathers the block's counts
+    if (threadIdx.x == 0) *reinterpret_cast<uint32_t *>(smem_raw) = 0;
   }
   __syncthreads();
+  uint32_t ins = 0;
+  if (threadIdx.x < cnt) {
+    const uint32_t fl = hit ? (hit & 0xffu) : verify_flags_from(acc.X, acc.Y, tot[threadIdx.x], R, meta);
+    out_flags[(base + t) & mask] = (uint8_t)fl;
+    if constexpr (SIGC) {
+      if (probed && !hit && (fl & HS_F_EQ))
+        ins = sig_insert(
+            sc, bucket, [&](int j) { return j < 8 ? R[j] : keep[(((j - 8) >> 2) * HS_BULK_THREADS + threadIdx.x) * 4 + (j & 3)]; }, fl);
+    }
+    __threadfence_system();
+  }
+  if constexpr (SIGC) {  // the block's counts, a byte each (at most 128), summed per warp and then in shared memory: one barrier
+    uint32_t *sum = reinterpret_cast<uint32_t *>(smem_raw);
+    const uint32_t w = __reduce_add_sync(0xffffffffu, (probed ? 1u : 0u) | (hit ? 1u << 8 : 0u) | (ins ? 1u << 16 : 0u) | (ins == 2 ? 1u << 24 : 0u));
+    if (lane == 0) atomicAdd(sum, w);
+    __syncthreads();
+    if (threadIdx.x == 0) sig_count(sc, req, *sum & 0xffu, (*sum >> 8) & 0xffu, (*sum >> 16) & 0xffu, *sum >> 24);
+  } else {
+    __syncthreads();
+  }
   if (threadIdx.x == 0 && atomicAdd(counters + req, cnt) == req_n - cnt) {  // thread 0 holds a record of the request
+    if constexpr (SIGC) sig_publish(sc, req);
     counters[req] = 0;
     __threadfence_system();
     done[req] = seq;
@@ -1303,7 +1557,8 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
   const uint32_t seq = ++c->small_seq ? c->small_seq : ++c->small_seq;  // never 0
   committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
   if (c->ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_tables, 0));
-  k_verify_small<<<(unsigned)n, 64, 0, c->stream>>>(d_in, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, d_out, c->d_small_counter, d_done, seq);
+  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(d_in, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, d_out, c->d_small_counter, d_done, seq,
+                                                           sig_cache_dev{});
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   volatile uint32_t *done = c->h_small_done;
@@ -1453,6 +1708,7 @@ struct hs_queue {
     uint32_t seq;
     uint64_t lo, hi;  // ring positions it covers
     bool bulk;        // k_verify_bulk on bulk_stream (one request), else k_verify_small on stream
+    uint32_t sig_gen;  // the signature cache's table it probed (0: launched without the cache)
   };
   std::deque<launch> inflight;  // in ring order
   uint64_t head = 0, launched = 0, tail = 0;
@@ -1468,6 +1724,13 @@ struct hs_queue {
   std::unordered_map<cert_key, cert_flight, cert_key_hash> cc_flights;  // keyed by the primary's span key
   std::vector<cert_req *> cc_ready;  // answered entirely at submit: the queue's thread completes them
   uint64_t cstats[HS_QUEUE_CERT_STATS] = {};  // hs_queue_cert_stats ([5] is cc_bytes)
+  // signature cache (hs_queue_sig_cache): off while d_sig is null.  The table, its key and bmask change only under c->mu after
+  // both streams drained; sig_gen (also under mu) numbers the tables, so counts of a replaced table's launches are not held.
+  sig_bucket *d_sig = nullptr;
+  uint64_t *d_sig_key = nullptr;
+  uint32_t sig_bmask = 0, sig_gen = 0;
+  uint32_t *d_sig_ctr = nullptr, *h_sig_ctr = nullptr, *d_sig_hctr = nullptr;  // HS_SIG_CTRS per ring slot (allocated on first use)
+  uint64_t sstats[HS_QUEUE_SIG_STATS] = {};  // hs_queue_sig_stats ([4]: inserts - evictions into the current table)
   std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
   std::condition_variable cv_work, cv_done;
   std::thread th;
@@ -1602,7 +1865,8 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         if (s.vidx == HS_NO_KEY) all = false;
       }
       const bool bulk = all && r.n >= HS_QUEUE_BULK_MIN;
-      if (!all) {
+      if (!all) {  // every record of a slow-path request rides as HS_NO_KEY: none of them probes or fills the signature cache
+        for (uint32_t i = 0; i < r.n; i++) q->h_ring[(p + i) & q->mask].vidx = HS_NO_KEY;
         r.seq = 0;
         slow.push_back(p);
       } else {
@@ -1653,11 +1917,22 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
           }
         }
         if (e == cudaSuccess) {
-          if (L.bulk)
-            k_verify_bulk<<<(n + HS_BULK_THREADS - 1) / HS_BULK_THREADS, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp,
-                                                                                                  q->d_flags, q->d_counters, q->d_done, L.seq);
-          else
-            k_verify_small<<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq);
+          const unsigned bulk_blocks = (n + HS_BULK_THREADS - 1) / HS_BULK_THREADS;
+          if (q->d_sig) {
+            const sig_cache_dev sc{q->d_sig, q->d_sig_key, q->sig_bmask, q->d_sig_ctr, q->d_sig_hctr};
+            L.sig_gen = q->sig_gen;
+            if (L.bulk)
+              k_verify_bulk<true><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters,
+                                                                         q->d_done, L.seq, sc);
+            else
+              k_verify_small<true><<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq, sc);
+          } else if (L.bulk) {
+            k_verify_bulk<false><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters,
+                                                                        q->d_done, L.seq, sig_cache_dev{});
+          } else {
+            k_verify_small<false><<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq,
+                                                   sig_cache_dev{});
+          }
           c->launches++;
           e = cudaGetLastError();
         }
@@ -1774,6 +2049,11 @@ static void queue_watch(hs_queue *q) {
             const uint32_t want = (q->modes[s] == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
             if (((volatile uint8_t *)q->h_flags)[s] & want) bits[i >> 5] |= 1u << (i & 31);
           }
+          if (L.sig_gen) {  // the completing block moved the request's signature-cache counts here before its completion word
+            const volatile uint32_t *sc = q->h_sig_ctr + HS_SIG_CTRS * (size_t)(p & q->mask);
+            for (int k = 0; k < HS_SIG_CTRS; k++) q->sstats[k] += sc[k];
+            if (L.sig_gen == q->sig_gen) q->sstats[4] += sc[2] - sc[3];
+          }
           queue_finish_locked(q, p, HS_OK, bits, fire);
         } else if (qe == cudaErrorNotReady) {
           open = true;
@@ -1851,6 +2131,10 @@ static void queue_free(hs_queue *q) {
   cudaFree(q->d_counters);
   cudaFree(q->d_stage);
   cudaFree(q->d_digs);
+  cudaFree(q->d_sig);
+  cudaFree(q->d_sig_key);
+  cudaFree(q->d_sig_ctr);
+  if (q->h_sig_ctr) cudaFreeHost(q->h_sig_ctr);
   delete q;
 }
 
@@ -3145,6 +3429,68 @@ int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]) {
   std::lock_guard<std::mutex> g(q->mu);
   q->cstats[5] = q->cc_bytes;
   memcpy(out, q->cstats, sizeof(q->cstats));
+  return HS_OK;
+}
+
+#define HS_QUEUE_SIG_MAX_ENTRIES (1ull << 26)  // 9.7 GB of table
+int hs_queue_sig_cache(hs_queue *q, size_t entries) {
+  if (!q || entries > HS_QUEUE_SIG_MAX_ENTRIES) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_cache: bad argument");
+  hs_ctx *c = q->c;
+  uint32_t buckets = 0;
+  if (entries)
+    for (buckets = 1; (size_t)buckets * HS_SIG_WAYS < entries;) buckets <<= 1;
+  std::lock_guard<std::mutex> g(c->mu);  // the dispatcher launches only while it holds c->mu
+  if (buckets == (q->d_sig ? q->sig_bmask + 1 : 0u)) return HS_OK;
+  HS_CUDA(c, cudaSetDevice(c->device));
+  // Drains the queue's streams: no launch that probes the old table survives these lines.
+  HS_CUDA(c, cudaStreamSynchronize(q->stream));
+  HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));
+  cudaFree(q->d_sig);
+  q->d_sig = nullptr;
+  {
+    std::lock_guard<std::mutex> gq(q->mu);
+    q->sig_gen++;
+    q->sstats[4] = 0;
+  }
+  if (!buckets) return HS_OK;
+  if (!q->d_sig_ctr) {  // first use: the per-slot counters and the bucket mix's key (random per queue)
+    uint64_t key[32];
+    std::random_device rd;
+    for (uint64_t &k : key) k = ((uint64_t)rd() << 32) ^ rd();
+    const size_t cb = (size_t)q->cap * HS_SIG_CTRS * 4;
+    cudaError_t e = cudaMalloc(&q->d_sig_key, sizeof(key));
+    if (e == cudaSuccess) e = cudaMemcpy(q->d_sig_key, key, sizeof(key), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaHostAlloc(&q->h_sig_ctr, cb, cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_sig_hctr, q->h_sig_ctr, 0);
+    if (e == cudaSuccess) e = cudaMalloc(&q->d_sig_ctr, cb);
+    if (e == cudaSuccess) e = cudaMemsetAsync(q->d_sig_ctr, 0, cb, q->stream);
+    if (e != cudaSuccess) {  // the cache stays off; a later call starts the first use over
+      cudaFree(q->d_sig_key);
+      cudaFree(q->d_sig_ctr);
+      if (q->h_sig_ctr) cudaFreeHost(q->h_sig_ctr);
+      q->d_sig_key = nullptr;
+      q->d_sig_ctr = q->h_sig_ctr = q->d_sig_hctr = nullptr;
+      return fail(c, HS_ERR_CUDA, "hs_queue_sig_cache", e);
+    }
+  }
+  sig_bucket *t = nullptr;
+  const size_t bytes = (size_t)buckets * sizeof(sig_bucket);
+  cudaError_t e = cudaMalloc(&t, bytes);
+  if (e == cudaSuccess) e = cudaMemsetAsync(t, 0, bytes, q->stream);  // ahead of every launch that probes it
+  if (e == cudaSuccess) e = cudaStreamSynchronize(q->stream);
+  if (e != cudaSuccess) {
+    cudaFree(t);
+    return fail(c, e == cudaErrorMemoryAllocation ? HS_ERR_NOMEM : HS_ERR_CUDA, "hs_queue_sig_cache", e);
+  }
+  q->sig_bmask = buckets - 1;
+  q->d_sig = t;
+  return HS_OK;
+}
+
+int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, q->sstats, sizeof(q->sstats));
   return HS_OK;
 }
 

@@ -450,6 +450,21 @@ class VerifyQueue:
         self.engine._check(self.lib.hs_queue_cert_stats(self.h, out), "hs_queue_cert_stats")
         return dict(zip(self.CERT_STATS, (int(x) for x in out)))
 
+    def sig_cache(self, entries):
+        """Turns the signature cache on (hs_queue_sig_cache): a table in HBM of at least `entries` records the queue's kernels
+        accepted, so a signature verified once (a Timeout's author vote, then the same vote in the TC) is a probe that hits instead
+        of a verify.  Verdicts do not change.  Resizing starts from an empty table; 0 turns it off (the default)."""
+        self.engine._check(self.lib.hs_queue_sig_cache(self.h, int(entries)), "hs_queue_sig_cache")
+
+    SIG_STATS = ("probed", "hits", "inserts", "evictions", "entries_held")
+
+    def sig_stats(self):
+        """Counters of the signature cache over completed launches (hs_queue_sig_stats): records probed, hits, inserts, inserts
+        that evicted a live entry, and the entries held now."""
+        out = (ctypes.c_uint64 * len(self.SIG_STATS))()
+        self.engine._check(self.lib.hs_queue_sig_stats(self.h, out), "hs_queue_sig_stats")
+        return dict(zip(self.SIG_STATS, (int(x) for x in out)))
+
     def close(self):
         """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""
         if getattr(self, "h", None):

@@ -212,6 +212,9 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *   - hs_queue_cert_cache (off by default) lets the queue verify a certificate that many requests carry once: during a view
  *     change every Timeout carries the same high_qc, and a copy that is in flight is joined and one that verified is a hit, so
  *     each Timeout puts only its author's record in the ring.  Verdicts do not change.
+ *   - hs_queue_sig_cache (off by default) lets the queue's kernels verify each accepted signature once: a TC's votes are the
+ *     Timeouts' author signatures the replica verified a moment earlier, so with the cache on they are probes that hit.  Verdicts
+ *     do not change.
  *   - hs_queue_destroy completes every request in flight (callbacks fire) and joins the thread; hs_ctx_destroy destroys the
  *     queues still attached to the context.  hs_kernel_launches counts the queue's launches; hs_queue_stats tells them apart. */
 typedef struct hs_queue hs_queue;
@@ -263,6 +266,24 @@ int hs_queue_cert_cache(hs_queue *q, size_t max_bytes);
 /* [0] spans looked up, [1] cache hits, [2] in-flight joins, [3] records answered without verifying them,
  * [4] spans inserted, [5] bytes held now */
 int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]);
+/* Signature cache of the queue's device path: a table in HBM of the records its kernels accepted, so a signature the node already
+ * verified (a Timeout's author vote, then the same vote inside the TC and the Block carrying it) costs a probe, not a verify.
+ *   - A cached record is (sig[64], pk[32], msg[32]) with the KEY BYTES, never a committee index (hs_committee_update reuses
+ *     indices), mapped to the record's flag byte (both verdicts), so a hit answers either mode exactly: a small-order key accepted
+ *     under batch-eq is still rejected strict.  A hit needs all 128 bytes equal; verdicts are bit for bit those of the same request
+ *     with the cache off, and committee changes do not flush the cache (a record's flags depend only on its bytes).
+ *   - Only records that verified under batch-eq with a registered key are inserted; rejected records are verified every time.
+ *   - Only device-path records take part: slow-path requests and riders neither probe nor insert.  Hit records keep their ring
+ *     slot and their place in the launch (only the curve arithmetic is skipped); the ring, arena, completion, tickets and
+ *     hs_queue_stats do not change.
+ * entries: 0 = off (the default: the queue launches exactly the kernels it launches without this call); otherwise the table holds
+ * at least `entries` records (buckets of 4 entries of 144 bytes, a power of two of buckets), at most 2^26.  Changing the size or
+ * turning it off first drains the queue's launches in flight and starts from an empty table.  HS_ERR_NOMEM: no device memory. */
+int hs_queue_sig_cache(hs_queue *q, size_t entries);
+#define HS_QUEUE_SIG_STATS 5
+/* Counters of completed launches: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live entry,
+ * [4] entries held now */
+int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

@@ -125,6 +125,14 @@ class VerifyQueue {
     e_.check(hs_queue_cert_stats(q_, s.data()), "hs_queue_cert_stats");
     return s;
   }
+  // hs_queue_sig_cache: a table of at least `entries` accepted records (0 = off, the default).  Verdicts do not change.
+  void sig_cache(size_t entries) { e_.check(hs_queue_sig_cache(q_, entries), "hs_queue_sig_cache"); }
+  // hs_queue_sig_stats: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live entry, [4] entries held now.
+  std::array<uint64_t, HS_QUEUE_SIG_STATS> sig_stats() const {
+    std::array<uint64_t, HS_QUEUE_SIG_STATS> s{};
+    e_.check(hs_queue_sig_stats(q_, s.data()), "hs_queue_sig_stats");
+    return s;
+  }
 
  private:
   struct Pending {

@@ -25,10 +25,11 @@ extern "C" {
 
 static ENABLE: Once = Once::new();
 
-/// Turns the cache on for the node-wide queue, once.  A failure leaves it off: every request is then verified in full, with
-/// the same verdicts.
+/// Turns the cache on for the node-wide queue, once, and the queue's signature cache with it.  A failure leaves a cache off:
+/// every request is then verified in full, with the same verdicts.
 pub(crate) fn enable(q: *mut HsQueue) {
     ENABLE.call_once(|| { let _ = unsafe { hs_queue_cert_cache(q, CERT_CACHE_BYTES) }; });
+    super::sig_cache::enable(q);
 }
 
 /// The cache's counters for the node's metrics: spans looked up, hits, in-flight joins, records answered without verifying them,

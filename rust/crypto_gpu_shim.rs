@@ -29,6 +29,10 @@ pub mod msgs_queue;
 /// (`msgs_queue::verify_timeout_queued`).
 #[path = "crypto_gpu_cert_cache.rs"]
 pub mod cert_cache;
+/// The queue's signature cache (hs_queue_sig_cache): a vote verified in a Timeout is a cache hit in the TC and the Block after
+/// it.  Turned on with the certificate cache (`cert_cache::enable`).
+#[path = "crypto_gpu_sig_cache.rs"]
+pub mod sig_cache;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

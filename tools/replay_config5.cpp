@@ -27,6 +27,10 @@
 // (a) by hashing the preimages on the caller's thread then hs_queue_submit_group, (b) by hs_queue_submit_msgs (the GPU hashes them),
 // (c) synchronously; latency and the caller thread's CPU time per certificate, plus hs_queue_digest_stats.
 //
+// TC after Timeouts (alone with argv[3] = tc_after_timeouts): N = 100, 1,000 and 4,000 Timeouts through the queue, then the TC made
+// of their author signatures and the Block carrying it: synchronous calls vs. the queue without vs. with its signature cache.
+// Signature-cache cost (alone with argv[3] = sig_cache_cost): the vote burst and replica_block sections with the cache off, then on.
+//
 // View change (last; alone with argv[3] = view_change): N = 100, 1,000 and 4,000 Timeouts released at once to 16 threads, nearly all
 // carrying the same high_qc, through (a) the queue without its certificate cache (synchronous fallback as the Rust module), (b) the
 // queue with it, (c) the synchronous batched calls; burst time, signatures verified and hs_queue_cert_stats.
@@ -86,6 +90,9 @@ static void on_vote(void *user, size_t, int status, const uint32_t *bitmap) {
   *v->lat = us_since(v->t0);
   __atomic_store_n(v->verdict, status == HS_OK ? (int)(bitmap[0] & 1u) : -1, __ATOMIC_RELEASE);
 }
+// Signature-cache entries of the queues the vote burst and replica_block sections create (0 = off, as in the default run; the
+// sig_cache_cost section runs them both ways).
+static size_t g_sig_entries = 0;
 // One committee size: `bursts` timed bursts (+3 warm-up) of N - f votes per arm.
 static int vote_burst(hs_ctx *ctx, int N, int bursts, bool last) {
   const int f = (N - 1) / 3, nv = N - f, nth = 16;
@@ -98,6 +105,7 @@ static int vote_burst(hs_ctx *ctx, int N, int bursts, bool last) {
   if (hs_committee_register(ctx, pks.data(), N, valid.data()) != HS_OK) return 1;
   hs_queue *q = nullptr;
   if (hs_queue_create(ctx, 0, &q) != HS_OK) return 1;
+  if (g_sig_entries && hs_queue_sig_cache(q, g_sig_entries) != HS_OK) return 1;
   burst_arm a, b, c;
   std::vector<hs_rec128> recs(nv);
   std::vector<int> want(nv), got(nv);
@@ -933,6 +941,289 @@ static int run_view_change(hs_ctx *ctx, int bursts) {
   return bad;
 }
 
+// The queue's signature-cache counters since `since` (hs_queue_sig_stats), as a JSON object.
+static void emit_sig_stats(hs_queue *q, const uint64_t (&since)[HS_QUEUE_SIG_STATS], const char *key = "sig_stats") {
+  static const char *names[HS_QUEUE_SIG_STATS] = {"probed", "hits", "inserts", "evictions", "entries_held"};
+  uint64_t s[HS_QUEUE_SIG_STATS] = {};
+  hs_queue_sig_stats(q, s);
+  printf("\"%s\": {", key);
+  for (int i = 0; i < HS_QUEUE_SIG_STATS; i++)
+    printf("\"%s\": %llu%s", names[i], (unsigned long long)(i == 4 ? s[i] : s[i] - since[i]), i + 1 < HS_QUEUE_SIG_STATS ? ", " : "");
+  printf("}");
+}
+
+// ---- the cost of a probe that misses (alone with argv[3] = sig_cache_cost): the leader vote burst (N = 100, 1,000) and
+// replica_block (N = 100 .. 6,000) with the signature cache off, then on.  Every section gets a queue of its own (the committees
+// share keys, so one queue would see the same votes again), and within one every vote and every Block is new: every probe misses
+// and every accepted record is inserted, so the difference is what the probe and the insert cost.
+#define SIG_COST_ENTRIES (1u << 16)
+static int run_sig_cache_cost(hs_ctx *ctx, int bursts) {
+  printf("\"sig_cache_cost\": {\"gpu\": \"%s\", \"entries\": %u, ", gpu_identity().c_str(), SIG_COST_ENTRIES);
+  int bad = 0;
+  for (int on = 0; on < 2; on++) {
+    g_sig_entries = on ? SIG_COST_ENTRIES : 0;
+    printf("\"%s\": {\"leader_vote_burst\": {", on ? "cache_on" : "cache_off");
+    for (int N : {100, 1000}) bad += vote_burst(ctx, N, bursts, N == 1000);
+    printf("}, \"replica_block\": {\"ring_records\": 16384, ");
+    for (int N : {100, 1000, 3000, 6000}) {
+      hs_queue *q = nullptr;
+      if (hs_queue_create(ctx, 16384, &q) != HS_OK || (on && hs_queue_sig_cache(q, SIG_COST_ENTRIES) != HS_OK)) return bad + 1;
+      const uint64_t z[HS_QUEUE_SIG_STATS] = {};
+      bad += replica_block(ctx, q, N, bursts, false);
+      const std::string key = "sig_stats_committee_" + std::to_string(N);
+      emit_sig_stats(q, z, key.c_str());
+      printf("%s", N == 6000 ? "" : ", ");
+      hs_queue_destroy(q);
+    }
+    printf("}}%s", on ? "" : ", ");
+  }
+  g_sig_entries = 0;
+  printf("}");
+  return bad;
+}
+
+// ---- TC after Timeouts (alone with argv[3] = tc_after_timeouts): one view change per round at N = 100, 1,000 and 4,000.  N
+// Timeouts go through the queue first (16 threads, hs_queue_submit_msgs, certificate cache on): record 0 the author's strict
+// signature over round || high_qc.round (16 bytes), records 1.. the shared high_qc's N - f batch-eq votes over hash || round (40
+// bytes); 1 % of the author signatures are corrupted.  Then the TC: the first N - f Timeouts' (author, signature, high_qc.round)
+// triples, strict, each over its own 16-byte preimage (the corrupted ones included: they must be rejected again).  Then the Block
+// carrying that TC: a strict author signature over the Block preimage, the QC's votes batch-eq, the TC's votes strict.  The TC and
+// the Block are timed (submit -> verdict, one at a time) in three arms:
+//   (a) synchronous: hs_verify_tcs (TC) / hs_verify_groups (Block), no Timeouts needed;
+//   (b) the queue without the signature cache;  (c) the queue with it.
+// Each of (b) and (c) has its own queue (16,384 records, certificate cache 64 MB) that saw the round's Timeouts first.
+struct tc_round {
+  std::vector<uint8_t> qsig, qpk, asig, apk, qp, bp, bsig;  // QC votes, Timeout authors (N), QC preimage, Block preimage, Block author
+  std::vector<uint8_t> tpre;                                // the Timeouts' 16-byte preimages (all equal: one high_qc)
+  std::vector<uint32_t> a_want, q_want;                     // oracle: authors strict, QC votes batch-eq
+  uint64_t round = 0, hq = 0;
+  uint32_t bkey = 0;
+  bool b_want = false;
+};
+static void tc_make(const committee_keys &k, int r, tc_round &t) {
+  const int N = k.N, nv = N - (N - 1) / 3;
+  t.round = 9000 + (uint64_t)r * 2;
+  t.hq = t.round - 1;
+  t.qp.resize(40);
+  for (int j = 0; j < 32; j++) t.qp[j] = (uint8_t)(r * 19 + j * 5 + 2);
+  memcpy(&t.qp[32], &t.hq, 8);
+  t.tpre.resize(16);
+  memcpy(&t.tpre[0], &t.round, 8);
+  memcpy(&t.tpre[8], &t.hq, 8);
+  t.bp.resize(136);
+  for (size_t j = 0; j < t.bp.size(); j++) t.bp[j] = (uint8_t)(r * 3 + j * 17 + 9);
+  uint8_t qd[32], td[32], bd[32];
+  hso_digest32(t.qp.data(), 40, qd);
+  hso_digest32(t.tpre.data(), 16, td);
+  hso_digest32(t.bp.data(), t.bp.size(), bd);
+  // one signing pass: N authors over td, nv QC votes over qd, the Block author over bd
+  const size_t n = (size_t)N + nv + 1;
+  std::vector<uint32_t> key(n);
+  std::vector<uint8_t> msgs(n * 32), sigs(n * 64);
+  std::vector<uint64_t> off(n + 1);
+  for (size_t i = 0; i < n; i++) {
+    const bool author = i < (size_t)N, qc = !author && i < n - 1;
+    key[i] = author ? (uint32_t)i : qc ? (uint32_t)(((i - N) * 7 + r) % N) : (uint32_t)((r + 1) % N);
+    memcpy(&msgs[i * 32], author ? td : qc ? qd : bd, 32);
+    off[i] = i * 32;
+  }
+  off[n] = n * 32;
+  hso_sign_batch(k.seeds.data(), k.pks.data(), key.data(), msgs.data(), off.data(), n, ncpu(), sigs.data());
+  t.asig.assign(sigs.begin(), sigs.begin() + (size_t)N * 64);
+  t.qsig.assign(sigs.begin() + (size_t)N * 64, sigs.begin() + (n - 1) * 64);
+  t.bsig.assign(sigs.end() - 64, sigs.end());
+  t.bkey = key[n - 1];
+  t.apk.resize((size_t)N * 32);
+  t.qpk.resize((size_t)nv * 32);
+  for (int i = 0; i < N; i++) {
+    memcpy(&t.apk[(size_t)i * 32], &k.pks[(size_t)key[i] * 32], 32);
+    if ((i * 37 + r * 11) % 100 == 0) t.asig[(size_t)i * 64 + (i + r) % 64] ^= 0x10;  // 1 % of the authors corrupted
+  }
+  for (int i = 0; i < nv; i++) memcpy(&t.qpk[(size_t)i * 32], &k.pks[(size_t)key[N + i] * 32], 32);
+  auto oracle = [&](const std::vector<uint8_t> &sig, const std::vector<uint8_t> &pk, const uint8_t *d, size_t cnt, uint32_t mode) {
+    std::vector<uint8_t> recs(cnt * 128);
+    for (size_t i = 0; i < cnt; i++) {
+      memcpy(&recs[i * 128], &sig[i * 64], 64);
+      memcpy(&recs[i * 128 + 64], &pk[i * 32], 32);
+      memcpy(&recs[i * 128 + 96], d, 32);
+    }
+    std::vector<uint32_t> w((cnt + 31) / 32);
+    hso_verify_rec128_batch(recs.data(), cnt, mode, ncpu(), w.data());
+    return w;
+  };
+  t.a_want = oracle(t.asig, t.apk, td, N, HS_MODE_STRICT);
+  t.q_want = oracle(t.qsig, t.qpk, qd, nv, HS_MODE_BATCH_EQ);
+  t.b_want = hso_verify_strict(t.bsig.data(), &k.pks[(size_t)t.bkey * 32], bd, 32) == 1;
+}
+// The round's N Timeouts through queue q from 16 threads (submit all, then wait for each); returns the verdict mismatches.
+static int tc_timeouts(hs_queue *q, const tc_round &t, int N) {
+  const int nv = N - (N - 1) / 3, nth = 16;
+  std::atomic<int> mism{0};
+  std::vector<std::thread> ts;
+  for (int th = 0; th < nth; th++)
+    ts.emplace_back([&, th] {
+      std::vector<uint8_t> sig((size_t)(1 + nv) * 64), pk((size_t)(1 + nv) * 32), modes(1 + nv, HS_MODE_BATCH_EQ), pre(56);
+      std::vector<uint32_t> midx(1 + nv, 1), bits((nv + 1 + 31) / 32);
+      const uint64_t off[3] = {0, 16, 56};
+      memcpy(&sig[64], t.qsig.data(), t.qsig.size());
+      memcpy(&pk[32], t.qpk.data(), t.qpk.size());
+      memcpy(pre.data(), t.tpre.data(), 16);
+      memcpy(&pre[16], t.qp.data(), 40);
+      modes[0] = HS_MODE_STRICT;
+      midx[0] = 0;
+      std::vector<std::pair<int, size_t>> tickets;
+      for (int i = th; i < N; i += nth) {
+        memcpy(sig.data(), &t.asig[(size_t)i * 64], 64);
+        memcpy(pk.data(), &t.apk[(size_t)i * 32], 32);
+        size_t ticket = 0;
+        int rc;
+        while ((rc = hs_queue_submit_msgs(q, pre.data(), off, 2, sig.data(), pk.data(), midx.data(), modes.data(), 1 + nv, nullptr, nullptr, &ticket)) ==
+               HS_ERR_NOMEM)
+          std::this_thread::yield();
+        if (rc != HS_OK) {
+          mism++;
+          continue;
+        }
+        tickets.emplace_back(i, ticket);
+      }
+      for (auto &[i, ticket] : tickets) {
+        if (hs_queue_wait(q, ticket, bits.data()) != HS_OK) {
+          mism++;
+          continue;
+        }
+        int m = bit(bits, 0) != bit(t.a_want, i);
+        for (int v = 0; v < nv; v++) m += bit(bits, v + 1) != bit(t.q_want, v);
+        mism += m;
+      }
+    });
+  for (auto &th : ts) th.join();
+  return mism.load();
+}
+static int tc_after_timeouts(hs_ctx *ctx, int N, int rounds, bool last) {
+  const committee_keys k = make_keys(N, 47);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  const int nv = N - (N - 1) / 3;
+  hs_queue *qs[2] = {nullptr, nullptr};  // arm (b): no signature cache, arm (c): with it
+  for (int a = 0; a < 2; a++)
+    if (hs_queue_create(ctx, 16384, &qs[a]) != HS_OK || hs_queue_cert_cache(qs[a], 64u << 20) != HS_OK) return 1;
+  if (hs_queue_sig_cache(qs[1], 1u << 16) != HS_OK) return 1;
+  uint64_t sig0[HS_QUEUE_SIG_STATS] = {}, tc_sig[2] = {0, 0}, blk_sig[2] = {0, 0};  // [probed, hits] of arm (c)'s TCs and Blocks
+  hs_queue_sig_stats(qs[1], sig0);
+  series lat[2][3];  // [TC, Block][arm]
+  int mism[2][3] = {{0, 0, 0}, {0, 0, 0}}, to_mism = 0, errors = 0;
+  tc_round t;
+  for (int r = 0; r < rounds + 1; r++) {
+    const bool timed = r >= 1;
+    tc_make(k, r, t);
+    // the TC: votes 0 .. nv - 1 are the first nv Timeouts' authors, each over its own copy of round || high_qc.round
+    std::vector<uint8_t> tc_pre((size_t)nv * 16), tc_modes(nv, HS_MODE_STRICT);
+    std::vector<uint64_t> tc_off(nv + 1), tc_hq(nv, t.hq);
+    std::vector<uint32_t> tc_midx(nv), tc_want((nv + 31) / 32);
+    for (int i = 0; i < nv; i++) {
+      memcpy(&tc_pre[(size_t)i * 16], t.tpre.data(), 16);
+      tc_off[i] = (uint64_t)i * 16;
+      tc_midx[i] = (uint32_t)i;
+      if (bit(t.a_want, i)) tc_want[i >> 5] |= 1u << (i & 31);
+    }
+    tc_off[nv] = (uint64_t)nv * 16;
+    // the Block carrying the TC: author, the QC's votes, the TC's votes
+    const size_t bn = 1 + 2 * (size_t)nv;
+    std::vector<uint8_t> b_pre, b_sig(bn * 64), b_pk(bn * 32), b_modes(bn);
+    std::vector<uint64_t> b_off{0};
+    std::vector<uint32_t> b_midx(bn), b_want((bn + 31) / 32);
+    auto add_pre = [&](const uint8_t *p, size_t len) {
+      b_pre.insert(b_pre.end(), p, p + len);
+      b_off.push_back(b_pre.size());
+    };
+    add_pre(t.bp.data(), t.bp.size());
+    add_pre(t.qp.data(), 40);
+    for (int i = 0; i < nv; i++) add_pre(t.tpre.data(), 16);
+    memcpy(b_sig.data(), t.bsig.data(), 64);
+    memcpy(b_pk.data(), &k.pks[(size_t)t.bkey * 32], 32);
+    memcpy(&b_sig[64], t.qsig.data(), t.qsig.size());
+    memcpy(&b_pk[32], t.qpk.data(), t.qpk.size());
+    memcpy(&b_sig[(1 + (size_t)nv) * 64], t.asig.data(), (size_t)nv * 64);
+    memcpy(&b_pk[(1 + (size_t)nv) * 32], t.apk.data(), (size_t)nv * 32);
+    for (size_t i = 0; i < bn; i++) {
+      const bool qc = i >= 1 && i <= (size_t)nv;
+      b_modes[i] = qc ? HS_MODE_BATCH_EQ : HS_MODE_STRICT;
+      b_midx[i] = i == 0 ? 0u : qc ? 1u : (uint32_t)(2 + i - 1 - nv);
+      const bool w = i == 0 ? t.b_want : qc ? bit(t.q_want, (int)i - 1) : bit(t.a_want, (int)(i - 1 - nv));
+      if (w) b_want[i >> 5] |= 1u << (i & 31);
+    }
+    for (int a = 0; a < 2; a++) to_mism += tc_timeouts(qs[a], t, N);
+    for (int c = 0; c < 2; c++) {  // c = 0: the TC, 1: the Block
+      const size_t n = c ? bn : (size_t)nv;
+      std::vector<uint32_t> bits((n + 31) / 32);
+      for (int a = 0; a < 3; a++) {
+        uint64_t s0[HS_QUEUE_SIG_STATS] = {}, s1[HS_QUEUE_SIG_STATS] = {};
+        if (a == 2) hs_queue_sig_stats(qs[1], s0);
+        std::fill(bits.begin(), bits.end(), 0u);
+        const auto t0 = clk::now();
+        int rc;
+        if (a == 0 && c == 0) {
+          uint32_t tcb = 0;
+          rc = hs_verify_tcs(ctx, &t.round, 1, t.apk.data(), nullptr, t.asig.data(), tc_hq.data(), std::vector<uint32_t>(n, 0).data(), n, bits.data(), &tcb);
+        } else if (a == 0) {
+          uint32_t gb = 0;
+          rc = hs_verify_groups(ctx, b_pre.data(), b_off.data(), b_off.size() - 1, b_sig.data(), b_pk.data(), nullptr, b_midx.data(),
+                                std::vector<uint32_t>(n, 0).data(), b_modes.data(), n, 1, bits.data(), &gb);
+        } else {
+          size_t ticket = 0;
+          hs_queue *q = qs[a - 1];
+          rc = c == 0 ? hs_queue_submit_msgs(q, tc_pre.data(), tc_off.data(), nv, t.asig.data(), t.apk.data(), tc_midx.data(), tc_modes.data(), n, nullptr,
+                                             nullptr, &ticket)
+                      : hs_queue_submit_msgs(q, b_pre.data(), b_off.data(), b_off.size() - 1, b_sig.data(), b_pk.data(), b_midx.data(), b_modes.data(), n,
+                                             nullptr, nullptr, &ticket);
+          if (rc == HS_OK) rc = hs_queue_wait(q, ticket, bits.data());
+        }
+        const double us = us_since(t0);
+        errors += rc != HS_OK;
+        if (a == 2) {
+          hs_queue_sig_stats(qs[1], s1);
+          if (timed) {
+            uint64_t *d = c ? blk_sig : tc_sig;
+            d[0] += s1[0] - s0[0];
+            d[1] += s1[1] - s0[1];
+          }
+        }
+        if (timed) {
+          lat[c][a].v.push_back(us);
+          const std::vector<uint32_t> &w = c ? b_want : tc_want;
+          for (size_t i = 0; i < n; i++) mism[c][a] += bit(bits, (int)i) != bit(w, (int)i);
+        }
+      }
+    }
+  }
+  printf("\"committee_%d\": {\"tc_votes\": %d, \"block_records\": %d, \"rounds\": %d, \"timeout_mismatches\": %d, \"errors\": %d, ", N, nv, 1 + 2 * nv, rounds,
+         to_mism, errors);
+  const char *cn[2] = {"tc", "block_with_tc"};
+  const char *an[2][3] = {{"a_sync_verify_tcs", "b_queue_no_sig_cache", "c_queue_sig_cache"},
+                          {"a_sync_verify_groups", "b_queue_no_sig_cache", "c_queue_sig_cache"}};
+  for (int c = 0; c < 2; c++) {
+    printf("\"%s\": {", cn[c]);
+    for (int a = 0; a < 3; a++)
+      printf("\"%s\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"mismatches\": %d}, ", an[c][a], lat[c][a].pct(0.5), lat[c][a].pct(0.99), mism[c][a]);
+    const uint64_t *d = c ? blk_sig : tc_sig;
+    printf("\"c_probed_per_round\": %.1f, \"c_hits_per_round\": %.1f}, ", (double)d[0] / rounds, (double)d[1] / rounds);
+  }
+  emit_sig_stats(qs[1], sig0);  // Timeouts, TCs and Blocks of every round, the warm-up round included
+  printf("}%s", last ? "" : ", ");
+  for (hs_queue *q : qs) hs_queue_destroy(q);
+  int m = to_mism + errors;
+  for (auto &row : mism)
+    for (int x : row) m += x;
+  return m;
+}
+static int run_tc_after_timeouts(hs_ctx *ctx, int rounds) {
+  printf("\"tc_after_timeouts\": {\"gpu\": \"%s\", \"threads\": 16, \"ring_records\": 16384, \"sig_cache_entries\": %u, ", gpu_identity().c_str(), 1u << 16);
+  int bad = 0;
+  for (int N : {100, 1000, 4000}) bad += tc_after_timeouts(ctx, N, rounds, N == 4000);
+  printf("}");
+  return bad;
+}
+
 int main(int argc, char **argv) {
   const int rounds = argc > 1 ? atoi(argv[1]) : 1000;
   hs_ctx *ctx = nullptr;
@@ -950,6 +1241,14 @@ int main(int argc, char **argv) {
   if (argc > 3 && strcmp(argv[3], "view_change") == 0) {
     printf("{");
     const int bad = run_view_change(ctx, argc > 2 ? atoi(argv[2]) : 10);
+    printf("}\n");
+    hs_ctx_destroy(ctx);
+    return bad ? 9 : 0;
+  }
+  if (argc > 3 && (strcmp(argv[3], "tc_after_timeouts") == 0 || strcmp(argv[3], "sig_cache_cost") == 0)) {
+    printf("{");
+    const bool tc = strcmp(argv[3], "tc_after_timeouts") == 0;
+    const int bad = tc ? run_tc_after_timeouts(ctx, argc > 2 ? atoi(argv[2]) : 10) : run_sig_cache_cost(ctx, argc > 2 ? atoi(argv[2]) : 20);
     printf("}\n");
     hs_ctx_destroy(ctx);
     return bad ? 9 : 0;

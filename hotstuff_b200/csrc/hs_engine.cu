@@ -735,6 +735,103 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
   }
 }
 
+// ------------------------------------------------------------------------------------------------ generic queue path (hs_queue_generic)
+// Queue requests the committee path cannot serve (no committee registered, or a key outside it), verified on the GPU instead of on
+// the dispatcher thread.  One launch carries every such request of one or more dispatches: record j is ring slot slots[(first + j)
+// & mask] (a mapped list the dispatcher writes), its key the 32 bytes at pks + 32 * slot (the queue's mapped key array).  A thread
+// verifies a record as k_verify_main<false> does: SHA-512(R || A || M), decompress A, a radix-16 window for [k](-A) from a per-thread
+// table of 8 multiples, the base comb for [S]B; then, as k_verify_bulk, the block's Z's share one inversion and verify_flags_from
+// writes both HS_F_EQ and HS_F_STRICT.  A block may hold records of several requests (and a request may span blocks), so completion
+// counts records: the add that completes a request fences the system and raises its completion word.  Rows are staged as in
+// k_verify_bulk, a warp's 32 records with 16-byte loads: each record's 128 bytes are one coalesced row wherever its slot is.
+// Sizing: 128 threads, 3 blocks per SM as k_verify_main<false> (the window table is per-thread local memory, not a spill).
+#define HS_GEN_THREADS 128
+__global__ void __launch_bounds__(HS_GEN_THREADS, HS_GENERIC_MINBLOCKS) k_queue_generic(const small_rec *__restrict__ ring, const uint8_t *__restrict__ pks,
+                                                                                      const uint32_t *__restrict__ slots, uint32_t first, uint32_t mask,
+                                                                                      uint32_t n, const ge_niels *__restrict__ btable, const comb_params cp,
+                                                                                      uint8_t *out_flags, uint32_t *counters, volatile uint32_t *done,
+                                                                                      uint32_t seq) {
+  // one buffer, two lives: record staging while loading, then the base comb's signed digits [digit][thread]
+  __shared__ __align__(16) unsigned char smem_raw[HS_MAX_DIGITS * HS_GEN_THREADS * 4];
+  static_assert(sizeof(smem_raw) >= (HS_GEN_THREADS / 32) * 256 * sizeof(uint4), "staging does not fit");
+  __shared__ fe tot[HS_GEN_THREADS];
+  const int lane = threadIdx.x & 31;
+  const uint32_t j = blockIdx.x * HS_GEN_THREADS + threadIdx.x;
+  const bool active = j < n;  // threads past n take every barrier with Z = 1 and store nothing
+  const uint32_t slot = active ? __ldg(slots + ((first + j) & mask)) : 0u;
+  uint4 q[8];
+  {
+    uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
+    const uint32_t warp_first = j & ~31u;
+#pragma unroll
+    for (int w = 0; w < 8; w++) {
+      const int c = w * 32 + lane, rec = c >> 3, part = c & 7;
+      const uint32_t s = __shfl_sync(0xffffffffu, slot, rec);
+      uint4 v = make_uint4(0, 0, 0, 0);
+      if (warp_first + rec < n) v = __ldg(reinterpret_cast<const uint4 *>(ring + s) + part);
+      sw[rec * 8 + (part ^ (rec & 7))] = v;
+    }
+    __syncwarp();
+#pragma unroll
+    for (int part = 0; part < 8; part++) q[part] = sw[lane * 8 + (part ^ (lane & 7))];
+  }
+  __syncthreads();  // the staging bytes become the digit slots
+  uint32_t R[8];
+  R[0] = q[0].x; R[1] = q[0].y; R[2] = q[0].z; R[3] = q[0].w; R[4] = q[1].x; R[5] = q[1].y; R[6] = q[1].z; R[7] = q[1].w;
+  const uint32_t req = q[6].y, req_n = q[6].z;  // small_rec: sig | msg | vidx | req | req_n
+  ge_ext acc;
+  uint32_t meta = 0;
+  if (active) {
+    uint32_t S[8], A[8], M[8], h[16];
+    S[0] = q[2].x; S[1] = q[2].y; S[2] = q[2].z; S[3] = q[2].w; S[4] = q[3].x; S[5] = q[3].y; S[6] = q[3].z; S[7] = q[3].w;
+    M[0] = q[4].x; M[1] = q[4].y; M[2] = q[4].z; M[3] = q[4].w; M[4] = q[5].x; M[5] = q[5].y; M[6] = q[5].z; M[7] = q[5].w;
+    const uint4 *a4 = reinterpret_cast<const uint4 *>(pks + 32 * (size_t)slot);
+    const uint4 a0 = __ldg(a4), a1 = __ldg(a4 + 1);
+    A[0] = a0.x; A[1] = a0.y; A[2] = a0.z; A[3] = a0.w; A[4] = a1.x; A[5] = a1.y; A[6] = a1.z; A[7] = a1.w;
+    sha512_ram32(h, R, A, M);
+    ge_cached tab[9];
+    meta = verify_generic_main(acc, R, S, A, h, btable, tab, reinterpret_cast<int32_t *>(smem_raw) + threadIdx.x, HS_GEN_THREADS, cp);
+  }
+  if (!(meta & HS_META_PARSE_OK)) {  // rejected records (and idle threads) keep the block's inversion well-defined
+    fe_set0(acc.X);
+    fe_set1(acc.Y);
+    fe_set1(acc.Z);
+  }
+  if (fe_is_zero(acc.Z)) {  // cannot happen for curve points; keeps one bad record from poisoning the block's inversion
+    fe_set1(acc.Z);
+    meta &= ~HS_META_PARSE_OK;
+  }
+  tot[threadIdx.x] = acc.Z;
+  __syncthreads();
+  if (threadIdx.x < HS_GEN_THREADS / 4) {  // lane l: 1 / Z of threads 4l .. 4l+3 from one inversion
+    const int b = threadIdx.x * 4;
+    fe q0 = tot[b], q1, q2, q3, inv, u;
+    fe_mul(q1, q0, tot[b + 1]);
+    fe_mul(q2, q1, tot[b + 2]);
+    fe_mul(q3, q2, tot[b + 3]);
+    fe_invert(inv, q3);
+    fe_mul(u, inv, q2);
+    fe_mul(inv, inv, tot[b + 3]);
+    tot[b + 3] = u;
+    fe_mul(u, inv, q1);
+    fe_mul(inv, inv, tot[b + 2]);
+    tot[b + 2] = u;
+    fe_mul(u, inv, q0);
+    fe_mul(inv, inv, tot[b + 1]);
+    tot[b + 1] = u;
+    tot[b] = inv;
+  }
+  __syncthreads();
+  if (!active) return;
+  out_flags[slot] = (uint8_t)verify_flags_from(acc.X, acc.Y, tot[threadIdx.x], R, meta);
+  __threadfence_system();
+  if (atomicAdd(counters + req, 1u) == req_n - 1) {
+    counters[req] = 0;
+    __threadfence_system();
+    done[req] = seq;
+  }
+}
+
 // A few LONG messages (one mempool batch is ~15 kB = 120 blocks, mempool/src/processor.rs:30): SHA-512 is sequential in its
 // 80 x nblk rounds, but the message schedule (45 % of the work) of different blocks is independent — lane l of the warp
 // expands block g + l into a shared K+W table, then the rounds run back to back from that table.  One warp per message.
@@ -1666,8 +1763,9 @@ struct hs_queue {
   uint8_t *h_flags = nullptr, *d_flags = nullptr;  // mapped pinned: verdict flags per record
   uint32_t *h_done = nullptr, *d_done = nullptr;   // mapped pinned: completion word per request slot (= launch sequence number)
   uint32_t *d_counters = nullptr;                  // device: records finished per request slot
-  std::vector<uint8_t> pk;                         // key bytes per record (host only: resolved to a table index at dispatch)
-  std::vector<uint8_t> modes;                      // HS_MODE_* per record (host only: picks the verdict flag of each record)
+  uint8_t *pk = nullptr, *d_pk = nullptr;          // mapped pinned: key bytes per record (32 B; resolved to a table index at
+                                                   // dispatch, read by k_queue_generic)
+  std::vector<uint8_t> modes;                     // HS_MODE_* per record (host only: picks the verdict flag of each record)
   std::vector<uint32_t> wbits;                     // dispatcher thread only: verdict bitmap being assembled (cap bits)
   cudaStream_t stream = nullptr;                   // k_verify_small launches: the device's highest priority
   cudaStream_t bulk_stream = nullptr;              // k_verify_bulk launches: a lower priority, so votes never wait behind them
@@ -1695,6 +1793,7 @@ struct hs_queue {
     uint32_t a_off, m, pre_bytes;  // its arena region: offset, preimages, preimage bytes
     uint64_t a_end;      // arena position past its region (0: none)
     cert_req *cr = nullptr;  // the ring part of a certificate-cache request: its verdicts go there (ticket and cb unused)
+    bool gen = false;        // set at dispatch: verified by k_queue_generic (hs_queue_generic on, a key outside the committee)
   };
   std::vector<req> reqs;  // by request slot
   struct result {
@@ -1707,10 +1806,20 @@ struct hs_queue {
   struct launch {
     uint32_t seq;
     uint64_t lo, hi;  // ring positions it covers
-    bool bulk;        // k_verify_bulk on bulk_stream (one request), else k_verify_small on stream
+    bool bulk;        // on bulk_stream: k_verify_bulk (one request) or k_queue_generic; else k_verify_small on stream
     uint32_t sig_gen;  // the signature cache's table it probed (0: launched without the cache)
+    bool generic = false;  // k_queue_generic: its requests are the gen ones in [lo, hi) with its seq, others lie between them
   };
-  std::deque<launch> inflight;  // in ring order
+  // Launches in flight, in launch order.  A generic launch's range interleaves with small and bulk ones, so this is not ring
+  // order: queue_release_locked takes the lowest lo of all of them.
+  std::deque<launch> inflight;
+  // hs_queue_generic: gen_on is written under c->mu (the dispatcher reads it there); at most one generic launch is in flight, and
+  // generic requests dispatched meanwhile wait in gpend (ring positions, dispatcher thread only) for the next one
+  std::atomic<bool> gen_on{false};
+  std::deque<uint64_t> gpend;
+  uint32_t *h_gslot = nullptr, *d_gslot = nullptr;   // mapped pinned: a generic launch's ring slots at positions [lo, lo + records)
+  qmsg_desc *h_gmlist = nullptr, *d_gmlist = nullptr;  // mapped pinned: its preimage requests' descriptors, from position lo on
+  uint64_t gstats[HS_QUEUE_GENERIC_STATS] = {};      // hs_queue_generic_stats
   uint64_t head = 0, launched = 0, tail = 0;
   size_t next_ticket = 1;
   uint32_t seq = 0;
@@ -1744,9 +1853,13 @@ struct queue_completion {
   queue_bits bits;
 };
 // Releases the ring space of the finished requests at the head — but never inside the range of a launch still in flight: its
-// blocks may still read those records (slow-path requests between two device requests ride along in the launch).
+// blocks may still read those records (slow-path requests between two device requests ride along in the launch).  The limit is
+// the lowest range start of ALL launches in flight: a generic launch's range holds requests of other launches, and its slot list
+// sits at its own positions, so finished requests inside it must not be released either.  Generic requests waiting in gpend are
+// unfinished, so release stops at them without a limit.
 static void queue_release_locked(hs_queue *q) {
-  const uint64_t limit = q->inflight.empty() ? q->launched : q->inflight.front().lo;
+  uint64_t limit = q->launched;
+  for (const hs_queue::launch &L : q->inflight) limit = std::min(limit, L.lo);
   while (q->head < limit && q->reqs[q->head & q->mask].finished) {
     hs_queue::req &h = q->reqs[q->head & q->mask];
     h.finished = false;
@@ -1842,9 +1955,18 @@ static void queue_fire(std::vector<queue_completion> &fire) {
 // around it: one launch per run of device requests between such requests.  A device request of HS_QUEUE_BULK_MIN records or more
 // closes the run the same way and gets a k_verify_bulk launch of its own on the bulk stream; the small launches of the same
 // dispatch are enqueued first.
+// With hs_queue_generic on, a request with a key outside the committee (every request, when none is registered) is a generic
+// request instead: it neither rides nor reaches the slow path.  It closes the run before it like a large rider, whatever its
+// size (k_verify_small must not touch its records: they complete through k_queue_generic's counts), and waits in gpend.  When no
+// generic launch is in flight, one k_queue_generic launch on the bulk stream, after this dispatch's other launches, takes every
+// request in gpend.  Requests left in gpend after the option is turned off take the slow path.
 static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   hs_ctx *c = q->c;
   std::vector<uint64_t> slow;
+  std::vector<uint64_t> greqs;  // the requests of this dispatch's generic launch, in ring order
+  hs_queue::launch G{0, 0, 0, true, 0, true};
+  uint64_t g_recs = 0;
+  bool g_ok = false;
   std::vector<queue_completion> fire;
   std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one, in ring order
   std::vector<char> ok;                // runs launched without a CUDA error (the first failure stops the rest)
@@ -1853,26 +1975,36 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   {
     std::lock_guard<std::mutex> g(c->mu);
     const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables && c->small_enabled;
+    const bool gen = q->gen_on.load();  // hs_queue_generic writes it under c->mu
+    if (!gen) {  // turned off with generic requests still waiting: they take the slow path, ahead of this range's
+      for (uint64_t p : q->gpend) q->reqs[p & q->mask].gen = false;
+      slow.assign(q->gpend.begin(), q->gpend.end());
+      q->gpend.clear();
+    }
     uint64_t rlo = hi, rhi = lo;  // the run being gathered
     for (uint64_t p = lo; p < hi;) {
       hs_queue::req &r = q->reqs[p & q->mask];
       bool all = committee;
       for (uint32_t i = 0; i < r.n; i++) {
         small_rec &s = q->h_ring[(p + i) & q->mask];
-        s.vidx = all ? host_key_lookup(c, q->pk.data() + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
+        s.vidx = all ? host_key_lookup(c, q->pk + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
         s.req = (uint32_t)(p & q->mask);
         s.req_n = r.n;
         if (s.vidx == HS_NO_KEY) all = false;
       }
       const bool bulk = all && r.n >= HS_QUEUE_BULK_MIN;
+      const bool generic = gen && !all;
+      r.gen = generic;
       if (!all) {  // every record of a slow-path request rides as HS_NO_KEY: none of them probes or fills the signature cache
         for (uint32_t i = 0; i < r.n; i++) q->h_ring[(p + i) & q->mask].vidx = HS_NO_KEY;
-        r.seq = 0;
-        slow.push_back(p);
+        r.seq = 0;  // a generic request's launch number is set when its launch is built
+        if (generic) q->gpend.push_back(p);
+        else slow.push_back(p);
       } else {
         r.seq = 1;  // the launch's number is set below
       }
-      if ((bulk || (!all && r.n > HS_SMALL_MAX)) && rlo < rhi) {  // no large riders, and no small request in a bulk launch
+      // no large riders, no generic request in a small launch, and no small request in a bulk launch
+      if ((bulk || (!all && (generic || r.n > HS_SMALL_MAX))) && rlo < rhi) {
         runs.push_back(hs_queue::launch{0, rlo, rhi, false});
         rlo = hi;
         rhi = lo;
@@ -1944,9 +2076,61 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         ok[k] = 1;
       }
     }
+    bool g_inflight = false;  // (inflight changes only on this thread)
+    for (const hs_queue::launch &L : q->inflight) g_inflight = g_inflight || L.generic;
+    if (gen && !g_inflight && !q->gpend.empty()) {  // the generic launch: its slot list and descriptors start at position lo
+      greqs.assign(q->gpend.begin(), q->gpend.end());
+      q->gpend.clear();
+      G.seq = ++q->seq ? q->seq : ++q->seq;
+      G.lo = greqs.front();
+      uint32_t n_msgs_req = 0;
+      uint64_t n_pre = 0, n_pre_bytes = 0;
+      for (uint64_t p : greqs) {
+        hs_queue::req &r = q->reqs[p & q->mask];
+        r.seq = G.seq;
+        if (r.msgs) {
+          q->h_gmlist[(G.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
+          n_pre += r.m;
+          n_pre_bytes += r.pre_bytes;
+        }
+        for (uint32_t i = 0; i < r.n; i++) q->h_gslot[(G.lo + g_recs++) & q->mask] = (uint32_t)((p + i) & q->mask);
+        G.hi = p + r.n;
+      }
+      const uint32_t base = (uint32_t)(G.lo & q->mask);
+      const bool earlier_failure = e != cudaSuccess;
+      if (e == cudaSuccess && n_msgs_req) {  // the Digests first, on the same stream
+        k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, q->bulk_stream>>>(q->d_gmlist, base, q->mask, q->d_arena, q->d_stage, q->d_digs, q->d_ring);
+        c->launches++;
+        e = cudaGetLastError();
+        if (e == cudaSuccess) {
+          dig_launched[0]++;
+          dig_launched[1] += n_pre;
+          dig_launched[2] += n_pre_bytes;
+        }
+      }
+      if (e == cudaSuccess) {
+        k_queue_generic<<<(unsigned)((g_recs + HS_GEN_THREADS - 1) / HS_GEN_THREADS), HS_GEN_THREADS, 0, q->bulk_stream>>>(
+            q->d_ring, q->d_pk, q->d_gslot, base, q->mask, (uint32_t)g_recs, c->d_btable, c->cp, q->d_flags, q->d_counters, q->d_done, G.seq);
+        c->launches++;
+        e = cudaGetLastError();
+      }
+      if (e == cudaSuccess) e = cudaEventRecord(q->ev_bulk_last, q->bulk_stream);
+      g_ok = e == cudaSuccess;
+      if (!g_ok && !earlier_failure) fail(c, HS_ERR_CUDA, "verify queue generic launch", e);
+    }
   }
   {
     std::lock_guard<std::mutex> g(q->mu);
+    if (!greqs.empty()) {
+      if (g_ok) {
+        q->inflight.push_back(G);
+        q->gstats[0]++;
+        q->gstats[1] += g_recs;
+        q->gstats[2] += greqs.size();
+      } else {
+        for (uint64_t p : greqs) queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
+      }
+    }
     for (uint64_t p : slow) {
       q->stats[4]++;
       q->stats[5] += q->reqs[p & q->mask].n;
@@ -1982,7 +2166,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       for (uint32_t i = 0; i < r.n; i++) {
         const uint32_t s = (uint32_t)((p + i) & q->mask);
         memcpy(&msig[(size_t)i * 64], q->h_ring[s].sig, 64);
-        memcpy(&mpk[(size_t)i * 32], q->pk.data() + 32 * (size_t)s, 32);
+        memcpy(&mpk[(size_t)i * 32], q->pk + 32 * (size_t)s, 32);
         mmode[i] = q->modes[s];
       }
       const uint8_t *a = q->h_arena + r.a_off;
@@ -1998,7 +2182,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         if (q->modes[s] != mode) continue;
         hs_rec128 x;
         memcpy(x.sig, q->h_ring[s].sig, 64);
-        memcpy(x.pk, q->pk.data() + 32 * (size_t)s, 32);
+        memcpy(x.pk, q->pk + 32 * (size_t)s, 32);
         memcpy(x.msg, q->h_ring[s].msg, 32);
         recs.push_back(x);
         idx.push_back(i);
@@ -2038,6 +2222,7 @@ static void queue_watch(hs_queue *q) {
       bool open = false;
       for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n) {
         hs_queue::req &r = q->reqs[p & q->mask];
+        if (L.generic && !(r.gen && r.seq == L.seq)) continue;  // a request of another launch between its generic requests
         const bool mine = r.seq == L.seq && !r.finished;
         if (((volatile uint32_t *)q->h_done)[p & q->mask] == L.seq) {
           if (!mine) continue;
@@ -2059,7 +2244,9 @@ static void queue_watch(hs_queue *q) {
           open = true;
         } else if (mine) {
           if (qe == cudaSuccess)
-            fail(q->c, HS_ERR_CUDA, L.bulk ? "verify queue: k_verify_bulk did not complete" : "verify queue: k_verify_small did not complete");
+            fail(q->c, HS_ERR_CUDA, L.generic ? "verify queue: k_queue_generic did not complete"
+                                    : L.bulk  ? "verify queue: k_verify_bulk did not complete"
+                                              : "verify queue: k_verify_small did not complete");
           queue_finish_locked(q, p, HS_ERR_CUDA, nullptr, fire);
         }
       }
@@ -2077,6 +2264,14 @@ static size_t queue_small_inflight_locked(const hs_queue *q) {
   for (const hs_queue::launch &L : q->inflight) k += !L.bulk;
   return k;
 }
+// Generic requests wait in gpend and no generic launch is in flight (or the option is off: they take the slow path).
+static bool queue_generic_ready_locked(const hs_queue *q) {
+  if (q->gpend.empty()) return false;
+  if (!q->gen_on.load()) return true;
+  for (const hs_queue::launch &L : q->inflight)
+    if (L.generic) return false;
+  return true;
+}
 
 static void queue_main(hs_queue *q) {
   cudaSetDevice(q->c->device);
@@ -2090,8 +2285,9 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_fire(fire);
       lk.lock();
-    } else if (q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) {
-      const uint64_t lo = q->launched, hi = q->tail;  // everything pending
+    } else if ((q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) || queue_generic_ready_locked(q)) {
+      // everything pending; only the waiting generic requests while the small launches are at their limit
+      const uint64_t lo = q->launched, hi = queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT ? q->tail : lo;
       q->launched = hi;
       lk.unlock();
       queue_dispatch(q, lo, hi);
@@ -2128,6 +2324,9 @@ static void queue_free(hs_queue *q) {
   if (q->h_done) cudaFreeHost(q->h_done);
   if (q->h_arena) cudaFreeHost(q->h_arena);
   if (q->h_mlist) cudaFreeHost(q->h_mlist);
+  if (q->pk) cudaFreeHost(q->pk);
+  if (q->h_gslot) cudaFreeHost(q->h_gslot);
+  if (q->h_gmlist) cudaFreeHost(q->h_gmlist);
   cudaFree(q->d_counters);
   cudaFree(q->d_stage);
   cudaFree(q->d_digs);
@@ -3079,7 +3278,6 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   q->cap = cap;
   q->mask = cap - 1;
   q->acap = cap * HS_QUEUE_ARENA_PER_RECORD;
-  q->pk.assign((size_t)cap * 32, 0);
   q->modes.assign(cap, 0);
   q->wbits.assign(cap / 32, 0);
   q->reqs.assign(cap, hs_queue::req{});
@@ -3096,6 +3294,7 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_arena, q->acap, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_mlist, (size_t)cap * sizeof(qmsg_desc), cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->pk, (size_t)cap * 32, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaMalloc(&q->d_stage, q->acap);
   if (e == cudaSuccess) e = cudaMalloc(&q->d_digs, (size_t)q->acap * 4);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_ring, q->h_ring, 0);
@@ -3103,11 +3302,13 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_done, q->h_done, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_arena, q->h_arena, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_mlist, q->h_mlist, 0);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_pk, q->pk, 0);
   if (e != cudaSuccess) {
     queue_free(q);
     return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
   }
   memset(q->h_done, 0, (size_t)cap * 4);
+  memset(q->pk, 0, (size_t)cap * 32);
   try {
     q->th = std::thread(queue_main, q);
   } catch (...) {
@@ -3140,7 +3341,7 @@ static int queue_put_recs_locked(hs_queue *q, const char *what, const hs_rec128 
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
     memcpy(q->h_ring[s].sig, recs[i].sig, 64);
     memcpy(q->h_ring[s].msg, recs[i].msg, 32);
-    memcpy(q->pk.data() + 32 * (size_t)s, recs[i].pk, 32);
+    memcpy(q->pk + 32 * (size_t)s, recs[i].pk, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)mode;
   }
   r.n = (uint32_t)sel.n;
@@ -3190,7 +3391,7 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
     const size_t i = sel[k];
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
     memcpy(q->h_ring[s].sig, sig + 64 * i, 64);
-    memcpy(q->pk.data() + 32 * (size_t)s, pk + 32 * i, 32);
+    memcpy(q->pk + 32 * (size_t)s, pk + 32 * i, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
     idx[k] = remap[msg_idx[i]];
   }
@@ -3491,6 +3692,37 @@ int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]) {
   if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_stats: bad argument");
   std::lock_guard<std::mutex> g(q->mu);
   memcpy(out, q->sstats, sizeof(q->sstats));
+  return HS_OK;
+}
+
+int hs_queue_generic(hs_queue *q, int on) {
+  if (!q) return fail(nullptr, HS_ERR_ARG, "hs_queue_generic: bad argument");
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> g(c->mu);  // the dispatcher reads the option and launches only while it holds c->mu
+  if (q->gen_on.load() == (on != 0)) return HS_OK;
+  HS_CUDA(c, cudaSetDevice(c->device));
+  if (on && !q->h_gslot) {  // first use: the slot list and the descriptor list of the generic launches
+    cudaError_t e = cudaHostAlloc(&q->h_gslot, (size_t)q->cap * 4, cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostAlloc(&q->h_gmlist, (size_t)q->cap * sizeof(qmsg_desc), cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_gslot, q->h_gslot, 0);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_gmlist, q->h_gmlist, 0);
+    if (e != cudaSuccess) {  // the option stays off; a later call starts the first use over
+      if (q->h_gslot) cudaFreeHost(q->h_gslot);
+      if (q->h_gmlist) cudaFreeHost(q->h_gmlist);
+      q->h_gslot = q->d_gslot = nullptr;
+      q->h_gmlist = q->d_gmlist = nullptr;
+      return fail(c, e == cudaErrorMemoryAllocation ? HS_ERR_NOMEM : HS_ERR_CUDA, "hs_queue_generic", e);
+    }
+  }
+  q->gen_on = on != 0;
+  if (!on) HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));  // no generic launch survives this line
+  return HS_OK;
+}
+
+int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_generic_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, q->gstats, sizeof(q->gstats));
   return HS_OK;
 }
 

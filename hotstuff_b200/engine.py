@@ -465,6 +465,22 @@ class VerifyQueue:
         self.engine._check(self.lib.hs_queue_sig_stats(self.h, out), "hs_queue_sig_stats")
         return dict(zip(self.SIG_STATS, (int(x) for x in out)))
 
+    def generic(self, on):
+        """Turns the generic-key device path on or off (hs_queue_generic): with it on, a request with a key outside the registered
+        committee (every request, when none is registered) is verified by a queue kernel on the GPU instead of synchronously on the
+        dispatcher thread, so it no longer holds up the other requests.  Verdicts do not change.  Off (the default) drains the
+        generic launches in flight."""
+        self.engine._check(self.lib.hs_queue_generic(self.h, 1 if on else 0), "hs_queue_generic")
+
+    GENERIC_STATS = ("launches", "records", "requests")
+
+    def generic_stats(self):
+        """Counters of the generic path (hs_queue_generic_stats): k_queue_generic launches, the records they carried, and the
+        requests."""
+        out = (ctypes.c_uint64 * len(self.GENERIC_STATS))()
+        self.engine._check(self.lib.hs_queue_generic_stats(self.h, out), "hs_queue_generic_stats")
+        return dict(zip(self.GENERIC_STATS, (int(x) for x in out)))
+
     def close(self):
         """Completes every request in flight (callbacks fire) and joins the dispatcher thread."""
         if getattr(self, "h", None):

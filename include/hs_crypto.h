@@ -198,7 +198,8 @@ int hs_verify_committee(hs_ctx *ctx, const uint32_t *validator_idx, const uint8_
  *     hs_verify_rec128(ctx, &recs[i], 1, modes[i], ..)).
  *   - Device path: only when a committee is registered (hs_committee_register) and every key of the request is in it.  Any
  *     other request is run by the queue's thread through hs_verify_rec128 itself (key cache / generic kernels; a group takes
- *     at most one strict and one batch-eq call): correct, but the slow path.  The device path has two kernels: requests of
+ *     at most one strict and one batch-eq call): correct, but the slow path, and it holds up the whole queue meanwhile;
+ *     hs_queue_generic (off by default) verifies those requests with a queue kernel instead.  The device path has two kernels: requests of
  *     fewer than 1,002 records (every hs_queue_submit, and smaller groups) share k_verify_small launches, a block per
  *     signature, on the queue's highest-priority stream; a group of 1,002 records or more (a committee of about 1,500 or
  *     more) gets a k_verify_bulk launch of its own, a thread per signature, on a second, lower-priority stream, so a vote's
@@ -284,6 +285,23 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries);
 /* Counters of completed launches: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live entry,
  * [4] entries held now */
 int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]);
+/* Generic-key device path of the queue.  0 = off (the default: the queue launches exactly the kernels it launches without this
+ * call, and a request the committee path cannot serve runs synchronously on the queue's thread).  On: such a request (no committee
+ * registered, or any key of the request outside it) is verified on the GPU instead, by k_queue_generic on the queue's
+ * lower-priority stream (a thread per record: decompress A, a radix-16 window for [k](-A), the base comb for [S]B), so it no longer
+ * holds up the dispatcher or the other requests' launches.  At most one such launch is in flight; it takes every generic request
+ * pending, and it does not count against the two small launches in flight.  preimage requests get their Digests from a
+ * k_queue_digests launch ahead of it on the same stream.
+ *   - Verdicts are bit for bit those of the same request with the option off, i.e. hs_verify_rec128 per record in its mode.
+ *   - Requests the generic path takes do not count in hs_queue_stats [4..5] (they count in hs_queue_generic_stats).
+ *   - Turning the option off drains the generic launches in flight; requests still waiting for one then take the slow path.
+ *   - Their records neither probe nor fill the signature cache: only device-path records with a registered key take part.  The
+ *     certificate cache works on them as on any request.  The key cache does not learn from queue requests.
+ * HS_ERR_NOMEM: no pinned host memory for the slot list (first use). */
+int hs_queue_generic(hs_queue *q, int on);
+#define HS_QUEUE_GENERIC_STATS 3
+/* [0] k_queue_generic launches, [1] records they carried, [2] requests */
+int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

@@ -133,6 +133,15 @@ class VerifyQueue {
     e_.check(hs_queue_sig_stats(q_, s.data()), "hs_queue_sig_stats");
     return s;
   }
+  // hs_queue_generic: verify requests with keys outside the committee on the GPU, not on the dispatcher thread (off by default;
+  // off drains the generic launches in flight).  Verdicts do not change.
+  void generic(bool on) { e_.check(hs_queue_generic(q_, on ? 1 : 0), "hs_queue_generic"); }
+  // hs_queue_generic_stats: [0] k_queue_generic launches, [1] records they carried, [2] requests.
+  std::array<uint64_t, HS_QUEUE_GENERIC_STATS> generic_stats() const {
+    std::array<uint64_t, HS_QUEUE_GENERIC_STATS> s{};
+    e_.check(hs_queue_generic_stats(q_, s.data()), "hs_queue_generic_stats");
+    return s;
+  }
 
  private:
   struct Pending {

@@ -37,7 +37,9 @@ pub(crate) fn queue() -> Option<*mut HsQueue> {
     QUEUE.get_or_init(|| {
         let c = ctx()?;
         let mut q = std::ptr::null_mut();
-        if unsafe { hs_queue_create(c, 0, &mut q) } == HS_OK && !q.is_null() { Some(Queue(q)) } else { None }
+        if unsafe { hs_queue_create(c, 0, &mut q) } != HS_OK || q.is_null() { return None; }
+        super::generic_queue::enable(q);
+        Some(Queue(q))
     }).as_ref().map(|q| q.0)
 }
 

@@ -33,6 +33,10 @@ pub mod cert_cache;
 /// it.  Turned on with the certificate cache (`cert_cache::enable`).
 #[path = "crypto_gpu_sig_cache.rs"]
 pub mod sig_cache;
+/// The queue's generic-key device path (hs_queue_generic): a request with a key outside the registered committee is verified by a
+/// queue kernel instead of holding up the queue's thread.  Turned on when the node-wide queue is created (`queue::queue`).
+#[path = "crypto_gpu_generic_queue.rs"]
+pub mod generic_queue;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

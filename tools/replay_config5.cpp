@@ -35,6 +35,9 @@
 // carrying the same high_qc, through (a) the queue without its certificate cache (synchronous fallback as the Rust module), (b) the
 // queue with it, (c) the synchronous batched calls; burst time, signatures verified and hs_queue_cert_stats.
 //
+// Foreign keys (alone with argv[3] = foreign_keys): single-record vote bursts with no committee registered, and bursts with one
+// request by an unregistered key (1 or 500 records) halfway through, with hs_queue_generic off and on (see run_foreign_keys).
+//
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
 #include <atomic>
@@ -1224,6 +1227,177 @@ static int run_tc_after_timeouts(hs_ctx *ctx, int rounds) {
   return bad;
 }
 
+// ---- requests with keys outside the committee (alone with argv[3] = foreign_keys): the queue's slow path (hs_queue_generic off: the
+// dispatcher thread verifies each such request synchronously) against its generic-key device path (on: k_queue_generic).
+//   (a) no committee registered: a vote burst of N - f single-record requests from 16 threads, N = 100 and 1,000: the queue with the
+//       option off, with it on, and the CPU oracle serially on one core;
+//   (b) the committee registered: the same burst (every key registered) with ONE request by an unregistered key (1 or 500 records,
+//       batch-eq) submitted once half the votes are in; p50 / p99 of the OTHER requests' latency with the option off and on, and
+//       the foreign request's own latency.
+// Every verdict, the foreign request's included, is checked against the oracle.
+struct fk_req {
+  clk::time_point *t0;
+  double *lat;
+  int *verdict;  // single-record request: its bit; the foreign group: 1 when every bit equals the oracle's, else 0
+  const std::vector<int> *want;  // the foreign group's oracle verdicts (null for a vote)
+};
+static void on_fk(void *user, size_t, int status, const uint32_t *bitmap) {
+  fk_req *r = (fk_req *)user;
+  *r->lat = us_since(*r->t0);
+  int v;
+  if (status != HS_OK) v = -1;
+  else if (!r->want) v = (int)(bitmap[0] & 1u);
+  else {
+    v = 1;
+    for (size_t i = 0; i < r->want->size(); i++) v &= (int)((bitmap[i >> 5] >> (i & 31)) & 1u) == (*r->want)[i];
+  }
+  __atomic_store_n(r->verdict, v, __ATOMIC_RELEASE);
+}
+static int foreign_keys_arm(hs_ctx *ctx, int N, bool committee, int generic, int n_foreign, int bursts, series &burst, series &vote,
+                            series &foreign, uint64_t gstats[HS_QUEUE_GENERIC_STATS], uint64_t qstats[HS_QUEUE_STATS], series *cpu) {
+  const int f = (N - 1) / 3, nv = N - f, nth = 16;
+  std::vector<uint8_t> seeds((size_t)N * 32), pks((size_t)N * 32), fseed(32), fpk(32);
+  for (int i = 0; i < N; i++) {
+    for (int j = 0; j < 32; j++) seeds[(size_t)i * 32 + j] = (uint8_t)(29 * i + 5 * j + 7 + (i >> 8));
+    hso_keygen(&seeds[(size_t)i * 32], &pks[(size_t)i * 32]);
+  }
+  for (int j = 0; j < 32; j++) fseed[j] = (uint8_t)(201 + 3 * j);
+  hso_keygen(fseed.data(), fpk.data());
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, pks.data(), committee ? N : 0, valid.data()) != HS_OK) return 1;
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 0, &q) != HS_OK || hs_queue_generic(q, generic) != HS_OK) return 1;
+  int bad = 0;
+  std::vector<hs_rec128> recs(nv), frecs(n_foreign);
+  std::vector<uint8_t> fmodes(n_foreign, HS_MODE_BATCH_EQ);
+  std::vector<int> want(nv), got(nv), fwant(n_foreign);
+  std::vector<double> lat(nv);
+  std::vector<fk_req> rq(nv);
+  for (int r = 0; r < bursts + 3; r++) {
+    const bool timed = r >= 3;
+    uint8_t pre[40], d[32];
+    for (int j = 0; j < 32; j++) pre[j] = (uint8_t)(r * 13 + j + 91 * generic);
+    const uint64_t round = 5000 + (uint64_t)r;
+    memcpy(pre + 32, &round, 8);
+    hso_digest32(pre, 40, d);
+    for (int i = 0; i < nv; i++) {
+      const int k = (i * 7 + r) % N;
+      hso_sign(&seeds[(size_t)k * 32], d, 32, recs[i].sig);
+      memcpy(recs[i].pk, &pks[(size_t)k * 32], 32);
+      memcpy(recs[i].msg, d, 32);
+      if ((i * 37 + r * 11) % 100 == 0) recs[i].sig[(i + r) % 64] ^= 0x10;  // 1 % corrupted
+    }
+    for (int i = 0; i < n_foreign; i++) {  // the foreign request: its key signs distinct Digests; 1 % corrupted
+      uint8_t m[8];
+      memcpy(m, &i, 4);
+      memcpy(m + 4, &r, 4);
+      hso_digest32(m, 8, frecs[i].msg);
+      hso_sign(fseed.data(), frecs[i].msg, 32, frecs[i].sig);
+      memcpy(frecs[i].pk, fpk.data(), 32);
+      if (i % 100 == 7) frecs[i].sig[40] ^= 1;
+      fwant[i] = (hso_verify_flags(frecs[i].sig, frecs[i].pk, frecs[i].msg, 32) & HSO_EQ_OK) ? 1 : 0;
+    }
+    clk::time_point t0 = clk::now();
+    for (int i = 0; i < nv; i++) {
+      want[i] = hso_verify_strict(recs[i].sig, recs[i].pk, recs[i].msg, 32);
+      lat[i] = us_since(t0);
+    }
+    if (timed && cpu) cpu->v.push_back(us_since(t0));
+    std::atomic<int> go{0}, submitted{0};
+    std::fill(got.begin(), got.end(), -2);
+    int fgot = -2;
+    double flat = 0;
+    fk_req fr{&t0, &flat, &fgot, &fwant};
+    std::vector<std::thread> ts;
+    for (int t = 0; t < nth; t++)
+      ts.emplace_back([&, t] {
+        while (!go.load()) {
+        }
+        for (int i = t; i < nv; i += nth) {
+          rq[i] = fk_req{&t0, &lat[i], &got[i], nullptr};
+          int rc;
+          while ((rc = hs_queue_submit(q, &recs[i], 1, HS_MODE_STRICT, on_fk, &rq[i], nullptr)) == HS_ERR_NOMEM) std::this_thread::yield();
+          if (rc != HS_OK) bad++;
+          submitted++;
+        }
+      });
+    if (n_foreign)  // the foreign request, once half the votes are in
+      ts.emplace_back([&] {
+        while (submitted.load() < nv / 2) {
+        }
+        int rc;
+        while ((rc = hs_queue_submit_group(q, frecs.data(), n_foreign, fmodes.data(), on_fk, &fr, nullptr)) == HS_ERR_NOMEM) std::this_thread::yield();
+        if (rc != HS_OK) bad++;
+      });
+    t0 = clk::now();
+    go = 1;
+    for (auto &t : ts) t.join();
+    for (int i = 0; i < nv; i++)
+      while (__atomic_load_n(&got[i], __ATOMIC_ACQUIRE) == -2) std::this_thread::yield();
+    if (n_foreign)
+      while (__atomic_load_n(&fgot, __ATOMIC_ACQUIRE) == -2) std::this_thread::yield();
+    for (int i = 0; i < nv; i++) bad += got[i] != want[i];
+    if (n_foreign) bad += fgot != 1;
+    if (timed) {
+      burst.v.push_back(*std::max_element(lat.begin(), lat.end()));
+      vote.v.insert(vote.v.end(), lat.begin(), lat.end());
+      if (n_foreign) foreign.v.push_back(flat);
+    }
+  }
+  hs_queue_generic_stats(q, gstats);
+  hs_queue_stats(q, qstats);
+  hs_queue_destroy(q);
+  hs_committee_register(ctx, nullptr, 0, nullptr);
+  return bad;
+}
+static int run_foreign_keys(hs_ctx *ctx, int bursts) {
+  printf("\"foreign_keys\": {\"gpu\": \"%s\", \"threads\": 16, \"bursts\": %d, ", gpu_identity().c_str(), bursts);
+  int bad = 0;
+  const char *arm[2] = {"queue_generic_off", "queue_generic_on"};
+  auto counters = [](const uint64_t *g, const uint64_t *s, int bursts) {
+    printf("\"generic_launches_per_burst\": %.2f, \"generic_requests_per_burst\": %.1f, \"slow_requests_per_burst\": %.1f, \"small_launches_per_burst\": %.1f",
+           (double)g[0] / (bursts + 3), (double)g[2] / (bursts + 3), (double)s[4] / (bursts + 3), (double)s[0] / (bursts + 3));
+  };
+  printf("\"no_committee\": {");
+  for (int N : {100, 1000}) {
+    printf("\"committee_%d\": {\"votes\": %d, ", N, N - (N - 1) / 3);
+    series cpu;
+    for (int g = 0; g < 2; g++) {
+      series burst, vote, none;
+      uint64_t gs[HS_QUEUE_GENERIC_STATS] = {}, qs[HS_QUEUE_STATS] = {};
+      const int b = foreign_keys_arm(ctx, N, false, g, 0, bursts, burst, vote, none, gs, qs, g ? nullptr : &cpu);
+      bad += b;
+      printf("\"%s\": {\"burst_p50_us\": %.1f, \"burst_min_us\": %.1f, \"vote_p50_us\": %.1f, \"vote_p99_us\": %.1f, ", arm[g], burst.pct(0.5), burst.pct(0.0),
+             vote.pct(0.5), vote.pct(0.99));
+      counters(gs, qs, bursts);
+      printf(", \"mismatches\": %d}, ", b);
+    }
+    printf("\"cpu_oracle_1core_serial\": {\"burst_p50_us\": %.1f}}%s", cpu.pct(0.5), N == 1000 ? "" : ", ");
+  }
+  printf("}, \"committee_registered_one_foreign_request\": {");
+  for (int N : {100, 1000}) {
+    printf("\"committee_%d\": {\"votes\": %d, ", N, N - (N - 1) / 3);
+    for (int nf : {0, 1, 500}) {
+      printf("\"foreign_records_%d\": {", nf);
+      for (int g = 0; g < 2; g++) {
+        series burst, vote, foreign;
+        uint64_t gs[HS_QUEUE_GENERIC_STATS] = {}, qs[HS_QUEUE_STATS] = {};
+        const int b = foreign_keys_arm(ctx, N, true, g, nf, bursts, burst, vote, foreign, gs, qs, nullptr);
+        bad += b;
+        printf("\"%s\": {\"other_requests_p50_us\": %.1f, \"other_requests_p99_us\": %.1f, \"burst_p50_us\": %.1f, \"foreign_request_p50_us\": %.1f, ", arm[g],
+               vote.pct(0.5), vote.pct(0.99), burst.pct(0.5), foreign.pct(0.5));
+        counters(gs, qs, bursts);
+        printf(", \"mismatches\": %d}%s", b, g || nf == 0 ? "" : ", ");
+        if (nf == 0) break;  // no foreign request: the option changes nothing
+      }
+      printf("}%s", nf == 500 ? "" : ", ");
+    }
+    printf("}%s", N == 1000 ? "" : ", ");
+  }
+  printf("}}");
+  return bad;
+}
+
 int main(int argc, char **argv) {
   const int rounds = argc > 1 ? atoi(argv[1]) : 1000;
   hs_ctx *ctx = nullptr;
@@ -1234,6 +1408,13 @@ int main(int argc, char **argv) {
   if (argc > 3 && strcmp(argv[3], "certificate_preimages") == 0) {
     printf("{");
     const int bad = run_certificate_preimages(ctx, argc > 2 ? atoi(argv[2]) : 20);
+    printf("}\n");
+    hs_ctx_destroy(ctx);
+    return bad ? 9 : 0;
+  }
+  if (argc > 3 && strcmp(argv[3], "foreign_keys") == 0) {
+    printf("{");
+    const int bad = run_foreign_keys(ctx, argc > 2 ? atoi(argv[2]) : 10);
     printf("}\n");
     hs_ctx_destroy(ctx);
     return bad ? 9 : 0;

@@ -68,6 +68,10 @@ SIGNATURES = {
     "hs_queue_sig_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_generic": (c_int, [c_void_p, c_int]),
     "hs_queue_generic_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_queue_batch": (c_int, [c_void_p, c_size_t, c_size_t]),
+    "hs_queue_submit_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t,
+                                      c_void_p, c_void_p, ctypes.POINTER(c_size_t)]),
+    "hs_queue_batch_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_destroy": (None, [c_void_p]),
 }
 

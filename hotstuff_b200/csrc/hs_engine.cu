@@ -1192,6 +1192,47 @@ __global__ void __launch_bounds__(256) k_group_and(const uint8_t *__restrict__ f
   const uint32_t word = __ballot_sync(0xffffffffu, ok);
   if (item_bitmap && (threadIdx.x & 31) == 0 && i < n_items) item_bitmap[i >> 5] = word;
 }
+// Completion of a verify-queue batch pass (hs_queue_submit_batch), in place of k_group_and + copies + a stream synchronise: item i's
+// verdict is flag bit STRICT or EQ by mode[i]; the item bits are balloted straight into the request's mapped result words (after the
+// group words) and a rejected item sets its group's bit in grej (device, zeroed ahead of the pass).  The last block to finish
+// (block counter + fence) writes the group words (1 = every item verified; a group with no items is 1) and the miss count into the
+// mapped result, fences to system scope, and raises the request's completion word tail[1] = seq for the queue's thread.
+__global__ void __launch_bounds__(256) k_batch_done(const uint8_t *__restrict__ flags, const uint8_t *__restrict__ mode, const uint32_t *__restrict__ grp,
+                                                    uint32_t n_items, uint32_t n_groups, uint32_t *grej, uint32_t *out, const uint32_t *miss_count,
+                                                    uint32_t *tail, uint32_t seq, uint32_t *counter) {
+  __shared__ int is_last;
+  const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+  const uint32_t gw = (n_groups + 31) / 32;
+  uint32_t ok = 0;
+  if (i < n_items) {
+    const uint32_t want = mode[i] == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT;
+    ok = (flags[i] & want) ? 1u : 0u;
+    if (!ok) {
+      const uint32_t j = grp[i];
+      atomicOr(grej + (j >> 5), 1u << (j & 31));
+    }
+  }
+  const uint32_t word = __ballot_sync(0xffffffffu, ok);
+  if ((threadIdx.x & 31) == 0 && i < n_items) out[gw + (i >> 5)] = word;
+  __threadfence_system();  // this block's item words and group bits before its count
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = atomicAdd(counter, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (!is_last) return;
+  __threadfence();
+  for (uint32_t w = threadIdx.x; w < gw; w += 256) {
+    const uint32_t valid = (w == gw - 1 && (n_groups & 31)) ? ((1u << (n_groups & 31)) - 1u) : 0xffffffffu;
+    out[w] = ~atomicOr(grej + w, 0u) & valid;
+  }
+  if (threadIdx.x == 0) tail[0] = miss_count ? *(volatile const uint32_t *)miss_count : n_items;
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    *counter = 0;
+    __threadfence_system();
+    *(volatile uint32_t *)(tail + 1) = seq;
+  }
+}
 // all-ones bitmap over n bits (unused high bits of the last word 0)
 __global__ void k_bitmap_ones(uint32_t *bm, size_t n) {
   const size_t w = (size_t)blockIdx.x * 256 + threadIdx.x;
@@ -1535,6 +1576,69 @@ static int learn_collect(hs_ctx *c, const in_layout &L, size_t n, bool have_look
   return HS_OK;
 }
 
+// Scratch and streams of one verify pass's main phase: the context's for run_verify, a verify queue's batch lane for its passes.
+struct pass_scratch {
+  fe *xyz;
+  uint8_t *meta;
+  uint32_t *vidx, *miss, *miss_count;  // k_key_lookup's outputs (table path with key bytes)
+  cudaStream_t side;                   // the generic pass over the lookup's misses
+  cudaEvent_t ev_side[2];
+  cudaEvent_t *prof;                   // nullable: events around k_verify_main<committee>
+};
+// The main phase on `stream`: with committee tables, [k_key_lookup, then k_verify_main<false> over the misses on S.side] beside
+// k_verify_main<true>; without, k_verify_main<false> over every record.  after_lookup(have_lookup) runs where run_verify collects
+// keys for the key cache.  L.vidx is set to the lookup's indices when it runs.
+template <class AfterLookup>
+static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool indexed, const pass_scratch &S, cudaStream_t stream,
+                       AfterLookup after_lookup) {
+  main_out O{S.xyz, S.meta, 0};
+  committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
+  if (committee) {
+    if (!indexed) {
+      key_table T{c->d_slots, c->slot_mask, c->d_pks, (uint32_t)c->n_keys};
+      HS_CUDA(c, cudaMemsetAsync(S.miss_count, 0, 4, stream));
+      k_key_lookup<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, T, S.vidx, S.miss, S.miss_count);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+      L.vidx = S.vidx;
+      O.side_pass = 1;
+      HS_TRY(after_lookup(true));
+      // Records whose key is not registered take the generic path over the compacted list.  One generic verify has a
+      // ~0.8 ms single-warp latency, so the pass runs on the high-priority side stream CONCURRENTLY with the committee
+      // pass (disjoint outputs); its length stays on the device (no host round trip).
+      HS_CUDA(c, cudaEventRecord(S.ev_side[0], stream));
+      HS_CUDA(c, cudaStreamWaitEvent(S.side, S.ev_side[0], 0));
+      unsigned grid = blocks_for(n, 32);
+      if (grid > c->n_sms * 8u) grid = c->n_sms * 8u;
+      k_verify_main<false><<<grid, 32, 0, S.side>>>(L, 0, S.miss_count, S.miss, c->d_btable, C, O, c->cp);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+      HS_CUDA(c, cudaEventRecord(S.ev_side[1], S.side));
+    }
+    if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[0], stream));
+    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
+    if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[1], stream));
+    c->launches++;
+    HS_CUDA(c, cudaGetLastError());
+    if (!indexed) HS_CUDA(c, cudaStreamWaitEvent(stream, S.ev_side[1], 0));
+  } else {
+    HS_TRY(after_lookup(false));
+    k_verify_main<false><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
+    c->launches++;
+    HS_CUDA(c, cudaGetLastError());
+  }
+  return HS_OK;
+}
+// Threads of k_verify_finish own `fin_group` records each; launched on `stream`.
+static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz, const uint8_t *meta, uint32_t mode, uint32_t *d_bitmap,
+                         uint8_t *d_flags_out, const peer_route &P, int fin_group, cudaStream_t stream) {
+  const size_t fin_threads = (n + fin_group - 1) / fin_group;
+  k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, d_flags_out, P, fin_group);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+
 // Runs lookup (optional) -> main (committee and/or generic) -> finish on `stream` for a device-resident layout.
 // use_lookup: L.pk is valid and a committee is registered -> resolve indices on the device.
 static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t *d_bitmap, cudaStream_t stream, bool indexed,
@@ -1560,50 +1664,18 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   }
   HS_TRY(ensure(c, XYZ, n * 3 * sizeof(fe)));
   HS_TRY(ensure(c, META, n));
-  main_out O{(fe *)XYZ.p, (uint8_t *)META.p, 0};
-  committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
   const bool committee = c->n_keys > 0 && (indexed || L.pk);
   if (!committee && !L.pk) return fail(c, HS_ERR_ARG, "verify without keys");
-  if (committee) {
-    if (!indexed) {
-      HS_TRY(ensure(c, c->vidx, n * 4));
-      HS_TRY(ensure(c, c->miss, n * 4));
-      key_table T{c->d_slots, c->slot_mask, c->d_pks, (uint32_t)c->n_keys};
-      HS_CUDA(c, cudaMemsetAsync(c->d_miss_count, 0, 4, stream));
-      k_key_lookup<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, T, (uint32_t *)c->vidx.p, (uint32_t *)c->miss.p, c->d_miss_count);
-      c->launches++;
-      HS_CUDA(c, cudaGetLastError());
-      L.vidx = (const uint32_t *)c->vidx.p;
-      O.side_pass = 1;
-      HS_TRY(learn_collect(c, L, n, true, stream));
-      // Records whose key is not registered take the generic path over the compacted list.  One generic verify has a
-      // ~0.8 ms single-warp latency, so the pass runs on the high-priority side stream CONCURRENTLY with the committee
-      // pass (disjoint outputs); its length stays on the device (no host round trip).
-      HS_CUDA(c, cudaEventRecord(c->ev_side[0], stream));
-      HS_CUDA(c, cudaStreamWaitEvent(c->stream_side, c->ev_side[0], 0));
-      unsigned grid = blocks_for(n, 32);
-      if (grid > c->n_sms * 8u) grid = c->n_sms * 8u;
-      k_verify_main<false><<<grid, 32, 0, c->stream_side>>>(L, 0, c->d_miss_count, (const uint32_t *)c->miss.p, c->d_btable, C, O, c->cp);
-      c->launches++;
-      HS_CUDA(c, cudaGetLastError());
-      HS_CUDA(c, cudaEventRecord(c->ev_side[1], c->stream_side));
-    }
-    if (c->profile_main) HS_CUDA(c, cudaEventRecord(c->ev_prof[0], stream));
-    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
-    if (c->profile_main) HS_CUDA(c, cudaEventRecord(c->ev_prof[1], stream));
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
-    if (!indexed) HS_CUDA(c, cudaStreamWaitEvent(stream, c->ev_side[1], 0));
-  } else {
-    HS_TRY(learn_collect(c, L, n, false, stream));
-    k_verify_main<false><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
+  if (committee && !indexed) {
+    HS_TRY(ensure(c, c->vidx, n * 4));
+    HS_TRY(ensure(c, c->miss, n * 4));
   }
+  const pass_scratch S{(fe *)XYZ.p, (uint8_t *)META.p, (uint32_t *)c->vidx.p, (uint32_t *)c->miss.p, c->d_miss_count, c->stream_side,
+                       {c->ev_side[0], c->ev_side[1]}, c->profile_main ? c->ev_prof : nullptr};
+  HS_TRY(launch_main(c, L, n, committee, indexed, S, stream, [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }));
   // small batches: small groups, so that enough blocks exist to hide each block's serial inversion; when the tail overlaps the next pass
   // (deferred mode) latency is hidden anyway and the 16-record group costs the fewest inversions
   const int fin_group = (defer || n >= (1u << 19)) ? 16 : (n >= (1u << 18) ? 8 : 4);
-  const size_t fin_threads = (n + fin_group - 1) / fin_group;
   peer_route P{};
   if (c->peer_armed) {
     P = c->peers;
@@ -1615,9 +1687,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_CUDA(c, cudaStreamWaitEvent(c->stream_tail, c->ev_main_done, 0));
     fin_stream = c->stream_tail;
   }
-  k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, fin_stream>>>(L, n, (const fe *)XYZ.p, (const uint8_t *)META.p, mode, d_bitmap, d_flags_out, P, fin_group);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p, (const uint8_t *)META.p, mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
   return HS_OK;
 }
@@ -1820,6 +1890,37 @@ struct hs_queue {
   uint32_t *h_gslot = nullptr, *d_gslot = nullptr;   // mapped pinned: a generic launch's ring slots at positions [lo, lo + records)
   qmsg_desc *h_gmlist = nullptr, *d_gmlist = nullptr;  // mapped pinned: its preimage requests' descriptors, from position lo on
   uint64_t gstats[HS_QUEUE_GENERIC_STATS] = {};      // hs_queue_generic_stats
+  // batch lane (hs_queue_batch): off while b_max_items is 0.  Requests wait in bq in submit order, each with a region of the mapped
+  // arena h_barena (b_acap bytes, positions growing without bound like the preimage arena's: [b_head, b_tail) in use); a region is
+  // filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at a time (b_cur, dispatcher thread),
+  // and regions are released in request order when their requests complete.  The lane's buffers and streams change only while the
+  // lane is off and bq is empty.
+  struct breq {
+    size_t ticket;
+    hs_queue_cb *cb;
+    void *user;
+    uint32_t n, n_groups, n_msgs;
+    uint64_t pre_bytes;
+    uint64_t a_off, a_end;  // region offset in the arena; arena position past it
+    uint64_t o_pre, o_sig, o_pk, o_mi, o_gi, o_mo, o_res, o_tail;  // sections, relative to the region (batch_layout)
+    uint32_t seq;           // the completion word k_batch_done writes
+    bool ready;
+  };
+  size_t b_max_items = 0, b_max_bytes = 0;
+  uint64_t b_acap = 0, b_head = 0, b_tail = 0;
+  uint8_t *h_barena = nullptr, *d_barena = nullptr;  // mapped pinned: request regions (inputs, then result words and the tail)
+  uint8_t *d_bmirror = nullptr;                     // device: the inputs of the region in flight, at the same offsets
+  uint32_t *d_bdig = nullptr;                       // device: the request's Digests, 32 bytes per preimage
+  fe *d_bxyz = nullptr;
+  uint8_t *d_bmeta = nullptr, *d_bflags = nullptr;
+  uint32_t *d_bvidx = nullptr, *d_bmiss = nullptr, *d_bmiss_count = nullptr, *d_bitems = nullptr, *d_bgrej = nullptr, *d_bcounter = nullptr;
+  cudaStream_t b_stream = nullptr, b_side = nullptr;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
+  cudaEvent_t b_ev[2] = {nullptr, nullptr};
+  std::deque<breq> bq;
+  breq *b_cur = nullptr;  // the request in flight (dispatcher thread; set and cleared under q->mu)
+  uint32_t b_seq = 0;
+  uint64_t bstats[HS_QUEUE_BATCH_STATS] = {};  // hs_queue_batch_stats
+  std::mutex b_cfg_mu;                          // serialises hs_queue_batch calls
   uint64_t head = 0, launched = 0, tail = 0;
   size_t next_ticket = 1;
   uint32_t seq = 0;
@@ -2205,10 +2306,13 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
 // its verdicts (the flags -> bits mapping of run_small).  A launch is retired once every request in its range — riders
 // included — has its word.  Every 4,096 passes both streams are queried: a CUDA error, or a drained stream with a word still
 // missing in a launch it ran, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
+static void batch_watch(hs_queue *q, bool query);
 static void queue_watch(hs_queue *q) {
   std::vector<queue_completion> fire;
   cudaError_t qes[2] = {cudaErrorNotReady, cudaErrorNotReady};  // [0] stream, [1] bulk_stream: a launch is judged by its own
-  if ((++q->spins & 0xfff) == 0) {  // queried BEFORE the words are read
+  const bool query = (++q->spins & 0xfff) == 0;
+  batch_watch(q, query);
+  if (query) {  // queried BEFORE the words are read
     qes[0] = cudaStreamQuery(q->stream);
     qes[1] = cudaStreamQuery(q->bulk_stream);
   }
@@ -2259,6 +2363,143 @@ static void queue_watch(hs_queue *q) {
   queue_fire(fire);
 }
 
+// ---- batch lane (hs_queue_submit_batch): one hs_verify_groups pass per request, on the lane's stream and scratch
+// A request's region: pre_off (u64, n_msgs + 1) | preimages | sig (64 B each) | pk (32 B each) | msg_idx (u32) | group_idx (u32) |
+// modes (u8) | result words (group words, then item words) | tail: [0] items outside the committee, [1] completion word.  Every
+// section starts 16-byte aligned.  The inputs (everything before the result words) cross the bus in one copy into the mirror.
+struct batch_layout {
+  uint64_t o_pre, o_sig, o_pk, o_mi, o_gi, o_mo, o_res, o_tail, size;
+};
+static batch_layout batch_layout_of(uint64_t n_msgs, uint64_t pre_bytes, uint64_t n, uint64_t n_groups) {
+  auto al = [](uint64_t x) { return (x + 15) & ~(uint64_t)15; };
+  batch_layout b;
+  b.o_pre = al(8 * (n_msgs + 1));
+  b.o_sig = b.o_pre + al(pre_bytes);
+  b.o_pk = b.o_sig + 64 * n;
+  b.o_mi = b.o_pk + 32 * n;
+  b.o_gi = b.o_mi + al(4 * n);
+  b.o_mo = b.o_gi + al(4 * n);
+  b.o_res = b.o_mo + al(n);
+  b.o_tail = b.o_res + al(4 * ((n_groups + 31) / 32 + (n + 31) / 32));
+  b.size = b.o_tail + 16;
+  return b;
+}
+static uint64_t batch_words(const hs_queue::breq &r) { return (r.n_groups + 31) / 32 + (r.n + 31) / 32; }
+
+// Completes the request in flight (dispatcher thread): its result words go to its callback or ticket, then its region is released.
+static void batch_complete(hs_queue *q, int status) {
+  std::vector<queue_completion> fire;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    const hs_queue::breq &r = *q->b_cur;
+    const uint32_t bits = (uint32_t)(32 * batch_words(r));
+    const uint32_t *res = status == HS_OK ? reinterpret_cast<const uint32_t *>(q->h_barena + r.a_off + r.o_res) : nullptr;
+    if (status == HS_OK) {
+      q->bstats[0]++;
+      q->bstats[1] += r.n;
+      q->bstats[2] += r.n_groups;
+      q->bstats[3] += r.pre_bytes;
+      q->bstats[4] += reinterpret_cast<const volatile uint32_t *>(q->h_barena + r.a_off + r.o_tail)[0];
+    }
+    if (r.cb) {
+      fire.push_back(queue_completion{r.cb, r.user, r.ticket, status, {}});
+      fire.back().bits.set(bits, res);
+    } else {
+      hs_queue::result &out = q->results[r.ticket];
+      out.done = true;
+      out.status = status;
+      out.bits.set(bits, res);
+    }
+    q->b_head = r.a_end;
+    q->b_cur = nullptr;
+    q->bq.pop_front();
+    q->cv_done.notify_all();
+  }
+  queue_fire(fire);
+}
+
+// Enqueues the pass of request r on the lane's streams, under c->mu only while it enqueues.  Touches no scratch, stream, event or
+// per-call state of the context, so synchronous calls, `_dev` calls and the queue's other launches can be in flight meanwhile.
+static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> g(c->mu);
+  cudaStream_t s = q->b_stream;
+  const uint8_t *m = q->d_bmirror + r.a_off;
+  HS_CUDA(c, cudaMemcpyAsync(q->d_bmirror + r.a_off, q->h_barena + r.a_off, r.o_res, cudaMemcpyHostToDevice, s));
+  k_digest32<<<blocks_for(r.n_msgs), HS_THREADS, 0, s>>>(m + r.o_pre, reinterpret_cast<const uint64_t *>(m), 0, r.n_msgs, q->d_bdig);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  in_layout L{m + r.o_sig, 64, m + r.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(q->d_bdig), 32, reinterpret_cast<const uint32_t *>(m + r.o_mi),
+              nullptr, 32, 0};
+  // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
+  const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables;
+  const pass_scratch S{q->d_bxyz, q->d_bmeta, q->d_bvidx, q->d_bmiss, q->d_bmiss_count, q->b_side, {q->b_ev[0], q->b_ev[1]}, nullptr};
+  HS_TRY(launch_main(c, L, r.n, committee, false, S, s, [](bool) { return HS_OK; }));
+  const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
+  HS_TRY(launch_finish(c, L, r.n, q->d_bxyz, q->d_bmeta, HS_MODE_STRICT, q->d_bitems, q->d_bflags, peer_route{}, fin_group, s));
+  HS_CUDA(c, cudaMemsetAsync(q->d_bgrej, 0, 4 * ((r.n_groups + 31) / 32), s));
+  uint8_t *res = q->d_barena + r.a_off;
+  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->d_bflags, m + r.o_mo, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->d_bgrej,
+                                                    reinterpret_cast<uint32_t *>(res + r.o_res), committee ? q->d_bmiss_count : nullptr,
+                                                    reinterpret_cast<uint32_t *>(res + r.o_tail), r.seq, q->d_bcounter);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+static void batch_dispatch(hs_queue *q) {
+  hs_queue::breq *r;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    r = q->b_cur = &q->bq.front();
+    r->seq = ++q->b_seq ? q->b_seq : ++q->b_seq;  // never 0: the region's tail was zeroed at submit
+  }
+  if (batch_launch(q, *r) != HS_OK) batch_complete(q, HS_ERR_CUDA);
+}
+// The request in flight is done when its completion word carries its number.  When `query`, the lane's streams are queried first: a
+// CUDA error, or both streams drained without the word, completes it with HS_ERR_CUDA (never an accept).
+static void batch_watch(hs_queue *q, bool query) {
+  if (!q->b_cur) return;
+  const hs_queue::breq &r = *q->b_cur;
+  cudaError_t qe[2] = {cudaErrorNotReady, cudaErrorNotReady};
+  if (query) {
+    qe[0] = cudaStreamQuery(q->b_stream);
+    qe[1] = cudaStreamQuery(q->b_side);
+  }
+  int status = -1;
+  for (cudaError_t x : qe)
+    if (x != cudaSuccess && x != cudaErrorNotReady) status = fail(q->c, HS_ERR_CUDA, "verify queue batch pass", x);
+  if (status < 0 && reinterpret_cast<const volatile uint32_t *>(q->h_barena + r.a_off + r.o_tail)[1] == r.seq) {
+    std::atomic_thread_fence(std::memory_order_acquire);
+    status = HS_OK;
+  } else if (status < 0 && qe[0] == cudaSuccess && qe[1] == cudaSuccess) {
+    status = fail(q->c, HS_ERR_CUDA, "verify queue: k_batch_done did not complete");
+  }
+  if (status >= 0) batch_complete(q, status);
+}
+static bool batch_ready_locked(const hs_queue *q) { return !q->b_cur && !q->bq.empty() && q->bq.front().ready; }
+// Releases the lane's buffers and streams (the lane is off and drained).
+static void batch_free(hs_queue *q) {
+  for (cudaStream_t s : {q->b_stream, q->b_side})
+    if (s) {
+      cudaStreamSynchronize(s);
+      cudaStreamDestroy(s);
+    }
+  for (cudaEvent_t &ev : q->b_ev)
+    if (ev) cudaEventDestroy(ev);
+  if (q->h_barena) cudaFreeHost(q->h_barena);
+  for (void *p : {(void *)q->d_bmirror, (void *)q->d_bdig, (void *)q->d_bxyz, (void *)q->d_bmeta, (void *)q->d_bflags, (void *)q->d_bvidx,
+                  (void *)q->d_bmiss, (void *)q->d_bmiss_count, (void *)q->d_bitems, (void *)q->d_bgrej, (void *)q->d_bcounter})
+    cudaFree(p);
+  q->b_stream = q->b_side = nullptr;
+  q->b_ev[0] = q->b_ev[1] = nullptr;
+  q->h_barena = q->d_barena = q->d_bmirror = nullptr;
+  q->d_bdig = nullptr;
+  q->d_bxyz = nullptr;
+  q->d_bmeta = q->d_bflags = nullptr;
+  q->d_bvidx = q->d_bmiss = q->d_bmiss_count = q->d_bitems = q->d_bgrej = q->d_bcounter = nullptr;
+  q->b_acap = 0;
+}
+
 static size_t queue_small_inflight_locked(const hs_queue *q) {
   size_t k = 0;
   for (const hs_queue::launch &L : q->inflight) k += !L.bulk;
@@ -2285,6 +2526,10 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_fire(fire);
       lk.lock();
+    } else if (batch_ready_locked(q)) {  // first: one short enqueue, and a vote burst would otherwise keep postponing it
+      lk.unlock();
+      batch_dispatch(q);
+      lk.lock();
     } else if ((q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) || queue_generic_ready_locked(q)) {
       // everything pending; only the waiting generic requests while the small launches are at their limit
       const uint64_t lo = q->launched, hi = queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT ? q->tail : lo;
@@ -2292,11 +2537,11 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_dispatch(q, lo, hi);
       lk.lock();
-    } else if (!q->inflight.empty()) {
+    } else if (!q->inflight.empty() || q->b_cur) {
       lk.unlock();
       queue_watch(q);
       lk.lock();
-    } else if (q->stop) {
+    } else if (q->stop && q->bq.empty()) {  // (a batch request still being copied in is announced on cv_work)
       break;
     } else {
       q->cv_work.wait(lk);
@@ -2334,6 +2579,7 @@ static void queue_free(hs_queue *q) {
   cudaFree(q->d_sig_key);
   cudaFree(q->d_sig_ctr);
   if (q->h_sig_ctr) cudaFreeHost(q->h_sig_ctr);
+  batch_free(q);
   delete q;
 }
 
@@ -3723,6 +3969,116 @@ int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]) {
   if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_generic_stats: bad argument");
   std::lock_guard<std::mutex> g(q->mu);
   memcpy(out, q->gstats, sizeof(q->gstats));
+  return HS_OK;
+}
+
+#define HS_QUEUE_BATCH_MAX_ITEMS (1u << 24)
+#define HS_QUEUE_BATCH_MAX_BYTES (1ull << 30)
+int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
+  if (!q || (max_items == 0) != (max_bytes == 0) || max_items > HS_QUEUE_BATCH_MAX_ITEMS || max_bytes > HS_QUEUE_BATCH_MAX_BYTES)
+    return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_batch: bad argument");
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> cfg(q->b_cfg_mu);
+  {
+    std::unique_lock<std::mutex> lk(q->mu);
+    if (max_items == q->b_max_items && max_bytes == q->b_max_bytes) return HS_OK;
+    q->b_max_items = q->b_max_bytes = 0;  // refuses new batch requests while the lane changes
+    q->cv_done.wait(lk, [q] { return q->bq.empty(); });
+  }
+  HS_CUDA(c, cudaSetDevice(c->device));
+  batch_free(q);
+  if (!max_items) return HS_OK;
+  uint64_t acap = 4096;  // two of the largest regions fit: one can be filled while the other's pass runs
+  while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->b_stream, cudaStreamNonBlocking, lo);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->b_side, cudaStreamNonBlocking, hi);
+  for (cudaEvent_t &ev : q->b_ev)
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_barena, acap, cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_barena, q->h_barena, 0);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmirror, acap);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bdig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bxyz, max_items * 3 * sizeof(fe));
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmeta, max_items);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bflags, max_items);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bvidx, max_items * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmiss, max_items * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmiss_count, 4);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bitems, (max_items + 31) / 32 * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bgrej, max_bytes + 16);  // group words of a region fit in max_bytes
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_bcounter, 4);
+  if (e == cudaSuccess) e = cudaMemset(q->d_bcounter, 0, 4);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    batch_free(q);
+    return fail(c, HS_ERR_NOMEM, "hs_queue_batch: no pinned host or device memory for the batch lane", e);
+  }
+  memset(q->h_barena, 0, acap);
+  std::lock_guard<std::mutex> g(q->mu);
+  q->b_acap = acap;
+  q->b_head = q->b_tail = 0;
+  q->b_max_items = max_items;
+  q->b_max_bytes = max_bytes;
+  return HS_OK;
+}
+
+int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                          const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *modes, size_t n_items, size_t n_groups, hs_queue_cb *cb,
+                          void *user, size_t *out_ticket) {
+  if (!q || !pre_off || !sig || !pk || !msg_idx || !group_idx || n_items == 0 || n_groups == 0 || n_msgs == 0 || n_items > HS_QUEUE_BATCH_MAX_ITEMS ||
+      n_groups > UINT32_MAX || n_msgs > UINT32_MAX)
+    return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_batch: bad argument");
+  if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages)) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: bad preimage offsets");
+  for (size_t i = 0; i < n_items; i++)
+    if (msg_idx[i] >= n_msgs || group_idx[i] >= n_groups || (modes && modes[i] > HS_MODE_BATCH_EQ))
+      return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: index or mode out of range");
+  const uint64_t pre_bytes = pre_off[n_msgs];
+  const batch_layout B = batch_layout_of(n_msgs, pre_bytes, n_items, n_groups);
+  hs_queue::breq *r;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: queue is being destroyed");
+    if (!q->b_max_items) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: the batch lane is off (hs_queue_batch)");
+    if (n_items > q->b_max_items || B.size > q->b_max_bytes) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: larger than the batch lane's limits");
+    uint64_t start = q->b_tail;
+    if ((start & (q->b_acap - 1)) + B.size > q->b_acap) start += q->b_acap - (start & (q->b_acap - 1));  // would cross the end: start over
+    if (start + B.size - q->b_head > q->b_acap) {  // arena full
+      if (q->b_head != q->b_tail) return HS_ERR_NOMEM;
+      start = q->b_head = q->b_tail = start;  // empty: the skipped tail is free too
+    }
+    q->b_tail = start + B.size;
+    const size_t ticket = q->next_ticket++;
+    q->bq.push_back(hs_queue::breq{ticket, cb, user, (uint32_t)n_items, (uint32_t)n_groups, (uint32_t)n_msgs, pre_bytes, start & (q->b_acap - 1),
+                                   start + B.size, B.o_pre, B.o_sig, B.o_pk, B.o_mi, B.o_gi, B.o_mo, B.o_res, B.o_tail, 0, false});
+    r = &q->bq.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
+    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)(32 * batch_words(*r)), {}};
+    if (out_ticket) *out_ticket = ticket;
+  }
+  // the region is this request's alone until it completes: fill it without holding q->mu
+  uint8_t *a = q->h_barena + r->a_off;
+  memcpy(a, pre_off, 8 * (n_msgs + 1));
+  if (pre_bytes) memcpy(a + B.o_pre, preimages, pre_bytes);
+  memcpy(a + B.o_sig, sig, 64 * n_items);
+  memcpy(a + B.o_pk, pk, 32 * n_items);
+  memcpy(a + B.o_mi, msg_idx, 4 * n_items);
+  memcpy(a + B.o_gi, group_idx, 4 * n_items);
+  if (modes) memcpy(a + B.o_mo, modes, n_items);
+  else memset(a + B.o_mo, HS_MODE_STRICT, n_items);
+  memset(a + B.o_res, 0, B.size - B.o_res);  // result words and the completion word
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    r->ready = true;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+
+int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_batch_stats: bad argument");
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, q->bstats, sizeof(q->bstats));
   return HS_OK;
 }
 

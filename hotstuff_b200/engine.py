@@ -326,8 +326,20 @@ class VerifyQueue:
     def _on_done(self, user, ticket, status, bitmap):
         with self._lock:
             fn, n = self._callbacks.pop(user)
-        words = np.ctypeslib.as_array(bitmap, shape=((n + 31) // 32,)).copy()
-        fn(int(ticket), int(status), bitmap_to_bools(words, n))
+        words = np.ctypeslib.as_array(bitmap, shape=(self._n_words(n),)).copy()
+        fn(int(ticket), int(status), self._bools(words, n))
+
+    @staticmethod
+    def _n_words(n):
+        """Words of a ticket's verdict bitmap: n is a record count, or (n_groups, n_items) for a batch ticket."""
+        return (n[0] + 31) // 32 + (n[1] + 31) // 32 if isinstance(n, tuple) else (n + 31) // 32
+
+    @staticmethod
+    def _bools(words, n):
+        if isinstance(n, tuple):  # a batch ticket: group words, then item words
+            gw = (n[0] + 31) // 32
+            return bitmap_to_bools(words[:gw], n[0]), bitmap_to_bools(words[gw:], n[1])
+        return bitmap_to_bools(words, n)
 
     def submit(self, recs, mode=MODE_STRICT, callback=None):
         """recs: (n,128) uint8 [sig64|pk32|msg32], 1 <= n <= 64.  Returns the ticket, or None when the ring is full (retry later)."""
@@ -363,6 +375,40 @@ class VerifyQueue:
             self.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk) if n else None,
             _ptr(mi) if n else None, _ptr(mo), n, cb, user, t))
 
+    def batch(self, max_items, max_bytes):
+        """Turns the batch lane on (hs_queue_batch): submit_batch requests of up to max_items items and max_bytes of arena region each.
+        (0, 0) turns it off (the default).  Resizing or turning it off first waits for every batch request already submitted."""
+        self.engine._check(self.lib.hs_queue_batch(self.h, int(max_items), int(max_bytes)), "hs_queue_batch")
+
+    def submit_batch(self, preimages, pre_off, sig, pk, msg_idx, group_idx, n_groups, modes=None, callback=None):
+        """Engine.verify_groups (with key bytes) as ONE non-blocking request on the batch lane (hs_queue_submit_batch): item i is
+        (sig[i], pk[i]) over SHA-512(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1]))[..32] in group group_idx[i], judged by
+        modes[i] (None = all strict).  poll / wait / the callback give (group bools, item bools), equal to verify_groups on the same
+        arrays.  Returns the ticket, or None when the lane's arena has no room now."""
+        pre = _u8(preimages)
+        off = np.ascontiguousarray(pre_off, dtype=np.uint64).reshape(-1)
+        sig = _u8(sig, 64).reshape(-1, 64)
+        pk = _u8(pk, 32).reshape(-1, 32)
+        mi = np.ascontiguousarray(msg_idx, dtype=np.uint32).reshape(-1)
+        gi = np.ascontiguousarray(group_idx, dtype=np.uint32).reshape(-1)
+        n = sig.shape[0]
+        mo = None if modes is None else np.ascontiguousarray(modes, dtype=np.uint8).reshape(-1)
+        if pk.shape[0] != n or mi.shape[0] != n or gi.shape[0] != n or (mo is not None and mo.shape[0] != n) or off.shape[0] < 1:
+            raise ValueError("submit_batch: %d signatures, %d keys, %d message indices, %d group indices, %s modes, %d offsets"
+                             % (n, pk.shape[0], mi.shape[0], gi.shape[0], "no" if mo is None else mo.shape[0], off.shape[0]))
+        return self._enqueue("hs_queue_submit_batch", (int(n_groups), n), callback, lambda cb, user, t: self.lib.hs_queue_submit_batch(
+            self.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk) if n else None,
+            _ptr(mi) if n else None, _ptr(gi) if n else None, _ptr(mo), n, int(n_groups), cb, user, t))
+
+    BATCH_STATS = ("passes", "items", "groups", "preimage_bytes", "outside_committee")
+
+    def batch_stats(self):
+        """Counters of completed batch passes (hs_queue_batch_stats): passes, items, groups, preimage bytes hashed, and items whose
+        key was outside the committee (every item when none is registered)."""
+        out = (ctypes.c_uint64 * len(self.BATCH_STATS))()
+        self.engine._check(self.lib.hs_queue_batch_stats(self.h, out), "hs_queue_batch_stats")
+        return dict(zip(self.BATCH_STATS, (int(x) for x in out)))
+
     def _submit(self, fn, name, recs, mode_arg, callback):
         recs = _u8(recs, 128).reshape(-1, 128)
         n = recs.shape[0]
@@ -394,16 +440,17 @@ class VerifyQueue:
         with self._lock:
             n = self._n.pop(ticket, None)
         self.engine._check(rc, "hs_queue ticket %d" % ticket)
-        return bitmap_to_bools(words, n)
+        return self._bools(words, n)
 
     def _words(self, ticket):
         """The verdict buffer of a ticket read by poll / wait: (n + 31) / 32 words (at least 2: an unknown ticket is an error)."""
         with self._lock:
             n = self._n.get(int(ticket), 64)
-        return np.zeros(max(2, (n + 31) // 32), dtype=np.uint32)
+        return np.zeros(max(2, self._n_words(n)), dtype=np.uint32)
 
     def poll(self, ticket):
-        """None while the request is in flight, else its verdicts (bool[n]); consumes the ticket."""
+        """None while the request is in flight, else its verdicts (bool[n]; a batch ticket: (group bools, item bools)); consumes the
+        ticket."""
         done = ctypes.c_int(0)
         words = self._words(ticket)
         rc = self.lib.hs_queue_poll(self.h, int(ticket), ctypes.byref(done), _ptr(words))
@@ -412,7 +459,8 @@ class VerifyQueue:
         return self._take(ticket, rc, words)
 
     def wait(self, ticket):
-        """Blocks until the request is done; returns its verdicts (bool[n]) and consumes the ticket."""
+        """Blocks until the request is done; returns its verdicts (bool[n]; a batch ticket: (group bools, item bools)) and consumes
+        the ticket."""
         words = self._words(ticket)
         rc = self.lib.hs_queue_wait(self.h, int(ticket), _ptr(words))
         return self._take(ticket, rc, words)

@@ -2,6 +2,7 @@
 the C ABI's hs_ingest_consensus_frames (hotstuff_b200/csrc/hs_ingest.cpp).  Replaces, for the crypto path, the reference's
 bincode::deserialize + per-signature walk (consensus/src/consensus.rs:33-39,138; crypto/src/lib.rs:94-112,178-182)."""
 import ctypes
+import threading
 
 import numpy as np
 
@@ -62,9 +63,40 @@ def submit_frame(queue, frame, callback=None):
     return g["info"][0], queue.submit_msgs(g["preimages"], g["pre_off"], g["sig"], g["pk"], g["msg_idx"], modes=g["mode"], callback=callback)
 
 
+def submit_frames(queue, frames, callback=None):
+    """Ingests many frames and submits every signature in them to a VerifyQueue's batch lane as ONE request
+    (VerifyQueue.submit_batch, group = frame).  Returns (ingest, ticket): ingest is what ingest_frames returns, ticket None when the
+    frames carry no signature (nothing is submitted) or the lane has no room now.  The verdicts are (frame bools, item bools in
+    ingest order); a frame without items is True.  The stake / duplicate pre-checks stay with the caller (verify_frames_queued)."""
+    g = ingest_frames(frames)
+    if len(g["sig"]) == 0:
+        return g, None
+    return g, queue.submit_batch(g["preimages"], g["pre_off"], g["sig"], g["pk"], g["msg_idx"], g["group_idx"], g["n_frames"], modes=g["mode"],
+                                 callback=callback)
+
+
 def verify_frames(frames, committee, engine):
     """Ingest + the reference's pre-checks + ONE engine pass.  Returns a list: None (valid), "Malformed", or the ConsensusError name
     the reference would raise first (same order as messages.verify_blocks).  SyncRequest frames are None (nothing to verify)."""
+    def run(g, keep, n):
+        return engine.verify_groups(g["preimages"], g["pre_off"], g["sig"][keep], g["msg_idx"][keep], g["group_idx"][keep], n, mode=g["mode"][keep],
+                                    pk=g["pk"][keep], want_items=True)[1]
+    return _verify_frames(frames, committee, run)
+
+
+def verify_frames_queued(frames, committee, queue):
+    """verify_frames with the pass on a VerifyQueue's batch lane (VerifyQueue.submit_batch): the same pre-checks, error names and error
+    order.  Waits for the lane when its arena has no room."""
+    def run(g, keep, n):
+        while (t := queue.submit_batch(g["preimages"], g["pre_off"], g["sig"][keep], g["pk"][keep], g["msg_idx"][keep], g["group_idx"][keep], n,
+                                       modes=g["mode"][keep])) is None:
+            threading.Event().wait(0.0005)  # no room now: back-pressure
+        return queue.wait(t)[1]
+    return _verify_frames(frames, committee, run)
+
+
+def _verify_frames(frames, committee, run):
+    """The pre-checks and verdict order of verify_frames; run(ingest, kept items mask, n_frames) -> item bools of the kept items."""
     g = ingest_frames(frames)
     info, pk = g["info"], g["pk"]
     n = g["n_frames"]
@@ -108,9 +140,7 @@ def verify_frames(frames, committee, engine):
     keep = ~skip
     items = np.zeros(len(skip), dtype=bool)
     if keep.any():
-        _, got = engine.verify_groups(g["preimages"], g["pre_off"], g["sig"][keep], g["msg_idx"][keep], g["group_idx"][keep], n, mode=g["mode"][keep],
-                                      pk=g["pk"][keep], want_items=True)
-        items[keep] = got
+        items[keep] = run(g, keep, n)
     for j in range(n):
         f = info[j]
         if out[j] is not None or f["kind"] == KIND_SYNC_REQUEST:

@@ -302,6 +302,30 @@ int hs_queue_generic(hs_queue *q, int on);
 #define HS_QUEUE_GENERIC_STATS 3
 /* [0] k_queue_generic launches, [1] records they carried, [2] requests */
 int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]);
+/* Batch lane: a whole hs_verify_groups pass as ONE non-blocking queue request (a 10,000-validator Block, a view-change burst of
+ * Timeouts, many ingested frames), verified by the throughput kernels of hs_verify_groups on the lane's own stream and scratch.  The
+ * context's mutex is held only while the pass's launches are enqueued, so the queue's vote launches and the synchronous entry
+ * points go on meanwhile.  Batch requests never enter the ring, take no part in the certificate or signature caches and do not
+ * count in the other queue counters; they run one pass at a time, in submit order.
+ * max_items / max_bytes bound one request (items; bytes of its arena region: offsets, preimages, signatures, keys, indices, modes,
+ * result words).  0, 0 = off (the default).  Resizing or turning it off first waits for every batch request already submitted.
+ * HS_ERR_NOMEM: no pinned host or device memory (the lane is then off). */
+int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes);
+/* hs_verify_groups as ONE non-blocking queue request.  The arrays and meaning are those of hs_verify_groups with key bytes.
+ * Item i is (sig[i], pk[i]) over Digest(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1])), in group group_idx[i],
+ * judged by modes[i] (NULL = all strict).  Group and item bits equal hs_verify_groups on the same arrays, bit for bit, with or
+ * without a registered committee (without one every item takes the generic kernel; the lane never teaches the key cache).
+ * Completion, tickets, poll / wait / callback work as for hs_queue_submit_group.  The bitmap has ceil(n_groups / 32) words of
+ * group bits, then ceil(n_items / 32) words of item bits.  A group with no items is 1.
+ * HS_ERR_ARG: the lane is off; n_items or n_groups is 0; bad offsets; msg_idx >= n_msgs; group_idx >= n_groups; a mode byte > 1;
+ * more items or region bytes than the lane's limits.  HS_ERR_NOMEM: no arena room right now (back-pressure). */
+int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig,
+                          const uint8_t *pk, const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *modes_or_null,
+                          size_t n_items, size_t n_groups, hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
+#define HS_QUEUE_BATCH_STATS 5
+/* Counters of completed batch passes: [0] batch passes, [1] items, [2] groups, [3] preimage bytes hashed, [4] items whose key was
+ * outside the committee (every item when no committee is registered) */
+int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

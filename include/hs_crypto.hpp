@@ -49,6 +49,11 @@ struct QueueFull : EngineError {
   QueueFull() : EngineError("hs_queue_submit: the verify queue's ring is full") {}
 };
 
+// Verdicts of a batch request (VerifyQueue::submit_batch): one per group, one per item.
+struct BatchVerdicts {
+  std::vector<bool> groups, items;
+};
+
 // RAII handle on hs_queue_* (hs_crypto.h): many tasks submit small verifies (a Vote, a Timeout / Block author, a small QC) at
 // once and share latency-path launches.  Each future yields the request's verdicts, bit-identical to hs_verify_rec128, or throws
 // EngineError on an engine failure (reject every signature).  Destruction completes every request in flight.
@@ -142,8 +147,51 @@ class VerifyQueue {
     e_.check(hs_queue_generic_stats(q_, s.data()), "hs_queue_generic_stats");
     return s;
   }
+  // hs_queue_batch: turn the batch lane on for requests of up to max_items items and max_bytes of arena region (0, 0 = off, the
+  // default).  Resizing or turning it off first waits for the batch requests already submitted.
+  void batch(size_t max_items, size_t max_bytes) { e_.check(hs_queue_batch(q_, max_items, max_bytes), "hs_queue_batch"); }
+  // hs_verify_groups with key bytes as ONE non-blocking request on the batch lane (hs_queue_submit_batch).  The future yields the
+  // group and item verdicts, bit for bit those of hs_verify_groups, or throws EngineError on an engine failure (reject every
+  // group).  Throws QueueFull when the lane's arena has no room now, EngineError on a bad argument or when the lane is off.
+  std::future<BatchVerdicts> submit_batch(const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                                          const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *modes, size_t n_items, size_t n_groups) {
+    auto *p = new BatchPending{std::promise<BatchVerdicts>(), n_items, n_groups};
+    std::future<BatchVerdicts> f = p->promise.get_future();
+    const int rc = hs_queue_submit_batch(q_, preimages, pre_off, n_msgs, sig, pk, msg_idx, group_idx, modes, n_items, n_groups, &VerifyQueue::batch_done,
+                                         p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit_batch");
+    }
+    return f;
+  }
+  // hs_queue_batch_stats: [0] batch passes, [1] items, [2] groups, [3] preimage bytes hashed, [4] items outside the committee.
+  std::array<uint64_t, HS_QUEUE_BATCH_STATS> batch_stats() const {
+    std::array<uint64_t, HS_QUEUE_BATCH_STATS> s{};
+    e_.check(hs_queue_batch_stats(q_, s.data()), "hs_queue_batch_stats");
+    return s;
+  }
 
  private:
+  struct BatchPending {
+    std::promise<BatchVerdicts> promise;
+    size_t n_items, n_groups;
+  };
+  // runs once per batch request on the queue's thread: the bitmap holds the group words, then the item words
+  static void batch_done(void *user, size_t, int status, const uint32_t *bitmap) {
+    BatchPending *p = static_cast<BatchPending *>(user);
+    if (status == HS_OK) {
+      BatchVerdicts v{std::vector<bool>(p->n_groups), std::vector<bool>(p->n_items)};
+      const uint32_t *items = bitmap + (p->n_groups + 31) / 32;
+      for (size_t j = 0; j < p->n_groups; j++) v.groups[j] = (bitmap[j >> 5] >> (j & 31)) & 1u;
+      for (size_t i = 0; i < p->n_items; i++) v.items[i] = (items[i >> 5] >> (i & 31)) & 1u;
+      p->promise.set_value(std::move(v));
+    } else {
+      p->promise.set_exception(std::make_exception_ptr(EngineError("verify queue batch: engine failure (status " + std::to_string(status) + ")")));
+    }
+    delete p;
+  }
   struct Pending {
     std::promise<std::vector<bool>> promise;
     size_t n;

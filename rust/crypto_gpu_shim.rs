@@ -37,6 +37,10 @@ pub mod sig_cache;
 /// queue kernel instead of holding up the queue's thread.  Turned on when the node-wide queue is created (`queue::queue`).
 #[path = "crypto_gpu_generic_queue.rs"]
 pub mod generic_queue;
+/// The queue's batch lane (hs_queue_submit_batch): a whole hs_verify_groups pass (a large Block, a collected view-change burst)
+/// awaited by a task instead of run under `spawn_blocking` (`batch_queue::verify_groups_queued`).
+#[path = "crypto_gpu_batch_queue.rs"]
+pub mod batch_queue;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

@@ -38,6 +38,9 @@
 // Foreign keys (alone with argv[3] = foreign_keys): single-record vote bursts with no committee registered, and bursts with one
 // request by an unregistered key (1 or 500 records) halfway through, with hs_queue_generic off and on (see run_foreign_keys).
 //
+// Batch lane (alone with argv[3] = batch_lane): a whole hs_verify_groups pass as one queue request, against hs_queue_submit_msgs and
+// the synchronous calls, for a Block alone, a Block during the vote burst and a collected view-change burst (see run_batch_lane).
+//
 // build: g++ -O2 -std=c++17 -pthread tools/replay_config5.cpp -Iinclude -Ioracle -Lhotstuff_b200 -lhs_crypto -Loracle -lhs_oracle -o tools/replay_config5
 #include <algorithm>
 #include <atomic>
@@ -1398,6 +1401,256 @@ static int run_foreign_keys(hs_ctx *ctx, int bursts) {
   return bad;
 }
 
+// ---- the batch lane (alone with argv[3] = batch_lane): a whole hs_verify_groups pass as one queue request (hs_queue_submit_batch)
+//   (a) replica_block, N = 1,000 .. 10,000: one Block (strict author over the Block preimage + N - f batch-eq QC votes over one
+//       40-byte preimage, 1 % corrupted) through hs_queue_submit_batch (one group) + hs_queue_wait, hs_queue_submit_msgs +
+//       hs_queue_wait, and the synchronous hs_verify_groups, one after another;
+//   (b) block_during_burst, N = 1,000 and 10,000: the leader's vote burst from 16 threads with that Block arriving once half the
+//       votes are in, on the lane or as hs_verify_groups from another thread; vote p50 / p99 and the Block's latency;
+//   (c) view change, N = 100 / 1,000 / 4,000: the burst's N Timeouts collected into one batch (a group per author, one group for
+//       the high_qc's votes) against Core::verify_timeouts' synchronous calls (hs_verify_tcs + one QC verify).
+// Every verdict of every arm is checked against the oracle.
+#define BL_MAX_ITEMS 32768
+#define BL_MAX_BYTES (8u << 20)
+static void bl_block(const committee_keys &k, int r, pre_cert &c) {  // make_pre_cert's Block without its TC
+  make_pre_cert(k, r, true, c);
+  const size_t n = 1 + (size_t)(k.N - (k.N - 1) / 3);
+  c.off.resize(3);
+  c.pre.resize(c.off[2]);
+  c.sig.resize(n * 64);
+  c.pk.resize(n * 32);
+  c.midx.resize(n);
+  c.modes.resize(n);
+  c.want.resize((n + 31) / 32);
+  if (n & 31) c.want.back() &= (1u << (n & 31)) - 1u;
+}
+static int bl_submit_wait(hs_queue *q, const pre_cert &c, uint32_t n_groups, const uint32_t *gidx, std::vector<uint32_t> &words) {
+  const size_t n = c.midx.size();
+  words.assign((n_groups + 31) / 32 + (n + 31) / 32, 0);
+  size_t ticket = 0;
+  int rc;
+  while ((rc = hs_queue_submit_batch(q, c.pre.data(), c.off.data(), c.off.size() - 1, c.sig.data(), c.pk.data(), c.midx.data(), gidx, c.modes.data(), n,
+                                     n_groups, nullptr, nullptr, &ticket)) == HS_ERR_NOMEM)
+    std::this_thread::yield();
+  return rc == HS_OK ? hs_queue_wait(q, ticket, words.data()) : rc;
+}
+static int bl_mismatch(const pre_cert &c, const uint32_t *item_bits) {
+  int m = 0;
+  for (size_t i = 0; i < c.midx.size(); i++) m += ((item_bits[i >> 5] >> (i & 31)) & 1u) != bit(c.want, (int)i);
+  return m;
+}
+static int bl_replica_block(hs_ctx *ctx, hs_queue *q, int N, int blocks, bool last) {
+  const committee_keys k = make_keys(N, 11);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  series lat[3];
+  int mism[3] = {0, 0, 0}, bad = 0;
+  pre_cert c;
+  for (int r = 0; r < blocks + 3; r++) {
+    const bool timed = r >= 3;
+    bl_block(k, r, c);
+    const size_t n = c.midx.size();
+    std::vector<uint32_t> zeros(n, 0), words, bits((n + 31) / 32);
+    for (int a = 0; a < 3; a++) {
+      const auto t0 = clk::now();
+      int rc;
+      const uint32_t *items = bits.data();
+      if (a == 0) {
+        rc = bl_submit_wait(q, c, 1, zeros.data(), words);
+        items = words.data() + 1;
+      } else if (a == 1) {
+        size_t ticket = 0;
+        rc = hs_queue_submit_msgs(q, c.pre.data(), c.off.data(), c.off.size() - 1, c.sig.data(), c.pk.data(), c.midx.data(), c.modes.data(), n, nullptr, nullptr,
+                                  &ticket);
+        if (rc == HS_OK) rc = hs_queue_wait(q, ticket, bits.data());
+      } else {
+        uint32_t gb = 0;
+        rc = hs_verify_groups(ctx, c.pre.data(), c.off.data(), c.off.size() - 1, c.sig.data(), c.pk.data(), nullptr, c.midx.data(), zeros.data(),
+                              c.modes.data(), n, 1, bits.data(), &gb);
+      }
+      const double t = us_since(t0);
+      bad += rc != HS_OK;
+      if (timed) {
+        lat[a].v.push_back(t);
+        mism[a] += bl_mismatch(c, items);
+      }
+    }
+  }
+  printf("\"committee_%d\": {\"records\": %zu, \"blocks\": %d, ", N, c.midx.size(), blocks);
+  const char *names[3] = {"a_submit_batch", "b_submit_msgs", "c_sync_verify_groups"};
+  for (int a = 0; a < 3; a++) printf("\"%s\": {\"p50_us\": %.1f, \"p99_us\": %.1f, \"mismatches\": %d}, ", names[a], lat[a].pct(0.5), lat[a].pct(0.99), mism[a]);
+  printf("\"errors\": %d}%s", bad, last ? "" : ", ");
+  return mism[0] + mism[1] + mism[2] + bad;
+}
+static int bl_block_during_burst(hs_ctx *ctx, int N, int bursts, bool last) {
+  const int f = (N - 1) / 3, nv = N - f, nth = 16;
+  const committee_keys k = make_keys(N, 23);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 16384, &q) != HS_OK || hs_queue_batch(q, BL_MAX_ITEMS, BL_MAX_BYTES) != HS_OK) return 1;
+  burst_arm arm[2];
+  series blk[2];
+  int blk_bad[2] = {0, 0};
+  std::vector<hs_rec128> votes(nv);
+  std::vector<int> want(nv), got(nv);
+  std::vector<double> lat(nv);
+  std::vector<burst_vote> bv(nv);
+  pre_cert c;
+  for (int r = 0; r < bursts + 3; r++) {
+    const bool timed = r >= 3;
+    bl_block(k, 1000 + r, c);  // the replica's Block (another round's certificate)
+    const size_t nb = c.midx.size();
+    std::vector<uint32_t> zeros(nb, 0);
+    uint8_t pre[40], d[32];
+    for (int j = 0; j < 32; j++) pre[j] = (uint8_t)(r * 13 + j);
+    const uint64_t round = 1000 + (uint64_t)r;
+    memcpy(pre + 32, &round, 8);
+    hso_digest32(pre, 40, d);
+    for (int i = 0; i < nv; i++) {
+      const int kk = (i * 7 + r) % N;
+      hso_sign(&k.seeds[(size_t)kk * 32], d, 32, votes[i].sig);
+      memcpy(votes[i].pk, &k.pks[(size_t)kk * 32], 32);
+      memcpy(votes[i].msg, d, 32);
+      if ((i * 37 + r * 11) % 100 == 0) votes[i].sig[(i + r) % 64] ^= 0x10;
+    }
+    std::vector<uint32_t> wb((nv + 31) / 32);
+    hso_verify_rec128_batch((const uint8_t *)votes.data(), nv, 0, ncpu(), wb.data());
+    for (int i = 0; i < nv; i++) want[i] = bit(wb, i);
+    for (int a = 0; a < 2; a++) {  // a = 0: the Block on the batch lane; a = 1: hs_verify_groups on another thread
+      std::atomic<int> go{0}, submitted{0}, bad{0}, blk_ok{0};
+      double blk_lat = 0;
+      std::vector<uint32_t> words, items((nb + 31) / 32);
+      std::vector<std::thread> ts;
+      std::fill(got.begin(), got.end(), -2);
+      clk::time_point t0;
+      for (int t = 0; t < nth; t++)
+        ts.emplace_back([&, t] {
+          while (!go.load()) {
+          }
+          for (int i = t; i < nv; i += nth) {
+            bv[i] = burst_vote{t0, &lat[i], &got[i]};
+            int rc;
+            while ((rc = hs_queue_submit(q, &votes[i], 1, HS_MODE_STRICT, on_vote, &bv[i], nullptr)) == HS_ERR_NOMEM) std::this_thread::yield();
+            if (rc != HS_OK) bad++;
+            submitted++;
+          }
+        });
+      ts.emplace_back([&] {  // the replica's connection task: its Block arrives when half the votes are in
+        while (submitted.load() < nv / 2) {
+        }
+        const auto tb = clk::now();
+        int rc;
+        if (a == 0) {
+          rc = bl_submit_wait(q, c, 1, zeros.data(), words);
+          if (rc == HS_OK) std::copy(words.begin() + 1, words.end(), items.begin());
+        } else {
+          uint32_t gb = 0;
+          rc = hs_verify_groups(ctx, c.pre.data(), c.off.data(), c.off.size() - 1, c.sig.data(), c.pk.data(), nullptr, c.midx.data(), zeros.data(),
+                                c.modes.data(), nb, 1, items.data(), &gb);
+        }
+        blk_lat = us_since(tb);
+        blk_ok = rc == HS_OK;
+      });
+      t0 = clk::now();
+      go = 1;
+      for (auto &t : ts) t.join();
+      for (int i = 0; i < nv; i++)
+        while (__atomic_load_n(&got[i], __ATOMIC_ACQUIRE) == -2) std::this_thread::yield();
+      if (timed) {
+        arm[a].total.v.push_back(*std::max_element(lat.begin(), lat.end()));
+        arm[a].vote.v.insert(arm[a].vote.v.end(), lat.begin(), lat.end());
+        for (int i = 0; i < nv; i++) arm[a].mismatches += got[i] != want[i];
+        arm[a].mismatches += bad.load();
+        blk[a].v.push_back(blk_lat);
+        blk_bad[a] += (blk_ok.load() != 1) + bl_mismatch(c, items.data());
+      }
+    }
+  }
+  printf("\"committee_%d\": {\"votes\": %d, \"block_records\": %zu, \"bursts\": %d, ", N, nv, c.midx.size(), bursts);
+  const char *names[2] = {"block_via_submit_batch", "block_via_sync_verify_groups_other_thread"};
+  for (int a = 0; a < 2; a++) {
+    printf("\"%s\": {\"block_p50_us\": %.1f, \"block_p99_us\": %.1f, \"block_mismatches\": %d, ", names[a], blk[a].pct(0.5), blk[a].pct(0.99), blk_bad[a]);
+    arm[a].emit("votes", bursts, true);
+    printf("}%s", a == 0 ? ", " : "");
+  }
+  printf("}%s", last ? "" : ", ");
+  hs_queue_destroy(q);
+  return arm[0].mismatches + arm[1].mismatches + blk_bad[0] + blk_bad[1];
+}
+// The view-change burst as one batch: group i = Timeout i's author (strict, over round || high_qc.round), group N = the high_qc's
+// votes (batch-eq, over hash || round).
+static int bl_view_change(hs_ctx *ctx, hs_queue *q, int N, int bursts, bool last) {
+  const committee_keys k = make_keys(N, 41);
+  std::vector<uint32_t> valid((N + 31) / 32);
+  if (hs_committee_register(ctx, k.pks.data(), N, valid.data()) != HS_OK) return 1;
+  series lat;
+  vc_arm sync_arm, scratch;
+  int mism = 0, bad = 0;
+  vc_burst v;
+  for (int b = 0; b < bursts + 2; b++) {
+    const bool timed = b >= 2;
+    vc_make(k, b, false, v);
+    pre_cert c;  // the collected burst in hs_verify_groups' arrays
+    c.pre.resize(56);
+    memcpy(c.pre.data(), &v.round, 8);
+    memcpy(c.pre.data() + 8, &v.hq, 8);
+    memcpy(c.pre.data() + 16, v.qc[0].pre, 40);
+    c.off = {0, 16, 56};
+    const size_t n = (size_t)N + v.nv;
+    std::vector<uint32_t> gidx(n);
+    c.sig = v.a_sig;
+    c.sig.insert(c.sig.end(), v.qc[0].sig.begin(), v.qc[0].sig.end());
+    c.pk = v.a_pk;
+    c.pk.insert(c.pk.end(), v.qc[0].pk.begin(), v.qc[0].pk.end());
+    c.midx.assign(n, 1);
+    c.modes.assign(n, HS_MODE_BATCH_EQ);
+    c.want.assign((n + 31) / 32, 0);
+    for (size_t i = 0; i < n; i++) {
+      const bool author = i < (size_t)N;
+      gidx[i] = author ? (uint32_t)i : (uint32_t)N;
+      if (author) c.midx[i] = 0, c.modes[i] = HS_MODE_STRICT;
+      if (author ? bit(v.a_want, (int)i) : bit(v.qc[0].want, (int)(i - N))) c.want[i >> 5] |= 1u << (i & 31);
+    }
+    std::vector<uint32_t> words;
+    const auto t0 = clk::now();
+    bad += bl_submit_wait(q, c, (uint32_t)N + 1, gidx.data(), words) != HS_OK;
+    const double t = us_since(t0);
+    const double ts = vc_sync_burst(ctx, v, timed ? sync_arm : scratch);
+    if (timed) {
+      lat.v.push_back(t);
+      sync_arm.t.v.push_back(ts);
+      mism += bl_mismatch(c, words.data() + (N + 1 + 31) / 32);
+    }
+  }
+  bad += scratch.mismatches + scratch.errors;
+  printf("\"committee_%d\": {\"timeouts_per_burst\": %d, \"batch_items\": %d, \"bursts\": %d, \"a_submit_batch\": {\"burst_p50_us\": %.1f, \"burst_p99_us\": %.1f, "
+         "\"mismatches\": %d}, \"b_sync_verify_tcs_plus_qc\": {\"burst_p50_us\": %.1f, \"burst_p99_us\": %.1f, \"mismatches\": %d}, \"errors\": %d}%s",
+         N, N, N + v.nv, bursts, lat.pct(0.5), lat.pct(0.99), mism, sync_arm.t.pct(0.5), sync_arm.t.pct(0.99), sync_arm.mismatches, bad + sync_arm.errors,
+         last ? "" : ", ");
+  return mism + bad + sync_arm.mismatches + sync_arm.errors;
+}
+static int run_batch_lane(hs_ctx *ctx, int reps) {
+  printf("\"batch_lane\": {\"gpu\": \"%s\", \"max_items\": %d, \"max_bytes\": %u, \"replica_block\": {\"ring_records\": 16384, ", gpu_identity().c_str(),
+         BL_MAX_ITEMS, BL_MAX_BYTES);
+  hs_queue *q = nullptr;
+  if (hs_queue_create(ctx, 16384, &q) != HS_OK || hs_queue_batch(q, BL_MAX_ITEMS, BL_MAX_BYTES) != HS_OK) return 1;
+  int bad = 0;
+  for (int N : {1000, 1500, 3000, 6000, 10000}) bad += bl_replica_block(ctx, q, N, reps, N == 10000);
+  printf("}, \"block_during_burst\": {\"threads\": 16, ");
+  bad += bl_block_during_burst(ctx, 1000, reps, false);
+  bad += bl_block_during_burst(ctx, 10000, reps, true);
+  printf("}, \"view_change\": {");
+  for (int N : {100, 1000, 4000}) bad += bl_view_change(ctx, q, N, reps, N == 4000);
+  printf("}, ");
+  uint64_t s[HS_QUEUE_BATCH_STATS] = {};
+  hs_queue_batch_stats(q, s);
+  printf("\"batch_stats\": {\"passes\": %llu, \"items\": %llu, \"groups\": %llu, \"preimage_bytes\": %llu, \"outside_committee\": %llu}}",
+         (unsigned long long)s[0], (unsigned long long)s[1], (unsigned long long)s[2], (unsigned long long)s[3], (unsigned long long)s[4]);
+  hs_queue_destroy(q);
+  return bad;
+}
+
 int main(int argc, char **argv) {
   const int rounds = argc > 1 ? atoi(argv[1]) : 1000;
   hs_ctx *ctx = nullptr;
@@ -1415,6 +1668,13 @@ int main(int argc, char **argv) {
   if (argc > 3 && strcmp(argv[3], "foreign_keys") == 0) {
     printf("{");
     const int bad = run_foreign_keys(ctx, argc > 2 ? atoi(argv[2]) : 10);
+    printf("}\n");
+    hs_ctx_destroy(ctx);
+    return bad ? 9 : 0;
+  }
+  if (argc > 3 && strcmp(argv[3], "batch_lane") == 0) {
+    printf("{");
+    const int bad = run_batch_lane(ctx, argc > 2 ? atoi(argv[2]) : 20);
     printf("}\n");
     hs_ctx_destroy(ctx);
     return bad ? 9 : 0;

@@ -32,6 +32,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <random>
 #include <string>
 #include <string_view>
@@ -1789,6 +1790,31 @@ struct queue_bits {
   }
   const uint32_t *data() const { return big.empty() ? inl : big.data(); }
 };
+// Where a request's verdicts go: its callback, or the results entry of its ticket when cb is null.  Every request kind opens and
+// closes its ticket through ticket_open_locked / ticket_close_locked.
+struct ticket_sink {
+  size_t ticket;
+  hs_queue_cb *cb;
+  void *user;
+};
+// A byte arena of cap bytes (a power of two) whose positions grow without bound like the ring's: [head, tail) is in use, and a
+// position's offset is position & (cap - 1).  A region is contiguous: one that would cross the arena's end starts at its beginning.
+struct byte_ring {
+  uint64_t cap = 0, head = 0, tail = 0;
+  // The start position of a free region of `size` <= cap bytes, or none when the arena has no room now.  Commits nothing (an empty
+  // arena may only move its start): the caller sets tail past the region once its request is accepted.
+  std::optional<uint64_t> take(uint64_t size) {
+    uint64_t start = tail;
+    if (off(start) + size > cap) start += cap - off(start);  // would cross the end: start over
+    if (start + size - head > cap) {                       // arena full
+      if (head != tail) return std::nullopt;
+      head = tail = start;  // empty: the skipped tail is free too
+    }
+    return start;
+  }
+  void release_to(uint64_t end) { head = std::max(head, end); }
+  uint64_t off(uint64_t pos) const { return pos & (cap - 1); }
+};
 // Certificate cache (hs_queue_cert_cache).  A span is the batch-eq records of one request that sign the same message, at least two
 // of them: a QC's votes.  Its key is a kind byte ('P': a preimage of hs_queue_submit_msgs, 'D': a Digest of hs_queue_submit_group),
 // the message's length and bytes, then (pk | sig) of each record in request order; lookups go through a hash of the key and match
@@ -1813,9 +1839,7 @@ enum { CERT_NEW, CERT_HIT, CERT_JOINED };
 // A request submitted with the cache on that has at least one span.  It completes when its ring part (the records that entered
 // the ring, if any) and every span it joined are done: `pending` counts them.
 struct cert_req {
-  size_t ticket;
-  hs_queue_cb *cb;
-  void *user;
+  ticket_sink sink;
   uint32_t n;
   std::vector<cert_span> spans;
   std::vector<uint32_t> ring_idx;  // the request's record of each ring record of its ring part
@@ -1842,27 +1866,23 @@ struct hs_queue {
   cudaEvent_t ev_last = nullptr;                   // recorded after every launch on `stream`: the ring is freed only after it
   cudaEvent_t ev_bulk_last = nullptr;              // the same for `bulk_stream`
   uint64_t stats[HS_QUEUE_STATS] = {};             // hs_queue_stats
-  // preimage requests (hs_queue_submit_msgs): a byte arena of HS_QUEUE_ARENA_PER_RECORD x cap bytes, positions growing without
-  // bound like the ring's ([a_head, a_tail) in use, offset = position & (acap - 1)); a request's region is contiguous (one that
-  // would cross the arena's end starts at its beginning) and is released with its ring slots
-  uint32_t acap = 0;
+  // preimage requests (hs_queue_submit_msgs): a byte arena of HS_QUEUE_ARENA_PER_RECORD x cap bytes; a request's region is
+  // released with its ring slots
+  byte_ring arena;
   uint8_t *h_arena = nullptr, *d_arena = nullptr;  // mapped pinned: the requests' regions (layout: qmsg_desc)
   uint8_t *d_stage = nullptr;                      // device: k_queue_digests' copy of the arena (same offsets)
   uint32_t *d_digs = nullptr;                      // device: digest slots, 32 bytes per 8 arena bytes
   qmsg_desc *h_mlist = nullptr, *d_mlist = nullptr;  // mapped pinned: a launch's descriptors at the ring slots of its range
-  uint64_t a_head = 0, a_tail = 0;
   uint64_t dstats[HS_QUEUE_DIGEST_STATS] = {};     // hs_queue_digest_stats
   struct req {
-    size_t ticket;
+    ticket_sink sink;
     uint32_t n;
-    hs_queue_cb *cb;
-    void *user;
     uint32_t seq;   // launch that verifies it (0: slow path)
     bool finished;
     bool msgs;           // a preimage request: its records' Digests are computed by k_queue_digests
     uint32_t a_off, m, pre_bytes;  // its arena region: offset, preimages, preimage bytes
     uint64_t a_end;      // arena position past its region (0: none)
-    cert_req *cr = nullptr;  // the ring part of a certificate-cache request: its verdicts go there (ticket and cb unused)
+    cert_req *cr = nullptr;  // the ring part of a certificate-cache request: its verdicts go there (sink unused)
     bool gen = false;        // set at dispatch: verified by k_queue_generic (hs_queue_generic on, a key outside the committee)
   };
   std::vector<req> reqs;  // by request slot
@@ -1891,14 +1911,11 @@ struct hs_queue {
   qmsg_desc *h_gmlist = nullptr, *d_gmlist = nullptr;  // mapped pinned: its preimage requests' descriptors, from position lo on
   uint64_t gstats[HS_QUEUE_GENERIC_STATS] = {};      // hs_queue_generic_stats
   // batch lane (hs_queue_batch): off while b_max_items is 0.  Requests wait in bq in submit order, each with a region of the mapped
-  // arena h_barena (b_acap bytes, positions growing without bound like the preimage arena's: [b_head, b_tail) in use); a region is
-  // filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at a time (b_cur, dispatcher thread),
-  // and regions are released in request order when their requests complete.  The lane's buffers and streams change only while the
-  // lane is off and bq is empty.
+  // arena h_barena (b_arena); a region is filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at
+  // a time (b_cur, dispatcher thread), and regions are released in request order when their requests complete.  The lane's buffers
+  // and streams change only while the lane is off and bq is empty.
   struct breq {
-    size_t ticket;
-    hs_queue_cb *cb;
-    void *user;
+    ticket_sink sink;
     uint32_t n, n_groups, n_msgs;
     uint64_t pre_bytes;
     uint64_t a_off, a_end;  // region offset in the arena; arena position past it
@@ -1907,7 +1924,7 @@ struct hs_queue {
     bool ready;
   };
   size_t b_max_items = 0, b_max_bytes = 0;
-  uint64_t b_acap = 0, b_head = 0, b_tail = 0;
+  byte_ring b_arena;
   uint8_t *h_barena = nullptr, *d_barena = nullptr;  // mapped pinned: request regions (inputs, then result words and the tail)
   uint8_t *d_bmirror = nullptr;                     // device: the inputs of the region in flight, at the same offsets
   uint32_t *d_bdig = nullptr;                       // device: the request's Digests, 32 bytes per preimage
@@ -1953,6 +1970,28 @@ struct queue_completion {
   int status;
   queue_bits bits;
 };
+// Issues ticket s.ticket, which is q->next_ticket, to a request just accepted (under q->mu): a polled ticket parks its results
+// entry of n_bits verdict bits.  A callback ticket never touches `results`.
+static void ticket_open_locked(hs_queue *q, const ticket_sink &s, uint32_t n_bits) {
+  q->next_ticket++;
+  if (!s.cb) q->results[s.ticket] = hs_queue::result{false, HS_OK, n_bits, {}};
+}
+// Completes ticket s (under q->mu) with n_bits verdict bits, all zero unless status is HS_OK (a failed request rejects every
+// record): its callback is returned in `fire`, to run after the lock is released, or its parked result is filled.
+static void ticket_close_locked(hs_queue *q, const ticket_sink &s, int status, uint32_t n_bits, const uint32_t *bits,
+                                std::vector<queue_completion> &fire) {
+  if (status != HS_OK) bits = nullptr;
+  if (s.cb) {
+    fire.push_back(queue_completion{s.cb, s.user, s.ticket, status, {}});
+    fire.back().bits.set(n_bits, bits);
+  } else {
+    hs_queue::result &res = q->results[s.ticket];
+    res.done = true;
+    res.status = status;
+    res.bits.set(n_bits, bits);
+    q->cv_done.notify_all();
+  }
+}
 // Releases the ring space of the finished requests at the head — but never inside the range of a launch still in flight: its
 // blocks may still read those records (slow-path requests between two device requests ride along in the launch).  The limit is
 // the lowest range start of ALL launches in flight: a generic launch's range holds requests of other launches, and its slot list
@@ -1965,21 +2004,12 @@ static void queue_release_locked(hs_queue *q) {
     hs_queue::req &h = q->reqs[q->head & q->mask];
     h.finished = false;
     q->head += h.n;
-    q->a_head = std::max(q->a_head, h.a_end);
+    q->arena.release_to(h.a_end);
   }
 }
-// Completes a certificate-cache request whose parts are all done (under q->mu), exactly as queue_finish_locked completes a request.
+// Completes a certificate-cache request whose parts are all done (under q->mu).
 static void cert_complete_locked(hs_queue *q, cert_req *cr, std::vector<queue_completion> &fire) {
-  if (cr->cb) {
-    fire.push_back(queue_completion{cr->cb, cr->user, cr->ticket, cr->status, {}});
-    fire.back().bits.set(cr->n, cr->status == HS_OK ? cr->bits.data() : nullptr);
-  } else {
-    hs_queue::result &res = q->results[cr->ticket];
-    res.done = true;
-    res.status = cr->status;
-    res.bits.set(cr->n, cr->status == HS_OK ? cr->bits.data() : nullptr);
-    q->cv_done.notify_all();
-  }
+  ticket_close_locked(q, cr->sink, cr->status, cr->n, cr->bits.data(), fire);
   delete cr;
 }
 static void cert_evict_locked(hs_queue *q, size_t limit) {  // least recently used first out, until at most `limit` bytes are held
@@ -2024,23 +2054,15 @@ static void cert_part_done_locked(hs_queue *q, cert_req *cr, int status, const u
   if (--cr->pending == 0) cert_complete_locked(q, cr, fire);
 }
 
-// Marks the request at ring position p finished (under q->mu): a polled ticket's result is parked, a callback is returned to be
-// fired after the lock is released.
+// Marks the request at ring position p finished (under q->mu) and completes its ticket, or its certificate-cache request's ring part.
 static void queue_finish_locked(hs_queue *q, uint64_t p, int status, const uint32_t *bits, std::vector<queue_completion> &fire) {
   hs_queue::req &r = q->reqs[p & q->mask];
   r.finished = true;
   if (r.cr) {
     cert_part_done_locked(q, r.cr, status, status == HS_OK ? bits : nullptr, fire);
     r.cr = nullptr;
-  } else if (r.cb) {
-    fire.push_back(queue_completion{r.cb, r.user, r.ticket, status, {}});
-    fire.back().bits.set(r.n, status == HS_OK ? bits : nullptr);
   } else {
-    hs_queue::result &res = q->results[r.ticket];
-    res.done = true;
-    res.status = status;
-    res.bits.set(r.n, status == HS_OK ? bits : nullptr);
-    q->cv_done.notify_all();
+    ticket_close_locked(q, r.sink, status, r.n, bits, fire);
   }
   queue_release_locked(q);
 }
@@ -2384,7 +2406,8 @@ static batch_layout batch_layout_of(uint64_t n_msgs, uint64_t pre_bytes, uint64_
   b.size = b.o_tail + 16;
   return b;
 }
-static uint64_t batch_words(const hs_queue::breq &r) { return (r.n_groups + 31) / 32 + (r.n + 31) / 32; }
+// A batch ticket's verdict bits: whole words, the group words then the item words.
+static uint32_t batch_bits(uint64_t n_groups, uint64_t n) { return (uint32_t)(32 * ((n_groups + 31) / 32 + (n + 31) / 32)); }
 
 // Completes the request in flight (dispatcher thread): its result words go to its callback or ticket, then its region is released.
 static void batch_complete(hs_queue *q, int status) {
@@ -2392,8 +2415,6 @@ static void batch_complete(hs_queue *q, int status) {
   {
     std::lock_guard<std::mutex> g(q->mu);
     const hs_queue::breq &r = *q->b_cur;
-    const uint32_t bits = (uint32_t)(32 * batch_words(r));
-    const uint32_t *res = status == HS_OK ? reinterpret_cast<const uint32_t *>(q->h_barena + r.a_off + r.o_res) : nullptr;
     if (status == HS_OK) {
       q->bstats[0]++;
       q->bstats[1] += r.n;
@@ -2401,19 +2422,11 @@ static void batch_complete(hs_queue *q, int status) {
       q->bstats[3] += r.pre_bytes;
       q->bstats[4] += reinterpret_cast<const volatile uint32_t *>(q->h_barena + r.a_off + r.o_tail)[0];
     }
-    if (r.cb) {
-      fire.push_back(queue_completion{r.cb, r.user, r.ticket, status, {}});
-      fire.back().bits.set(bits, res);
-    } else {
-      hs_queue::result &out = q->results[r.ticket];
-      out.done = true;
-      out.status = status;
-      out.bits.set(bits, res);
-    }
-    q->b_head = r.a_end;
+    ticket_close_locked(q, r.sink, status, batch_bits(r.n_groups, r.n), reinterpret_cast<const uint32_t *>(q->h_barena + r.a_off + r.o_res), fire);
+    q->b_arena.release_to(r.a_end);
     q->b_cur = nullptr;
     q->bq.pop_front();
-    q->cv_done.notify_all();
+    q->cv_done.notify_all();  // for callback tickets too: hs_queue_batch waits for bq to drain
   }
   queue_fire(fire);
 }
@@ -2497,7 +2510,7 @@ static void batch_free(hs_queue *q) {
   q->d_bxyz = nullptr;
   q->d_bmeta = q->d_bflags = nullptr;
   q->d_bvidx = q->d_bmiss = q->d_bmiss_count = q->d_bitems = q->d_bgrej = q->d_bcounter = nullptr;
-  q->b_acap = 0;
+  q->b_arena = byte_ring{};
 }
 
 static size_t queue_small_inflight_locked(const hs_queue *q) {
@@ -3523,7 +3536,7 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   q->c = c;
   q->cap = cap;
   q->mask = cap - 1;
-  q->acap = cap * HS_QUEUE_ARENA_PER_RECORD;
+  q->arena.cap = cap * HS_QUEUE_ARENA_PER_RECORD;
   q->modes.assign(cap, 0);
   q->wbits.assign(cap / 32, 0);
   q->reqs.assign(cap, hs_queue::req{});
@@ -3538,11 +3551,11 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_done, (size_t)cap * 4, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaMalloc(&q->d_counters, (size_t)cap * 4);
   if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_arena, q->acap, cudaHostAllocMapped);
+  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_arena, q->arena.cap, cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->h_mlist, (size_t)cap * sizeof(qmsg_desc), cudaHostAllocMapped);
   if (e == cudaSuccess) e = cudaHostAlloc(&q->pk, (size_t)cap * 32, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_stage, q->acap);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_digs, (size_t)q->acap * 4);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_stage, q->arena.cap);
+  if (e == cudaSuccess) e = cudaMalloc(&q->d_digs, q->arena.cap * 4);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_ring, q->h_ring, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_flags, q->h_flags, 0);
   if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_done, q->h_done, 0);
@@ -3613,15 +3626,11 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
       pre_bytes += pre_off[j + 1] - pre_off[j];
     }
   const uint64_t size = qmsg_bytes(m, n, pre_bytes);
-  if (size > q->acap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more preimage bytes than the queue's arena holds");
-  uint64_t start = q->a_tail;
-  if ((start & (q->acap - 1)) + size > q->acap) start += q->acap - (start & (q->acap - 1));  // would cross the end: start over
-  if (start + size - q->a_head > q->acap) {  // arena full
-    if (q->a_head != q->a_tail) return HS_ERR_NOMEM;
-    start = q->a_head = q->a_tail = start;  // empty: the skipped tail is free too
-  }
+  if (size > q->arena.cap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: more preimage bytes than the queue's arena holds");
+  const std::optional<uint64_t> start = q->arena.take(size);
+  if (!start) return HS_ERR_NOMEM;
   if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
-  uint8_t *a = q->h_arena + (start & (q->acap - 1));
+  uint8_t *a = q->h_arena + q->arena.off(*start);
   uint64_t *off = reinterpret_cast<uint64_t *>(a);
   uint32_t *idx = reinterpret_cast<uint32_t *>(a + 8 * ((size_t)m + 1));
   uint8_t *pre = a + qmsg_o_pre(m, n);
@@ -3643,13 +3652,12 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
   }
   r.n = (uint32_t)n;
   r.msgs = true;
-  r.a_off = (uint32_t)(start & (q->acap - 1));
+  r.a_off = (uint32_t)q->arena.off(*start);
   r.m = m;
   r.pre_bytes = (uint32_t)pre_bytes;
-  r.a_end = start + size;
+  r.a_end = q->arena.tail = *start + size;
   q->reqs[q->tail & q->mask] = r;
   q->tail += n;
-  q->a_tail = start + size;
   q->dstats[3]++;
   return HS_OK;
 }
@@ -3671,7 +3679,7 @@ static std::unique_ptr<cert_req> cert_spans(char kind, size_t n, const uint8_t *
   std::unique_ptr<cert_req> cr;
   for (std::vector<uint32_t> &g : groups) {
     if (g.size() < 2) continue;
-    if (!cr) cr.reset(new cert_req{0, cb, user, (uint32_t)n, {}, {}, 0, HS_OK, std::vector<uint32_t>((n + 31) / 32, 0u)});
+    if (!cr) cr.reset(new cert_req{{0, cb, user}, (uint32_t)n, {}, {}, 0, HS_OK, std::vector<uint32_t>((n + 31) / 32, 0u)});
     const std::string_view m = msg(g[0]);
     const uint64_t len = m.size();
     std::string key;
@@ -3689,6 +3697,23 @@ static std::unique_ptr<cert_req> cert_spans(char kind, size_t n, const uint8_t *
   return cr;
 }
 
+// Submits one request of any kind: under q->mu, put(s) takes the request's room and records it with sink s (s.ticket is the ticket
+// it gets), returning HS_OK, or an error that leaves the queue as it was.  The ticket is issued only when put accepted the request.
+template <class Put>
+static int queue_submit(hs_queue *q, const char *what, ticket_sink s, uint32_t n_bits, size_t *out_ticket, Put put) {
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
+    s.ticket = q->next_ticket;
+    const int rc = put(s);
+    if (rc != HS_OK) return rc;
+    ticket_open_locked(q, s, n_bits);
+    if (out_ticket) *out_ticket = s.ticket;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+
 // Submits a request that has spans, with the cache on.  Under q->mu each span is a hit, a join of an identical span pending or in
 // flight in an earlier request, or new; `put(sel, r)` enters the records of no hit or joined span into the ring as request r.  When
 // there are none the request is answered entirely here and the queue's thread completes it.  Nothing changes on an error.
@@ -3697,9 +3722,7 @@ static int cert_submit(hs_queue *q, const char *what, std::unique_ptr<cert_req> 
   std::vector<int32_t> span_of(cr->n, -1);
   for (size_t j = 0; j < cr->spans.size(); j++)
     for (uint32_t i : cr->spans[j].idx) span_of[i] = (int32_t)j;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
+  return queue_submit(q, what, cr->sink, cr->n, out_ticket, [&](const ticket_sink &s) {
     for (cert_span &sp : cr->spans) {
       const cert_key k{sp.h, sp.key};
       sp.role = q->cc_map.count(k) ? CERT_HIT : q->cc_flights.count(k) ? CERT_JOINED : CERT_NEW;
@@ -3715,8 +3738,7 @@ static int cert_submit(hs_queue *q, const char *what, std::unique_ptr<cert_req> 
       cr->pending++;
     }
     cr->ring_idx = std::move(sel);
-    cr->ticket = q->next_ticket++;
-    if (!cr->cb) q->results[cr->ticket] = hs_queue::result{false, HS_OK, cr->n, {}};
+    cr->sink = s;
     q->cstats[0] += cr->spans.size();
     for (cert_span &sp : cr->spans) {
       const cert_key k{sp.h, sp.key};
@@ -3735,34 +3757,28 @@ static int cert_submit(hs_queue *q, const char *what, std::unique_ptr<cert_req> 
       }
       q->cstats[3] += sp.idx.size();
     }
-    if (out_ticket) *out_ticket = cr->ticket;
     if (cr->pending == 0) q->cc_ready.push_back(cr.get());
     cr.release();  // owned by the queue until it completes
-  }
-  q->cv_work.notify_one();
+    return HS_OK;
+  });
+}
+
+// Reads one of the queue's counter arrays for an hs_queue_*stats entry point.
+template <size_t N>
+static int queue_read_stats(hs_queue *q, const char *what, uint64_t *out, uint64_t (hs_queue::*arr)[N]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, (std::string(what) + ": bad argument").c_str());
+  std::lock_guard<std::mutex> g(q->mu);
+  q->cstats[5] = q->cc_bytes;  // hs_queue_cert_stats' [5]: the key bytes held now
+  memcpy(out, q->*arr, sizeof(q->*arr));
   return HS_OK;
 }
 }  // extern "C++"
 
-// Copies one request into the ring (arguments already checked): record i is judged by modes[i], or by `mode` when modes is null.
-static int queue_enqueue(hs_queue *q, const char *what, const hs_rec128 *recs, size_t n, uint32_t mode, const uint8_t *modes, hs_queue_cb *cb,
-                         void *user, size_t *out_ticket) {
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    if (q->stop) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": queue is being destroyed").c_str());
-    const int rc = queue_put_recs_locked(q, what, recs, queue_sel{nullptr, n}, mode, modes, hs_queue::req{q->next_ticket, 0, cb, user, 0, false});
-    if (rc != HS_OK) return rc;
-    const size_t ticket = q->next_ticket++;
-    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
-    if (out_ticket) *out_ticket = ticket;
-  }
-  q->cv_work.notify_one();
-  return HS_OK;
-}
-
 int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb, void *user, size_t *out_ticket) {
   if (!q || !recs || n == 0 || n > HS_SMALL_MAX || mode > 1) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit: bad argument");
-  return queue_enqueue(q, "hs_queue_submit", recs, n, mode, nullptr, cb, user, out_ticket);
+  return queue_submit(q, "hs_queue_submit", ticket_sink{0, cb, user}, (uint32_t)n, out_ticket, [&](const ticket_sink &s) {
+    return queue_put_recs_locked(q, "hs_queue_submit", recs, queue_sel{nullptr, n}, mode, nullptr, hs_queue::req{s});
+  });
 }
 
 // With the certificate cache on, the ring capacity limits the records that enter the ring (checked under the lock), not n.
@@ -3778,13 +3794,13 @@ int hs_queue_submit_group(hs_queue *q, const hs_rec128 *recs, size_t n, const ui
   if (cache)
     cr = cert_spans('D', n, modes, cb, user, [&](size_t i) { return std::string_view(reinterpret_cast<const char *>(recs[i].msg), 32); },
                     [&](size_t i) { return recs[i].pk; }, [&](size_t i) { return recs[i].sig; });
-  if (!cr) {
-    if (n > q->cap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
-    return queue_enqueue(q, "hs_queue_submit_group", recs, n, HS_MODE_STRICT, modes, cb, user, out_ticket);
-  }
-  return cert_submit(q, "hs_queue_submit_group", std::move(cr), out_ticket, [&](queue_sel sel, const hs_queue::req &r) {
+  const auto put = [&](queue_sel sel, const hs_queue::req &r) {
     return queue_put_recs_locked(q, "hs_queue_submit_group", recs, sel, HS_MODE_STRICT, modes, r);
-  });
+  };
+  if (cr) return cert_submit(q, "hs_queue_submit_group", std::move(cr), out_ticket, put);
+  if (n > q->cap) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_group: bad argument");
+  return queue_submit(q, "hs_queue_submit_group", ticket_sink{0, cb, user}, (uint32_t)n, out_ticket,
+                      [&](const ticket_sink &s) { return put(queue_sel{nullptr, n}, hs_queue::req{s}); });
 }
 
 int hs_queue_submit_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
@@ -3807,17 +3823,8 @@ int hs_queue_submit_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *
     return queue_put_msgs_locked(q, preimages, pre_off, n_msgs, sig, pk, msg_idx, modes, sel, r);
   };
   if (cr) return cert_submit(q, "hs_queue_submit_msgs", std::move(cr), out_ticket, put);
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_msgs: queue is being destroyed");
-    const int rc = put(queue_sel{nullptr, n}, hs_queue::req{q->next_ticket, 0, cb, user, 0, false});
-    if (rc != HS_OK) return rc;
-    const size_t ticket = q->next_ticket++;
-    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)n, {}};
-    if (out_ticket) *out_ticket = ticket;
-  }
-  q->cv_work.notify_one();
-  return HS_OK;
+  return queue_submit(q, "hs_queue_submit_msgs", ticket_sink{0, cb, user}, (uint32_t)n, out_ticket,
+                      [&](const ticket_sink &s) { return put(queue_sel{nullptr, n}, hs_queue::req{s}); });
 }
 
 int hs_queue_poll(hs_queue *q, size_t ticket, int *done, uint32_t *out_bitmap) {
@@ -3849,18 +3856,10 @@ int hs_queue_wait(hs_queue *q, size_t ticket, uint32_t *out_bitmap) {
   }
 }
 
-int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  memcpy(out, q->stats, sizeof(q->stats));
-  return HS_OK;
-}
+int hs_queue_stats(hs_queue *q, uint64_t out[HS_QUEUE_STATS]) { return queue_read_stats(q, "hs_queue_stats", out, &hs_queue::stats); }
 
 int hs_queue_digest_stats(hs_queue *q, uint64_t out[HS_QUEUE_DIGEST_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_digest_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  memcpy(out, q->dstats, sizeof(q->dstats));
-  return HS_OK;
+  return queue_read_stats(q, "hs_queue_digest_stats", out, &hs_queue::dstats);
 }
 
 int hs_queue_cert_cache(hs_queue *q, size_t max_bytes) {
@@ -3872,11 +3871,7 @@ int hs_queue_cert_cache(hs_queue *q, size_t max_bytes) {
 }
 
 int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_cert_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  q->cstats[5] = q->cc_bytes;
-  memcpy(out, q->cstats, sizeof(q->cstats));
-  return HS_OK;
+  return queue_read_stats(q, "hs_queue_cert_stats", out, &hs_queue::cstats);
 }
 
 #define HS_QUEUE_SIG_MAX_ENTRIES (1ull << 26)  // 9.7 GB of table
@@ -3935,10 +3930,7 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries) {
 }
 
 int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  memcpy(out, q->sstats, sizeof(q->sstats));
-  return HS_OK;
+  return queue_read_stats(q, "hs_queue_sig_stats", out, &hs_queue::sstats);
 }
 
 int hs_queue_generic(hs_queue *q, int on) {
@@ -3966,10 +3958,7 @@ int hs_queue_generic(hs_queue *q, int on) {
 }
 
 int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_generic_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  memcpy(out, q->gstats, sizeof(q->gstats));
-  return HS_OK;
+  return queue_read_stats(q, "hs_queue_generic_stats", out, &hs_queue::gstats);
 }
 
 #define HS_QUEUE_BATCH_MAX_ITEMS (1u << 24)
@@ -4017,8 +4006,7 @@ int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
   }
   memset(q->h_barena, 0, acap);
   std::lock_guard<std::mutex> g(q->mu);
-  q->b_acap = acap;
-  q->b_head = q->b_tail = 0;
+  q->b_arena = byte_ring{acap, 0, 0};
   q->b_max_items = max_items;
   q->b_max_bytes = max_bytes;
   return HS_OK;
@@ -4036,26 +4024,19 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
       return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: index or mode out of range");
   const uint64_t pre_bytes = pre_off[n_msgs];
   const batch_layout B = batch_layout_of(n_msgs, pre_bytes, n_items, n_groups);
-  hs_queue::breq *r;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    if (q->stop) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: queue is being destroyed");
+  hs_queue::breq *r = nullptr;
+  const int rc = queue_submit(q, "hs_queue_submit_batch", ticket_sink{0, cb, user}, batch_bits(n_groups, n_items), out_ticket, [&](const ticket_sink &s) {
     if (!q->b_max_items) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: the batch lane is off (hs_queue_batch)");
     if (n_items > q->b_max_items || B.size > q->b_max_bytes) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: larger than the batch lane's limits");
-    uint64_t start = q->b_tail;
-    if ((start & (q->b_acap - 1)) + B.size > q->b_acap) start += q->b_acap - (start & (q->b_acap - 1));  // would cross the end: start over
-    if (start + B.size - q->b_head > q->b_acap) {  // arena full
-      if (q->b_head != q->b_tail) return HS_ERR_NOMEM;
-      start = q->b_head = q->b_tail = start;  // empty: the skipped tail is free too
-    }
-    q->b_tail = start + B.size;
-    const size_t ticket = q->next_ticket++;
-    q->bq.push_back(hs_queue::breq{ticket, cb, user, (uint32_t)n_items, (uint32_t)n_groups, (uint32_t)n_msgs, pre_bytes, start & (q->b_acap - 1),
-                                   start + B.size, B.o_pre, B.o_sig, B.o_pk, B.o_mi, B.o_gi, B.o_mo, B.o_res, B.o_tail, 0, false});
+    const std::optional<uint64_t> start = q->b_arena.take(B.size);
+    if (!start) return HS_ERR_NOMEM;
+    q->b_arena.tail = *start + B.size;
+    q->bq.push_back(hs_queue::breq{s, (uint32_t)n_items, (uint32_t)n_groups, (uint32_t)n_msgs, pre_bytes, q->b_arena.off(*start), q->b_arena.tail,
+                                   B.o_pre, B.o_sig, B.o_pk, B.o_mi, B.o_gi, B.o_mo, B.o_res, B.o_tail, 0, false});
     r = &q->bq.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
-    if (!cb) q->results[ticket] = hs_queue::result{false, HS_OK, (uint32_t)(32 * batch_words(*r)), {}};
-    if (out_ticket) *out_ticket = ticket;
-  }
+    return HS_OK;
+  });
+  if (rc != HS_OK) return rc;
   // the region is this request's alone until it completes: fill it without holding q->mu
   uint8_t *a = q->h_barena + r->a_off;
   memcpy(a, pre_off, 8 * (n_msgs + 1));
@@ -4076,10 +4057,7 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
 }
 
 int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]) {
-  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_batch_stats: bad argument");
-  std::lock_guard<std::mutex> g(q->mu);
-  memcpy(out, q->bstats, sizeof(q->bstats));
-  return HS_OK;
+  return queue_read_stats(q, "hs_queue_batch_stats", out, &hs_queue::bstats);
 }
 
 void hs_queue_destroy(hs_queue *q) {

@@ -72,35 +72,49 @@ __device__ __forceinline__ void load32(uint32_t (&w)[8], const uint8_t *p) {
 #pragma unroll
   for (int i = 0; i < 8; i++) w[i] = __ldg(s + i);
 }
+// 32 bytes held as two 16-byte vectors -> 8 words
+__device__ __forceinline__ void unpack8(uint32_t (&w)[8], uint4 lo, uint4 hi) {
+  w[0] = lo.x; w[1] = lo.y; w[2] = lo.z; w[3] = lo.w;
+  w[4] = hi.x; w[5] = hi.y; w[6] = hi.z; w[7] = hi.w;
+}
+// A 32-byte Digest (the first 8 words of a SHA-512 output) as two 16-byte stores; dst is 16-byte aligned.
+__device__ __forceinline__ void store_digest32(uint32_t *dst, const uint32_t *h) {
+  uint4 *d = reinterpret_cast<uint4 *>(dst);
+  d[0] = make_uint4(h[0], h[1], h[2], h[3]);
+  d[1] = make_uint4(h[4], h[5], h[6], h[7]);
+}
 
-// A warp loads 32 rows of 128 bytes (row r at base + (warp_first + r) * stride, 16-byte aligned) with fully coalesced
-// 16-byte accesses, parks them in shared memory under an XOR swizzle, and every lane then reads back its own row
-// conflict-free.  Rows past n read as zeros.  Every lane of the warp must call it.
-__device__ __forceinline__ void warp_stage_rows128(uint4 (&q)[8], const uint8_t *__restrict__ base, size_t stride, size_t n, size_t warp_first,
-                                                   uint4 *smem_warp) {
-  const int lane = threadIdx.x & 31;
+// A warp loads 32 rows of 128 bytes (rows warp_first .. warp_first + 31 of n; row(r) is the 16-byte aligned address of row
+// warp_first + r) with fully coalesced 16-byte accesses, parks them in shared memory under an XOR swizzle, and every lane then
+// reads back its own row conflict-free.  Rows past n read as zeros.  Every lane of the warp must call it, with lane = threadIdx.x
+// & 31.  row() runs on every lane for every r, in range or not, so it may hold a full-warp shuffle.  The caller synchronises (warp
+// or block) before smem_warp is written again.
+template <class I, class Row>
+__device__ __forceinline__ void warp_stage_rows128(uint4 (&q)[8], I n, I warp_first, Row row, uint4 *smem_warp, int lane) {
 #pragma unroll
   for (int j = 0; j < 8; j++) {
-    int c = j * 32 + lane;  // chunk index inside the warp's 4 KB
-    int rec = c >> 3, part = c & 7;
+    const int c = j * 32 + lane;  // chunk index inside the warp's 4 KB
+    const int rec = c >> 3, part = c & 7;
+    const uint4 *src = row(rec);  // outside the branch below: a shuffle there would diverge
     uint4 v = make_uint4(0, 0, 0, 0);
-    if (warp_first + rec < n) v = __ldg(reinterpret_cast<const uint4 *>(base + (warp_first + rec) * stride) + part);
+    if (warp_first + rec < n) v = __ldg(src + part);
     smem_warp[rec * 8 + (part ^ (rec & 7))] = v;
   }
   __syncwarp();
 #pragma unroll
   for (int part = 0; part < 8; part++) q[part] = smem_warp[lane * 8 + (part ^ (lane & 7))];
-  __syncwarp();
 }
 // packed hs_rec128 records: sig.R | sig.S | pk | msg
 __device__ __forceinline__ void warp_load_rec128(uint32_t (&sig_r)[8], uint32_t (&sig_s)[8], uint32_t (&pk)[8], uint32_t (&msg)[8],
-                                                 const uint4 *__restrict__ recs, size_t n, size_t warp_first, uint4 *smem_warp) {
+                                                 const uint8_t *__restrict__ recs, size_t n, size_t warp_first, uint4 *smem_warp) {
   uint4 q[8];
-  warp_stage_rows128(q, reinterpret_cast<const uint8_t *>(recs), 128, n, warp_first, smem_warp);
-  sig_r[0] = q[0].x; sig_r[1] = q[0].y; sig_r[2] = q[0].z; sig_r[3] = q[0].w; sig_r[4] = q[1].x; sig_r[5] = q[1].y; sig_r[6] = q[1].z; sig_r[7] = q[1].w;
-  sig_s[0] = q[2].x; sig_s[1] = q[2].y; sig_s[2] = q[2].z; sig_s[3] = q[2].w; sig_s[4] = q[3].x; sig_s[5] = q[3].y; sig_s[6] = q[3].z; sig_s[7] = q[3].w;
-  pk[0] = q[4].x; pk[1] = q[4].y; pk[2] = q[4].z; pk[3] = q[4].w; pk[4] = q[5].x; pk[5] = q[5].y; pk[6] = q[5].z; pk[7] = q[5].w;
-  msg[0] = q[6].x; msg[1] = q[6].y; msg[2] = q[6].z; msg[3] = q[6].w; msg[4] = q[7].x; msg[5] = q[7].y; msg[6] = q[7].z; msg[7] = q[7].w;
+  warp_stage_rows128(q, n, warp_first, [&](int r) { return reinterpret_cast<const uint4 *>(recs + (warp_first + r) * 128); }, smem_warp,
+                     threadIdx.x & 31);
+  __syncwarp();  // k_verify_main takes a block barrier next anyway; without this one its code schedules differently
+  unpack8(sig_r, q[0], q[1]);
+  unpack8(sig_s, q[2], q[3]);
+  unpack8(pk, q[4], q[5]);
+  unpack8(msg, q[6], q[7]);
 }
 
 // ------------------------------------------------------------------------------------------------ committee key lookup
@@ -210,7 +224,7 @@ __global__ void __launch_bounds__(HS_THREADS, COMMITTEE ? HS_MAIN_MINBLOCKS : HS
   if (L.aos128 && !index_list) {
     uint32_t M[8];
     __syncthreads();  // the previous grid-stride iteration's digits live in the same shared bytes
-    warp_load_rec128(R, S, A, M, reinterpret_cast<const uint4 *>(L.sig), n, warp_first, stage[threadIdx.x >> 5]);
+    warp_load_rec128(R, S, A, M, L.sig, n, warp_first, stage[threadIdx.x >> 5]);
     __syncthreads();
     if (COMMITTEE) {
       v = __ldg(L.vidx + i);
@@ -463,6 +477,23 @@ __device__ __forceinline__ uint32_t *sig_smem() {
   return s;
 }
 
+// Completion step of the queue kernels: k of request slot `req`'s req_n records are done.  Before this add the caller has stored
+// those records' flags and fenced them to system scope, and (cache on) added its counts with sig_count, so the add that completes
+// the request comes after every record's flags and counts.  That add publishes the cache counts (SIGC), resets the slot's counter
+// for its next request, fences to system scope and only then sets the request's completion word to seq.  The queue's watcher
+// thread takes that word as its only signal: on seeing it, it reads the request's flags and counts from mapped memory and may hand
+// the slot to a new request at once.  req_n is a reference so that a field of the mapped ring is read after the add.
+template <bool SIGC>
+__device__ __forceinline__ void queue_complete(uint32_t *counters, volatile uint32_t *done, uint32_t seq, uint32_t req, const uint32_t &req_n,
+                                               uint32_t k, const sig_cache_dev &sc) {
+  if (atomicAdd(counters + req, k) == req_n - k) {
+    if constexpr (SIGC) sig_publish(sc, req);
+    counters[req] = 0;
+    __threadfence_system();
+    done[req] = seq;
+  }
+}
+
 // SIGC: probe and fill the signature cache.  The cache-off instantiation is the kernel without it, instruction for instruction.
 template <bool SIGC>
 __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict__ ring, uint32_t base, uint32_t mask, const ge_niels *__restrict__ btable,
@@ -508,12 +539,7 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
         const uint32_t req = rec->req;
         sig_count(sc, req, 1, 1, 0, 0);
         __threadfence_system();
-        if (atomicAdd(counters + req, 1u) == rec->req_n - 1) {
-          sig_publish(sc, req);
-          counters[req] = 0;
-          __threadfence_system();
-          done[req] = seq;
-        }
+        queue_complete<SIGC>(counters, done, seq, req, rec->req_n, 1u, sc);
       }
       return;
     }
@@ -582,13 +608,40 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
       sig_count(sc, rec->req, have_key ? 1u : 0u, 0, ins != 0, ins == 2);
     }
     __threadfence_system();
-    const uint32_t req = rec->req;
-    if (atomicAdd(counters + req, 1u) == rec->req_n - 1) {
-      if constexpr (SIGC) sig_publish(sc, req);
-      counters[req] = 0;
-      __threadfence_system();
-      done[req] = seq;
-    }
+    queue_complete<SIGC>(counters, done, seq, rec->req, rec->req_n, 1u, sc);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ block-wide inversion
+// Montgomery's trick over a block of 128 threads: tot[t] becomes 1 / tot[t].  Lane l of warp 0 multiplies tot[4l .. 4l+3], inverts
+// that product once and back-substitutes.  Every tot[t] must be nonzero.  The caller takes a barrier before (tot stored) and after
+// (tot read back).
+__device__ __forceinline__ void block_invert4(fe (&tot)[128]) {
+  if (threadIdx.x < 32) {
+    const int b = threadIdx.x * 4;
+    fe q0 = tot[b], q1, q2, q3, inv, u;
+    fe_mul(q1, q0, tot[b + 1]);
+    fe_mul(q2, q1, tot[b + 2]);
+    fe_mul(q3, q2, tot[b + 3]);
+    fe_invert(inv, q3);
+    fe_mul(u, inv, q2);        // 1 / tot[b+3]
+    fe_mul(inv, inv, tot[b + 3]);
+    tot[b + 3] = u;
+    fe_mul(u, inv, q1);        // 1 / tot[b+2]
+    fe_mul(inv, inv, tot[b + 2]);
+    tot[b + 2] = u;
+    fe_mul(u, inv, q0);        // 1 / tot[b+1]
+    fe_mul(inv, inv, tot[b + 1]);
+    tot[b + 1] = u;
+    tot[b] = inv;              // 1 / tot[b]
+  }
+}
+// A zero Z cannot come from a curve point.  Setting it to 1 and clearing the record's parse bit keeps one bad record from poisoning
+// the block's shared inversion.
+__device__ __forceinline__ void guard_zero_z(fe &Z, uint32_t &meta) {
+  if (fe_is_zero(Z)) {
+    fe_set1(Z);
+    meta &= ~HS_META_PARSE_OK;
   }
 }
 
@@ -596,9 +649,8 @@ __global__ void __launch_bounds__(64) k_verify_small(const small_rec *__restrict
 // A certificate of a large committee (thousands of votes) as ONE queue request: k_verify_small would spend a 64-thread block and a
 // square-root chain on every signature, several waves of them.  Here a THREAD verifies a signature as k_verify_main<true> does,
 // straight from the queue's mapped ring (logical record i = ring slot (base + i) & mask, so a group may wrap the ring's end), and
-// the block finishes its own records: the block's Z's share one batched inversion (Montgomery's trick through shared memory, warp 0
-// inverting the product of 4 threads' Z's per lane, as in k_verify_finish), then the affine comparison with R's encoding — no
-// decompression of R, no global scratch, no second launch.  Flags and completion as in k_verify_small: both HS_F_EQ and HS_F_STRICT
+// the block finishes its own records: the block's Z's share one batched inversion (block_invert4), then the affine comparison with
+// R's encoding — no decompression of R, no global scratch, no second launch.  Flags and completion as in k_verify_small: both HS_F_EQ and HS_F_STRICT
 // per record, one counter add per block, and the block that completes the request raises its completion word.  One launch carries
 // exactly one request (n records).
 // Sizing: 128 threads, at least 3 blocks per SM.  R and the request fields stay live across the comb, so the 4-block budget of
@@ -623,24 +675,13 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
   const uint32_t cnt = (n - first < HS_BULK_THREADS) ? n - first : HS_BULK_THREADS;  // records of this block (the last one is partial)
   // (threads past n compute on a zero record and store nothing: every thread reaches the barriers below)
   uint4 q[8];
-  {  // a warp stages its 32 records (128 B each) with coalesced 16-byte loads, then each lane reads its own row back
-    uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
-    const uint32_t warp_first = first + (threadIdx.x & ~31u);
-#pragma unroll
-    for (int j = 0; j < 8; j++) {
-      const int c = j * 32 + lane, rec = c >> 3, part = c & 7;
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (warp_first + rec < n) v = __ldg(reinterpret_cast<const uint4 *>(ring + ((base + warp_first + rec) & mask)) + part);
-      sw[rec * 8 + (part ^ (rec & 7))] = v;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int part = 0; part < 8; part++) q[part] = sw[lane * 8 + (part ^ (lane & 7))];
-  }
+  uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
+  const uint32_t warp_first = first + (threadIdx.x & ~31u);
+  warp_stage_rows128(q, n, warp_first, [&](int r) { return reinterpret_cast<const uint4 *>(ring + ((base + warp_first + r) & mask)); }, sw, lane);
   __syncthreads();  // the staging bytes become the digit slots
   uint32_t R[8], S[8], A[8], h[16];
-  R[0] = q[0].x; R[1] = q[0].y; R[2] = q[0].z; R[3] = q[0].w; R[4] = q[1].x; R[5] = q[1].y; R[6] = q[1].z; R[7] = q[1].w;
-  S[0] = q[2].x; S[1] = q[2].y; S[2] = q[2].z; S[3] = q[2].w; S[4] = q[3].x; S[5] = q[3].y; S[6] = q[3].z; S[7] = q[3].w;
+  unpack8(R, q[0], q[1]);
+  unpack8(S, q[2], q[3]);
   uint32_t v = q[6].x;  // small_rec: sig | msg | vidx | req | req_n
   const uint32_t req = q[6].y, req_n = q[6].z;
   const bool have_key = v < C.n_keys;  // HS_NO_KEY (cannot reach this path: kept as in k_verify_small) rejects the record
@@ -652,7 +693,7 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
   const bool probed = SIGC && have_key && threadIdx.x < cnt;
   {
     uint32_t M[8];
-    M[0] = q[4].x; M[1] = q[4].y; M[2] = q[4].z; M[3] = q[4].w; M[4] = q[5].x; M[5] = q[5].y; M[6] = q[5].z; M[7] = q[5].w;
+    unpack8(M, q[4], q[5]);
     load32(A, C.pks + (size_t)v * 32);  // hash the registered key bytes, as k_verify_main<true>
     if constexpr (SIGC) {
       keep = sig_smem<24 * HS_BULK_THREADS>();
@@ -680,30 +721,10 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
     fe_set1(acc.Z);
   }
   if (!have_key) meta = 0;
-  if (fe_is_zero(acc.Z)) {  // cannot happen for curve points; keeps one bad record from poisoning the block's inversion
-    fe_set1(acc.Z);
-    meta &= ~HS_META_PARSE_OK;
-  }
+  guard_zero_z(acc.Z, meta);
   tot[threadIdx.x] = acc.Z;
   __syncthreads();
-  if (threadIdx.x < HS_BULK_THREADS / 4) {  // lane l: 1 / Z of threads 4l .. 4l+3 from one inversion
-    const int b = threadIdx.x * 4;
-    fe q0 = tot[b], q1, q2, q3, inv, u;
-    fe_mul(q1, q0, tot[b + 1]);
-    fe_mul(q2, q1, tot[b + 2]);
-    fe_mul(q3, q2, tot[b + 3]);
-    fe_invert(inv, q3);
-    fe_mul(u, inv, q2);
-    fe_mul(inv, inv, tot[b + 3]);
-    tot[b + 3] = u;
-    fe_mul(u, inv, q1);
-    fe_mul(inv, inv, tot[b + 2]);
-    tot[b + 2] = u;
-    fe_mul(u, inv, q0);
-    fe_mul(inv, inv, tot[b + 1]);
-    tot[b + 1] = u;
-    tot[b] = inv;
-  }
+  block_invert4(tot);
   if constexpr (SIGC) {  // the digit slots are free now (every thread is past the comb): word 0 gathers the block's counts
     if (threadIdx.x == 0) *reinterpret_cast<uint32_t *>(smem_raw) = 0;
   }
@@ -728,12 +749,7 @@ __global__ void __launch_bounds__(HS_BULK_THREADS, HS_BULK_MINBLOCKS) k_verify_b
   } else {
     __syncthreads();
   }
-  if (threadIdx.x == 0 && atomicAdd(counters + req, cnt) == req_n - cnt) {  // thread 0 holds a record of the request
-    if constexpr (SIGC) sig_publish(sc, req);
-    counters[req] = 0;
-    __threadfence_system();
-    done[req] = seq;
-  }
+  if (threadIdx.x == 0) queue_complete<SIGC>(counters, done, seq, req, req_n, cnt, sc);  // thread 0 holds a record of the request
 }
 
 // ------------------------------------------------------------------------------------------------ generic queue path (hs_queue_generic)
@@ -761,34 +777,20 @@ __global__ void __launch_bounds__(HS_GEN_THREADS, HS_GENERIC_MINBLOCKS) k_queue_
   const bool active = j < n;  // threads past n take every barrier with Z = 1 and store nothing
   const uint32_t slot = active ? __ldg(slots + ((first + j) & mask)) : 0u;
   uint4 q[8];
-  {
-    uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
-    const uint32_t warp_first = j & ~31u;
-#pragma unroll
-    for (int w = 0; w < 8; w++) {
-      const int c = w * 32 + lane, rec = c >> 3, part = c & 7;
-      const uint32_t s = __shfl_sync(0xffffffffu, slot, rec);
-      uint4 v = make_uint4(0, 0, 0, 0);
-      if (warp_first + rec < n) v = __ldg(reinterpret_cast<const uint4 *>(ring + s) + part);
-      sw[rec * 8 + (part ^ (rec & 7))] = v;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int part = 0; part < 8; part++) q[part] = sw[lane * 8 + (part ^ (lane & 7))];
-  }
+  uint4 *sw = reinterpret_cast<uint4 *>(smem_raw) + (threadIdx.x >> 5) * 256;
+  warp_stage_rows128(q, n, j & ~31u, [&](int r) { return reinterpret_cast<const uint4 *>(ring + __shfl_sync(0xffffffffu, slot, r)); }, sw, lane);
   __syncthreads();  // the staging bytes become the digit slots
   uint32_t R[8];
-  R[0] = q[0].x; R[1] = q[0].y; R[2] = q[0].z; R[3] = q[0].w; R[4] = q[1].x; R[5] = q[1].y; R[6] = q[1].z; R[7] = q[1].w;
+  unpack8(R, q[0], q[1]);
   const uint32_t req = q[6].y, req_n = q[6].z;  // small_rec: sig | msg | vidx | req | req_n
   ge_ext acc;
   uint32_t meta = 0;
   if (active) {
     uint32_t S[8], A[8], M[8], h[16];
-    S[0] = q[2].x; S[1] = q[2].y; S[2] = q[2].z; S[3] = q[2].w; S[4] = q[3].x; S[5] = q[3].y; S[6] = q[3].z; S[7] = q[3].w;
-    M[0] = q[4].x; M[1] = q[4].y; M[2] = q[4].z; M[3] = q[4].w; M[4] = q[5].x; M[5] = q[5].y; M[6] = q[5].z; M[7] = q[5].w;
+    unpack8(S, q[2], q[3]);
+    unpack8(M, q[4], q[5]);
     const uint4 *a4 = reinterpret_cast<const uint4 *>(pks + 32 * (size_t)slot);
-    const uint4 a0 = __ldg(a4), a1 = __ldg(a4 + 1);
-    A[0] = a0.x; A[1] = a0.y; A[2] = a0.z; A[3] = a0.w; A[4] = a1.x; A[5] = a1.y; A[6] = a1.z; A[7] = a1.w;
+    unpack8(A, __ldg(a4), __ldg(a4 + 1));
     sha512_ram32(h, R, A, M);
     ge_cached tab[9];
     meta = verify_generic_main(acc, R, S, A, h, btable, tab, reinterpret_cast<int32_t *>(smem_raw) + threadIdx.x, HS_GEN_THREADS, cp);
@@ -798,39 +800,15 @@ __global__ void __launch_bounds__(HS_GEN_THREADS, HS_GENERIC_MINBLOCKS) k_queue_
     fe_set1(acc.Y);
     fe_set1(acc.Z);
   }
-  if (fe_is_zero(acc.Z)) {  // cannot happen for curve points; keeps one bad record from poisoning the block's inversion
-    fe_set1(acc.Z);
-    meta &= ~HS_META_PARSE_OK;
-  }
+  guard_zero_z(acc.Z, meta);
   tot[threadIdx.x] = acc.Z;
   __syncthreads();
-  if (threadIdx.x < HS_GEN_THREADS / 4) {  // lane l: 1 / Z of threads 4l .. 4l+3 from one inversion
-    const int b = threadIdx.x * 4;
-    fe q0 = tot[b], q1, q2, q3, inv, u;
-    fe_mul(q1, q0, tot[b + 1]);
-    fe_mul(q2, q1, tot[b + 2]);
-    fe_mul(q3, q2, tot[b + 3]);
-    fe_invert(inv, q3);
-    fe_mul(u, inv, q2);
-    fe_mul(inv, inv, tot[b + 3]);
-    tot[b + 3] = u;
-    fe_mul(u, inv, q1);
-    fe_mul(inv, inv, tot[b + 2]);
-    tot[b + 2] = u;
-    fe_mul(u, inv, q0);
-    fe_mul(inv, inv, tot[b + 1]);
-    tot[b + 1] = u;
-    tot[b] = inv;
-  }
+  block_invert4(tot);
   __syncthreads();
   if (!active) return;
   out_flags[slot] = (uint8_t)verify_flags_from(acc.X, acc.Y, tot[threadIdx.x], R, meta);
   __threadfence_system();
-  if (atomicAdd(counters + req, 1u) == req_n - 1) {
-    counters[req] = 0;
-    __threadfence_system();
-    done[req] = seq;
-  }
+  queue_complete<false>(counters, done, seq, req, req_n, 1u, {});
 }
 
 // A few LONG messages (one mempool batch is ~15 kB = 120 blocks, mempool/src/processor.rs:30): SHA-512 is sequential in its
@@ -863,9 +841,7 @@ __global__ void __launch_bounds__(32) k_digest32_long(const uint8_t *__restrict_
   if (lane == 0) {
     uint32_t h[16];
     sha512_output_words(s, h);
-    uint4 *dst = reinterpret_cast<uint4 *>(out + i * 8);
-    dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
-    dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+    store_digest32(out + i * 8, h);
   }
 }
 
@@ -925,8 +901,7 @@ __global__ void k_peer_sync_only(const peer_route P) { peer_signal_and_wait(P); 
 // ------------------------------------------------------------------------------------------------ phase 2: finish
 __device__ __forceinline__ void fe_load_global(fe &r, const fe *p) {
   const uint4 *s = reinterpret_cast<const uint4 *>(p);
-  uint4 a = s[0], b = s[1];
-  r.v[0] = a.x; r.v[1] = a.y; r.v[2] = a.z; r.v[3] = a.w; r.v[4] = b.x; r.v[5] = b.y; r.v[6] = b.z; r.v[7] = b.w;
+  unpack8(r.v, s[0], s[1]);
 }
 // One thread owns `group` (16, 8 or 4: fewer for small batches, so that enough blocks exist to hide the one serial field inversion
 // each block waits for — at 126 k records the 16-record form ran 62 blocks for 110 us) consecutive records.  Montgomery's trick at two levels so that ONE
@@ -955,24 +930,7 @@ __global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_
   }
   tot[threadIdx.x] = run;
   __syncthreads();
-  if (threadIdx.x < 32) {
-    const int b = threadIdx.x * 4;
-    fe q0 = tot[b], q1, q2, q3, inv, u;
-    fe_mul(q1, q0, tot[b + 1]);
-    fe_mul(q2, q1, tot[b + 2]);
-    fe_mul(q3, q2, tot[b + 3]);
-    fe_invert(inv, q3);
-    fe_mul(u, inv, q2);        // 1 / tot[b+3]
-    fe_mul(inv, inv, tot[b + 3]);
-    tot[b + 3] = u;
-    fe_mul(u, inv, q1);        // 1 / tot[b+2]
-    fe_mul(inv, inv, tot[b + 2]);
-    tot[b + 2] = u;
-    fe_mul(u, inv, q0);        // 1 / tot[b+1]
-    fe_mul(inv, inv, tot[b + 1]);
-    tot[b + 1] = u;
-    tot[b] = inv;              // 1 / tot[b]
-  }
+  block_invert4(tot);
   __syncthreads();
   uint32_t bits = 0;
   if (cnt) {
@@ -1071,9 +1029,7 @@ __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restri
   const uint8_t *m = off ? data + off[i] : data + i * fixed_len;
   const uint64_t len = off ? off[i + 1] - off[i] : fixed_len;
   sha512_prefix_msg(h, pre, 0, m, len);
-  uint4 *dst = reinterpret_cast<uint4 *>(out + i * 8);
-  dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
-  dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  store_digest32(out + i * 8, h);
 }
 
 // Verify queue requests that carry signed preimages instead of Digests (hs_queue_submit_msgs).  A request's region of the queue's
@@ -1112,9 +1068,7 @@ __global__ void __launch_bounds__(HS_QDIG_THREADS) k_queue_digests(const qmsg_de
     uint32_t h[16];
     const uint64_t none[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     sha512_prefix_msg(h, none, 0, pre + pre_off[j], pre_off[j + 1] - pre_off[j]);
-    uint4 *o = reinterpret_cast<uint4 *>(dig + (size_t)j * 8);
-    o[0] = make_uint4(h[0], h[1], h[2], h[3]);
-    o[1] = make_uint4(h[4], h[5], h[6], h[7]);
+    store_digest32(dig + (size_t)j * 8, h);
   }
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < d.n; i += HS_QDIG_THREADS) {
@@ -1141,7 +1095,9 @@ __global__ void __launch_bounds__(HS_THREADS) k_digest32_fixed(const uint8_t *__
 #pragma unroll 1
   for (uint64_t b = 0; b < nfull; b++) {
     uint4 q[8];
-    warp_stage_rows128(q, data + b * 128, len, n, warp_first, stage[threadIdx.x >> 5]);
+    warp_stage_rows128(q, n, warp_first, [&](int r) { return reinterpret_cast<const uint4 *>(data + b * 128 + (warp_first + r) * len); },
+                       stage[threadIdx.x >> 5], threadIdx.x & 31);
+    __syncwarp();  // the next block is staged into the same rows
     uint64_t w[16];
 #pragma unroll
     for (int k = 0; k < 8; k++) {
@@ -1159,12 +1115,15 @@ __global__ void __launch_bounds__(HS_THREADS) k_digest32_fixed(const uint8_t *__
   }
   uint32_t h[16];
   sha512_output_words(s, h);
-  uint4 *dst = reinterpret_cast<uint4 *>(out + i * 8);
-  dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
-  dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  store_digest32(out + i * 8, h);
 }
 
 // ------------------------------------------------------------------------------------------------ per-QC AND
+// word w of an all-ones bitmap over n bits (unused high bits of the last word 0)
+template <class T>
+__host__ __device__ inline uint32_t bitmap_word_ones(const T &n, const T &w) {
+  return ((n & 31) && w == (n + 31) / 32 - 1) ? ((1u << (n & 31)) - 1u) : 0xffffffffu;
+}
 // vote i belongs to certificate qc_idx[i]; a rejected vote clears its certificate's bit (qc bitmap pre-set to all ones)
 __global__ void __launch_bounds__(256) k_qc_and(const uint32_t *__restrict__ vote_bitmap, const uint32_t *__restrict__ qc_idx, size_t n_votes,
                                                 size_t n_qc, uint32_t *__restrict__ qc_bitmap) {
@@ -1221,10 +1180,7 @@ __global__ void __launch_bounds__(256) k_batch_done(const uint8_t *__restrict__ 
   __syncthreads();
   if (!is_last) return;
   __threadfence();
-  for (uint32_t w = threadIdx.x; w < gw; w += 256) {
-    const uint32_t valid = (w == gw - 1 && (n_groups & 31)) ? ((1u << (n_groups & 31)) - 1u) : 0xffffffffu;
-    out[w] = ~atomicOr(grej + w, 0u) & valid;
-  }
+  for (uint32_t w = threadIdx.x; w < gw; w += 256) out[w] = bitmap_word_ones(n_groups, w) & ~atomicOr(grej + w, 0u);
   if (threadIdx.x == 0) tail[0] = miss_count ? *(volatile const uint32_t *)miss_count : n_items;
   __threadfence_system();
   __syncthreads();
@@ -1237,8 +1193,7 @@ __global__ void __launch_bounds__(256) k_batch_done(const uint8_t *__restrict__ 
 // all-ones bitmap over n bits (unused high bits of the last word 0)
 __global__ void k_bitmap_ones(uint32_t *bm, size_t n) {
   const size_t w = (size_t)blockIdx.x * 256 + threadIdx.x;
-  const size_t words = (n + 31) / 32;
-  if (w < words) bm[w] = (w == words - 1 && (n & 31)) ? ((1u << (n & 31)) - 1u) : 0xffffffffu;
+  if (w < (n + 31) / 32) bm[w] = bitmap_word_ones(n, w);
 }
 // TC::verify (consensus/src/messages.rs:307-311) and Timeout::digest (:268-275): the message of vote i is
 // SHA-512(tc_round_le || high_qc_round_le)[..32] — 16 bytes of which 8 differ per vote; built and hashed here from the two
@@ -1262,9 +1217,7 @@ __global__ void __launch_bounds__(HS_THREADS) k_tc_digests(const uint64_t *__res
   sha512_compress(s, w);
   uint32_t h[16];
   sha512_output_words(s, h);
-  uint4 *dst = reinterpret_cast<uint4 *>(out + i * 8);
-  dst[0] = make_uint4(h[0], h[1], h[2], h[3]);
-  dst[1] = make_uint4(h[4], h[5], h[6], h[7]);
+  store_digest32(out + i * 8, h);
 }
 
 // ------------------------------------------------------------------------------------------------ load generation: keygen / sign
@@ -3015,7 +2968,7 @@ int hs_verify_qcs(hs_ctx *c, const uint8_t *preimages, size_t n_qc, const uint8_
   if (!c || !out_qc_bitmap || (n_qc && !preimages) || (n_votes && (!sig || !qc_idx || (!pk && !vidx) || n_qc == 0)))
     return fail(c, HS_ERR_ARG, "hs_verify_qcs: bad argument");
   const size_t qc_words = (n_qc + 31) / 32, vote_words = (n_votes + 31) / 32;
-  for (size_t w = 0; w < qc_words; w++) out_qc_bitmap[w] = (w == qc_words - 1 && (n_qc & 31)) ? ((1u << (n_qc & 31)) - 1u) : 0xffffffffu;
+  for (size_t w = 0; w < qc_words; w++) out_qc_bitmap[w] = bitmap_word_ones(n_qc, w);
   if (n_votes == 0) return HS_OK;
   for (size_t i = 0; i < n_votes; i++)
     if (qc_idx[i] >= n_qc) return fail(c, HS_ERR_ARG, "hs_verify_qcs: qc_idx out of range");
@@ -3083,7 +3036,7 @@ int hs_verify_tcs(hs_ctx *c, const uint64_t *tc_rounds, size_t n_tc, const uint8
   if (!c || !out_tc_bitmap || (n_tc && !tc_rounds) || (n_votes && (!sig || !high_qc_rounds || (!pk && !vidx) || n_tc == 0)) || (!tc_idx && n_votes && n_tc != n_votes))
     return fail(c, HS_ERR_ARG, "hs_verify_tcs: bad argument");
   const size_t tc_words = (n_tc + 31) / 32, vote_words = (n_votes + 31) / 32;
-  for (size_t w = 0; w < tc_words; w++) out_tc_bitmap[w] = (w == tc_words - 1 && (n_tc & 31)) ? ((1u << (n_tc & 31)) - 1u) : 0xffffffffu;
+  for (size_t w = 0; w < tc_words; w++) out_tc_bitmap[w] = bitmap_word_ones(n_tc, w);
   if (n_votes == 0) return HS_OK;
   if (tc_idx)
     for (size_t i = 0; i < n_votes; i++)
@@ -3131,7 +3084,7 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
   if (!c || !out_group_bitmap || (n_msgs && !pre_off) || (n_items && (!sig || !msg_idx || !group_idx || (!pk && !vidx) || n_msgs == 0 || n_groups == 0)))
     return fail(c, HS_ERR_ARG, "hs_verify_groups: bad argument");
   const size_t g_words = (n_groups + 31) / 32, i_words = (n_items + 31) / 32;
-  for (size_t w = 0; w < g_words; w++) out_group_bitmap[w] = (w == g_words - 1 && (n_groups & 31)) ? ((1u << (n_groups & 31)) - 1u) : 0xffffffffu;
+  for (size_t w = 0; w < g_words; w++) out_group_bitmap[w] = bitmap_word_ones(n_groups, w);
   if (n_items == 0) return HS_OK;
   if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages)) return fail(c, HS_ERR_ARG, "hs_verify_groups: bad preimage offsets");
   for (size_t i = 0; i < n_items; i++)
@@ -3381,8 +3334,7 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
       HS_TRY(run_small(c, n, HS_MODE_BATCH_EQ, bm2, nullptr));
       int ok2 = 1;
       for (size_t w = 0; w < words; w++) {
-        const uint32_t want = (w == words - 1 && (n & 31)) ? ((1u << (n & 31)) - 1u) : 0xffffffffu;
-        if (bm2[w] != want) ok2 = 0;
+        if (bm2[w] != bitmap_word_ones(n, w)) ok2 = 0;
         if (out_bitmap_or_null) out_bitmap_or_null[w] = bm2[w];
       }
       *all_ok = ok2;
@@ -3404,10 +3356,8 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
   }
   HS_TRY(finish_bitmap(c, n, bm));
   int ok = 1;
-  for (size_t w = 0; w < words; w++) {
-    uint32_t want = (w == words - 1 && (n & 31)) ? ((1u << (n & 31)) - 1u) : 0xffffffffu;
-    if (bm[w] != want) ok = 0;
-  }
+  for (size_t w = 0; w < words; w++)
+    if (bm[w] != bitmap_word_ones(n, w)) ok = 0;
   *all_ok = ok;
   return HS_OK;
 }

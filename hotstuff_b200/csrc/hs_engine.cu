@@ -1257,30 +1257,131 @@ __global__ void __launch_bounds__(HS_THREADS) k_sign_digests(const uint8_t *__re
 }
 
 // ================================================================================================ host side
-struct dev_buf {
-  void *p = nullptr;
+// ---- resource owners: the only code that creates or releases a CUDA resource, or looks up a mapped buffer's device alias
+// (hs_host_alloc / hs_host_free aside: they hand pinned memory to the caller).  Every buffer, stream, event and IPC mapping of a
+// context or a queue is held by one owner and released by its destructor or reset(), after whatever synchronisation its holder
+// performs first.  An owner converts to its raw handle: launches, CUDA calls and
+// the structs passed to kernels take that.  Owners move but never copy.
+template <class H, auto Release>
+class owned {
+ public:
+  owned() = default;
+  owned(owned &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+  owned &operator=(owned &&o) noexcept {
+    if (this != &o) reset(std::exchange(o.h_, nullptr));
+    return *this;
+  }
+  ~owned() { reset(); }
+  void reset(H h = nullptr) {
+    if (h_) Release(h_);
+    h_ = h;
+  }
+  H get() const { return h_; }
+  operator H() const { return h_; }
+
+ private:
+  H h_ = nullptr;
+};
+template <class T>
+using dev_mem = owned<T *, cudaFree>;  // cudaMalloc
+template <class T>
+using pinned = owned<T *, cudaFreeHost>;  // cudaMallocHost
+using stream_h = owned<cudaStream_t, cudaStreamDestroy>;
+using event_h = owned<cudaEvent_t, cudaEventDestroy>;
+using ipc_mapping = owned<void *, cudaIpcCloseMemHandle>;  // cudaIpcOpenMemHandle
+// Mapped pinned memory (cudaHostAllocMapped): the host pointer, and its device alias, looked up once by alloc().
+template <class T>
+struct mapped {
+  pinned<T> h;
+  T *d = nullptr;
+};
+
+// Creates a resource into o through fn(&handle).  The old resource is released FIRST, so peak memory never holds both; on failure o
+// stays empty.
+template <class H, auto R, class Fn>
+static cudaError_t acquire(owned<H, R> &o, Fn fn) {
+  o.reset();
+  H h = nullptr;
+  const cudaError_t e = fn(&h);
+  if (e == cudaSuccess) o.reset(h);
+  return e;
+}
+template <class T>
+static cudaError_t alloc(dev_mem<T> &m, size_t bytes) {
+  return acquire(m, [&](T **p) { return cudaMalloc(p, bytes); });
+}
+template <class T>
+static cudaError_t alloc(pinned<T> &m, size_t bytes) {
+  return acquire(m, [&](T **p) { return cudaMallocHost(p, bytes); });
+}
+template <class T>
+static cudaError_t alloc(mapped<T> &m, size_t bytes) {
+  m.d = nullptr;
+  const cudaError_t e = acquire(m.h, [&](T **p) { return cudaHostAlloc(p, bytes, cudaHostAllocMapped); });
+  return e == cudaSuccess ? cudaHostGetDevicePointer(&m.d, m.h, 0) : e;
+}
+static cudaError_t create(stream_h &s, int priority = 0) {  // priority 0 is the default stream priority
+  return acquire(s, [&](cudaStream_t *p) { return cudaStreamCreateWithPriority(p, cudaStreamNonBlocking, priority); });
+}
+static cudaError_t create(event_h &ev, unsigned flags = cudaEventDisableTiming) {
+  return acquire(ev, [&](cudaEvent_t *p) { return cudaEventCreateWithFlags(p, flags); });
+}
+static cudaError_t ipc_open(ipc_mapping &m, cudaIpcMemHandle_t h) {
+  return acquire(m, [&](void **p) { return cudaIpcOpenMemHandle(p, h, cudaIpcMemLazyEnablePeerAccess); });
+}
+// ---- end of resource owners
+
+struct dev_buf {  // grow-only device scratch (ensure())
+  dev_mem<void> p;
   size_t cap = 0;
+};
+// The committee's or the key cache's tables: keys, key flags, the key hash table and the per-key comb tables.  Built whole in a local
+// and moved in, so a failed registration or key-cache allocation leaves none of them.
+struct key_store {
+  dev_mem<uint8_t> pks;
+  dev_mem<uint8_t> key_flags;
+  dev_mem<ge_niels> atables;
+  dev_mem<uint32_t> slots;
+};
+// Key-cache learning: the unknown keys of a pass and their count, their pinned host copies, and the events.  Allocated whole on first use.
+struct learn_bufs {
+  dev_mem<uint8_t> keys;
+  dev_mem<uint32_t> n;
+  pinned<uint8_t> h_keys;
+  pinned<uint32_t> h_n;
+  pinned<uint32_t> h_miss_total;  // total misses of the pass whose keys are parked
+  event_h ev;
+  event_h ev_tables;  // recorded after the latest table build of the key cache; every pass waits for it (any stream)
+};
+// Latency path: mapped pinned staging (inputs, verdict flags, completion word) and the device block counter.
+struct small_staging {
+  mapped<small_rec> in;
+  mapped<uint8_t> out;
+  mapped<uint32_t> done;
+  dev_mem<uint32_t> counter;
+};
+// Multi-GPU peer routing: this rank's result buffer (cudaMalloc'd: [2][total_words][HS_MAX_PEERS flags][timeout flag, block counter])
+// and the mappings of the other ranks' buffers.
+struct peer_bufs {
+  dev_mem<uint32_t> own;
+  ipc_mapping mapped[HS_MAX_PEERS];
 };
 struct hs_ctx {
   int device = 0;
   unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
-  cudaStream_t stream = nullptr, stream2 = nullptr, stream_side = nullptr;
-  cudaEvent_t ev[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr}, ev_side[2] = {nullptr, nullptr};
-  ge_niels *d_btable = nullptr;
+  stream_h stream, stream2, stream_side;
+  event_h ev[2], ev_done[2], ev_side[2];
+  dev_mem<ge_niels> d_btable;
   comb_params cp{};
   size_t a_table_entries = 0;
   int wa_forced = 0;
   // committee
   size_t n_keys = 0;
-  uint8_t *d_pks = nullptr;
-  uint8_t *d_key_flags = nullptr;
-  ge_niels *d_atables = nullptr;
-  uint32_t *d_slots = nullptr;
+  key_store keys;
   uint32_t slot_mask = 0;
   // grow-only device scratch
   dev_buf in[2], digest[2], xyz, meta, vidx, miss, out;
-  uint32_t *d_miss_count = nullptr;
-  uint32_t *h_miss_count = nullptr;  // pinned
+  dev_mem<uint32_t> d_miss_count;
   // key cache: tables for keys that were never registered but keep showing up (learned between calls)
   bool explicit_committee = false;   // hs_committee_register was called with keys: the set is fixed, nothing is learned
   bool cache_wanted = true, cache_enabled = true;
@@ -1290,40 +1391,32 @@ struct hs_ctx {
   std::vector<uint8_t> h_key_live;   // explicit committee: 1 = slot holds a live validator, 0 = removed (free for reuse)
   size_t table_budget = 0;           // bytes the per-key tables may use (0 = ~62 % of the device)
   size_t key_capacity = 0;           // explicit committee: table slots allocated (>= n_keys; spare slots serve hs_committee_update)
-  uint8_t *d_learn_keys = nullptr, *h_learn_keys = nullptr;
-  uint32_t *d_learn_n = nullptr, *h_learn_n = nullptr;
-  cudaEvent_t ev_learn = nullptr;
-  cudaEvent_t ev_tables = nullptr;   // recorded after the latest table build of the key cache; every pass waits for it (any stream)
+  learn_bufs learn;
   bool learn_pending = false;
   bool cache_full = false;           // no free slot: only the miss RATE is watched (a mostly-missing full cache is reset)
   uint64_t calls_since_reset = HS_CACHE_RESET_MIN_CALLS;
-  size_t learn_records = 0;          // records of the pass whose misses are parked in h_learn_*
-  uint32_t *h_miss_total = nullptr;  // pinned: total misses of that pass
+  size_t learn_records = 0;          // records of the pass whose misses are parked in learn.h_*
   // multi-GPU peer routing
   peer_route peers{};
   int peer_rank = 0;
   size_t peer_total_words = 0;
-  uint32_t *peer_own = nullptr;       // cudaMalloc'd: [2][total_words][HS_MAX_PEERS flags][timeout flag, block counter]
-  void *peer_mapped[HS_MAX_PEERS] = {};
+  peer_bufs peer;
   bool peer_armed = false;
   uint32_t peer_epoch = 0;
-  // latency path: mapped pinned staging (inputs, verdict flags, completion word) + device block counter
-  small_rec *h_small_in = nullptr;
-  uint8_t *h_small_out = nullptr;
-  uint32_t *h_small_done = nullptr;
-  uint32_t *d_small_counter = nullptr;
+  // latency path
+  small_staging small;
   uint32_t small_seq = 0;
   bool small_enabled = true;
   // deferred-results mode (hs_set_deferred): the latency-bound tail of a `_dev` verify pass (finish kernel, peer exchange, per-QC AND)
   // runs on an internal stream so that it overlaps the main kernel of the NEXT pass; two scratch sets alternate
   bool deferred = false;
-  cudaStream_t stream_tail = nullptr;
-  cudaEvent_t ev_main_done = nullptr, ev_tail[2] = {nullptr, nullptr}, ev_results = nullptr;
+  stream_h stream_tail;
+  event_h ev_main_done, ev_tail[2], ev_results;
   dev_buf xyz2, meta2;
   int flip = 0;
   // optional timing of the dominant kernel alone (bench.py's roofline): events around k_verify_main<committee>
   bool profile_main = false;
-  cudaEvent_t ev_prof[2] = {nullptr, nullptr};
+  event_h ev_prof[2];
   std::atomic<uint64_t> launches{0};
   std::mutex mu;
   std::mutex err_mu;                  // guards err only: fail() is also reached from argument checks taken before `mu`
@@ -1356,14 +1449,10 @@ static int fail(hs_ctx *c, int code, const char *what, cudaError_t e = cudaSucce
 
 static int ensure(hs_ctx *c, dev_buf &b, size_t need) {
   if (need <= b.cap) return HS_OK;
-  if (b.p) {
-    cudaDeviceSynchronize();  // the old block may still be in flight on another stream
-    cudaFree(b.p);
-  }
-  b.p = nullptr;
+  if (b.p) cudaDeviceSynchronize();  // the old block may still be in flight on another stream
   b.cap = 0;
   size_t want = need + need / 4 + 4096;
-  cudaError_t e = cudaMalloc(&b.p, want);
+  cudaError_t e = alloc(b.p, want);  // frees the old block first
   if (e != cudaSuccess) return fail(c, HS_ERR_NOMEM, "cudaMalloc scratch", e);
   b.cap = want;
   return HS_OK;
@@ -1393,14 +1482,7 @@ static void set_window(comb_params &cp, bool a, int w) {
 
 // ---- key cache -----------------------------------------------------------------------------------------------------
 static void cache_release(hs_ctx *c) {
-  cudaFree(c->d_pks);
-  cudaFree(c->d_key_flags);
-  cudaFree(c->d_atables);
-  cudaFree(c->d_slots);
-  c->d_pks = nullptr;
-  c->d_key_flags = nullptr;
-  c->d_atables = nullptr;
-  c->d_slots = nullptr;
+  c->keys = {};
   c->n_keys = 0;
   c->h_pks.clear();
   c->h_slots.clear();
@@ -1427,11 +1509,13 @@ static int cache_allocate(hs_ctx *c) {
   while (cap < 2 * c->cache_cap) cap <<= 1;
   set_window(c->cp, true, wa);
   c->a_table_entries = comb_table_entries(wa);
-  HS_CUDA(c, cudaMalloc(&c->d_pks, c->cache_cap * 32));
-  HS_CUDA(c, cudaMalloc(&c->d_key_flags, c->cache_cap));
-  HS_CUDA(c, cudaMalloc(&c->d_slots, (size_t)cap * 4));
-  HS_CUDA(c, cudaMalloc(&c->d_atables, c->cache_cap * sizeof(ge_niels) * c->a_table_entries));
-  HS_CUDA(c, cudaMemset(c->d_slots, 0xff, (size_t)cap * 4));
+  key_store K;
+  HS_CUDA(c, alloc(K.pks, c->cache_cap * 32));
+  HS_CUDA(c, alloc(K.key_flags, c->cache_cap));
+  HS_CUDA(c, alloc(K.slots, (size_t)cap * 4));
+  HS_CUDA(c, alloc(K.atables, c->cache_cap * sizeof(ge_niels) * c->a_table_entries));
+  HS_CUDA(c, cudaMemset(K.slots, 0xff, (size_t)cap * 4));
+  c->keys = std::move(K);
   c->slot_mask = cap - 1;
   c->h_slots.assign(cap, HS_NO_KEY);
   c->h_pks.clear();
@@ -1441,26 +1525,26 @@ static int cache_allocate(hs_ctx *c) {
 // dedupe them, append the new ones to the store and build their comb tables on `stream` before this pass's lookup runs.
 static int learn_process(hs_ctx *c, cudaStream_t stream) {
   if (!c->learn_pending) return HS_OK;
-  if (cudaEventQuery(c->ev_learn) != cudaSuccess) return HS_OK;  // copy still in flight: try again on the next call
+  if (cudaEventQuery(c->learn.ev) != cudaSuccess) return HS_OK;  // copy still in flight: try again on the next call
   c->learn_pending = false;
   c->calls_since_reset++;
   if (!c->cache_enabled || c->explicit_committee) return HS_OK;
   if (c->cache_full) {
     // Full cache that no longer matches the traffic (e.g. the validator set rotated): more than half of the last pass missed.
     // Start over — the next passes relearn the keys that are actually in use.  (No per-key eviction; see DESIGN.md §8.)
-    if (c->learn_records >= 64 && (size_t)*c->h_miss_total * 2 > c->learn_records && c->calls_since_reset >= HS_CACHE_RESET_MIN_CALLS) {
+    if (c->learn_records >= 64 && (size_t)*c->learn.h_miss_total * 2 > c->learn_records && c->calls_since_reset >= HS_CACHE_RESET_MIN_CALLS) {
       c->calls_since_reset = 0;
       c->n_keys = 0;
       c->h_pks.clear();
       std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
-      HS_CUDA(c, cudaMemsetAsync(c->d_slots, 0xff, c->h_slots.size() * 4, stream));
+      HS_CUDA(c, cudaMemsetAsync(c->keys.slots, 0xff, c->h_slots.size() * 4, stream));
       c->cache_full = false;
     }
     return HS_OK;
   }
-  const uint32_t got = *c->h_learn_n < HS_LEARN_MAX ? *c->h_learn_n : HS_LEARN_MAX;
+  const uint32_t got = *c->learn.h_n < HS_LEARN_MAX ? *c->learn.h_n : HS_LEARN_MAX;
   if (got == 0) return HS_OK;
-  if (!c->d_atables) {
+  if (!c->keys.atables) {
     HS_TRY(cache_allocate(c));
     if (!c->cache_enabled) return HS_OK;
   }
@@ -1468,7 +1552,7 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
   size_t n_new = 0;
   const uint32_t mask = c->slot_mask;
   for (uint32_t t = 0; t < got && old_n + n_new < c->cache_cap && n_new < HS_LEARN_PER_CALL; t++) {
-    const uint8_t *key = c->h_learn_keys + 32 * (size_t)t;
+    const uint8_t *key = c->learn.h_keys + 32 * (size_t)t;
     uint32_t w[8];
     memcpy(w, key, 32);
     uint32_t h = key_hash(w) & mask;
@@ -1486,15 +1570,15 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
     n_new++;
   }
   if (n_new == 0) return HS_OK;
-  HS_CUDA(c, cudaMemcpyAsync(c->d_pks + old_n * 32, c->h_pks.data() + old_n * 32, n_new * 32, cudaMemcpyHostToDevice, stream));
-  HS_CUDA(c, cudaMemcpyAsync(c->d_slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, stream));
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + old_n * 32, c->h_pks.data() + old_n * 32, n_new * 32, cudaMemcpyHostToDevice, stream));
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, stream));
   size_t threads = n_new * (size_t)c->cp.na * ((1u << (c->cp.wa - 1)) / HS_BUILD_BLOCK);
-  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(c->d_pks + old_n * 32, n_new, 1, c->cp.wa, c->cp.na,
-                                                                c->d_atables + old_n * c->a_table_entries, c->d_key_flags + old_n);
+  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(c->keys.pks + old_n * 32, n_new, 1, c->cp.wa, c->cp.na,
+                                                                c->keys.atables + old_n * c->a_table_entries, c->keys.key_flags + old_n);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   // (no synchronisation: copies from pageable memory return once the source is staged, so the host vectors may change afterwards)
-  HS_CUDA(c, cudaEventRecord(c->ev_tables, stream));  // passes on OTHER streams (host entry points vs a _dev caller's stream) wait for the build
+  HS_CUDA(c, cudaEventRecord(c->learn.ev_tables, stream));  // passes on OTHER streams (host entry points vs a _dev caller's stream) wait for the build
   c->n_keys = old_n + n_new;
   if (c->n_keys >= c->cache_cap) c->cache_full = true;  // no free slot: unknown keys stay on the generic path until a reset
   return HS_OK;
@@ -1502,30 +1586,33 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
 // After the lookup of a pass: park the unknown keys for learn_process().
 static int learn_collect(hs_ctx *c, const in_layout &L, size_t n, bool have_lookup, cudaStream_t stream) {
   if (!c->cache_enabled || c->explicit_committee || c->learn_pending || !L.pk) return HS_OK;
-  if (!c->d_learn_keys) {
-    HS_CUDA(c, cudaMalloc(&c->d_learn_keys, (size_t)HS_LEARN_MAX * 32));
-    HS_CUDA(c, cudaMalloc(&c->d_learn_n, 4));
-    HS_CUDA(c, cudaMallocHost(&c->h_learn_keys, (size_t)HS_LEARN_MAX * 32));
-    HS_CUDA(c, cudaMallocHost(&c->h_learn_n, 4));
-    HS_CUDA(c, cudaMallocHost(&c->h_miss_total, 4));
-    HS_CUDA(c, cudaEventCreateWithFlags(&c->ev_learn, cudaEventDisableTiming));
-    HS_CUDA(c, cudaEventCreateWithFlags(&c->ev_tables, cudaEventDisableTiming));
+  if (!c->learn.keys) {  // first use: every buffer, or none
+    learn_bufs B;
+    HS_CUDA(c, alloc(B.keys, (size_t)HS_LEARN_MAX * 32));
+    HS_CUDA(c, alloc(B.n, 4));
+    HS_CUDA(c, alloc(B.h_keys, (size_t)HS_LEARN_MAX * 32));
+    HS_CUDA(c, alloc(B.h_n, 4));
+    HS_CUDA(c, alloc(B.h_miss_total, 4));
+    HS_CUDA(c, create(B.ev));
+    HS_CUDA(c, create(B.ev_tables));
+    c->learn = std::move(B);
   }
+  learn_bufs &B = c->learn;
   c->learn_records = n;
   if (c->cache_full) {  // only watch the miss rate
     if (!have_lookup) return HS_OK;
-    HS_CUDA(c, cudaMemcpyAsync(c->h_miss_total, c->d_miss_count, 4, cudaMemcpyDeviceToHost, stream));
-    HS_CUDA(c, cudaEventRecord(c->ev_learn, stream));
+    HS_CUDA(c, cudaMemcpyAsync(B.h_miss_total, c->d_miss_count, 4, cudaMemcpyDeviceToHost, stream));
+    HS_CUDA(c, cudaEventRecord(B.ev, stream));
     c->learn_pending = true;
     return HS_OK;
   }
-  k_gather_keys<<<blocks_for(HS_LEARN_MAX, 256), 256, 0, stream>>>(L, n, have_lookup ? (const uint32_t *)c->miss.p : nullptr,
-                                                                     have_lookup ? c->d_miss_count : nullptr, HS_LEARN_MAX, c->d_learn_keys, c->d_learn_n);
+  k_gather_keys<<<blocks_for(HS_LEARN_MAX, 256), 256, 0, stream>>>(L, n, have_lookup ? (const uint32_t *)c->miss.p.get() : nullptr,
+                                                                     have_lookup ? c->d_miss_count.get() : nullptr, HS_LEARN_MAX, B.keys, B.n);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  HS_CUDA(c, cudaMemcpyAsync(c->h_learn_n, c->d_learn_n, 4, cudaMemcpyDeviceToHost, stream));
-  HS_CUDA(c, cudaMemcpyAsync(c->h_learn_keys, c->d_learn_keys, (size_t)HS_LEARN_MAX * 32, cudaMemcpyDeviceToHost, stream));
-  HS_CUDA(c, cudaEventRecord(c->ev_learn, stream));
+  HS_CUDA(c, cudaMemcpyAsync(B.h_n, B.n, 4, cudaMemcpyDeviceToHost, stream));
+  HS_CUDA(c, cudaMemcpyAsync(B.h_keys, B.keys, (size_t)HS_LEARN_MAX * 32, cudaMemcpyDeviceToHost, stream));
+  HS_CUDA(c, cudaEventRecord(B.ev, stream));
   c->learn_pending = true;
   return HS_OK;
 }
@@ -1537,7 +1624,7 @@ struct pass_scratch {
   uint32_t *vidx, *miss, *miss_count;  // k_key_lookup's outputs (table path with key bytes)
   cudaStream_t side;                   // the generic pass over the lookup's misses
   cudaEvent_t ev_side[2];
-  cudaEvent_t *prof;                   // nullable: events around k_verify_main<committee>
+  const event_h *prof;                 // nullable: events around k_verify_main<committee>
 };
 // The main phase on `stream`: with committee tables, [k_key_lookup, then k_verify_main<false> over the misses on S.side] beside
 // k_verify_main<true>; without, k_verify_main<false> over every record.  after_lookup(have_lookup) runs where run_verify collects
@@ -1546,10 +1633,10 @@ template <class AfterLookup>
 static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool indexed, const pass_scratch &S, cudaStream_t stream,
                        AfterLookup after_lookup) {
   main_out O{S.xyz, S.meta, 0};
-  committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
+  committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
   if (committee) {
     if (!indexed) {
-      key_table T{c->d_slots, c->slot_mask, c->d_pks, (uint32_t)c->n_keys};
+      key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)c->n_keys};
       HS_CUDA(c, cudaMemsetAsync(S.miss_count, 0, 4, stream));
       k_key_lookup<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, T, S.vidx, S.miss, S.miss_count);
       c->launches++;
@@ -1608,7 +1695,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   }
   if (indexed && (!c->explicit_committee || c->n_keys == 0)) return fail(c, HS_ERR_ARG, "committee-indexed verify without a registered committee");
   if (!indexed) HS_TRY(learn_process(c, stream));
-  if (c->ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(stream, c->ev_tables, 0));
+  if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(stream, c->learn.ev_tables, 0));
   const bool defer = c->deferred && stream != c->stream;  // host-pointer entry points (internal stream) always complete in stream order
   dev_buf &XYZ = (defer && c->flip) ? c->xyz2 : c->xyz, &META = (defer && c->flip) ? c->meta2 : c->meta;
   const int set = defer ? c->flip : 0;
@@ -1624,7 +1711,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_TRY(ensure(c, c->vidx, n * 4));
     HS_TRY(ensure(c, c->miss, n * 4));
   }
-  const pass_scratch S{(fe *)XYZ.p, (uint8_t *)META.p, (uint32_t *)c->vidx.p, (uint32_t *)c->miss.p, c->d_miss_count, c->stream_side,
+  const pass_scratch S{(fe *)XYZ.p.get(), (uint8_t *)META.p.get(), (uint32_t *)c->vidx.p.get(), (uint32_t *)c->miss.p.get(), c->d_miss_count, c->stream_side,
                        {c->ev_side[0], c->ev_side[1]}, c->profile_main ? c->ev_prof : nullptr};
   HS_TRY(launch_main(c, L, n, committee, indexed, S, stream, [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }));
   // small batches: small groups, so that enough blocks exist to hide each block's serial inversion; when the tail overlaps the next pass
@@ -1641,7 +1728,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_CUDA(c, cudaStreamWaitEvent(c->stream_tail, c->ev_main_done, 0));
     fin_stream = c->stream_tail;
   }
-  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p, (const uint8_t *)META.p, mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
+  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
   return HS_OK;
 }
@@ -1661,28 +1748,22 @@ static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
   }
   return HS_NO_KEY;
 }
-static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->d_atables; }
-// c->h_small_in[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
+static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->keys.atables; }
+// c->small.in.h[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
 // mapped host memory.
 static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, uint8_t *out_flags_or_null) {
-  small_rec *d_in = nullptr;
-  uint8_t *d_out = nullptr;
-  uint32_t *d_done = nullptr;
-  HS_CUDA(c, cudaHostGetDevicePointer(&d_in, c->h_small_in, 0));
-  HS_CUDA(c, cudaHostGetDevicePointer(&d_out, c->h_small_out, 0));
-  HS_CUDA(c, cudaHostGetDevicePointer(&d_done, c->h_small_done, 0));
   for (size_t i = 0; i < n; i++) {
-    c->h_small_in[i].req = 0;
-    c->h_small_in[i].req_n = (uint32_t)n;
+    c->small.in.h[i].req = 0;
+    c->small.in.h[i].req_n = (uint32_t)n;
   }
   const uint32_t seq = ++c->small_seq ? c->small_seq : ++c->small_seq;  // never 0
-  committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
-  if (c->ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_tables, 0));
-  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(d_in, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, d_out, c->d_small_counter, d_done, seq,
-                                                           sig_cache_dev{});
+  committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
+  if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->learn.ev_tables, 0));
+  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(c->small.in.d, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, c->small.out.d, c->small.counter,
+                                                           c->small.done.d, seq, sig_cache_dev{});
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  volatile uint32_t *done = c->h_small_done;
+  volatile uint32_t *done = c->small.done.h;
   bool finished = false;
   for (uint64_t spin = 0; spin < (1ull << 34); spin++) {
     if (*done == seq) {
@@ -1702,7 +1783,7 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
   for (size_t w = 0; w < (n + 31) / 32; w++) out_bitmap[w] = 0;
   const uint32_t want = (mode == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
   for (size_t i = 0; i < n; i++) {
-    const uint8_t fl = ((volatile uint8_t *)c->h_small_out)[i];
+    const uint8_t fl = ((volatile uint8_t *)c->small.out.h)[i];
     if (out_flags_or_null) out_flags_or_null[i] = fl;
     if (fl & want) out_bitmap[i >> 5] |= 1u << (i & 31);
   }
@@ -1803,29 +1884,51 @@ struct cert_req {
 struct cert_flight {  // the identical spans waiting on a span its primary request is verifying
   std::vector<std::pair<cert_req *, const cert_span *>> joiners;
 };
+// hs_queue_generic's lists (allocated whole on first use): a generic launch's ring slots at positions [lo, lo + records), and its
+// preimage requests' descriptors from position lo on.
+struct generic_lists {
+  mapped<uint32_t> slot;
+  mapped<qmsg_desc> mlist;
+};
+// hs_queue_sig_cache's bucket-mix key and HS_SIG_CTRS counters per ring slot, on the device and mapped (allocated whole on first use).
+struct sig_counters {
+  dev_mem<uint64_t> key;
+  dev_mem<uint32_t> ctr;
+  mapped<uint32_t> hctr;
+};
+// The batch lane's arena, scratch, streams and events (hs_queue_batch builds them whole, or not at all).
+struct batch_lane {
+  mapped<uint8_t> arena;    // request regions (inputs, then result words and the tail)
+  dev_mem<uint8_t> mirror;  // the inputs of the region in flight, at the same offsets
+  dev_mem<uint32_t> dig;    // the request's Digests, 32 bytes per preimage
+  dev_mem<fe> xyz;
+  dev_mem<uint8_t> meta, flags;
+  dev_mem<uint32_t> vidx, miss, miss_count, items, grej, counter;
+  stream_h stream, side;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
+  event_h ev[2];
+};
 struct hs_queue {
   hs_ctx *c = nullptr;
   uint32_t cap = 0, mask = 0;
-  small_rec *h_ring = nullptr, *d_ring = nullptr;  // mapped pinned: sig | msg | vidx | req | req_n per record
-  uint8_t *h_flags = nullptr, *d_flags = nullptr;  // mapped pinned: verdict flags per record
-  uint32_t *h_done = nullptr, *d_done = nullptr;   // mapped pinned: completion word per request slot (= launch sequence number)
-  uint32_t *d_counters = nullptr;                  // device: records finished per request slot
-  uint8_t *pk = nullptr, *d_pk = nullptr;          // mapped pinned: key bytes per record (32 B; resolved to a table index at
-                                                   // dispatch, read by k_queue_generic)
-  std::vector<uint8_t> modes;                     // HS_MODE_* per record (host only: picks the verdict flag of each record)
-  std::vector<uint32_t> wbits;                     // dispatcher thread only: verdict bitmap being assembled (cap bits)
-  cudaStream_t stream = nullptr;                   // k_verify_small launches: the device's highest priority
-  cudaStream_t bulk_stream = nullptr;              // k_verify_bulk launches: a lower priority, so votes never wait behind them
-  cudaEvent_t ev_last = nullptr;                   // recorded after every launch on `stream`: the ring is freed only after it
-  cudaEvent_t ev_bulk_last = nullptr;              // the same for `bulk_stream`
-  uint64_t stats[HS_QUEUE_STATS] = {};             // hs_queue_stats
+  mapped<small_rec> ring;                // sig | msg | vidx | req | req_n per record
+  mapped<uint8_t> flags;                 // verdict flags per record
+  mapped<uint32_t> done;                 // completion word per request slot (= launch sequence number)
+  dev_mem<uint32_t> d_counters;          // records finished per request slot
+  mapped<uint8_t> pk;                    // key bytes per record (32 B; resolved to a table index at dispatch, read by k_queue_generic)
+  std::vector<uint8_t> modes;            // HS_MODE_* per record (host only: picks the verdict flag of each record)
+  std::vector<uint32_t> wbits;           // dispatcher thread only: verdict bitmap being assembled (cap bits)
+  stream_h stream;                       // k_verify_small launches: the device's highest priority
+  stream_h bulk_stream;                  // k_verify_bulk launches: a lower priority, so votes never wait behind them
+  event_h ev_last;                       // recorded after every launch on `stream`: the ring is freed only after it
+  event_h ev_bulk_last;                  // the same for `bulk_stream`
+  uint64_t stats[HS_QUEUE_STATS] = {};   // hs_queue_stats
   // preimage requests (hs_queue_submit_msgs): a byte arena of HS_QUEUE_ARENA_PER_RECORD x cap bytes; a request's region is
   // released with its ring slots
   byte_ring arena;
-  uint8_t *h_arena = nullptr, *d_arena = nullptr;  // mapped pinned: the requests' regions (layout: qmsg_desc)
-  uint8_t *d_stage = nullptr;                      // device: k_queue_digests' copy of the arena (same offsets)
-  uint32_t *d_digs = nullptr;                      // device: digest slots, 32 bytes per 8 arena bytes
-  qmsg_desc *h_mlist = nullptr, *d_mlist = nullptr;  // mapped pinned: a launch's descriptors at the ring slots of its range
+  mapped<uint8_t> arena_buf;             // the requests' regions (layout: qmsg_desc)
+  dev_mem<uint8_t> d_stage;              // k_queue_digests' copy of the arena (same offsets)
+  dev_mem<uint32_t> d_digs;              // digest slots, 32 bytes per 8 arena bytes
+  mapped<qmsg_desc> mlist;               // a launch's descriptors at the ring slots of its range
   uint64_t dstats[HS_QUEUE_DIGEST_STATS] = {};     // hs_queue_digest_stats
   struct req {
     ticket_sink sink;
@@ -1860,11 +1963,10 @@ struct hs_queue {
   // generic requests dispatched meanwhile wait in gpend (ring positions, dispatcher thread only) for the next one
   std::atomic<bool> gen_on{false};
   std::deque<uint64_t> gpend;
-  uint32_t *h_gslot = nullptr, *d_gslot = nullptr;   // mapped pinned: a generic launch's ring slots at positions [lo, lo + records)
-  qmsg_desc *h_gmlist = nullptr, *d_gmlist = nullptr;  // mapped pinned: its preimage requests' descriptors, from position lo on
+  generic_lists gen_bufs;
   uint64_t gstats[HS_QUEUE_GENERIC_STATS] = {};      // hs_queue_generic_stats
   // batch lane (hs_queue_batch): off while b_max_items is 0.  Requests wait in bq in submit order, each with a region of the mapped
-  // arena h_barena (b_arena); a region is filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at
+  // arena lane.arena (b_arena); a region is filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at
   // a time (b_cur, dispatcher thread), and regions are released in request order when their requests complete.  The lane's buffers
   // and streams change only while the lane is off and bq is empty.
   struct breq {
@@ -1878,14 +1980,7 @@ struct hs_queue {
   };
   size_t b_max_items = 0, b_max_bytes = 0;
   byte_ring b_arena;
-  uint8_t *h_barena = nullptr, *d_barena = nullptr;  // mapped pinned: request regions (inputs, then result words and the tail)
-  uint8_t *d_bmirror = nullptr;                     // device: the inputs of the region in flight, at the same offsets
-  uint32_t *d_bdig = nullptr;                       // device: the request's Digests, 32 bytes per preimage
-  fe *d_bxyz = nullptr;
-  uint8_t *d_bmeta = nullptr, *d_bflags = nullptr;
-  uint32_t *d_bvidx = nullptr, *d_bmiss = nullptr, *d_bmiss_count = nullptr, *d_bitems = nullptr, *d_bgrej = nullptr, *d_bcounter = nullptr;
-  cudaStream_t b_stream = nullptr, b_side = nullptr;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
-  cudaEvent_t b_ev[2] = {nullptr, nullptr};
+  batch_lane lane;
   std::deque<breq> bq;
   breq *b_cur = nullptr;  // the request in flight (dispatcher thread; set and cleared under q->mu)
   uint32_t b_seq = 0;
@@ -1906,10 +2001,9 @@ struct hs_queue {
   uint64_t cstats[HS_QUEUE_CERT_STATS] = {};  // hs_queue_cert_stats ([5] is cc_bytes)
   // signature cache (hs_queue_sig_cache): off while d_sig is null.  The table, its key and bmask change only under c->mu after
   // both streams drained; sig_gen (also under mu) numbers the tables, so counts of a replaced table's launches are not held.
-  sig_bucket *d_sig = nullptr;
-  uint64_t *d_sig_key = nullptr;
+  dev_mem<sig_bucket> d_sig;
   uint32_t sig_bmask = 0, sig_gen = 0;
-  uint32_t *d_sig_ctr = nullptr, *h_sig_ctr = nullptr, *d_sig_hctr = nullptr;  // HS_SIG_CTRS per ring slot (allocated on first use)
+  sig_counters sigc;
   uint64_t sstats[HS_QUEUE_SIG_STATS] = {};  // hs_queue_sig_stats ([4]: inserts - evictions into the current table)
   std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
   std::condition_variable cv_work, cv_done;
@@ -2050,7 +2144,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   cudaError_t e = cudaSuccess;
   {
     std::lock_guard<std::mutex> g(c->mu);
-    const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables && c->small_enabled;
+    const bool committee = c->explicit_committee && c->n_keys > 0 && c->keys.atables && c->small_enabled;
     const bool gen = q->gen_on.load();  // hs_queue_generic writes it under c->mu
     if (!gen) {  // turned off with generic requests still waiting: they take the slow path, ahead of this range's
       for (uint64_t p : q->gpend) q->reqs[p & q->mask].gen = false;
@@ -2062,8 +2156,8 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       hs_queue::req &r = q->reqs[p & q->mask];
       bool all = committee;
       for (uint32_t i = 0; i < r.n; i++) {
-        small_rec &s = q->h_ring[(p + i) & q->mask];
-        s.vidx = all ? host_key_lookup(c, q->pk + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
+        small_rec &s = q->ring.h[(p + i) & q->mask];
+        s.vidx = all ? host_key_lookup(c, q->pk.h + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
         s.req = (uint32_t)(p & q->mask);
         s.req_n = r.n;
         if (s.vidx == HS_NO_KEY) all = false;
@@ -2072,7 +2166,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       const bool generic = gen && !all;
       r.gen = generic;
       if (!all) {  // every record of a slow-path request rides as HS_NO_KEY: none of them probes or fills the signature cache
-        for (uint32_t i = 0; i < r.n; i++) q->h_ring[(p + i) & q->mask].vidx = HS_NO_KEY;
+        for (uint32_t i = 0; i < r.n; i++) q->ring.h[(p + i) & q->mask].vidx = HS_NO_KEY;
         r.seq = 0;  // a generic request's launch number is set when its launch is built
         if (generic) q->gpend.push_back(p);
         else slow.push_back(p);
@@ -2094,7 +2188,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       p += r.n;
     }
     if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi, false});
-    committee_tables C{c->d_pks, c->d_key_flags, (uint32_t)c->n_keys, c->d_atables, c->a_table_entries};
+    committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
     ok.assign(runs.size(), 0);
     for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {  // pass 0: the small launches, pass 1: the bulk ones
       for (size_t k = 0; k < runs.size(); k++) {
@@ -2108,14 +2202,14 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
           if (!r.seq) continue;
           r.seq = L.seq;
           if (!r.msgs) continue;
-          q->h_mlist[(L.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
+          q->mlist.h[(L.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
           n_pre += r.m;
           n_pre_bytes += r.pre_bytes;
         }
         const uint32_t n = (uint32_t)(L.hi - L.lo), base = (uint32_t)(L.lo & q->mask);
         cudaStream_t s = L.bulk ? q->bulk_stream : q->stream;
         if (n_msgs_req) {  // the Digests first, on the verify launch's stream
-          k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, s>>>(q->d_mlist, base, q->mask, q->d_arena, q->d_stage, q->d_digs, q->d_ring);
+          k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, s>>>(q->mlist.d, base, q->mask, q->arena_buf.d, q->d_stage, q->d_digs, q->ring.d);
           c->launches++;
           e = cudaGetLastError();
           if (e == cudaSuccess) {
@@ -2127,18 +2221,18 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         if (e == cudaSuccess) {
           const unsigned bulk_blocks = (n + HS_BULK_THREADS - 1) / HS_BULK_THREADS;
           if (q->d_sig) {
-            const sig_cache_dev sc{q->d_sig, q->d_sig_key, q->sig_bmask, q->d_sig_ctr, q->d_sig_hctr};
+            const sig_cache_dev sc{q->d_sig, q->sigc.key, q->sig_bmask, q->sigc.ctr, q->sigc.hctr.d};
             L.sig_gen = q->sig_gen;
             if (L.bulk)
-              k_verify_bulk<true><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters,
-                                                                         q->d_done, L.seq, sc);
+              k_verify_bulk<true><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->ring.d, base, q->mask, n, c->d_btable, C, c->cp, q->flags.d, q->d_counters,
+                                                                         q->done.d, L.seq, sc);
             else
-              k_verify_small<true><<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq, sc);
+              k_verify_small<true><<<n, 64, 0, s>>>(q->ring.d, base, q->mask, c->d_btable, C, c->cp, q->flags.d, q->d_counters, q->done.d, L.seq, sc);
           } else if (L.bulk) {
-            k_verify_bulk<false><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->d_ring, base, q->mask, n, c->d_btable, C, c->cp, q->d_flags, q->d_counters,
-                                                                        q->d_done, L.seq, sig_cache_dev{});
+            k_verify_bulk<false><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->ring.d, base, q->mask, n, c->d_btable, C, c->cp, q->flags.d, q->d_counters,
+                                                                        q->done.d, L.seq, sig_cache_dev{});
           } else {
-            k_verify_small<false><<<n, 64, 0, s>>>(q->d_ring, base, q->mask, c->d_btable, C, c->cp, q->d_flags, q->d_counters, q->d_done, L.seq,
+            k_verify_small<false><<<n, 64, 0, s>>>(q->ring.d, base, q->mask, c->d_btable, C, c->cp, q->flags.d, q->d_counters, q->done.d, L.seq,
                                                    sig_cache_dev{});
           }
           c->launches++;
@@ -2165,17 +2259,17 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         hs_queue::req &r = q->reqs[p & q->mask];
         r.seq = G.seq;
         if (r.msgs) {
-          q->h_gmlist[(G.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
+          q->gen_bufs.mlist.h[(G.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
           n_pre += r.m;
           n_pre_bytes += r.pre_bytes;
         }
-        for (uint32_t i = 0; i < r.n; i++) q->h_gslot[(G.lo + g_recs++) & q->mask] = (uint32_t)((p + i) & q->mask);
+        for (uint32_t i = 0; i < r.n; i++) q->gen_bufs.slot.h[(G.lo + g_recs++) & q->mask] = (uint32_t)((p + i) & q->mask);
         G.hi = p + r.n;
       }
       const uint32_t base = (uint32_t)(G.lo & q->mask);
       const bool earlier_failure = e != cudaSuccess;
       if (e == cudaSuccess && n_msgs_req) {  // the Digests first, on the same stream
-        k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, q->bulk_stream>>>(q->d_gmlist, base, q->mask, q->d_arena, q->d_stage, q->d_digs, q->d_ring);
+        k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, q->bulk_stream>>>(q->gen_bufs.mlist.d, base, q->mask, q->arena_buf.d, q->d_stage, q->d_digs, q->ring.d);
         c->launches++;
         e = cudaGetLastError();
         if (e == cudaSuccess) {
@@ -2186,7 +2280,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       }
       if (e == cudaSuccess) {
         k_queue_generic<<<(unsigned)((g_recs + HS_GEN_THREADS - 1) / HS_GEN_THREADS), HS_GEN_THREADS, 0, q->bulk_stream>>>(
-            q->d_ring, q->d_pk, q->d_gslot, base, q->mask, (uint32_t)g_recs, c->d_btable, c->cp, q->d_flags, q->d_counters, q->d_done, G.seq);
+            q->ring.d, q->pk.d, q->gen_bufs.slot.d, base, q->mask, (uint32_t)g_recs, c->d_btable, c->cp, q->flags.d, q->d_counters, q->done.d, G.seq);
         c->launches++;
         e = cudaGetLastError();
       }
@@ -2241,11 +2335,11 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       idx.assign(r.n, 0);  // group_idx
       for (uint32_t i = 0; i < r.n; i++) {
         const uint32_t s = (uint32_t)((p + i) & q->mask);
-        memcpy(&msig[(size_t)i * 64], q->h_ring[s].sig, 64);
-        memcpy(&mpk[(size_t)i * 32], q->pk + 32 * (size_t)s, 32);
+        memcpy(&msig[(size_t)i * 64], q->ring.h[s].sig, 64);
+        memcpy(&mpk[(size_t)i * 32], q->pk.h + 32 * (size_t)s, 32);
         mmode[i] = q->modes[s];
       }
-      const uint8_t *a = q->h_arena + r.a_off;
+      const uint8_t *a = q->arena_buf.h + r.a_off;
       uint32_t group_bit = 0;
       rc = hs_verify_groups(c, a + qmsg_o_pre(r.m, r.n), reinterpret_cast<const uint64_t *>(a), r.m, msig.data(), mpk.data(), nullptr,
                             reinterpret_cast<const uint32_t *>(a + 8 * ((size_t)r.m + 1)), idx.data(), mmode.data(), r.n, 1, q->wbits.data(), &group_bit);
@@ -2257,9 +2351,9 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         const uint32_t s = (uint32_t)((p + i) & q->mask);
         if (q->modes[s] != mode) continue;
         hs_rec128 x;
-        memcpy(x.sig, q->h_ring[s].sig, 64);
-        memcpy(x.pk, q->pk + 32 * (size_t)s, 32);
-        memcpy(x.msg, q->h_ring[s].msg, 32);
+        memcpy(x.sig, q->ring.h[s].sig, 64);
+        memcpy(x.pk, q->pk.h + 32 * (size_t)s, 32);
+        memcpy(x.msg, q->ring.h[s].msg, 32);
         recs.push_back(x);
         idx.push_back(i);
       }
@@ -2303,7 +2397,7 @@ static void queue_watch(hs_queue *q) {
         hs_queue::req &r = q->reqs[p & q->mask];
         if (L.generic && !(r.gen && r.seq == L.seq)) continue;  // a request of another launch between its generic requests
         const bool mine = r.seq == L.seq && !r.finished;
-        if (((volatile uint32_t *)q->h_done)[p & q->mask] == L.seq) {
+        if (((volatile uint32_t *)q->done.h)[p & q->mask] == L.seq) {
           if (!mine) continue;
           std::atomic_thread_fence(std::memory_order_acquire);
           uint32_t *bits = q->wbits.data();
@@ -2311,10 +2405,10 @@ static void queue_watch(hs_queue *q) {
           for (uint32_t i = 0; i < r.n; i++) {  // the kernel writes both flags: each record's mode picks its verdict
             const uint32_t s = (uint32_t)((p + i) & q->mask);
             const uint32_t want = (q->modes[s] == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
-            if (((volatile uint8_t *)q->h_flags)[s] & want) bits[i >> 5] |= 1u << (i & 31);
+            if (((volatile uint8_t *)q->flags.h)[s] & want) bits[i >> 5] |= 1u << (i & 31);
           }
           if (L.sig_gen) {  // the completing block moved the request's signature-cache counts here before its completion word
-            const volatile uint32_t *sc = q->h_sig_ctr + HS_SIG_CTRS * (size_t)(p & q->mask);
+            const volatile uint32_t *sc = q->sigc.hctr.h + HS_SIG_CTRS * (size_t)(p & q->mask);
             for (int k = 0; k < HS_SIG_CTRS; k++) q->sstats[k] += sc[k];
             if (L.sig_gen == q->sig_gen) q->sstats[4] += sc[2] - sc[3];
           }
@@ -2373,9 +2467,9 @@ static void batch_complete(hs_queue *q, int status) {
       q->bstats[1] += r.n;
       q->bstats[2] += r.n_groups;
       q->bstats[3] += r.pre_bytes;
-      q->bstats[4] += reinterpret_cast<const volatile uint32_t *>(q->h_barena + r.a_off + r.o_tail)[0];
+      q->bstats[4] += reinterpret_cast<const volatile uint32_t *>(q->lane.arena.h + r.a_off + r.o_tail)[0];
     }
-    ticket_close_locked(q, r.sink, status, batch_bits(r.n_groups, r.n), reinterpret_cast<const uint32_t *>(q->h_barena + r.a_off + r.o_res), fire);
+    ticket_close_locked(q, r.sink, status, batch_bits(r.n_groups, r.n), reinterpret_cast<const uint32_t *>(q->lane.arena.h + r.a_off + r.o_res), fire);
     q->b_arena.release_to(r.a_end);
     q->b_cur = nullptr;
     q->bq.pop_front();
@@ -2389,25 +2483,25 @@ static void batch_complete(hs_queue *q, int status) {
 static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
   hs_ctx *c = q->c;
   std::lock_guard<std::mutex> g(c->mu);
-  cudaStream_t s = q->b_stream;
-  const uint8_t *m = q->d_bmirror + r.a_off;
-  HS_CUDA(c, cudaMemcpyAsync(q->d_bmirror + r.a_off, q->h_barena + r.a_off, r.o_res, cudaMemcpyHostToDevice, s));
-  k_digest32<<<blocks_for(r.n_msgs), HS_THREADS, 0, s>>>(m + r.o_pre, reinterpret_cast<const uint64_t *>(m), 0, r.n_msgs, q->d_bdig);
+  cudaStream_t s = q->lane.stream;
+  const uint8_t *m = q->lane.mirror + r.a_off;
+  HS_CUDA(c, cudaMemcpyAsync(q->lane.mirror + r.a_off, q->lane.arena.h + r.a_off, r.o_res, cudaMemcpyHostToDevice, s));
+  k_digest32<<<blocks_for(r.n_msgs), HS_THREADS, 0, s>>>(m + r.o_pre, reinterpret_cast<const uint64_t *>(m), 0, r.n_msgs, q->lane.dig);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  in_layout L{m + r.o_sig, 64, m + r.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(q->d_bdig), 32, reinterpret_cast<const uint32_t *>(m + r.o_mi),
+  in_layout L{m + r.o_sig, 64, m + r.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(q->lane.dig.get()), 32, reinterpret_cast<const uint32_t *>(m + r.o_mi),
               nullptr, 32, 0};
   // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
-  const bool committee = c->explicit_committee && c->n_keys > 0 && c->d_atables;
-  const pass_scratch S{q->d_bxyz, q->d_bmeta, q->d_bvidx, q->d_bmiss, q->d_bmiss_count, q->b_side, {q->b_ev[0], q->b_ev[1]}, nullptr};
+  const bool committee = c->explicit_committee && c->n_keys > 0 && c->keys.atables;
+  const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
   HS_TRY(launch_main(c, L, r.n, committee, false, S, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
-  HS_TRY(launch_finish(c, L, r.n, q->d_bxyz, q->d_bmeta, HS_MODE_STRICT, q->d_bitems, q->d_bflags, peer_route{}, fin_group, s));
-  HS_CUDA(c, cudaMemsetAsync(q->d_bgrej, 0, 4 * ((r.n_groups + 31) / 32), s));
-  uint8_t *res = q->d_barena + r.a_off;
-  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->d_bflags, m + r.o_mo, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->d_bgrej,
-                                                    reinterpret_cast<uint32_t *>(res + r.o_res), committee ? q->d_bmiss_count : nullptr,
-                                                    reinterpret_cast<uint32_t *>(res + r.o_tail), r.seq, q->d_bcounter);
+  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, q->lane.items, q->lane.flags, peer_route{}, fin_group, s));
+  HS_CUDA(c, cudaMemsetAsync(q->lane.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
+  uint8_t *res = q->lane.arena.d + r.a_off;
+  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->lane.flags, m + r.o_mo, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->lane.grej,
+                                                    reinterpret_cast<uint32_t *>(res + r.o_res), committee ? q->lane.miss_count.get() : nullptr,
+                                                    reinterpret_cast<uint32_t *>(res + r.o_tail), r.seq, q->lane.counter);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -2428,13 +2522,13 @@ static void batch_watch(hs_queue *q, bool query) {
   const hs_queue::breq &r = *q->b_cur;
   cudaError_t qe[2] = {cudaErrorNotReady, cudaErrorNotReady};
   if (query) {
-    qe[0] = cudaStreamQuery(q->b_stream);
-    qe[1] = cudaStreamQuery(q->b_side);
+    qe[0] = cudaStreamQuery(q->lane.stream);
+    qe[1] = cudaStreamQuery(q->lane.side);
   }
   int status = -1;
   for (cudaError_t x : qe)
     if (x != cudaSuccess && x != cudaErrorNotReady) status = fail(q->c, HS_ERR_CUDA, "verify queue batch pass", x);
-  if (status < 0 && reinterpret_cast<const volatile uint32_t *>(q->h_barena + r.a_off + r.o_tail)[1] == r.seq) {
+  if (status < 0 && reinterpret_cast<const volatile uint32_t *>(q->lane.arena.h + r.a_off + r.o_tail)[1] == r.seq) {
     std::atomic_thread_fence(std::memory_order_acquire);
     status = HS_OK;
   } else if (status < 0 && qe[0] == cudaSuccess && qe[1] == cudaSuccess) {
@@ -2443,27 +2537,10 @@ static void batch_watch(hs_queue *q, bool query) {
   if (status >= 0) batch_complete(q, status);
 }
 static bool batch_ready_locked(const hs_queue *q) { return !q->b_cur && !q->bq.empty() && q->bq.front().ready; }
-// Releases the lane's buffers and streams (the lane is off and drained).
-static void batch_free(hs_queue *q) {
-  for (cudaStream_t s : {q->b_stream, q->b_side})
-    if (s) {
-      cudaStreamSynchronize(s);
-      cudaStreamDestroy(s);
-    }
-  for (cudaEvent_t &ev : q->b_ev)
-    if (ev) cudaEventDestroy(ev);
-  if (q->h_barena) cudaFreeHost(q->h_barena);
-  for (void *p : {(void *)q->d_bmirror, (void *)q->d_bdig, (void *)q->d_bxyz, (void *)q->d_bmeta, (void *)q->d_bflags, (void *)q->d_bvidx,
-                  (void *)q->d_bmiss, (void *)q->d_bmiss_count, (void *)q->d_bitems, (void *)q->d_bgrej, (void *)q->d_bcounter})
-    cudaFree(p);
-  q->b_stream = q->b_side = nullptr;
-  q->b_ev[0] = q->b_ev[1] = nullptr;
-  q->h_barena = q->d_barena = q->d_bmirror = nullptr;
-  q->d_bdig = nullptr;
-  q->d_bxyz = nullptr;
-  q->d_bmeta = q->d_bflags = nullptr;
-  q->d_bvidx = q->d_bmiss = q->d_bmiss_count = q->d_bitems = q->d_bgrej = q->d_bcounter = nullptr;
-  q->b_arena = byte_ring{};
+// Waits for the lane's last pass (the lane is off and bq is empty): its buffers may be released after this.
+static void batch_drain(hs_queue *q) {
+  if (q->lane.stream) cudaStreamSynchronize(q->lane.stream);
+  if (q->lane.side) cudaStreamSynchronize(q->lane.side);
 }
 
 static size_t queue_small_inflight_locked(const hs_queue *q) {
@@ -2523,30 +2600,11 @@ static void queue_free(hs_queue *q) {
   q->cv_work.notify_all();
   if (q->th.joinable()) q->th.join();  // the thread finishes every request first
   cudaSetDevice(q->c->device);
-  for (cudaEvent_t ev : {q->ev_last, q->ev_bulk_last}) {  // the last launches' blocks have exited before the ring goes
-    if (!ev) continue;
-    cudaEventSynchronize(ev);
-    cudaEventDestroy(ev);
-  }
-  if (q->stream) cudaStreamDestroy(q->stream);
-  if (q->bulk_stream) cudaStreamDestroy(q->bulk_stream);
-  if (q->h_ring) cudaFreeHost(q->h_ring);
-  if (q->h_flags) cudaFreeHost(q->h_flags);
-  if (q->h_done) cudaFreeHost(q->h_done);
-  if (q->h_arena) cudaFreeHost(q->h_arena);
-  if (q->h_mlist) cudaFreeHost(q->h_mlist);
-  if (q->pk) cudaFreeHost(q->pk);
-  if (q->h_gslot) cudaFreeHost(q->h_gslot);
-  if (q->h_gmlist) cudaFreeHost(q->h_gmlist);
-  cudaFree(q->d_counters);
-  cudaFree(q->d_stage);
-  cudaFree(q->d_digs);
-  cudaFree(q->d_sig);
-  cudaFree(q->d_sig_key);
-  cudaFree(q->d_sig_ctr);
-  if (q->h_sig_ctr) cudaFreeHost(q->h_sig_ctr);
-  batch_free(q);
-  delete q;
+  // the last launches' blocks have exited before the ring goes
+  if (q->ev_last) cudaEventSynchronize(q->ev_last);
+  if (q->ev_bulk_last) cudaEventSynchronize(q->ev_bulk_last);
+  batch_drain(q);
+  delete q;  // the owners release the rest
 }
 
 // Digest of n fixed-size messages: staged/coalesced kernel when every message starts 16-byte aligned and has at least one
@@ -2593,37 +2651,36 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
   int sms = 0;
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   c->n_sms = (unsigned)sms;
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = create(c->stream);
+  if (e == cudaSuccess) e = create(c->stream2);
   if (e == cudaSuccess) {
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    e = cudaStreamCreateWithPriority(&c->stream_side, cudaStreamNonBlocking, hi);
+    e = create(c->stream_side, hi);
   }
   for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-    e = cudaEventCreateWithFlags(&c->ev[i], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_done[i], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_side[i], cudaEventDisableTiming);
+    e = create(c->ev[i]);
+    if (e == cudaSuccess) e = create(c->ev_done[i]);
+    if (e == cudaSuccess) e = create(c->ev_side[i]);
   }
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_miss_count, 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&c->h_miss_count, 4);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream_tail, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_main_done, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_results, cudaEventDisableTiming);
-  for (int i = 0; i < 2 && e == cudaSuccess; i++) e = cudaEventCreateWithFlags(&c->ev_tail[i], cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaHostAlloc(&c->h_small_in, HS_SMALL_MAX * sizeof(small_rec), cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&c->h_small_out, 256, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&c->h_small_done, 64, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_small_counter, 4);
-  if (e == cudaSuccess) e = cudaMemset(c->d_small_counter, 0, 4);
-  if (e == cudaSuccess) *c->h_small_done = 0;
+  if (e == cudaSuccess) e = alloc(c->d_miss_count, 4);
+  if (e == cudaSuccess) e = create(c->stream_tail);
+  if (e == cudaSuccess) e = create(c->ev_main_done);
+  if (e == cudaSuccess) e = create(c->ev_results);
+  for (int i = 0; i < 2 && e == cudaSuccess; i++) e = create(c->ev_tail[i]);
+  if (e == cudaSuccess) e = alloc(c->small.in, HS_SMALL_MAX * sizeof(small_rec));
+  if (e == cudaSuccess) e = alloc(c->small.out, 256);
+  if (e == cudaSuccess) e = alloc(c->small.done, 64);
+  if (e == cudaSuccess) e = alloc(c->small.counter, 4);
+  if (e == cudaSuccess) e = cudaMemset(c->small.counter, 0, 4);
+  if (e == cudaSuccess) *c->small.done.h = 0;
   c->small_enabled = !(getenv("HS_SMALL_PATH") && getenv("HS_SMALL_PATH")[0] == '0');
   set_window(c->cp, false, wb);
   set_window(c->cp, true, 12);
   c->wa_forced = (int)((flags >> 8) & 0xffu);
   if (const char *b = getenv("HS_TABLE_BUDGET_MB")) c->table_budget = (size_t)strtoull(b, nullptr, 10) << 20;
   c->cache_wanted = c->cache_enabled = !(flags & HS_FLAG_NO_KEY_CACHE) && !(getenv("HS_KEY_CACHE") && getenv("HS_KEY_CACHE")[0] == '0');
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_btable, sizeof(ge_niels) * comb_table_entries(wb));
+  if (e == cudaSuccess) e = alloc(c->d_btable, sizeof(ge_niels) * comb_table_entries(wb));
   if (e == cudaSuccess) {
     if (launch_build(c, nullptr, 1, 0, wb, c->cp.nb, c->d_btable, nullptr) != HS_OK) e = cudaGetLastError();
   }
@@ -2647,44 +2704,7 @@ void hs_ctx_destroy(hs_ctx *c) {
   for (hs_queue *q : qs) queue_free(q);  // completes their requests (callbacks fire) and joins their threads
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
-  cudaFree(c->d_btable);
-  cudaFree(c->d_pks);
-  cudaFree(c->d_key_flags);
-  cudaFree(c->d_atables);
-  cudaFree(c->d_slots);
-  cudaFree(c->d_miss_count);
-  if (c->h_miss_count) cudaFreeHost(c->h_miss_count);
-  cudaFree(c->xyz2.p);
-  cudaFree(c->meta2.p);
-  for (cudaEvent_t ev : {c->ev_main_done, c->ev_tail[0], c->ev_tail[1], c->ev_results})
-    if (ev) cudaEventDestroy(ev);
-  if (c->stream_tail) cudaStreamDestroy(c->stream_tail);
-  if (c->h_small_in) cudaFreeHost(c->h_small_in);
-  if (c->h_small_out) cudaFreeHost(c->h_small_out);
-  if (c->h_small_done) cudaFreeHost(c->h_small_done);
-  cudaFree(c->d_small_counter);
-  for (dev_buf *b : {&c->in[0], &c->in[1], &c->digest[0], &c->digest[1], &c->xyz, &c->meta, &c->vidx, &c->miss, &c->out}) cudaFree(b->p);
-  cudaFree(c->d_learn_keys);
-  cudaFree(c->d_learn_n);
-  if (c->h_learn_keys) cudaFreeHost(c->h_learn_keys);
-  if (c->h_learn_n) cudaFreeHost(c->h_learn_n);
-  if (c->h_miss_total) cudaFreeHost(c->h_miss_total);
-  if (c->ev_learn) cudaEventDestroy(c->ev_learn);
-  if (c->ev_tables) cudaEventDestroy(c->ev_tables);
-  for (int i = 0; i < 2; i++)
-    if (c->ev_prof[i]) cudaEventDestroy(c->ev_prof[i]);
-  for (int p = 0; p < HS_MAX_PEERS; p++)
-    if (c->peer_mapped[p]) cudaIpcCloseMemHandle(c->peer_mapped[p]);
-  cudaFree(c->peer_own);
-  for (int i = 0; i < 2; i++) {
-    if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-    if (c->ev_done[i]) cudaEventDestroy(c->ev_done[i]);
-    if (c->ev_side[i]) cudaEventDestroy(c->ev_side[i]);
-  }
-  if (c->stream_side) cudaStreamDestroy(c->stream_side);
-  if (c->stream) cudaStreamDestroy(c->stream);
-  if (c->stream2) cudaStreamDestroy(c->stream2);
-  delete c;
+  delete c;  // the owners release the rest
 }
 
 const char *hs_last_error(const hs_ctx *c) { return c ? c->err.c_str() : "null context"; }
@@ -2721,7 +2741,7 @@ int hs_profile_enable(hs_ctx *c, int on) {
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
   for (int i = 0; i < 2 && on; i++)
-    if (!c->ev_prof[i]) HS_CUDA(c, cudaEventCreate(&c->ev_prof[i]));
+    if (!c->ev_prof[i]) HS_CUDA(c, create(c->ev_prof[i], cudaEventDefault));
   c->profile_main = on != 0;
   return HS_OK;
 }
@@ -2791,25 +2811,26 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
     if (capk * comb_table_entries(w) * sizeof(ge_niels) <= budget) break;
   }
   if (sc_ndigits_rt(wa) + c->cp.nb > HS_MAX_DIGITS) return fail(c, HS_ERR_ARG, "window combination exceeds HS_MAX_DIGITS");
-  cudaError_t e = cudaMalloc(&c->d_pks, capk * 32);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_key_flags, capk);
-  if (e == cudaSuccess) e = cudaMemset(c->d_key_flags, 0, capk);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_slots, (size_t)cap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_atables, capk * sizeof(ge_niels) * comb_table_entries(wa));
+  key_store K;  // the old tables were released above
+  cudaError_t e = alloc(K.pks, capk * 32);
+  if (e == cudaSuccess) e = alloc(K.key_flags, capk);
+  if (e == cudaSuccess) e = cudaMemset(K.key_flags, 0, capk);
+  if (e == cudaSuccess) e = alloc(K.slots, (size_t)cap * 4);
+  if (e == cudaSuccess) e = alloc(K.atables, capk * sizeof(ge_niels) * comb_table_entries(wa));
   if (e != cudaSuccess) {
     cudaGetLastError();
-    cache_release(c);
     return fail(c, HS_ERR_NOMEM, "committee tables do not fit in device memory", e);
   }
+  c->keys = std::move(K);
   set_window(c->cp, true, wa);
   c->a_table_entries = comb_table_entries(wa);
   int rc = HS_OK;
-  e = cudaMemcpyAsync(c->d_pks, pks, N * 32, cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) rc = launch_build(c, c->d_pks, N, 1, wa, c->cp.na, c->d_atables, c->d_key_flags);
+  e = cudaMemcpyAsync(c->keys.pks, pks, N * 32, cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(c->keys.slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags);
   if (e == cudaSuccess && rc == HS_OK) e = cudaStreamSynchronize(c->stream);
   std::vector<uint8_t> fl(N);
-  if (e == cudaSuccess && rc == HS_OK) e = cudaMemcpy(fl.data(), c->d_key_flags, N, cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess && rc == HS_OK) e = cudaMemcpy(fl.data(), c->keys.key_flags, N, cudaMemcpyDeviceToHost);
   if (e != cudaSuccess || rc != HS_OK) {
     cache_release(c);
     return rc != HS_OK ? rc : fail(c, HS_ERR_CUDA, "committee registration", e);
@@ -2847,7 +2868,7 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
     if (remove_idx[i] >= c->n_keys) return fail(c, HS_ERR_ARG, "hs_committee_update: remove index out of range");
   for (size_t i = 0; i < n_remove; i++) {
     c->h_key_live[remove_idx[i]] = 0;
-    HS_CUDA(c, cudaMemsetAsync(c->d_key_flags + remove_idx[i], 0, 1, c->stream));
+    HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + remove_idx[i], 0, 1, c->stream));
   }
   auto find = [&](const uint8_t *key) -> uint32_t {
     uint32_t w[8];
@@ -2877,8 +2898,8 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
       } else return fail(c, HS_ERR_NOMEM, "hs_committee_update: no free table slot (re-register the committee)");
       memcpy(c->h_pks.data() + 32 * (size_t)idx, key, 32);
       c->h_key_live[idx] = 1;
-      HS_CUDA(c, cudaMemcpyAsync(c->d_pks + 32 * (size_t)idx, key, 32, cudaMemcpyHostToDevice, c->stream));
-      HS_TRY(launch_build(c, c->d_pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->d_atables + (size_t)idx * c->a_table_entries, c->d_key_flags + idx));
+      HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)idx, key, 32, cudaMemcpyHostToDevice, c->stream));
+      HS_TRY(launch_build(c, c->keys.pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->keys.atables + (size_t)idx * c->a_table_entries, c->keys.key_flags + idx));
       added.push_back(idx);
     }
     out_add_idx[i] = idx;
@@ -2900,7 +2921,7 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
     }
     if (!dup) c->h_slots[h] = (uint32_t)i;
   }
-  HS_CUDA(c, cudaMemcpyAsync(c->d_slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaStreamSynchronize(c->stream));
   return HS_OK;
 }
@@ -2979,8 +3000,8 @@ int hs_verify_qcs(hs_ctx *c, const uint8_t *preimages, size_t n_qc, const uint8_
                o_qi = o_key + ((n_votes * key_bytes + 15) & ~(size_t)15), total = o_qi + n_votes * 4;
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, (vote_words + qc_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
-  uint32_t *d_votes = (uint32_t *)c->out.p, *d_qc = d_votes + vote_words;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  uint32_t *d_votes = (uint32_t *)c->out.p.get(), *d_qc = d_votes + vote_words;
   HS_CUDA(c, cudaMemcpyAsync(d + o_pre, preimages, n_qc * 40, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_votes * 64, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_key, pk ? (const void *)pk : (const void *)vidx, n_votes * key_bytes, cudaMemcpyHostToDevice, c->stream));
@@ -3048,8 +3069,8 @@ int hs_verify_tcs(hs_ctx *c, const uint64_t *tc_rounds, size_t n_tc, const uint8
                o_key = o_sig + n_votes * 64, o_ti = o_key + ((n_votes * key_bytes + 15) & ~(size_t)15), total = o_ti + n_votes * 4;
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, (vote_words + tc_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
-  uint32_t *d_votes = (uint32_t *)c->out.p, *d_tc = d_votes + vote_words;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  uint32_t *d_votes = (uint32_t *)c->out.p.get(), *d_tc = d_votes + vote_words;
   HS_CUDA(c, cudaMemcpyAsync(d + o_r, tc_rounds, n_tc * 8, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_hq, high_qc_rounds, n_votes * 8, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_votes * 64, cudaMemcpyHostToDevice, c->stream));
@@ -3098,8 +3119,8 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
                total = o_fl + al(n_items);
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, (i_words + g_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
-  uint32_t *d_items = (uint32_t *)c->out.p, *d_groups = d_items + i_words;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  uint32_t *d_items = (uint32_t *)c->out.p.get(), *d_groups = d_items + i_words;
   HS_CUDA(c, cudaMemcpyAsync(d + o_off, pre_off, (n_msgs + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   if (pre_bytes) HS_CUDA(c, cudaMemcpyAsync(d + o_pre, preimages, pre_bytes, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_items * 64, cudaMemcpyHostToDevice, c->stream));
@@ -3169,7 +3190,7 @@ int hs_sign_digests(hs_ctx *c, const uint8_t *seeds, const uint8_t *pks, size_t 
   const size_t o_seed = 0, o_pk = n_keys * 32, o_ki = o_pk + n_keys * 32, o_d = o_ki + ((n * 4 + 15) & ~(size_t)15), total = o_d + n * 32;
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, n * 64));
-  uint8_t *d = (uint8_t *)c->in[0].p;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
   HS_CUDA(c, cudaMemcpyAsync(d + o_seed, seeds, n_keys * 32, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_pk, pks, n_keys * 32, cudaMemcpyHostToDevice, c->stream));
   if (key_idx) HS_CUDA(c, cudaMemcpyAsync(d + o_ki, key_idx, n * 4, cudaMemcpyHostToDevice, c->stream));
@@ -3186,32 +3207,29 @@ int hs_peer_setup(hs_ctx *c, int rank, int world, size_t total_words, uint8_t ha
     return fail(c, HS_ERR_ARG, "hs_peer_setup: bad argument (total_words must be a multiple of world)");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  if (c->peer_own) {  // a new geometry (another workload): drop the old buffers.  Every rank must have drained its stream first.
+  if (c->peer.own) {  // a new geometry (another workload): drop the old buffers.  Every rank must have drained its stream first.
     HS_CUDA(c, cudaDeviceSynchronize());
-    for (int p = 0; p < HS_MAX_PEERS; p++)
-      if (c->peer_mapped[p]) {
-        cudaIpcCloseMemHandle(c->peer_mapped[p]);
-        c->peer_mapped[p] = nullptr;
-      }
-    cudaFree(c->peer_own);
-    c->peer_own = nullptr;
+    c->peer = {};  // nothing points at them after this: a failure below leaves peer routing unset
+    c->peers = peer_route{};
     c->peer_epoch = 0;
     c->peer_armed = false;
   }
   const size_t bytes = (2 * total_words + HS_MAX_PEERS + 16) * 4;
-  HS_CUDA(c, cudaMalloc(&c->peer_own, bytes));
-  HS_CUDA(c, cudaMemset(c->peer_own, 0, bytes));
+  dev_mem<uint32_t> own;
+  HS_CUDA(c, alloc(own, bytes));
+  HS_CUDA(c, cudaMemset(own, 0, bytes));
   cudaIpcMemHandle_t h;
-  HS_CUDA(c, cudaIpcGetMemHandle(&h, c->peer_own));
+  HS_CUDA(c, cudaIpcGetMemHandle(&h, own));
   static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
   memcpy(handle_out, &h, 64);
+  c->peer.own = std::move(own);
   c->peer_rank = rank;
   c->peer_total_words = total_words;
   c->peers = peer_route{};
   c->peers.n = world;
   c->peers.my_rank = rank;
   c->peers.total_words = total_words;
-  c->peers.buf[rank] = c->peer_own;
+  c->peers.buf[rank] = c->peer.own;
   return HS_OK;
 }
 int hs_peer_open(hs_ctx *c, int peer_rank, const uint8_t handle[64]) {
@@ -3220,15 +3238,16 @@ int hs_peer_open(hs_ctx *c, int peer_rank, const uint8_t handle[64]) {
   HS_CUDA(c, cudaSetDevice(c->device));
   cudaIpcMemHandle_t h;
   memcpy(&h, handle, 64);
-  void *p = nullptr;
-  HS_CUDA(c, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-  c->peer_mapped[peer_rank] = p;
-  c->peers.buf[peer_rank] = (uint32_t *)p;
+  ipc_mapping &m = c->peer.mapped[peer_rank];
+  if (m) HS_CUDA(c, cudaDeviceSynchronize());  // reopened: a pass may still write through the earlier mapping, closed below
+  c->peers.buf[peer_rank] = nullptr;
+  HS_CUDA(c, ipc_open(m, h));
+  c->peers.buf[peer_rank] = static_cast<uint32_t *>(m.get());
   return HS_OK;
 }
 /* Arms the NEXT `_dev` verify call on this context: its bitmap goes to every rank's buffer at word_offset (fused all-gather). */
 int hs_peer_next(hs_ctx *c, size_t word_offset, uint32_t epoch) {
-  if (!c || !c->peer_own) return fail(c, HS_ERR_ARG, "hs_peer_next: peers not set up");
+  if (!c || !c->peer.own) return fail(c, HS_ERR_ARG, "hs_peer_next: peers not set up");
   std::lock_guard<std::mutex> g(c->mu);
   for (int p = 0; p < c->peers.n; p++)
     if (!c->peers.buf[p]) return fail(c, HS_ERR_ARG, "hs_peer_next: a peer buffer is not mapped");
@@ -3241,12 +3260,12 @@ int hs_peer_next(hs_ctx *c, size_t word_offset, uint32_t epoch) {
   return HS_OK;
 }
 /* Device pointer of this rank's copy of the full bitmap of the most recently armed epoch, and whether a peer wait ever timed out. */
-void *hs_peer_bitmap(hs_ctx *c) { return (c && c->peer_own) ? (void *)(c->peer_own + (size_t)(c->peer_epoch & 1u) * c->peer_total_words) : nullptr; }
+void *hs_peer_bitmap(hs_ctx *c) { return (c && c->peer.own) ? (void *)(c->peer.own + (size_t)(c->peer_epoch & 1u) * c->peer_total_words) : nullptr; }
 int hs_peer_timed_out(hs_ctx *c) {
-  if (!c || !c->peer_own) return 0;
+  if (!c || !c->peer.own) return 0;
   uint32_t v = 0;
   cudaSetDevice(c->device);
-  cudaMemcpy(&v, c->peer_own + 2 * c->peer_total_words + HS_MAX_PEERS, 4, cudaMemcpyDeviceToHost);
+  cudaMemcpy(&v, c->peer.own + 2 * c->peer_total_words + HS_MAX_PEERS, 4, cudaMemcpyDeviceToHost);
   return (int)v;
 }
 
@@ -3269,9 +3288,9 @@ int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, 
       const uint32_t idx = host_key_lookup(c, recs[i].pk);
       if (idx == HS_NO_KEY) all = false;
       else {
-        memcpy(c->h_small_in[i].sig, recs[i].sig, 64);
-        memcpy(c->h_small_in[i].msg, recs[i].msg, 32);
-        c->h_small_in[i].vidx = idx;
+        memcpy(c->small.in.h[i].sig, recs[i].sig, 64);
+        memcpy(c->small.in.h[i].msg, recs[i].msg, 32);
+        c->small.in.h[i].vidx = idx;
       }
     }
     if (all) return run_small(c, n, mode, out_bitmap, nullptr);
@@ -3279,7 +3298,7 @@ int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, 
   HS_TRY(ensure(c, c->in[0], n * sizeof(hs_rec128)));
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
   HS_CUDA(c, cudaMemcpyAsync(c->in[0].p, recs, n * sizeof(hs_rec128), cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(run_verify(c, layout_rec128(c->in[0].p), n, mode, (uint32_t *)c->out.p, c->stream, false));
+  HS_TRY(run_verify(c, layout_rec128(c->in[0].p), n, mode, (uint32_t *)c->out.p.get(), c->stream, false));
   return finish_bitmap(c, n, out_bitmap);
 }
 int hs_verify_strict_batch(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t *out_bitmap) {
@@ -3298,13 +3317,13 @@ int hs_verify_var(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint8_
   size_t o_sig = 0, o_pk = n * 64, o_off = o_pk + n * 32, o_msg = o_off + (n + 1) * 8, total = o_msg + off[n];
   HS_TRY(ensure(c, c->in[0], total + 8));
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
   HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n * 64, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_pk, pk, n * 32, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   if (off[n]) HS_CUDA(c, cudaMemcpyAsync(d + o_msg, msgs, off[n], cudaMemcpyHostToDevice, c->stream));
   in_layout L{d + o_sig, 64, d + o_pk, 32, nullptr, d + o_msg, 0, nullptr, (const uint64_t *)(d + o_off), 0, 0};
-  HS_TRY(run_verify(c, L, n, mode, (uint32_t *)c->out.p, c->stream, false));
+  HS_TRY(run_verify(c, L, n, mode, (uint32_t *)c->out.p.get(), c->stream, false));
   return finish_bitmap(c, n, out_bitmap);
 }
 
@@ -3324,9 +3343,9 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
       const uint32_t idx = host_key_lookup(c, votes[i].pk);
       if (idx == HS_NO_KEY) all = false;
       else {
-        memcpy(c->h_small_in[i].sig, votes[i].sig, 64);
-        memcpy(c->h_small_in[i].msg, digest, 32);
-        c->h_small_in[i].vidx = idx;
+        memcpy(c->small.in.h[i].sig, votes[i].sig, 64);
+        memcpy(c->small.in.h[i].msg, digest, 32);
+        c->small.in.h[i].vidx = idx;
       }
     }
     if (all) {
@@ -3343,11 +3362,11 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
   }
   HS_TRY(ensure(c, c->in[0], n * sizeof(hs_vote) + 32));
   HS_TRY(ensure(c, c->out, words * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
   HS_CUDA(c, cudaMemcpyAsync(d, digest, 32, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + 32, votes, n * sizeof(hs_vote), cudaMemcpyHostToDevice, c->stream));
   in_layout L{d + 32 + 32, sizeof(hs_vote), d + 32, sizeof(hs_vote), nullptr, d, 0, nullptr, nullptr, 32, 0};
-  HS_TRY(run_verify(c, L, n, HS_MODE_BATCH_EQ, (uint32_t *)c->out.p, c->stream, false));
+  HS_TRY(run_verify(c, L, n, HS_MODE_BATCH_EQ, (uint32_t *)c->out.p.get(), c->stream, false));
   std::vector<uint32_t> tmp;
   uint32_t *bm = out_bitmap_or_null;
   if (!bm) {
@@ -3374,16 +3393,16 @@ int hs_verify_committee(hs_ctx *c, const uint32_t *vidx, const uint8_t *sig, con
   HS_CUDA(c, cudaSetDevice(c->device));
   if (small_eligible(c, n) && c->explicit_committee) {  // latency path
     for (size_t i = 0; i < n; i++) {
-      memcpy(c->h_small_in[i].sig, sig + 64 * i, 64);
-      memcpy(c->h_small_in[i].msg, digests + 32 * (size_t)(midx ? midx[i] : 0), 32);
-      c->h_small_in[i].vidx = vidx[i];
+      memcpy(c->small.in.h[i].sig, sig + 64 * i, 64);
+      memcpy(c->small.in.h[i].msg, digests + 32 * (size_t)(midx ? midx[i] : 0), 32);
+      c->small.in.h[i].vidx = vidx[i];
     }
     return run_small(c, n, mode, out_bitmap, nullptr);
   }
   size_t o_sig = 0, o_v = n * 64, o_m = o_v + n * 4, o_d = o_m + (midx ? n * 4 : 0), total = o_d + n_msgs * 32;
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
   HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n * 64, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_v, vidx, n * 4, cudaMemcpyHostToDevice, c->stream));
   if (midx) HS_CUDA(c, cudaMemcpyAsync(d + o_m, midx, n * 4, cudaMemcpyHostToDevice, c->stream));
@@ -3402,12 +3421,12 @@ int hs_digest32_batch(hs_ctx *c, const uint8_t *data, const uint64_t *off, size_
   size_t o_off = 0, o_data = (n + 1) * 8, total = o_data + off[n];
   HS_TRY(ensure(c, c->in[0], total + 8));
   HS_TRY(ensure(c, c->out, n * 32));
-  uint8_t *d = (uint8_t *)c->in[0].p;
+  uint8_t *d = (uint8_t *)c->in[0].p.get();
   HS_CUDA(c, cudaMemcpyAsync(d + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   if (off[n]) HS_CUDA(c, cudaMemcpyAsync(d + o_data, data, off[n], cudaMemcpyHostToDevice, c->stream));
   if (n <= 64 && off[n] / n >= 1024) {
     // a few long messages (mempool batches): one warp per message, schedules expanded in parallel across lanes
-    k_digest32_long<<<(unsigned)n, 32, 0, c->stream>>>(d + o_data, (const uint64_t *)(d + o_off), n, (uint32_t *)c->out.p);
+    k_digest32_long<<<(unsigned)n, 32, 0, c->stream>>>(d + o_data, (const uint64_t *)(d + o_off), n, (uint32_t *)c->out.p.get());
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
   } else {
@@ -3457,7 +3476,7 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
     const int b = (int)(j & 1);
     const size_t want = (j == 0 && first) ? first : CH;
     const size_t cnt = (n - lo < want) ? (n - lo) : want;
-    uint8_t *d = (uint8_t *)c->in[b].p;
+    uint8_t *d = (uint8_t *)c->in[b].p.get();
     const size_t o_sig = 0, o_key = cnt * 64, o_msg = o_key + ((cnt * key_bytes + 15) & ~(size_t)15);
     if (j >= 2) HS_CUDA(c, cudaStreamWaitEvent(c->stream2, c->ev_done[b], 0));  // staging buffer b is free again
     HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig + lo * 64, cnt * 64, cudaMemcpyHostToDevice, c->stream2));
@@ -3467,7 +3486,7 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
     HS_CUDA(c, cudaEventRecord(c->ev[b], c->stream2));
     HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev[b], 0));
     HS_TRY(hs_verify_msgs_dev(c, d + o_sig, vidx ? nullptr : d + o_key, vidx ? d + o_key : nullptr, d + o_msg, msg_len, cnt, mode,
-                              c->digest[b].p, (uint32_t *)c->out.p + lo / 32, c->stream));
+                              c->digest[b].p, (uint32_t *)c->out.p.get() + lo / 32, c->stream));
     HS_CUDA(c, cudaEventRecord(c->ev_done[b], c->stream));
     lo += cnt;
   }
@@ -3481,7 +3500,7 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   uint32_t cap = HS_SMALL_MAX;  // a request of 64 records must fit
   while (cap < (ring_records ? ring_records : HS_QUEUE_DEFAULT_RECORDS)) cap <<= 1;
   HS_CUDA(c, cudaSetDevice(c->device));
-  hs_queue *q = new (std::nothrow) hs_queue();
+  std::unique_ptr<hs_queue> q(new (std::nothrow) hs_queue());  // on failure below, its owners release what was allocated
   if (!q) return fail(c, HS_ERR_NOMEM, "hs_queue_create: out of host memory");
   q->c = c;
   q->cap = cap;
@@ -3492,43 +3511,33 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   q->reqs.assign(cap, hs_queue::req{});
   int lo = 0, hi = 0;
   cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->stream, cudaStreamNonBlocking, hi);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->bulk_stream, cudaStreamNonBlocking, lo);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->ev_last, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->ev_bulk_last, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_ring, (size_t)cap * sizeof(small_rec), cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_flags, cap, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_done, (size_t)cap * 4, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_counters, (size_t)cap * 4);
+  if (e == cudaSuccess) e = create(q->stream, hi);
+  if (e == cudaSuccess) e = create(q->bulk_stream, lo);
+  if (e == cudaSuccess) e = create(q->ev_last);
+  if (e == cudaSuccess) e = create(q->ev_bulk_last);
+  if (e == cudaSuccess) e = alloc(q->ring, (size_t)cap * sizeof(small_rec));
+  if (e == cudaSuccess) e = alloc(q->flags, cap);
+  if (e == cudaSuccess) e = alloc(q->done, (size_t)cap * 4);
+  if (e == cudaSuccess) e = alloc(q->d_counters, (size_t)cap * 4);
   if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_arena, q->arena.cap, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_mlist, (size_t)cap * sizeof(qmsg_desc), cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->pk, (size_t)cap * 32, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_stage, q->arena.cap);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_digs, q->arena.cap * 4);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_ring, q->h_ring, 0);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_flags, q->h_flags, 0);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_done, q->h_done, 0);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_arena, q->h_arena, 0);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_mlist, q->h_mlist, 0);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_pk, q->pk, 0);
-  if (e != cudaSuccess) {
-    queue_free(q);
-    return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
-  }
-  memset(q->h_done, 0, (size_t)cap * 4);
-  memset(q->pk, 0, (size_t)cap * 32);
+  if (e == cudaSuccess) e = alloc(q->arena_buf, q->arena.cap);
+  if (e == cudaSuccess) e = alloc(q->mlist, (size_t)cap * sizeof(qmsg_desc));
+  if (e == cudaSuccess) e = alloc(q->pk, (size_t)cap * 32);
+  if (e == cudaSuccess) e = alloc(q->d_stage, q->arena.cap);
+  if (e == cudaSuccess) e = alloc(q->d_digs, q->arena.cap * 4);
+  if (e != cudaSuccess) return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
+  memset(q->done.h, 0, (size_t)cap * 4);
+  memset(q->pk.h, 0, (size_t)cap * 32);
   try {
-    q->th = std::thread(queue_main, q);
+    q->th = std::thread(queue_main, q.get());
   } catch (...) {
-    queue_free(q);
     return fail(c, HS_ERR_NOMEM, "hs_queue_create: cannot start the dispatcher thread");
   }
   {
     std::lock_guard<std::mutex> g(c->queues_mu);
-    c->queues.push_back(q);
+    c->queues.push_back(q.get());
   }
-  *out = q;
+  *out = q.release();
   return HS_OK;
 }
 
@@ -3548,9 +3557,9 @@ static int queue_put_recs_locked(hs_queue *q, const char *what, const hs_rec128 
   for (size_t k = 0; k < sel.n; k++) {
     const size_t i = sel[k];
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
-    memcpy(q->h_ring[s].sig, recs[i].sig, 64);
-    memcpy(q->h_ring[s].msg, recs[i].msg, 32);
-    memcpy(q->pk + 32 * (size_t)s, recs[i].pk, 32);
+    memcpy(q->ring.h[s].sig, recs[i].sig, 64);
+    memcpy(q->ring.h[s].msg, recs[i].msg, 32);
+    memcpy(q->pk.h + 32 * (size_t)s, recs[i].pk, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)mode;
   }
   r.n = (uint32_t)sel.n;
@@ -3580,7 +3589,7 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
   const std::optional<uint64_t> start = q->arena.take(size);
   if (!start) return HS_ERR_NOMEM;
   if (q->tail - q->head + n > q->cap) return HS_ERR_NOMEM;  // ring full: back-pressure, not an engine failure
-  uint8_t *a = q->h_arena + q->arena.off(*start);
+  uint8_t *a = q->arena_buf.h + q->arena.off(*start);
   uint64_t *off = reinterpret_cast<uint64_t *>(a);
   uint32_t *idx = reinterpret_cast<uint32_t *>(a + 8 * ((size_t)m + 1));
   uint8_t *pre = a + qmsg_o_pre(m, n);
@@ -3595,8 +3604,8 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
   for (size_t k = 0; k < n; k++) {
     const size_t i = sel[k];
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
-    memcpy(q->h_ring[s].sig, sig + 64 * i, 64);
-    memcpy(q->pk + 32 * (size_t)s, pk + 32 * i, 32);
+    memcpy(q->ring.h[s].sig, sig + 64 * i, 64);
+    memcpy(q->pk.h + 32 * (size_t)s, pk + 32 * i, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
     idx[k] = remap[msg_idx[i]];
   }
@@ -3837,45 +3846,35 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries) {
   // Drains the queue's streams: no launch that probes the old table survives these lines.
   HS_CUDA(c, cudaStreamSynchronize(q->stream));
   HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));
-  cudaFree(q->d_sig);
-  q->d_sig = nullptr;
+  q->d_sig.reset();
   {
     std::lock_guard<std::mutex> gq(q->mu);
     q->sig_gen++;
     q->sstats[4] = 0;
   }
   if (!buckets) return HS_OK;
-  if (!q->d_sig_ctr) {  // first use: the per-slot counters and the bucket mix's key (random per queue)
+  if (!q->sigc.ctr) {  // first use: the per-slot counters and the bucket mix's key (random per queue)
     uint64_t key[32];
     std::random_device rd;
     for (uint64_t &k : key) k = ((uint64_t)rd() << 32) ^ rd();
     const size_t cb = (size_t)q->cap * HS_SIG_CTRS * 4;
-    cudaError_t e = cudaMalloc(&q->d_sig_key, sizeof(key));
-    if (e == cudaSuccess) e = cudaMemcpy(q->d_sig_key, key, sizeof(key), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaHostAlloc(&q->h_sig_ctr, cb, cudaHostAllocMapped);
-    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_sig_hctr, q->h_sig_ctr, 0);
-    if (e == cudaSuccess) e = cudaMalloc(&q->d_sig_ctr, cb);
-    if (e == cudaSuccess) e = cudaMemsetAsync(q->d_sig_ctr, 0, cb, q->stream);
-    if (e != cudaSuccess) {  // the cache stays off; a later call starts the first use over
-      cudaFree(q->d_sig_key);
-      cudaFree(q->d_sig_ctr);
-      if (q->h_sig_ctr) cudaFreeHost(q->h_sig_ctr);
-      q->d_sig_key = nullptr;
-      q->d_sig_ctr = q->h_sig_ctr = q->d_sig_hctr = nullptr;
-      return fail(c, HS_ERR_CUDA, "hs_queue_sig_cache", e);
-    }
+    sig_counters S;
+    cudaError_t e = alloc(S.key, sizeof(key));
+    if (e == cudaSuccess) e = cudaMemcpy(S.key, key, sizeof(key), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = alloc(S.hctr, cb);
+    if (e == cudaSuccess) e = alloc(S.ctr, cb);
+    if (e == cudaSuccess) e = cudaMemsetAsync(S.ctr, 0, cb, q->stream);
+    if (e != cudaSuccess) return fail(c, HS_ERR_CUDA, "hs_queue_sig_cache", e);  // the cache stays off; a later call starts over
+    q->sigc = std::move(S);
   }
-  sig_bucket *t = nullptr;
+  dev_mem<sig_bucket> t;
   const size_t bytes = (size_t)buckets * sizeof(sig_bucket);
-  cudaError_t e = cudaMalloc(&t, bytes);
+  cudaError_t e = alloc(t, bytes);
   if (e == cudaSuccess) e = cudaMemsetAsync(t, 0, bytes, q->stream);  // ahead of every launch that probes it
   if (e == cudaSuccess) e = cudaStreamSynchronize(q->stream);
-  if (e != cudaSuccess) {
-    cudaFree(t);
-    return fail(c, e == cudaErrorMemoryAllocation ? HS_ERR_NOMEM : HS_ERR_CUDA, "hs_queue_sig_cache", e);
-  }
+  if (e != cudaSuccess) return fail(c, e == cudaErrorMemoryAllocation ? HS_ERR_NOMEM : HS_ERR_CUDA, "hs_queue_sig_cache", e);
   q->sig_bmask = buckets - 1;
-  q->d_sig = t;
+  q->d_sig = std::move(t);
   return HS_OK;
 }
 
@@ -3889,18 +3888,13 @@ int hs_queue_generic(hs_queue *q, int on) {
   std::lock_guard<std::mutex> g(c->mu);  // the dispatcher reads the option and launches only while it holds c->mu
   if (q->gen_on.load() == (on != 0)) return HS_OK;
   HS_CUDA(c, cudaSetDevice(c->device));
-  if (on && !q->h_gslot) {  // first use: the slot list and the descriptor list of the generic launches
-    cudaError_t e = cudaHostAlloc(&q->h_gslot, (size_t)q->cap * 4, cudaHostAllocMapped);
-    if (e == cudaSuccess) e = cudaHostAlloc(&q->h_gmlist, (size_t)q->cap * sizeof(qmsg_desc), cudaHostAllocMapped);
-    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_gslot, q->h_gslot, 0);
-    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_gmlist, q->h_gmlist, 0);
-    if (e != cudaSuccess) {  // the option stays off; a later call starts the first use over
-      if (q->h_gslot) cudaFreeHost(q->h_gslot);
-      if (q->h_gmlist) cudaFreeHost(q->h_gmlist);
-      q->h_gslot = q->d_gslot = nullptr;
-      q->h_gmlist = q->d_gmlist = nullptr;
+  if (on && !q->gen_bufs.slot.h) {  // first use: the slot list and the descriptor list of the generic launches
+    generic_lists G;
+    cudaError_t e = alloc(G.slot, (size_t)q->cap * 4);
+    if (e == cudaSuccess) e = alloc(G.mlist, (size_t)q->cap * sizeof(qmsg_desc));
+    if (e != cudaSuccess)  // the option stays off; a later call starts the first use over
       return fail(c, e == cudaErrorMemoryAllocation ? HS_ERR_NOMEM : HS_ERR_CUDA, "hs_queue_generic", e);
-    }
+    q->gen_bufs = std::move(G);
   }
   q->gen_on = on != 0;
   if (!on) HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));  // no generic launch survives this line
@@ -3925,36 +3919,38 @@ int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
     q->cv_done.wait(lk, [q] { return q->bq.empty(); });
   }
   HS_CUDA(c, cudaSetDevice(c->device));
-  batch_free(q);
+  batch_drain(q);
+  q->lane = {};  // released before the new lane is allocated
+  q->b_arena = byte_ring{};
   if (!max_items) return HS_OK;
   uint64_t acap = 4096;  // two of the largest regions fit: one can be filled while the other's pass runs
   while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
+  batch_lane B;
   int lo = 0, hi = 0;
   cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->b_stream, cudaStreamNonBlocking, lo);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&q->b_side, cudaStreamNonBlocking, hi);
-  for (cudaEvent_t &ev : q->b_ev)
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaHostAlloc(&q->h_barena, acap, cudaHostAllocMapped);
-  if (e == cudaSuccess) e = cudaHostGetDevicePointer(&q->d_barena, q->h_barena, 0);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmirror, acap);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bdig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bxyz, max_items * 3 * sizeof(fe));
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmeta, max_items);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bflags, max_items);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bvidx, max_items * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmiss, max_items * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bmiss_count, 4);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bitems, (max_items + 31) / 32 * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bgrej, max_bytes + 16);  // group words of a region fit in max_bytes
-  if (e == cudaSuccess) e = cudaMalloc(&q->d_bcounter, 4);
-  if (e == cudaSuccess) e = cudaMemset(q->d_bcounter, 0, 4);
+  if (e == cudaSuccess) e = create(B.stream, lo);
+  if (e == cudaSuccess) e = create(B.side, hi);
+  for (event_h &ev : B.ev)
+    if (e == cudaSuccess) e = create(ev);
+  if (e == cudaSuccess) e = alloc(B.arena, acap);
+  if (e == cudaSuccess) e = alloc(B.mirror, acap);
+  if (e == cudaSuccess) e = alloc(B.dig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
+  if (e == cudaSuccess) e = alloc(B.xyz, max_items * 3 * sizeof(fe));
+  if (e == cudaSuccess) e = alloc(B.meta, max_items);
+  if (e == cudaSuccess) e = alloc(B.flags, max_items);
+  if (e == cudaSuccess) e = alloc(B.vidx, max_items * 4);
+  if (e == cudaSuccess) e = alloc(B.miss, max_items * 4);
+  if (e == cudaSuccess) e = alloc(B.miss_count, 4);
+  if (e == cudaSuccess) e = alloc(B.items, (max_items + 31) / 32 * 4);
+  if (e == cudaSuccess) e = alloc(B.grej, max_bytes + 16);  // group words of a region fit in max_bytes
+  if (e == cudaSuccess) e = alloc(B.counter, 4);
+  if (e == cudaSuccess) e = cudaMemset(B.counter, 0, 4);
   if (e != cudaSuccess) {
     cudaGetLastError();
-    batch_free(q);
     return fail(c, HS_ERR_NOMEM, "hs_queue_batch: no pinned host or device memory for the batch lane", e);
   }
-  memset(q->h_barena, 0, acap);
+  memset(B.arena.h, 0, acap);
+  q->lane = std::move(B);
   std::lock_guard<std::mutex> g(q->mu);
   q->b_arena = byte_ring{acap, 0, 0};
   q->b_max_items = max_items;
@@ -3988,7 +3984,7 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
   });
   if (rc != HS_OK) return rc;
   // the region is this request's alone until it completes: fill it without holding q->mu
-  uint8_t *a = q->h_barena + r->a_off;
+  uint8_t *a = q->lane.arena.h + r->a_off;
   memcpy(a, pre_off, 8 * (n_msgs + 1));
   if (pre_bytes) memcpy(a + B.o_pre, preimages, pre_bytes);
   memcpy(a + B.o_sig, sig, 64 * n_items);

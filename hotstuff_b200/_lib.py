@@ -29,6 +29,8 @@ SIGNATURES = {
                                  c_void_p, c_void_p]),
     "hs_verify_qc_votes_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "hs_qc_and_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
+    "hs_verify_groups_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
+                                     c_void_p]),
     "hs_ingest_consensus_frames": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "hs_committee_register": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "hs_committee_update": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),

@@ -910,9 +910,12 @@ __device__ __forceinline__ void fe_load_global(fe &r, const fe *p) {
 // phase C back-substitution + affine comparison with R's encoding.  Two neighbouring lanes combine their 16 verdicts into
 // one bitmap word, which goes to the local bitmap or — armed by hs_peer_next — straight into every peer's buffer, after
 // which the last block of the grid exchanges the epoch flags with the peers (no separate signal / wait launches).
-__global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
-                                                               uint32_t mode, uint32_t *__restrict__ bitmap, uint8_t *flags_out, const peer_route P,
-                                                               const int group) {
+// verdict(i, fl) turns record i's flags into its bit: one mode for the pass (k_verify_finish) or record i's own mode byte
+// (k_verify_finish_modes).
+template <class Verdict>
+__device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
+                                                   Verdict verdict, uint32_t *__restrict__ bitmap, uint8_t *flags_out, const peer_route &P,
+                                                   const int group) {
   __shared__ fe tot[HS_THREADS];
   const size_t t = (size_t)blockIdx.x * HS_THREADS + threadIdx.x;
   const size_t first = t * (size_t)group;
@@ -953,7 +956,7 @@ __global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_
       if (zero_z) m &= ~HS_META_PARSE_OK;
       const uint32_t fl = verify_flags_from(X, Y, zinv, R, m);
       if (flags_out) flags_out[i] = (uint8_t)fl;
-      const uint32_t ok = (mode == HS_MODE_STRICT) ? (fl & HS_F_STRICT) : (fl & HS_F_EQ);
+      const uint32_t ok = verdict(i, fl);
       if (ok) bits |= 1u << c;
     }
   }
@@ -984,6 +987,20 @@ __global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_
       if (threadIdx.x == 0) P.buf[P.my_rank][HS_PEER_CTRL(P) + 1] = 0;
     }
   }
+}
+__global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
+                                                               uint32_t mode, uint32_t *__restrict__ bitmap, uint8_t *flags_out, const peer_route P,
+                                                               const int group) {
+  verify_finish_body(L, n, xyz, meta, [&](size_t, uint32_t fl) { return (mode == HS_MODE_STRICT) ? (fl & HS_F_STRICT) : (fl & HS_F_EQ); }, bitmap,
+                     flags_out, P, group);
+}
+// Per-record verdict modes (hs_verify_groups_dev): the rule of k_group_and and k_batch_done, so every word written locally or stored
+// into the peers' buffers is a final item verdict — HS_MODE_BATCH_EQ selects HS_F_EQ, any other byte HS_F_STRICT.
+__global__ void __launch_bounds__(HS_THREADS) k_verify_finish_modes(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
+                                                                     const uint8_t *__restrict__ item_mode, uint32_t *__restrict__ bitmap, uint8_t *flags_out,
+                                                                     const peer_route P, const int group) {
+  verify_finish_body(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & (item_mode[i] == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT); }, bitmap,
+                     flags_out, P, group);
 }
 
 // ------------------------------------------------------------------------------------------------ table construction
@@ -1381,6 +1398,7 @@ struct hs_ctx {
   uint32_t slot_mask = 0;
   // grow-only device scratch
   dev_buf in[2], digest[2], xyz, meta, vidx, miss, out;
+  dev_buf group_digests;  // hs_verify_groups_dev: Digests of the pass's preimages (read by the main kernels only, so one set serves deferred mode)
   dev_mem<uint32_t> d_miss_count;
   // key cache: tables for keys that were never registered but keep showing up (learned between calls)
   bool explicit_committee = false;   // hs_committee_register was called with keys: the set is fixed, nothing is learned
@@ -1670,11 +1688,15 @@ static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool i
   }
   return HS_OK;
 }
-// Threads of k_verify_finish own `fin_group` records each; launched on `stream`.
-static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz, const uint8_t *meta, uint32_t mode, uint32_t *d_bitmap,
-                         uint8_t *d_flags_out, const peer_route &P, int fin_group, cudaStream_t stream) {
+// Threads of k_verify_finish own `fin_group` records each; launched on `stream`.  d_item_mode (device, nullable): record i is judged
+// by its own mode byte (k_verify_finish_modes) instead of `mode`.
+static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz, const uint8_t *meta, uint32_t mode, const uint8_t *d_item_mode,
+                         uint32_t *d_bitmap, uint8_t *d_flags_out, const peer_route &P, int fin_group, cudaStream_t stream) {
   const size_t fin_threads = (n + fin_group - 1) / fin_group;
-  k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, d_flags_out, P, fin_group);
+  if (d_item_mode)
+    k_verify_finish_modes<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, d_item_mode, d_bitmap, d_flags_out, P, fin_group);
+  else
+    k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, d_flags_out, P, fin_group);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -1682,8 +1704,9 @@ static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz,
 
 // Runs lookup (optional) -> main (committee and/or generic) -> finish on `stream` for a device-resident layout.
 // use_lookup: L.pk is valid and a committee is registered -> resolve indices on the device.
+// d_item_mode (device, nullable): per-record verdict modes in place of `mode`; read by the finish kernel (on the tail stream when deferred).
 static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t *d_bitmap, cudaStream_t stream, bool indexed,
-                      uint8_t *d_flags_out = nullptr) {
+                      uint8_t *d_flags_out = nullptr, const uint8_t *d_item_mode = nullptr) {
   if (n == 0) {
     if (c->peer_armed) {  // an empty shard still owes its peers the epoch flag
       c->peer_armed = false;
@@ -1728,7 +1751,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_CUDA(c, cudaStreamWaitEvent(c->stream_tail, c->ev_main_done, 0));
     fin_stream = c->stream_tail;
   }
-  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
+  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_item_mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
   return HS_OK;
 }
@@ -2496,7 +2519,7 @@ static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
   const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
   HS_TRY(launch_main(c, L, r.n, committee, false, S, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
-  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, q->lane.items, q->lane.flags, peer_route{}, fin_group, s));
+  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, nullptr, q->lane.items, q->lane.flags, peer_route{}, fin_group, s));
   HS_CUDA(c, cudaMemsetAsync(q->lane.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
   uint8_t *res = q->lane.arena.d + r.a_off;
   k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->lane.flags, m + r.o_mo, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->lane.grej,
@@ -3046,6 +3069,25 @@ int hs_qc_and_dev(hs_ctx *c, const void *d_vote_bitmap, const void *d_qc_idx, si
   c->launches += (n_qc ? 1 : 0) + (n_votes ? 1 : 0);
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
+}
+
+// ---- device-resident mixed groups: hs_verify_groups with every array in HBM, enqueued on `stream`.  Digest of every preimage
+// (k_digest32), then one verify pass whose finish kernel judges item i by d_mode[i], so the item words it writes — locally or into
+// every peer's buffer when armed — are final; group verdicts come from hs_qc_and_dev over them.
+int hs_verify_groups_dev(hs_ctx *c, const void *d_pre, const void *d_off, size_t n_msgs, const void *d_sig, const void *d_pk, const void *d_vidx,
+                         const void *d_msg_idx, const void *d_mode, size_t n_items, void *d_item_bitmap, void *stream) {
+  if (!c || (n_items && (!d_pre || !d_off || !d_sig || (!d_pk && !d_vidx) || !d_msg_idx || !d_item_bitmap)))
+    return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: bad argument");
+  if (n_items && n_msgs == 0) return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: items without preimages");
+  if (n_items && !d_pk && (!c->explicit_committee || c->n_keys == 0))
+    return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: committee-indexed items without a registered committee");
+  HS_CUDA(c, cudaSetDevice(c->device));
+  if (n_items == 0) return run_verify(c, in_layout{}, 0, HS_MODE_STRICT, nullptr, (cudaStream_t)stream, false);  // an armed route still signals
+  HS_TRY(ensure(c, c->group_digests, n_msgs * 32));
+  uint8_t *dig = (uint8_t *)c->group_digests.p.get();
+  HS_TRY(hs_digest32_dev(c, d_pre, d_off, n_msgs, dig, stream));
+  in_layout L{(const uint8_t *)d_sig, 64, (const uint8_t *)d_pk, 32, (const uint32_t *)d_vidx, dig, 32, (const uint32_t *)d_msg_idx, nullptr, 32, 0};
+  return run_verify(c, L, n_items, HS_MODE_STRICT, (uint32_t *)d_item_bitmap, (cudaStream_t)stream, d_pk == nullptr, nullptr, (const uint8_t *)d_mode);
 }
 
 // ---- TC::verify / Timeout::verify for many certificates (consensus/src/messages.rs:250-265,290-315)

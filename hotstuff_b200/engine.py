@@ -281,6 +281,13 @@ class Engine:
         self._check(self.lib.hs_qc_and_dev(self.h, d_vote_bitmap.data_ptr(), d_qc_idx.data_ptr(), n_votes, n_qc, d_qc_bitmap.data_ptr(), self._stream()),
                     "hs_qc_and_dev")
 
+    def verify_groups_dev(self, d_pre, d_off, n_msgs, d_sig, d_msg_idx, d_item_bitmap, n_items, d_mode=None, d_pk=None, d_vidx=None):
+        """hs_verify_groups_dev: verify_groups with device arrays, enqueued on torch's current stream.  d_item_bitmap receives each item's
+        verdict in its own mode (d_mode None = all strict); group verdicts: qc_and_dev(d_item_bitmap, d_group_idx, n_items, n_groups, ..)."""
+        ptr = lambda t: None if t is None else t.data_ptr()
+        self._check(self.lib.hs_verify_groups_dev(self.h, ptr(d_pre), ptr(d_off), n_msgs, ptr(d_sig), ptr(d_pk), ptr(d_vidx), ptr(d_msg_idx),
+                                                  ptr(d_mode), n_items, ptr(d_item_bitmap), self._stream()), "hs_verify_groups_dev")
+
     def keygen_batch_dev(self, d_seeds, d_pks, n):
         self._check(self.lib.hs_keygen_batch_dev(self.h, d_seeds.data_ptr(), n, d_pks.data_ptr(), self._stream()), "hs_keygen_batch_dev")
 

@@ -43,6 +43,40 @@ def verify_sharded(verify_fn, n, rank, world, device=None, group=None):
     return np.unpackbits(full.cpu().numpy().view(np.uint8), bitorder="little")[:n].astype(bool)
 
 
+def verify_groups_sharded(engine, d_pre, d_off, d_sig, d_msg_idx, d_group_idx, n_groups, d_group_bitmap, rank, world, d_mode=None,
+                          d_pk=None, d_vidx=None, peer=None, group=None):
+    """A mixed certificate burst (Blocks, Timeouts with their high_qcs, TCs: items of both verdict modes) sharded over ranks.  Every
+    argument but the preimages (d_pre, d_off: given whole to every rank) is the FULL per-item device array; this rank verifies the items
+    shard_range(n_items, rank, world) gives it through Engine.verify_groups_dev, whose finish kernel judges each item in its own mode, so
+    the words it produces are final.  They reach every rank through `peer` (a PeerAllGather over n_items, armed here) or, without one,
+    the ncclAllGather fallback.  The per-group AND then runs on every rank over the whole gathered item bitmap with the whole d_group_idx,
+    so every rank ends with every group verdict in d_group_bitmap.  Returns the gathered item bitmap ((n_items + 31) // 32 words).
+    Deferred mode works on both paths; the bitmaps are then complete after engine.results_wait().  With `peer`, the AND follows the finish
+    kernel on the engine's tail stream.  On the fallback the collective runs on the caller's stream, which the tail stream does not wait
+    for, so this call waits on the host for the gathered bitmap before it enqueues the AND, and makes the caller's stream wait for the
+    AND: deferral hides nothing there."""
+    import torch
+    n = d_msg_idx.numel()
+    lo, hi, per = shard_range(n, rank, world)
+    shard = lambda t: None if t is None else t[lo:hi]
+    d_local = torch.zeros(max(1, per // 32), dtype=torch.int32, device=d_msg_idx.device)
+    if peer is not None:
+        peer.arm()
+    engine.verify_groups_dev(d_pre, d_off, d_off.numel() - 1, shard(d_sig), shard(d_msg_idx), d_local, hi - lo, d_mode=shard(d_mode), d_pk=shard(d_pk),
+                             d_vidx=shard(d_vidx))
+    if peer is not None:
+        full = peer.bitmap()
+    else:
+        engine.results_wait()  # deferred mode: the words come from the engine's tail stream, the collective reads them on this one
+        full = all_gather_bitmap(d_local[: (hi - lo + 31) // 32], n, world, group)
+        if full.is_cuda:  # deferred mode runs the AND on the tail stream, which does not wait for the collective on this stream
+            torch.cuda.current_stream(full.device).synchronize()
+    engine.qc_and_dev(full, d_group_idx, n, n_groups, d_group_bitmap)
+    if peer is None:
+        engine.results_wait()  # `full` is torch memory: it may be reused in this stream's order only after the AND has read it
+    return full
+
+
 class PeerAllGather:
     """Fused all-gather of the accept bitmap: the verify finish kernel stores its words straight into every rank's result
     buffer over NVLink (include/hs_crypto.h, hs_peer_*).  `ncclAllGather` (all_gather_bitmap above) is the baseline it replaces."""

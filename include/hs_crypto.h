@@ -358,7 +358,27 @@ int hs_verify_msgs_dev(hs_ctx *ctx, const void *d_sig, const void *d_pk_or_null,
  * hs_verify_qcs, used when the votes of many QCs are sharded across GPUs (BASELINE config[3]). */
 int hs_verify_qc_votes_dev(hs_ctx *ctx, const void *d_qc_digests, const void *d_pk_or_null, const void *d_validator_idx_or_null, const void *d_sig,
                            const void *d_qc_idx, size_t n_votes, void *d_vote_bitmap, void *stream);
+/* d_qc_bitmap bit j = AND of the bits of d_vote_bitmap whose d_qc_idx is j (no such bit -> 1), over n_votes bits.  The same AND reduces
+ * the item bitmap of hs_verify_groups_dev to group verdicts: pass the items' group indices as d_qc_idx and the group count as n_qc. */
 int hs_qc_and_dev(hs_ctx *ctx, const void *d_vote_bitmap, const void *d_qc_idx, size_t n_votes, size_t n_qc, void *d_qc_bitmap, void *stream);
+
+/* hs_verify_groups with every array in device memory, enqueued on `stream`.  Item i is (sig[i], key_i) over
+ * Digest(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i]+1])), hashed on the GPU, judged by mode[i] (NULL = all strict).
+ * d_item_bitmap bit i = item i's verdict in ITS OWN mode.  Group verdicts: hs_qc_and_dev(d_item_bitmap, d_group_idx, ...).
+ *   - Arrays: preimages (bytes), pre_off (uint64, n_msgs + 1), sig (64 B each), pk (32 B each) or validator_idx (uint32; used when pk is
+ *     NULL: the committee-indexed form, which needs a registered committee), msg_idx (uint32), mode (uint8), d_item_bitmap (uint32 words).
+ *   - Mode bytes: HS_MODE_BATCH_EQ (1) selects the verify_batch condition; ANY other value selects strict (the rule of hs_verify_groups'
+ *     group AND; the host form rejects bytes > 1, this one cannot see them).
+ *   - Device arrays are trusted, as in hs_verify_var_dev and hs_digest32_dev: offsets, indices and lengths are not checked.  HS_ERR_ARG
+ *     covers only what the host can see: NULL pointers, n_items > 0 with n_msgs == 0, the committee-indexed form without a committee.
+ *   - Keys take the paths of every other pass: key bytes are looked up in the committee (misses take the generic kernel), without a
+ *     committee the key cache or the generic kernel.  The engine hashes the preimages into its own scratch.
+ *   - Deferred mode (hs_set_deferred) and hs_peer_next work as for the other `_dev` verify calls: the finish kernel runs on the tail
+ *     stream; an armed call stores its item words into every peer's buffer at word_offset (and n_items == 0 still sends the epoch flag).
+ *     sig, pk / validator_idx and mode must stay valid until hs_results_wait. */
+int hs_verify_groups_dev(hs_ctx *ctx, const void *d_preimages, const void *d_pre_off /* n_msgs + 1 */, size_t n_msgs, const void *d_sig,
+                         const void *d_pk_or_null, const void *d_validator_idx_or_null, const void *d_msg_idx, const void *d_mode_or_null,
+                         size_t n_items, void *d_item_bitmap, void *stream);
 
 /* ---- load generation: RFC 8032 key generation and signing of 32-byte digests ON THE GPU ---------------------------------------
  * generate_keypair / Signature::new (crypto/src/lib.rs:167-175,185-191) for input synthesis only: the node itself signs one

@@ -41,6 +41,10 @@ pub mod generic_queue;
 /// awaited by a task instead of run under `spawn_blocking` (`batch_queue::verify_groups_queued`).
 #[path = "crypto_gpu_batch_queue.rs"]
 pub mod batch_queue;
+/// The device-resident certificate pass (hs_verify_groups_dev): Blocks, Timeouts and TCs whose arrays are already in HBM, enqueued on
+/// the caller's stream (`groups_dev::verify_groups_dev`).
+#[path = "crypto_gpu_groups_dev.rs"]
+pub mod groups_dev;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

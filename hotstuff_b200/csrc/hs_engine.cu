@@ -910,12 +910,14 @@ __device__ __forceinline__ void fe_load_global(fe &r, const fe *p) {
 // phase C back-substitution + affine comparison with R's encoding.  Two neighbouring lanes combine their 16 verdicts into
 // one bitmap word, which goes to the local bitmap or — armed by hs_peer_next — straight into every peer's buffer, after
 // which the last block of the grid exchanges the epoch flags with the peers (no separate signal / wait launches).
+// The verify flag that decides a record's verdict in `mode`: HS_MODE_BATCH_EQ selects HS_F_EQ, any other value HS_F_STRICT (the
+// host entry points reject values above 1; device mode bytes are not checked).
+__host__ __device__ inline uint32_t mode_flag(uint32_t mode) { return mode == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT; }
 // verdict(i, fl) turns record i's flags into its bit: one mode for the pass (k_verify_finish) or record i's own mode byte
 // (k_verify_finish_modes).
 template <class Verdict>
 __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
-                                                   Verdict verdict, uint32_t *__restrict__ bitmap, uint8_t *flags_out, const peer_route &P,
-                                                   const int group) {
+                                                   Verdict verdict, uint32_t *__restrict__ bitmap, const peer_route &P, const int group) {
   __shared__ fe tot[HS_THREADS];
   const size_t t = (size_t)blockIdx.x * HS_THREADS + threadIdx.x;
   const size_t first = t * (size_t)group;
@@ -955,7 +957,6 @@ __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n,
       uint32_t m = meta[i];
       if (zero_z) m &= ~HS_META_PARSE_OK;
       const uint32_t fl = verify_flags_from(X, Y, zinv, R, m);
-      if (flags_out) flags_out[i] = (uint8_t)fl;
       const uint32_t ok = verdict(i, fl);
       if (ok) bits |= 1u << c;
     }
@@ -989,18 +990,15 @@ __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n,
   }
 }
 __global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
-                                                               uint32_t mode, uint32_t *__restrict__ bitmap, uint8_t *flags_out, const peer_route P,
-                                                               const int group) {
-  verify_finish_body(L, n, xyz, meta, [&](size_t, uint32_t fl) { return (mode == HS_MODE_STRICT) ? (fl & HS_F_STRICT) : (fl & HS_F_EQ); }, bitmap,
-                     flags_out, P, group);
+                                                               uint32_t mode, uint32_t *__restrict__ bitmap, const peer_route P, const int group) {
+  verify_finish_body(L, n, xyz, meta, [&](size_t, uint32_t fl) { return fl & mode_flag(mode); }, bitmap, P, group);
 }
-// Per-record verdict modes (hs_verify_groups_dev): the rule of k_group_and and k_batch_done, so every word written locally or stored
-// into the peers' buffers is a final item verdict — HS_MODE_BATCH_EQ selects HS_F_EQ, any other byte HS_F_STRICT.
+// Per-record verdict modes (hs_verify_groups_dev, hs_verify_groups, the queue's batch lane): every word written locally or stored into
+// the peers' buffers is a final item verdict.
 __global__ void __launch_bounds__(HS_THREADS) k_verify_finish_modes(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
-                                                                     const uint8_t *__restrict__ item_mode, uint32_t *__restrict__ bitmap, uint8_t *flags_out,
-                                                                     const peer_route P, const int group) {
-  verify_finish_body(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & (item_mode[i] == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT); }, bitmap,
-                     flags_out, P, group);
+                                                                     const uint8_t *__restrict__ item_mode, uint32_t *__restrict__ bitmap, const peer_route P,
+                                                                     const int group) {
+  verify_finish_body(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & mode_flag(item_mode[i]); }, bitmap, P, group);
 }
 
 // ------------------------------------------------------------------------------------------------ table construction
@@ -1152,38 +1150,20 @@ __global__ void __launch_bounds__(256) k_qc_and(const uint32_t *__restrict__ vot
   }
 }
 
-// item i belongs to group grp[i]; its verdict is flag bit STRICT or EQ by mode[i] (nullptr = all strict).  A rejected item
-// clears its group's bit (group bitmap pre-set to ones); the item verdicts are also packed into item_bitmap (nullable).
-__global__ void __launch_bounds__(256) k_group_and(const uint8_t *__restrict__ flags, const uint8_t *__restrict__ mode, const uint32_t *__restrict__ grp,
-                                                   size_t n_items, size_t n_groups, uint32_t *__restrict__ item_bitmap, uint32_t *__restrict__ group_bitmap) {
-  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
-  uint32_t ok = 0;
-  if (i < n_items) {
-    const uint32_t want = (mode && mode[i] == HS_MODE_BATCH_EQ) ? HS_F_EQ : HS_F_STRICT;
-    ok = (flags[i] & want) ? 1u : 0u;
-    if (!ok) {
-      const uint32_t j = grp[i];
-      if (j < n_groups) atomicAnd(group_bitmap + (j >> 5), ~(1u << (j & 31)));
-    }
-  }
-  const uint32_t word = __ballot_sync(0xffffffffu, ok);
-  if (item_bitmap && (threadIdx.x & 31) == 0 && i < n_items) item_bitmap[i >> 5] = word;
-}
-// Completion of a verify-queue batch pass (hs_queue_submit_batch), in place of k_group_and + copies + a stream synchronise: item i's
-// verdict is flag bit STRICT or EQ by mode[i]; the item bits are balloted straight into the request's mapped result words (after the
-// group words) and a rejected item sets its group's bit in grej (device, zeroed ahead of the pass).  The last block to finish
-// (block counter + fence) writes the group words (1 = every item verified; a group with no items is 1) and the miss count into the
-// mapped result, fences to system scope, and raises the request's completion word tail[1] = seq for the queue's thread.
-__global__ void __launch_bounds__(256) k_batch_done(const uint8_t *__restrict__ flags, const uint8_t *__restrict__ mode, const uint32_t *__restrict__ grp,
-                                                    uint32_t n_items, uint32_t n_groups, uint32_t *grej, uint32_t *out, const uint32_t *miss_count,
-                                                    uint32_t *tail, uint32_t seq, uint32_t *counter) {
+// Completion of a verify-queue batch pass (hs_queue_submit_batch), in place of k_qc_and + copies + a stream synchronise: item i's
+// verdict is bit i of `items` (k_verify_finish_modes); the item bits are balloted straight into the request's mapped result words
+// (after the group words) and a rejected item sets its group's bit in grej (device, zeroed ahead of the pass).  The last block to
+// finish (block counter + fence) writes the group words (1 = every item verified; a group with no items is 1) and the miss count into
+// the mapped result, fences to system scope, and raises the request's completion word tail[1] = seq for the queue's thread.
+__global__ void __launch_bounds__(256) k_batch_done(const uint32_t *__restrict__ items, const uint32_t *__restrict__ grp, uint32_t n_items,
+                                                    uint32_t n_groups, uint32_t *grej, uint32_t *out, const uint32_t *miss_count, uint32_t *tail,
+                                                    uint32_t seq, uint32_t *counter) {
   __shared__ int is_last;
   const uint32_t i = blockIdx.x * 256 + threadIdx.x;
   const uint32_t gw = (n_groups + 31) / 32;
   uint32_t ok = 0;
   if (i < n_items) {
-    const uint32_t want = mode[i] == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT;
-    ok = (flags[i] & want) ? 1u : 0u;
+    ok = (items[i >> 5] >> (i & 31)) & 1u;
     if (!ok) {
       const uint32_t j = grp[i];
       atomicOr(grej + (j >> 5), 1u << (j & 31));
@@ -1691,12 +1671,12 @@ static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool i
 // Threads of k_verify_finish own `fin_group` records each; launched on `stream`.  d_item_mode (device, nullable): record i is judged
 // by its own mode byte (k_verify_finish_modes) instead of `mode`.
 static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz, const uint8_t *meta, uint32_t mode, const uint8_t *d_item_mode,
-                         uint32_t *d_bitmap, uint8_t *d_flags_out, const peer_route &P, int fin_group, cudaStream_t stream) {
+                         uint32_t *d_bitmap, const peer_route &P, int fin_group, cudaStream_t stream) {
   const size_t fin_threads = (n + fin_group - 1) / fin_group;
   if (d_item_mode)
-    k_verify_finish_modes<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, d_item_mode, d_bitmap, d_flags_out, P, fin_group);
+    k_verify_finish_modes<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, d_item_mode, d_bitmap, P, fin_group);
   else
-    k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, d_flags_out, P, fin_group);
+    k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, P, fin_group);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -1706,7 +1686,7 @@ static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz,
 // use_lookup: L.pk is valid and a committee is registered -> resolve indices on the device.
 // d_item_mode (device, nullable): per-record verdict modes in place of `mode`; read by the finish kernel (on the tail stream when deferred).
 static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t *d_bitmap, cudaStream_t stream, bool indexed,
-                      uint8_t *d_flags_out = nullptr, const uint8_t *d_item_mode = nullptr) {
+                      const uint8_t *d_item_mode = nullptr) {
   if (n == 0) {
     if (c->peer_armed) {  // an empty shard still owes its peers the epoch flag
       c->peer_armed = false;
@@ -1751,7 +1731,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_CUDA(c, cudaStreamWaitEvent(c->stream_tail, c->ev_main_done, 0));
     fin_stream = c->stream_tail;
   }
-  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_item_mode, d_bitmap, d_flags_out, P, fin_group, fin_stream));
+  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_item_mode, d_bitmap, P, fin_group, fin_stream));
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
   return HS_OK;
 }
@@ -1774,7 +1754,7 @@ static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
 static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->keys.atables; }
 // c->small.in.h[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
 // mapped host memory.
-static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, uint8_t *out_flags_or_null) {
+static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap) {
   for (size_t i = 0; i < n; i++) {
     c->small.in.h[i].req = 0;
     c->small.in.h[i].req_n = (uint32_t)n;
@@ -1804,12 +1784,9 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap, u
     if (*done != seq) return fail(c, HS_ERR_CUDA, "k_verify_small did not complete");
   }
   for (size_t w = 0; w < (n + 31) / 32; w++) out_bitmap[w] = 0;
-  const uint32_t want = (mode == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
-  for (size_t i = 0; i < n; i++) {
-    const uint8_t fl = ((volatile uint8_t *)c->small.out.h)[i];
-    if (out_flags_or_null) out_flags_or_null[i] = fl;
-    if (fl & want) out_bitmap[i >> 5] |= 1u << (i & 31);
-  }
+  const uint32_t want = mode_flag(mode);
+  for (size_t i = 0; i < n; i++)
+    if (((volatile uint8_t *)c->small.out.h)[i] & want) out_bitmap[i >> 5] |= 1u << (i & 31);
   return HS_OK;
 }
 
@@ -1925,7 +1902,7 @@ struct batch_lane {
   dev_mem<uint8_t> mirror;  // the inputs of the region in flight, at the same offsets
   dev_mem<uint32_t> dig;    // the request's Digests, 32 bytes per preimage
   dev_mem<fe> xyz;
-  dev_mem<uint8_t> meta, flags;
+  dev_mem<uint8_t> meta;
   dev_mem<uint32_t> vidx, miss, miss_count, items, grej, counter;
   stream_h stream, side;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
   event_h ev[2];
@@ -2427,8 +2404,7 @@ static void queue_watch(hs_queue *q) {
           std::fill(bits, bits + (r.n + 31) / 32, 0u);
           for (uint32_t i = 0; i < r.n; i++) {  // the kernel writes both flags: each record's mode picks its verdict
             const uint32_t s = (uint32_t)((p + i) & q->mask);
-            const uint32_t want = (q->modes[s] == HS_MODE_STRICT) ? HS_F_STRICT : HS_F_EQ;
-            if (((volatile uint8_t *)q->flags.h)[s] & want) bits[i >> 5] |= 1u << (i & 31);
+            if (((volatile uint8_t *)q->flags.h)[s] & mode_flag(q->modes[s])) bits[i >> 5] |= 1u << (i & 31);
           }
           if (L.sig_gen) {  // the completing block moved the request's signature-cache counts here before its completion word
             const volatile uint32_t *sc = q->sigc.hctr.h + HS_SIG_CTRS * (size_t)(p & q->mask);
@@ -2519,10 +2495,10 @@ static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
   const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
   HS_TRY(launch_main(c, L, r.n, committee, false, S, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
-  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, nullptr, q->lane.items, q->lane.flags, peer_route{}, fin_group, s));
+  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, m + r.o_mo, q->lane.items, peer_route{}, fin_group, s));
   HS_CUDA(c, cudaMemsetAsync(q->lane.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
   uint8_t *res = q->lane.arena.d + r.a_off;
-  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->lane.flags, m + r.o_mo, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->lane.grej,
+  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->lane.items, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->lane.grej,
                                                     reinterpret_cast<uint32_t *>(res + r.o_res), committee ? q->lane.miss_count.get() : nullptr,
                                                     reinterpret_cast<uint32_t *>(res + r.o_tail), r.seq, q->lane.counter);
   c->launches++;
@@ -3034,9 +3010,7 @@ int hs_verify_qcs(hs_ctx *c, const uint8_t *preimages, size_t n_qc, const uint8_
   k_digest32<<<blocks_for(n_qc), HS_THREADS, 0, c->stream>>>(d + o_pre, nullptr, 40, n_qc, (uint32_t *)(d + o_dig));
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  in_layout L{d + o_sig, 64, pk ? d + o_key : nullptr, 32, pk ? nullptr : (const uint32_t *)(d + o_key), d + o_dig, 32, (const uint32_t *)(d + o_qi),
-              nullptr, 32, 0};
-  HS_TRY(run_verify(c, L, n_votes, HS_MODE_BATCH_EQ, d_votes, c->stream, pk == nullptr));
+  HS_TRY(hs_verify_qc_votes_dev(c, d + o_dig, pk ? d + o_key : nullptr, pk ? nullptr : d + o_key, d + o_sig, d + o_qi, n_votes, d_votes, c->stream));
   k_qc_and<<<blocks_for(n_votes, 256), 256, 0, c->stream>>>(d_votes, (const uint32_t *)(d + o_qi), n_votes, n_qc, d_qc);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
@@ -3087,7 +3061,7 @@ int hs_verify_groups_dev(hs_ctx *c, const void *d_pre, const void *d_off, size_t
   uint8_t *dig = (uint8_t *)c->group_digests.p.get();
   HS_TRY(hs_digest32_dev(c, d_pre, d_off, n_msgs, dig, stream));
   in_layout L{(const uint8_t *)d_sig, 64, (const uint8_t *)d_pk, 32, (const uint32_t *)d_vidx, dig, 32, (const uint32_t *)d_msg_idx, nullptr, 32, 0};
-  return run_verify(c, L, n_items, HS_MODE_STRICT, (uint32_t *)d_item_bitmap, (cudaStream_t)stream, d_pk == nullptr, nullptr, (const uint8_t *)d_mode);
+  return run_verify(c, L, n_items, HS_MODE_STRICT, (uint32_t *)d_item_bitmap, (cudaStream_t)stream, d_pk == nullptr, (const uint8_t *)d_mode);
 }
 
 // ---- TC::verify / Timeout::verify for many certificates (consensus/src/messages.rs:250-265,290-315)
@@ -3156,9 +3130,8 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
   HS_CUDA(c, cudaSetDevice(c->device));
   const size_t key_bytes = pk ? 32 : 4, pre_bytes = pre_off[n_msgs];
   auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_off = 0, o_pre = al((n_msgs + 1) * 8), o_dig = o_pre + al(pre_bytes + 8), o_sig = o_dig + n_msgs * 32, o_key = o_sig + n_items * 64,
-               o_mi = o_key + al(n_items * key_bytes), o_gi = o_mi + al(n_items * 4), o_mo = o_gi + al(n_items * 4), o_fl = o_mo + al(n_items),
-               total = o_fl + al(n_items);
+  const size_t o_off = 0, o_pre = al((n_msgs + 1) * 8), o_sig = o_pre + al(pre_bytes + 8), o_key = o_sig + n_items * 64,
+               o_mi = o_key + al(n_items * key_bytes), o_gi = o_mi + al(n_items * 4), o_mo = o_gi + al(n_items * 4), total = o_mo + al(n_items);
   HS_TRY(ensure(c, c->in[0], total));
   HS_TRY(ensure(c, c->out, (i_words + g_words) * 4));
   uint8_t *d = (uint8_t *)c->in[0].p.get();
@@ -3171,12 +3144,9 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
   HS_CUDA(c, cudaMemcpyAsync(d + o_gi, group_idx, n_items * 4, cudaMemcpyHostToDevice, c->stream));
   if (mode) HS_CUDA(c, cudaMemcpyAsync(d + o_mo, mode, n_items, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d_groups, out_group_bitmap, g_words * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_digest32_dev(c, d + o_pre, d + o_off, n_msgs, d + o_dig, c->stream));
-  in_layout L{d + o_sig, 64, pk ? d + o_key : nullptr, 32, pk ? nullptr : (const uint32_t *)(d + o_key), d + o_dig, 32, (const uint32_t *)(d + o_mi),
-              nullptr, 32, 0};
-  HS_TRY(run_verify(c, L, n_items, HS_MODE_STRICT, d_items, c->stream, pk == nullptr, d + o_fl));
-  k_group_and<<<blocks_for(n_items, 256), 256, 0, c->stream>>>(d + o_fl, mode ? d + o_mo : nullptr, (const uint32_t *)(d + o_gi), n_items, n_groups, d_items,
-                                                               d_groups);
+  HS_TRY(hs_verify_groups_dev(c, d + o_pre, d + o_off, n_msgs, d + o_sig, pk ? d + o_key : nullptr, pk ? nullptr : d + o_key, d + o_mi,
+                              mode ? d + o_mo : nullptr, n_items, d_items, c->stream));
+  k_qc_and<<<blocks_for(n_items, 256), 256, 0, c->stream>>>(d_items, (const uint32_t *)(d + o_gi), n_items, n_groups, d_groups);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   if (out_item_bitmap) HS_CUDA(c, cudaMemcpyAsync(out_item_bitmap, d_items, i_words * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -3335,12 +3305,12 @@ int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, 
         c->small.in.h[i].vidx = idx;
       }
     }
-    if (all) return run_small(c, n, mode, out_bitmap, nullptr);
+    if (all) return run_small(c, n, mode, out_bitmap);
   }
   HS_TRY(ensure(c, c->in[0], n * sizeof(hs_rec128)));
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
   HS_CUDA(c, cudaMemcpyAsync(c->in[0].p, recs, n * sizeof(hs_rec128), cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(run_verify(c, layout_rec128(c->in[0].p), n, mode, (uint32_t *)c->out.p.get(), c->stream, false));
+  HS_TRY(hs_verify_rec128_dev(c, c->in[0].p, n, mode, c->out.p, c->stream));
   return finish_bitmap(c, n, out_bitmap);
 }
 int hs_verify_strict_batch(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t *out_bitmap) {
@@ -3364,8 +3334,7 @@ int hs_verify_var(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint8_
   HS_CUDA(c, cudaMemcpyAsync(d + o_pk, pk, n * 32, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaMemcpyAsync(d + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
   if (off[n]) HS_CUDA(c, cudaMemcpyAsync(d + o_msg, msgs, off[n], cudaMemcpyHostToDevice, c->stream));
-  in_layout L{d + o_sig, 64, d + o_pk, 32, nullptr, d + o_msg, 0, nullptr, (const uint64_t *)(d + o_off), 0, 0};
-  HS_TRY(run_verify(c, L, n, mode, (uint32_t *)c->out.p.get(), c->stream, false));
+  HS_TRY(hs_verify_var_dev(c, d + o_sig, d + o_pk, d + o_msg, d + o_off, n, mode, c->out.p, c->stream));
   return finish_bitmap(c, n, out_bitmap);
 }
 
@@ -3392,7 +3361,7 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
     }
     if (all) {
       uint32_t bm2[(HS_SMALL_MAX + 31) / 32];
-      HS_TRY(run_small(c, n, HS_MODE_BATCH_EQ, bm2, nullptr));
+      HS_TRY(run_small(c, n, HS_MODE_BATCH_EQ, bm2));
       int ok2 = 1;
       for (size_t w = 0; w < words; w++) {
         if (bm2[w] != bitmap_word_ones(n, w)) ok2 = 0;
@@ -3439,7 +3408,7 @@ int hs_verify_committee(hs_ctx *c, const uint32_t *vidx, const uint8_t *sig, con
       memcpy(c->small.in.h[i].msg, digests + 32 * (size_t)(midx ? midx[i] : 0), 32);
       c->small.in.h[i].vidx = vidx[i];
     }
-    return run_small(c, n, mode, out_bitmap, nullptr);
+    return run_small(c, n, mode, out_bitmap);
   }
   size_t o_sig = 0, o_v = n * 64, o_m = o_v + n * 4, o_d = o_m + (midx ? n * 4 : 0), total = o_d + n_msgs * 32;
   HS_TRY(ensure(c, c->in[0], total));
@@ -3979,7 +3948,6 @@ int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
   if (e == cudaSuccess) e = alloc(B.dig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
   if (e == cudaSuccess) e = alloc(B.xyz, max_items * 3 * sizeof(fe));
   if (e == cudaSuccess) e = alloc(B.meta, max_items);
-  if (e == cudaSuccess) e = alloc(B.flags, max_items);
   if (e == cudaSuccess) e = alloc(B.vidx, max_items * 4);
   if (e == cudaSuccess) e = alloc(B.miss, max_items * 4);
   if (e == cudaSuccess) e = alloc(B.miss_count, 4);

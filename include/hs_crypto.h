@@ -367,8 +367,8 @@ int hs_qc_and_dev(hs_ctx *ctx, const void *d_vote_bitmap, const void *d_qc_idx, 
  * d_item_bitmap bit i = item i's verdict in ITS OWN mode.  Group verdicts: hs_qc_and_dev(d_item_bitmap, d_group_idx, ...).
  *   - Arrays: preimages (bytes), pre_off (uint64, n_msgs + 1), sig (64 B each), pk (32 B each) or validator_idx (uint32; used when pk is
  *     NULL: the committee-indexed form, which needs a registered committee), msg_idx (uint32), mode (uint8), d_item_bitmap (uint32 words).
- *   - Mode bytes: HS_MODE_BATCH_EQ (1) selects the verify_batch condition; ANY other value selects strict (the rule of hs_verify_groups'
- *     group AND; the host form rejects bytes > 1, this one cannot see them).
+ *   - Mode bytes: HS_MODE_BATCH_EQ (1) selects the verify_batch condition; ANY other value selects strict (hs_verify_groups, which
+ *     runs this pass, rejects bytes > 1 first; this form cannot see them).
  *   - Device arrays are trusted, as in hs_verify_var_dev and hs_digest32_dev: offsets, indices and lengths are not checked.  HS_ERR_ARG
  *     covers only what the host can see: NULL pointers, n_items > 0 with n_msgs == 0, the committee-indexed form without a committee.
  *   - Keys take the paths of every other pass: key bytes are looked up in the committee (misses take the generic kernel), without a

@@ -112,25 +112,34 @@ def test_hits_after_a_verified_block(engine, oracle, keys, queues):
 
 
 def test_eight_threads_submitting_identical_timeouts_join(engine, oracle, keys, queues):
-    """8 threads submit Timeouts with the same 1,335-vote QC at once: one verifies it, the others join it (or hit once it is done)."""
+    """8 threads submit Timeouts with the same 1,335-vote QC at once: one verifies it, the others join it (or hit once it is done).
+    The threads' submits are serialised by the binding and the GIL, and take about as long as the QC's GPU pass, so the QC is held in
+    flight: as the threads are released, records signed by keys outside the committee are submitted first, and the queue's thread
+    verifies them on its slow path (about a millisecond each) before it can see the QC's pass complete."""
     q, plain = queues
     rng = np.random.default_rng(2)
     qc = make_qc(oracle, keys, 1335, rng)
     ts = [timeout(oracle, keys, qc, rng, corrupt=i == 5) for i in range(8)]
-    go = threading.Barrier(8)
+    f_seeds = rng.integers(0, 256, size=(4, 32), dtype=np.uint8)
+    f_pks, f_dig = oracle.keygen_batch(f_seeds), np.frombuffer(rng.bytes(4 * 32), np.uint8).reshape(4, 32)
+    f_sig = oracle.sign_batch(f_seeds, f_pks, np.arange(4, dtype=np.uint32), f_dig.reshape(-1), np.arange(5, dtype=np.uint64) * 32)
+    slow = np.concatenate([f_sig, f_pks, f_dig], axis=1)
+    held = []
+    go = threading.Barrier(8, action=lambda: held.extend(q.submit(slow[i:i + 1]) for i in range(4)))
     out = [None] * 8
 
     def run(i):
         go.wait()
         out[i] = q.wait(submit(q, ts[i]))
 
-    c0 = q.cert_stats()
+    c0, s0 = q.cert_stats(), q.stats()
     th = [threading.Thread(target=run, args=(i,)) for i in range(8)]
     [t.start() for t in th]
     [t.join() for t in th]
     d = delta(c0, q.cert_stats())
     assert d["lookups"] == 8 and d["inserted"] == 1 and d["hits"] + d["joins"] == 7 and d["joins"] >= 1, d
     assert d["records_answered"] == 7 * 1335
+    assert [bool(q.wait(t)[0]) for t in held] == list(oracle.verify_rec128(slow, mode=0)) and delta(s0, q.stats())["slow_requests"] == 4
     for t, bits in zip(ts, out):
         check(oracle, plain, t, bits)
     # the same from one thread without waiting in between: every later copy finds the QC in flight or verified

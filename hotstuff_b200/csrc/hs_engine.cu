@@ -21,6 +21,8 @@
 //   (one warp per long message, schedules expanded across lanes).
 // Front ends: QC / TC / Timeout / Block groups with on-GPU digests and per-certificate AND; load-generation keygen / signer.
 #include <cuda_runtime.h>
+#include <algorithm>
+#include <array>
 #include <atomic>
 #include <condition_variable>
 #include <cstdint>
@@ -28,6 +30,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <initializer_list>
 #include <list>
 #include <memory>
 #include <mutex>
@@ -1457,6 +1460,61 @@ static int ensure(hs_ctx *c, dev_buf &b, size_t need) {
 }
 static inline unsigned blocks_for(size_t n, unsigned per = HS_THREADS) { return (unsigned)((n + per - 1) / per); }
 
+// A host entry point's inputs, staged into one grow-only device buffer.  add() declares the sections in order: each starts 16-byte
+// aligned and is followed by `slack` spare bytes; src == nullptr reserves the bytes without copying them.  upload() ensures the
+// buffer and copies every non-empty section that has a source.  ptr() is valid only after upload(), since ensure() may move the
+// buffer, and is a valid address even for a section of 0 bytes.
+struct h2d_stage {
+  struct section {
+    const void *src;
+    size_t off, bytes;
+  };
+  std::array<section, 8> sec;  // at() in add() throws on a ninth section
+  size_t n = 0, total = 0;
+  uint8_t *base = nullptr;
+  size_t add(const void *src, size_t bytes, size_t slack = 0) {
+    const size_t off = (total + 15) & ~(size_t)15;
+    sec.at(n) = {src, off, bytes};
+    total = off + bytes + slack;
+    return n++;
+  }
+  int upload(hs_ctx *c, dev_buf &buf, cudaStream_t stream) {
+    HS_TRY(ensure(c, buf, total));
+    base = (uint8_t *)buf.p.get();
+    for (size_t k = 0; k < n; k++)
+      if (sec[k].src && sec[k].bytes) HS_CUDA(c, cudaMemcpyAsync(base + sec[k].off, sec[k].src, sec[k].bytes, cudaMemcpyHostToDevice, stream));
+    return HS_OK;
+  }
+  uint8_t *ptr(size_t k) const { return base + sec[k].off; }
+};
+// A host entry point's results: every copy with a destination, on the context's stream, then one wait for the stream.
+struct d2h_copy {
+  void *dst;  // nullable: an output the caller did not ask for
+  const void *src;
+  size_t bytes;
+};
+static int readback(hs_ctx *c, std::initializer_list<d2h_copy> copies) {
+  for (const d2h_copy &r : copies)
+    if (r.dst) HS_CUDA(c, cudaMemcpyAsync(r.dst, r.src, r.bytes, cudaMemcpyDeviceToHost, c->stream));
+  HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  return HS_OK;
+}
+// The words of an all-ones bitmap over n bits: the initial group words of a certificate pass, kept off the caller's buffer so that a
+// call that fails leaves it unwritten.
+static std::vector<uint32_t> bitmap_ones(size_t n) {
+  std::vector<uint32_t> bm((n + 31) / 32);
+  for (size_t w = 0; w < bm.size(); w++) bm[w] = bitmap_word_ones(n, w);
+  return bm;
+}
+// Clears bit j of d_groups when an item with d_group_idx == j is rejected, over an item bitmap of n_items bits.
+static int launch_qc_and(hs_ctx *c, const uint32_t *d_items, const uint32_t *d_group_idx, size_t n_items, size_t n_groups, uint32_t *d_groups,
+                         cudaStream_t stream) {
+  k_qc_and<<<blocks_for(n_items, 256), 256, 0, stream>>>(d_items, d_group_idx, n_items, n_groups, d_groups);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+
 
 static int launch_build(hs_ctx *c, const uint8_t *d_encs, size_t n_points, int negate, int W, int n_windows, ge_niels *tables, uint8_t *flags) {
   size_t threads = n_points * (size_t)n_windows * ((1u << (W - 1)) / HS_BUILD_BLOCK);
@@ -1752,6 +1810,24 @@ static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
   return HS_NO_KEY;
 }
 static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->keys.atables; }
+// Record i of a latency-path call: its signature, its 32-byte message and its key's table index.
+struct small_src {
+  const uint8_t *sig, *msg;
+  uint32_t vidx;
+};
+// Fills c->small.in.h[0 .. n) from rec(i) and reports whether every key index resolved (!= HS_NO_KEY).
+template <class Rec>
+static bool small_stage(hs_ctx *c, size_t n, Rec rec) {
+  bool all = true;
+  for (size_t i = 0; i < n; i++) {
+    const small_src s = rec(i);
+    memcpy(c->small.in.h[i].sig, s.sig, 64);
+    memcpy(c->small.in.h[i].msg, s.msg, 32);
+    c->small.in.h[i].vidx = s.vidx;
+    all = all && s.vidx != HS_NO_KEY;
+  }
+  return all;
+}
 // c->small.in.h[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
 // mapped host memory.
 static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap) {
@@ -2987,37 +3063,32 @@ int hs_verify_qcs(hs_ctx *c, const uint8_t *preimages, size_t n_qc, const uint8_
                   const uint32_t *qc_idx, size_t n_votes, uint32_t *out_vote_bitmap, uint32_t *out_qc_bitmap) {
   if (!c || !out_qc_bitmap || (n_qc && !preimages) || (n_votes && (!sig || !qc_idx || (!pk && !vidx) || n_qc == 0)))
     return fail(c, HS_ERR_ARG, "hs_verify_qcs: bad argument");
-  const size_t qc_words = (n_qc + 31) / 32, vote_words = (n_votes + 31) / 32;
-  for (size_t w = 0; w < qc_words; w++) out_qc_bitmap[w] = bitmap_word_ones(n_qc, w);
-  if (n_votes == 0) return HS_OK;
   for (size_t i = 0; i < n_votes; i++)
     if (qc_idx[i] >= n_qc) return fail(c, HS_ERR_ARG, "hs_verify_qcs: qc_idx out of range");
+  const size_t qc_words = (n_qc + 31) / 32, vote_words = (n_votes + 31) / 32;
+  const std::vector<uint32_t> ones = bitmap_ones(n_qc);
+  if (n_votes == 0) {
+    std::copy(ones.begin(), ones.end(), out_qc_bitmap);
+    return HS_OK;
+  }
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  const size_t key_bytes = pk ? 32 : 4;
-  const size_t o_pre = 0, o_dig = (n_qc * 40 + 15) & ~(size_t)15, o_sig = o_dig + n_qc * 32, o_key = o_sig + n_votes * 64,
-               o_qi = o_key + ((n_votes * key_bytes + 15) & ~(size_t)15), total = o_qi + n_votes * 4;
-  HS_TRY(ensure(c, c->in[0], total));
+  h2d_stage S;
+  const size_t s_pre = S.add(preimages, n_qc * 40), s_dig = S.add(nullptr, n_qc * 32), s_sig = S.add(sig, n_votes * 64),
+               s_key = S.add(pk ? (const void *)pk : (const void *)vidx, n_votes * (pk ? 32 : 4)), s_qi = S.add(qc_idx, n_votes * 4);
   HS_TRY(ensure(c, c->out, (vote_words + qc_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  HS_TRY(S.upload(c, c->in[0], c->stream));
   uint32_t *d_votes = (uint32_t *)c->out.p.get(), *d_qc = d_votes + vote_words;
-  HS_CUDA(c, cudaMemcpyAsync(d + o_pre, preimages, n_qc * 40, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_votes * 64, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_key, pk ? (const void *)pk : (const void *)vidx, n_votes * key_bytes, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_qi, qc_idx, n_votes * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d_qc, out_qc_bitmap, qc_words * 4, cudaMemcpyHostToDevice, c->stream));  // all ones (tail cleared)
+  const uint32_t *d_qi = (const uint32_t *)S.ptr(s_qi);
+  HS_CUDA(c, cudaMemcpyAsync(d_qc, ones.data(), qc_words * 4, cudaMemcpyHostToDevice, c->stream));
   // QC::digest = SHA-512(hash || round_le)[..32] for every certificate (messages.rs:201-208)
-  k_digest32<<<blocks_for(n_qc), HS_THREADS, 0, c->stream>>>(d + o_pre, nullptr, 40, n_qc, (uint32_t *)(d + o_dig));
+  k_digest32<<<blocks_for(n_qc), HS_THREADS, 0, c->stream>>>(S.ptr(s_pre), nullptr, 40, n_qc, (uint32_t *)S.ptr(s_dig));
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  HS_TRY(hs_verify_qc_votes_dev(c, d + o_dig, pk ? d + o_key : nullptr, pk ? nullptr : d + o_key, d + o_sig, d + o_qi, n_votes, d_votes, c->stream));
-  k_qc_and<<<blocks_for(n_votes, 256), 256, 0, c->stream>>>(d_votes, (const uint32_t *)(d + o_qi), n_votes, n_qc, d_qc);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
-  if (out_vote_bitmap) HS_CUDA(c, cudaMemcpyAsync(out_vote_bitmap, d_votes, vote_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(out_qc_bitmap, d_qc, qc_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  HS_TRY(hs_verify_qc_votes_dev(c, S.ptr(s_dig), pk ? S.ptr(s_key) : nullptr, pk ? nullptr : S.ptr(s_key), S.ptr(s_sig), d_qi, n_votes, d_votes,
+                                c->stream));
+  HS_TRY(launch_qc_and(c, d_votes, d_qi, n_votes, n_qc, d_qc, c->stream));
+  return readback(c, {{out_vote_bitmap, d_votes, vote_words * 4}, {out_qc_bitmap, d_qc, qc_words * 4}});
 }
 
 // ---- device-resident QC verification (strong-scaling path of BASELINE config[3]: the votes of many QCs sharded over ranks)
@@ -3038,10 +3109,9 @@ int hs_qc_and_dev(hs_ctx *c, const void *d_vote_bitmap, const void *d_qc_idx, si
   HS_CUDA(c, cudaSetDevice(c->device));
   cudaStream_t st = (c->deferred && (cudaStream_t)stream != c->stream) ? c->stream_tail : (cudaStream_t)stream;  // deferred: after the finish kernel on the tail stream
   if (n_qc) k_bitmap_ones<<<blocks_for((n_qc + 31) / 32, 256), 256, 0, st>>>((uint32_t *)d_qc_bitmap, n_qc);
-  if (n_votes)
-    k_qc_and<<<blocks_for(n_votes, 256), 256, 0, st>>>((const uint32_t *)d_vote_bitmap, (const uint32_t *)d_qc_idx, n_votes, n_qc, (uint32_t *)d_qc_bitmap);
-  c->launches += (n_qc ? 1 : 0) + (n_votes ? 1 : 0);
+  c->launches += n_qc ? 1 : 0;
   HS_CUDA(c, cudaGetLastError());
+  if (n_votes) HS_TRY(launch_qc_and(c, (const uint32_t *)d_vote_bitmap, (const uint32_t *)d_qc_idx, n_votes, n_qc, (uint32_t *)d_qc_bitmap, st));
   return HS_OK;
 }
 
@@ -3072,44 +3142,35 @@ int hs_verify_tcs(hs_ctx *c, const uint64_t *tc_rounds, size_t n_tc, const uint8
                   const uint64_t *high_qc_rounds, const uint32_t *tc_idx, size_t n_votes, uint32_t *out_vote_bitmap, uint32_t *out_tc_bitmap) {
   if (!c || !out_tc_bitmap || (n_tc && !tc_rounds) || (n_votes && (!sig || !high_qc_rounds || (!pk && !vidx) || n_tc == 0)) || (!tc_idx && n_votes && n_tc != n_votes))
     return fail(c, HS_ERR_ARG, "hs_verify_tcs: bad argument");
-  const size_t tc_words = (n_tc + 31) / 32, vote_words = (n_votes + 31) / 32;
-  for (size_t w = 0; w < tc_words; w++) out_tc_bitmap[w] = bitmap_word_ones(n_tc, w);
-  if (n_votes == 0) return HS_OK;
   if (tc_idx)
     for (size_t i = 0; i < n_votes; i++)
       if (tc_idx[i] >= n_tc) return fail(c, HS_ERR_ARG, "hs_verify_tcs: tc_idx out of range");
+  const size_t tc_words = (n_tc + 31) / 32, vote_words = (n_votes + 31) / 32;
+  const std::vector<uint32_t> ones = bitmap_ones(n_tc);
+  if (n_votes == 0) {
+    std::copy(ones.begin(), ones.end(), out_tc_bitmap);
+    return HS_OK;
+  }
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  const size_t key_bytes = pk ? 32 : 4;
-  const size_t o_r = 0, o_hq = (n_tc * 8 + 15) & ~(size_t)15, o_dig = o_hq + ((n_votes * 8 + 15) & ~(size_t)15), o_sig = o_dig + n_votes * 32,
-               o_key = o_sig + n_votes * 64, o_ti = o_key + ((n_votes * key_bytes + 15) & ~(size_t)15), total = o_ti + n_votes * 4;
-  HS_TRY(ensure(c, c->in[0], total));
+  h2d_stage S;
+  const size_t s_r = S.add(tc_rounds, n_tc * 8), s_hq = S.add(high_qc_rounds, n_votes * 8), s_dig = S.add(nullptr, n_votes * 32),
+               s_sig = S.add(sig, n_votes * 64), s_key = S.add(pk ? (const void *)pk : (const void *)vidx, n_votes * (pk ? 32 : 4)),
+               s_ti = S.add(tc_idx, n_votes * 4);
   HS_TRY(ensure(c, c->out, (vote_words + tc_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  HS_TRY(S.upload(c, c->in[0], c->stream));
   uint32_t *d_votes = (uint32_t *)c->out.p.get(), *d_tc = d_votes + vote_words;
-  HS_CUDA(c, cudaMemcpyAsync(d + o_r, tc_rounds, n_tc * 8, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_hq, high_qc_rounds, n_votes * 8, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_votes * 64, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_key, pk ? (const void *)pk : (const void *)vidx, n_votes * key_bytes, cudaMemcpyHostToDevice, c->stream));
-  if (tc_idx) HS_CUDA(c, cudaMemcpyAsync(d + o_ti, tc_idx, n_votes * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d_tc, out_tc_bitmap, tc_words * 4, cudaMemcpyHostToDevice, c->stream));
-  k_tc_digests<<<blocks_for(n_votes), HS_THREADS, 0, c->stream>>>((const uint64_t *)(d + o_r), tc_idx ? (const uint32_t *)(d + o_ti) : nullptr,
-                                                                  (const uint64_t *)(d + o_hq), n_votes, n_tc, (uint32_t *)(d + o_dig));
+  const uint32_t *d_ti = tc_idx ? (const uint32_t *)S.ptr(s_ti) : nullptr;
+  if (tc_idx) HS_CUDA(c, cudaMemcpyAsync(d_tc, ones.data(), tc_words * 4, cudaMemcpyHostToDevice, c->stream));
+  k_tc_digests<<<blocks_for(n_votes), HS_THREADS, 0, c->stream>>>((const uint64_t *)S.ptr(s_r), d_ti, (const uint64_t *)S.ptr(s_hq), n_votes, n_tc,
+                                                                  (uint32_t *)S.ptr(s_dig));
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  in_layout L{d + o_sig, 64, pk ? d + o_key : nullptr, 32, pk ? nullptr : (const uint32_t *)(d + o_key), d + o_dig, 32, nullptr, nullptr, 32, 0};
+  in_layout L{S.ptr(s_sig), 64, pk ? S.ptr(s_key) : nullptr, 32, pk ? nullptr : (const uint32_t *)S.ptr(s_key), S.ptr(s_dig), 32, nullptr, nullptr, 32, 0};
   HS_TRY(run_verify(c, L, n_votes, HS_MODE_STRICT, d_votes, c->stream, pk == nullptr));
-  if (tc_idx) {
-    k_qc_and<<<blocks_for(n_votes, 256), 256, 0, c->stream>>>(d_votes, (const uint32_t *)(d + o_ti), n_votes, n_tc, d_tc);
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
-    HS_CUDA(c, cudaMemcpyAsync(out_tc_bitmap, d_tc, tc_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  } else {
-    HS_CUDA(c, cudaMemcpyAsync(out_tc_bitmap, d_votes, vote_words * 4, cudaMemcpyDeviceToHost, c->stream));  // one vote per certificate
-  }
-  if (out_vote_bitmap) HS_CUDA(c, cudaMemcpyAsync(out_vote_bitmap, d_votes, vote_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  if (tc_idx) HS_TRY(launch_qc_and(c, d_votes, d_ti, n_votes, n_tc, d_tc, c->stream));
+  // without tc_idx, vote i is certificate i
+  return readback(c, {{out_vote_bitmap, d_votes, vote_words * 4}, {out_tc_bitmap, tc_idx ? d_tc : d_votes, tc_words * 4}});
 }
 
 // ---- mixed groups: Block::verify for many blocks (messages.rs:54-76) = author signature (strict) + QC votes (batch-eq) + TC
@@ -3120,39 +3181,29 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
                      uint32_t *out_item_bitmap, uint32_t *out_group_bitmap) {
   if (!c || !out_group_bitmap || (n_msgs && !pre_off) || (n_items && (!sig || !msg_idx || !group_idx || (!pk && !vidx) || n_msgs == 0 || n_groups == 0)))
     return fail(c, HS_ERR_ARG, "hs_verify_groups: bad argument");
-  const size_t g_words = (n_groups + 31) / 32, i_words = (n_items + 31) / 32;
-  for (size_t w = 0; w < g_words; w++) out_group_bitmap[w] = bitmap_word_ones(n_groups, w);
-  if (n_items == 0) return HS_OK;
-  if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages)) return fail(c, HS_ERR_ARG, "hs_verify_groups: bad preimage offsets");
+  if (n_items && (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages))) return fail(c, HS_ERR_ARG, "hs_verify_groups: bad preimage offsets");
   for (size_t i = 0; i < n_items; i++)
     if (msg_idx[i] >= n_msgs || group_idx[i] >= n_groups || (mode && mode[i] > 1)) return fail(c, HS_ERR_ARG, "hs_verify_groups: index out of range");
+  const size_t g_words = (n_groups + 31) / 32, i_words = (n_items + 31) / 32;
+  const std::vector<uint32_t> ones = bitmap_ones(n_groups);
+  if (n_items == 0) {
+    std::copy(ones.begin(), ones.end(), out_group_bitmap);
+    return HS_OK;
+  }
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  const size_t key_bytes = pk ? 32 : 4, pre_bytes = pre_off[n_msgs];
-  auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
-  const size_t o_off = 0, o_pre = al((n_msgs + 1) * 8), o_sig = o_pre + al(pre_bytes + 8), o_key = o_sig + n_items * 64,
-               o_mi = o_key + al(n_items * key_bytes), o_gi = o_mi + al(n_items * 4), o_mo = o_gi + al(n_items * 4), total = o_mo + al(n_items);
-  HS_TRY(ensure(c, c->in[0], total));
+  h2d_stage S;
+  const size_t s_off = S.add(pre_off, (n_msgs + 1) * 8), s_pre = S.add(preimages, pre_off[n_msgs], 8), s_sig = S.add(sig, n_items * 64),
+               s_key = S.add(pk ? (const void *)pk : (const void *)vidx, n_items * (pk ? 32 : 4)), s_mi = S.add(msg_idx, n_items * 4),
+               s_gi = S.add(group_idx, n_items * 4), s_mo = S.add(mode, n_items);
   HS_TRY(ensure(c, c->out, (i_words + g_words) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
+  HS_TRY(S.upload(c, c->in[0], c->stream));
   uint32_t *d_items = (uint32_t *)c->out.p.get(), *d_groups = d_items + i_words;
-  HS_CUDA(c, cudaMemcpyAsync(d + o_off, pre_off, (n_msgs + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  if (pre_bytes) HS_CUDA(c, cudaMemcpyAsync(d + o_pre, preimages, pre_bytes, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n_items * 64, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_key, pk ? (const void *)pk : (const void *)vidx, n_items * key_bytes, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_mi, msg_idx, n_items * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_gi, group_idx, n_items * 4, cudaMemcpyHostToDevice, c->stream));
-  if (mode) HS_CUDA(c, cudaMemcpyAsync(d + o_mo, mode, n_items, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d_groups, out_group_bitmap, g_words * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_verify_groups_dev(c, d + o_pre, d + o_off, n_msgs, d + o_sig, pk ? d + o_key : nullptr, pk ? nullptr : d + o_key, d + o_mi,
-                              mode ? d + o_mo : nullptr, n_items, d_items, c->stream));
-  k_qc_and<<<blocks_for(n_items, 256), 256, 0, c->stream>>>(d_items, (const uint32_t *)(d + o_gi), n_items, n_groups, d_groups);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
-  if (out_item_bitmap) HS_CUDA(c, cudaMemcpyAsync(out_item_bitmap, d_items, i_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(out_group_bitmap, d_groups, g_words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  HS_CUDA(c, cudaMemcpyAsync(d_groups, ones.data(), g_words * 4, cudaMemcpyHostToDevice, c->stream));
+  HS_TRY(hs_verify_groups_dev(c, S.ptr(s_pre), S.ptr(s_off), n_msgs, S.ptr(s_sig), pk ? S.ptr(s_key) : nullptr, pk ? nullptr : S.ptr(s_key),
+                              S.ptr(s_mi), mode ? S.ptr(s_mo) : nullptr, n_items, d_items, c->stream));
+  HS_TRY(launch_qc_and(c, d_items, (const uint32_t *)S.ptr(s_gi), n_items, n_groups, d_groups, c->stream));
+  return readback(c, {{out_item_bitmap, d_items, i_words * 4}, {out_group_bitmap, d_groups, g_words * 4}});
 }
 
 // ---- load generation (SURVEY §8f.4): RFC 8032 keygen / signing of 32-byte digests on the GPU
@@ -3182,13 +3233,12 @@ int hs_keygen_batch(hs_ctx *c, const uint8_t *seeds, size_t n, uint8_t *out_pks)
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  HS_TRY(ensure(c, c->in[0], n * 32));
+  h2d_stage S;
+  const size_t s_seed = S.add(seeds, n * 32);
   HS_TRY(ensure(c, c->out, n * 32));
-  HS_CUDA(c, cudaMemcpyAsync(c->in[0].p, seeds, n * 32, cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_keygen_batch_dev(c, c->in[0].p, n, c->out.p, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(out_pks, c->out.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  HS_TRY(hs_keygen_batch_dev(c, S.ptr(s_seed), n, c->out.p, c->stream));
+  return readback(c, {{out_pks, c->out.p.get(), n * 32}});
 }
 int hs_sign_digests(hs_ctx *c, const uint8_t *seeds, const uint8_t *pks, size_t n_keys, const uint32_t *key_idx, const uint8_t *digests, size_t n,
                     uint8_t *out_sig) {
@@ -3199,18 +3249,12 @@ int hs_sign_digests(hs_ctx *c, const uint8_t *seeds, const uint8_t *pks, size_t 
       if (key_idx[i] >= n_keys) return fail(c, HS_ERR_ARG, "hs_sign_digests: key index out of range");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  const size_t o_seed = 0, o_pk = n_keys * 32, o_ki = o_pk + n_keys * 32, o_d = o_ki + ((n * 4 + 15) & ~(size_t)15), total = o_d + n * 32;
-  HS_TRY(ensure(c, c->in[0], total));
+  h2d_stage S;
+  const size_t s_seed = S.add(seeds, n_keys * 32), s_pk = S.add(pks, n_keys * 32), s_ki = S.add(key_idx, n * 4), s_d = S.add(digests, n * 32);
   HS_TRY(ensure(c, c->out, n * 64));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
-  HS_CUDA(c, cudaMemcpyAsync(d + o_seed, seeds, n_keys * 32, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_pk, pks, n_keys * 32, cudaMemcpyHostToDevice, c->stream));
-  if (key_idx) HS_CUDA(c, cudaMemcpyAsync(d + o_ki, key_idx, n * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_d, digests, n * 32, cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_sign_digests_dev(c, d + o_seed, d + o_pk, n_keys, key_idx ? d + o_ki : nullptr, d + o_d, n, c->out.p, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(out_sig, c->out.p, n * 64, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  HS_TRY(hs_sign_digests_dev(c, S.ptr(s_seed), S.ptr(s_pk), n_keys, key_idx ? S.ptr(s_ki) : nullptr, S.ptr(s_d), n, c->out.p, c->stream));
+  return readback(c, {{out_sig, c->out.p.get(), n * 64}});
 }
 
 // ---- multi-GPU peer routing (one process per GPU; handles are exchanged by the host, e.g. torch.distributed.all_gather_object)
@@ -3282,36 +3326,20 @@ int hs_peer_timed_out(hs_ctx *c) {
 }
 
 // ---- host-pointer entry points
-static int finish_bitmap(hs_ctx *c, size_t n, uint32_t *out_bitmap) {
-  size_t words = (n + 31) / 32;
-  HS_CUDA(c, cudaMemcpyAsync(out_bitmap, c->out.p, words * 4, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
-}
-
 int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, uint32_t *out_bitmap) {
   if (!c || mode > 1 || (n && (!recs || !out_bitmap))) return fail(c, HS_ERR_ARG, "hs_verify_rec128: bad argument");
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  if (small_eligible(c, n)) {  // latency path: every key must already have a table (registered or learned)
-    bool all = true;
-    for (size_t i = 0; i < n && all; i++) {
-      const uint32_t idx = host_key_lookup(c, recs[i].pk);
-      if (idx == HS_NO_KEY) all = false;
-      else {
-        memcpy(c->small.in.h[i].sig, recs[i].sig, 64);
-        memcpy(c->small.in.h[i].msg, recs[i].msg, 32);
-        c->small.in.h[i].vidx = idx;
-      }
-    }
-    if (all) return run_small(c, n, mode, out_bitmap);
-  }
-  HS_TRY(ensure(c, c->in[0], n * sizeof(hs_rec128)));
+  // latency path: every key must already have a table (registered or learned)
+  if (small_eligible(c, n) && small_stage(c, n, [&](size_t i) { return small_src{recs[i].sig, recs[i].msg, host_key_lookup(c, recs[i].pk)}; }))
+    return run_small(c, n, mode, out_bitmap);
+  h2d_stage S;
+  const size_t s_recs = S.add(recs, n * sizeof(hs_rec128));
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
-  HS_CUDA(c, cudaMemcpyAsync(c->in[0].p, recs, n * sizeof(hs_rec128), cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_verify_rec128_dev(c, c->in[0].p, n, mode, c->out.p, c->stream));
-  return finish_bitmap(c, n, out_bitmap);
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  HS_TRY(hs_verify_rec128_dev(c, S.ptr(s_recs), n, mode, c->out.p, c->stream));
+  return readback(c, {{out_bitmap, c->out.p.get(), ((n + 31) / 32) * 4}});
 }
 int hs_verify_strict_batch(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t *out_bitmap) {
   return hs_verify_rec128(c, recs, n, HS_MODE_STRICT, out_bitmap);
@@ -3325,17 +3353,12 @@ int hs_verify_var(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint8_
   if (off[n] && !msgs) return fail(c, HS_ERR_ARG, "hs_verify_var: null msgs");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  // device layout: [sig n*64][pk n*32][off (n+1)*8][msgs] — every section 8-byte aligned
-  size_t o_sig = 0, o_pk = n * 64, o_off = o_pk + n * 32, o_msg = o_off + (n + 1) * 8, total = o_msg + off[n];
-  HS_TRY(ensure(c, c->in[0], total + 8));
+  h2d_stage S;
+  const size_t s_sig = S.add(sig, n * 64), s_pk = S.add(pk, n * 32), s_off = S.add(off, (n + 1) * 8), s_msg = S.add(msgs, off[n], 8);
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
-  HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n * 64, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_pk, pk, n * 32, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  if (off[n]) HS_CUDA(c, cudaMemcpyAsync(d + o_msg, msgs, off[n], cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_verify_var_dev(c, d + o_sig, d + o_pk, d + o_msg, d + o_off, n, mode, c->out.p, c->stream));
-  return finish_bitmap(c, n, out_bitmap);
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  HS_TRY(hs_verify_var_dev(c, S.ptr(s_sig), S.ptr(s_pk), S.ptr(s_msg), S.ptr(s_off), n, mode, c->out.p, c->stream));
+  return readback(c, {{out_bitmap, c->out.p.get(), ((n + 31) / 32) * 4}});
 }
 
 int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vote *votes, size_t n, int *all_ok, uint32_t *out_bitmap_or_null) {
@@ -3347,44 +3370,26 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
   }
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  size_t words = (n + 31) / 32;
-  if (small_eligible(c, n)) {  // latency path (the 2f+1 = 3 votes of a 4-node QC)
-    bool all = true;
-    for (size_t i = 0; i < n && all; i++) {
-      const uint32_t idx = host_key_lookup(c, votes[i].pk);
-      if (idx == HS_NO_KEY) all = false;
-      else {
-        memcpy(c->small.in.h[i].sig, votes[i].sig, 64);
-        memcpy(c->small.in.h[i].msg, digest, 32);
-        c->small.in.h[i].vidx = idx;
-      }
-    }
-    if (all) {
-      uint32_t bm2[(HS_SMALL_MAX + 31) / 32];
-      HS_TRY(run_small(c, n, HS_MODE_BATCH_EQ, bm2));
-      int ok2 = 1;
-      for (size_t w = 0; w < words; w++) {
-        if (bm2[w] != bitmap_word_ones(n, w)) ok2 = 0;
-        if (out_bitmap_or_null) out_bitmap_or_null[w] = bm2[w];
-      }
-      *all_ok = ok2;
-      return HS_OK;
-    }
-  }
-  HS_TRY(ensure(c, c->in[0], n * sizeof(hs_vote) + 32));
-  HS_TRY(ensure(c, c->out, words * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
-  HS_CUDA(c, cudaMemcpyAsync(d, digest, 32, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + 32, votes, n * sizeof(hs_vote), cudaMemcpyHostToDevice, c->stream));
-  in_layout L{d + 32 + 32, sizeof(hs_vote), d + 32, sizeof(hs_vote), nullptr, d, 0, nullptr, nullptr, 32, 0};
-  HS_TRY(run_verify(c, L, n, HS_MODE_BATCH_EQ, (uint32_t *)c->out.p.get(), c->stream, false));
+  const size_t words = (n + 31) / 32;
   std::vector<uint32_t> tmp;
   uint32_t *bm = out_bitmap_or_null;
   if (!bm) {
     tmp.resize(words);
     bm = tmp.data();
   }
-  HS_TRY(finish_bitmap(c, n, bm));
+  // latency path (the 2f+1 = 3 votes of a 4-node QC)
+  if (small_eligible(c, n) && small_stage(c, n, [&](size_t i) { return small_src{votes[i].sig, digest, host_key_lookup(c, votes[i].pk)}; })) {
+    HS_TRY(run_small(c, n, HS_MODE_BATCH_EQ, bm));
+  } else {
+    h2d_stage S;
+    const size_t s_dig = S.add(digest, 32), s_votes = S.add(votes, n * sizeof(hs_vote));
+    HS_TRY(ensure(c, c->out, words * 4));
+    HS_TRY(S.upload(c, c->in[0], c->stream));
+    const uint8_t *v = S.ptr(s_votes);  // hs_vote: pk | sig
+    in_layout L{v + 32, sizeof(hs_vote), v, sizeof(hs_vote), nullptr, S.ptr(s_dig), 0, nullptr, nullptr, 32, 0};
+    HS_TRY(run_verify(c, L, n, HS_MODE_BATCH_EQ, (uint32_t *)c->out.p.get(), c->stream, false));
+    HS_TRY(readback(c, {{bm, c->out.p.get(), words * 4}}));
+  }
   int ok = 1;
   for (size_t w = 0; w < words; w++)
     if (bm[w] != bitmap_word_ones(n, w)) ok = 0;
@@ -3402,24 +3407,16 @@ int hs_verify_committee(hs_ctx *c, const uint32_t *vidx, const uint8_t *sig, con
       if (midx[i] >= n_msgs) return fail(c, HS_ERR_ARG, "hs_verify_committee: msg_idx out of range");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  if (small_eligible(c, n) && c->explicit_committee) {  // latency path
-    for (size_t i = 0; i < n; i++) {
-      memcpy(c->small.in.h[i].sig, sig + 64 * i, 64);
-      memcpy(c->small.in.h[i].msg, digests + 32 * (size_t)(midx ? midx[i] : 0), 32);
-      c->small.in.h[i].vidx = vidx[i];
-    }
+  if (small_eligible(c, n) && c->explicit_committee) {  // latency path: the indices as given (the kernel rejects one without a key)
+    small_stage(c, n, [&](size_t i) { return small_src{sig + 64 * i, digests + 32 * (size_t)(midx ? midx[i] : 0), vidx[i]}; });
     return run_small(c, n, mode, out_bitmap);
   }
-  size_t o_sig = 0, o_v = n * 64, o_m = o_v + n * 4, o_d = o_m + (midx ? n * 4 : 0), total = o_d + n_msgs * 32;
-  HS_TRY(ensure(c, c->in[0], total));
+  h2d_stage S;
+  const size_t s_sig = S.add(sig, n * 64), s_v = S.add(vidx, n * 4), s_m = S.add(midx, midx ? n * 4 : 0), s_d = S.add(digests, n_msgs * 32);
   HS_TRY(ensure(c, c->out, ((n + 31) / 32) * 4));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
-  HS_CUDA(c, cudaMemcpyAsync(d + o_sig, sig, n * 64, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_v, vidx, n * 4, cudaMemcpyHostToDevice, c->stream));
-  if (midx) HS_CUDA(c, cudaMemcpyAsync(d + o_m, midx, n * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaMemcpyAsync(d + o_d, digests, n_msgs * 32, cudaMemcpyHostToDevice, c->stream));
-  HS_TRY(hs_verify_committee_dev(c, d + o_v, d + o_sig, midx ? d + o_m : nullptr, d + o_d, n, mode, c->out.p, c->stream));
-  return finish_bitmap(c, n, out_bitmap);
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  HS_TRY(hs_verify_committee_dev(c, S.ptr(s_v), S.ptr(s_sig), midx ? S.ptr(s_m) : nullptr, S.ptr(s_d), n, mode, c->out.p, c->stream));
+  return readback(c, {{out_bitmap, c->out.p.get(), ((n + 31) / 32) * 4}});
 }
 
 int hs_digest32_batch(hs_ctx *c, const uint8_t *data, const uint64_t *off, size_t n, uint8_t *out) {
@@ -3429,23 +3426,19 @@ int hs_digest32_batch(hs_ctx *c, const uint8_t *data, const uint64_t *off, size_
   if (off[n] && !data) return fail(c, HS_ERR_ARG, "hs_digest32_batch: null data");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  size_t o_off = 0, o_data = (n + 1) * 8, total = o_data + off[n];
-  HS_TRY(ensure(c, c->in[0], total + 8));
+  h2d_stage S;
+  const size_t s_off = S.add(off, (n + 1) * 8), s_data = S.add(data, off[n], 8);
   HS_TRY(ensure(c, c->out, n * 32));
-  uint8_t *d = (uint8_t *)c->in[0].p.get();
-  HS_CUDA(c, cudaMemcpyAsync(d + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-  if (off[n]) HS_CUDA(c, cudaMemcpyAsync(d + o_data, data, off[n], cudaMemcpyHostToDevice, c->stream));
+  HS_TRY(S.upload(c, c->in[0], c->stream));
   if (n <= 64 && off[n] / n >= 1024) {
     // a few long messages (mempool batches): one warp per message, schedules expanded in parallel across lanes
-    k_digest32_long<<<(unsigned)n, 32, 0, c->stream>>>(d + o_data, (const uint64_t *)(d + o_off), n, (uint32_t *)c->out.p.get());
+    k_digest32_long<<<(unsigned)n, 32, 0, c->stream>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, (uint32_t *)c->out.p.get());
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
   } else {
-    HS_TRY(hs_digest32_dev(c, d + o_data, d + o_off, n, c->out.p, c->stream));
+    HS_TRY(hs_digest32_dev(c, S.ptr(s_data), S.ptr(s_off), n, c->out.p, c->stream));
   }
-  HS_CUDA(c, cudaMemcpyAsync(out, c->out.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
-  return HS_OK;
+  return readback(c, {{out, c->out.p.get(), n * 32}});
 }
 
 // Reference-shaped end-to-end call: verdict_i = Signature::verify(Digest(msg_i), key_i) for fixed-size messages, with the
@@ -3481,12 +3474,10 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
   }
   // (A short "ramp" first chunk was tried and measured slower — 7.1e7 vs 7.6e7 verifies/s: every extra chunk costs one more
   // generic-pass latency when the batch contains unknown keys.)
-  const size_t first = 0;
   size_t lo = 0;
   for (size_t j = 0; lo < n; j++) {
     const int b = (int)(j & 1);
-    const size_t want = (j == 0 && first) ? first : CH;
-    const size_t cnt = (n - lo < want) ? (n - lo) : want;
+    const size_t cnt = (n - lo < CH) ? (n - lo) : CH;
     uint8_t *d = (uint8_t *)c->in[b].p.get();
     const size_t o_sig = 0, o_key = cnt * 64, o_msg = o_key + ((cnt * key_bytes + 15) & ~(size_t)15);
     if (j >= 2) HS_CUDA(c, cudaStreamWaitEvent(c->stream2, c->ev_done[b], 0));  // staging buffer b is free again
@@ -3501,7 +3492,7 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
     HS_CUDA(c, cudaEventRecord(c->ev_done[b], c->stream));
     lo += cnt;
   }
-  return finish_bitmap(c, n, out_bitmap);
+  return readback(c, {{out_bitmap, c->out.p.get(), ((n + 31) / 32) * 4}});
 }
 
 // ---- verify queue

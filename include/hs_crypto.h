@@ -9,7 +9,8 @@
  * Conventions
  *   - Every function returns 0 (HS_OK) when the engine ran; verdicts are in the output buffers.  Non-zero = engine
  *     failure (CUDA error, bad argument): the caller must treat every signature of that call as REJECTED
- *     (reference behaviour: any Err drops the message, consensus/src/core.rs:434-439).  There is no CPU fallback.
+ *     (reference behaviour: any Err drops the message, consensus/src/core.rs:434-439).  There is no CPU fallback.  A
+ *     host-pointer verify call that returns HS_ERR_ARG writes nothing to its output bitmaps.
  *   - Malformed inputs (S >= l, non-decompressible A or R, ...) are verdict 0, never an error.
  *   - Host-pointer entry points copy inputs to the device, run, and copy results back before returning; nothing is
  *     retained.  `_dev` entry points take device pointers and a cudaStream_t (as void*) and return after enqueueing.

@@ -75,6 +75,7 @@ SIGNATURES = {
                                       c_void_p, c_void_p, ctypes.POINTER(c_size_t)]),
     "hs_queue_batch_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_destroy": (None, [c_void_p]),
+    "hs_self_test": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_u32)]),
 }
 
 # hs_queue_cb: void (void *user, size_t ticket, int status, const uint32_t *bitmap)

@@ -30,7 +30,7 @@ def _sources(d, exts):
 
 
 def build_engine(force=False, verbose=False):
-    srcs = _sources(CSRC, (".cu", ".cuh", ".cpp")) + [os.path.join(ROOT, "include", "hs_crypto.h")]
+    srcs = _sources(CSRC, (".cu", ".cuh", ".cpp", ".h")) + [os.path.join(ROOT, "include", "hs_crypto.h")]
     if not force and _newer(LIB, srcs):
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"

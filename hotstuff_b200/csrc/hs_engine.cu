@@ -44,6 +44,7 @@
 #include <vector>
 
 #include "../../include/hs_crypto.h"
+#include "hs_selftest_vectors.h"
 #include "verify_core.cuh"
 
 #define HS_THREADS 128
@@ -1682,19 +1683,29 @@ struct pass_scratch {
   cudaEvent_t ev_side[2];
   const event_h *prof;                 // nullable: events around k_verify_main<committee>
 };
+// The per-key tables a verify pass reads and the windows they were built at: the context's (registered committee or key cache), or
+// the scratch set of hs_self_test.  The base-point table is always the context's.
+struct pass_tables {
+  committee_tables C;
+  key_table T;
+  comb_params cp;
+};
+static pass_tables ctx_tables(const hs_ctx *c) {
+  return pass_tables{{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries},
+                     {c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)c->n_keys}, c->cp};
+}
 // The main phase on `stream`: with committee tables, [k_key_lookup, then k_verify_main<false> over the misses on S.side] beside
 // k_verify_main<true>; without, k_verify_main<false> over every record.  after_lookup(have_lookup) runs where run_verify collects
 // keys for the key cache.  L.vidx is set to the lookup's indices when it runs.
 template <class AfterLookup>
-static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool indexed, const pass_scratch &S, cudaStream_t stream,
-                       AfterLookup after_lookup) {
+static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool indexed, const pass_tables &K, const pass_scratch &S,
+                       cudaStream_t stream, AfterLookup after_lookup) {
   main_out O{S.xyz, S.meta, 0};
-  committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
+  const committee_tables &C = K.C;
   if (committee) {
     if (!indexed) {
-      key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)c->n_keys};
       HS_CUDA(c, cudaMemsetAsync(S.miss_count, 0, 4, stream));
-      k_key_lookup<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, T, S.vidx, S.miss, S.miss_count);
+      k_key_lookup<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, K.T, S.vidx, S.miss, S.miss_count);
       c->launches++;
       HS_CUDA(c, cudaGetLastError());
       L.vidx = S.vidx;
@@ -1707,20 +1718,20 @@ static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool i
       HS_CUDA(c, cudaStreamWaitEvent(S.side, S.ev_side[0], 0));
       unsigned grid = blocks_for(n, 32);
       if (grid > c->n_sms * 8u) grid = c->n_sms * 8u;
-      k_verify_main<false><<<grid, 32, 0, S.side>>>(L, 0, S.miss_count, S.miss, c->d_btable, C, O, c->cp);
+      k_verify_main<false><<<grid, 32, 0, S.side>>>(L, 0, S.miss_count, S.miss, c->d_btable, C, O, K.cp);
       c->launches++;
       HS_CUDA(c, cudaGetLastError());
       HS_CUDA(c, cudaEventRecord(S.ev_side[1], S.side));
     }
     if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[0], stream));
-    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
+    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, K.cp);
     if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[1], stream));
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
     if (!indexed) HS_CUDA(c, cudaStreamWaitEvent(stream, S.ev_side[1], 0));
   } else {
     HS_TRY(after_lookup(false));
-    k_verify_main<false><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, c->cp);
+    k_verify_main<false><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, K.cp);
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
   }
@@ -1774,7 +1785,8 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   }
   const pass_scratch S{(fe *)XYZ.p.get(), (uint8_t *)META.p.get(), (uint32_t *)c->vidx.p.get(), (uint32_t *)c->miss.p.get(), c->d_miss_count, c->stream_side,
                        {c->ev_side[0], c->ev_side[1]}, c->profile_main ? c->ev_prof : nullptr};
-  HS_TRY(launch_main(c, L, n, committee, indexed, S, stream, [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }));
+  HS_TRY(launch_main(c, L, n, committee, indexed, ctx_tables(c), S, stream,
+                     [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }));
   // small batches: small groups, so that enough blocks exist to hide each block's serial inversion; when the tail overlaps the next pass
   // (deferred mode) latency is hidden anyway and the 16-record group costs the fewest inversions
   const int fin_group = (defer || n >= (1u << 19)) ? 16 : (n >= (1u << 18) ? 8 : 4);
@@ -2569,7 +2581,7 @@ static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
   // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
   const bool committee = c->explicit_committee && c->n_keys > 0 && c->keys.atables;
   const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
-  HS_TRY(launch_main(c, L, r.n, committee, false, S, s, [](bool) { return HS_OK; }));
+  HS_TRY(launch_main(c, L, r.n, committee, false, ctx_tables(c), S, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
   HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, m + r.o_mo, q->lane.items, peer_route{}, fin_group, s));
   HS_CUDA(c, cudaMemsetAsync(q->lane.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
@@ -2839,6 +2851,25 @@ void hs_host_free(void *p) {
 }
 
 // ---- committee registration
+// Table slots (capk: N plus spares) and per-key window (wa) that registering N keys picks now.
+static int committee_geometry(hs_ctx *c, size_t N, size_t &capk, int &wa) {
+  // widest per-key window whose tables fit in the budget: ~62 % of the device by default (80 GB H100: 16 bits up to
+  // ~1 k keys, 15 up to ~1.8 k, 14 up to ~3.3 k, 13 up to ~6.3 k, 12 up to ~11 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device
+  size_t free_b = 0, total_b = 0;
+  HS_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+  size_t budget = total_b / 100 * 62;
+  if (c->table_budget) budget = c->table_budget;
+  if (budget > free_b - free_b / 8) budget = free_b - free_b / 8;
+  // spare slots (1/16 of the set, at least 16) let hs_committee_update add validators without rebuilding anything
+  capk = N + (N / 16 > 16 ? N / 16 : 16);
+  wa = 8;
+  for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8}) {  // 17 bits: 15 windows (94 MB per key: committees up to ~500 keys on 80 GB); 18 would still need 15
+    if (c->wa_forced && w != c->wa_forced) continue;
+    wa = w;
+    if (capk * comb_table_entries(w) * sizeof(ge_niels) <= budget) break;
+  }
+  return HS_OK;
+}
 static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, uint32_t *out_valid_bitmap) {
   HS_CUDA(c, cudaSetDevice(c->device));
   // Drains every stream of the device, the verify queues' included: a queue enqueues a launch only while it holds c->mu, so
@@ -2853,15 +2884,9 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
   // host-side hash table (hashing only; first occurrence of a duplicated key wins)
   uint32_t cap = 16;
   std::vector<uint32_t> slots;
-  // widest per-key window whose tables fit in the budget: ~62 % of the device by default (80 GB H100: 16 bits up to
-  // ~1 k keys, 15 up to ~1.8 k, 14 up to ~3.3 k, 13 up to ~6.3 k, 12 up to ~11 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device
-  size_t free_b = 0, total_b = 0;
-  HS_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-  size_t budget = total_b / 100 * 62;
-  if (c->table_budget) budget = c->table_budget;
-  if (budget > free_b - free_b / 8) budget = free_b - free_b / 8;
-  // spare slots (1/16 of the set, at least 16) let hs_committee_update add validators without rebuilding anything
-  const size_t capk = N + (N / 16 > 16 ? N / 16 : 16);
+  size_t capk = 0;
+  int wa = 8;
+  HS_TRY(committee_geometry(c, N, capk, wa));
   while (cap < 2 * capk) cap <<= 1;
   slots.clear();
   slots.assign(cap, HS_NO_KEY);
@@ -2878,12 +2903,6 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
       h = (h + 1) & (cap - 1);
     }
     if (!dup) slots[h] = (uint32_t)i;
-  }
-  int wa = 8;
-  for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8}) {  // 17 bits: 15 windows (94 MB per key: committees up to ~500 keys on 80 GB); 18 would still need 15
-    if (c->wa_forced && w != c->wa_forced) continue;
-    wa = w;
-    if (capk * comb_table_entries(w) * sizeof(ge_niels) <= budget) break;
   }
   if (sc_ndigits_rt(wa) + c->cp.nb > HS_MAX_DIGITS) return fail(c, HS_ERR_ARG, "window combination exceeds HS_MAX_DIGITS");
   key_store K;  // the old tables were released above
@@ -4022,3 +4041,447 @@ void hs_queue_destroy(hs_queue *q) {
 }
 
 }  // extern "C"
+
+// ================================================================================================ known-answer self-test (hs_self_test)
+// Drives the existing kernels on private scratch, at the context's base window and a chosen per-key window, and compares their
+// verdicts, digests, keys and signatures with answers compiled into the library.  Nothing of the context is written but its launch
+// counter and its last-error text: the scratch key tables, the hash table, the queue ring, the signature table and the streams are
+// the call's own and are released before it returns.
+
+#define HS_SELFTEST_MAX_RECORDS 4096u
+#define HS_SELFTEST_FIN_GROUP 4  // records per thread of k_verify_finish, as run_verify picks for small passes
+
+namespace {
+// The records of one run: those with a 32-byte message (every path) and every record as a variable-length message (the var-length
+// path), each with its expected verdicts (bit 0 strict, bit 1 batch-eq) and its name for the error text.
+struct st_set {
+  std::vector<hs_rec128> r32;
+  std::vector<uint8_t> e32;
+  std::vector<std::string> n32;
+  std::vector<uint8_t> sig, pk, msgs;
+  std::vector<uint64_t> off{0};
+  std::vector<uint8_t> ev;
+  std::vector<std::string> nv;
+  void add(const std::string &name, const uint8_t *s, const uint8_t *k, const uint8_t *m, size_t len, uint8_t expect) {
+    if (len == 32) {
+      hs_rec128 r;
+      memcpy(r.sig, s, 64);
+      memcpy(r.pk, k, 32);
+      memcpy(r.msg, m, 32);
+      r32.push_back(r);
+      e32.push_back(expect);
+      n32.push_back(name);
+    }
+    sig.insert(sig.end(), s, s + 64);
+    pk.insert(pk.end(), k, k + 32);
+    msgs.insert(msgs.end(), m, m + len);
+    off.push_back(msgs.size());
+    ev.push_back(expect);
+    nv.push_back(name);
+  }
+};
+// Failed paths, and the first mismatch found.
+struct st_result {
+  uint32_t failed = 0;
+  std::string first;
+  void mismatch(uint32_t bit, const std::string &what) {
+    if (!failed) first = "hs_self_test: " + what;
+    failed |= bit;
+  }
+};
+// got(i): record i's verdict bits; checked bits: 3, or 1 << mode[i] when mode is given (k_verify_finish_modes).
+template <class Got>
+void st_compare(st_result &R, uint32_t bit, const char *path, const std::vector<std::string> &names, const std::vector<uint8_t> &expect,
+                const uint8_t *mode, Got got) {
+  for (size_t i = 0; i < expect.size(); i++) {
+    const uint32_t mask = mode ? 1u << mode[i] : 3u, g = got(i) & mask, want = expect[i] & mask;
+    if (g == want) continue;
+    char buf[256];
+    snprintf(buf, sizeof buf, "%s: %s (record %zu): got strict=%s batch_eq=%s, expected strict=%s batch_eq=%s", path, names[i].c_str(), i,
+             (mask & 1) ? ((g & 1) ? "1" : "0") : "-", (mask & 2) ? ((g & 2) ? "1" : "0") : "-", (mask & 1) ? ((want & 1) ? "1" : "0") : "-",
+             (mask & 2) ? ((want & 2) ? "1" : "0") : "-");
+    R.mismatch(bit, buf);
+    return;
+  }
+}
+// Waits for the private streams when it goes out of scope: declared after the buffers a helper launches on, it keeps every return path
+// from releasing memory that work in flight still uses.
+struct st_drain {
+  cudaStream_t a, b;
+  ~st_drain() {
+    cudaStreamSynchronize(a);
+    if (b) cudaStreamSynchronize(b);
+  }
+};
+uint8_t st_flag_bits(uint8_t fl) { return ((fl & HS_F_STRICT) ? 1u : 0u) | ((fl & HS_F_EQ) ? 2u : 0u); }
+uint8_t st_bitmap_bits(const std::vector<uint32_t> &strict, const std::vector<uint32_t> &eq, size_t i) {
+  return (uint8_t)(((strict[i >> 5] >> (i & 31)) & 1u) | (((eq[i >> 5] >> (i & 31)) & 1u) << 1));
+}
+}  // namespace
+
+// Device results of one path, read back on the private stream.
+static int st_read(hs_ctx *c, cudaStream_t st, void *dst, const void *src, size_t bytes) {
+  HS_CUDA(c, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st));
+  HS_CUDA(c, cudaStreamSynchronize(st));
+  return HS_OK;
+}
+
+// The three Digest kernels over the SHA-512 known answers, and k_keygen / k_sign_digests over the seeded keys.
+static int st_digest_and_sign_paths(hs_ctx *c, const comb_params &cp, cudaStream_t st, st_result &R) {
+  const size_t n = HS_ST_N_DIGEST_KATS;
+  std::vector<uint64_t> off(n + 1);
+  for (size_t i = 0; i < n; i++) off[i] = hs_st_digest_kats[i].off;
+  off[n] = HS_ST_KAT_MSG_BYTES;
+  std::vector<uint8_t> seeds(32 * (HS_ST_N_SEEDS + 1)), pks(32 * HS_ST_N_SEEDS), dig(32 * HS_ST_N_SIGNATURES);
+  std::vector<uint32_t> key_idx(HS_ST_N_SIGNATURES);
+  memcpy(seeds.data(), hs_st_seeds, 32 * HS_ST_N_SEEDS);
+  memcpy(seeds.data() + 32 * HS_ST_N_SEEDS, hs_st_tv1_seed, 32);
+  memcpy(pks.data(), hs_st_seed_pks, 32 * HS_ST_N_SEEDS);
+  for (size_t i = 0; i < HS_ST_N_SIGNATURES; i++) {
+    memcpy(dig.data() + 32 * i, hs_st_signatures[i].digest, 32);
+    key_idx[i] = hs_st_signatures[i].key;
+  }
+  dev_buf buf;
+  h2d_stage S;
+  const size_t s_off = S.add(off.data(), off.size() * 8), s_data = S.add(hs_st_kat_msgs, HS_ST_KAT_MSG_BYTES, 8), s_out = S.add(nullptr, 32 * n),
+               s_seed = S.add(seeds.data(), seeds.size()), s_pk = S.add(pks.data(), pks.size()), s_ki = S.add(key_idx.data(), key_idx.size() * 4),
+               s_dig = S.add(dig.data(), dig.size()), s_res = S.add(nullptr, 64 * (HS_ST_N_SEEDS + 1 + HS_ST_N_SIGNATURES));
+  HS_TRY(S.upload(c, buf, st));
+  const st_drain drain{st, nullptr};
+  uint32_t *d_out = (uint32_t *)S.ptr(s_out);
+  std::vector<uint8_t> got(32 * n);
+  auto check_digests = [&](uint32_t bit, const char *path, size_t i) {
+    if (memcmp(got.data() + 32 * i, hs_st_digest_kats[i].digest, 32) == 0) return;
+    char b[160];
+    snprintf(b, sizeof b, "%s: digest known answer %zu (%u bytes): wrong Digest", path, i, hs_st_digest_kats[i].len);
+    R.mismatch(bit, b);
+  };
+  k_digest32<<<blocks_for(n), HS_THREADS, 0, st>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), 0, n, d_out);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(st_read(c, st, got.data(), d_out, 32 * n));
+  for (size_t i = 0; i < n; i++) check_digests(HS_SELFTEST_DIGEST, "k_digest32", i);
+  HS_CUDA(c, cudaMemsetAsync(d_out, 0, 32 * n, st));
+  k_digest32_long<<<(unsigned)n, 32, 0, st>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, d_out);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(st_read(c, st, got.data(), d_out, 32 * n));
+  for (size_t i = 0; i < n; i++) check_digests(HS_SELFTEST_DIGEST_LONG, "k_digest32_long", i);
+  // k_digest32_fixed takes 16-byte aligned messages of at least one full block, one launch per length
+  for (size_t i = 0; i < n; i++) {
+    const hs_st_digest_kat &k = hs_st_digest_kats[i];
+    if (k.len < 128 || (k.len & 15)) continue;
+    dev_mem<uint8_t> m;
+    HS_CUDA(c, alloc(m, k.len));
+    const st_drain drain_m{st, nullptr};
+    HS_CUDA(c, cudaMemcpyAsync(m, hs_st_kat_msgs + k.off, k.len, cudaMemcpyHostToDevice, st));
+    HS_CUDA(c, cudaMemsetAsync(d_out, 0, 32, st));
+    HS_TRY(launch_digest_fixed(c, m, k.len, 1, d_out, st));
+    HS_TRY(st_read(c, st, got.data() + 32 * i, d_out, 32));
+    check_digests(HS_SELFTEST_DIGEST_FIXED, "k_digest32_fixed", i);
+  }
+  // keys of the seeded test keys and RFC 8032 TEST 1, then the signatures of 32-byte digests
+  uint8_t *d_res = S.ptr(s_res);
+  k_keygen<<<1, HS_THREADS, 0, st>>>(S.ptr(s_seed), HS_ST_N_SEEDS + 1, c->d_btable, cp, d_res);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  uint8_t *d_sig = d_res + 32 * (HS_ST_N_SEEDS + 1);
+  k_sign_digests<<<1, HS_THREADS, 0, st>>>(S.ptr(s_seed), S.ptr(s_pk), (const uint32_t *)S.ptr(s_ki), S.ptr(s_dig), HS_ST_N_SIGNATURES, HS_ST_N_SEEDS,
+                                           c->d_btable, cp, d_sig);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  std::vector<uint8_t> res(32 * (HS_ST_N_SEEDS + 1) + 64 * HS_ST_N_SIGNATURES);
+  HS_TRY(st_read(c, st, res.data(), d_res, res.size()));
+  for (size_t i = 0; i <= HS_ST_N_SEEDS; i++) {
+    const uint8_t *want = i < HS_ST_N_SEEDS ? hs_st_seed_pks[i] : hs_st_tv1_pk;
+    if (memcmp(res.data() + 32 * i, want, 32) == 0) continue;
+    R.mismatch(HS_SELFTEST_SIGN, i < HS_ST_N_SEEDS ? "k_keygen: seeded key " + std::to_string(i) + ": wrong public key"
+                                                   : std::string("k_keygen: RFC 8032 TEST 1: wrong public key"));
+    break;
+  }
+  for (size_t i = 0; i < HS_ST_N_SIGNATURES; i++) {
+    if (memcmp(res.data() + 32 * (HS_ST_N_SEEDS + 1) + 64 * i, hs_st_signatures[i].sig, 64) == 0) continue;
+    R.mismatch(HS_SELFTEST_SIGN, "k_sign_digests: signature " + std::to_string(i) + ": wrong signature");
+    break;
+  }
+  return HS_OK;
+}
+
+// The scratch per-key tables: the set's distinct keys, built by k_build_comb at window cp.wa like a registration, and a hash table built
+// on the host over every key but `foreign`, whose records therefore miss k_key_lookup and take the side-stream generic pass.
+struct st_keys {
+  std::vector<uint8_t> pks;  // distinct keys, 32 bytes each, in first-seen order
+  std::unordered_map<std::string, uint32_t> index;
+  std::vector<uint32_t> slots;
+  key_store K;
+  uint32_t idx(const uint8_t *pk) const { return index.at(std::string((const char *)pk, 32)); }
+};
+static int st_build_keys(hs_ctx *c, const st_set &T, const comb_params &cp, st_keys &KS, pass_tables &K, cudaStream_t st) {
+  const size_t n = KS.pks.size() / 32, entries = comb_table_entries(cp.wa);
+  uint32_t cap = 16;
+  while (cap < 2 * n) cap <<= 1;
+  const uint32_t foreign = T.r32.empty() ? HS_NO_KEY : KS.idx(T.r32[0].pk);
+  KS.slots.assign(cap, HS_NO_KEY);
+  for (uint32_t i = 0; i < n; i++) {
+    if (i == foreign) continue;
+    uint32_t w[8];
+    memcpy(w, KS.pks.data() + 32 * (size_t)i, 32);
+    uint32_t h = key_hash(w) & (cap - 1);
+    while (KS.slots[h] != HS_NO_KEY) h = (h + 1) & (cap - 1);
+    KS.slots[h] = i;
+  }
+  cudaError_t e = alloc(KS.K.pks, n * 32);
+  if (e == cudaSuccess) e = alloc(KS.K.key_flags, n);
+  if (e == cudaSuccess) e = alloc(KS.K.slots, (size_t)cap * 4);
+  if (e == cudaSuccess) e = alloc(KS.K.atables, n * entries * sizeof(ge_niels));
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, HS_ERR_NOMEM, "hs_self_test: the scratch key tables do not fit in device memory", e);
+  }
+  HS_CUDA(c, cudaMemcpyAsync(KS.K.pks, KS.pks.data(), n * 32, cudaMemcpyHostToDevice, st));
+  HS_CUDA(c, cudaMemcpyAsync(KS.K.slots, KS.slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, st));
+  const size_t threads = n * (size_t)cp.na * ((1u << (cp.wa - 1)) / HS_BUILD_BLOCK);
+  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, st>>>(KS.K.pks, n, 1, cp.wa, cp.na, KS.K.atables, KS.K.key_flags);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  K = pass_tables{{KS.K.pks, KS.K.key_flags, (uint32_t)n, KS.K.atables, entries}, {KS.K.slots, cap - 1, KS.K.pks, (uint32_t)n}, cp};
+  return HS_OK;
+}
+
+// Every verify path over the set: the throughput passes (k_verify_main + k_verify_finish in both modes, k_verify_finish_modes) and the
+// queue kernels on a private mapped ring.
+static int st_verify_paths(hs_ctx *c, const st_set &T, const st_keys &KS, const pass_tables &K, cudaStream_t st, cudaStream_t side,
+                           st_result &R) {
+  const size_t n = T.r32.size(), nv = T.ev.size(), nmax = std::max(n, nv);
+  std::vector<uint32_t> vidx(n);
+  std::vector<uint8_t> modes(n);
+  for (size_t i = 0; i < n; i++) {
+    vidx[i] = KS.idx(T.r32[i].pk);
+    modes[i] = (uint8_t)(i & 1);
+  }
+  const size_t words = (nmax + 31) / 32;
+  dev_buf buf;
+  h2d_stage S;
+  const size_t s_recs = S.add(T.r32.data(), n * sizeof(hs_rec128)), s_vidx = S.add(vidx.data(), n * 4), s_modes = S.add(modes.data(), n),
+               s_sig = S.add(T.sig.data(), nv * 64), s_pk = S.add(T.pk.data(), nv * 32), s_off = S.add(T.off.data(), (nv + 1) * 8),
+               s_msg = S.add(T.msgs.data(), T.msgs.size(), 8);
+  HS_TRY(S.upload(c, buf, st));
+  dev_mem<fe> xyz;
+  dev_mem<uint8_t> meta;
+  dev_mem<uint32_t> lk, bm;  // lk: the lookup's indices, misses and miss count; bm: the strict, batch-eq and mixed-mode bitmaps
+  HS_CUDA(c, alloc(xyz, nmax * 3 * sizeof(fe)));
+  HS_CUDA(c, alloc(meta, nmax));
+  HS_CUDA(c, alloc(lk, 2 * n * 4 + 4));
+  HS_CUDA(c, alloc(bm, 3 * words * 4));
+  event_h ev_side[2];
+  for (event_h &ev : ev_side) HS_CUDA(c, create(ev));
+  const st_drain drain{st, side};
+  const pass_scratch PS{xyz, meta, lk, lk + n, lk + 2 * n, side, {ev_side[0], ev_side[1]}, nullptr};
+  std::vector<uint32_t> strict(words), eq(words), mixed(words);
+  // one main phase, then the finish kernel in both modes (and with mixed mode bytes), the bitmaps compared with the expectations
+  auto pass = [&](uint32_t bit, const char *path, in_layout L, bool var, bool committee, bool indexed, uint32_t modes_bit) -> int {
+    const size_t cnt = var ? nv : n;
+    if (cnt == 0) return HS_OK;
+    HS_CUDA(c, cudaMemsetAsync(bm, 0, 3 * words * 4, st));
+    HS_TRY(launch_main(c, L, cnt, committee, indexed, K, PS, st, [](bool) { return HS_OK; }));
+    HS_TRY(launch_finish(c, L, cnt, PS.xyz, PS.meta, HS_MODE_STRICT, nullptr, bm, peer_route{}, HS_SELFTEST_FIN_GROUP, st));
+    HS_TRY(launch_finish(c, L, cnt, PS.xyz, PS.meta, HS_MODE_BATCH_EQ, nullptr, bm + words, peer_route{}, HS_SELFTEST_FIN_GROUP, st));
+    if (modes_bit)
+      HS_TRY(launch_finish(c, L, cnt, PS.xyz, PS.meta, HS_MODE_STRICT, S.ptr(s_modes), bm + 2 * words, peer_route{}, HS_SELFTEST_FIN_GROUP, st));
+    HS_CUDA(c, cudaMemcpyAsync(strict.data(), bm, words * 4, cudaMemcpyDeviceToHost, st));
+    HS_CUDA(c, cudaMemcpyAsync(eq.data(), bm + words, words * 4, cudaMemcpyDeviceToHost, st));
+    HS_TRY(st_read(c, st, mixed.data(), bm + 2 * words, words * 4));
+    st_compare(R, bit, path, var ? T.nv : T.n32, var ? T.ev : T.e32, nullptr, [&](size_t i) { return st_bitmap_bits(strict, eq, i); });
+    if (modes_bit)
+      st_compare(R, modes_bit, "k_verify_finish_modes", T.n32, T.e32, modes.data(),
+                 [&](size_t i) { return (uint8_t)(((mixed[i >> 5] >> (i & 31)) & 1u) << modes[i]); });
+    return HS_OK;
+  };
+  const uint8_t *recs = S.ptr(s_recs);
+  HS_TRY(pass(HS_SELFTEST_GENERIC, "k_verify_main<generic> (packed records)", layout_rec128(recs), false, false, false, 0));
+  HS_TRY(pass(HS_SELFTEST_VAR, "k_verify_main<generic> (variable-length messages)",
+              in_layout{S.ptr(s_sig), 64, S.ptr(s_pk), 32, nullptr, S.ptr(s_msg), 0, nullptr, (const uint64_t *)S.ptr(s_off), 0, 0}, true, false, false, 0));
+  HS_TRY(pass(HS_SELFTEST_COMMITTEE, "k_verify_main<committee> (committee indices)",
+              in_layout{recs, 128, nullptr, 0, (const uint32_t *)S.ptr(s_vidx), recs + 96, 128, nullptr, nullptr, 32, 0}, false, true, true,
+              HS_SELFTEST_MODES));
+  HS_TRY(pass(HS_SELFTEST_LOOKUP, "k_key_lookup + k_verify_main<committee> + side pass", layout_rec128(recs), false, true, false, 0));
+  if (n == 0) return HS_OK;
+
+  // the queue kernels: one request of n records in slot 0 of a private mapped ring
+  uint32_t cap = HS_SMALL_MAX;
+  while (cap < n) cap <<= 1;
+  const uint32_t mask = cap - 1, buckets = std::max(cap / 2, 16u);
+  mapped<small_rec> ring;
+  mapped<uint8_t> flags, pk;
+  mapped<uint32_t> done, slot, hctr;
+  dev_mem<uint32_t> counters, ctr;
+  dev_mem<sig_bucket> table;
+  dev_mem<uint64_t> key;
+  HS_CUDA(c, alloc(ring, (size_t)cap * sizeof(small_rec)));
+  HS_CUDA(c, alloc(flags, cap));
+  HS_CUDA(c, alloc(pk, (size_t)cap * 32));
+  HS_CUDA(c, alloc(done, (size_t)cap * 4));
+  HS_CUDA(c, alloc(slot, (size_t)cap * 4));
+  HS_CUDA(c, alloc(hctr, (size_t)cap * 4 * HS_SIG_CTRS));
+  HS_CUDA(c, alloc(counters, (size_t)cap * 4));
+  HS_CUDA(c, alloc(ctr, (size_t)cap * 4 * HS_SIG_CTRS));
+  HS_CUDA(c, alloc(table, (size_t)buckets * sizeof(sig_bucket)));
+  HS_CUDA(c, alloc(key, 32 * 8));
+  const st_drain drain_ring{st, nullptr};
+  uint64_t kh[32];
+  uint64_t z = 0x243f6a8885a308d3ull;  // any fixed key: the table is private and short-lived
+  for (uint64_t &k : kh) k = (z += 0x9e3779b97f4a7c15ull) ^ (z >> 29);
+  HS_CUDA(c, cudaMemcpyAsync(key, kh, sizeof kh, cudaMemcpyHostToDevice, st));
+  HS_CUDA(c, cudaMemsetAsync(counters, 0, (size_t)cap * 4, st));
+  HS_CUDA(c, cudaMemsetAsync(ctr, 0, (size_t)cap * 4 * HS_SIG_CTRS, st));
+  memset(ring.h, 0, (size_t)cap * sizeof(small_rec));
+  memset(done.h, 0, (size_t)cap * 4);
+  for (uint32_t i = 0; i < n; i++) {
+    memcpy(ring.h[i].sig, T.r32[i].sig, 64);
+    memcpy(ring.h[i].msg, T.r32[i].msg, 32);
+    ring.h[i].vidx = vidx[i];
+    ring.h[i].req = 0;
+    ring.h[i].req_n = (uint32_t)n;
+    memcpy(pk.h + 32 * (size_t)i, T.r32[i].pk, 32);
+    slot.h[i] = i;
+  }
+  const sig_cache_dev sc{table, key, buckets - 1, ctr, hctr.d};
+  const unsigned blocks = (unsigned)((n + HS_BULK_THREADS - 1) / HS_BULK_THREADS);
+  uint32_t seq = 0;
+  // launch(seq) enqueues one kernel over the request; its completion word and its records' flags are then compared
+  auto queue_pass = [&](uint32_t bit, const char *path, auto launch) -> int {
+    memset(flags.h, 0, cap);
+    launch(++seq);
+    c->launches++;
+    HS_CUDA(c, cudaGetLastError());
+    HS_CUDA(c, cudaStreamSynchronize(st));
+    if (((volatile uint32_t *)done.h)[0] != seq) {
+      R.mismatch(bit, std::string(path) + ": the request did not complete");
+      return HS_OK;
+    }
+    st_compare(R, bit, path, T.n32, T.e32, nullptr, [&](size_t i) { return st_flag_bits(flags.h[i]); });
+    return HS_OK;
+  };
+  const ge_niels *bt = c->d_btable;
+  const pass_tables &P = K;
+  HS_TRY(queue_pass(HS_SELFTEST_SMALL, "k_verify_small", [&](uint32_t s) {
+    k_verify_small<false><<<(unsigned)n, 64, 0, st>>>(ring.d, 0, mask, bt, P.C, P.cp, flags.d, counters, done.d, s, sig_cache_dev{});
+  }));
+  HS_TRY(queue_pass(HS_SELFTEST_BULK, "k_verify_bulk", [&](uint32_t s) {
+    k_verify_bulk<false><<<blocks, HS_BULK_THREADS, 0, st>>>(ring.d, 0, mask, (uint32_t)n, bt, P.C, P.cp, flags.d, counters, done.d, s, sig_cache_dev{});
+  }));
+  HS_TRY(queue_pass(HS_SELFTEST_QUEUE_GENERIC, "k_queue_generic", [&](uint32_t s) {
+    k_queue_generic<<<blocks, HS_GEN_THREADS, 0, st>>>(ring.d, pk.d, slot.d, 0, mask, (uint32_t)n, bt, P.cp, flags.d, counters, done.d, s);
+  }));
+  // the signature-cache instantiations run twice on an empty table: the first run probes, misses and inserts, the second answers from it
+  for (int cached = 0; cached < 2; cached++) {
+    HS_CUDA(c, cudaMemsetAsync(table, 0, (size_t)buckets * sizeof(sig_bucket), st));
+    for (int run = 0; run < 2; run++) {
+      if (cached == 0)
+        HS_TRY(queue_pass(HS_SELFTEST_SMALL_CACHE, run ? "k_verify_small<cache> (cache filled)" : "k_verify_small<cache> (empty cache)",
+                          [&](uint32_t s) {
+                            k_verify_small<true><<<(unsigned)n, 64, 0, st>>>(ring.d, 0, mask, bt, P.C, P.cp, flags.d, counters, done.d, s, sc);
+                          }));
+      else
+        HS_TRY(queue_pass(HS_SELFTEST_BULK_CACHE, run ? "k_verify_bulk<cache> (cache filled)" : "k_verify_bulk<cache> (empty cache)",
+                          [&](uint32_t s) {
+                            k_verify_bulk<true><<<blocks, HS_BULK_THREADS, 0, st>>>(ring.d, 0, mask, (uint32_t)n, bt, P.C, P.cp, flags.d, counters,
+                                                                                    done.d, s, sc);
+                          }));
+    }
+  }
+  return HS_OK;
+}
+
+// k_queue_digests over the SHA-512 known answers: one request of one record per preimage on a private ring; each record's msg field
+// must receive its preimage's Digest.
+static int st_queue_digest_path(hs_ctx *c, cudaStream_t st, st_result &R) {
+  const uint32_t m = HS_ST_N_DIGEST_KATS, n = HS_ST_N_DIGEST_KATS, cap = HS_SMALL_MAX;
+  const uint64_t bytes = qmsg_bytes(m, n, HS_ST_KAT_MSG_BYTES);
+  mapped<uint8_t> arena;
+  mapped<qmsg_desc> list;
+  mapped<small_rec> ring;
+  dev_mem<uint8_t> stage;
+  dev_mem<uint32_t> digs;
+  HS_CUDA(c, alloc(arena, bytes));
+  HS_CUDA(c, alloc(list, sizeof(qmsg_desc)));
+  HS_CUDA(c, alloc(ring, (size_t)cap * sizeof(small_rec)));
+  HS_CUDA(c, alloc(stage, bytes));
+  HS_CUDA(c, alloc(digs, bytes * 4));
+  const st_drain drain{st, nullptr};
+  memset(arena.h, 0, bytes);
+  memset(ring.h, 0, (size_t)cap * sizeof(small_rec));
+  uint64_t *off = reinterpret_cast<uint64_t *>(arena.h.get());
+  uint32_t *msg_idx = reinterpret_cast<uint32_t *>(arena.h + 8 * ((size_t)m + 1));
+  for (uint32_t i = 0; i < m; i++) {
+    off[i] = hs_st_digest_kats[i].off;
+    msg_idx[i] = i;
+  }
+  off[m] = HS_ST_KAT_MSG_BYTES;
+  memcpy(arena.h + qmsg_o_pre(m, n), hs_st_kat_msgs, HS_ST_KAT_MSG_BYTES);
+  *list.h = qmsg_desc{0, m, n, 0, HS_ST_KAT_MSG_BYTES, {0, 0, 0}};
+  k_queue_digests<<<1, HS_QDIG_THREADS, 0, st>>>(list.d, 0, cap - 1, arena.d, stage, digs, ring.d);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  HS_CUDA(c, cudaStreamSynchronize(st));
+  for (uint32_t i = 0; i < n; i++) {
+    if (memcmp(ring.h[i].msg, hs_st_digest_kats[i].digest, 32) == 0) continue;
+    R.mismatch(HS_SELFTEST_QUEUE_DIGESTS, "k_queue_digests: digest known answer " + std::to_string(i) + ": wrong Digest");
+    break;
+  }
+  return HS_OK;
+}
+
+static int self_test_locked(hs_ctx *c, int key_bits, const hs_rec128 *recs, const uint8_t *expect, size_t n, uint32_t *out_failed) {
+  HS_CUDA(c, cudaSetDevice(c->device));
+  st_set T;
+  if (!recs) {
+    for (const hs_st_vector &v : hs_st_vectors) T.add(v.name, v.sig, v.pk, hs_st_vec_msgs + v.msg_off, v.msg_len, v.expect);
+  } else {
+    for (size_t i = 0; i < n; i++) T.add("caller record " + std::to_string(i), recs[i].sig, recs[i].pk, recs[i].msg, 32, expect[i]);
+  }
+  st_keys KS;
+  for (size_t i = 0; i < T.ev.size(); i++) {
+    const std::string k((const char *)T.pk.data() + 32 * i, 32);
+    if (KS.index.emplace(k, (uint32_t)(KS.pks.size() / 32)).second) KS.pks.insert(KS.pks.end(), k.begin(), k.end());
+  }
+  int wa = key_bits;
+  if (wa == 0 && c->keys.atables) wa = c->cp.wa;  // the registered committee's window, or the key cache's
+  if (wa == 0) {                                  // neither: the window registering these keys would get now
+    size_t capk = 0;
+    HS_TRY(committee_geometry(c, KS.pks.size() / 32, capk, wa));
+  }
+  comb_params cp = c->cp;
+  set_window(cp, true, wa);
+  if (cp.na + cp.nb > HS_MAX_DIGITS) return fail(c, HS_ERR_ARG, "hs_self_test: window combination exceeds HS_MAX_DIGITS");
+  stream_h st, side;  // private: the work of this call only (the drain below waits for both before any scratch is released)
+  int lo = 0, hi = 0;
+  HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+  HS_CUDA(c, create(st));
+  HS_CUDA(c, create(side, hi));
+  st_result R;
+  {
+    const st_drain drain{st, side};
+    pass_tables K;
+    HS_TRY(st_build_keys(c, T, cp, KS, K, st));
+    if (!recs) {
+      HS_TRY(st_digest_and_sign_paths(c, cp, st, R));
+      HS_TRY(st_queue_digest_path(c, st, R));
+    }
+    HS_TRY(st_verify_paths(c, T, KS, K, st, side, R));
+  }
+  HS_CUDA(c, cudaGetLastError());
+  *out_failed = R.failed;
+  return R.failed ? fail(c, HS_ERR_SELFTEST, R.first.c_str()) : HS_OK;
+}
+
+extern "C" int hs_self_test(hs_ctx *c, int key_bits, const hs_rec128 *recs, const uint8_t *expect, size_t n, uint32_t *out_failed_paths) {
+  if (out_failed_paths) *out_failed_paths = 0;
+  if (!c || !out_failed_paths || (key_bits != 0 && (key_bits < 8 || key_bits > 17))) return fail(c, HS_ERR_ARG, "hs_self_test: bad argument");
+  if (recs ? (!expect || n == 0 || n > HS_SELFTEST_MAX_RECORDS) : (expect || n != 0))
+    return fail(c, HS_ERR_ARG, "hs_self_test: caller records need expectations and 1 .. 4096 records; the built-in set takes none");
+  for (size_t i = 0; recs && i < n; i++)
+    if (expect[i] > 3) return fail(c, HS_ERR_ARG, "hs_self_test: an expectation byte uses bits other than 0 and 1");
+  std::lock_guard<std::mutex> g(c->mu);
+  return self_test_locked(c, key_bits, recs, expect, n, out_failed_paths);
+}

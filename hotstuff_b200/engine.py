@@ -12,6 +12,7 @@ from . import _lib
 
 MODE_STRICT = 0    # Signature::verify      (crypto/src/lib.rs:200-204)
 MODE_BATCH_EQ = 1  # Signature::verify_batch (crypto/src/lib.rs:206-219), per-signature condition
+HS_ERR_SELFTEST = 4  # hs_self_test: a path gave a wrong answer
 
 
 class EngineError(RuntimeError):
@@ -84,6 +85,27 @@ class Engine:
     @property
     def kernel_launches(self):
         return int(self.lib.hs_kernel_launches(self.h))
+
+    def self_test(self, key_bits=0, recs=None, expect=None):
+        """Known-answer self-test of every device path at this context's geometry (hs_self_test).  recs: (n,128) uint8 records and
+        expect: n bytes (bit 0 strict, bit 1 batch-eq), or None for the built-in set; key_bits: 0 = the per-key window in use, 8..17 to
+        force one.  Returns the mask of failing paths (HS_SELFTEST_* bits; 0 = every answer right, hs_last_error names the first
+        mismatch otherwise).  Raises EngineError on a bad argument, no device memory for the scratch tables or a CUDA error."""
+        failed = ctypes.c_uint32(0)
+        if recs is None:
+            rc = self.lib.hs_self_test(self.h, int(key_bits), None, None if expect is None else _ptr(_u8(expect)), 0, ctypes.byref(failed))
+        else:
+            recs = _u8(recs, 128).reshape(-1, 128)
+            exp = None if expect is None else _u8(expect)
+            rc = self.lib.hs_self_test(self.h, int(key_bits), _ptr(recs), _ptr(exp), recs.shape[0], ctypes.byref(failed))
+        if rc == HS_ERR_SELFTEST:
+            return int(failed.value)
+        self._check(rc, "hs_self_test")
+        return 0
+
+    @property
+    def last_error(self):
+        return self.lib.hs_last_error(self.h).decode()
 
     # ---- host-buffer API -------------------------------------------------------------------------------------
     def verify_rec128(self, recs, mode=MODE_STRICT):

@@ -30,6 +30,7 @@ extern "C" {
 #define HS_ERR_CUDA 1
 #define HS_ERR_ARG 2
 #define HS_ERR_NOMEM 3
+#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer */
 
 /* verdict selector for the verify entry points */
 #define HS_MODE_STRICT 0u /* Signature::verify semantics  = dalek verify_strict          (crypto/src/lib.rs:200-204) */
@@ -339,6 +340,45 @@ int hs_digest32_batch(hs_ctx *ctx, const uint8_t *data, const uint64_t *off, siz
  * over it, overlapping the host->device copy of one chunk with the kernels of the previous one. */
 int hs_verify_msgs(hs_ctx *ctx, const uint8_t *sig /* n x 64 */, const uint8_t *pk_or_null /* n x 32 */, const uint32_t *validator_idx_or_null,
                    const uint8_t *msgs, size_t msg_len, size_t n, uint32_t mode, uint32_t *out_bitmap);
+
+/* ---- known-answer self-test: every device path at this context's table geometry ------------------------------------------
+ * A node has no CPU verifier behind the engine, and its table geometry is chosen at run time (base window from hs_ctx_create, per-key
+ * window from the table budget and free memory).  This call drives every kernel below on private scratch and compares the answers with
+ * ones compiled into the library (the golden vectors: RFC 8032, the reference crate's test signatures, adversarial and small-order
+ * cases, the SHA-512 known answers).  Call it at start-up, after hs_committee_register: a failure means this box gives wrong verdicts,
+ * not an error code, and the engine must not be used.
+ *   - recs == NULL: the built-in set (expect == NULL, n == 0).  Otherwise the caller's n (1 .. 4,096) records with their expected
+ *     verdicts run through every verify path: expect[i] bit 0 = the strict verdict, bit 1 = the batch-eq verdict.  The Digest,
+ *     k_queue_digests and signer paths run only with the built-in set.  Built-in vectors whose message is not 32 bytes take only the
+ *     variable-length path.
+ *   - key_bits: 0 = the per-key window in use (the registered committee's, or the key cache's when it holds tables; with neither,
+ *     the window registering the set's keys would pick under the current budget), or 8 .. 17 to force one.  The base-point table is
+ *     always the context's own.  The committee paths use scratch tables for the set's distinct keys, built at that window (the 39
+ *     distinct keys of the built-in set: about 0.3 GB at 13 bits, 3.7 GB at 17) and released before the call returns.
+ *   - Returns HS_OK with *out_failed_paths = 0; HS_ERR_SELFTEST with one HS_SELFTEST_* bit per failing path, hs_last_error naming the
+ *     first mismatch (path, vector name or record index, got and expected bits); HS_ERR_ARG for bad sizes, recs without expect, an
+ *     expect byte above 3 or key_bits out of range; HS_ERR_NOMEM when the scratch tables do not fit in device memory.
+ *   - Isolation: holds the context's mutex and runs on private streams; the registered committee, the key cache and its learning, the
+ *     deferred scratch sets, the peer route, profiling and every verify queue (ring, caches, counters, stats) are not touched, so
+ *     queues may keep working meanwhile.  Its launches count in hs_kernel_launches.  Like every host-pointer entry point it must not
+ *     be mixed with deferred `_dev` passes in flight. */
+#define HS_SELFTEST_DIGEST (1u << 0)          /* k_digest32 */
+#define HS_SELFTEST_DIGEST_FIXED (1u << 1)    /* k_digest32_fixed */
+#define HS_SELFTEST_DIGEST_LONG (1u << 2)     /* k_digest32_long */
+#define HS_SELFTEST_GENERIC (1u << 3)         /* k_verify_main<generic> on packed records + k_verify_finish, both modes */
+#define HS_SELFTEST_VAR (1u << 4)             /* the same over variable-length messages */
+#define HS_SELFTEST_COMMITTEE (1u << 5)       /* k_verify_main<committee> with committee indices + k_verify_finish, both modes */
+#define HS_SELFTEST_LOOKUP (1u << 6)          /* k_key_lookup + k_verify_main<committee>, a key outside the table on the side-stream pass */
+#define HS_SELFTEST_MODES (1u << 7)           /* k_verify_finish_modes, mixed mode bytes */
+#define HS_SELFTEST_SMALL (1u << 8)           /* k_verify_small */
+#define HS_SELFTEST_SMALL_CACHE (1u << 9)     /* k_verify_small with a signature table, empty then filled */
+#define HS_SELFTEST_BULK (1u << 10)           /* k_verify_bulk */
+#define HS_SELFTEST_BULK_CACHE (1u << 11)     /* k_verify_bulk with a signature table, empty then filled */
+#define HS_SELFTEST_QUEUE_GENERIC (1u << 12)  /* k_queue_generic */
+#define HS_SELFTEST_QUEUE_DIGESTS (1u << 13)  /* k_queue_digests */
+#define HS_SELFTEST_SIGN (1u << 14)           /* k_keygen + k_sign_digests */
+#define HS_SELFTEST_VERIFY_PATHS 0x1ff8u      /* GENERIC .. QUEUE_GENERIC: the paths caller records run through */
+int hs_self_test(hs_ctx *ctx, int key_bits, const hs_rec128 *recs_or_null, const uint8_t *expect_or_null, size_t n, uint32_t *out_failed_paths);
 
 /* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) ------------------- */
 int hs_verify_rec128_dev(hs_ctx *ctx, const void *d_recs, size_t n, uint32_t mode, void *d_bitmap, void *stream);

@@ -39,6 +39,16 @@ class Engine {
   void check(int rc, const char *what) const {
     if (rc != HS_OK) throw EngineError(std::string(what) + ": " + hs_last_error(ctx_));
   }
+  // Known-answer self-test of every device path at this context's geometry (hs_self_test, built-in set, key_bits 0 = the window in
+  // use): 0 when every answer is right, else the HS_SELFTEST_* bits of the failing paths (error() names the first mismatch).  Throws
+  // EngineError when the test cannot run (no device memory for its scratch tables, CUDA error).
+  uint32_t self_test(int key_bits = 0) const {
+    uint32_t failed = 0;
+    const int rc = hs_self_test(ctx_, key_bits, nullptr, nullptr, 0, &failed);
+    if (rc != HS_ERR_SELFTEST) check(rc, "hs_self_test");
+    return failed;
+  }
+  std::string error() const { return hs_last_error(ctx_); }
 
  private:
   hs_ctx *ctx_ = nullptr;

@@ -12,6 +12,7 @@
 //   * batch front ends for the consensus call sites: many QCs (view-change burst), TC votes, and whole bincode frames
 //     (ingest_frames + verify_ingested: the receiver path of consensus.rs:138 without building the message structs first).
 use std::os::raw::c_int;
+use std::sync::atomic::{AtomicBool, Ordering};
 use std::sync::OnceLock;
 
 /// The verify queue (hs_queue_*): concurrent single-message verifies share latency-path launches (`queue::verify_queued`).
@@ -86,15 +87,19 @@ extern "C" {
                         msg_idx: *const u32, group_idx: *const u32, mode: *const u8, n_items: usize, n_groups: usize,
                         out_item_bitmap: *mut u32, out_group_bitmap: *mut u32) -> c_int;
     fn hs_ingest_consensus_frames(frames: *const u8, off: *const u64, n: usize, info: *mut HsFrameInfo, out: *mut HsIngestOut) -> c_int;
+    fn hs_self_test(ctx: *mut HsCtx, key_bits: c_int, recs: *const HsRec128, expect: *const u8, n: usize, out_failed_paths: *mut u32) -> c_int;
 }
 
 struct Ctx(*mut HsCtx);
 unsafe impl Send for Ctx {}
 unsafe impl Sync for Ctx {}            // host-pointer entry points are serialised on the context's mutex
 static CTX: OnceLock<Option<Ctx>> = OnceLock::new();
+/// Set when `self_test` fails: the engine gives wrong answers on this box, so every call below answers None (the dalek path).
+static DISABLED: AtomicBool = AtomicBool::new(false);
 
-/// None when no GPU / the library failed to initialise: every caller below then stays on the CPU path.
+/// None when no GPU / the library failed to initialise / the self-test failed: every caller below then stays on the CPU path.
 fn ctx() -> Option<*mut HsCtx> {
+    if DISABLED.load(Ordering::Acquire) { return None; }
     CTX.get_or_init(|| {
         let mut p = std::ptr::null_mut();
         if unsafe { hs_ctx_create(&mut p, 0, 0) } == HS_OK && !p.is_null() { Some(Ctx(p)) } else { None }
@@ -116,6 +121,17 @@ pub fn register_committee(keys: &[[u8; 32]]) -> Result<(), GpuError> {
     if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
     let bad: Vec<usize> = (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect();
     if bad.is_empty() { Ok(()) } else { Err(GpuError::InvalidKeys(bad)) }
+}
+/// Known-answer self-test of every GPU path at the context's table geometry (hs_self_test, built-in vectors, the window in use).  Call
+/// it once at start-up, after `register_committee`.  On any failure the GPU is switched off for the life of the process: every call
+/// below then returns None and the caller takes its dalek / sha2 path.
+pub fn self_test() -> Result<(), GpuError> {
+    let c = ctx().ok_or(GpuError::Unavailable)?;
+    let mut failed = 0u32;
+    let rc = unsafe { hs_self_test(c, 0, std::ptr::null(), std::ptr::null(), 0, &mut failed) };
+    if rc == HS_OK && failed == 0 { return Ok(()); }
+    DISABLED.store(true, Ordering::Release);
+    Err(GpuError::Engine(format!("self-test failed (status {}, paths {:#x}): {}", rc, failed, last_error(c))))
 }
 /// Incremental epoch change: returns the table indices of the added validators.
 pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {

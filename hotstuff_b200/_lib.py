@@ -76,6 +76,17 @@ SIGNATURES = {
     "hs_queue_batch_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_destroy": (None, [c_void_p]),
     "hs_self_test": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_u32)]),
+    "hs_multi_create": (c_int, [ctypes.POINTER(c_void_p), c_void_p, c_size_t, c_u32]),
+    "hs_multi_destroy": (None, [c_void_p]),
+    "hs_multi_last_error": (ctypes.c_char_p, [c_void_p]),
+    "hs_multi_members": (c_size_t, [c_void_p]),
+    "hs_multi_member": (c_void_p, [c_void_p, c_size_t]),
+    "hs_multi_committee_register": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
+    "hs_multi_committee_update": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
+    "hs_multi_verify_rec128": (c_int, [c_void_p, c_void_p, c_size_t, c_u32, c_void_p]),
+    "hs_multi_verify_msgs": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_u32, c_void_p]),
+    "hs_multi_verify_groups": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                       c_size_t, c_void_p, c_void_p]),
 }
 
 # hs_queue_cb: void (void *user, size_t ticket, int status, const uint32_t *bitmap)

@@ -34,7 +34,8 @@ def build_engine(force=False, verbose=False):
     if not force and _newer(LIB, srcs):
         return LIB
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, os.path.join(CSRC, "hs_engine.cu"), os.path.join(CSRC, "hs_ingest.cpp")]
+    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, os.path.join(CSRC, "hs_engine.cu"), os.path.join(CSRC, "hs_ingest.cpp"),
+                                                                                 os.path.join(CSRC, "hs_multi.cpp")]
     subprocess.check_call(cmd, cwd=ROOT)
     return LIB
 

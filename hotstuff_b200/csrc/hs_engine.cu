@@ -44,6 +44,7 @@
 #include <vector>
 
 #include "../../include/hs_crypto.h"
+#include "hs_args.h"
 #include "hs_selftest_vectors.h"
 #include "verify_core.cuh"
 
@@ -2723,6 +2724,27 @@ static in_layout layout_rec128(const void *d_recs) {
   return in_layout{r, 128, r + 64, 128, nullptr, r + 96, 128, nullptr, nullptr, 32, 1};
 }
 
+// ---- argument checks shared with the multi-device context (hs_args.h)
+const char *hs_args::rec128(const hs_rec128 *recs, size_t n, uint32_t mode, const uint32_t *out_bitmap) {
+  return (mode > 1 || (n && (!recs || !out_bitmap))) ? "bad argument" : nullptr;
+}
+const char *hs_args::msgs(const uint8_t *sig, const uint8_t *pk, const uint32_t *vidx, const uint8_t *msgs, size_t msg_len, size_t n, uint32_t mode,
+                          const uint32_t *out_bitmap) {
+  return (mode > 1 || (n && (!sig || (!pk && !vidx) || !msgs || !out_bitmap || msg_len == 0))) ? "bad argument" : nullptr;
+}
+const char *hs_args::groups(const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                            const uint32_t *vidx, const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *mode, size_t n_items,
+                            size_t n_groups, const uint32_t *out_group_bitmap) {
+  if (!out_group_bitmap || (n_msgs && !pre_off) || (n_items && (!sig || !msg_idx || !group_idx || (!pk && !vidx) || n_msgs == 0 || n_groups == 0)))
+    return "bad argument";
+  if (n_items && (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages))) return "bad preimage offsets";
+  for (size_t i = 0; i < n_items; i++)
+    if (msg_idx[i] >= n_msgs || group_idx[i] >= n_groups || (mode && mode[i] > 1)) return "index out of range";
+  return nullptr;
+}
+// HS_ERR_ARG with "<entry point>: <reason>" when a shared check above refuses the call
+static int fail_args(hs_ctx *c, const char *entry, const char *why) { return fail(c, HS_ERR_ARG, (std::string(entry) + ": " + why).c_str()); }
+
 extern "C" {
 
 int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
@@ -3198,11 +3220,9 @@ int hs_verify_tcs(hs_ctx *c, const uint64_t *tc_rounds, size_t n_tc, const uint8
 int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
                      const uint32_t *vidx, const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *mode, size_t n_items, size_t n_groups,
                      uint32_t *out_item_bitmap, uint32_t *out_group_bitmap) {
-  if (!c || !out_group_bitmap || (n_msgs && !pre_off) || (n_items && (!sig || !msg_idx || !group_idx || (!pk && !vidx) || n_msgs == 0 || n_groups == 0)))
-    return fail(c, HS_ERR_ARG, "hs_verify_groups: bad argument");
-  if (n_items && (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages))) return fail(c, HS_ERR_ARG, "hs_verify_groups: bad preimage offsets");
-  for (size_t i = 0; i < n_items; i++)
-    if (msg_idx[i] >= n_msgs || group_idx[i] >= n_groups || (mode && mode[i] > 1)) return fail(c, HS_ERR_ARG, "hs_verify_groups: index out of range");
+  if (!c) return HS_ERR_ARG;
+  if (const char *why = hs_args::groups(preimages, pre_off, n_msgs, sig, pk, vidx, msg_idx, group_idx, mode, n_items, n_groups, out_group_bitmap))
+    return fail_args(c, "hs_verify_groups", why);
   const size_t g_words = (n_groups + 31) / 32, i_words = (n_items + 31) / 32;
   const std::vector<uint32_t> ones = bitmap_ones(n_groups);
   if (n_items == 0) {
@@ -3346,7 +3366,8 @@ int hs_peer_timed_out(hs_ctx *c) {
 
 // ---- host-pointer entry points
 int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, uint32_t *out_bitmap) {
-  if (!c || mode > 1 || (n && (!recs || !out_bitmap))) return fail(c, HS_ERR_ARG, "hs_verify_rec128: bad argument");
+  if (!c) return HS_ERR_ARG;
+  if (const char *why = hs_args::rec128(recs, n, mode, out_bitmap)) return fail_args(c, "hs_verify_rec128", why);
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
@@ -3464,8 +3485,8 @@ int hs_digest32_batch(hs_ctx *c, const uint8_t *data, const uint64_t *off, size_
 // H2D copy of chunk j+1 overlapped with the kernels of chunk j (two streams, two staging buffers).
 int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint32_t *vidx, const uint8_t *msgs, size_t msg_len, size_t n,
                    uint32_t mode, uint32_t *out_bitmap) {
-  if (!c || mode > 1 || (n && (!sig || (!pk && !vidx) || !msgs || !out_bitmap || msg_len == 0)))
-    return fail(c, HS_ERR_ARG, "hs_verify_msgs: bad argument");
+  if (!c) return HS_ERR_ARG;
+  if (const char *why = hs_args::msgs(sig, pk, vidx, msgs, msg_len, n, mode, out_bitmap)) return fail_args(c, "hs_verify_msgs", why);
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));

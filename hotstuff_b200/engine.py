@@ -49,12 +49,21 @@ class Engine:
         self.device = int(device)
         self.n_keys = 0
         self._queues = []
+        self._owned = True
+
+    @classmethod
+    def _view(cls, lib, h, device):
+        """A non-owning Engine on a context another object owns (MultiEngine.member): close() leaves the context alone."""
+        e = cls.__new__(cls)
+        e.lib, e.h, e.device, e.n_keys, e._queues, e._owned = lib, h, int(device), 0, [], False
+        return e
 
     def close(self):
         for q in list(getattr(self, "_queues", [])):
             q.close()
         if getattr(self, "h", None):
-            self.lib.hs_ctx_destroy(self.h)
+            if getattr(self, "_owned", True):
+                self.lib.hs_ctx_destroy(self.h)
             self.h = None
 
     def queue(self, ring_records=0):
@@ -110,11 +119,7 @@ class Engine:
     # ---- host-buffer API -------------------------------------------------------------------------------------
     def verify_rec128(self, recs, mode=MODE_STRICT):
         """recs: (n,128) uint8 [sig64|pk32|msg32] -> bool[n]"""
-        recs = _u8(recs, 128).reshape(-1, 128)
-        n = recs.shape[0]
-        bm = np.zeros((n + 31) // 32, dtype=np.uint32)
-        self._check(self.lib.hs_verify_rec128(self.h, _ptr(recs), n, mode, _ptr(bm)), "hs_verify_rec128")
-        return bitmap_to_bools(bm, n)
+        return _verify_rec128(self, self.lib.hs_verify_rec128, "hs_verify_rec128", recs, mode)
 
     def verify_strict_batch(self, recs):
         recs = _u8(recs, 128).reshape(-1, 128)
@@ -184,22 +189,8 @@ class Engine:
 
     def verify_groups(self, preimages, pre_off, sig, msg_idx, group_idx, n_groups, mode=None, pk=None, validator_idx=None, want_items=False):
         """hs_verify_groups: items over GPU-hashed variable-length preimages, per-item verdict mode, per-group AND."""
-        pre = _u8(preimages)
-        off = np.ascontiguousarray(pre_off, dtype=np.uint64)
-        sig = _u8(sig, 64).reshape(-1, 64)
-        n = sig.shape[0]
-        mi = np.ascontiguousarray(msg_idx, dtype=np.uint32)
-        gi = np.ascontiguousarray(group_idx, dtype=np.uint32)
-        mo = None if mode is None else np.ascontiguousarray(mode, dtype=np.uint8)
-        assert (pk is None) != (validator_idx is None) and mi.shape[0] == n == gi.shape[0]
-        pk = None if pk is None else _u8(pk, 32).reshape(-1, 32)
-        vidx = None if validator_idx is None else np.ascontiguousarray(validator_idx, dtype=np.uint32)
-        gbm = np.zeros(max(1, (n_groups + 31) // 32), dtype=np.uint32)
-        ibm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32) if want_items else None
-        self._check(self.lib.hs_verify_groups(self.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk), _ptr(vidx),
-                                              _ptr(mi) if n else None, _ptr(gi) if n else None, _ptr(mo), n, n_groups, _ptr(ibm), _ptr(gbm)), "hs_verify_groups")
-        out = bitmap_to_bools(gbm, n_groups)
-        return (out, bitmap_to_bools(ibm, n)) if want_items else out
+        return _verify_groups(self, self.lib.hs_verify_groups, "hs_verify_groups", preimages, pre_off, sig, msg_idx, group_idx, n_groups, mode, pk,
+                              validator_idx, want_items)
 
     def keygen_batch(self, seeds):
         """RFC 8032 public keys of n 32-byte seeds, computed on the GPU (load generation; hs_keygen_batch)."""
@@ -220,21 +211,11 @@ class Engine:
         return out
 
     def committee_register(self, pks):
-        pks = _u8(pks, 32).reshape(-1, 32)
-        n = pks.shape[0]
-        bm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
-        self._check(self.lib.hs_committee_register(self.h, _ptr(pks) if n else None, n, _ptr(bm)), "hs_committee_register")
-        self.n_keys = n
-        return bitmap_to_bools(bm, n)
+        return _committee_register(self, self.lib.hs_committee_register, "hs_committee_register", pks)
 
     def committee_update(self, add=None, remove=None):
         """Incremental epoch change (hs_committee_update): returns the indices assigned to the added keys."""
-        add = np.zeros((0, 32), np.uint8) if add is None else _u8(add, 32).reshape(-1, 32)
-        rem = np.zeros(0, np.uint32) if remove is None else np.ascontiguousarray(remove, dtype=np.uint32)
-        out = np.zeros(max(1, add.shape[0]), dtype=np.uint32)
-        self._check(self.lib.hs_committee_update(self.h, _ptr(add) if add.shape[0] else None, add.shape[0], _ptr(rem) if rem.shape[0] else None,
-                                                 rem.shape[0], _ptr(out)), "hs_committee_update")
-        return out[: add.shape[0]]
+        return _committee_update(self, self.lib.hs_committee_update, "hs_committee_update", add, remove)
 
     def set_table_budget(self, nbytes):
         self._check(self.lib.hs_set_table_budget(self.h, int(nbytes)), "hs_set_table_budget")
@@ -261,15 +242,7 @@ class Engine:
 
     def verify_msgs(self, sig, msgs, msg_len, pk=None, validator_idx=None, mode=MODE_STRICT):
         """Reference-shaped call: verdict_i = Signature::verify(Digest(msg_i), key_i); msgs = n fixed-size messages."""
-        sig = _u8(sig, 64).reshape(-1, 64)
-        n = sig.shape[0]
-        msgs = _u8(msgs)
-        assert msgs.size == n * msg_len and (pk is None) != (validator_idx is None)
-        pk = None if pk is None else _u8(pk, 32).reshape(-1, 32)
-        vidx = None if validator_idx is None else np.ascontiguousarray(validator_idx, dtype=np.uint32)
-        bm = np.zeros((n + 31) // 32, dtype=np.uint32)
-        self._check(self.lib.hs_verify_msgs(self.h, _ptr(sig), _ptr(pk), _ptr(vidx), _ptr(msgs), msg_len, n, mode, _ptr(bm)), "hs_verify_msgs")
-        return bitmap_to_bools(bm, n)
+        return _verify_msgs(self, self.lib.hs_verify_msgs, "hs_verify_msgs", sig, msgs, msg_len, pk, validator_idx, mode)
 
     # ---- device-resident API (torch tensors on this engine's device; enqueued on torch's current stream) -------
     @staticmethod
@@ -329,6 +302,133 @@ class Engine:
 
     def digest32_dev(self, d_data, d_off, d_out, n):
         self._check(self.lib.hs_digest32_dev(self.h, d_data.data_ptr(), d_off.data_ptr(), n, d_out.data_ptr(), self._stream()), "hs_digest32_dev")
+
+
+# Marshalling of the host-pointer calls that Engine and MultiEngine both make: fn is the C entry point, owner.h its handle and
+# owner._check its error check.
+def _verify_rec128(owner, fn, name, recs, mode):
+    recs = _u8(recs, 128).reshape(-1, 128)
+    n = recs.shape[0]
+    bm = np.zeros((n + 31) // 32, dtype=np.uint32)
+    owner._check(fn(owner.h, _ptr(recs), n, mode, _ptr(bm)), name)
+    return bitmap_to_bools(bm, n)
+
+
+def _verify_msgs(owner, fn, name, sig, msgs, msg_len, pk, validator_idx, mode):
+    sig = _u8(sig, 64).reshape(-1, 64)
+    n = sig.shape[0]
+    msgs = _u8(msgs)
+    assert msgs.size == n * msg_len and (pk is None) != (validator_idx is None)
+    pk = None if pk is None else _u8(pk, 32).reshape(-1, 32)
+    vidx = None if validator_idx is None else np.ascontiguousarray(validator_idx, dtype=np.uint32)
+    bm = np.zeros((n + 31) // 32, dtype=np.uint32)
+    owner._check(fn(owner.h, _ptr(sig), _ptr(pk), _ptr(vidx), _ptr(msgs), msg_len, n, mode, _ptr(bm)), name)
+    return bitmap_to_bools(bm, n)
+
+
+def _verify_groups(owner, fn, name, preimages, pre_off, sig, msg_idx, group_idx, n_groups, mode, pk, validator_idx, want_items):
+    pre = _u8(preimages)
+    off = np.ascontiguousarray(pre_off, dtype=np.uint64)
+    sig = _u8(sig, 64).reshape(-1, 64)
+    n = sig.shape[0]
+    mi = np.ascontiguousarray(msg_idx, dtype=np.uint32)
+    gi = np.ascontiguousarray(group_idx, dtype=np.uint32)
+    mo = None if mode is None else np.ascontiguousarray(mode, dtype=np.uint8)
+    assert (pk is None) != (validator_idx is None) and mi.shape[0] == n == gi.shape[0]
+    pk = None if pk is None else _u8(pk, 32).reshape(-1, 32)
+    vidx = None if validator_idx is None else np.ascontiguousarray(validator_idx, dtype=np.uint32)
+    gbm = np.zeros(max(1, (n_groups + 31) // 32), dtype=np.uint32)
+    ibm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32) if want_items else None
+    owner._check(fn(owner.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk), _ptr(vidx),
+                    _ptr(mi) if n else None, _ptr(gi) if n else None, _ptr(mo), n, n_groups, _ptr(ibm), _ptr(gbm)), name)
+    out = bitmap_to_bools(gbm, n_groups)
+    return (out, bitmap_to_bools(ibm, n)) if want_items else out
+
+
+def _committee_register(owner, fn, name, pks):
+    pks = _u8(pks, 32).reshape(-1, 32)
+    n = pks.shape[0]
+    bm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
+    owner._check(fn(owner.h, _ptr(pks) if n else None, n, _ptr(bm)), name)
+    owner.n_keys = n
+    return bitmap_to_bools(bm, n)
+
+
+def _committee_update(owner, fn, name, add, remove):
+    add = np.zeros((0, 32), np.uint8) if add is None else _u8(add, 32).reshape(-1, 32)
+    rem = np.zeros(0, np.uint32) if remove is None else np.ascontiguousarray(remove, dtype=np.uint32)
+    out = np.zeros(max(1, add.shape[0]), dtype=np.uint32)
+    owner._check(fn(owner.h, _ptr(add) if add.shape[0] else None, add.shape[0], _ptr(rem) if rem.shape[0] else None, rem.shape[0], _ptr(out)), name)
+    return out[: add.shape[0]]
+
+
+class MultiEngine:
+    """Python handle on one hs_multi: several member contexts in this process (include/hs_crypto.h, hs_multi_*).  A host-pointer verify
+    call of at least HS_MULTI_MIN_SHARD records per member is sharded across the members; a smaller one runs whole on one member, chosen
+    round-robin.  Verdicts equal the same Engine call bit for bit.  devices may list a device more than once."""
+
+    MIN_SHARD = 4096  # HS_MULTI_MIN_SHARD
+
+    def __init__(self, devices, base_window=0, key_window=0, key_cache=True):
+        self.lib = _lib.load()
+        devs = np.ascontiguousarray([int(d) for d in devices], dtype=np.int32)
+        h = ctypes.c_void_p()
+        flags = (int(base_window) & 0xff) | ((int(key_window) & 0xff) << 8) | (0 if key_cache else 0x10000)
+        rc = self.lib.hs_multi_create(ctypes.byref(h), _ptr(devs) if devs.size else None, devs.size, flags)
+        if rc != 0 or not h:
+            raise EngineError("hs_multi_create(devices=%s) failed with status %d (no GPU / bad ordinal / CUDA error); there is no CPU fallback"
+                              % (list(devs), rc))
+        self.h = h
+        self.devices = [int(d) for d in devs]
+        self.n_keys = 0
+        self._members = [Engine._view(self.lib, self.lib.hs_multi_member(h, i), d) for i, d in enumerate(self.devices)]
+
+    def member(self, i):
+        """Member i as a non-owning Engine: every single-device call works on it.  Do not change its committee directly."""
+        return self._members[i]
+
+    def __len__(self):
+        return len(self._members)
+
+    def close(self):
+        """Closes the queues created on the members, then destroys the members and joins the worker threads."""
+        for e in getattr(self, "_members", []):
+            e.close()
+        if getattr(self, "h", None):
+            self.lib.hs_multi_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, rc, what):
+        if rc != 0:
+            raise EngineError("%s failed: status %d: %s" % (what, rc, self.lib.hs_multi_last_error(self.h).decode()))
+
+    @property
+    def last_error(self):
+        return self.lib.hs_multi_last_error(self.h).decode()
+
+    def register_committee(self, pks):
+        """hs_multi_committee_register: the same committee on every member; returns the keys' validity (bool[N])."""
+        return _committee_register(self, self.lib.hs_multi_committee_register, "hs_multi_committee_register", pks)
+
+    def update_committee(self, add=None, remove=None):
+        """hs_multi_committee_update: returns the indices assigned to the added keys (the same on every member)."""
+        return _committee_update(self, self.lib.hs_multi_committee_update, "hs_multi_committee_update", add, remove)
+
+    def verify_rec128(self, recs, mode=MODE_STRICT):
+        return _verify_rec128(self, self.lib.hs_multi_verify_rec128, "hs_multi_verify_rec128", recs, mode)
+
+    def verify_msgs(self, sig, msgs, msg_len, pk=None, validator_idx=None, mode=MODE_STRICT):
+        return _verify_msgs(self, self.lib.hs_multi_verify_msgs, "hs_multi_verify_msgs", sig, msgs, msg_len, pk, validator_idx, mode)
+
+    def verify_groups(self, preimages, pre_off, sig, msg_idx, group_idx, n_groups, mode=None, pk=None, validator_idx=None, want_items=False):
+        return _verify_groups(self, self.lib.hs_multi_verify_groups, "hs_multi_verify_groups", preimages, pre_off, sig, msg_idx, group_idx, n_groups,
+                              mode, pk, validator_idx, want_items)
 
 
 class VerifyQueue:

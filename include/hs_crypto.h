@@ -457,6 +457,54 @@ int hs_peer_next(hs_ctx *ctx, size_t word_offset, uint32_t epoch);
 void *hs_peer_bitmap(hs_ctx *ctx);
 int hs_peer_timed_out(hs_ctx *ctx);
 
+/* ---- several GPUs in one process: a multi-device context that shards the host-pointer verify calls ------------------------------
+ * A node is one process (its Core task and its mempool Processors call `crypto` from it), so it cannot reach a second GPU through the
+ * one-process-per-GPU route above.  A multi-device context is n_devices ordinary contexts, its MEMBERS, plus host code that splits a call
+ * across them.
+ *   - Verdicts: every output is bit for bit what the same single-context call returns, with or without a registered committee, in both
+ *     modes and with mixed mode bytes.  Members may run different table geometries (each picks its per-key window from its own free memory
+ *     and budget); verdicts do not depend on geometry.
+ *   - Sharding: a call is sharded only when every member gets at least HS_MULTI_MIN_SHARD records.  Member i then verifies a contiguous
+ *     record range; every range but the last starts at a multiple of 32 records, so each member writes whole words of the caller's bitmap.
+ *     hs_multi_verify_groups gives each member its item range with the whole preimage arrays and n_groups; each member ANDs its items into
+ *     group words of its own (a group with no item in its range stays 1) and the caller's group words are the AND of the members' words.
+ *   - A smaller call runs whole on one member, chosen round-robin, without the multi-context's lock: small calls from several threads run
+ *     on different GPUs at once, and calls of up to 64 records keep the one-launch latency path.
+ *   - Threads and locks: hs_multi_create starts one worker thread per member after the first; the calling thread runs member 0's range.
+ *     Sharded calls and committee changes are serialised on the multi-context's mutex, and each member still serialises on its own, so a
+ *     verify queue created on a member (hs_multi_member) keeps working beside them.  A device may be listed more than once.
+ *   - Errors: the argument checks of hs_verify_rec128 / hs_verify_msgs / hs_verify_groups cover the whole call before any member runs, so
+ *     HS_ERR_ARG writes nothing.  A member's failure returns that member's status and hs_multi_last_error names the member (index, device)
+ *     with its hs_last_error; the outputs are then undefined and the caller rejects every signature of the call.
+ *   - Committee: hs_multi_committee_register registers on every member at once.  If any member fails, or the members' out_valid_bitmap
+ *     differ (HS_ERR_CUDA), every member ends with NO committee.  hs_multi_committee_update must give every member the same out_add_idx;
+ *     a mismatch is HS_ERR_CUDA, and after any failure of it the members may differ: re-register.  The committee-indexed forms need every
+ *     member registered through these two calls: never change a member's committee directly.
+ *   - Pinned memory from hs_host_alloc (cudaMallocHost) is portable under UVA: every member DMAs from the caller's pinned buffers directly.
+ *   - hs_multi_destroy joins the workers and destroys the members (and the verify queues created on them); it must not race with calls.
+ *     A failed hs_multi_create (n_devices == 0, a bad ordinal, no memory) leaves no thread and no member behind. */
+#define HS_MULTI_MIN_SHARD 4096 /* records per member below which a call runs whole on one member */
+typedef struct hs_multi hs_multi;
+/* flags as hs_ctx_create, applied to every member. */
+int hs_multi_create(hs_multi **out, const int *devices, size_t n_devices, uint32_t flags);
+void hs_multi_destroy(hs_multi *m);
+/* The last failure on this multi-context (never NULL): a member's failure names the member (index, device) and its hs_last_error. */
+const char *hs_multi_last_error(const hs_multi *m);
+size_t hs_multi_members(const hs_multi *m);
+/* Member i (borrowed; NULL when out of range): every single-device entry point works on it. */
+hs_ctx *hs_multi_member(hs_multi *m, size_t i);
+int hs_multi_committee_register(hs_multi *m, const uint8_t *pks /* N x 32 */, size_t N, uint32_t *out_valid_bitmap);
+int hs_multi_committee_update(hs_multi *m, const uint8_t *add_pks /* n_add x 32 */, size_t n_add, const uint32_t *remove_idx, size_t n_remove,
+                              uint32_t *out_add_idx);
+/* The arguments and outputs of hs_verify_rec128, hs_verify_msgs and hs_verify_groups. */
+int hs_multi_verify_rec128(hs_multi *m, const hs_rec128 *recs, size_t n, uint32_t mode, uint32_t *out_bitmap);
+int hs_multi_verify_msgs(hs_multi *m, const uint8_t *sig /* n x 64 */, const uint8_t *pk_or_null /* n x 32 */, const uint32_t *validator_idx_or_null,
+                         const uint8_t *msgs, size_t msg_len, size_t n, uint32_t mode, uint32_t *out_bitmap);
+int hs_multi_verify_groups(hs_multi *m, const uint8_t *preimages, const uint64_t *pre_off /* n_msgs + 1 */, size_t n_msgs,
+                           const uint8_t *sig /* n_items x 64 */, const uint8_t *pk_or_null, const uint32_t *validator_idx_or_null,
+                           const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *mode_or_null, size_t n_items, size_t n_groups,
+                           uint32_t *out_item_bitmap_or_null, uint32_t *out_group_bitmap);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,6 +9,7 @@
 #include <cstdint>
 #include <cstring>
 #include <future>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -32,7 +33,12 @@ class Engine {
   explicit Engine(int device = 0, uint32_t flags = 0) {
     if (hs_ctx_create(&ctx_, device, flags) != HS_OK) throw EngineError("hs_ctx_create failed (no GPU?) — there is no CPU fallback");
   }
-  ~Engine() { hs_ctx_destroy(ctx_); }
+  // A non-owning Engine on a context another object owns (MultiEngine::member): the destructor leaves the context alone.
+  struct Borrowed {};
+  Engine(hs_ctx *ctx, Borrowed) : ctx_(ctx), owned_(false) {}
+  ~Engine() {
+    if (owned_) hs_ctx_destroy(ctx_);
+  }
   Engine(const Engine &) = delete;
   Engine &operator=(const Engine &) = delete;
   hs_ctx *raw() const { return ctx_; }
@@ -52,6 +58,71 @@ class Engine {
 
  private:
   hs_ctx *ctx_ = nullptr;
+  bool owned_ = true;
+};
+
+// RAII handle on hs_multi_* (hs_crypto.h): several member contexts in this process.  A verify call of at least HS_MULTI_MIN_SHARD records
+// per member is sharded across the members, a smaller one runs whole on one member (round-robin); verdicts equal the same Engine call
+// bit for bit.  Outputs are bitmaps as in the C ABI: bit (i & 31) of word (i >> 5).  Destroy every VerifyQueue made on a member first.
+class MultiEngine {
+ public:
+  explicit MultiEngine(const std::vector<int> &devices, uint32_t flags = 0) {
+    if (hs_multi_create(&m_, devices.data(), devices.size(), flags) != HS_OK)
+      throw EngineError("hs_multi_create failed (no GPU, bad ordinal?) — there is no CPU fallback");
+    for (size_t i = 0; i < devices.size(); i++) members_.emplace_back(new Engine(hs_multi_member(m_, i), Engine::Borrowed{}));
+  }
+  ~MultiEngine() {
+    members_.clear();
+    hs_multi_destroy(m_);
+  }
+  MultiEngine(const MultiEngine &) = delete;
+  MultiEngine &operator=(const MultiEngine &) = delete;
+  hs_multi *raw() const { return m_; }
+  size_t size() const { return members_.size(); }
+  // Member i: every single-device call works on it (a VerifyQueue, say).  Do not change its committee directly.
+  const Engine &member(size_t i) const { return *members_.at(i); }
+  void check(int rc, const char *what) const {
+    if (rc != HS_OK) throw EngineError(std::string(what) + ": " + hs_multi_last_error(m_));
+  }
+  std::string error() const { return hs_multi_last_error(m_); }
+  // The same committee on every member; returns ceil(N / 32) words of key validity.
+  std::vector<uint32_t> register_committee(const uint8_t *pks, size_t N) {
+    std::vector<uint32_t> valid((N + 31) / 32);
+    check(hs_multi_committee_register(m_, pks, N, valid.data()), "hs_multi_committee_register");
+    return valid;
+  }
+  // Returns the indices of the added keys, the same on every member.
+  std::vector<uint32_t> update_committee(const uint8_t *add_pks, size_t n_add, const uint32_t *remove_idx, size_t n_remove) {
+    std::vector<uint32_t> idx(n_add);
+    check(hs_multi_committee_update(m_, add_pks, n_add, remove_idx, n_remove, idx.data()), "hs_multi_committee_update");
+    return idx;
+  }
+  std::vector<uint32_t> verify_rec128(const hs_rec128 *recs, size_t n, uint32_t mode = HS_MODE_STRICT) {
+    std::vector<uint32_t> bm((n + 31) / 32);
+    check(hs_multi_verify_rec128(m_, recs, n, mode, bm.data()), "hs_multi_verify_rec128");
+    return bm;
+  }
+  // key_i = pk[i] (pk != nullptr) or committee key validator_idx[i].
+  std::vector<uint32_t> verify_msgs(const uint8_t *sig, const uint8_t *pk, const uint32_t *validator_idx, const uint8_t *msgs, size_t msg_len, size_t n,
+                                    uint32_t mode = HS_MODE_STRICT) {
+    std::vector<uint32_t> bm((n + 31) / 32);
+    check(hs_multi_verify_msgs(m_, sig, pk, validator_idx, msgs, msg_len, n, mode, bm.data()), "hs_multi_verify_msgs");
+    return bm;
+  }
+  // Group words; item words go to out_item_bitmap when it is not null.
+  std::vector<uint32_t> verify_groups(const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                                      const uint32_t *validator_idx, const uint32_t *msg_idx, const uint32_t *group_idx, const uint8_t *modes,
+                                      size_t n_items, size_t n_groups, uint32_t *out_item_bitmap = nullptr) {
+    std::vector<uint32_t> groups((n_groups + 31) / 32);
+    check(hs_multi_verify_groups(m_, preimages, pre_off, n_msgs, sig, pk, validator_idx, msg_idx, group_idx, modes, n_items, n_groups, out_item_bitmap,
+                                 groups.data()),
+          "hs_multi_verify_groups");
+    return groups;
+  }
+
+ private:
+  hs_multi *m_ = nullptr;
+  std::vector<std::unique_ptr<Engine>> members_;
 };
 
 // The verify queue's ring has no room for the request right now (HS_ERR_NOMEM): back-pressure, retry once requests complete.

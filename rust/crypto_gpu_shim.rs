@@ -46,6 +46,10 @@ pub mod batch_queue;
 /// the caller's stream (`groups_dev::verify_groups_dev`).
 #[path = "crypto_gpu_groups_dev.rs"]
 pub mod groups_dev;
+/// Several GPUs from this one process (hs_multi_*): large verifies sharded across them, small ones spread round-robin
+/// (`multi::Multi`).
+#[path = "crypto_gpu_multi.rs"]
+pub mod multi;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

@@ -140,27 +140,36 @@ __host__ __device__ inline uint32_t key_hash(const uint32_t *w) {
   }
   return h;
 }
+// The key index the table maps key bytes k to (HS_NO_KEY: none) and, when found, the hash slot holding it.  BOUNDED (hs_table_audit,
+// which must not trust the table it checks): an index at or past T.n_keys is a non-match instead of an address.
+template <bool BOUNDED>
+__device__ __forceinline__ uint32_t key_probe(const key_table &T, const uint32_t (&k)[8], uint32_t &pos) {
+  uint32_t h = key_hash(k) & T.mask;
+  for (uint32_t probe = 0; probe <= T.mask; probe++) {
+    uint32_t idx = __ldg(T.slots + h);
+    if (idx == HS_NO_KEY) break;
+    if (!BOUNDED || idx < T.n_keys) {
+      const uint32_t *cand = reinterpret_cast<const uint32_t *>(T.pks + (size_t)idx * 32);
+      uint32_t diff = 0;
+#pragma unroll
+      for (int j = 0; j < 8; j++) diff |= __ldg(cand + j) ^ k[j];
+      if (diff == 0) {
+        pos = h;
+        return idx;
+      }
+    }
+    h = (h + 1) & T.mask;
+  }
+  return HS_NO_KEY;
+}
 __global__ void __launch_bounds__(256) k_key_lookup(in_layout L, size_t n, key_table T, uint32_t *__restrict__ out_vidx,
                                                     uint32_t *__restrict__ miss_list, uint32_t *__restrict__ miss_count) {
   const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
   if (i >= n) return;
   uint32_t k[8];
   load32(k, L.pk + i * L.pk_stride);
-  uint32_t found = HS_NO_KEY;
-  uint32_t h = key_hash(k) & T.mask;
-  for (uint32_t probe = 0; probe <= T.mask; probe++) {
-    uint32_t idx = __ldg(T.slots + h);
-    if (idx == HS_NO_KEY) break;
-    const uint32_t *cand = reinterpret_cast<const uint32_t *>(T.pks + (size_t)idx * 32);
-    uint32_t diff = 0;
-#pragma unroll
-    for (int j = 0; j < 8; j++) diff |= __ldg(cand + j) ^ k[j];
-    if (diff == 0) {
-      found = idx;
-      break;
-    }
-    h = (h + 1) & T.mask;
-  }
+  uint32_t pos;
+  const uint32_t found = key_probe<false>(T, k, pos);
   out_vidx[i] = found;
   if (found == HS_NO_KEY) miss_list[atomicAdd(miss_count, 1u)] = (uint32_t)i;  // compacted list for the generic pass
 }
@@ -1039,6 +1048,106 @@ __global__ void __launch_bounds__(HS_THREADS) k_build_comb(const uint8_t *__rest
   comb_build_block(tables + p * ((size_t)n_windows * comb_window_stride(W)), P, W, w, b * HS_BUILD_BLOCK, HS_BUILD_BLOCK, prod);
 }
 
+// ------------------------------------------------------------------------------------------------ table audit (hs_table_audit)
+// Findings: HS_AUDIT_* bits OR-ed into bits[0] (the base table), bits[1] (hash entries naming no slot in use) and bits[2 + s] (slot s),
+// and the first finding's audit_key() kept by an atomic minimum, so the message does not depend on scheduling.
+struct audit_out {
+  unsigned long long *first;
+  uint32_t *bits;
+};
+__device__ __forceinline__ void audit_report(const audit_out &O, size_t bits_idx, uint32_t cls, uint64_t key) {
+  atomicOr(O.bits + bits_idx, cls);
+  atomicMin(O.first, (unsigned long long)key);
+}
+// KEY / FLAG / LOOKUP: thread i < n_slots checks slot i, thread n_slots + j checks hash entry j.  live: the engine's liveness mirror
+// (1 byte per slot); expect_pks / expect_live: the caller's map (nullable).  Writes auditable[s] = live and the key decompresses: the
+// slots whose comb table k_table_audit then checks.
+__global__ void __launch_bounds__(256) k_slot_audit(key_table T, const uint8_t *__restrict__ key_flags, const uint8_t *__restrict__ live,
+                                                    const uint8_t *__restrict__ expect_pks, const uint32_t *__restrict__ expect_live, int expect,
+                                                    uint8_t *__restrict__ auditable, audit_out O) {
+  const size_t n_slots = T.n_keys;
+  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+  if (i < n_slots) {
+    const uint32_t is_live = live[i] ? 1u : 0u;
+    uint32_t k[8];
+    load32(k, T.pks + i * 32);
+    uint32_t cls = 0;
+    if (expect) {
+      const uint32_t want_live = expect_live ? (expect_live[i >> 5] >> (i & 31)) & 1u : 1u;
+      if (want_live != is_live) cls |= HS_AUDIT_KEY;
+      if (expect_pks && is_live && want_live) {
+        uint32_t e[8], d = 0;
+        load32(e, expect_pks + i * 32);
+#pragma unroll
+        for (int j = 0; j < 8; j++) d |= e[j] ^ k[j];
+        if (d) cls |= HS_AUDIT_KEY;
+      }
+    }
+    ge_ext P;
+    const uint32_t ok = ge_decompress(P, k);
+    const uint32_t want_flag = is_live ? (ok | (ge_enc_is_small_order(k) << 1)) : 0u;
+    if (key_flags[i] != want_flag) cls |= HS_AUDIT_FLAG;
+    if (is_live) {
+      uint32_t pos;
+      const uint32_t idx = key_probe<true>(T, k, pos);
+      if (idx == HS_NO_KEY || !live[idx]) cls |= HS_AUDIT_LOOKUP;
+    }
+    auditable[i] = (uint8_t)(is_live & ok);
+    if (cls) audit_report(O, 2 + i, cls, audit_key(i + 1, 0, 0));
+  } else if (i - n_slots <= T.mask) {
+    const uint32_t j = (uint32_t)(i - n_slots), idx = T.slots[j];
+    if (idx == HS_NO_KEY) return;
+    if (idx >= n_slots) {
+      audit_report(O, 1, HS_AUDIT_LOOKUP, audit_key(n_slots + 1, 0, 0));
+      return;
+    }
+    uint32_t k[8], pos = HS_NO_KEY;
+    load32(k, T.pks + (size_t)idx * 32);
+    if (!live[idx] || key_probe<true>(T, k, pos) != idx || pos != j) audit_report(O, 2 + idx, HS_AUDIT_LOOKUP, audit_key(idx + 1, 0, 0));
+  }
+}
+// TABLE / BASE: a warp per run of 32 consecutive entries of one window of one table, lane l entry first + l (coalesced 96-byte loads);
+// entry m - 1 comes from lane l - 1 by shuffles, and entry 1 of the window is one broadcast load.  The lane of entry 1 also checks the
+// window link, or for window 0 the anchor.  pks == nullptr: one table, the base-point table (anchor B); otherwise table s is slot s's,
+// anchored on -A of its stored bytes, and only the slots k_slot_audit marked auditable are read.  Short blocks: the lowest-priority
+// stream's blocks give way to verify launches at every block boundary.
+#define HS_AUDIT_WARPS 4
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, size_t n_tables, size_t table_entries,
+                                                                       int W, int n_windows, const uint8_t *__restrict__ pks,
+                                                                       const uint8_t *__restrict__ auditable, audit_out O) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t H = (uint64_t)1 << (W - 1), runs = (H + 1 + 31) / 32;
+  const uint64_t g = (uint64_t)blockIdx.x * HS_AUDIT_WARPS + (threadIdx.x >> 5);
+  const uint64_t t = g / (runs * n_windows);
+  if (t >= n_tables || (pks && !auditable[t])) return;  // whole warps leave together
+  const uint32_t win = (uint32_t)((g / runs) % n_windows);
+  const uint32_t m = (uint32_t)((g % runs) * 32 + lane);
+  const ge_niels *wt = tables + t * table_entries + (size_t)win * comb_window_stride(W);
+  const bool in = m <= H;
+  ge_niels e, prev, one;
+  niels_load_stream(e, wt + (in ? m : H));
+  niels_load(one, wt + 1);
+  {
+    uint32_t *pe = reinterpret_cast<uint32_t *>(&e), *pp = reinterpret_cast<uint32_t *>(&prev);
+#pragma unroll
+    for (int j = 0; j < 24; j++) pp[j] = __shfl_up_sync(0xffffffffu, pe[j], 1);
+  }
+  if (lane == 0 && m > 0) niels_load(prev, wt + m - 1);
+  uint32_t ok = in ? audit_entry_local(e, prev, one, m) : 1u;
+  if (m == 1) {
+    if (win == 0) {
+      ge_ext P;
+      audit_anchor_point(P, pks ? reinterpret_cast<const uint32_t *>(pks + t * 32) : nullptr);
+      ok &= audit_anchor(e, P);
+    } else {
+      ge_niels last;
+      niels_load(last, wt - comb_window_stride(W) + H);
+      ok &= audit_link(e, last);
+    }
+  }
+  if (!ok) audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
+}
+
 // ------------------------------------------------------------------------------------------------ Digest kernels
 __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restrict__ data, const uint64_t *__restrict__ off, uint64_t fixed_len,
                                                           size_t n, uint32_t *__restrict__ out) {
@@ -1355,6 +1464,12 @@ struct learn_bufs {
   event_h ev;
   event_h ev_tables;  // recorded after the latest table build of the key cache; every pass waits for it (any stream)
 };
+// hs_table_audit: its private lowest-priority stream, the event recorded after its kernels, and its scratch.  Created on first use.
+struct audit_state {
+  stream_h stream;
+  event_h done;
+  dev_buf scratch;
+};
 // Latency path: mapped pinned staging (inputs, verdict flags, completion word) and the device block counter.
 struct small_staging {
   mapped<small_rec> in;
@@ -1399,6 +1514,11 @@ struct hs_ctx {
   bool cache_full = false;           // no free slot: only the miss RATE is watched (a mostly-missing full cache is reset)
   uint64_t calls_since_reset = HS_CACHE_RESET_MIN_CALLS;
   size_t learn_records = 0;          // records of the pass whose misses are parked in learn.h_*
+  // key-table generation: bumped (under mu) by every path that frees or rewrites the per-key tables, key bytes, flags or hash table, so
+  // an audit that ran across such a change reports nothing.  Those paths first wait for audit.done (or synchronise the device).
+  uint64_t key_gen = 0;
+  std::mutex audit_mu;               // one hs_table_audit at a time: it owns `audit` for the whole call, `mu` only briefly
+  audit_state audit;
   // multi-GPU peer routing
   peer_route peers{};
   int peer_rank = 0;
@@ -1539,7 +1659,14 @@ static void set_window(comb_params &cp, bool a, int w) {
 }
 
 // ---- key cache -----------------------------------------------------------------------------------------------------
-static void cache_release(hs_ctx *c) {
+// Before a key-cache path rewrites tables, key bytes or the hash table on `stream`: an audit's kernels in flight finish first.
+static int audit_fence(hs_ctx *c, cudaStream_t stream) {
+  c->key_gen++;
+  if (c->audit.done) HS_CUDA(c, cudaStreamWaitEvent(stream, c->audit.done, 0));
+  return HS_OK;
+}
+static void cache_release(hs_ctx *c) {  // callers have synchronised the device
+  c->key_gen++;
   c->keys = {};
   c->n_keys = 0;
   c->h_pks.clear();
@@ -1573,6 +1700,7 @@ static int cache_allocate(hs_ctx *c) {
   HS_CUDA(c, alloc(K.slots, (size_t)cap * 4));
   HS_CUDA(c, alloc(K.atables, c->cache_cap * sizeof(ge_niels) * c->a_table_entries));
   HS_CUDA(c, cudaMemset(K.slots, 0xff, (size_t)cap * 4));
+  c->key_gen++;  // nothing to wait for: the store had no tables, so no audit reads it
   c->keys = std::move(K);
   c->slot_mask = cap - 1;
   c->h_slots.assign(cap, HS_NO_KEY);
@@ -1592,6 +1720,7 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
     // Start over — the next passes relearn the keys that are actually in use.  (No per-key eviction; see DESIGN.md §8.)
     if (c->learn_records >= 64 && (size_t)*c->learn.h_miss_total * 2 > c->learn_records && c->calls_since_reset >= HS_CACHE_RESET_MIN_CALLS) {
       c->calls_since_reset = 0;
+      HS_TRY(audit_fence(c, stream));
       c->n_keys = 0;
       c->h_pks.clear();
       std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
@@ -1628,6 +1757,7 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
     n_new++;
   }
   if (n_new == 0) return HS_OK;
+  HS_TRY(audit_fence(c, stream));
   HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + old_n * 32, c->h_pks.data() + old_n * 32, n_new * 32, cudaMemcpyHostToDevice, stream));
   HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, stream));
   size_t threads = n_new * (size_t)c->cp.na * ((1u << (c->cp.wa - 1)) / HS_BUILD_BLOCK);
@@ -2811,6 +2941,7 @@ void hs_ctx_destroy(hs_ctx *c) {
     qs.swap(c->queues);
   }
   for (hs_queue *q : qs) queue_free(q);  // completes their requests (callbacks fire) and joins their threads
+  { std::lock_guard<std::mutex> a(c->audit_mu); }  // an audit still waiting on its kernels returns before its tables go
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   delete c;  // the owners release the rest
@@ -2979,9 +3110,10 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
   std::lock_guard<std::mutex> g(c->mu);
   if (!c->explicit_committee) return fail(c, HS_ERR_ARG, "hs_committee_update: no committee registered");
   HS_CUDA(c, cudaSetDevice(c->device));
-  HS_CUDA(c, cudaDeviceSynchronize());  // epoch boundary: nothing of the old set may be in flight (verify queue launches included)
+  HS_CUDA(c, cudaDeviceSynchronize());  // epoch boundary: nothing of the old set may be in flight (verify queue launches and audits included)
   for (size_t i = 0; i < n_remove; i++)
     if (remove_idx[i] >= c->n_keys) return fail(c, HS_ERR_ARG, "hs_committee_update: remove index out of range");
+  c->key_gen++;
   for (size_t i = 0; i < n_remove; i++) {
     c->h_key_live[remove_idx[i]] = 0;
     HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + remove_idx[i], 0, 1, c->stream));
@@ -4505,4 +4637,100 @@ extern "C" int hs_self_test(hs_ctx *c, int key_bits, const hs_rec128 *recs, cons
     if (expect[i] > 3) return fail(c, HS_ERR_ARG, "hs_self_test: an expectation byte uses bits other than 0 and 1");
   std::lock_guard<std::mutex> g(c->mu);
   return self_test_locked(c, key_bits, recs, expect, n, out_failed_paths);
+}
+
+// ---- audit of the live key tables (hs_table_audit)
+extern "C" size_t hs_key_slots(const hs_ctx *c) { return (c && c->keys.atables) ? c->n_keys : 0; }
+
+// The message for the first finding: audit_key() decoded, with the slot's classes for a finding about the slot itself.
+static std::string audit_message(uint64_t first, size_t n_slots, const uint32_t *bits) {
+  const uint64_t code = first >> 32;
+  const uint32_t wfield = (uint32_t)(first >> 26) & 63u, entry = (uint32_t)first & ((1u << 26) - 1);
+  const std::string at = wfield ? ": window " + std::to_string(wfield - 1) + ", entry " + std::to_string(entry) : std::string();
+  if (code == 0) return "hs_table_audit: base-point table" + at + " is not the multiple of B it must hold (BASE)";
+  if (code > n_slots) return "hs_table_audit: a device hash-table entry names a slot past the " + std::to_string(n_slots) + " in use (LOOKUP)";
+  const size_t s = (size_t)code - 1;
+  if (wfield) return "hs_table_audit: slot " + std::to_string(s) + ": comb table" + at + " is not the multiple of -A it must hold (TABLE)";
+  std::string m = "hs_table_audit: slot " + std::to_string(s) + ":";
+  if (bits[2 + s] & HS_AUDIT_KEY) m += " stored key bytes or liveness differ from the expectation (KEY);";
+  if (bits[2 + s] & HS_AUDIT_FLAG) m += " device flag byte disagrees with liveness and decompression (FLAG);";
+  if (bits[2 + s] & HS_AUDIT_LOOKUP) m += " device hash table does not map its key bytes to a live slot with them (LOOKUP);";
+  m.pop_back();
+  return m;
+}
+
+extern "C" int hs_table_audit(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots, uint8_t *out_slot_bits,
+                              uint32_t *out_failed) {
+  if (!c || !out_failed) return fail(c, HS_ERR_ARG, "hs_table_audit: bad argument");
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  audit_state &A = c->audit;
+  uint64_t gen = 0;
+  size_t res_bytes = 0;
+  const uint8_t *d_res = nullptr;
+  {
+    // Under the context's mutex: check, snapshot the slots and their liveness, upload, enqueue.  Nothing here waits for a kernel.
+    std::lock_guard<std::mutex> g(c->mu);
+    HS_CUDA(c, cudaSetDevice(c->device));
+    const size_t n = c->keys.atables ? c->n_keys : 0;
+    if (n_slots != n) return fail_args(c, "hs_table_audit", ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
+    if (expect_pks && n && !c->explicit_committee) return fail_args(c, "hs_table_audit", "key-cache tables are audited with expect_pks == NULL");
+    if (!A.stream) {
+      int lo = 0, hi = 0;
+      HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+      HS_CUDA(c, create(A.stream, lo));
+      HS_CUDA(c, create(A.done));
+    }
+    std::vector<uint8_t> live(n, 1);
+    if (c->explicit_committee) std::copy(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin());
+    res_bytes = 8 + 4 * (2 + n);
+    h2d_stage in;
+    const size_t s_res = in.add(nullptr, res_bytes), s_pks = in.add(expect_pks, expect_pks ? n * 32 : 0),
+                 s_live = in.add(expect_live, expect_live ? 4 * ((n + 31) / 32) : 0), s_mirror = in.add(live.data(), n),
+                 s_ok = in.add(nullptr, n);
+    HS_TRY(in.upload(c, A.scratch, A.stream));
+    uint8_t *res = in.ptr(s_res);
+    HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
+    HS_CUDA(c, cudaMemsetAsync(res + 8, 0, res_bytes - 8, A.stream));
+    const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
+    if (n) {
+      const key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)n};
+      k_slot_audit<<<blocks_for(n + (size_t)c->slot_mask + 1, 256), 256, 0, A.stream>>>(
+          T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
+          expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+    }
+    auto launch_tables = [&](const ge_niels *tables, size_t n_tables, size_t entries, int W, int n_windows, const uint8_t *pks) -> int {
+      const uint64_t warps = (uint64_t)n_tables * n_windows * ((((uint64_t)1 << (W - 1)) + 1 + 31) / 32);
+      k_table_audit<<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, A.stream>>>(
+          tables, n_tables, entries, W, n_windows, pks, in.ptr(s_ok), O);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+      return HS_OK;
+    };
+    if (n) HS_TRY(launch_tables(c->keys.atables, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks));
+    HS_TRY(launch_tables(c->d_btable, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr));
+    HS_CUDA(c, cudaEventRecord(A.done, A.stream));
+    gen = c->key_gen;
+    d_res = res;
+  }
+  // Without the mutex: wait for the kernels and read the findings back (A is this call's alone under audit_mu).
+  std::vector<uint8_t> h(res_bytes);
+  HS_CUDA(c, cudaEventSynchronize(A.done));
+  HS_CUDA(c, cudaMemcpyAsync(h.data(), d_res, res_bytes, cudaMemcpyDeviceToHost, A.stream));
+  HS_CUDA(c, cudaStreamSynchronize(A.stream));
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    if (c->key_gen != gen) return fail_args(c, "hs_table_audit", "key tables changed during the audit; run it again");
+  }
+  uint64_t first;
+  memcpy(&first, h.data(), 8);
+  const uint32_t *bits = reinterpret_cast<const uint32_t *>(h.data() + 8);
+  uint32_t failed = (bits[0] ? HS_AUDIT_BASE : 0u) | bits[1];
+  for (size_t s = 0; s < n_slots; s++) {
+    failed |= bits[2 + s];
+    if (out_slot_bits) out_slot_bits[s] = (uint8_t)bits[2 + s];
+  }
+  *out_failed = failed;
+  return failed ? fail(c, HS_ERR_SELFTEST, audit_message(first, n_slots, bits).c_str()) : HS_OK;
 }

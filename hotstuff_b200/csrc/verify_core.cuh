@@ -386,6 +386,90 @@ HS_HD void comb_build_block(ge_niels *table, const ge_ext &P, int W, int win, in
   }
 }
 
+// ---- table audit (hs_table_audit): every entry of a built comb table checked against the layout above with the curve arithmetic the
+// verify paths use, never with comb_build_block.  An entry passes when it is canonical, its third coordinate is 2dxy of the first two,
+// and it is the previous entry of its window plus entry 1; entry 0 must be the identity, entry 1 of window 0 the table's point, and entry
+// 1 of window i + 1 twice entry 2^(w-1) of window i.  By induction every entry is then m * 2^(w i) * P.
+// An affine Niels entry as an extended point scaled by 4 (its X = 4x, Y = 4y, Z = 4, T = 4xy): 1 multiplication.
+HS_HD void audit_niels_to_ext(ge_ext &p, const ge_niels &e) { ge_from_signed_niels(p, e.ymx, e.ypx); }
+// (X : Y : Z) equals the point of entry e: with e's 2x = ypx - ymx and 2y = ypx + ymx, compare (2X : 2Y : Z) with (2x, 2y).
+HS_HD uint32_t audit_proj_is_entry(const fe &X, const fe &Y, const fe &Z, const ge_niels &e) {
+  fe x2, y2, X2, Y2;
+  fe_sub(x2, e.ypx, e.ymx);
+  fe_add(y2, e.ypx, e.ymx);
+  fe_add(X2, X, X);
+  fe_add(Y2, Y, Y);
+  return ge_proj_equals_affine(X2, Y2, Z, x2, y2);
+}
+HS_HD uint32_t audit_fe_is_canonical(const fe &a) {
+  fe t;
+  fe_canon(t, a);
+  uint32_t d = 0;
+  for (int i = 0; i < 8; i++) d |= t.v[i] ^ a.v[i];
+  return d == 0;
+}
+// The checks of entry m (> 0: m - 1 is prev) that need no other window: identity for m = 0; otherwise canonical coordinates,
+// 2 xy2d == d (ypx^2 - ymx^2), and for m >= 2 e == prev + one (one = entry 1 of the same window).  1 = pass.
+HS_HD uint32_t audit_entry_local(const ge_niels &e, const ge_niels &prev, const ge_niels &one, uint32_t m) {
+  if (m == 0) {
+    uint32_t d = (e.ypx.v[0] ^ 1u) | (e.ymx.v[0] ^ 1u) | e.xy2d.v[0];
+    for (int i = 1; i < 8; i++) d |= e.ypx.v[i] | e.ymx.v[i] | e.xy2d.v[i];
+    return d == 0;
+  }
+  uint32_t ok = audit_fe_is_canonical(e.ypx) & audit_fe_is_canonical(e.ymx) & audit_fe_is_canonical(e.xy2d);
+  {
+    fe a, b, d;
+    fe_sqr(a, e.ypx);
+    fe_sqr(b, e.ymx);
+    fe_sub(a, a, b);
+    fe_const(d, HS_CONST(HS_D));
+    fe_mul(a, a, d);
+    fe_add(b, e.xy2d, e.xy2d);
+    ok &= fe_eq(a, b);
+  }
+  if (m >= 2) {
+    ge_ext p;
+    audit_niels_to_ext(p, prev);
+    ge_p1p1 c;
+    ge_madd_signed_p1p1(c, p, one, 0);
+    fe X, Y, Z;
+    fe_mul(X, c.E, c.F);
+    fe_mul(Y, c.G, c.H);
+    fe_mul(Z, c.F, c.G);
+    ok &= audit_proj_is_entry(X, Y, Z, e);
+  }
+  return ok;
+}
+// Window link: entry 1 of window i + 1 (one) == 2 * entry 2^(w-1) of window i (last).
+HS_HD uint32_t audit_link(const ge_niels &one, const ge_niels &last) {
+  ge_ext p;
+  audit_niels_to_ext(p, last);
+  ge_p1p1 c;
+  ge_dbl_p1p1(c, p);
+  fe X, Y, Z;
+  fe_mul(X, c.E, c.F);
+  fe_mul(Y, c.G, c.H);
+  fe_mul(Z, c.F, c.G);
+  return audit_proj_is_entry(X, Y, Z, one);
+}
+// The point entry 1 of window 0 must hold: -A for the 32-byte key enc (returns 0 when it does not decompress), B for enc == nullptr.
+HS_HD uint32_t audit_anchor_point(ge_ext &P, const uint32_t *enc) {
+  if (!enc) {
+    ge_basepoint(P);
+    return 1;
+  }
+  uint32_t w[8];
+  for (int i = 0; i < 8; i++) w[i] = enc[i];
+  ge_ext A;
+  const uint32_t ok = ge_decompress(A, w);
+  ge_neg(P, A);
+  return ok;
+}
+HS_HD uint32_t audit_anchor(const ge_niels &one, const ge_ext &P) { return audit_proj_is_entry(P.X, P.Y, P.Z, one); }
+// The first finding of an audit, as one 64-bit key whose minimum is the first in (slot, window, entry) order: code 0 = the base table,
+// s + 1 = key slot s; window field 0 = a finding about the slot itself (key bytes, flag, lookup), i + 1 = window i of its table.
+HS_HD uint64_t audit_key(uint64_t code, uint32_t wfield, uint32_t entry) { return (code << 32) | ((uint64_t)wfield << 26) | entry; }
+
 // ---- signing (load generation only: SURVEY §8f.4 — the reference node signs on the CPU, one signature per request,
 // crypto/src/lib.rs:185-191; this exists to synthesise 2^20-scale benchmark / test inputs in milliseconds).  RFC 8032 §5.1.6:
 //   (a, prefix) = clamp / split of SHA-512(seed);  r = SHA-512(prefix || M) mod l;  R = [r]B;  k = SHA-512(R || A || M) mod l;

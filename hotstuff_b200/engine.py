@@ -113,6 +113,30 @@ class Engine:
         return 0
 
     @property
+    def key_slots(self):
+        """Key slots in use (hs_key_slots): the committee's, spares taken by updates included, or the key cache's learned keys."""
+        return int(self.lib.hs_key_slots(self.h))
+
+    def table_audit(self, expect=None, live=None):
+        """Audit of the live key tables on the GPU (hs_table_audit).  expect: (key_slots, 32) uint8, the node's index -> key map, or None
+        to check the engine against itself; live: a uint32 bitmap of the slots expected live (None: every slot).  Returns (failed,
+        slot_bits): the HS_AUDIT_* mask (0 = every check passed, last_error names the first finding otherwise) and one uint8 of
+        HS_AUDIT_* bits per slot.  Raises EngineError on a bad argument (key_slots changed, expect given for key-cache tables), when the
+        tables changed while the audit ran (call again), and on no memory or a CUDA error."""
+        n = self.key_slots if expect is None else _u8(expect, 32).reshape(-1, 32).shape[0]
+        exp = None if expect is None else _u8(expect, 32).reshape(-1, 32)
+        lv = None if live is None else np.ascontiguousarray(live, dtype=np.uint32)
+        if lv is not None and lv.size < (n + 31) // 32:
+            raise ValueError("table_audit: %d live words for %d slots" % (lv.size, n))
+        bits = np.zeros(max(1, n), dtype=np.uint8)
+        failed = ctypes.c_uint32(0)
+        rc = self.lib.hs_table_audit(self.h, _ptr(exp) if n and exp is not None else None, _ptr(lv) if lv is not None and lv.size else None, n,
+                                     _ptr(bits), ctypes.byref(failed))
+        if rc != HS_ERR_SELFTEST:
+            self._check(rc, "hs_table_audit")
+        return int(failed.value), bits[:n]
+
+    @property
     def last_error(self):
         return self.lib.hs_last_error(self.h).decode()
 

@@ -30,7 +30,7 @@ extern "C" {
 #define HS_ERR_CUDA 1
 #define HS_ERR_ARG 2
 #define HS_ERR_NOMEM 3
-#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer */
+#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer; hs_table_audit: a table, slot or lookup entry is wrong */
 
 /* verdict selector for the verify entry points */
 #define HS_MODE_STRICT 0u /* Signature::verify semantics  = dalek verify_strict          (crypto/src/lib.rs:200-204) */
@@ -379,6 +379,43 @@ int hs_verify_msgs(hs_ctx *ctx, const uint8_t *sig /* n x 64 */, const uint8_t *
 #define HS_SELFTEST_SIGN (1u << 14)           /* k_keygen + k_sign_digests */
 #define HS_SELFTEST_VERIFY_PATHS 0x1ff8u      /* GENERIC .. QUEUE_GENERIC: the paths caller records run through */
 int hs_self_test(hs_ctx *ctx, int key_bits, const hs_rec128 *recs_or_null, const uint8_t *expect_or_null, size_t n, uint32_t *out_failed_paths);
+
+/* ---- audit of the live key tables: every comb-table entry, key slot and lookup entry against the key it must hold ------------------
+ * hs_self_test proves the kernels on scratch tables; this call checks the state the node actually verifies against, which lives for the
+ * whole process: the per-key comb tables, the slot -> key bytes array with its flags, the device hash table from key bytes to slot, and
+ * the base-point table.  A slot reached from key X's bytes whose table holds multiples of key Y would accept Y's signatures as X's, so
+ * call it at start-up (after hs_self_test), after every committee change, and periodically on a live node.
+ *   - Tables: entry 0 of every window is exactly (1, 1, 0); every coordinate is canonical; 2 xy2d == d ((y+x)^2 - (y-x)^2); entry m is
+ *     entry m - 1 plus entry 1 of its window; entry 1 of window i + 1 is twice entry 2^(w-1) of window i; entry 1 of window 0 is -A,
+ *     decompressed from the slot's stored bytes (B for the base-point table).  By induction every entry is the multiple it must be.
+ *   - Slots: KEY compares the stored bytes and the engine's liveness with the caller's map; FLAG checks the device flag byte against the
+ *     liveness and the key's decompression; LOOKUP probes the device hash table with every live slot's bytes (it must reach a live slot
+ *     with those bytes: registration keeps the first of duplicated keys) and checks that every hash entry names a live slot its own bytes
+ *     reach.  A live slot whose key does not decompress has no table to check.
+ *   - n_slots must equal hs_key_slots(ctx).  expect_pks (n_slots x 32, nullable) is the caller's index -> key map, for example the
+ *     registration order updated with every out_add_idx; NULL checks the engine against itself.  expect_live (one bit per slot, nullable:
+ *     every slot live) is compared with the engine's liveness whenever either expectation is given.  Key-cache tables take expect_pks == NULL.
+ *     The base-point table is always checked; a context without per-key tables checks only it, with n_slots = 0.
+ *   - Returns HS_OK with *out_failed = 0; HS_ERR_SELFTEST with the HS_AUDIT_* bits OR-ed into *out_failed, each slot's bits in
+ *     out_slot_bits (nullable) and hs_last_error naming the first finding (slot, class, window and entry for a table finding).
+ *     HS_ERR_ARG writes nothing: bad pointers, n_slots != hs_key_slots, expect_pks for key-cache tables, or key tables that changed while
+ *     the audit ran (a registration, update or key-cache build: call it again).  HS_ERR_NOMEM / HS_ERR_CUDA as elsewhere.
+ *   - Isolation: the context's mutex is held only to check the arguments, snapshot the slots and enqueue; the kernels run on a private
+ *     stream of the lowest priority and the call waits for them without the mutex, so verify queues keep launching.  Reads every table and
+ *     mirror and writes none; the verify queues, their caches and counters, the deferred scratch and the peer route are not touched.  Its
+ *     launches count in hs_kernel_launches.  Audits of one context run one at a time.  `_dev` verify passes take no mutex and may grow
+ *     the key cache, so they must not overlap an audit of the same context. */
+/* Key slots in use: the registered committee's (N plus the spare slots hs_committee_update has taken, freed ones included), or the
+ * key cache's learned keys; 0 when the context holds no per-key tables. */
+size_t hs_key_slots(const hs_ctx *ctx);
+#define HS_AUDIT_KEY    (1u << 0) /* the slot's stored key bytes, or whether it is live, differ from the caller's expectation */
+#define HS_AUDIT_FLAG   (1u << 1) /* the slot's device flag byte disagrees with its liveness and with whether its key decompresses */
+#define HS_AUDIT_LOOKUP (1u << 2) /* the device hash table does not take the slot's key bytes to it (or to a live slot with the same
+                                     bytes), or a hash entry names this slot although it is not live */
+#define HS_AUDIT_TABLE  (1u << 3) /* an entry of the slot's comb table is not the multiple of -A it must hold */
+#define HS_AUDIT_BASE   (1u << 4) /* out_failed only: an entry of the base-point table is not the multiple of B it must hold */
+int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
+                   size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_failed);
 
 /* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) ------------------- */
 int hs_verify_rec128_dev(hs_ctx *ctx, const void *d_recs, size_t n, uint32_t mode, void *d_bitmap, void *stream);

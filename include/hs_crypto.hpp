@@ -54,6 +54,24 @@ class Engine {
     if (rc != HS_ERR_SELFTEST) check(rc, "hs_self_test");
     return failed;
   }
+  // Key slots in use (hs_key_slots): the committee's, spare slots taken by updates included, or the key cache's learned keys.
+  size_t key_slots() const { return hs_key_slots(ctx_); }
+  // Audit of the live key tables (hs_table_audit): 0 when every check passes, else the HS_AUDIT_* bits (error() names the first
+  // finding).  expect: the node's index -> key map (key_slots() entries, nullptr = the engine against itself); live: one bit per slot
+  // expected live (nullptr = all); slot_bits (nullable) receives each slot's HS_AUDIT_* bits.  Throws EngineError on a bad argument,
+  // tables that changed during the audit (call again), no device memory or a CUDA error.
+  uint32_t table_audit(const std::vector<std::array<uint8_t, 32>> *expect = nullptr, const std::vector<uint32_t> *live = nullptr,
+                       std::vector<uint8_t> *slot_bits = nullptr) const {
+    const size_t n = expect ? expect->size() : key_slots();
+    if (live && live->size() < (n + 31) / 32) throw EngineError("table_audit: live bitmap shorter than the slots");
+    std::vector<uint8_t> bits(n);
+    uint32_t failed = 0;
+    const int rc = hs_table_audit(ctx_, expect && n ? expect->front().data() : nullptr, live && !live->empty() ? live->data() : nullptr, n,
+                                  bits.data(), &failed);
+    if (rc != HS_ERR_SELFTEST) check(rc, "hs_table_audit");
+    if (slot_bits) *slot_bits = std::move(bits);
+    return failed;
+  }
   std::string error() const { return hs_last_error(ctx_); }
 
  private:

@@ -13,7 +13,7 @@
 //     (ingest_frames + verify_ingested: the receiver path of consensus.rs:138 without building the message structs first).
 use std::os::raw::c_int;
 use std::sync::atomic::{AtomicBool, Ordering};
-use std::sync::OnceLock;
+use std::sync::{Mutex, OnceLock};
 
 /// The verify queue (hs_queue_*): concurrent single-message verifies share latency-path launches (`queue::verify_queued`).
 #[path = "crypto_gpu_queue.rs"]
@@ -67,6 +67,7 @@ pub struct HsIngestOut { pub cap_items: usize, pub cap_msgs: usize, pub cap_pre_
 pub const HS_FRAME_MALFORMED: u8 = 255;
 
 pub const HS_OK: c_int = 0;
+pub const HS_ERR_ARG: c_int = 2;
 pub const HS_ERR_NOMEM: c_int = 3;
 /// Smallest signature count sent to the GPU (below it the dalek path is faster on this hardware; see the header comment).
 pub const GPU_MIN_SIGS: usize = 2;
@@ -92,6 +93,7 @@ extern "C" {
                         out_item_bitmap: *mut u32, out_group_bitmap: *mut u32) -> c_int;
     fn hs_ingest_consensus_frames(frames: *const u8, off: *const u64, n: usize, info: *mut HsFrameInfo, out: *mut HsIngestOut) -> c_int;
     fn hs_self_test(ctx: *mut HsCtx, key_bits: c_int, recs: *const HsRec128, expect: *const u8, n: usize, out_failed_paths: *mut u32) -> c_int;
+    fn hs_table_audit(ctx: *mut HsCtx, expect_pks: *const u8, expect_live: *const u32, n_slots: usize, out_slot_bits: *mut u8, out_failed: *mut u32) -> c_int;
 }
 
 struct Ctx(*mut HsCtx);
@@ -100,6 +102,9 @@ unsafe impl Sync for Ctx {}            // host-pointer entry points are serialis
 static CTX: OnceLock<Option<Ctx>> = OnceLock::new();
 /// Set when `self_test` fails: the engine gives wrong answers on this box, so every call below answers None (the dalek path).
 static DISABLED: AtomicBool = AtomicBool::new(false);
+/// The node-side index -> key map of the registered committee (None = a freed index): registration order, then every update's
+/// removals and returned indices.  `audit_tables` checks the engine's slots against it after every change.
+static KEYS: Mutex<Vec<Option<[u8; 32]>>> = Mutex::new(Vec::new());
 
 /// None when no GPU / the library failed to initialise / the self-test failed: every caller below then stays on the CPU path.
 fn ctx() -> Option<*mut HsCtx> {
@@ -122,7 +127,8 @@ pub fn register_committee(keys: &[[u8; 32]]) -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut valid = vec![0u32; (keys.len() + 31) / 32];
     let rc = unsafe { hs_committee_register(c, keys.as_ptr() as *const u8, keys.len(), valid.as_mut_ptr()) };
-    if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    if rc != HS_OK { KEYS.lock().unwrap().clear(); return Err(GpuError::Engine(last_error(c))); }
+    *KEYS.lock().unwrap() = keys.iter().map(|k| Some(*k)).collect();
     let bad: Vec<usize> = (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect();
     if bad.is_empty() { Ok(()) } else { Err(GpuError::InvalidKeys(bad)) }
 }
@@ -133,17 +139,44 @@ pub fn self_test() -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut failed = 0u32;
     let rc = unsafe { hs_self_test(c, 0, std::ptr::null(), std::ptr::null(), 0, &mut failed) };
-    if rc == HS_OK && failed == 0 { return Ok(()); }
+    if rc == HS_OK && failed == 0 { return audit_tables(&KEYS.lock().unwrap()); }
     DISABLED.store(true, Ordering::Release);
     Err(GpuError::Engine(format!("self-test failed (status {}, paths {:#x}): {}", rc, failed, last_error(c))))
+}
+/// Audit of the live key tables (hs_table_audit): every comb-table entry, key slot and lookup entry of the engine against `expected`,
+/// the node's index -> key map (None = a freed index).  `self_test` and `update_committee` call it; a live node may also call it
+/// periodically from a blocking task.  On a finding the GPU is switched off for the life of the process, as after a failed self-test.
+/// Tables that changed while it ran (a committee change from another task) are audited again.
+pub fn audit_tables(expected: &[Option<[u8; 32]>]) -> Result<(), GpuError> {
+    let c = ctx().ok_or(GpuError::Unavailable)?;
+    let pks: Vec<u8> = expected.iter().flat_map(|k| k.unwrap_or([0u8; 32])).collect();
+    let mut live = vec![0u32; (expected.len() + 31) / 32];
+    for (i, k) in expected.iter().enumerate() { if k.is_some() { live[i / 32] |= 1 << (i % 32); } }
+    let mut failed = 0u32;
+    let mut rc = HS_OK;
+    for _ in 0..3 {
+        rc = unsafe { hs_table_audit(c, if expected.is_empty() { std::ptr::null() } else { pks.as_ptr() }, live.as_ptr(), expected.len(),
+                                     std::ptr::null_mut(), &mut failed) };
+        if !(rc == HS_ERR_ARG && last_error(c).contains("changed during the audit")) { break; }
+    }
+    if rc == HS_OK && failed == 0 { return Ok(()); }
+    DISABLED.store(true, Ordering::Release);
+    Err(GpuError::Engine(format!("table audit failed (status {}, classes {:#x}): {}", rc, failed, last_error(c))))
 }
 /// Incremental epoch change: returns the table indices of the added validators.
 pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut out = vec![0u32; add.len().max(1)];
+    let mut keys = KEYS.lock().unwrap();  // held across the update and its audit: the map and the engine change together
     let rc = unsafe { hs_committee_update(c, add.as_ptr() as *const u8, add.len(), remove_idx.as_ptr(), remove_idx.len(), out.as_mut_ptr()) };
     if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
     out.truncate(add.len());
+    for &i in remove_idx { keys[i as usize] = None; }
+    for (k, &i) in add.iter().zip(out.iter()) {
+        if i as usize >= keys.len() { keys.resize(i as usize + 1, None); }
+        keys[i as usize] = Some(*k);
+    }
+    audit_tables(&keys)?;
     Ok(out)
 }
 

@@ -1483,6 +1483,7 @@ struct peer_bufs {
   dev_mem<uint32_t> own;
   ipc_mapping mapped[HS_MAX_PEERS];
 };
+enum : uint8_t { SLOT_LIVE = 1, SLOT_REPAIR = 2 };  // hs_ctx::h_key_live values of a slot in use
 struct hs_ctx {
   int device = 0;
   unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
@@ -1506,7 +1507,7 @@ struct hs_ctx {
   size_t cache_cap = 4096;           // keys
   std::vector<uint8_t> h_pks;        // host mirrors of d_pks / d_slots (key cache and hs_committee_update)
   std::vector<uint32_t> h_slots;
-  std::vector<uint8_t> h_key_live;   // explicit committee: 1 = slot holds a live validator, 0 = removed (free for reuse)
+  std::vector<uint8_t> h_key_live;   // explicit committee: SLOT_LIVE, SLOT_REPAIR (live, out of service during hs_table_repair) or 0 = removed (free for reuse)
   size_t table_budget = 0;           // bytes the per-key tables may use (0 = ~62 % of the device)
   size_t key_capacity = 0;           // explicit committee: table slots allocated (>= n_keys; spare slots serve hs_committee_update)
   learn_bufs learn;
@@ -1638,9 +1639,10 @@ static int launch_qc_and(hs_ctx *c, const uint32_t *d_items, const uint32_t *d_g
 }
 
 
-static int launch_build(hs_ctx *c, const uint8_t *d_encs, size_t n_points, int negate, int W, int n_windows, ge_niels *tables, uint8_t *flags) {
+static int launch_build(hs_ctx *c, const uint8_t *d_encs, size_t n_points, int negate, int W, int n_windows, ge_niels *tables, uint8_t *flags,
+                        cudaStream_t stream) {
   size_t threads = n_points * (size_t)n_windows * ((1u << (W - 1)) / HS_BUILD_BLOCK);
-  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, c->stream>>>(d_encs, n_points, negate, W, n_windows, tables, flags);
+  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(d_encs, n_points, negate, W, n_windows, tables, flags);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -2921,7 +2923,7 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
   c->cache_wanted = c->cache_enabled = !(flags & HS_FLAG_NO_KEY_CACHE) && !(getenv("HS_KEY_CACHE") && getenv("HS_KEY_CACHE")[0] == '0');
   if (e == cudaSuccess) e = alloc(c->d_btable, sizeof(ge_niels) * comb_table_entries(wb));
   if (e == cudaSuccess) {
-    if (launch_build(c, nullptr, 1, 0, wb, c->cp.nb, c->d_btable, nullptr) != HS_OK) e = cudaGetLastError();
+    if (launch_build(c, nullptr, 1, 0, wb, c->cp.nb, c->d_btable, nullptr, c->stream) != HS_OK) e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess) {
@@ -3074,7 +3076,7 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
   int rc = HS_OK;
   e = cudaMemcpyAsync(c->keys.pks, pks, N * 32, cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(c->keys.slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags);
+  if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags, c->stream);
   if (e == cudaSuccess && rc == HS_OK) e = cudaStreamSynchronize(c->stream);
   std::vector<uint8_t> fl(N);
   if (e == cudaSuccess && rc == HS_OK) e = cudaMemcpy(fl.data(), c->keys.key_flags, N, cudaMemcpyDeviceToHost);
@@ -3100,6 +3102,31 @@ int hs_committee_register(hs_ctx *c, const uint8_t *pks, size_t N, uint32_t *out
   if (!c || (N && !pks) || N >= HS_NO_KEY) return fail(c, HS_ERR_ARG, "hs_committee_register: bad argument");
   std::lock_guard<std::mutex> g(c->mu);
   return committee_register_locked(c, pks, N, out_valid_bitmap);
+}
+
+// Rebuilds the open-addressing table from the host mirror (deletions leave no tombstones; the first of duplicated key bytes wins) over
+// the slots in service: every learned key of the key cache, a committee's live slots but those under repair (SLOT_REPAIR).  Publishes
+// it on the context's stream and waits, so that every launch enqueued afterwards, on any stream, probes the new table.
+static int publish_hash(hs_ctx *c) {
+  std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
+  for (size_t i = 0; i < c->n_keys; i++) {
+    if (c->explicit_committee && c->h_key_live[i] != SLOT_LIVE) continue;
+    uint32_t w[8];
+    memcpy(w, c->h_pks.data() + 32 * i, 32);
+    uint32_t h = key_hash(w) & c->slot_mask;
+    bool dup = false;
+    while (c->h_slots[h] != HS_NO_KEY) {
+      if (memcmp(c->h_pks.data() + 32 * (size_t)c->h_slots[h], c->h_pks.data() + 32 * i, 32) == 0) {
+        dup = true;
+        break;
+      }
+      h = (h + 1) & c->slot_mask;
+    }
+    if (!dup) c->h_slots[h] = (uint32_t)i;
+  }
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  return HS_OK;
 }
 
 // Incremental epoch change (consensus/src/config.rs Committee: a few validators join / leave): removed indices stop
@@ -3147,30 +3174,13 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
       memcpy(c->h_pks.data() + 32 * (size_t)idx, key, 32);
       c->h_key_live[idx] = 1;
       HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)idx, key, 32, cudaMemcpyHostToDevice, c->stream));
-      HS_TRY(launch_build(c, c->keys.pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->keys.atables + (size_t)idx * c->a_table_entries, c->keys.key_flags + idx));
+      HS_TRY(launch_build(c, c->keys.pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->keys.atables + (size_t)idx * c->a_table_entries,
+                          c->keys.key_flags + idx, c->stream));
       added.push_back(idx);
     }
     out_add_idx[i] = idx;
   }
-  // rebuild the open-addressing table from the live keys (deletions leave no tombstones) and publish it
-  std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
-  for (size_t i = 0; i < c->n_keys; i++) {
-    if (!c->h_key_live[i]) continue;
-    uint32_t w[8];
-    memcpy(w, c->h_pks.data() + 32 * i, 32);
-    uint32_t h = key_hash(w) & c->slot_mask;
-    bool dup = false;
-    while (c->h_slots[h] != HS_NO_KEY) {
-      if (memcmp(c->h_pks.data() + 32 * (size_t)c->h_slots[h], c->h_pks.data() + 32 * i, 32) == 0) {
-        dup = true;
-        break;
-      }
-      h = (h + 1) & c->slot_mask;
-    }
-    if (!dup) c->h_slots[h] = (uint32_t)i;
-  }
-  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
-  HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  HS_TRY(publish_hash(c));
   return HS_OK;
 }
 /* Upper bound (bytes) for the per-key tables of the NEXT registration / key-cache allocation; 0 = default (~62 % of the device). */
@@ -4008,6 +4018,7 @@ int hs_queue_cert_stats(hs_queue *q, uint64_t out[HS_QUEUE_CERT_STATS]) {
 }
 
 #define HS_QUEUE_SIG_MAX_ENTRIES (1ull << 26)  // 9.7 GB of table
+static int sig_cache_set_locked(hs_queue *q, uint32_t buckets);
 int hs_queue_sig_cache(hs_queue *q, size_t entries) {
   if (!q || entries > HS_QUEUE_SIG_MAX_ENTRIES) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_cache: bad argument");
   hs_ctx *c = q->c;
@@ -4016,6 +4027,12 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries) {
     for (buckets = 1; (size_t)buckets * HS_SIG_WAYS < entries;) buckets <<= 1;
   std::lock_guard<std::mutex> g(c->mu);  // the dispatcher launches only while it holds c->mu
   if (buckets == (q->d_sig ? q->sig_bmask + 1 : 0u)) return HS_OK;
+  return sig_cache_set_locked(q, buckets);
+}
+// Replaces q's signature-cache table by an empty one of `buckets` buckets (0: off), under c->mu.  hs_table_repair empties the cache by
+// replacing the table with one of the same size.
+static int sig_cache_set_locked(hs_queue *q, uint32_t buckets) {
+  hs_ctx *c = q->c;
   HS_CUDA(c, cudaSetDevice(c->device));
   // Drains the queue's streams: no launch that probes the old table survives these lines.
   HS_CUDA(c, cudaStreamSynchronize(q->stream));
@@ -4659,78 +4676,248 @@ static std::string audit_message(uint64_t first, size_t n_slots, const uint32_t 
   return m;
 }
 
+// k_table_audit over n_tables tables on `stream` (auditable: nullable for the base-point table).
+static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *tables, size_t n_tables, size_t entries, int W, int n_windows,
+                              const uint8_t *pks, const uint8_t *auditable, const audit_out &O) {
+  const uint64_t warps = (uint64_t)n_tables * n_windows * ((((uint64_t)1 << (W - 1)) + 1 + 31) / 32);
+  k_table_audit<<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, stream>>>(tables, n_tables, entries, W,
+                                                                                                                n_windows, pks, auditable, O);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+
+// One complete audit: enqueued under c->mu by audit_enqueue_locked, then waited for and read back without it by audit_collect.  Its
+// caller holds audit_mu, so the audit's stream, event and scratch are its own.
+struct audit_run {
+  uint64_t gen = 0;              // key_gen when the kernels were enqueued
+  size_t n_slots = 0;
+  const uint8_t *d_res = nullptr;
+  std::vector<uint8_t> res;      // the first finding's audit_key() (8 bytes), then bits[2 + n_slots]
+  uint64_t first() const {
+    uint64_t f;
+    memcpy(&f, res.data(), 8);
+    return f;
+  }
+  const uint32_t *bits() const { return reinterpret_cast<const uint32_t *>(res.data() + 8); }
+  uint32_t failed() const {
+    uint32_t f = (bits()[0] ? HS_AUDIT_BASE : 0u) | bits()[1];
+    for (size_t s = 0; s < n_slots; s++) f |= bits()[2 + s];
+    return f;
+  }
+};
+// Checks the arguments, snapshots the slots and their liveness, uploads and enqueues.  Nothing here waits for a kernel.
+static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots,
+                                audit_run &r) {
+  audit_state &A = c->audit;
+  HS_CUDA(c, cudaSetDevice(c->device));
+  const size_t n = c->keys.atables ? c->n_keys : 0;
+  if (n_slots != n) return fail_args(c, entry, ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
+  if (expect_pks && n && !c->explicit_committee) return fail_args(c, entry, "key-cache tables are audited with expect_pks == NULL");
+  if (!A.stream) {
+    int lo = 0, hi = 0;
+    HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    HS_CUDA(c, create(A.stream, lo));
+    HS_CUDA(c, create(A.done));
+  }
+  std::vector<uint8_t> live(n, 1);
+  if (c->explicit_committee) std::copy(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin());
+  const size_t res_bytes = 8 + 4 * (2 + n);
+  h2d_stage in;
+  const size_t s_res = in.add(nullptr, res_bytes), s_pks = in.add(expect_pks, expect_pks ? n * 32 : 0),
+               s_live = in.add(expect_live, expect_live ? 4 * ((n + 31) / 32) : 0), s_mirror = in.add(live.data(), n),
+               s_ok = in.add(nullptr, n);
+  HS_TRY(in.upload(c, A.scratch, A.stream));
+  uint8_t *res = in.ptr(s_res);
+  HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
+  HS_CUDA(c, cudaMemsetAsync(res + 8, 0, res_bytes - 8, A.stream));
+  const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
+  if (n) {
+    const key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)n};
+    k_slot_audit<<<blocks_for(n + (size_t)c->slot_mask + 1, 256), 256, 0, A.stream>>>(
+        T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
+        expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
+    c->launches++;
+    HS_CUDA(c, cudaGetLastError());
+    HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
+  }
+  HS_TRY(launch_table_audit(c, A.stream, c->d_btable, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
+  HS_CUDA(c, cudaEventRecord(A.done, A.stream));
+  r.gen = c->key_gen;
+  r.n_slots = n;
+  r.d_res = res;
+  r.res.resize(res_bytes);
+  return HS_OK;
+}
+// Without c->mu: waits for the kernels and reads the findings back.  HS_ERR_ARG (`changed`) when the key tables changed meanwhile.
+static int audit_collect(hs_ctx *c, const char *entry, const char *changed, audit_run &r) {
+  audit_state &A = c->audit;
+  HS_CUDA(c, cudaEventSynchronize(A.done));
+  HS_CUDA(c, cudaMemcpyAsync(r.res.data(), r.d_res, r.res.size(), cudaMemcpyDeviceToHost, A.stream));
+  HS_CUDA(c, cudaStreamSynchronize(A.stream));
+  std::lock_guard<std::mutex> g(c->mu);
+  if (c->key_gen != r.gen) return fail_args(c, entry, changed);
+  return HS_OK;
+}
+
 extern "C" int hs_table_audit(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots, uint8_t *out_slot_bits,
                               uint32_t *out_failed) {
   if (!c || !out_failed) return fail(c, HS_ERR_ARG, "hs_table_audit: bad argument");
   std::lock_guard<std::mutex> ga(c->audit_mu);
-  audit_state &A = c->audit;
-  uint64_t gen = 0;
-  size_t res_bytes = 0;
-  const uint8_t *d_res = nullptr;
-  {
-    // Under the context's mutex: check, snapshot the slots and their liveness, upload, enqueue.  Nothing here waits for a kernel.
-    std::lock_guard<std::mutex> g(c->mu);
-    HS_CUDA(c, cudaSetDevice(c->device));
-    const size_t n = c->keys.atables ? c->n_keys : 0;
-    if (n_slots != n) return fail_args(c, "hs_table_audit", ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
-    if (expect_pks && n && !c->explicit_committee) return fail_args(c, "hs_table_audit", "key-cache tables are audited with expect_pks == NULL");
-    if (!A.stream) {
-      int lo = 0, hi = 0;
-      HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-      HS_CUDA(c, create(A.stream, lo));
-      HS_CUDA(c, create(A.done));
-    }
-    std::vector<uint8_t> live(n, 1);
-    if (c->explicit_committee) std::copy(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin());
-    res_bytes = 8 + 4 * (2 + n);
-    h2d_stage in;
-    const size_t s_res = in.add(nullptr, res_bytes), s_pks = in.add(expect_pks, expect_pks ? n * 32 : 0),
-                 s_live = in.add(expect_live, expect_live ? 4 * ((n + 31) / 32) : 0), s_mirror = in.add(live.data(), n),
-                 s_ok = in.add(nullptr, n);
-    HS_TRY(in.upload(c, A.scratch, A.stream));
-    uint8_t *res = in.ptr(s_res);
-    HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
-    HS_CUDA(c, cudaMemsetAsync(res + 8, 0, res_bytes - 8, A.stream));
-    const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
-    if (n) {
-      const key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)n};
-      k_slot_audit<<<blocks_for(n + (size_t)c->slot_mask + 1, 256), 256, 0, A.stream>>>(
-          T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
-          expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
-      c->launches++;
-      HS_CUDA(c, cudaGetLastError());
-    }
-    auto launch_tables = [&](const ge_niels *tables, size_t n_tables, size_t entries, int W, int n_windows, const uint8_t *pks) -> int {
-      const uint64_t warps = (uint64_t)n_tables * n_windows * ((((uint64_t)1 << (W - 1)) + 1 + 31) / 32);
-      k_table_audit<<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, A.stream>>>(
-          tables, n_tables, entries, W, n_windows, pks, in.ptr(s_ok), O);
-      c->launches++;
-      HS_CUDA(c, cudaGetLastError());
-      return HS_OK;
-    };
-    if (n) HS_TRY(launch_tables(c->keys.atables, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks));
-    HS_TRY(launch_tables(c->d_btable, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr));
-    HS_CUDA(c, cudaEventRecord(A.done, A.stream));
-    gen = c->key_gen;
-    d_res = res;
-  }
-  // Without the mutex: wait for the kernels and read the findings back (A is this call's alone under audit_mu).
-  std::vector<uint8_t> h(res_bytes);
-  HS_CUDA(c, cudaEventSynchronize(A.done));
-  HS_CUDA(c, cudaMemcpyAsync(h.data(), d_res, res_bytes, cudaMemcpyDeviceToHost, A.stream));
-  HS_CUDA(c, cudaStreamSynchronize(A.stream));
+  audit_run r;
   {
     std::lock_guard<std::mutex> g(c->mu);
-    if (c->key_gen != gen) return fail_args(c, "hs_table_audit", "key tables changed during the audit; run it again");
+    HS_TRY(audit_enqueue_locked(c, "hs_table_audit", expect_pks, expect_live, n_slots, r));
   }
-  uint64_t first;
-  memcpy(&first, h.data(), 8);
-  const uint32_t *bits = reinterpret_cast<const uint32_t *>(h.data() + 8);
-  uint32_t failed = (bits[0] ? HS_AUDIT_BASE : 0u) | bits[1];
-  for (size_t s = 0; s < n_slots; s++) {
-    failed |= bits[2 + s];
-    if (out_slot_bits) out_slot_bits[s] = (uint8_t)bits[2 + s];
-  }
+  HS_TRY(audit_collect(c, "hs_table_audit", "key tables changed during the audit; run it again", r));
+  const uint32_t failed = r.failed();
+  for (size_t s = 0; s < n_slots && out_slot_bits; s++) out_slot_bits[s] = (uint8_t)r.bits()[2 + s];
   *out_failed = failed;
-  return failed ? fail(c, HS_ERR_SELFTEST, audit_message(first, n_slots, bits).c_str()) : HS_OK;
+  return failed ? fail(c, HS_ERR_SELFTEST, audit_message(r.first(), n_slots, r.bits()).c_str()) : HS_OK;
 }
+
+// ---- repair of what the audit finds (hs_table_repair)
+// Empties the signature cache and the certificate cache of every verify queue of the context (under c->mu, the device drained): a
+// record accepted against a wrong table must not be answered from a cache.  Requests in flight complete as they would.
+static int flush_queue_caches(hs_ctx *c) {
+  std::lock_guard<std::mutex> gq(c->queues_mu);
+  for (hs_queue *q : c->queues) {
+    if (q->d_sig) HS_TRY(sig_cache_set_locked(q, q->sig_bmask + 1));
+    std::lock_guard<std::mutex> g(q->mu);
+    cert_evict_locked(q, 0);
+  }
+  return HS_OK;
+}
+
+// Repairs the findings of audit `first` from the authority (the caller's map, else the host mirror), under the lock `g` of c->mu.
+// The base-point table is rebuilt in place with the device drained.  Slots with a KEY, FLAG or TABLE finding that the authority holds
+// dead are taken out of service as a removal would; the others (R) are rebuilt.  A committee's R is taken out of service (flag 0,
+// SLOT_REPAIR: out of the hash table), rebuilt and proven on the audit's stream without the mutex, and each slot whose table passes
+// goes back.  The key cache's R is rebuilt with the mutex held throughout: a learned key taken out of the hash table would be learned
+// again.  HS_ERR_ARG `changed` when the key tables changed during the repair; what the repair took out of service is put back first.
+static int repair_locked(hs_ctx *c, std::unique_lock<std::mutex> &g, const audit_run &first, const uint8_t *expect_pks,
+                         const uint32_t *expect_live, const char *changed) {
+  audit_state &A = c->audit;
+  if (c->key_gen != first.gen) return fail_args(c, "hs_table_repair", changed);
+  HS_CUDA(c, cudaSetDevice(c->device));
+  HS_CUDA(c, cudaDeviceSynchronize());  // nothing that read a wrong table is in flight, verify queue launches included
+  const bool committee = c->explicit_committee;
+  const uint32_t *bits = first.bits();
+  if (bits[0]) {
+    HS_TRY(launch_build(c, nullptr, 1, 0, c->cp.wb, c->cp.nb, c->d_btable, nullptr, c->stream));
+    HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  std::vector<uint32_t> R;
+  for (size_t s = 0; s < first.n_slots; s++) {
+    if (!(bits[2 + s] & (HS_AUDIT_KEY | HS_AUDIT_FLAG | HS_AUDIT_TABLE))) continue;
+    const bool live = !committee || (expect_live ? (expect_live[s >> 5] >> (s & 31)) & 1u : (expect_pks || c->h_key_live[s]));
+    if (live) {
+      R.push_back((uint32_t)s);
+      if (expect_pks) memcpy(c->h_pks.data() + 32 * s, expect_pks + 32 * s, 32);
+    }
+    if (committee) c->h_key_live[s] = live ? SLOT_REPAIR : 0;
+    HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + s, 0, 1, c->stream));
+  }
+  if (first.n_slots) HS_TRY(publish_hash(c));  // also the whole repair of a LOOKUP finding
+  HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  HS_TRY(flush_queue_caches(c));
+  const uint64_t gen = ++c->key_gen;
+  if (R.empty()) return HS_OK;
+  // Rebuild R on the audit's stream: key bytes, table, flag byte into staging; then k_table_audit over each table on its own.
+  const size_t per = 24;  // an audit_out of one table (8 + 4 * 3 bytes, 8-aligned): bits[2] is the slot's
+  h2d_stage st;
+  const size_t s_flags = st.add(nullptr, R.size()), s_res = st.add(nullptr, per * R.size());
+  HS_TRY(st.upload(c, A.scratch, A.stream));
+  HS_CUDA(c, cudaMemsetAsync(st.ptr(s_flags), 0, st.total - st.sec[s_flags].off, A.stream));
+  for (size_t k = 0; k < R.size(); k++) {
+    const size_t s = R[k];
+    ge_niels *table = c->keys.atables + s * c->a_table_entries;
+    uint8_t *res = st.ptr(s_res) + per * k;
+    HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * s, c->h_pks.data() + 32 * s, 32, cudaMemcpyHostToDevice, A.stream));
+    HS_TRY(launch_build(c, c->keys.pks + 32 * s, 1, 1, c->cp.wa, c->cp.na, table, st.ptr(s_flags) + k, A.stream));
+    HS_TRY(launch_table_audit(c, A.stream, table, 1, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks + 32 * s, st.ptr(s_flags) + k,
+                              audit_out{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)}));
+  }
+  HS_CUDA(c, cudaEventRecord(A.done, A.stream));  // the key-cache paths, registration and updates wait for it before they rewrite
+  std::vector<uint8_t> h(per * R.size() + R.size());
+  if (committee) g.unlock();
+  cudaError_t e = cudaEventSynchronize(A.done);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), st.ptr(s_flags), R.size(), cudaMemcpyDeviceToHost, A.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data() + R.size(), st.ptr(s_res), per * R.size(), cudaMemcpyDeviceToHost, A.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(A.stream);
+  if (committee) g.lock();
+  if (e != cudaSuccess) return fail(c, HS_ERR_CUDA, "hs_table_repair: rebuild", e);  // R stays out of service
+  // Back into service: each slot of R an update or a registration did not take over meanwhile, whose table passed (a key that does
+  // not decompress has none to prove).  A slot whose table failed stays out of service, and the final audit reports it.
+  for (size_t k = 0; k < R.size(); k++) {
+    const size_t s = R[k];
+    if (committee && (!c->explicit_committee || s >= c->n_keys || c->h_key_live[s] != SLOT_REPAIR)) continue;
+    uint32_t slot_bits;
+    memcpy(&slot_bits, h.data() + R.size() + per * k + 8 + 8, 4);
+    if ((h[k] & 1u) && slot_bits) continue;
+    HS_CUDA(c, cudaMemcpyAsync(c->keys.key_flags + s, h.data() + k, 1, cudaMemcpyHostToDevice, c->stream));
+    if (committee) c->h_key_live[s] = SLOT_LIVE;
+  }
+  if (committee && c->explicit_committee) HS_TRY(publish_hash(c));
+  HS_CUDA(c, cudaStreamSynchronize(c->stream));
+  const bool same = c->key_gen == gen;
+  c->key_gen++;
+  return same ? HS_OK : fail_args(c, "hs_table_repair", changed);
+}
+
+extern "C" int hs_table_repair(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots, uint8_t *out_slot_bits,
+                               uint32_t *out_found, uint32_t *out_failed) {
+  if (!c || !out_found || !out_failed) return fail(c, HS_ERR_ARG, "hs_table_repair: bad argument");
+  const char *changed = "key tables changed during the repair; run it again";
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  audit_run first, last;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    HS_TRY(audit_enqueue_locked(c, "hs_table_repair", expect_pks, expect_live, n_slots, first));
+  }
+  HS_TRY(audit_collect(c, "hs_table_repair", changed, first));
+  const uint32_t found = first.failed();
+  if (found) {
+    {
+      std::unique_lock<std::mutex> g(c->mu);
+      HS_TRY(repair_locked(c, g, first, expect_pks, expect_live, changed));
+      HS_TRY(audit_enqueue_locked(c, "hs_table_repair", expect_pks, expect_live, n_slots, last));
+    }
+    HS_TRY(audit_collect(c, "hs_table_repair", changed, last));
+  }
+  const uint32_t failed = found ? last.failed() : 0u;
+  for (size_t s = 0; s < n_slots && out_slot_bits; s++) out_slot_bits[s] = (uint8_t)first.bits()[2 + s];
+  *out_found = found;
+  *out_failed = failed;
+  return failed ? fail(c, HS_ERR_SELFTEST, audit_message(last.first(), n_slots, last.bits()).c_str()) : HS_OK;
+}
+
+#ifdef HS_TEST_HOOKS
+// Test builds only (never declared in include/hs_crypto.h, never in the product library): XORs one byte of a key slot's comb table
+// (index = slot, byte_offset into its table), of the base-point table (index = entry, byte_offset into it), of a slot's key bytes
+// (index = slot, byte_offset < 32) or a slot's flag byte (index = slot, byte_offset 0), on an idle context.  It cannot reach the hash
+// table, the one stored value that becomes an address, so a poke can change verdicts but cannot make a kernel fault.
+enum { POKE_TABLE = 0, POKE_BASE = 1, POKE_KEY = 2, POKE_FLAG = 3 };
+extern "C" int hs_test_poke(hs_ctx *c, int region, size_t index, size_t byte_offset, uint8_t xor_mask) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> g(c->mu);
+  HS_CUDA(c, cudaSetDevice(c->device));
+  HS_CUDA(c, cudaDeviceSynchronize());
+  const size_t n = c->keys.atables ? c->n_keys : 0;
+  uint8_t *p = nullptr;
+  if (region == POKE_TABLE && index < n && byte_offset < c->a_table_entries * sizeof(ge_niels))
+    p = reinterpret_cast<uint8_t *>(c->keys.atables + index * c->a_table_entries) + byte_offset;
+  else if (region == POKE_BASE && index < comb_table_entries(c->cp.wb) && byte_offset < sizeof(ge_niels))
+    p = reinterpret_cast<uint8_t *>(c->d_btable + index) + byte_offset;
+  else if (region == POKE_KEY && index < n && byte_offset < 32)
+    p = c->keys.pks + 32 * index + byte_offset;
+  else if (region == POKE_FLAG && index < n && byte_offset == 0)
+    p = c->keys.key_flags + index;
+  if (!p) return fail_args(c, "hs_test_poke", "region, index or offset out of range");
+  uint8_t v = 0;
+  HS_CUDA(c, cudaMemcpy(&v, p, 1, cudaMemcpyDeviceToHost));
+  v ^= xor_mask;
+  HS_CUDA(c, cudaMemcpy(p, &v, 1, cudaMemcpyHostToDevice));
+  return HS_OK;
+}
+#endif

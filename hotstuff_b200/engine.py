@@ -136,6 +136,24 @@ class Engine:
             self._check(rc, "hs_table_audit")
         return int(failed.value), bits[:n]
 
+    def table_repair(self, expect=None, live=None):
+        """Repair of what the audit finds (hs_table_repair), from the same authority: expect / live as for table_audit, else the engine's
+        host mirror.  Returns (found, failed, slot_bits): the HS_AUDIT_* classes the first audit found, those the final audit still finds
+        (0 = every finding repaired; last_error names the first one left otherwise) and the first audit's uint8 of HS_AUDIT_* bits per
+        slot, i.e. the slots repaired.  Raises EngineError as table_audit does."""
+        n = self.key_slots if expect is None else _u8(expect, 32).reshape(-1, 32).shape[0]
+        exp = None if expect is None else _u8(expect, 32).reshape(-1, 32)
+        lv = None if live is None else np.ascontiguousarray(live, dtype=np.uint32)
+        if lv is not None and lv.size < (n + 31) // 32:
+            raise ValueError("table_repair: %d live words for %d slots" % (lv.size, n))
+        bits = np.zeros(max(1, n), dtype=np.uint8)
+        found, failed = ctypes.c_uint32(0), ctypes.c_uint32(0)
+        rc = self.lib.hs_table_repair(self.h, _ptr(exp) if n and exp is not None else None, _ptr(lv) if lv is not None and lv.size else None, n,
+                                      _ptr(bits), ctypes.byref(found), ctypes.byref(failed))
+        if rc != HS_ERR_SELFTEST:
+            self._check(rc, "hs_table_repair")
+        return int(found.value), int(failed.value), bits[:n]
+
     @property
     def last_error(self):
         return self.lib.hs_last_error(self.h).decode()

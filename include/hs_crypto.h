@@ -30,7 +30,7 @@ extern "C" {
 #define HS_ERR_CUDA 1
 #define HS_ERR_ARG 2
 #define HS_ERR_NOMEM 3
-#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer; hs_table_audit: a table, slot or lookup entry is wrong */
+#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer; hs_table_audit / hs_table_repair: a table, slot or lookup entry is wrong */
 
 /* verdict selector for the verify entry points */
 #define HS_MODE_STRICT 0u /* Signature::verify semantics  = dalek verify_strict          (crypto/src/lib.rs:200-204) */
@@ -416,6 +416,30 @@ size_t hs_key_slots(const hs_ctx *ctx);
 #define HS_AUDIT_BASE   (1u << 4) /* out_failed only: an entry of the base-point table is not the multiple of B it must hold */
 int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
                    size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_failed);
+
+/* ---- repair of what the audit finds: the failing key slots, lookup entries and the base-point table, rebuilt in place -------------
+ * Runs hs_table_audit, repairs every finding, and proves the result with a complete audit.  The arguments are hs_table_audit's, with
+ * its rules (n_slots == hs_key_slots, expect_pks == NULL for key-cache tables).  What a slot must hold comes from one authority: the
+ * caller's map when expect_pks / expect_live are given, otherwise the engine's host mirror; never from the device bytes.
+ *   - A slot with a KEY, FLAG or TABLE finding that the authority holds live gets the authority's key bytes, a rebuilt comb table and a
+ *     rebuilt flag byte; one it holds dead is taken out of service, as hs_committee_update's removal would.  The device hash table is
+ *     rebuilt from the authority (all a LOOKUP finding needs); a BASE finding rebuilds the base-point table.
+ *   - While a committee's slots are rebuilt, verification goes on: the slots are first taken out of service (their key bytes miss the
+ *     committee and take the generic path with correct verdicts; committee-indexed calls naming them reject), rebuilt and proven by the
+ *     audit's checks on the audit's private lowest-priority stream without the context's mutex, and put back one by one as each passes.
+ *     A slot that fails stays out of service and is reported.  Key-cache slots, and the base-point table, are rebuilt with the mutex
+ *     held and the device drained: verification waits for them.
+ *   - Any finding empties the signature cache and the certificate cache of every verify queue of the context (their completed entries;
+ *     requests in flight complete as they would), so nothing accepted against a wrong table is answered from a cache.
+ *   - *out_found: the classes the first audit found, out_slot_bits (nullable): its per-slot bits (the slots repaired), *out_failed: the
+ *     classes the final audit still finds.  HS_OK iff *out_failed == 0; otherwise HS_ERR_SELFTEST and hs_last_error names the first
+ *     residual finding, worded as hs_table_audit words it.  On a clean context it is one audit and changes nothing.
+ *   - HS_ERR_ARG writes nothing: bad pointers, the audit's argument errors, or key tables that changed during the repair (a
+ *     registration or update from another thread: the slots it left to the repair are back in service; call it again).
+ *   - Repairs and audits of one context run one at a time; `_dev` verify passes must not overlap a repair, as for an audit.  A
+ *     multi-device context is repaired member by member (hs_multi_member) with the same map. */
+int hs_table_repair(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
+                    size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_found, uint32_t *out_failed);
 
 /* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) ------------------- */
 int hs_verify_rec128_dev(hs_ctx *ctx, const void *d_recs, size_t n, uint32_t mode, void *d_bitmap, void *stream);

@@ -72,6 +72,22 @@ class Engine {
     if (slot_bits) *slot_bits = std::move(bits);
     return failed;
   }
+  // Repair of what the audit finds (hs_table_repair), from the same authority: `expect` / `live` as for table_audit, else the engine's
+  // mirror.  Returns the classes the final audit still finds (0: repaired, or nothing was wrong); found receives the classes the first
+  // audit found, slot_bits (nullable) its per-slot bits.  Throws EngineError as table_audit does.
+  uint32_t table_repair(const std::vector<std::array<uint8_t, 32>> *expect = nullptr, const std::vector<uint32_t> *live = nullptr,
+                        uint32_t *found = nullptr, std::vector<uint8_t> *slot_bits = nullptr) const {
+    const size_t n = expect ? expect->size() : key_slots();
+    if (live && live->size() < (n + 31) / 32) throw EngineError("table_repair: live bitmap shorter than the slots");
+    std::vector<uint8_t> bits(n);
+    uint32_t f = 0, failed = 0;
+    const int rc = hs_table_repair(ctx_, expect && n ? expect->front().data() : nullptr, live && !live->empty() ? live->data() : nullptr, n,
+                                   bits.data(), &f, &failed);
+    if (rc != HS_ERR_SELFTEST) check(rc, "hs_table_repair");
+    if (found) *found = f;
+    if (slot_bits) *slot_bits = std::move(bits);
+    return failed;
+  }
   std::string error() const { return hs_last_error(ctx_); }
 
  private:

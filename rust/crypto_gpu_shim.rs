@@ -69,6 +69,7 @@ pub const HS_FRAME_MALFORMED: u8 = 255;
 pub const HS_OK: c_int = 0;
 pub const HS_ERR_ARG: c_int = 2;
 pub const HS_ERR_NOMEM: c_int = 3;
+pub const HS_ERR_SELFTEST: c_int = 4;
 /// Smallest signature count sent to the GPU (below it the dalek path is faster on this hardware; see the header comment).
 pub const GPU_MIN_SIGS: usize = 2;
 /// A Digest call goes to the GPU only with at least this many messages in flight (SHA-512 is sequential inside one message).
@@ -94,6 +95,8 @@ extern "C" {
     fn hs_ingest_consensus_frames(frames: *const u8, off: *const u64, n: usize, info: *mut HsFrameInfo, out: *mut HsIngestOut) -> c_int;
     fn hs_self_test(ctx: *mut HsCtx, key_bits: c_int, recs: *const HsRec128, expect: *const u8, n: usize, out_failed_paths: *mut u32) -> c_int;
     fn hs_table_audit(ctx: *mut HsCtx, expect_pks: *const u8, expect_live: *const u32, n_slots: usize, out_slot_bits: *mut u8, out_failed: *mut u32) -> c_int;
+    fn hs_table_repair(ctx: *mut HsCtx, expect_pks: *const u8, expect_live: *const u32, n_slots: usize, out_slot_bits: *mut u8, out_found: *mut u32,
+                       out_failed: *mut u32) -> c_int;
 }
 
 struct Ctx(*mut HsCtx);
@@ -145,7 +148,9 @@ pub fn self_test() -> Result<(), GpuError> {
 }
 /// Audit of the live key tables (hs_table_audit): every comb-table entry, key slot and lookup entry of the engine against `expected`,
 /// the node's index -> key map (None = a freed index).  `self_test` and `update_committee` call it; a live node may also call it
-/// periodically from a blocking task.  On a finding the GPU is switched off for the life of the process, as after a failed self-test.
+/// periodically from a blocking task.  A finding is repaired once from the same map (hs_table_repair: only the failing slots, lookup
+/// entries or base-point table are rebuilt, and the caches of verified records are emptied); the GPU stays on when the repair's own
+/// final audit is clean, and is switched off for the life of the process, as after a failed self-test, only when the repair fails.
 /// Tables that changed while it ran (a committee change from another task) are audited again.
 pub fn audit_tables(expected: &[Option<[u8; 32]>]) -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
@@ -160,6 +165,12 @@ pub fn audit_tables(expected: &[Option<[u8; 32]>]) -> Result<(), GpuError> {
         if !(rc == HS_ERR_ARG && last_error(c).contains("changed during the audit")) { break; }
     }
     if rc == HS_OK && failed == 0 { return Ok(()); }
+    if rc == HS_ERR_SELFTEST {
+        let mut found = 0u32;
+        rc = unsafe { hs_table_repair(c, if expected.is_empty() { std::ptr::null() } else { pks.as_ptr() }, live.as_ptr(), expected.len(),
+                                      std::ptr::null_mut(), &mut found, &mut failed) };
+        if rc == HS_OK { return Ok(()); }
+    }
     DISABLED.store(true, Ordering::Release);
     Err(GpuError::Engine(format!("table audit failed (status {}, classes {:#x}): {}", rc, failed, last_error(c))))
 }

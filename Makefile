@@ -7,8 +7,8 @@ CSRC := hotstuff_b200/csrc
 all: lib oracle hostemu
 
 lib: hotstuff_b200/libhs_crypto.so
-hotstuff_b200/libhs_crypto.so: $(CSRC)/hs_engine.cu $(CSRC)/hs_ingest.cpp $(wildcard $(CSRC)/*.cuh) include/hs_crypto.h
-	$(NVCC) $(NVCCFLAGS) -o $@ $(CSRC)/hs_engine.cu $(CSRC)/hs_ingest.cpp
+hotstuff_b200/libhs_crypto.so: $(CSRC)/hs_engine.cu $(CSRC)/hs_ingest.cpp $(CSRC)/hs_multi.cpp $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/hs_crypto.h
+	$(NVCC) $(NVCCFLAGS) -o $@ $(CSRC)/hs_engine.cu $(CSRC)/hs_ingest.cpp $(CSRC)/hs_multi.cpp
 
 # test infrastructure only (never linked into the product)
 oracle:

@@ -46,11 +46,11 @@
 #include "../../include/hs_crypto.h"
 #include "hs_args.h"
 #include "hs_selftest_vectors.h"
+#include "key_index.h"
 #include "verify_core.cuh"
 
 #define HS_THREADS 128
 #define HS_FINISH_GROUP 16  // signatures whose Z's share one inversion
-#define HS_NO_KEY 0xffffffffu
 #define HS_LEARN_MAX 8192u  // unknown keys examined per call
 #define HS_LEARN_PER_CALL 1024u  // new tables built per call at most (bounds the latency a flood of one-off keys can add to one call)
 #define HS_CACHE_RESET_MIN_CALLS 64u  // a full cache is cleared at most once per this many verify calls
@@ -123,23 +123,14 @@ __device__ __forceinline__ void warp_load_rec128(uint32_t (&sig_r)[8], uint32_t 
 }
 
 // ------------------------------------------------------------------------------------------------ committee key lookup
-// Open-addressing hash table over the registered keys: slot -> key index (HS_NO_KEY = empty).  Built on the host at
-// registration (hashing only), probed here by one thread per record.
+// Open-addressing hash table over the registered keys: slot -> key index (HS_NO_KEY = empty).  Built on the host by key_index
+// (key_index.h), probed here by one thread per record.
 struct key_table {
   const uint32_t *slots;
   uint32_t mask;  // capacity - 1 (power of two)
   const uint8_t *pks;
   uint32_t n_keys;
 };
-__host__ __device__ inline uint32_t key_hash(const uint32_t *w) {
-  uint32_t h = 0x9e3779b9u;
-  for (int i = 0; i < 8; i++) {
-    h ^= w[i];
-    h *= 0x85ebca6bu;
-    h ^= h >> 15;
-  }
-  return h;
-}
 // The key index the table maps key bytes k to (HS_NO_KEY: none) and, when found, the hash slot holding it.  BOUNDED (hs_table_audit,
 // which must not trust the table it checks): an index at or past T.n_keys is a non-match instead of an address.
 template <bool BOUNDED>
@@ -1454,6 +1445,19 @@ struct key_store {
   dev_mem<ge_niels> atables;
   dev_mem<uint32_t> slots;
 };
+// A key store of n_slots slots with tables at window wa and a hash table of hash_slots entries, empty on `stream`: flags 0, hash slots
+// 0xff (HS_NO_KEY).  Moved into `out` only when every allocation succeeded.
+static cudaError_t make_key_store(key_store &out, size_t n_slots, size_t hash_slots, int wa, cudaStream_t stream) {
+  key_store K;
+  cudaError_t e = alloc(K.pks, n_slots * 32);
+  if (e == cudaSuccess) e = alloc(K.key_flags, n_slots);
+  if (e == cudaSuccess) e = alloc(K.slots, hash_slots * 4);
+  if (e == cudaSuccess) e = alloc(K.atables, n_slots * comb_table_entries(wa) * sizeof(ge_niels));
+  if (e == cudaSuccess) e = cudaMemsetAsync(K.key_flags, 0, n_slots, stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(K.slots, 0xff, hash_slots * 4, stream);
+  if (e == cudaSuccess) out = std::move(K);
+  return e;
+}
 // Key-cache learning: the unknown keys of a pass and their count, their pinned host copies, and the events.  Allocated whole on first use.
 struct learn_bufs {
   dev_mem<uint8_t> keys;
@@ -1496,7 +1500,6 @@ struct hs_ctx {
   // committee
   size_t n_keys = 0;
   key_store keys;
-  uint32_t slot_mask = 0;
   // grow-only device scratch
   dev_buf in[2], digest[2], xyz, meta, vidx, miss, out;
   dev_buf group_digests;  // hs_verify_groups_dev: Digests of the pass's preimages (read by the main kernels only, so one set serves deferred mode)
@@ -1505,8 +1508,8 @@ struct hs_ctx {
   bool explicit_committee = false;   // hs_committee_register was called with keys: the set is fixed, nothing is learned
   bool cache_wanted = true, cache_enabled = true;
   size_t cache_cap = 4096;           // keys
-  std::vector<uint8_t> h_pks;        // host mirrors of d_pks / d_slots (key cache and hs_committee_update)
-  std::vector<uint32_t> h_slots;
+  std::vector<uint8_t> h_pks;        // host mirrors of keys.pks / keys.slots (key cache and hs_committee_update)
+  key_index h_index;
   std::vector<uint8_t> h_key_live;   // explicit committee: SLOT_LIVE, SLOT_REPAIR (live, out of service during hs_table_repair) or 0 = removed (free for reuse)
   size_t table_budget = 0;           // bytes the per-key tables may use (0 = ~62 % of the device)
   size_t key_capacity = 0;           // explicit committee: table slots allocated (>= n_keys; spare slots serve hs_committee_update)
@@ -1548,6 +1551,11 @@ struct hs_ctx {
   std::mutex queues_mu;               // guards queues only (hs_ctx_destroy tears them down without holding `mu`)
   std::vector<hs_queue *> queues;     // verify queues attached to this context
 };
+// The context holds per-key tables: a registered committee's or learned keys'.  Registration, hs_committee_update and learn_process
+// raise n_keys only once `keys` is in place, and cache_release clears both, so n_keys > 0 alone implies the second term.
+static bool has_key_tables(const hs_ctx *c) { return c->n_keys > 0 && c->keys.atables; }
+// A committee is registered: its key set is fixed and nothing is learned.  explicit_committee is set only once the store is in place.
+static bool committee_registered(const hs_ctx *c) { return c->explicit_committee && has_key_tables(c); }
 
 static int fail(hs_ctx *c, int code, const char *what, cudaError_t e = cudaSuccess) {
   if (c) {
@@ -1672,12 +1680,12 @@ static void cache_release(hs_ctx *c) {  // callers have synchronised the device
   c->keys = {};
   c->n_keys = 0;
   c->h_pks.clear();
-  c->h_slots.clear();
+  c->h_index = {};
   c->h_key_live.clear();
   c->key_capacity = 0;
 }
 // lazily allocate the store for cache_cap learned keys (14-bit windows: 14 MB per key, narrower if memory is short)
-static int cache_allocate(hs_ctx *c) {
+static int cache_allocate(hs_ctx *c, cudaStream_t stream) {
   size_t free_b = 0, total_b = 0;
   HS_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
   size_t lim = free_b / 2;
@@ -1692,20 +1700,11 @@ static int cache_allocate(hs_ctx *c) {
     c->cache_enabled = false;  // not enough memory: stay on the generic path
     return HS_OK;
   }
-  uint32_t cap = 16;
-  while (cap < 2 * c->cache_cap) cap <<= 1;
   set_window(c->cp, true, wa);
   c->a_table_entries = comb_table_entries(wa);
-  key_store K;
-  HS_CUDA(c, alloc(K.pks, c->cache_cap * 32));
-  HS_CUDA(c, alloc(K.key_flags, c->cache_cap));
-  HS_CUDA(c, alloc(K.slots, (size_t)cap * 4));
-  HS_CUDA(c, alloc(K.atables, c->cache_cap * sizeof(ge_niels) * c->a_table_entries));
-  HS_CUDA(c, cudaMemset(K.slots, 0xff, (size_t)cap * 4));
+  HS_CUDA(c, make_key_store(c->keys, c->cache_cap, key_index::capacity_for(c->cache_cap), wa, stream));
   c->key_gen++;  // nothing to wait for: the store had no tables, so no audit reads it
-  c->keys = std::move(K);
-  c->slot_mask = cap - 1;
-  c->h_slots.assign(cap, HS_NO_KEY);
+  c->h_index.reset(c->cache_cap);
   c->h_pks.clear();
   return HS_OK;
 }
@@ -1725,8 +1724,8 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
       HS_TRY(audit_fence(c, stream));
       c->n_keys = 0;
       c->h_pks.clear();
-      std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
-      HS_CUDA(c, cudaMemsetAsync(c->keys.slots, 0xff, c->h_slots.size() * 4, stream));
+      c->h_index.clear();
+      HS_CUDA(c, cudaMemsetAsync(c->keys.slots, 0xff, c->h_index.slots.size() * 4, stream));
       c->cache_full = false;
     }
     return HS_OK;
@@ -1734,39 +1733,23 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
   const uint32_t got = *c->learn.h_n < HS_LEARN_MAX ? *c->learn.h_n : HS_LEARN_MAX;
   if (got == 0) return HS_OK;
   if (!c->keys.atables) {
-    HS_TRY(cache_allocate(c));
+    HS_TRY(cache_allocate(c, stream));
     if (!c->cache_enabled) return HS_OK;
   }
   const size_t old_n = c->n_keys;
   size_t n_new = 0;
-  const uint32_t mask = c->slot_mask;
   for (uint32_t t = 0; t < got && old_n + n_new < c->cache_cap && n_new < HS_LEARN_PER_CALL; t++) {
     const uint8_t *key = c->learn.h_keys + 32 * (size_t)t;
-    uint32_t w[8];
-    memcpy(w, key, 32);
-    uint32_t h = key_hash(w) & mask;
-    bool present = false;
-    while (c->h_slots[h] != HS_NO_KEY) {
-      if (memcmp(c->h_pks.data() + 32 * (size_t)c->h_slots[h], key, 32) == 0) {
-        present = true;
-        break;
-      }
-      h = (h + 1) & mask;
-    }
-    if (present) continue;
-    c->h_slots[h] = (uint32_t)(old_n + n_new);
     c->h_pks.insert(c->h_pks.end(), key, key + 32);
-    n_new++;
+    if (c->h_index.insert_absent(c->h_pks.data(), (uint32_t)(old_n + n_new))) n_new++;
+    else c->h_pks.resize(32 * (old_n + n_new));  // already learned
   }
   if (n_new == 0) return HS_OK;
   HS_TRY(audit_fence(c, stream));
   HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + old_n * 32, c->h_pks.data() + old_n * 32, n_new * 32, cudaMemcpyHostToDevice, stream));
-  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, stream));
-  size_t threads = n_new * (size_t)c->cp.na * ((1u << (c->cp.wa - 1)) / HS_BUILD_BLOCK);
-  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(c->keys.pks + old_n * 32, n_new, 1, c->cp.wa, c->cp.na,
-                                                                c->keys.atables + old_n * c->a_table_entries, c->keys.key_flags + old_n);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_index.slots.data(), c->h_index.slots.size() * 4, cudaMemcpyHostToDevice, stream));
+  HS_TRY(launch_build(c, c->keys.pks + old_n * 32, n_new, 1, c->cp.wa, c->cp.na, c->keys.atables + old_n * c->a_table_entries,
+                      c->keys.key_flags + old_n, stream));
   // (no synchronisation: copies from pageable memory return once the source is staged, so the host vectors may change afterwards)
   HS_CUDA(c, cudaEventRecord(c->learn.ev_tables, stream));  // passes on OTHER streams (host entry points vs a _dev caller's stream) wait for the build
   c->n_keys = old_n + n_new;
@@ -1823,9 +1806,15 @@ struct pass_tables {
   key_table T;
   comb_params cp;
 };
-static pass_tables ctx_tables(const hs_ctx *c) {
-  return pass_tables{{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries},
-                     {c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)c->n_keys}, c->cp};
+// The view of key store S whose first n_keys slots hold tables of `entries` entries at window cp.wa, found through `index`.
+static pass_tables store_tables(const key_store &S, const key_index &index, size_t n_keys, size_t entries, const comb_params &cp) {
+  return pass_tables{{S.pks, S.key_flags, (uint32_t)n_keys, S.atables, entries}, {S.slots, index.mask, S.pks, (uint32_t)n_keys}, cp};
+}
+static pass_tables ctx_tables(const hs_ctx *c) { return store_tables(c->keys, c->h_index, c->n_keys, c->a_table_entries, c->cp); }
+// A pass on `stream` reads the key cache's tables only after their latest build, which learn_process may have enqueued on another stream.
+static int wait_key_cache_build(hs_ctx *c, cudaStream_t stream) {
+  if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(stream, c->learn.ev_tables, 0));
+  return HS_OK;
 }
 // The main phase on `stream`: with committee tables, [k_key_lookup, then k_verify_main<false> over the misses on S.side] beside
 // k_verify_main<true>; without, k_verify_main<false> over every record.  after_lookup(have_lookup) runs where run_verify collects
@@ -1898,9 +1887,9 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     }
     return HS_OK;
   }
-  if (indexed && (!c->explicit_committee || c->n_keys == 0)) return fail(c, HS_ERR_ARG, "committee-indexed verify without a registered committee");
+  if (indexed && !committee_registered(c)) return fail(c, HS_ERR_ARG, "committee-indexed verify without a registered committee");
   if (!indexed) HS_TRY(learn_process(c, stream));
-  if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(stream, c->learn.ev_tables, 0));
+  HS_TRY(wait_key_cache_build(c, stream));
   const bool defer = c->deferred && stream != c->stream;  // host-pointer entry points (internal stream) always complete in stream order
   dev_buf &XYZ = (defer && c->flip) ? c->xyz2 : c->xyz, &META = (defer && c->flip) ? c->meta2 : c->meta;
   const int set = defer ? c->flip : 0;
@@ -1910,7 +1899,7 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   }
   HS_TRY(ensure(c, XYZ, n * 3 * sizeof(fe)));
   HS_TRY(ensure(c, META, n));
-  const bool committee = c->n_keys > 0 && (indexed || L.pk);
+  const bool committee = has_key_tables(c) && (indexed || L.pk);
   if (!committee && !L.pk) return fail(c, HS_ERR_ARG, "verify without keys");
   if (committee && !indexed) {
     HS_TRY(ensure(c, c->vidx, n * 4));
@@ -1942,19 +1931,9 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
 // ---- latency path (host side)
 // key bytes -> table index through the host mirror of the device hash table (registered committee or learned cache)
 static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
-  if (c->n_keys == 0 || c->h_slots.empty()) return HS_NO_KEY;
-  uint32_t w[8];
-  memcpy(w, key, 32);
-  uint32_t h = key_hash(w) & c->slot_mask;
-  for (uint32_t probe = 0; probe <= c->slot_mask; probe++) {
-    const uint32_t idx = c->h_slots[h];
-    if (idx == HS_NO_KEY) return HS_NO_KEY;
-    if (idx < c->n_keys && memcmp(c->h_pks.data() + 32 * (size_t)idx, key, 32) == 0) return idx;
-    h = (h + 1) & c->slot_mask;
-  }
-  return HS_NO_KEY;
+  return c->h_index.find(c->h_pks.data(), key, [c](uint32_t idx) { return idx < c->n_keys; });
 }
-static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && c->n_keys > 0 && c->keys.atables; }
+static bool small_eligible(const hs_ctx *c, size_t n) { return c->small_enabled && n >= 1 && n <= HS_SMALL_MAX && has_key_tables(c); }
 // Record i of a latency-path call: its signature, its 32-byte message and its key's table index.
 struct small_src {
   const uint8_t *sig, *msg;
@@ -1981,10 +1960,9 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap) {
     c->small.in.h[i].req_n = (uint32_t)n;
   }
   const uint32_t seq = ++c->small_seq ? c->small_seq : ++c->small_seq;  // never 0
-  committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
-  if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->learn.ev_tables, 0));
-  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(c->small.in.d, 0, HS_SMALL_MAX - 1, c->d_btable, C, c->cp, c->small.out.d, c->small.counter,
-                                                           c->small.done.d, seq, sig_cache_dev{});
+  HS_TRY(wait_key_cache_build(c, c->stream));
+  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(c->small.in.d, 0, HS_SMALL_MAX - 1, c->d_btable, ctx_tables(c).C, c->cp, c->small.out.d,
+                                                           c->small.counter, c->small.done.d, seq, sig_cache_dev{});
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   volatile uint32_t *done = c->small.done.h;
@@ -2365,7 +2343,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   cudaError_t e = cudaSuccess;
   {
     std::lock_guard<std::mutex> g(c->mu);
-    const bool committee = c->explicit_committee && c->n_keys > 0 && c->keys.atables && c->small_enabled;
+    const bool committee = committee_registered(c) && c->small_enabled;
     const bool gen = q->gen_on.load();  // hs_queue_generic writes it under c->mu
     if (!gen) {  // turned off with generic requests still waiting: they take the slow path, ahead of this range's
       for (uint64_t p : q->gpend) q->reqs[p & q->mask].gen = false;
@@ -2409,7 +2387,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       p += r.n;
     }
     if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi, false});
-    committee_tables C{c->keys.pks, c->keys.key_flags, (uint32_t)c->n_keys, c->keys.atables, c->a_table_entries};
+    const committee_tables C = ctx_tables(c).C;
     ok.assign(runs.size(), 0);
     for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {  // pass 0: the small launches, pass 1: the bulk ones
       for (size_t k = 0; k < runs.size(); k++) {
@@ -2712,7 +2690,7 @@ static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
   in_layout L{m + r.o_sig, 64, m + r.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(q->lane.dig.get()), 32, reinterpret_cast<const uint32_t *>(m + r.o_mi),
               nullptr, 32, 0};
   // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
-  const bool committee = c->explicit_committee && c->n_keys > 0 && c->keys.atables;
+  const bool committee = committee_registered(c);
   const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
   HS_TRY(launch_main(c, L, r.n, committee, false, ctx_tables(c), S, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
@@ -2952,7 +2930,7 @@ void hs_ctx_destroy(hs_ctx *c) {
 const char *hs_last_error(const hs_ctx *c) { return c ? c->err.c_str() : "null context"; }
 size_t hs_cached_keys(const hs_ctx *c) { return (c && !c->explicit_committee) ? c->n_keys : 0; }
 void hs_window_bits(const hs_ctx *c, int *key_bits, int *base_bits) {
-  if (key_bits) *key_bits = (c && c->n_keys) ? c->cp.wa : 0;
+  if (key_bits) *key_bits = (c && has_key_tables(c)) ? c->cp.wa : 0;
   if (base_bits) *base_bits = c ? c->cp.wb : 0;
 }
 uint64_t hs_kernel_launches(const hs_ctx *c) { return c ? c->launches.load() : 0; }
@@ -3036,46 +3014,23 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
   c->explicit_committee = false;   // set only once the new tables are complete: a failed registration leaves NO committee
   c->cache_enabled = c->cache_wanted;
   if (N == 0) return HS_OK;        // clears the committee and hands key handling back to the cache (if enabled)
-  // host-side hash table (hashing only; first occurrence of a duplicated key wins)
-  uint32_t cap = 16;
-  std::vector<uint32_t> slots;
   size_t capk = 0;
   int wa = 8;
   HS_TRY(committee_geometry(c, N, capk, wa));
-  while (cap < 2 * capk) cap <<= 1;
-  slots.clear();
-  slots.assign(cap, HS_NO_KEY);
-  for (size_t i = 0; i < N; i++) {
-    uint32_t w[8];
-    memcpy(w, pks + 32 * i, 32);
-    uint32_t h = key_hash(w) & (cap - 1);
-    bool dup = false;
-    while (slots[h] != HS_NO_KEY) {
-      if (memcmp(pks + 32 * (size_t)slots[h], pks + 32 * i, 32) == 0) {
-        dup = true;
-        break;
-      }
-      h = (h + 1) & (cap - 1);
-    }
-    if (!dup) slots[h] = (uint32_t)i;
-  }
+  key_index index;
+  index.reset(capk);
+  index.build(pks, N, [](size_t) { return true; });
   if (sc_ndigits_rt(wa) + c->cp.nb > HS_MAX_DIGITS) return fail(c, HS_ERR_ARG, "window combination exceeds HS_MAX_DIGITS");
-  key_store K;  // the old tables were released above
-  cudaError_t e = alloc(K.pks, capk * 32);
-  if (e == cudaSuccess) e = alloc(K.key_flags, capk);
-  if (e == cudaSuccess) e = cudaMemset(K.key_flags, 0, capk);
-  if (e == cudaSuccess) e = alloc(K.slots, (size_t)cap * 4);
-  if (e == cudaSuccess) e = alloc(K.atables, capk * sizeof(ge_niels) * comb_table_entries(wa));
+  cudaError_t e = make_key_store(c->keys, capk, index.slots.size(), wa, c->stream);  // the old tables were released above
   if (e != cudaSuccess) {
     cudaGetLastError();
     return fail(c, HS_ERR_NOMEM, "committee tables do not fit in device memory", e);
   }
-  c->keys = std::move(K);
   set_window(c->cp, true, wa);
   c->a_table_entries = comb_table_entries(wa);
   int rc = HS_OK;
   e = cudaMemcpyAsync(c->keys.pks, pks, N * 32, cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(c->keys.slots, slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(c->keys.slots, index.slots.data(), index.slots.size() * 4, cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags, c->stream);
   if (e == cudaSuccess && rc == HS_OK) e = cudaStreamSynchronize(c->stream);
   std::vector<uint8_t> fl(N);
@@ -3084,12 +3039,11 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
     cache_release(c);
     return rc != HS_OK ? rc : fail(c, HS_ERR_CUDA, "committee registration", e);
   }
-  c->slot_mask = cap - 1;
   c->n_keys = N;
   c->key_capacity = capk;
   c->explicit_committee = true;
   c->h_pks.assign(pks, pks + N * 32);  // host mirror: hs_committee_update edits the set incrementally
-  c->h_slots = slots;
+  c->h_index = std::move(index);
   c->h_key_live.assign(N, 1);
   if (out_valid_bitmap) {
     for (size_t w = 0; w < (N + 31) / 32; w++) out_valid_bitmap[w] = 0;
@@ -3108,23 +3062,8 @@ int hs_committee_register(hs_ctx *c, const uint8_t *pks, size_t N, uint32_t *out
 // the slots in service: every learned key of the key cache, a committee's live slots but those under repair (SLOT_REPAIR).  Publishes
 // it on the context's stream and waits, so that every launch enqueued afterwards, on any stream, probes the new table.
 static int publish_hash(hs_ctx *c) {
-  std::fill(c->h_slots.begin(), c->h_slots.end(), HS_NO_KEY);
-  for (size_t i = 0; i < c->n_keys; i++) {
-    if (c->explicit_committee && c->h_key_live[i] != SLOT_LIVE) continue;
-    uint32_t w[8];
-    memcpy(w, c->h_pks.data() + 32 * i, 32);
-    uint32_t h = key_hash(w) & c->slot_mask;
-    bool dup = false;
-    while (c->h_slots[h] != HS_NO_KEY) {
-      if (memcmp(c->h_pks.data() + 32 * (size_t)c->h_slots[h], c->h_pks.data() + 32 * i, 32) == 0) {
-        dup = true;
-        break;
-      }
-      h = (h + 1) & c->slot_mask;
-    }
-    if (!dup) c->h_slots[h] = (uint32_t)i;
-  }
-  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_slots.data(), c->h_slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
+  c->h_index.build(c->h_pks.data(), c->n_keys, [c](size_t i) { return !c->explicit_committee || c->h_key_live[i] == SLOT_LIVE; });
+  HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_index.slots.data(), c->h_index.slots.size() * 4, cudaMemcpyHostToDevice, c->stream));
   HS_CUDA(c, cudaStreamSynchronize(c->stream));
   return HS_OK;
 }
@@ -3145,24 +3084,14 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
     c->h_key_live[remove_idx[i]] = 0;
     HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + remove_idx[i], 0, 1, c->stream));
   }
-  auto find = [&](const uint8_t *key) -> uint32_t {
-    uint32_t w[8];
-    memcpy(w, key, 32);
-    uint32_t h = key_hash(w) & c->slot_mask;
-    while (c->h_slots[h] != HS_NO_KEY) {
-      const uint32_t idx = c->h_slots[h];
-      if (c->h_key_live[idx] && memcmp(c->h_pks.data() + 32 * (size_t)idx, key, 32) == 0) return idx;
-      h = (h + 1) & c->slot_mask;
-    }
-    return HS_NO_KEY;
-  };
+  // The published table plus this call's additions, so that the same key twice in one call takes one slot.  A failed update leaves
+  // the context's index as published.
+  key_index index = c->h_index;
+  auto live = [c](uint32_t idx) { return c->h_key_live[idx] != 0; };
   size_t next_free = 0;
-  std::vector<uint32_t> added;
   for (size_t i = 0; i < n_add; i++) {
     const uint8_t *key = add_pks + 32 * i;
-    uint32_t idx = find(key);
-    for (uint32_t a : added)  // the same key twice in one call
-      if (idx == HS_NO_KEY && memcmp(c->h_pks.data() + 32 * (size_t)a, key, 32) == 0) idx = a;
+    uint32_t idx = index.find(c->h_pks.data(), key, live);
     if (idx == HS_NO_KEY) {
       while (next_free < c->n_keys && c->h_key_live[next_free]) next_free++;
       if (next_free < c->n_keys) idx = (uint32_t)next_free;
@@ -3173,10 +3102,10 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
       } else return fail(c, HS_ERR_NOMEM, "hs_committee_update: no free table slot (re-register the committee)");
       memcpy(c->h_pks.data() + 32 * (size_t)idx, key, 32);
       c->h_key_live[idx] = 1;
+      index.insert_absent(c->h_pks.data(), idx, live);
       HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)idx, key, 32, cudaMemcpyHostToDevice, c->stream));
       HS_TRY(launch_build(c, c->keys.pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->keys.atables + (size_t)idx * c->a_table_entries,
                           c->keys.key_flags + idx, c->stream));
-      added.push_back(idx);
     }
     out_add_idx[i] = idx;
   }
@@ -3306,7 +3235,7 @@ int hs_verify_groups_dev(hs_ctx *c, const void *d_pre, const void *d_off, size_t
   if (!c || (n_items && (!d_pre || !d_off || !d_sig || (!d_pk && !d_vidx) || !d_msg_idx || !d_item_bitmap)))
     return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: bad argument");
   if (n_items && n_msgs == 0) return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: items without preimages");
-  if (n_items && !d_pk && (!c->explicit_committee || c->n_keys == 0))
+  if (n_items && !d_pk && !committee_registered(c))
     return fail(c, HS_ERR_ARG, "hs_verify_groups_dev: committee-indexed items without a registered committee");
   HS_CUDA(c, cudaSetDevice(c->device));
   if (n_items == 0) return run_verify(c, in_layout{}, 0, HS_MODE_STRICT, nullptr, (cudaStream_t)stream, false);  // an armed route still signals
@@ -3589,7 +3518,7 @@ int hs_verify_committee(hs_ctx *c, const uint32_t *vidx, const uint8_t *sig, con
       if (midx[i] >= n_msgs) return fail(c, HS_ERR_ARG, "hs_verify_committee: msg_idx out of range");
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
-  if (small_eligible(c, n) && c->explicit_committee) {  // latency path: the indices as given (the kernel rejects one without a key)
+  if (small_eligible(c, n) && committee_registered(c)) {  // latency path: the indices as given (the kernel rejects one without a key)
     small_stage(c, n, [&](size_t i) { return small_src{sig + 64 * i, digests + 32 * (size_t)(midx ? midx[i] : 0), vidx[i]}; });
     return run_small(c, n, mode, out_bitmap);
   }
@@ -3650,7 +3579,7 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
   }
   HS_TRY(ensure(c, c->xyz, chunk_cap * 3 * sizeof(fe)));
   HS_TRY(ensure(c, c->meta, chunk_cap));
-  if (!vidx && c->n_keys) {
+  if (!vidx && has_key_tables(c)) {
     HS_TRY(ensure(c, c->vidx, chunk_cap * 4));
     HS_TRY(ensure(c, c->miss, chunk_cap * 4));
   }
@@ -4382,39 +4311,24 @@ static int st_digest_and_sign_paths(hs_ctx *c, const comb_params &cp, cudaStream
 struct st_keys {
   std::vector<uint8_t> pks;  // distinct keys, 32 bytes each, in first-seen order
   std::unordered_map<std::string, uint32_t> index;
-  std::vector<uint32_t> slots;
+  key_index h_index;
   key_store K;
   uint32_t idx(const uint8_t *pk) const { return index.at(std::string((const char *)pk, 32)); }
 };
 static int st_build_keys(hs_ctx *c, const st_set &T, const comb_params &cp, st_keys &KS, pass_tables &K, cudaStream_t st) {
-  const size_t n = KS.pks.size() / 32, entries = comb_table_entries(cp.wa);
-  uint32_t cap = 16;
-  while (cap < 2 * n) cap <<= 1;
+  const size_t n = KS.pks.size() / 32;
   const uint32_t foreign = T.r32.empty() ? HS_NO_KEY : KS.idx(T.r32[0].pk);
-  KS.slots.assign(cap, HS_NO_KEY);
-  for (uint32_t i = 0; i < n; i++) {
-    if (i == foreign) continue;
-    uint32_t w[8];
-    memcpy(w, KS.pks.data() + 32 * (size_t)i, 32);
-    uint32_t h = key_hash(w) & (cap - 1);
-    while (KS.slots[h] != HS_NO_KEY) h = (h + 1) & (cap - 1);
-    KS.slots[h] = i;
-  }
-  cudaError_t e = alloc(KS.K.pks, n * 32);
-  if (e == cudaSuccess) e = alloc(KS.K.key_flags, n);
-  if (e == cudaSuccess) e = alloc(KS.K.slots, (size_t)cap * 4);
-  if (e == cudaSuccess) e = alloc(KS.K.atables, n * entries * sizeof(ge_niels));
+  KS.h_index.reset(n);
+  KS.h_index.build(KS.pks.data(), n, [foreign](size_t i) { return i != foreign; });
+  const cudaError_t e = make_key_store(KS.K, n, KS.h_index.slots.size(), cp.wa, st);
   if (e != cudaSuccess) {
     cudaGetLastError();
     return fail(c, HS_ERR_NOMEM, "hs_self_test: the scratch key tables do not fit in device memory", e);
   }
   HS_CUDA(c, cudaMemcpyAsync(KS.K.pks, KS.pks.data(), n * 32, cudaMemcpyHostToDevice, st));
-  HS_CUDA(c, cudaMemcpyAsync(KS.K.slots, KS.slots.data(), (size_t)cap * 4, cudaMemcpyHostToDevice, st));
-  const size_t threads = n * (size_t)cp.na * ((1u << (cp.wa - 1)) / HS_BUILD_BLOCK);
-  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, st>>>(KS.K.pks, n, 1, cp.wa, cp.na, KS.K.atables, KS.K.key_flags);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
-  K = pass_tables{{KS.K.pks, KS.K.key_flags, (uint32_t)n, KS.K.atables, entries}, {KS.K.slots, cap - 1, KS.K.pks, (uint32_t)n}, cp};
+  HS_CUDA(c, cudaMemcpyAsync(KS.K.slots, KS.h_index.slots.data(), KS.h_index.slots.size() * 4, cudaMemcpyHostToDevice, st));
+  HS_TRY(launch_build(c, KS.K.pks, n, 1, cp.wa, cp.na, KS.K.atables, KS.K.key_flags, st));
+  K = store_tables(KS.K, KS.h_index, n, comb_table_entries(cp.wa), cp);
   return HS_OK;
 }
 
@@ -4657,7 +4571,7 @@ extern "C" int hs_self_test(hs_ctx *c, int key_bits, const hs_rec128 *recs, cons
 }
 
 // ---- audit of the live key tables (hs_table_audit)
-extern "C" size_t hs_key_slots(const hs_ctx *c) { return (c && c->keys.atables) ? c->n_keys : 0; }
+extern "C" size_t hs_key_slots(const hs_ctx *c) { return (c && has_key_tables(c)) ? c->n_keys : 0; }
 
 // The message for the first finding: audit_key() decoded, with the slot's classes for a finding about the slot itself.
 static std::string audit_message(uint64_t first, size_t n_slots, const uint32_t *bits) {
@@ -4711,7 +4625,7 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
                                 audit_run &r) {
   audit_state &A = c->audit;
   HS_CUDA(c, cudaSetDevice(c->device));
-  const size_t n = c->keys.atables ? c->n_keys : 0;
+  const size_t n = has_key_tables(c) ? c->n_keys : 0;
   if (n_slots != n) return fail_args(c, entry, ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
   if (expect_pks && n && !c->explicit_committee) return fail_args(c, entry, "key-cache tables are audited with expect_pks == NULL");
   if (!A.stream) {
@@ -4733,8 +4647,8 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
   HS_CUDA(c, cudaMemsetAsync(res + 8, 0, res_bytes - 8, A.stream));
   const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
   if (n) {
-    const key_table T{c->keys.slots, c->slot_mask, c->keys.pks, (uint32_t)n};
-    k_slot_audit<<<blocks_for(n + (size_t)c->slot_mask + 1, 256), 256, 0, A.stream>>>(
+    const key_table T = ctx_tables(c).T;
+    k_slot_audit<<<blocks_for(n + (size_t)T.mask + 1, 256), 256, 0, A.stream>>>(
         T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
         expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
     c->launches++;
@@ -4903,7 +4817,7 @@ extern "C" int hs_test_poke(hs_ctx *c, int region, size_t index, size_t byte_off
   std::lock_guard<std::mutex> g(c->mu);
   HS_CUDA(c, cudaSetDevice(c->device));
   HS_CUDA(c, cudaDeviceSynchronize());
-  const size_t n = c->keys.atables ? c->n_keys : 0;
+  const size_t n = has_key_tables(c) ? c->n_keys : 0;
   uint8_t *p = nullptr;
   if (region == POKE_TABLE && index < n && byte_offset < c->a_table_entries * sizeof(ge_niels))
     p = reinterpret_cast<uint8_t *>(c->keys.atables + index * c->a_table_entries) + byte_offset;

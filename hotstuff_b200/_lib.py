@@ -79,6 +79,7 @@ SIGNATURES = {
     "hs_key_slots": (c_size_t, [c_void_p]),
     "hs_table_audit": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32)]),
     "hs_table_repair": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32), ctypes.POINTER(c_u32)]),
+    "hs_explain_rec128": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "hs_multi_create": (c_int, [ctypes.POINTER(c_void_p), c_void_p, c_size_t, c_u32]),
     "hs_multi_destroy": (None, [c_void_p]),
     "hs_multi_last_error": (ctypes.c_char_p, [c_void_p]),

@@ -1139,6 +1139,23 @@ __global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_ni
   if (!ok) audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
 }
 
+// ------------------------------------------------------------------------------------------------ explanation of a verdict
+// hs_explain_rec128: a thread per packed hs_rec128 record, grid-stride, one HS_WHY_* byte out per record.  It reads the records and
+// nothing else (explain_record is table-free), and loads them with its own plain per-thread loads: it runs on rejected records only.
+__global__ void __launch_bounds__(HS_THREADS) k_explain(const uint8_t *__restrict__ recs, size_t n, uint8_t *__restrict__ out_why) {
+  for (size_t i = (size_t)blockIdx.x * HS_THREADS + threadIdx.x; i < n; i += (size_t)gridDim.x * HS_THREADS) {
+    const uint8_t *r = recs + i * 128;
+    uint32_t R[8], S[8], A[8], M[8], h[16];
+    load32(R, r);
+    load32(S, r + 32);
+    load32(A, r + 64);
+    load32(M, r + 96);
+    sha512_ram32(h, R, A, M);
+    ge_cached tab[9];
+    out_why[i] = (uint8_t)explain_record(R, S, A, h, tab);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ Digest kernels
 __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restrict__ data, const uint64_t *__restrict__ off, uint64_t fixed_len,
                                                           size_t n, uint32_t *__restrict__ out) {
@@ -4804,6 +4821,24 @@ extern "C" int hs_table_repair(hs_ctx *c, const uint8_t *expect_pks, const uint3
   *out_found = found;
   *out_failed = failed;
   return failed ? fail(c, HS_ERR_SELFTEST, audit_message(last.first(), n_slots, last.bits()).c_str()) : HS_OK;
+}
+
+// ---- explanation of a verdict (hs_explain_rec128): k_explain over the staged records, on the context's stream.  No context table is
+// read and no key-cache, queue or committee state is touched, so only the staging and result buffers need the mutex.
+extern "C" int hs_explain_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint8_t *out_why) {
+  if (!c || (n && (!recs || !out_why))) return fail(c, HS_ERR_ARG, "hs_explain_rec128: bad argument");
+  if (n == 0) return HS_OK;
+  std::lock_guard<std::mutex> g(c->mu);
+  HS_CUDA(c, cudaSetDevice(c->device));
+  h2d_stage S;
+  const size_t s_recs = S.add(recs, n * sizeof(hs_rec128));
+  HS_TRY(ensure(c, c->out, n));
+  HS_TRY(S.upload(c, c->in[0], c->stream));
+  const unsigned grid = (unsigned)std::min<size_t>(blocks_for(n), (size_t)c->n_sms * 4);
+  k_explain<<<grid, HS_THREADS, 0, c->stream>>>(S.ptr(s_recs), n, (uint8_t *)c->out.p.get());
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return readback(c, {{out_why, c->out.p.get(), n}});
 }
 
 #ifdef HS_TEST_HOOKS

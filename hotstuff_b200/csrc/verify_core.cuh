@@ -20,6 +20,7 @@
 //   Every lane executes the same operation sequence (identity entry for digit 0), so warps never diverge.
 #pragma once
 #include <cstdint>
+#include "../../include/hs_crypto.h"  // HS_WHY_*: the per-check bits of explain_record are the C ABI's
 #include "fe.cuh"
 #include "ge.cuh"
 #include "sc.cuh"
@@ -469,6 +470,42 @@ HS_HD uint32_t audit_anchor(const ge_niels &one, const ge_ext &P) { return audit
 // The first finding of an audit, as one 64-bit key whose minimum is the first in (slot, window, entry) order: code 0 = the base table,
 // s + 1 = key slot s; window field 0 = a finding about the slot itself (key bytes, flag, lookup), i + 1 = window i of its table.
 HS_HD uint64_t audit_key(uint64_t code, uint32_t wfield, uint32_t entry) { return (code << 32) | ((uint64_t)wfield << 26) | entry; }
+
+// ---- explanation of a verdict (hs_explain_rec128): every check of the decision procedure above as its own HS_WHY_* bit, evaluated
+// independently (no "first failure"), with no table of any kind and without the fast paths' shortcuts: [S]B and [k](-A) both by the
+// radix-16 window with B as an ordinary variable point (never btable or a comb), the equation as a projective compare with R
+// decompressed (never ge_matches_encoding), and small order by three doublings of the decompressed point (never
+// ge_enc_is_small_order, the encoding list the fast paths use), so the two small-order methods check each other.
+//   strict verdict   <=> why == 0
+//   batch-eq verdict <=> (why & ~(HS_WHY_A_SMALL | HS_WHY_R_SMALL)) == 0
+// [8]P == identity, for a decompressed (affine) P: (X : Y : Z) == (0 : 1 : 1).
+HS_HD uint32_t explain_is_small_order(const ge_ext &P) {
+  ge_ext t;
+  ge_dbl(t, P);
+  ge_dbl(t, t);
+  ge_dbl(t, t);
+  return fe_is_zero(t.X) & fe_eq(t.Y, t.Z);
+}
+// h = SHA-512(R || A || M) as 16 words (k = h mod l).  tab: 9 cached entries of thread-private scratch, as ge_scalarmult_window4 takes.
+HS_HD uint32_t explain_record(const uint32_t (&R)[8], const uint32_t (&S)[8], const uint32_t (&A)[8], const uint32_t (&h)[16], ge_cached *tab) {
+  uint32_t why = sc_is_canonical(S) ? 0u : HS_WHY_S_NONCANONICAL;
+  ge_ext Apt, Rpt;
+  if (!ge_decompress(Apt, A)) why |= HS_WHY_A_INVALID;
+  else if (explain_is_small_order(Apt)) why |= HS_WHY_A_SMALL;
+  if (!ge_decompress(Rpt, R)) why |= HS_WHY_R_INVALID;
+  else if (explain_is_small_order(Rpt)) why |= HS_WHY_R_SMALL;
+  if (why & (HS_WHY_S_NONCANONICAL | HS_WHY_A_INVALID | HS_WHY_R_INVALID)) return why;
+  uint32_t k[8];
+  sc_reduce512(k, h);
+  ge_ext negA, B, kA, sB, Rp;
+  ge_neg(negA, Apt);
+  ge_scalarmult_window4(kA, negA, k, tab);
+  ge_basepoint(B);
+  ge_scalarmult_window4(sB, B, S, tab);
+  ge_add_ext(Rp, sB, kA);
+  if (!ge_proj_equals_affine(Rp.X, Rp.Y, Rp.Z, Rpt.X, Rpt.Y)) why |= HS_WHY_EQUATION;
+  return why;
+}
 
 // ---- signing (load generation only: SURVEY §8f.4 — the reference node signs on the CPU, one signature per request,
 // crypto/src/lib.rs:185-191; this exists to synthesise 2^20-scale benchmark / test inputs in milliseconds).  RFC 8032 §5.1.6:

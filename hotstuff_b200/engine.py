@@ -13,6 +13,13 @@ from . import _lib
 MODE_STRICT = 0    # Signature::verify      (crypto/src/lib.rs:200-204)
 MODE_BATCH_EQ = 1  # Signature::verify_batch (crypto/src/lib.rs:206-219), per-signature condition
 HS_ERR_SELFTEST = 4  # hs_self_test: a path gave a wrong answer
+# hs_explain_rec128: one bit per check of the decision procedure a record fails (include/hs_crypto.h)
+WHY_S_NONCANONICAL = 1  # S >= l
+WHY_A_INVALID = 2       # A does not decompress
+WHY_R_INVALID = 4       # R does not decompress
+WHY_A_SMALL = 8         # [8]A is the identity
+WHY_R_SMALL = 16        # [8]R is the identity
+WHY_EQUATION = 32       # S, A, R parse and [S]B + [k](-A) != R
 
 
 class EngineError(RuntimeError):
@@ -153,6 +160,15 @@ class Engine:
         if rc != HS_ERR_SELFTEST:
             self._check(rc, "hs_table_repair")
         return int(found.value), int(failed.value), bits[:n]
+
+    def explain(self, recs):
+        """Table-free re-check of (n,128) uint8 records (hs_explain_rec128) -> uint8[n] of WHY_* bits, one per failed check.  The strict
+        verdict is 1 iff the byte is 0; the batch-eq verdict is 1 iff it has no bit outside WHY_A_SMALL | WHY_R_SMALL."""
+        recs = _u8(recs, 128).reshape(-1, 128)
+        n = recs.shape[0]
+        why = np.zeros(max(1, n), dtype=np.uint8)
+        self._check(self.lib.hs_explain_rec128(self.h, _ptr(recs), n, _ptr(why)), "hs_explain_rec128")
+        return why[:n]
 
     @property
     def last_error(self):

@@ -441,6 +441,36 @@ int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 3
 int hs_table_repair(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
                     size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_found, uint32_t *out_failed);
 
+/* ---- explanation of a verdict: a table-free re-check that names every check a record fails ------------------------------------
+ * A verify call answers 0 for malformed bytes, a small-order key or R, a signature over another message and a false reject by the
+ * engine alike.  This call re-checks records by a separate method and reports each check of the decision procedure as its own bit
+ * (out_why[i], one byte per record).  Every bit is evaluated on its own; there is no "first failure":
+ *   HS_WHY_S_NONCANONICAL  S >= l
+ *   HS_WHY_A_INVALID       A does not decompress (dalek's tolerant rules)
+ *   HS_WHY_R_INVALID       R does not decompress
+ *   HS_WHY_A_SMALL         A decompresses and [8]A is the identity
+ *   HS_WHY_R_SMALL         R decompresses and [8]R is the identity
+ *   HS_WHY_EQUATION        S, A and R all parse and [S]B + [k](-A) != R as points (cofactorless, k = SHA-512(R || A || msg) mod l);
+ *                          clear when any of them does not parse
+ * The mask restates both verdicts:  strict verdict 1  <=>  why == 0;
+ *                                   batch-eq verdict 1  <=>  (why & ~(HS_WHY_A_SMALL | HS_WHY_R_SMALL)) == 0.
+ *   - Use: explain the rejected record of a rejected message (log the mask with it).  A record the verify paths rejected but this call
+ *     finds valid in its mode is an engine fault, not a bad signature: audit and repair the tables (hs_table_repair) and answer that
+ *     message on another verifier.
+ *   - Method: one thread per record computes [S]B and [k](-A) with a radix-16 window on the points themselves (B included), and decides
+ *     small order by three doublings.  It reads no context table: no per-key comb table, key slot, key flag or hash table, and not the
+ *     base-point table.  So it does not depend on the committee, the table geometry, the key cache, or an audit or repair in progress.
+ *     It is slower than a verify and meant for the rare rejected record, not for every record.
+ *   - Isolation: it does not teach the key cache and touches no verify queue (ring, caches, counters).  Its launches count in
+ *     hs_kernel_launches.  n == 0 returns HS_OK and launches nothing; NULL recs or out_why with n > 0 is HS_ERR_ARG and writes nothing. */
+#define HS_WHY_S_NONCANONICAL 1u
+#define HS_WHY_A_INVALID 2u
+#define HS_WHY_R_INVALID 4u
+#define HS_WHY_A_SMALL 8u
+#define HS_WHY_R_SMALL 16u
+#define HS_WHY_EQUATION 32u
+int hs_explain_rec128(hs_ctx *ctx, const hs_rec128 *recs, size_t n, uint8_t *out_why /* n */);
+
 /* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) ------------------- */
 int hs_verify_rec128_dev(hs_ctx *ctx, const void *d_recs, size_t n, uint32_t mode, void *d_bitmap, void *stream);
 int hs_verify_var_dev(hs_ctx *ctx, const void *d_sig, const void *d_pk, const void *d_msgs, const void *d_off, size_t n,

@@ -88,6 +88,13 @@ class Engine {
     if (slot_bits) *slot_bits = std::move(bits);
     return failed;
   }
+  // Table-free re-check of n records (hs_explain_rec128): one byte of HS_WHY_* bits per record, one bit per failed check.  Strict
+  // verdict 1 <=> 0; batch-eq verdict 1 <=> no bit outside HS_WHY_A_SMALL | HS_WHY_R_SMALL.  Throws EngineError on a CUDA error.
+  std::vector<uint8_t> explain(const hs_rec128 *recs, size_t n) const {
+    std::vector<uint8_t> why(n);
+    check(hs_explain_rec128(ctx_, recs, n, why.data()), "hs_explain_rec128");
+    return why;
+  }
   std::string error() const { return hs_last_error(ctx_); }
 
  private:

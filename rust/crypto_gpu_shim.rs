@@ -70,6 +70,15 @@ pub const HS_OK: c_int = 0;
 pub const HS_ERR_ARG: c_int = 2;
 pub const HS_ERR_NOMEM: c_int = 3;
 pub const HS_ERR_SELFTEST: c_int = 4;
+/// Verdict mode bytes (HS_MODE_*): 0 = Signature::verify (strict), 1 = the per-signature condition of Signature::verify_batch.
+pub const HS_MODE_BATCH_EQ: u8 = 1;
+/// hs_explain_rec128's bits, one per check a record fails: S >= l, A / R do not decompress, A / R of small order, the equation.
+pub const HS_WHY_S_NONCANONICAL: u8 = 1;
+pub const HS_WHY_A_INVALID: u8 = 2;
+pub const HS_WHY_R_INVALID: u8 = 4;
+pub const HS_WHY_A_SMALL: u8 = 8;
+pub const HS_WHY_R_SMALL: u8 = 16;
+pub const HS_WHY_EQUATION: u8 = 32;
 /// Smallest signature count sent to the GPU (below it the dalek path is faster on this hardware; see the header comment).
 pub const GPU_MIN_SIGS: usize = 2;
 /// A Digest call goes to the GPU only with at least this many messages in flight (SHA-512 is sequential inside one message).
@@ -97,6 +106,7 @@ extern "C" {
     fn hs_table_audit(ctx: *mut HsCtx, expect_pks: *const u8, expect_live: *const u32, n_slots: usize, out_slot_bits: *mut u8, out_failed: *mut u32) -> c_int;
     fn hs_table_repair(ctx: *mut HsCtx, expect_pks: *const u8, expect_live: *const u32, n_slots: usize, out_slot_bits: *mut u8, out_found: *mut u32,
                        out_failed: *mut u32) -> c_int;
+    fn hs_explain_rec128(ctx: *mut HsCtx, recs: *const HsRec128, n: usize, out_why: *mut u8) -> c_int;
 }
 
 struct Ctx(*mut HsCtx);
@@ -173,6 +183,24 @@ pub fn audit_tables(expected: &[Option<[u8; 32]>]) -> Result<(), GpuError> {
     }
     DISABLED.store(true, Ordering::Release);
     Err(GpuError::Engine(format!("table audit failed (status {}, classes {:#x}): {}", rc, failed, last_error(c))))
+}
+/// Why one rejected message was rejected: its first rejected record, that record's HS_WHY_* mask, and whether the engine's verdict
+/// disagrees with the mask (`engine_fault`: the engine rejected a record that the table-free re-check finds valid in its mode).
+#[derive(Debug, Clone, Copy)]
+pub struct Explained { pub index: usize, pub why: u8, pub engine_fault: bool }
+/// Explains a rejected message: `recs` are its records, `modes` their verdict modes (HS_MODE_*) and `verdicts` the bits the engine
+/// returned for them.  Only the first rejected record is re-checked (hs_explain_rec128, a table-free re-check on the GPU), so a flood of
+/// junk signatures costs one extra record per rejected message, not one per signature.  On `engine_fault` the caller audits and repairs
+/// the tables (`audit_tables`) and answers that message on the dalek path.  None = no record was rejected, no GPU, or the re-check
+/// failed (keep the rejection).
+pub fn explain_rejected(recs: &[HsRec128], modes: &[u8], verdicts: &[bool]) -> Option<Explained> {
+    let index = verdicts.iter().position(|ok| !ok)?;
+    let c = ctx()?;
+    let mut why = 0u8;
+    let rc = unsafe { hs_explain_rec128(c, &recs[index], 1, &mut why) };
+    if rc != HS_OK { return None; }
+    let valid = if modes[index] == HS_MODE_BATCH_EQ { why & !(HS_WHY_A_SMALL | HS_WHY_R_SMALL) == 0 } else { why == 0 };
+    Some(Explained { index, why, engine_fault: valid })
 }
 /// Incremental epoch change: returns the table indices of the added validators.
 pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {

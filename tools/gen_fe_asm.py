@@ -458,14 +458,30 @@ def check_addsub(pr, is_sub):
         if rnd.random() < 0.3:
             y = (top - x + rnd.randrange(-60, 60)) & top if not is_sub else (x + rnd.randrange(-60, 60)) & top
         cases.append((x, y))
-    trace = set()
+    # crafted: the ripple alone (the folded low limb carries or borrows, the limbs above do not all pass it on) and the second wrap
+    # (a + b within 38 of 2^257 for add; a - b within 38 of -2^256 for sub)
+    for _ in range(200):
+        hi = rnd.getrandbits(224) << 32
+        if is_sub:
+            x = rnd.randrange(37)
+            cases.append((x, (x - hi - rnd.randrange(38)) % (1 << 256)))              # (x - y) mod 2^256 = hi + (< 38), hi != 0
+            cases.append((x, top - rnd.randrange(37 - x)))                              # x - y + 2^256 - 38 < 0
+        else:
+            cases.append((hi | (M32 - rnd.randrange(38)), top - hi))                   # sum = 2^256 + (< 2^32), within 38 of 2^256 + 2^32
+            x = top - rnd.randrange(19)
+            cases.append((x, top - rnd.randrange(19)))                                 # sum > 2^257 - 38
+    ripples = wraps = 0
+    tag = "sub" if is_sub else "add"
     for x, y in cases:
         env = {"a%d" % i: v for i, v in enumerate(limbs(x))}
         env.update({"b%d" % i: v for i, v in enumerate(limbs(y))})
+        trace = set()
         out = pr.run(env, trace)
         r = sum(out["r%d" % i] << (32 * i) for i in range(8))
         assert r < (1 << 256) and r % P == ((x - y) if is_sub else (x + y)) % P, (hex(x), hex(y), hex(r))
-    assert trace, "rare path never exercised"
+        ripples += ("L_" + tag) in trace
+        wraps += out.get("w_" + tag, 0) != 0
+    assert ripples >= 300 and wraps >= 150, ("%s: ripple / second wrap too rarely taken" % tag, ripples, wraps)
 
 
 def check_reduce_split():
@@ -528,7 +544,35 @@ def limbs(v, n=8):
     return [(v >> (32 * i)) & M32 for i in range(n)]
 
 
+def crafted_products(rnd, n):
+    """Products that take the out-of-line ripple of the final fold and, mostly, its second wrap: with M = 2p = 2^256 - 38, a odd and
+    b = s a^-1 mod M for a small s in [39, 75], a * b = s + j M.  The first fold leaves s + q M for a small q, and when q >= 2 that is
+    (q - 1) 2^256 + (2^256 + s - 38 q): limbs 1..7 all ones, so the final +38 (q - 1) carries out of every limb and wraps to s."""
+    out = []
+    while len(out) < n:
+        a = rnd.getrandbits(256) | 1
+        if a % P:
+            out.append((a, rnd.randrange(39, 76) * pow(a, -1, 2 * P) % (2 * P)))
+    return out
+
+
+def crafted_squares():
+    """The same for squares: a = sqrt(s) mod p for the squares s in [39, 200), its parity chosen so that a^2 = s mod 2p."""
+    out = []
+    for s in range(39, 200):
+        if pow(s, (P - 1) // 2, P) != 1:
+            continue
+        x = pow(s, (P + 3) // 8, P)
+        if x * x % P != s:
+            x = x * pow(2, (P - 1) // 4, P) % P
+        for a in (x, P - x):
+            out.append(a + P if a % 2 == 0 else a)
+    return out
+
+
 def check(pr, is_sqr):
+    """pr against Python integers on specials, random and crafted inputs; the crafted ones must take the fold's ripple and second
+    wrap often enough that both out-of-line paths are proven, not just present."""
     rnd = random.Random(1234)
     specials = [0, 1, 2, P - 1, P, P + 1, 2 * P, 2 * P + 1, (1 << 256) - 1, (1 << 256) - 38, (1 << 256) - 39,
                 (1 << 255), (1 << 255) - 1, M32, M32 << 224, int("f" * 8 + "0" * 8, 16) * ((1 << 256) // ((1 << 64) - 1))]
@@ -540,15 +584,21 @@ def check(pr, is_sqr):
         if rnd.random() < 0.3:
             y = ((1 << 256) - 1) >> rnd.randrange(64)
         cases.append((x, y))
+    cases += [(a, a) for a in crafted_squares()] if is_sqr else crafted_products(rnd, 200)
+    ripples = wraps = 0
     for x, y in cases:
         if is_sqr:
             y = x
         env = {"a%d" % i: v for i, v in enumerate(limbs(x))}
         env.update({"b%d" % i: v for i, v in enumerate(limbs(y))})
-        out = pr.run(env)
+        trace = set()
+        out = pr.run(env, trace)
         r = sum(out["r%d" % i] << (32 * i) for i in range(8))
         assert r < (1 << 256)
         assert r % P == (x * y) % P, (hex(x), hex(y), hex(r))
+        ripples += "L_red" in trace
+        wraps += out.get("w_red", 0) != 0
+    assert ripples >= (40 if is_sqr else 150) and wraps >= (40 if is_sqr else 150), ("fold ripple / second wrap too rarely taken", ripples, wraps)
 
 
 def emit_function(name, pr, nin):
@@ -580,8 +630,10 @@ def count(pr):
     return w, other
 
 
-if __name__ == "__main__":
-    m, s = gen_mul(), gen_sqr(split=os.environ.get('HS_SQR_SPLIT', '1') == '1')
+def render(sqr_split=True, karatsuba=False):
+    """Generate every sequence, run every check above on it, and return the text of fe_asm.cuh (the committed file is this text:
+    tests/test_device_arith_edges.py compares them byte for byte).  karatsuba: also emit fe_mul_karatsuba_asm."""
+    m, s = gen_mul(), gen_sqr(split=sqr_split)
     mk = gen_mul_karatsuba()   # experiment (the three short products triple the carry materialisations); emitted only on request
     check(mk, False)
     check(m, False)
@@ -594,8 +646,13 @@ if __name__ == "__main__":
            "// GF(2^255-19) multiply / square on 8 saturated 32-bit limbs; mad.lo.cc/madc.hi.cc pairs fuse to IMAD.WIDE.U32.X.\n"
            "// Every sequence below was simulated against Python big integers by the generator before being emitted.\n"
            "#pragma once\n#include <cstdint>\n\n")
-    txt = (hdr + emit_function("fe_mul_asm", m, 2) + "\n" + (emit_function("fe_mul_karatsuba_asm", mk, 2) + "\n" if os.environ.get("HS_GEN_KARATSUBA") == "1" else "") + emit_function("fe_sqr_asm", s, 1) + "\n" +
-           emit_function("fe_add_asm", ad, 2) + "\n" + emit_function("fe_sub_asm", sb, 2))
+    return (hdr + emit_function("fe_mul_asm", m, 2) + "\n" + (emit_function("fe_mul_karatsuba_asm", mk, 2) + "\n" if karatsuba else "") + emit_function("fe_sqr_asm", s, 1) + "\n" +
+            emit_function("fe_add_asm", ad, 2) + "\n" + emit_function("fe_sub_asm", sb, 2))
+
+
+if __name__ == "__main__":
+    txt = render(sqr_split=os.environ.get('HS_SQR_SPLIT', '1') == '1', karatsuba=os.environ.get("HS_GEN_KARATSUBA") == "1")
     path = os.path.join(ROOT, "hotstuff_b200", "csrc", "fe_asm.cuh")
     open(path, "w").write(txt)
+    m, mk, s = gen_mul(), gen_mul_karatsuba(), gen_sqr(split=os.environ.get('HS_SQR_SPLIT', '1') == '1')
     print("mul: %d wide-mads + %d other ops; karatsuba mul: %d + %d; sqr: %d wide-mads + %d other ops -> %s" % (count(m) + count(mk) + count(s) + (path,)))

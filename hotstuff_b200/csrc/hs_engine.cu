@@ -1491,13 +1491,25 @@ struct audit_state {
   event_h done;
   dev_buf scratch;
 };
-// Latency path: mapped pinned staging (inputs, verdict flags, completion word) and the device block counter.
-struct small_staging {
-  mapped<small_rec> in;
-  mapped<uint8_t> out;
-  mapped<uint32_t> done;
-  dev_mem<uint32_t> counter;
+// A ring of slots that k_verify_small, k_verify_bulk, k_queue_generic and k_queue_digests work over (slot = position & mask): the
+// latency path's (one request in slot 0), a verify queue's and the self-test's.
+struct ring_bufs {
+  mapped<small_rec> recs;      // sig | msg | vidx | req | req_n per record
+  mapped<uint8_t> flags;       // verdict flags per record
+  mapped<uint32_t> done;       // completion word per request slot (= launch sequence number)
+  dev_mem<uint32_t> counters;  // records finished per request slot
 };
+// Allocates r for cap slots.  When it returns, the completion words and the counters are 0.
+static cudaError_t make_ring(ring_bufs &r, uint32_t cap, cudaStream_t stream) {
+  cudaError_t e = alloc(r.recs, (size_t)cap * sizeof(small_rec));
+  if (e == cudaSuccess) e = alloc(r.flags, cap);
+  if (e == cudaSuccess) e = alloc(r.done, (size_t)cap * 4);
+  if (e == cudaSuccess) e = alloc(r.counters, (size_t)cap * 4);
+  if (e == cudaSuccess) e = cudaMemsetAsync(r.counters, 0, (size_t)cap * 4, stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);  // the ring's kernels may run on other streams
+  if (e == cudaSuccess) memset(r.done.h, 0, (size_t)cap * 4);
+  return e;
+}
 // Multi-GPU peer routing: this rank's result buffer (cudaMalloc'd: [2][total_words][HS_MAX_PEERS flags][timeout flag, block counter])
 // and the mappings of the other ranks' buffers.
 struct peer_bufs {
@@ -1548,7 +1560,7 @@ struct hs_ctx {
   bool peer_armed = false;
   uint32_t peer_epoch = 0;
   // latency path
-  small_staging small;
+  ring_bufs small;  // HS_SMALL_MAX slots
   uint32_t small_seq = 0;
   bool small_enabled = true;
   // deferred-results mode (hs_set_deferred): the latency-bound tail of a `_dev` verify pass (finish kernel, peer exchange, per-QC AND)
@@ -1945,6 +1957,41 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   return HS_OK;
 }
 
+// ---- the ring kernels' launches: each is the only launch of its kernel, counts it and returns the launch error
+// k_verify_bulk (one thread per record) or k_verify_small (one block per record) over ring positions [base, base + n), completing
+// with seq; the signature-cache instantiation when sc has a table.
+template <bool SIGC>
+static cudaError_t launch_ring_verify_as(hs_ctx *c, const ring_bufs &r, uint32_t mask, uint32_t base, uint32_t n, bool bulk,
+                                         const committee_tables &C, const comb_params &cp, const sig_cache_dev &sc, uint32_t seq, cudaStream_t s) {
+  if (bulk)
+    k_verify_bulk<SIGC><<<blocks_for(n, HS_BULK_THREADS), HS_BULK_THREADS, 0, s>>>(r.recs.d, base, mask, n, c->d_btable, C, cp, r.flags.d, r.counters,
+                                                                                 r.done.d, seq, sc);
+  else
+    k_verify_small<SIGC><<<n, 64, 0, s>>>(r.recs.d, base, mask, c->d_btable, C, cp, r.flags.d, r.counters, r.done.d, seq, sc);
+  c->launches++;
+  return cudaGetLastError();
+}
+static cudaError_t launch_ring_verify(hs_ctx *c, const ring_bufs &r, uint32_t mask, uint32_t base, uint32_t n, bool bulk, const committee_tables &C,
+                                      const comb_params &cp, const sig_cache_dev &sc, uint32_t seq, cudaStream_t s) {
+  return sc.b ? launch_ring_verify_as<true>(c, r, mask, base, n, bulk, C, cp, sc, seq, s)
+              : launch_ring_verify_as<false>(c, r, mask, base, n, bulk, C, cp, sc, seq, s);
+}
+// k_queue_generic over the n ring slots listed in slots[] from position base on, the records' keys in pks.
+static cudaError_t launch_queue_generic(hs_ctx *c, const ring_bufs &r, const uint8_t *pks, const uint32_t *slots, uint32_t mask, uint32_t base,
+                                        uint32_t n, const comb_params &cp, uint32_t seq, cudaStream_t s) {
+  k_queue_generic<<<blocks_for(n, HS_GEN_THREADS), HS_GEN_THREADS, 0, s>>>(r.recs.d, pks, slots, base, mask, n, c->d_btable, cp, r.flags.d,
+                                                                         r.counters, r.done.d, seq);
+  c->launches++;
+  return cudaGetLastError();
+}
+// k_queue_digests over the n_desc descriptors in list from position base on: the Digests of their preimages into the records' msg.
+static cudaError_t launch_queue_digests(hs_ctx *c, const ring_bufs &r, const qmsg_desc *list, uint32_t mask, uint32_t base, uint32_t n_desc,
+                                        const uint8_t *arena, uint8_t *stage, uint32_t *digs, cudaStream_t s) {
+  k_queue_digests<<<n_desc, HS_QDIG_THREADS, 0, s>>>(list, base, mask, arena, stage, digs, r.recs.d);
+  c->launches++;
+  return cudaGetLastError();
+}
+
 // ---- latency path (host side)
 // key bytes -> table index through the host mirror of the device hash table (registered committee or learned cache)
 static uint32_t host_key_lookup(const hs_ctx *c, const uint8_t *key) {
@@ -1956,32 +2003,29 @@ struct small_src {
   const uint8_t *sig, *msg;
   uint32_t vidx;
 };
-// Fills c->small.in.h[0 .. n) from rec(i) and reports whether every key index resolved (!= HS_NO_KEY).
+// Fills c->small.recs.h[0 .. n) from rec(i) and reports whether every key index resolved (!= HS_NO_KEY).
 template <class Rec>
 static bool small_stage(hs_ctx *c, size_t n, Rec rec) {
   bool all = true;
   for (size_t i = 0; i < n; i++) {
     const small_src s = rec(i);
-    memcpy(c->small.in.h[i].sig, s.sig, 64);
-    memcpy(c->small.in.h[i].msg, s.msg, 32);
-    c->small.in.h[i].vidx = s.vidx;
+    memcpy(c->small.recs.h[i].sig, s.sig, 64);
+    memcpy(c->small.recs.h[i].msg, s.msg, 32);
+    c->small.recs.h[i].vidx = s.vidx;
     all = all && s.vidx != HS_NO_KEY;
   }
   return all;
 }
-// c->small.in.h[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
+// c->small.recs.h[0 .. n) is filled: one launch (one request in slot 0), then poll the completion word the last block writes to
 // mapped host memory.
 static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap) {
   for (size_t i = 0; i < n; i++) {
-    c->small.in.h[i].req = 0;
-    c->small.in.h[i].req_n = (uint32_t)n;
+    c->small.recs.h[i].req = 0;
+    c->small.recs.h[i].req_n = (uint32_t)n;
   }
   const uint32_t seq = ++c->small_seq ? c->small_seq : ++c->small_seq;  // never 0
   HS_TRY(wait_key_cache_build(c, c->stream));
-  k_verify_small<false><<<(unsigned)n, 64, 0, c->stream>>>(c->small.in.d, 0, HS_SMALL_MAX - 1, c->d_btable, ctx_tables(c).C, c->cp, c->small.out.d,
-                                                           c->small.counter, c->small.done.d, seq, sig_cache_dev{});
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_CUDA(c, launch_ring_verify(c, c->small, HS_SMALL_MAX - 1, 0, (uint32_t)n, false, ctx_tables(c).C, c->cp, sig_cache_dev{}, seq, c->stream));
   volatile uint32_t *done = c->small.done.h;
   bool finished = false;
   for (uint64_t spin = 0; spin < (1ull << 34); spin++) {
@@ -2002,7 +2046,7 @@ static int run_small(hs_ctx *c, size_t n, uint32_t mode, uint32_t *out_bitmap) {
   for (size_t w = 0; w < (n + 31) / 32; w++) out_bitmap[w] = 0;
   const uint32_t want = mode_flag(mode);
   for (size_t i = 0; i < n; i++)
-    if (((volatile uint8_t *)c->small.out.h)[i] & want) out_bitmap[i >> 5] |= 1u << (i & 31);
+    if (((volatile uint8_t *)c->small.flags.h)[i] & want) out_bitmap[i >> 5] |= 1u << (i & 31);
   return HS_OK;
 }
 
@@ -2126,11 +2170,8 @@ struct batch_lane {
 struct hs_queue {
   hs_ctx *c = nullptr;
   uint32_t cap = 0, mask = 0;
-  mapped<small_rec> ring;                // sig | msg | vidx | req | req_n per record
-  mapped<uint8_t> flags;                 // verdict flags per record
-  mapped<uint32_t> done;                 // completion word per request slot (= launch sequence number)
-  dev_mem<uint32_t> d_counters;          // records finished per request slot
-  mapped<uint8_t> pk;                    // key bytes per record (32 B; resolved to a table index at dispatch, read by k_queue_generic)
+  ring_bufs ring;                        // cap slots
+  mapped<uint8_t> pk;                   // key bytes per record (32 B; resolved to a table index at dispatch, read by k_queue_generic)
   std::vector<uint8_t> modes;            // HS_MODE_* per record (host only: picks the verdict flag of each record)
   std::vector<uint32_t> wbits;           // dispatcher thread only: verdict bitmap being assembled (cap bits)
   stream_h stream;                       // k_verify_small launches: the device's highest priority
@@ -2334,6 +2375,31 @@ static void queue_fire(std::vector<queue_completion> &fire) {
   fire.clear();
 }
 
+// The Digests of one launch's preimage requests, on the launch's stream ahead of its verify: the descriptors of the preimage requests
+// among those at positions ps go to `list` from position lo on, and one k_queue_digests launch takes them.  dig counts what was
+// enqueued: launches, preimages and preimage bytes (hs_queue_digest_stats).
+static cudaError_t queue_digests(hs_queue *q, mapped<qmsg_desc> &list, uint64_t lo, const std::vector<uint64_t> &ps, cudaStream_t s,
+                                 uint64_t (&dig)[3]) {
+  uint32_t n_desc = 0;
+  uint64_t n_pre = 0, n_pre_bytes = 0;
+  for (uint64_t p : ps) {
+    const hs_queue::req &r = q->reqs[p & q->mask];
+    if (!r.msgs) continue;
+    list.h[(lo + n_desc++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
+    n_pre += r.m;
+    n_pre_bytes += r.pre_bytes;
+  }
+  if (n_desc == 0) return cudaSuccess;
+  const cudaError_t e =
+      launch_queue_digests(q->c, q->ring, list.d, q->mask, (uint32_t)(lo & q->mask), n_desc, q->arena_buf.d, q->d_stage, q->d_digs, s);
+  if (e == cudaSuccess) {
+    dig[0]++;
+    dig[1] += n_pre;
+    dig[2] += n_pre_bytes;
+  }
+  return e;
+}
+
 // Dispatches the pending requests [lo, hi): under c->mu, keys are resolved through the host mirror of the key hash table and
 // one launch covers every request whose keys are all registered; the others then run through hs_verify_rec128 on this thread.
 // A slow-path request of at most 64 records between two device requests rides along in the launch (its blocks find no table
@@ -2356,6 +2422,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
   std::vector<queue_completion> fire;
   std::vector<hs_queue::launch> runs;  // ring ranges [lo, hi) to launch, first device request to past the last one, in ring order
   std::vector<char> ok;                // runs launched without a CUDA error (the first failure stops the rest)
+  std::vector<uint64_t> dev;           // the device-path requests of the run being launched (slow-path riders carry no digest)
   uint64_t dig_launched[3] = {0, 0, 0};  // k_queue_digests launches, their preimages and preimage bytes (hs_queue_digest_stats)
   cudaError_t e = cudaSuccess;
   {
@@ -2372,7 +2439,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       hs_queue::req &r = q->reqs[p & q->mask];
       bool all = committee;
       for (uint32_t i = 0; i < r.n; i++) {
-        small_rec &s = q->ring.h[(p + i) & q->mask];
+        small_rec &s = q->ring.recs.h[(p + i) & q->mask];
         s.vidx = all ? host_key_lookup(c, q->pk.h + 32 * (size_t)((p + i) & q->mask)) : HS_NO_KEY;
         s.req = (uint32_t)(p & q->mask);
         s.req_n = r.n;
@@ -2382,7 +2449,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       const bool generic = gen && !all;
       r.gen = generic;
       if (!all) {  // every record of a slow-path request rides as HS_NO_KEY: none of them probes or fills the signature cache
-        for (uint32_t i = 0; i < r.n; i++) q->ring.h[(p + i) & q->mask].vidx = HS_NO_KEY;
+        for (uint32_t i = 0; i < r.n; i++) q->ring.recs.h[(p + i) & q->mask].vidx = HS_NO_KEY;
         r.seq = 0;  // a generic request's launch number is set when its launch is built
         if (generic) q->gpend.push_back(p);
         else slow.push_back(p);
@@ -2405,55 +2472,25 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
     }
     if (rlo < rhi) runs.push_back(hs_queue::launch{0, rlo, rhi, false});
     const committee_tables C = ctx_tables(c).C;
+    const sig_cache_dev sc = q->d_sig ? sig_cache_dev{q->d_sig, q->sigc.key, q->sig_bmask, q->sigc.ctr, q->sigc.hctr.d} : sig_cache_dev{};
     ok.assign(runs.size(), 0);
     for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {  // pass 0: the small launches, pass 1: the bulk ones
       for (size_t k = 0; k < runs.size(); k++) {
         hs_queue::launch &L = runs[k];
         if (L.bulk != (pass == 1)) continue;
         L.seq = ++q->seq ? q->seq : ++q->seq;  // never 0
-        uint32_t n_msgs_req = 0;  // the run's device-path preimage requests (slow-path riders carry no digest)
-        uint64_t n_pre = 0, n_pre_bytes = 0;
+        L.sig_gen = q->d_sig ? q->sig_gen : 0;
+        dev.clear();
         for (uint64_t p = L.lo; p < L.hi; p += q->reqs[p & q->mask].n) {
           hs_queue::req &r = q->reqs[p & q->mask];
           if (!r.seq) continue;
           r.seq = L.seq;
-          if (!r.msgs) continue;
-          q->mlist.h[(L.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
-          n_pre += r.m;
-          n_pre_bytes += r.pre_bytes;
+          dev.push_back(p);
         }
-        const uint32_t n = (uint32_t)(L.hi - L.lo), base = (uint32_t)(L.lo & q->mask);
         cudaStream_t s = L.bulk ? q->bulk_stream : q->stream;
-        if (n_msgs_req) {  // the Digests first, on the verify launch's stream
-          k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, s>>>(q->mlist.d, base, q->mask, q->arena_buf.d, q->d_stage, q->d_digs, q->ring.d);
-          c->launches++;
-          e = cudaGetLastError();
-          if (e == cudaSuccess) {
-            dig_launched[0]++;
-            dig_launched[1] += n_pre;
-            dig_launched[2] += n_pre_bytes;
-          }
-        }
-        if (e == cudaSuccess) {
-          const unsigned bulk_blocks = (n + HS_BULK_THREADS - 1) / HS_BULK_THREADS;
-          if (q->d_sig) {
-            const sig_cache_dev sc{q->d_sig, q->sigc.key, q->sig_bmask, q->sigc.ctr, q->sigc.hctr.d};
-            L.sig_gen = q->sig_gen;
-            if (L.bulk)
-              k_verify_bulk<true><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->ring.d, base, q->mask, n, c->d_btable, C, c->cp, q->flags.d, q->d_counters,
-                                                                         q->done.d, L.seq, sc);
-            else
-              k_verify_small<true><<<n, 64, 0, s>>>(q->ring.d, base, q->mask, c->d_btable, C, c->cp, q->flags.d, q->d_counters, q->done.d, L.seq, sc);
-          } else if (L.bulk) {
-            k_verify_bulk<false><<<bulk_blocks, HS_BULK_THREADS, 0, s>>>(q->ring.d, base, q->mask, n, c->d_btable, C, c->cp, q->flags.d, q->d_counters,
-                                                                        q->done.d, L.seq, sig_cache_dev{});
-          } else {
-            k_verify_small<false><<<n, 64, 0, s>>>(q->ring.d, base, q->mask, c->d_btable, C, c->cp, q->flags.d, q->d_counters, q->done.d, L.seq,
-                                                   sig_cache_dev{});
-          }
-          c->launches++;
-          e = cudaGetLastError();
-        }
+        e = queue_digests(q, q->mlist, L.lo, dev, s, dig_launched);
+        if (e == cudaSuccess)
+          e = launch_ring_verify(c, q->ring, q->mask, (uint32_t)(L.lo & q->mask), (uint32_t)(L.hi - L.lo), L.bulk, C, c->cp, sc, L.seq, s);
         if (e == cudaSuccess) e = L.bulk ? cudaEventRecord(q->ev_bulk_last, q->bulk_stream) : cudaEventRecord(q->ev_last, q->stream);
         if (e != cudaSuccess) {
           fail(c, HS_ERR_CUDA, "verify queue launch", e);
@@ -2469,37 +2506,17 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       q->gpend.clear();
       G.seq = ++q->seq ? q->seq : ++q->seq;
       G.lo = greqs.front();
-      uint32_t n_msgs_req = 0;
-      uint64_t n_pre = 0, n_pre_bytes = 0;
       for (uint64_t p : greqs) {
         hs_queue::req &r = q->reqs[p & q->mask];
         r.seq = G.seq;
-        if (r.msgs) {
-          q->gen_bufs.mlist.h[(G.lo + n_msgs_req++) & q->mask] = qmsg_desc{r.a_off, r.m, r.n, (uint32_t)(p & q->mask), r.pre_bytes, {0, 0, 0}};
-          n_pre += r.m;
-          n_pre_bytes += r.pre_bytes;
-        }
         for (uint32_t i = 0; i < r.n; i++) q->gen_bufs.slot.h[(G.lo + g_recs++) & q->mask] = (uint32_t)((p + i) & q->mask);
         G.hi = p + r.n;
       }
-      const uint32_t base = (uint32_t)(G.lo & q->mask);
       const bool earlier_failure = e != cudaSuccess;
-      if (e == cudaSuccess && n_msgs_req) {  // the Digests first, on the same stream
-        k_queue_digests<<<n_msgs_req, HS_QDIG_THREADS, 0, q->bulk_stream>>>(q->gen_bufs.mlist.d, base, q->mask, q->arena_buf.d, q->d_stage, q->d_digs, q->ring.d);
-        c->launches++;
-        e = cudaGetLastError();
-        if (e == cudaSuccess) {
-          dig_launched[0]++;
-          dig_launched[1] += n_pre;
-          dig_launched[2] += n_pre_bytes;
-        }
-      }
-      if (e == cudaSuccess) {
-        k_queue_generic<<<(unsigned)((g_recs + HS_GEN_THREADS - 1) / HS_GEN_THREADS), HS_GEN_THREADS, 0, q->bulk_stream>>>(
-            q->ring.d, q->pk.d, q->gen_bufs.slot.d, base, q->mask, (uint32_t)g_recs, c->d_btable, c->cp, q->flags.d, q->d_counters, q->done.d, G.seq);
-        c->launches++;
-        e = cudaGetLastError();
-      }
+      if (e == cudaSuccess) e = queue_digests(q, q->gen_bufs.mlist, G.lo, greqs, q->bulk_stream, dig_launched);
+      if (e == cudaSuccess)
+        e = launch_queue_generic(c, q->ring, q->pk.d, q->gen_bufs.slot.d, q->mask, (uint32_t)(G.lo & q->mask), (uint32_t)g_recs, c->cp, G.seq,
+                                 q->bulk_stream);
       if (e == cudaSuccess) e = cudaEventRecord(q->ev_bulk_last, q->bulk_stream);
       g_ok = e == cudaSuccess;
       if (!g_ok && !earlier_failure) fail(c, HS_ERR_CUDA, "verify queue generic launch", e);
@@ -2551,7 +2568,7 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
       idx.assign(r.n, 0);  // group_idx
       for (uint32_t i = 0; i < r.n; i++) {
         const uint32_t s = (uint32_t)((p + i) & q->mask);
-        memcpy(&msig[(size_t)i * 64], q->ring.h[s].sig, 64);
+        memcpy(&msig[(size_t)i * 64], q->ring.recs.h[s].sig, 64);
         memcpy(&mpk[(size_t)i * 32], q->pk.h + 32 * (size_t)s, 32);
         mmode[i] = q->modes[s];
       }
@@ -2567,9 +2584,9 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
         const uint32_t s = (uint32_t)((p + i) & q->mask);
         if (q->modes[s] != mode) continue;
         hs_rec128 x;
-        memcpy(x.sig, q->ring.h[s].sig, 64);
+        memcpy(x.sig, q->ring.recs.h[s].sig, 64);
         memcpy(x.pk, q->pk.h + 32 * (size_t)s, 32);
-        memcpy(x.msg, q->ring.h[s].msg, 32);
+        memcpy(x.msg, q->ring.recs.h[s].msg, 32);
         recs.push_back(x);
         idx.push_back(i);
       }
@@ -2613,14 +2630,14 @@ static void queue_watch(hs_queue *q) {
         hs_queue::req &r = q->reqs[p & q->mask];
         if (L.generic && !(r.gen && r.seq == L.seq)) continue;  // a request of another launch between its generic requests
         const bool mine = r.seq == L.seq && !r.finished;
-        if (((volatile uint32_t *)q->done.h)[p & q->mask] == L.seq) {
+        if (((volatile uint32_t *)q->ring.done.h)[p & q->mask] == L.seq) {
           if (!mine) continue;
           std::atomic_thread_fence(std::memory_order_acquire);
           uint32_t *bits = q->wbits.data();
           std::fill(bits, bits + (r.n + 31) / 32, 0u);
           for (uint32_t i = 0; i < r.n; i++) {  // the kernel writes both flags: each record's mode picks its verdict
             const uint32_t s = (uint32_t)((p + i) & q->mask);
-            if (((volatile uint8_t *)q->flags.h)[s] & mode_flag(q->modes[s])) bits[i >> 5] |= 1u << (i & 31);
+            if (((volatile uint8_t *)q->ring.flags.h)[s] & mode_flag(q->modes[s])) bits[i >> 5] |= 1u << (i & 31);
           }
           if (L.sig_gen) {  // the completing block moved the request's signature-cache counts here before its completion word
             const volatile uint32_t *sc = q->sigc.hctr.h + HS_SIG_CTRS * (size_t)(p & q->mask);
@@ -2838,6 +2855,13 @@ static int launch_digest_fixed(hs_ctx *c, const uint8_t *d_msgs, size_t msg_len,
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
 }
+// Digest of a few long messages: one warp per message, schedules expanded in parallel across lanes.
+static int launch_digest_long(hs_ctx *c, const uint8_t *d_data, const uint64_t *d_off, size_t n, uint32_t *d_out, cudaStream_t stream) {
+  k_digest32_long<<<(unsigned)n, 32, 0, stream>>>(d_data, d_off, n, d_out);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
 
 // off[0] == 0 and off[i] <= off[i+1]: a decreasing offset would make a length wrap to ~2^64 on the device
 static bool offsets_ok(const uint64_t *off, size_t n) {
@@ -2904,12 +2928,7 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
   if (e == cudaSuccess) e = create(c->ev_main_done);
   if (e == cudaSuccess) e = create(c->ev_results);
   for (int i = 0; i < 2 && e == cudaSuccess; i++) e = create(c->ev_tail[i]);
-  if (e == cudaSuccess) e = alloc(c->small.in, HS_SMALL_MAX * sizeof(small_rec));
-  if (e == cudaSuccess) e = alloc(c->small.out, 256);
-  if (e == cudaSuccess) e = alloc(c->small.done, 64);
-  if (e == cudaSuccess) e = alloc(c->small.counter, 4);
-  if (e == cudaSuccess) e = cudaMemset(c->small.counter, 0, 4);
-  if (e == cudaSuccess) *c->small.done.h = 0;
+  if (e == cudaSuccess) e = make_ring(c->small, HS_SMALL_MAX, c->stream);
   c->small_enabled = !(getenv("HS_SMALL_PATH") && getenv("HS_SMALL_PATH")[0] == '0');
   set_window(c->cp, false, wb);
   set_window(c->cp, true, 12);
@@ -3558,14 +3577,10 @@ int hs_digest32_batch(hs_ctx *c, const uint8_t *data, const uint64_t *off, size_
   const size_t s_off = S.add(off, (n + 1) * 8), s_data = S.add(data, off[n], 8);
   HS_TRY(ensure(c, c->out, n * 32));
   HS_TRY(S.upload(c, c->in[0], c->stream));
-  if (n <= 64 && off[n] / n >= 1024) {
-    // a few long messages (mempool batches): one warp per message, schedules expanded in parallel across lanes
-    k_digest32_long<<<(unsigned)n, 32, 0, c->stream>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, (uint32_t *)c->out.p.get());
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
-  } else {
+  if (n <= 64 && off[n] / n >= 1024)  // a few long messages (mempool batches)
+    HS_TRY(launch_digest_long(c, S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, (uint32_t *)c->out.p.get(), c->stream));
+  else
     HS_TRY(hs_digest32_dev(c, S.ptr(s_data), S.ptr(s_off), n, c->out.p, c->stream));
-  }
   return readback(c, {{out, c->out.p.get(), n * 32}});
 }
 
@@ -3645,18 +3660,13 @@ int hs_queue_create(hs_ctx *c, size_t ring_records, hs_queue **out) {
   if (e == cudaSuccess) e = create(q->bulk_stream, lo);
   if (e == cudaSuccess) e = create(q->ev_last);
   if (e == cudaSuccess) e = create(q->ev_bulk_last);
-  if (e == cudaSuccess) e = alloc(q->ring, (size_t)cap * sizeof(small_rec));
-  if (e == cudaSuccess) e = alloc(q->flags, cap);
-  if (e == cudaSuccess) e = alloc(q->done, (size_t)cap * 4);
-  if (e == cudaSuccess) e = alloc(q->d_counters, (size_t)cap * 4);
-  if (e == cudaSuccess) e = cudaMemset(q->d_counters, 0, (size_t)cap * 4);
+  if (e == cudaSuccess) e = make_ring(q->ring, cap, q->stream);
   if (e == cudaSuccess) e = alloc(q->arena_buf, q->arena.cap);
   if (e == cudaSuccess) e = alloc(q->mlist, (size_t)cap * sizeof(qmsg_desc));
   if (e == cudaSuccess) e = alloc(q->pk, (size_t)cap * 32);
   if (e == cudaSuccess) e = alloc(q->d_stage, q->arena.cap);
   if (e == cudaSuccess) e = alloc(q->d_digs, q->arena.cap * 4);
   if (e != cudaSuccess) return fail(c, HS_ERR_CUDA, "hs_queue_create", e);
-  memset(q->done.h, 0, (size_t)cap * 4);
   memset(q->pk.h, 0, (size_t)cap * 32);
   try {
     q->th = std::thread(queue_main, q.get());
@@ -3687,8 +3697,8 @@ static int queue_put_recs_locked(hs_queue *q, const char *what, const hs_rec128 
   for (size_t k = 0; k < sel.n; k++) {
     const size_t i = sel[k];
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
-    memcpy(q->ring.h[s].sig, recs[i].sig, 64);
-    memcpy(q->ring.h[s].msg, recs[i].msg, 32);
+    memcpy(q->ring.recs.h[s].sig, recs[i].sig, 64);
+    memcpy(q->ring.recs.h[s].msg, recs[i].msg, 32);
     memcpy(q->pk.h + 32 * (size_t)s, recs[i].pk, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)mode;
   }
@@ -3734,7 +3744,7 @@ static int queue_put_msgs_locked(hs_queue *q, const uint8_t *preimages, const ui
   for (size_t k = 0; k < n; k++) {
     const size_t i = sel[k];
     const uint32_t s = (uint32_t)((q->tail + k) & q->mask);
-    memcpy(q->ring.h[s].sig, sig + 64 * i, 64);
+    memcpy(q->ring.recs.h[s].sig, sig + 64 * i, 64);
     memcpy(q->pk.h + 32 * (size_t)s, pk + 32 * i, 32);
     q->modes[s] = modes ? modes[i] : (uint8_t)HS_MODE_STRICT;
     idx[k] = remap[msg_idx[i]];
@@ -4242,8 +4252,9 @@ static int st_read(hs_ctx *c, cudaStream_t st, void *dst, const void *src, size_
   return HS_OK;
 }
 
-// The three Digest kernels over the SHA-512 known answers, and k_keygen / k_sign_digests over the seeded keys.
-static int st_digest_and_sign_paths(hs_ctx *c, const comb_params &cp, cudaStream_t st, st_result &R) {
+// The three Digest kernels over the SHA-512 known answers, and k_keygen / k_sign_digests over the seeded keys, each through the launch
+// the product uses.  Keygen and signing read only the base-point window of the context's cp, which the self-test's cp shares.
+static int st_digest_and_sign_paths(hs_ctx *c, cudaStream_t st, st_result &R) {
   const size_t n = HS_ST_N_DIGEST_KATS;
   std::vector<uint64_t> off(n + 1);
   for (size_t i = 0; i < n; i++) off[i] = hs_st_digest_kats[i].off;
@@ -4272,15 +4283,11 @@ static int st_digest_and_sign_paths(hs_ctx *c, const comb_params &cp, cudaStream
     snprintf(b, sizeof b, "%s: digest known answer %zu (%u bytes): wrong Digest", path, i, hs_st_digest_kats[i].len);
     R.mismatch(bit, b);
   };
-  k_digest32<<<blocks_for(n), HS_THREADS, 0, st>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), 0, n, d_out);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(hs_digest32_dev(c, S.ptr(s_data), S.ptr(s_off), n, d_out, st));
   HS_TRY(st_read(c, st, got.data(), d_out, 32 * n));
   for (size_t i = 0; i < n; i++) check_digests(HS_SELFTEST_DIGEST, "k_digest32", i);
   HS_CUDA(c, cudaMemsetAsync(d_out, 0, 32 * n, st));
-  k_digest32_long<<<(unsigned)n, 32, 0, st>>>(S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, d_out);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(launch_digest_long(c, S.ptr(s_data), (const uint64_t *)S.ptr(s_off), n, d_out, st));
   HS_TRY(st_read(c, st, got.data(), d_out, 32 * n));
   for (size_t i = 0; i < n; i++) check_digests(HS_SELFTEST_DIGEST_LONG, "k_digest32_long", i);
   // k_digest32_fixed takes 16-byte aligned messages of at least one full block, one launch per length
@@ -4298,14 +4305,9 @@ static int st_digest_and_sign_paths(hs_ctx *c, const comb_params &cp, cudaStream
   }
   // keys of the seeded test keys and RFC 8032 TEST 1, then the signatures of 32-byte digests
   uint8_t *d_res = S.ptr(s_res);
-  k_keygen<<<1, HS_THREADS, 0, st>>>(S.ptr(s_seed), HS_ST_N_SEEDS + 1, c->d_btable, cp, d_res);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
-  uint8_t *d_sig = d_res + 32 * (HS_ST_N_SEEDS + 1);
-  k_sign_digests<<<1, HS_THREADS, 0, st>>>(S.ptr(s_seed), S.ptr(s_pk), (const uint32_t *)S.ptr(s_ki), S.ptr(s_dig), HS_ST_N_SIGNATURES, HS_ST_N_SEEDS,
-                                           c->d_btable, cp, d_sig);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_TRY(hs_keygen_batch_dev(c, S.ptr(s_seed), HS_ST_N_SEEDS + 1, d_res, st));
+  HS_TRY(hs_sign_digests_dev(c, S.ptr(s_seed), S.ptr(s_pk), HS_ST_N_SEEDS, S.ptr(s_ki), S.ptr(s_dig), HS_ST_N_SIGNATURES,
+                             d_res + 32 * (HS_ST_N_SEEDS + 1), st));
   std::vector<uint8_t> res(32 * (HS_ST_N_SEEDS + 1) + 64 * HS_ST_N_SIGNATURES);
   HS_TRY(st_read(c, st, res.data(), d_res, res.size()));
   for (size_t i = 0; i <= HS_ST_N_SEEDS; i++) {
@@ -4412,19 +4414,16 @@ static int st_verify_paths(hs_ctx *c, const st_set &T, const st_keys &KS, const 
   uint32_t cap = HS_SMALL_MAX;
   while (cap < n) cap <<= 1;
   const uint32_t mask = cap - 1, buckets = std::max(cap / 2, 16u);
-  mapped<small_rec> ring;
-  mapped<uint8_t> flags, pk;
-  mapped<uint32_t> done, slot, hctr;
-  dev_mem<uint32_t> counters, ctr;
+  ring_bufs ring;
+  mapped<uint8_t> pk;
+  mapped<uint32_t> slot, hctr;
+  dev_mem<uint32_t> ctr;
   dev_mem<sig_bucket> table;
   dev_mem<uint64_t> key;
-  HS_CUDA(c, alloc(ring, (size_t)cap * sizeof(small_rec)));
-  HS_CUDA(c, alloc(flags, cap));
+  HS_CUDA(c, make_ring(ring, cap, st));
   HS_CUDA(c, alloc(pk, (size_t)cap * 32));
-  HS_CUDA(c, alloc(done, (size_t)cap * 4));
   HS_CUDA(c, alloc(slot, (size_t)cap * 4));
   HS_CUDA(c, alloc(hctr, (size_t)cap * 4 * HS_SIG_CTRS));
-  HS_CUDA(c, alloc(counters, (size_t)cap * 4));
   HS_CUDA(c, alloc(ctr, (size_t)cap * 4 * HS_SIG_CTRS));
   HS_CUDA(c, alloc(table, (size_t)buckets * sizeof(sig_bucket)));
   HS_CUDA(c, alloc(key, 32 * 8));
@@ -4433,63 +4432,48 @@ static int st_verify_paths(hs_ctx *c, const st_set &T, const st_keys &KS, const 
   uint64_t z = 0x243f6a8885a308d3ull;  // any fixed key: the table is private and short-lived
   for (uint64_t &k : kh) k = (z += 0x9e3779b97f4a7c15ull) ^ (z >> 29);
   HS_CUDA(c, cudaMemcpyAsync(key, kh, sizeof kh, cudaMemcpyHostToDevice, st));
-  HS_CUDA(c, cudaMemsetAsync(counters, 0, (size_t)cap * 4, st));
   HS_CUDA(c, cudaMemsetAsync(ctr, 0, (size_t)cap * 4 * HS_SIG_CTRS, st));
-  memset(ring.h, 0, (size_t)cap * sizeof(small_rec));
-  memset(done.h, 0, (size_t)cap * 4);
+  memset(ring.recs.h, 0, (size_t)cap * sizeof(small_rec));
   for (uint32_t i = 0; i < n; i++) {
-    memcpy(ring.h[i].sig, T.r32[i].sig, 64);
-    memcpy(ring.h[i].msg, T.r32[i].msg, 32);
-    ring.h[i].vidx = vidx[i];
-    ring.h[i].req = 0;
-    ring.h[i].req_n = (uint32_t)n;
+    memcpy(ring.recs.h[i].sig, T.r32[i].sig, 64);
+    memcpy(ring.recs.h[i].msg, T.r32[i].msg, 32);
+    ring.recs.h[i].vidx = vidx[i];
+    ring.recs.h[i].req = 0;
+    ring.recs.h[i].req_n = (uint32_t)n;
     memcpy(pk.h + 32 * (size_t)i, T.r32[i].pk, 32);
     slot.h[i] = i;
   }
-  const sig_cache_dev sc{table, key, buckets - 1, ctr, hctr.d};
-  const unsigned blocks = (unsigned)((n + HS_BULK_THREADS - 1) / HS_BULK_THREADS);
   uint32_t seq = 0;
   // launch(seq) enqueues one kernel over the request; its completion word and its records' flags are then compared
   auto queue_pass = [&](uint32_t bit, const char *path, auto launch) -> int {
-    memset(flags.h, 0, cap);
-    launch(++seq);
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
+    memset(ring.flags.h, 0, cap);
+    HS_CUDA(c, launch(++seq));
     HS_CUDA(c, cudaStreamSynchronize(st));
-    if (((volatile uint32_t *)done.h)[0] != seq) {
+    if (((volatile uint32_t *)ring.done.h)[0] != seq) {
       R.mismatch(bit, std::string(path) + ": the request did not complete");
       return HS_OK;
     }
-    st_compare(R, bit, path, T.n32, T.e32, nullptr, [&](size_t i) { return st_flag_bits(flags.h[i]); });
+    st_compare(R, bit, path, T.n32, T.e32, nullptr, [&](size_t i) { return st_flag_bits(ring.flags.h[i]); });
     return HS_OK;
   };
-  const ge_niels *bt = c->d_btable;
-  const pass_tables &P = K;
-  HS_TRY(queue_pass(HS_SELFTEST_SMALL, "k_verify_small", [&](uint32_t s) {
-    k_verify_small<false><<<(unsigned)n, 64, 0, st>>>(ring.d, 0, mask, bt, P.C, P.cp, flags.d, counters, done.d, s, sig_cache_dev{});
-  }));
-  HS_TRY(queue_pass(HS_SELFTEST_BULK, "k_verify_bulk", [&](uint32_t s) {
-    k_verify_bulk<false><<<blocks, HS_BULK_THREADS, 0, st>>>(ring.d, 0, mask, (uint32_t)n, bt, P.C, P.cp, flags.d, counters, done.d, s, sig_cache_dev{});
-  }));
-  HS_TRY(queue_pass(HS_SELFTEST_QUEUE_GENERIC, "k_queue_generic", [&](uint32_t s) {
-    k_queue_generic<<<blocks, HS_GEN_THREADS, 0, st>>>(ring.d, pk.d, slot.d, 0, mask, (uint32_t)n, bt, P.cp, flags.d, counters, done.d, s);
-  }));
-  // the signature-cache instantiations run twice on an empty table: the first run probes, misses and inserts, the second answers from it
+  // k_verify_small and k_verify_bulk without the signature cache, then k_queue_generic, then the two with the cache, each twice on an
+  // empty table: the first run probes, misses and inserts, the second answers from it
+  const sig_cache_dev sc{table, key, buckets - 1, ctr, hctr.d};
+  static const uint32_t bits[2][2] = {{HS_SELFTEST_SMALL, HS_SELFTEST_BULK}, {HS_SELFTEST_SMALL_CACHE, HS_SELFTEST_BULK_CACHE}};
   for (int cached = 0; cached < 2; cached++) {
-    HS_CUDA(c, cudaMemsetAsync(table, 0, (size_t)buckets * sizeof(sig_bucket), st));
-    for (int run = 0; run < 2; run++) {
-      if (cached == 0)
-        HS_TRY(queue_pass(HS_SELFTEST_SMALL_CACHE, run ? "k_verify_small<cache> (cache filled)" : "k_verify_small<cache> (empty cache)",
-                          [&](uint32_t s) {
-                            k_verify_small<true><<<(unsigned)n, 64, 0, st>>>(ring.d, 0, mask, bt, P.C, P.cp, flags.d, counters, done.d, s, sc);
-                          }));
-      else
-        HS_TRY(queue_pass(HS_SELFTEST_BULK_CACHE, run ? "k_verify_bulk<cache> (cache filled)" : "k_verify_bulk<cache> (empty cache)",
-                          [&](uint32_t s) {
-                            k_verify_bulk<true><<<blocks, HS_BULK_THREADS, 0, st>>>(ring.d, 0, mask, (uint32_t)n, bt, P.C, P.cp, flags.d, counters,
-                                                                                    done.d, s, sc);
-                          }));
+    for (int bulk = 0; bulk < 2; bulk++) {
+      if (cached) HS_CUDA(c, cudaMemsetAsync(table, 0, (size_t)buckets * sizeof(sig_bucket), st));
+      const std::string kernel = bulk ? "k_verify_bulk" : "k_verify_small";
+      for (int run = 0; run <= cached; run++) {
+        const std::string path = cached ? kernel + (run ? "<cache> (cache filled)" : "<cache> (empty cache)") : kernel;
+        HS_TRY(queue_pass(bits[cached][bulk], path.c_str(), [&](uint32_t s) {
+          return launch_ring_verify(c, ring, mask, 0, (uint32_t)n, bulk, K.C, K.cp, cached ? sc : sig_cache_dev{}, s, st);
+        }));
+      }
     }
+    if (!cached)
+      HS_TRY(queue_pass(HS_SELFTEST_QUEUE_GENERIC, "k_queue_generic",
+                        [&](uint32_t s) { return launch_queue_generic(c, ring, pk.d, slot.d, mask, 0, (uint32_t)n, K.cp, s, st); }));
   }
   return HS_OK;
 }
@@ -4501,17 +4485,17 @@ static int st_queue_digest_path(hs_ctx *c, cudaStream_t st, st_result &R) {
   const uint64_t bytes = qmsg_bytes(m, n, HS_ST_KAT_MSG_BYTES);
   mapped<uint8_t> arena;
   mapped<qmsg_desc> list;
-  mapped<small_rec> ring;
+  ring_bufs ring;
   dev_mem<uint8_t> stage;
   dev_mem<uint32_t> digs;
   HS_CUDA(c, alloc(arena, bytes));
   HS_CUDA(c, alloc(list, sizeof(qmsg_desc)));
-  HS_CUDA(c, alloc(ring, (size_t)cap * sizeof(small_rec)));
+  HS_CUDA(c, make_ring(ring, cap, st));
   HS_CUDA(c, alloc(stage, bytes));
   HS_CUDA(c, alloc(digs, bytes * 4));
   const st_drain drain{st, nullptr};
   memset(arena.h, 0, bytes);
-  memset(ring.h, 0, (size_t)cap * sizeof(small_rec));
+  memset(ring.recs.h, 0, (size_t)cap * sizeof(small_rec));
   uint64_t *off = reinterpret_cast<uint64_t *>(arena.h.get());
   uint32_t *msg_idx = reinterpret_cast<uint32_t *>(arena.h + 8 * ((size_t)m + 1));
   for (uint32_t i = 0; i < m; i++) {
@@ -4521,12 +4505,10 @@ static int st_queue_digest_path(hs_ctx *c, cudaStream_t st, st_result &R) {
   off[m] = HS_ST_KAT_MSG_BYTES;
   memcpy(arena.h + qmsg_o_pre(m, n), hs_st_kat_msgs, HS_ST_KAT_MSG_BYTES);
   *list.h = qmsg_desc{0, m, n, 0, HS_ST_KAT_MSG_BYTES, {0, 0, 0}};
-  k_queue_digests<<<1, HS_QDIG_THREADS, 0, st>>>(list.d, 0, cap - 1, arena.d, stage, digs, ring.d);
-  c->launches++;
-  HS_CUDA(c, cudaGetLastError());
+  HS_CUDA(c, launch_queue_digests(c, ring, list.d, cap - 1, 0, 1, arena.d, stage, digs, st));
   HS_CUDA(c, cudaStreamSynchronize(st));
   for (uint32_t i = 0; i < n; i++) {
-    if (memcmp(ring.h[i].msg, hs_st_digest_kats[i].digest, 32) == 0) continue;
+    if (memcmp(ring.recs.h[i].msg, hs_st_digest_kats[i].digest, 32) == 0) continue;
     R.mismatch(HS_SELFTEST_QUEUE_DIGESTS, "k_queue_digests: digest known answer " + std::to_string(i) + ": wrong Digest");
     break;
   }
@@ -4566,7 +4548,7 @@ static int self_test_locked(hs_ctx *c, int key_bits, const hs_rec128 *recs, cons
     pass_tables K;
     HS_TRY(st_build_keys(c, T, cp, KS, K, st));
     if (!recs) {
-      HS_TRY(st_digest_and_sign_paths(c, cp, st, R));
+      HS_TRY(st_digest_and_sign_paths(c, st, R));
       HS_TRY(st_queue_digest_path(c, st, R));
     }
     HS_TRY(st_verify_paths(c, T, KS, K, st, side, R));

@@ -74,6 +74,11 @@ SIGNATURES = {
     "hs_queue_submit_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t,
                                       c_void_p, c_void_p, ctypes.POINTER(c_size_t)]),
     "hs_queue_batch_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_queue_explain": (c_int, [c_void_p, c_size_t, c_size_t]),
+    "hs_queue_submit_explain": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t)]),
+    "hs_queue_submit_explain_msgs": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p,
+                                             ctypes.POINTER(c_size_t)]),
+    "hs_queue_explain_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_destroy": (None, [c_void_p]),
     "hs_self_test": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_u32)]),
     "hs_key_slots": (c_size_t, [c_void_p]),

@@ -1156,6 +1156,78 @@ __global__ void __launch_bounds__(HS_THREADS) k_explain(const uint8_t *__restric
   }
 }
 
+// The verify queue's explain lane (hs_queue_submit_explain, hs_queue_submit_explain_msgs).  A request's region of the lane's mapped
+// arena is recs (n x 128 B: sig | pk | Digest, the Digest field unused for a preimage request) | pre_off (u64, m + 1) | msg_idx (u32, n)
+// | the m preimages | why bytes (n) | tail: [0] records done (in the device mirror), [1] completion word.  A Digest request (m = 0) has
+// no preimage sections.  Every section starts 16-byte aligned.
+struct xq_layout {
+  uint64_t o_off, o_mi, o_pre, o_why, o_tail, size;
+};
+__host__ __device__ inline xq_layout xq_layout_of(uint64_t n, uint64_t m, uint64_t pre_bytes) {
+  auto al = [](uint64_t x) { return (x + 15) & ~(uint64_t)15; };
+  xq_layout L;
+  L.o_off = 128 * n;
+  L.o_mi = L.o_off + (m ? al(8 * (m + 1)) : 0);
+  L.o_pre = L.o_mi + (m ? al(4 * n) : 0);
+  L.o_why = L.o_pre + al(pre_bytes);
+  L.o_tail = L.o_why + al(n);
+  L.size = L.o_tail + 16;
+  return L;
+}
+// One explain launch's requests, in submit order: request k's records are the launch's records [first, first + n).
+struct xq_desc {
+  uint64_t off;        // region offset in the arena (and in its device mirror)
+  uint32_t n, first;   // records; index of its record 0 in the launch
+  uint32_t m;          // preimages (0: a Digest request)
+  uint32_t pre_bytes;  // preimage bytes
+  uint32_t seq;        // the completion word's value
+  uint32_t pad;
+};
+static_assert(sizeof(xq_desc) == 32, "xq_desc is 32 bytes");
+// A thread per record, grid-stride over the launch's n records (the grid is a fixed share of the SMs: see launch_queue_explain).  The
+// thread finds its request in the descriptor list, reads its record from the region's device mirror, hashes its preimage with
+// sha512_prefix_msg when it has one (Digest = SHA-512(preimage)[..32]) and runs explain_record exactly as k_explain does.  Its why byte
+// goes to the mapped arena; the add that completes a request fences to system scope and raises the request's completion word.  It reads
+// the regions and nothing else: no context table, key slot, flag or hash table, and no base-point table.
+__global__ void __launch_bounds__(HS_THREADS) k_queue_explain(const xq_desc *__restrict__ list, uint32_t n_desc, uint32_t n,
+                                                              uint8_t *mirror, uint8_t *arena) {
+  for (uint32_t j = blockIdx.x * HS_THREADS + threadIdx.x; j < n; j += gridDim.x * HS_THREADS) {
+    uint32_t lo = 0, hi = n_desc;  // the last request whose first record is <= j
+    while (hi - lo > 1) {
+      const uint32_t mid = (lo + hi) / 2;
+      if (list[mid].first <= j) lo = mid;
+      else hi = mid;
+    }
+    const xq_desc d = list[lo];
+    const xq_layout L = xq_layout_of(d.n, d.m, d.pre_bytes);
+    const uint32_t i = j - d.first;
+    uint8_t *reg = mirror + d.off;
+    const uint8_t *r = reg + 128 * (size_t)i;
+    uint32_t R[8], S[8], A[8], M[8], h[16];
+    load32(R, r);
+    load32(S, r + 32);
+    load32(A, r + 64);
+    if (d.m) {
+      const uint64_t *pre_off = reinterpret_cast<const uint64_t *>(reg + L.o_off);
+      const uint32_t k = reinterpret_cast<const uint32_t *>(reg + L.o_mi)[i];
+      const uint64_t none[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      sha512_prefix_msg(h, none, 0, reg + L.o_pre + pre_off[k], pre_off[k + 1] - pre_off[k]);
+#pragma unroll
+      for (int w = 0; w < 8; w++) M[w] = h[w];
+    } else {
+      load32(M, r + 96);
+    }
+    sha512_ram32(h, R, A, M);
+    ge_cached tab[9];
+    arena[d.off + L.o_why + i] = (uint8_t)explain_record(R, S, A, h, tab);
+    __threadfence_system();
+    if (atomicAdd(reinterpret_cast<uint32_t *>(reg + L.o_tail), 1u) == d.n - 1) {
+      __threadfence_system();
+      reinterpret_cast<volatile uint32_t *>(arena + d.off + L.o_tail)[1] = d.seq;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ Digest kernels
 __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restrict__ data, const uint64_t *__restrict__ off, uint64_t fixed_len,
                                                           size_t n, uint32_t *__restrict__ out) {
@@ -1991,6 +2063,19 @@ static cudaError_t launch_queue_digests(hs_ctx *c, const ring_bufs &r, const qms
   c->launches++;
   return cudaGetLastError();
 }
+// The explain lane's share of the device: at most one block of HS_THREADS per HS_QUEUE_EXPLAIN_SM_DIV multiprocessors (33 blocks, 4,224
+// records in flight, on a 132-SM H100).  A k_queue_explain block holds its SM's registers for a whole re-check (about 1.4 ms), so a
+// large explain launch takes at most that share of the SMs from the verify launches; more records run grid-stride, one wave after another.
+#define HS_QUEUE_EXPLAIN_SM_DIV 4
+// k_queue_explain over the n records of the n_desc requests in list, reading their regions from mirror, writing why bytes and
+// completion words into the mapped arena.
+static cudaError_t launch_queue_explain(hs_ctx *c, const xq_desc *list, uint32_t n_desc, uint32_t n, uint8_t *mirror, uint8_t *arena,
+                                        cudaStream_t s) {
+  const unsigned grid = (unsigned)std::min<size_t>(blocks_for(n), std::max<size_t>(1, c->n_sms / HS_QUEUE_EXPLAIN_SM_DIV));
+  k_queue_explain<<<grid, HS_THREADS, 0, s>>>(list, n_desc, n, mirror, arena);
+  c->launches++;
+  return cudaGetLastError();
+}
 
 // ---- latency path (host side)
 // key bytes -> table index through the host mirror of the device hash table (registered committee or learned cache)
@@ -2167,6 +2252,14 @@ struct batch_lane {
   stream_h stream, side;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
   event_h ev[2];
 };
+// The explain lane's arena, its device mirror, the launch's request list and its stream (hs_queue_explain builds them whole, or not at
+// all).
+struct explain_lane {
+  mapped<uint8_t> arena;    // request regions (records and preimages, then why bytes and the tail)
+  dev_mem<uint8_t> mirror;  // the regions of the launch in flight, at the same offsets (k_queue_explain reads them and counts in them)
+  mapped<xq_desc> list;     // the launch's requests
+  stream_h stream;          // the device's lowest priority
+};
 struct hs_queue {
   hs_ctx *c = nullptr;
   uint32_t cap = 0, mask = 0;
@@ -2243,6 +2336,27 @@ struct hs_queue {
   uint32_t b_seq = 0;
   uint64_t bstats[HS_QUEUE_BATCH_STATS] = {};  // hs_queue_batch_stats
   std::mutex b_cfg_mu;                          // serialises hs_queue_batch calls
+  // explain lane (hs_queue_explain): off while x_max_records is 0.  Requests wait in xq in submit order, each with a region of the
+  // mapped arena xlane.arena (x_arena), filled outside q->mu and launchable once `ready`.  One k_queue_explain launch is in flight at a
+  // time: the first x_launched requests of xq (dispatcher thread; set and cleared under q->mu).  Each completes as soon as its
+  // completion word is up; the launch's regions are released, and its requests leave xq, when all of them have.  The lane's buffers and
+  // stream change only while the lane is off and xq is empty.
+  struct xreq {
+    ticket_sink sink;
+    uint32_t n, m, pre_bytes;
+    uint64_t a_off, a_pos, a_end;  // region offset in the arena; arena positions of its start and past its end
+    uint32_t seq;                  // the completion word k_queue_explain writes (set at launch)
+    bool ready, done;
+  };
+  size_t x_max_records = 0, x_max_bytes = 0;
+  byte_ring x_arena;
+  explain_lane xlane;
+  std::deque<xreq> xq;
+  size_t x_launched = 0;    // requests of the launch in flight (0: none)
+  uint64_t x_launch_recs = 0;
+  uint32_t x_seq = 0;
+  uint64_t xstats[HS_QUEUE_EXPLAIN_STATS] = {};  // hs_queue_explain_stats
+  std::mutex x_cfg_mu;                           // serialises hs_queue_explain calls
   uint64_t head = 0, launched = 0, tail = 0;
   size_t next_ticket = 1;
   uint32_t seq = 0;
@@ -2609,11 +2723,13 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
 // included — has its word.  Every 4,096 passes both streams are queried: a CUDA error, or a drained stream with a word still
 // missing in a launch it ran, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
 static void batch_watch(hs_queue *q, bool query);
+static void explain_watch(hs_queue *q, bool query);
 static void queue_watch(hs_queue *q) {
   std::vector<queue_completion> fire;
   cudaError_t qes[2] = {cudaErrorNotReady, cudaErrorNotReady};  // [0] stream, [1] bulk_stream: a launch is judged by its own
   const bool query = (++q->spins & 0xfff) == 0;
   batch_watch(q, query);
+  explain_watch(q, query);
   if (query) {  // queried BEFORE the words are read
     qes[0] = cudaStreamQuery(q->stream);
     qes[1] = cudaStreamQuery(q->bulk_stream);
@@ -2775,6 +2891,101 @@ static void batch_drain(hs_queue *q) {
   if (q->lane.side) cudaStreamSynchronize(q->lane.side);
 }
 
+// ---- explain lane (hs_queue_submit_explain, hs_queue_submit_explain_msgs): k_queue_explain over every ready request, on the lane's stream
+// An explain ticket's bits: the why bytes packed four to a word, little-endian.
+static uint32_t explain_bits(uint64_t n) { return (uint32_t)(32 * ((n + 3) / 4)); }
+static bool explain_ready_locked(const hs_queue *q) { return !q->x_launched && !q->xq.empty() && q->xq.front().ready; }
+// Retires the launch in flight once every request of it has completed and their callbacks have run (under q->mu): counts it when it ran
+// (ok), releases its regions and drops its requests.  hs_queue_explain waits for xq to empty, so a resize returns after the callbacks.
+static void explain_retire_locked(hs_queue *q, bool ok) {
+  if (ok) {
+    q->xstats[0]++;
+    q->xstats[1] += q->x_launch_recs;
+    q->xstats[2] += q->x_launched;
+  }
+  q->x_arena.release_to(q->xq[q->x_launched - 1].a_end);
+  q->xq.erase(q->xq.begin(), q->xq.begin() + (long)q->x_launched);
+  q->x_launched = 0;
+  q->cv_done.notify_all();  // for callback tickets too: hs_queue_explain waits for xq to drain
+}
+// One launch takes every ready request at the front of xq.  Their regions are one span of arena positions, which crosses the bus in at
+// most two copies (the span may wrap once) into the mirror; the context's mutex is held only while the copies and the launch are
+// enqueued, and the launch reads no context table, so nothing else of the context waits for it.
+static void explain_dispatch(hs_queue *q) {
+  hs_ctx *c = q->c;
+  uint32_t k = 0;
+  uint64_t recs = 0, p0 = 0, p1 = 0;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    const uint32_t seq = ++q->x_seq ? q->x_seq : ++q->x_seq;  // never 0: the regions' tails were zeroed at submit
+    for (; k < q->xq.size() && q->xq[k].ready; k++) {
+      hs_queue::xreq &r = q->xq[k];
+      r.seq = seq;
+      q->xlane.list.h[k] = xq_desc{r.a_off, r.n, (uint32_t)recs, r.m, r.pre_bytes, seq, 0};
+      recs += r.n;
+    }
+    q->x_launched = k;
+    q->x_launch_recs = recs;
+    p0 = q->xq.front().a_pos;
+    p1 = q->xq[k - 1].a_end;
+  }
+  cudaError_t e;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    cudaStream_t s = q->xlane.stream;
+    const uint64_t o0 = q->x_arena.off(p0), first = std::min(p1 - p0, q->x_arena.cap - o0);
+    e = cudaMemcpyAsync(q->xlane.mirror + o0, q->xlane.arena.h + o0, first, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && p1 - p0 > first) e = cudaMemcpyAsync(q->xlane.mirror.get(), q->xlane.arena.h, p1 - p0 - first, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = launch_queue_explain(c, q->xlane.list.d, k, (uint32_t)recs, q->xlane.mirror, q->xlane.arena.d, s);
+    if (e != cudaSuccess) fail(c, HS_ERR_CUDA, "verify queue explain launch", e);
+  }
+  if (e == cudaSuccess) return;
+  std::vector<queue_completion> fire;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    for (uint32_t i = 0; i < k; i++) ticket_close_locked(q, q->xq[i].sink, HS_ERR_CUDA, explain_bits(q->xq[i].n), nullptr, fire);
+  }
+  queue_fire(fire);
+  std::lock_guard<std::mutex> g(q->mu);
+  explain_retire_locked(q, false);
+}
+// Completes each request of the launch in flight whose completion word carries the launch's number.  When `query`, the lane's stream is
+// queried first: a CUDA error, or a drained stream with a word still missing, completes the open requests with HS_ERR_CUDA (never an
+// explanation).
+static void explain_watch(hs_queue *q, bool query) {
+  if (!q->x_launched) return;  // (set and cleared on this thread)
+  cudaError_t qe = query ? cudaStreamQuery(q->xlane.stream) : cudaErrorNotReady;
+  if (qe != cudaSuccess && qe != cudaErrorNotReady) fail(q->c, HS_ERR_CUDA, "verify queue explain launch", qe);
+  std::vector<queue_completion> fire;
+  bool open = false, ok = true;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    for (size_t k = 0; k < q->x_launched; k++) {
+      hs_queue::xreq &r = q->xq[k];
+      if (r.done) continue;
+      const xq_layout L = xq_layout_of(r.n, r.m, r.pre_bytes);
+      const uint8_t *a = q->xlane.arena.h + r.a_off;
+      if (reinterpret_cast<const volatile uint32_t *>(a + L.o_tail)[1] == r.seq) {
+        std::atomic_thread_fence(std::memory_order_acquire);
+        ticket_close_locked(q, r.sink, HS_OK, explain_bits(r.n), reinterpret_cast<const uint32_t *>(a + L.o_why), fire);
+        r.done = true;
+      } else if (qe == cudaErrorNotReady) {
+        open = true;
+      } else {
+        if (qe == cudaSuccess) fail(q->c, HS_ERR_CUDA, "verify queue: k_queue_explain did not complete");
+        ticket_close_locked(q, r.sink, HS_ERR_CUDA, explain_bits(r.n), nullptr, fire);
+        r.done = true;
+        ok = false;
+      }
+    }
+  }
+  queue_fire(fire);
+  if (!open) {
+    std::lock_guard<std::mutex> g(q->mu);
+    explain_retire_locked(q, ok);
+  }
+}
+
 static size_t queue_small_inflight_locked(const hs_queue *q) {
   size_t k = 0;
   for (const hs_queue::launch &L : q->inflight) k += !L.bulk;
@@ -2805,6 +3016,10 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       batch_dispatch(q);
       lk.lock();
+    } else if (explain_ready_locked(q)) {  // the same for the explain lane
+      lk.unlock();
+      explain_dispatch(q);
+      lk.lock();
     } else if ((q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) || queue_generic_ready_locked(q)) {
       // everything pending; only the waiting generic requests while the small launches are at their limit
       const uint64_t lo = q->launched, hi = queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT ? q->tail : lo;
@@ -2812,11 +3027,11 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_dispatch(q, lo, hi);
       lk.lock();
-    } else if (!q->inflight.empty() || q->b_cur) {
+    } else if (!q->inflight.empty() || q->b_cur || q->x_launched) {
       lk.unlock();
       queue_watch(q);
       lk.lock();
-    } else if (q->stop && q->bq.empty()) {  // (a batch request still being copied in is announced on cv_work)
+    } else if (q->stop && q->bq.empty() && q->xq.empty()) {  // (a batch or explain request still being copied in is announced on cv_work)
       break;
     } else {
       q->cv_work.wait(lk);
@@ -2836,6 +3051,7 @@ static void queue_free(hs_queue *q) {
   if (q->ev_last) cudaEventSynchronize(q->ev_last);
   if (q->ev_bulk_last) cudaEventSynchronize(q->ev_bulk_last);
   batch_drain(q);
+  if (q->xlane.stream) cudaStreamSynchronize(q->xlane.stream);
   delete q;  // the owners release the rest
 }
 
@@ -4150,6 +4366,110 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
 
 int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]) {
   return queue_read_stats(q, "hs_queue_batch_stats", out, &hs_queue::bstats);
+}
+
+#define HS_QUEUE_EXPLAIN_MAX_RECORDS (1u << 24)
+#define HS_QUEUE_EXPLAIN_MAX_BYTES (1ull << 30)
+int hs_queue_explain(hs_queue *q, size_t max_records, size_t max_bytes) {
+  if (!q || (max_records == 0) != (max_bytes == 0) || max_records > HS_QUEUE_EXPLAIN_MAX_RECORDS || max_bytes > HS_QUEUE_EXPLAIN_MAX_BYTES)
+    return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_explain: bad argument");
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> cfg(q->x_cfg_mu);
+  {
+    std::unique_lock<std::mutex> lk(q->mu);
+    if (max_records == q->x_max_records && max_bytes == q->x_max_bytes) return HS_OK;
+    q->x_max_records = q->x_max_bytes = 0;  // refuses new explain requests while the lane changes
+    q->cv_done.wait(lk, [q] { return q->xq.empty(); });
+  }
+  HS_CUDA(c, cudaSetDevice(c->device));
+  if (q->xlane.stream) HS_CUDA(c, cudaStreamSynchronize(q->xlane.stream));
+  q->xlane = {};  // released before the new lane is allocated
+  q->x_arena = byte_ring{};
+  if (!max_records) return HS_OK;
+  uint64_t acap = 4096;  // two of the largest regions fit: one can be filled while the other's launch runs
+  while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
+  const uint64_t max_reqs = acap / xq_layout_of(1, 0, 0).size + 1;  // regions the arena holds at once
+  explain_lane X;
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = create(X.stream, lo);
+  if (e == cudaSuccess) e = alloc(X.arena, acap);
+  if (e == cudaSuccess) e = alloc(X.mirror, acap);
+  if (e == cudaSuccess) e = alloc(X.list, max_reqs * sizeof(xq_desc));
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, HS_ERR_NOMEM, "hs_queue_explain: no pinned host or device memory for the explain lane", e);
+  }
+  memset(X.arena.h, 0, acap);
+  q->xlane = std::move(X);
+  std::lock_guard<std::mutex> g(q->mu);
+  q->x_arena = byte_ring{acap, 0, 0};
+  q->x_max_records = max_records;
+  q->x_max_bytes = max_bytes;
+  return HS_OK;
+}
+
+// Submits one explain request of n records whose region is laid out by L: under q->mu the request takes its region, then fill(region)
+// writes its records (and preimages) without the lock, and the request becomes ready.
+extern "C++" {
+template <class Fill>
+static int explain_submit(hs_queue *q, const char *what, size_t n, uint64_t m, uint64_t pre_bytes, ticket_sink sink, size_t *out_ticket, Fill fill) {
+  const xq_layout L = xq_layout_of(n, m, pre_bytes);
+  hs_queue::xreq *r = nullptr;
+  const int rc = queue_submit(q, what, sink, explain_bits(n), out_ticket, [&](const ticket_sink &s) {
+    if (!q->x_max_records) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": the explain lane is off (hs_queue_explain)").c_str());
+    if (n > q->x_max_records || L.size > q->x_max_bytes)
+      return fail(q->c, HS_ERR_ARG, (std::string(what) + ": larger than the explain lane's limits").c_str());
+    const std::optional<uint64_t> start = q->x_arena.take(L.size);
+    if (!start) return HS_ERR_NOMEM;
+    q->x_arena.tail = *start + L.size;
+    q->xq.push_back(hs_queue::xreq{s, (uint32_t)n, (uint32_t)m, (uint32_t)pre_bytes, q->x_arena.off(*start), *start, q->x_arena.tail, 0, false, false});
+    r = &q->xq.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
+    return HS_OK;
+  });
+  if (rc != HS_OK) return rc;
+  uint8_t *a = q->xlane.arena.h + r->a_off;
+  fill(a, L);
+  memset(a + L.o_why, 0, L.size - L.o_why);  // why bytes (the last word's unused bytes stay 0), the count and the completion word
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    r->ready = true;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
+}  // extern "C++"
+
+int hs_queue_submit_explain(hs_queue *q, const hs_rec128 *recs, size_t n, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !recs || n == 0 || n > HS_QUEUE_EXPLAIN_MAX_RECORDS) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_explain: bad argument");
+  return explain_submit(q, "hs_queue_submit_explain", n, 0, 0, ticket_sink{0, cb, user}, out_ticket,
+                        [&](uint8_t *a, const xq_layout &) { memcpy(a, recs, n * sizeof(hs_rec128)); });
+}
+
+int hs_queue_submit_explain_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
+                                 const uint32_t *msg_idx, size_t n, hs_queue_cb *cb, void *user, size_t *out_ticket) {
+  if (!q || !pre_off || !sig || !pk || !msg_idx || n == 0 || n > HS_QUEUE_EXPLAIN_MAX_RECORDS || n_msgs == 0 || n_msgs > UINT32_MAX)
+    return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_explain_msgs: bad argument");
+  if (!offsets_ok(pre_off, n_msgs) || (pre_off[n_msgs] && !preimages) || pre_off[n_msgs] > HS_QUEUE_EXPLAIN_MAX_BYTES)
+    return fail(q->c, HS_ERR_ARG, "hs_queue_submit_explain_msgs: bad preimage offsets");
+  for (size_t i = 0; i < n; i++)
+    if (msg_idx[i] >= n_msgs) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_explain_msgs: message index out of range");
+  const uint64_t pre_bytes = pre_off[n_msgs];
+  return explain_submit(q, "hs_queue_submit_explain_msgs", n, n_msgs, pre_bytes, ticket_sink{0, cb, user}, out_ticket,
+                        [&](uint8_t *a, const xq_layout &L) {
+                          for (size_t i = 0; i < n; i++) {
+                            memcpy(a + 128 * i, sig + 64 * i, 64);
+                            memcpy(a + 128 * i + 64, pk + 32 * i, 32);
+                            memset(a + 128 * i + 96, 0, 32);
+                          }
+                          memcpy(a + L.o_off, pre_off, 8 * (n_msgs + 1));
+                          memcpy(a + L.o_mi, msg_idx, 4 * n);
+                          if (pre_bytes) memcpy(a + L.o_pre, preimages, pre_bytes);
+                        });
+}
+
+int hs_queue_explain_stats(hs_queue *q, uint64_t out[HS_QUEUE_EXPLAIN_STATS]) {
+  return queue_read_stats(q, "hs_queue_explain_stats", out, &hs_queue::xstats);
 }
 
 void hs_queue_destroy(hs_queue *q) {

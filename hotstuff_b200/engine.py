@@ -489,6 +489,10 @@ class MultiEngine:
                               mode, pk, validator_idx, want_items)
 
 
+class _WhyCount(int):
+    """The record count of an explain ticket: its words hold one why byte per record, four to a word."""
+
+
 class VerifyQueue:
     """hs_queue_* (include/hs_crypto.h): submit 1..64 records (submit) or a whole certificate (submit_group, or submit_msgs with the
     signed preimages instead of their Digests) without blocking;
@@ -518,11 +522,16 @@ class VerifyQueue:
 
     @staticmethod
     def _n_words(n):
-        """Words of a ticket's verdict bitmap: n is a record count, or (n_groups, n_items) for a batch ticket."""
+        """Words of a ticket's verdict bitmap: n is a record count, or (n_groups, n_items) for a batch ticket (the why bytes of an
+        explain ticket: (n + 3) / 4 words)."""
+        if isinstance(n, _WhyCount):
+            return (n + 3) // 4
         return (n[0] + 31) // 32 + (n[1] + 31) // 32 if isinstance(n, tuple) else (n + 31) // 32
 
     @staticmethod
     def _bools(words, n):
+        if isinstance(n, _WhyCount):  # an explain ticket: one HS_WHY_* byte per record
+            return words.view(np.uint8)[:n].copy()
         if isinstance(n, tuple):  # a batch ticket: group words, then item words
             gw = (n[0] + 31) // 32
             return bitmap_to_bools(words[:gw], n[0]), bitmap_to_bools(words[gw:], n[1])
@@ -596,6 +605,46 @@ class VerifyQueue:
         self.engine._check(self.lib.hs_queue_batch_stats(self.h, out), "hs_queue_batch_stats")
         return dict(zip(self.BATCH_STATS, (int(x) for x in out)))
 
+    def explain(self, max_records, max_bytes):
+        """Turns the explain lane on (hs_queue_explain): submit_explain / submit_explain_msgs requests of up to max_records records and
+        max_bytes of arena region each.  (0, 0) turns it off (the default).  Resizing or turning it off first waits for every explain
+        request already submitted."""
+        self.engine._check(self.lib.hs_queue_explain(self.h, int(max_records), int(max_bytes)), "hs_queue_explain")
+
+    def submit_explain(self, recs, callback=None):
+        """Engine.explain as ONE non-blocking request on the explain lane (hs_queue_submit_explain).  recs: (n,128) uint8.  poll / wait /
+        the callback give uint8[n] of HS_WHY_* masks, byte for byte those of Engine.explain.  Returns the ticket, or None when the lane's
+        arena has no room now (back-pressure)."""
+        recs = _u8(recs, 128).reshape(-1, 128)
+        n = recs.shape[0]
+        return self._enqueue("hs_queue_submit_explain", _WhyCount(n), callback,
+                             lambda cb, user, t: self.lib.hs_queue_submit_explain(self.h, _ptr(recs) if n else None, n, cb, user, t))
+
+    def submit_explain_msgs(self, preimages, pre_off, sig, pk, msg_idx, callback=None):
+        """The same with the signed preimages instead of their Digests (hs_queue_submit_explain_msgs), in the arrays of submit_msgs
+        without modes: record i is (sig[i], pk[i]) over SHA-512(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1]))[..32], hashed
+        on the GPU.  Returns the ticket, or None when the lane's arena has no room now."""
+        pre = _u8(preimages)
+        off = np.ascontiguousarray(pre_off, dtype=np.uint64).reshape(-1)
+        sig = _u8(sig, 64).reshape(-1, 64)
+        pk = _u8(pk, 32).reshape(-1, 32)
+        mi = np.ascontiguousarray(msg_idx, dtype=np.uint32).reshape(-1)
+        n = sig.shape[0]
+        if pk.shape[0] != n or mi.shape[0] != n or off.shape[0] < 1:
+            raise ValueError("submit_explain_msgs: %d signatures, %d keys, %d message indices, %d offsets" % (n, pk.shape[0], mi.shape[0], off.shape[0]))
+        return self._enqueue("hs_queue_submit_explain_msgs", _WhyCount(n), callback, lambda cb, user, t: self.lib.hs_queue_submit_explain_msgs(
+            self.h, _ptr(pre) if pre.size else None, _ptr(off), off.shape[0] - 1, _ptr(sig) if n else None, _ptr(pk) if n else None,
+            _ptr(mi) if n else None, n, cb, user, t))
+
+    EXPLAIN_STATS = ("launches", "records", "requests")
+
+    def explain_stats(self):
+        """Counters of completed explain launches (hs_queue_explain_stats): k_queue_explain launches, the records they carried, and the
+        requests."""
+        out = (ctypes.c_uint64 * len(self.EXPLAIN_STATS))()
+        self.engine._check(self.lib.hs_queue_explain_stats(self.h, out), "hs_queue_explain_stats")
+        return dict(zip(self.EXPLAIN_STATS, (int(x) for x in out)))
+
     def _submit(self, fn, name, recs, mode_arg, callback):
         recs = _u8(recs, 128).reshape(-1, 128)
         n = recs.shape[0]
@@ -636,8 +685,8 @@ class VerifyQueue:
         return np.zeros(max(2, self._n_words(n)), dtype=np.uint32)
 
     def poll(self, ticket):
-        """None while the request is in flight, else its verdicts (bool[n]; a batch ticket: (group bools, item bools)); consumes the
-        ticket."""
+        """None while the request is in flight, else its verdicts (bool[n]; a batch ticket: (group bools, item bools); an explain
+        ticket: uint8[n] of why masks); consumes the ticket."""
         done = ctypes.c_int(0)
         words = self._words(ticket)
         rc = self.lib.hs_queue_poll(self.h, int(ticket), ctypes.byref(done), _ptr(words))
@@ -646,8 +695,8 @@ class VerifyQueue:
         return self._take(ticket, rc, words)
 
     def wait(self, ticket):
-        """Blocks until the request is done; returns its verdicts (bool[n]; a batch ticket: (group bools, item bools)) and consumes
-        the ticket."""
+        """Blocks until the request is done; returns its verdicts (bool[n]; a batch ticket: (group bools, item bools); an explain
+        ticket: uint8[n] of why masks) and consumes the ticket."""
         words = self._words(ticket)
         rc = self.lib.hs_queue_wait(self.h, int(ticket), _ptr(words))
         return self._take(ticket, rc, words)

@@ -328,6 +328,41 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
 /* Counters of completed batch passes: [0] batch passes, [1] items, [2] groups, [3] preimage bytes hashed, [4] items whose key was
  * outside the committee (every item when no committee is registered) */
 int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]);
+/* Explain lane: hs_explain_rec128 as a non-blocking queue request, for the records of a message a node has already seen rejected.  The
+ * synchronous call holds the context's mutex for its whole re-check (about 1.4 ms), and every queue launch needs that mutex to enqueue;
+ * the lane holds it only while its launch is enqueued, so explaining junk from a peer no longer holds up the votes.
+ *   - One k_queue_explain launch takes every explain request pending when it is launched (a thread per record, the re-check of
+ *     hs_explain_rec128), on the lane's own stream at the device's lowest priority; at most one is in flight, and it does not count
+ *     against the two small launches in flight.  Its grid is at most one block of 128 threads per 4 SMs (33 blocks, 4,224 records per
+ *     wave on a 132-SM H100), grid-stride beyond that, so a large request leaves three quarters of the SMs to the verify launches.
+ *   - The lane reads no context table (no comb table, key slot, key flag or hash table, and not the base-point table) and takes no ring
+ *     slot: explain records live in the lane's own mapped arena.  Committee changes, audits and repairs therefore neither drain it nor
+ *     change its answers.
+ *   - Isolation: explain requests take no part in the certificate or signature caches, do not teach the key cache and do not move
+ *     hs_queue_stats, hs_queue_digest_stats, hs_queue_generic_stats or hs_queue_batch_stats.  hs_queue_destroy completes every explain
+ *     request in flight (callbacks fire).
+ * max_records / max_bytes bound one request (records; bytes of its arena region: 128 per record, plus for the preimage form the offsets,
+ * indices and preimage bytes, plus the why bytes, each section rounded up to 16, plus 16).  0, 0 = off (the default: the queue launches
+ * exactly the kernels it launches without this call).  Resizing or turning it off first waits for every explain request already
+ * submitted.  HS_ERR_NOMEM: no pinned host or device memory (the lane is then off). */
+int hs_queue_explain(hs_queue *q, size_t max_records, size_t max_bytes);
+/* hs_explain_rec128(ctx, recs, n, ..) as ONE non-blocking queue request: the mask of record i is byte for byte what that call returns.
+ * Completion, tickets, poll / wait / callback work as for hs_queue_submit_group, but the uint32_t words hold the why bytes packed
+ * little-endian: byte i (bits 8 (i & 3) .. 8 (i & 3) + 7 of word i >> 2) is record i's HS_WHY_* mask, and there are (n + 3) / 4 words
+ * (unused bytes of the last word are 0).  A failed request (status HS_ERR_CUDA) has all-zero words: it explains nothing.
+ * HS_ERR_ARG: the lane is off, n = 0, NULL recs, or more records or region bytes than the lane's limits.  HS_ERR_NOMEM: no arena room
+ * right now (back-pressure: explain later, or not at all).  An explanation is advisory: a refused request never changes a verdict. */
+int hs_queue_submit_explain(hs_queue *q, const hs_rec128 *recs, size_t n, hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
+/* The same with the signed preimages instead of their Digests, in the arrays of hs_queue_submit_msgs without the modes: record i is
+ * (sig[i], pk[i]) over Digest = SHA-512(preimages[pre_off[msg_idx[i]] .. pre_off[msg_idx[i] + 1]))[..32], hashed on the GPU by the
+ * record's own thread.  Its mask equals hs_explain_rec128 on the record built with that Digest.  HS_ERR_ARG as hs_queue_submit_explain,
+ * and for the checks of hs_queue_submit_msgs: bad offsets, n_msgs = 0, msg_idx[i] >= n_msgs. */
+int hs_queue_submit_explain_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off /* n_msgs + 1 */, size_t n_msgs,
+                                 const uint8_t *sig /* n x 64 */, const uint8_t *pk /* n x 32 */, const uint32_t *msg_idx /* n */, size_t n,
+                                 hs_queue_cb *cb_or_null, void *user, size_t *out_ticket);
+#define HS_QUEUE_EXPLAIN_STATS 3
+/* Counters of completed explain launches: [0] k_queue_explain launches, [1] records, [2] requests */
+int hs_queue_explain_stats(hs_queue *q, uint64_t out[HS_QUEUE_EXPLAIN_STATS]);
 void hs_queue_destroy(hs_queue *q);
 
 /* ---- Digest surface: out[i] = SHA-512(data[off[i] .. off[i+1]))[0..32] ------------------------------------------ */

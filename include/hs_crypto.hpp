@@ -294,8 +294,60 @@ class VerifyQueue {
     e_.check(hs_queue_batch_stats(q_, s.data()), "hs_queue_batch_stats");
     return s;
   }
+  // hs_queue_explain: turn the explain lane on for requests of up to max_records records and max_bytes of arena region (0, 0 = off,
+  // the default).  Resizing or turning it off first waits for the explain requests already submitted.
+  void explain(size_t max_records, size_t max_bytes) { e_.check(hs_queue_explain(q_, max_records, max_bytes), "hs_queue_explain"); }
+  // Engine::explain as ONE non-blocking request on the explain lane (hs_queue_submit_explain).  The future yields one HS_WHY_* byte per
+  // record, byte for byte those of hs_explain_rec128, or throws EngineError on an engine failure (explain nothing).  Throws QueueFull
+  // when the lane's arena has no room now, EngineError on a bad argument or when the lane is off.
+  std::future<std::vector<uint8_t>> submit_explain(const hs_rec128 *recs, size_t n) {
+    auto *p = new WhyPending{std::promise<std::vector<uint8_t>>(), n};
+    std::future<std::vector<uint8_t>> f = p->promise.get_future();
+    const int rc = hs_queue_submit_explain(q_, recs, n, &VerifyQueue::why_done, p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit_explain");
+    }
+    return f;
+  }
+  // The same with the signed preimages instead of their Digests (hs_queue_submit_explain_msgs): the arrays of submit_msgs without modes.
+  std::future<std::vector<uint8_t>> submit_explain_msgs(const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig,
+                                                        const uint8_t *pk, const uint32_t *msg_idx, size_t n) {
+    auto *p = new WhyPending{std::promise<std::vector<uint8_t>>(), n};
+    std::future<std::vector<uint8_t>> f = p->promise.get_future();
+    const int rc = hs_queue_submit_explain_msgs(q_, preimages, pre_off, n_msgs, sig, pk, msg_idx, n, &VerifyQueue::why_done, p, nullptr);
+    if (rc != HS_OK) {
+      delete p;
+      if (rc == HS_ERR_NOMEM) throw QueueFull();
+      e_.check(rc, "hs_queue_submit_explain_msgs");
+    }
+    return f;
+  }
+  // hs_queue_explain_stats: [0] k_queue_explain launches, [1] records they carried, [2] requests.
+  std::array<uint64_t, HS_QUEUE_EXPLAIN_STATS> explain_stats() const {
+    std::array<uint64_t, HS_QUEUE_EXPLAIN_STATS> s{};
+    e_.check(hs_queue_explain_stats(q_, s.data()), "hs_queue_explain_stats");
+    return s;
+  }
 
  private:
+  struct WhyPending {
+    std::promise<std::vector<uint8_t>> promise;
+    size_t n;
+  };
+  // runs once per explain request on the queue's thread: the words hold the why bytes, byte i of the little-endian packing = record i
+  static void why_done(void *user, size_t, int status, const uint32_t *bitmap) {
+    WhyPending *p = static_cast<WhyPending *>(user);
+    if (status == HS_OK) {
+      std::vector<uint8_t> v(p->n);
+      for (size_t i = 0; i < p->n; i++) v[i] = (uint8_t)(bitmap[i >> 2] >> (8 * (i & 3)));
+      p->promise.set_value(std::move(v));
+    } else {
+      p->promise.set_exception(std::make_exception_ptr(EngineError("verify queue explain: engine failure (status " + std::to_string(status) + ")")));
+    }
+    delete p;
+  }
   struct BatchPending {
     std::promise<BatchVerdicts> promise;
     size_t n_items, n_groups;

@@ -42,6 +42,10 @@ pub mod generic_queue;
 /// awaited by a task instead of run under `spawn_blocking` (`batch_queue::verify_groups_queued`).
 #[path = "crypto_gpu_batch_queue.rs"]
 pub mod batch_queue;
+/// The queue's explain lane (hs_queue_submit_explain): every rejected record of a rejected message explained in one non-blocking
+/// request, without holding the context's mutex for the re-check (`explain_queue::explain_rejected_queued`).
+#[path = "crypto_gpu_explain_queue.rs"]
+pub mod explain_queue;
 /// The device-resident certificate pass (hs_verify_groups_dev): Blocks, Timeouts and TCs whose arrays are already in HBM, enqueued on
 /// the caller's stream (`groups_dev::verify_groups_dev`).
 #[path = "crypto_gpu_groups_dev.rs"]

@@ -30,6 +30,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <deque>
+#include <type_traits>
 #include <initializer_list>
 #include <list>
 #include <memory>
@@ -1007,22 +1008,24 @@ __global__ void __launch_bounds__(HS_THREADS) k_verify_finish_modes(in_layout L,
 }
 
 // ------------------------------------------------------------------------------------------------ table construction
-// thread = (point p, window w, block b of HS_BUILD_BLOCK entries)
+// thread = (point p, window w, block b of HS_BUILD_BLOCK entries).  slots (nullable): point p is slot slots[p], its key at encs + 32
+// slots[p] and its table at slot slots[p] of `tables`; its flag byte still goes to key_flags[p].  Without a list, slot p.
 #define HS_BUILD_BLOCK 64
-__global__ void __launch_bounds__(HS_THREADS) k_build_comb(const uint8_t *__restrict__ encs, size_t n_points, int negate, int W, int n_windows,
-                                                            ge_niels *tables, uint8_t *key_flags) {
+__global__ void __launch_bounds__(HS_THREADS) k_build_comb(const uint8_t *__restrict__ encs, const uint32_t *__restrict__ slots, size_t n_points,
+                                                            int negate, int W, int n_windows, ge_niels *tables, uint8_t *key_flags) {
   const int entries = 1 << (W - 1);
   const int blocks_per_window = entries / HS_BUILD_BLOCK;
   const size_t t = (size_t)blockIdx.x * HS_THREADS + threadIdx.x;
   const size_t per_point = (size_t)n_windows * blocks_per_window;
   const size_t p = t / per_point;
   if (p >= n_points) return;
+  const size_t s = slots ? slots[p] : p;
   const int w = (int)((t % per_point) / blocks_per_window);
   const int b = (int)(t % blocks_per_window);
   ge_ext P;
   if (encs) {
     uint32_t e[8];
-    load32(e, encs + p * 32);
+    load32(e, encs + s * 32);
     uint32_t ok = ge_decompress(P, e);
     uint32_t small = ge_enc_is_small_order(e);
     if (w == 0 && b == 0 && key_flags) key_flags[p] = (uint8_t)((ok & 1u) | (small << 1));
@@ -1036,7 +1039,7 @@ __global__ void __launch_bounds__(HS_THREADS) k_build_comb(const uint8_t *__rest
     P = Q;
   }
   fe prod[HS_BUILD_BLOCK];
-  comb_build_block(tables + p * ((size_t)n_windows * comb_window_stride(W)), P, W, w, b * HS_BUILD_BLOCK, HS_BUILD_BLOCK, prod);
+  comb_build_block(tables + s * ((size_t)n_windows * comb_window_stride(W)), P, W, w, b * HS_BUILD_BLOCK, HS_BUILD_BLOCK, prod);
 }
 
 // ------------------------------------------------------------------------------------------------ table audit (hs_table_audit)
@@ -1100,20 +1103,25 @@ __global__ void __launch_bounds__(256) k_slot_audit(key_table T, const uint8_t *
 // TABLE / BASE: a warp per run of 32 consecutive entries of one window of one table, lane l entry first + l (coalesced 96-byte loads);
 // entry m - 1 comes from lane l - 1 by shuffles, and entry 1 of the window is one broadcast load.  The lane of entry 1 also checks the
 // window link, or for window 0 the anchor.  pks == nullptr: one table, the base-point table (anchor B); otherwise table s is slot s's,
-// anchored on -A of its stored bytes, and only the slots k_slot_audit marked auditable are read.  Short blocks: the lowest-priority
-// stream's blocks give way to verify launches at every block boundary.
+// anchored on -A of its stored bytes, and only the slots k_slot_audit marked auditable are read.  LISTED: table t is slot slots[t]'s
+// (key bytes and table), with auditable[t] and the findings at list position t; otherwise slot t's, and `slots` is not read (the full
+// audit keeps the code it had before the list).  Short blocks: the lowest-priority stream's blocks give way to verify launches at every
+// block boundary.
 #define HS_AUDIT_WARPS 4
-__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, size_t n_tables, size_t table_entries,
-                                                                       int W, int n_windows, const uint8_t *__restrict__ pks,
-                                                                       const uint8_t *__restrict__ auditable, audit_out O) {
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, const uint32_t *__restrict__ slots,
+                                                                       size_t n_tables, size_t table_entries, int W, int n_windows,
+                                                                       const uint8_t *__restrict__ pks, const uint8_t *__restrict__ auditable,
+                                                                       audit_out O) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t H = (uint64_t)1 << (W - 1), runs = (H + 1 + 31) / 32;
   const uint64_t g = (uint64_t)blockIdx.x * HS_AUDIT_WARPS + (threadIdx.x >> 5);
   const uint64_t t = g / (runs * n_windows);
   if (t >= n_tables || (pks && !auditable[t])) return;  // whole warps leave together
+  const uint64_t s = LISTED ? slots[t] : t;
   const uint32_t win = (uint32_t)((g / runs) % n_windows);
   const uint32_t m = (uint32_t)((g % runs) * 32 + lane);
-  const ge_niels *wt = tables + t * table_entries + (size_t)win * comb_window_stride(W);
+  const ge_niels *wt = tables + s * table_entries + (size_t)win * comb_window_stride(W);
   const bool in = m <= H;
   ge_niels e, prev, one;
   niels_load_stream(e, wt + (in ? m : H));
@@ -1128,7 +1136,7 @@ __global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_ni
   if (m == 1) {
     if (win == 0) {
       ge_ext P;
-      audit_anchor_point(P, pks ? reinterpret_cast<const uint32_t *>(pks + t * 32) : nullptr);
+      audit_anchor_point(P, pks ? reinterpret_cast<const uint32_t *>(pks + s * 32) : nullptr);
       ok &= audit_anchor(e, P);
     } else {
       ge_niels last;
@@ -1588,7 +1596,16 @@ struct peer_bufs {
   dev_mem<uint32_t> own;
   ipc_mapping mapped[HS_MAX_PEERS];
 };
-enum : uint8_t { SLOT_LIVE = 1, SLOT_REPAIR = 2 };  // hs_ctx::h_key_live values of a slot in use
+enum : uint8_t { SLOT_LIVE = 1, SLOT_REPAIR = 2, SLOT_STAGED = 3 };  // hs_ctx::h_key_live values of a slot in use
+// A staged committee change (hs_committee_stage): its slots are SLOT_STAGED in h_key_live, out of service, until the commit.
+struct committee_stage {
+  bool busy = false;            // the stage holds slots: being built, or built and proved
+  bool ready = false;           // built and proved: hs_committee_commit applies it
+  std::vector<uint32_t> fresh;  // the slots it took, lowest free first, then spares (those past n_keys are consecutive from it)
+  std::vector<uint8_t> keys;    // their key bytes (32 each)
+  std::vector<uint8_t> flags;   // their proved flag bytes
+  std::vector<uint32_t> remove; // the slots the commit takes out of service
+};
 struct hs_ctx {
   int device = 0;
   unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
@@ -1611,7 +1628,9 @@ struct hs_ctx {
   size_t cache_cap = 4096;           // keys
   std::vector<uint8_t> h_pks;        // host mirrors of keys.pks / keys.slots (key cache and hs_committee_update)
   key_index h_index;
-  std::vector<uint8_t> h_key_live;   // explicit committee: SLOT_LIVE, SLOT_REPAIR (live, out of service during hs_table_repair) or 0 = removed (free for reuse)
+  std::vector<uint8_t> h_key_live;   // explicit committee: SLOT_LIVE, SLOT_REPAIR (live, out of service during hs_table_repair), SLOT_STAGED
+                                     // (taken by a stage, past n_keys for a spare) or 0 = removed (free for reuse)
+  committee_stage stage;             // guarded by mu
   size_t table_budget = 0;           // bytes the per-key tables may use (0 = ~62 % of the device)
   size_t key_capacity = 0;           // explicit committee: table slots allocated (>= n_keys; spare slots serve hs_committee_update)
   learn_bufs learn;
@@ -1748,10 +1767,11 @@ static int launch_qc_and(hs_ctx *c, const uint32_t *d_items, const uint32_t *d_g
 }
 
 
-static int launch_build(hs_ctx *c, const uint8_t *d_encs, size_t n_points, int negate, int W, int n_windows, ge_niels *tables, uint8_t *flags,
-                        cudaStream_t stream) {
+// k_build_comb over n_points points: slots 0 .. n_points - 1 of d_encs / tables, or with d_slots the listed slots (flags by list position).
+static int launch_build(hs_ctx *c, const uint8_t *d_encs, const uint32_t *d_slots, size_t n_points, int negate, int W, int n_windows,
+                        ge_niels *tables, uint8_t *flags, cudaStream_t stream) {
   size_t threads = n_points * (size_t)n_windows * ((1u << (W - 1)) / HS_BUILD_BLOCK);
-  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(d_encs, n_points, negate, W, n_windows, tables, flags);
+  k_build_comb<<<blocks_for(threads), HS_THREADS, 0, stream>>>(d_encs, d_slots, n_points, negate, W, n_windows, tables, flags);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -1783,6 +1803,7 @@ static void cache_release(hs_ctx *c) {  // callers have synchronised the device
   c->h_pks.clear();
   c->h_index = {};
   c->h_key_live.clear();
+  c->stage = {};  // a registration discards a pending stage: its slots went with the store
   c->key_capacity = 0;
 }
 // lazily allocate the store for cache_cap learned keys (14-bit windows: 14 MB per key, narrower if memory is short)
@@ -1849,7 +1870,7 @@ static int learn_process(hs_ctx *c, cudaStream_t stream) {
   HS_TRY(audit_fence(c, stream));
   HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + old_n * 32, c->h_pks.data() + old_n * 32, n_new * 32, cudaMemcpyHostToDevice, stream));
   HS_CUDA(c, cudaMemcpyAsync(c->keys.slots, c->h_index.slots.data(), c->h_index.slots.size() * 4, cudaMemcpyHostToDevice, stream));
-  HS_TRY(launch_build(c, c->keys.pks + old_n * 32, n_new, 1, c->cp.wa, c->cp.na, c->keys.atables + old_n * c->a_table_entries,
+  HS_TRY(launch_build(c, c->keys.pks + old_n * 32, nullptr, n_new, 1, c->cp.wa, c->cp.na, c->keys.atables + old_n * c->a_table_entries,
                       c->keys.key_flags + old_n, stream));
   // (no synchronisation: copies from pageable memory return once the source is staged, so the host vectors may change afterwards)
   HS_CUDA(c, cudaEventRecord(c->learn.ev_tables, stream));  // passes on OTHER streams (host entry points vs a _dev caller's stream) wait for the build
@@ -3153,7 +3174,7 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
   c->cache_wanted = c->cache_enabled = !(flags & HS_FLAG_NO_KEY_CACHE) && !(getenv("HS_KEY_CACHE") && getenv("HS_KEY_CACHE")[0] == '0');
   if (e == cudaSuccess) e = alloc(c->d_btable, sizeof(ge_niels) * comb_table_entries(wb));
   if (e == cudaSuccess) {
-    if (launch_build(c, nullptr, 1, 0, wb, c->cp.nb, c->d_btable, nullptr, c->stream) != HS_OK) e = cudaGetLastError();
+    if (launch_build(c, nullptr, nullptr, 1, 0, wb, c->cp.nb, c->d_btable, nullptr, c->stream) != HS_OK) e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess) {
@@ -3283,7 +3304,7 @@ static int committee_register_locked(hs_ctx *c, const uint8_t *pks, size_t N, ui
   int rc = HS_OK;
   e = cudaMemcpyAsync(c->keys.pks, pks, N * 32, cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(c->keys.slots, index.slots.data(), index.slots.size() * 4, cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags, c->stream);
+  if (e == cudaSuccess) rc = launch_build(c, c->keys.pks, nullptr, N, 1, wa, c->cp.na, c->keys.atables, c->keys.key_flags, c->stream);
   if (e == cudaSuccess && rc == HS_OK) e = cudaStreamSynchronize(c->stream);
   std::vector<uint8_t> fl(N);
   if (e == cudaSuccess && rc == HS_OK) e = cudaMemcpy(fl.data(), c->keys.key_flags, N, cudaMemcpyDeviceToHost);
@@ -3320,9 +3341,56 @@ static int publish_hash(hs_ctx *c) {
   return HS_OK;
 }
 
+// The slots hs_committee_update gives added keys, chosen on copies of the mirrors: a key in service keeps its index, the same key twice
+// takes one slot, a new key takes the lowest free slot, then a spare.  Each slot taken is marked `mark` in `live`.  full: no slot was
+// left for key idx.size(), and the keys before it are planned.
+struct slot_plan {
+  std::vector<uint8_t> live, pks;  // h_key_live and h_pks with the additions (longer by the spares taken)
+  std::vector<uint32_t> idx;       // the index of each added key
+  std::vector<uint32_t> fresh;     // the slots taken, in order
+  bool full = false;
+};
+static void plan_adds(const hs_ctx *c, const uint8_t *add_pks, size_t n_add, uint8_t mark, slot_plan &P) {
+  P.live = c->h_key_live;
+  P.pks = c->h_pks;
+  // The published table plus this call's additions, so that the same key twice in one call takes one slot.
+  key_index index = c->h_index;
+  auto live = [&P](uint32_t idx) { return P.live[idx] != 0; };
+  size_t next_free = 0;
+  for (size_t i = 0; i < n_add; i++) {
+    const uint8_t *key = add_pks + 32 * i;
+    uint32_t idx = index.find(P.pks.data(), key, live);
+    if (idx == HS_NO_KEY) {
+      while (next_free < P.live.size() && P.live[next_free]) next_free++;
+      if (next_free < P.live.size()) idx = (uint32_t)next_free;
+      else if (P.live.size() < c->key_capacity) {
+        idx = (uint32_t)P.live.size();
+        P.live.push_back(0);
+        P.pks.resize(P.live.size() * 32);
+      } else {
+        P.full = true;
+        return;
+      }
+      memcpy(P.pks.data() + 32 * (size_t)idx, key, 32);
+      P.live[idx] = mark;
+      index.insert_absent(P.pks.data(), idx, live);
+      P.fresh.push_back(idx);
+    }
+    P.idx.push_back(idx);
+  }
+}
+// Frees a pending or in-progress stage's slots (hs_committee_update, hs_committee_discard, a failed stage): they go back to free, and
+// the spares it took are no longer held.  After a commit nothing is SLOT_STAGED, so this only forgets the stage.
+static void stage_drop(hs_ctx *c) {
+  for (uint32_t s : c->stage.fresh)
+    if (s < c->h_key_live.size() && c->h_key_live[s] == SLOT_STAGED) c->h_key_live[s] = 0;
+  if (c->explicit_committee && c->h_key_live.size() > c->n_keys) c->h_key_live.resize(c->n_keys);
+  c->stage = {};
+}
+
 // Incremental epoch change (consensus/src/config.rs Committee: a few validators join / leave): removed indices stop
 // verifying (flag cleared, hash slot dropped), added keys take a free slot — a removed one or a spare — and only THEIR tables
-// are built (~0.25 ms per key); every other validator keeps its index and its table.
+// are built, in one k_build_comb launch; every other validator keeps its index and its table.  It discards a pending stage.
 int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const uint32_t *remove_idx, size_t n_remove, uint32_t *out_add_idx) {
   if (!c || (n_add && (!add_pks || !out_add_idx)) || (n_remove && !remove_idx)) return fail(c, HS_ERR_ARG, "hs_committee_update: bad argument");
   std::lock_guard<std::mutex> g(c->mu);
@@ -3331,35 +3399,34 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
   HS_CUDA(c, cudaDeviceSynchronize());  // epoch boundary: nothing of the old set may be in flight (verify queue launches and audits included)
   for (size_t i = 0; i < n_remove; i++)
     if (remove_idx[i] >= c->n_keys) return fail(c, HS_ERR_ARG, "hs_committee_update: remove index out of range");
+  stage_drop(c);
   c->key_gen++;
   for (size_t i = 0; i < n_remove; i++) {
     c->h_key_live[remove_idx[i]] = 0;
     HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + remove_idx[i], 0, 1, c->stream));
   }
-  // The published table plus this call's additions, so that the same key twice in one call takes one slot.  A failed update leaves
-  // the context's index as published.
-  key_index index = c->h_index;
-  auto live = [c](uint32_t idx) { return c->h_key_live[idx] != 0; };
-  size_t next_free = 0;
-  for (size_t i = 0; i < n_add; i++) {
-    const uint8_t *key = add_pks + 32 * i;
-    uint32_t idx = index.find(c->h_pks.data(), key, live);
-    if (idx == HS_NO_KEY) {
-      while (next_free < c->n_keys && c->h_key_live[next_free]) next_free++;
-      if (next_free < c->n_keys) idx = (uint32_t)next_free;
-      else if (c->n_keys < c->key_capacity) {
-        idx = (uint32_t)c->n_keys++;
-        c->h_key_live.push_back(0);
-        c->h_pks.resize(c->n_keys * 32);
-      } else return fail(c, HS_ERR_NOMEM, "hs_committee_update: no free table slot (re-register the committee)");
-      memcpy(c->h_pks.data() + 32 * (size_t)idx, key, 32);
-      c->h_key_live[idx] = 1;
-      index.insert_absent(c->h_pks.data(), idx, live);
-      HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)idx, key, 32, cudaMemcpyHostToDevice, c->stream));
-      HS_TRY(launch_build(c, c->keys.pks + 32 * (size_t)idx, 1, 1, c->cp.wa, c->cp.na, c->keys.atables + (size_t)idx * c->a_table_entries,
-                          c->keys.key_flags + idx, c->stream));
-    }
-    out_add_idx[i] = idx;
+  // A failed update leaves the context's index as published; the keys planned before a lack of slots are still placed and built.
+  slot_plan P;
+  plan_adds(c, add_pks, n_add, SLOT_LIVE, P);
+  c->h_key_live = std::move(P.live);
+  c->h_pks = std::move(P.pks);
+  c->n_keys = c->h_key_live.size();
+  std::copy(P.idx.begin(), P.idx.end(), out_add_idx);
+  const size_t n_new = P.fresh.size();
+  if (n_new) {
+    for (uint32_t s : P.fresh)
+      HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)s, c->h_pks.data() + 32 * (size_t)s, 32, cudaMemcpyHostToDevice, c->stream));
+    h2d_stage st;
+    const size_t s_slots = st.add(P.fresh.data(), 4 * n_new), s_flags = st.add(nullptr, n_new);
+    HS_TRY(st.upload(c, c->in[0], c->stream));
+    HS_TRY(launch_build(c, c->keys.pks, reinterpret_cast<const uint32_t *>(st.ptr(s_slots)), n_new, 1, c->cp.wa, c->cp.na, c->keys.atables,
+                        st.ptr(s_flags), c->stream));
+    for (size_t k = 0; k < n_new; k++)
+      HS_CUDA(c, cudaMemcpyAsync(c->keys.key_flags + P.fresh[k], st.ptr(s_flags) + k, 1, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  if (P.full) {
+    HS_CUDA(c, cudaStreamSynchronize(c->stream));
+    return fail(c, HS_ERR_NOMEM, "hs_committee_update: no free table slot (re-register the committee)");
   }
   HS_TRY(publish_hash(c));
   return HS_OK;
@@ -4666,7 +4733,7 @@ static int st_build_keys(hs_ctx *c, const st_set &T, const comb_params &cp, st_k
   }
   HS_CUDA(c, cudaMemcpyAsync(KS.K.pks, KS.pks.data(), n * 32, cudaMemcpyHostToDevice, st));
   HS_CUDA(c, cudaMemcpyAsync(KS.K.slots, KS.h_index.slots.data(), KS.h_index.slots.size() * 4, cudaMemcpyHostToDevice, st));
-  HS_TRY(launch_build(c, KS.K.pks, n, 1, cp.wa, cp.na, KS.K.atables, KS.K.key_flags, st));
+  HS_TRY(launch_build(c, KS.K.pks, nullptr, n, 1, cp.wa, cp.na, KS.K.atables, KS.K.key_flags, st));
   K = store_tables(KS.K, KS.h_index, n, comb_table_entries(cp.wa), cp);
   return HS_OK;
 }
@@ -4909,17 +4976,33 @@ static std::string audit_message(uint64_t first, size_t n_slots, const uint32_t 
   return m;
 }
 
-// k_table_audit over n_tables tables on `stream` (auditable: nullable for the base-point table).
-static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *tables, size_t n_tables, size_t entries, int W, int n_windows,
-                              const uint8_t *pks, const uint8_t *auditable, const audit_out &O) {
+// k_table_audit over n_tables tables on `stream`: tables 0 .. n_tables - 1, or with d_slots the listed slots' (auditable and findings by
+// list position).  auditable: nullable for the base-point table.
+static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *tables, const uint32_t *d_slots, size_t n_tables, size_t entries,
+                              int W, int n_windows, const uint8_t *pks, const uint8_t *auditable, const audit_out &O) {
   const uint64_t warps = (uint64_t)n_tables * n_windows * ((((uint64_t)1 << (W - 1)) + 1 + 31) / 32);
-  k_table_audit<<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, stream>>>(tables, n_tables, entries, W,
-                                                                                                                n_windows, pks, auditable, O);
+  const auto launch = [&](auto listed) {
+    k_table_audit<decltype(listed)::value><<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, stream>>>(
+        tables, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
+  };
+  if (d_slots) launch(std::true_type{});
+  else launch(std::false_type{});
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
 }
 
+// The audit's private stream of the lowest priority and its event, created on first use.
+static int audit_stream(hs_ctx *c) {
+  audit_state &A = c->audit;
+  if (!A.stream) {
+    int lo = 0, hi = 0;
+    HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    HS_CUDA(c, create(A.stream, lo));
+    HS_CUDA(c, create(A.done));
+  }
+  return HS_OK;
+}
 // One complete audit: enqueued under c->mu by audit_enqueue_locked, then waited for and read back without it by audit_collect.  Its
 // caller holds audit_mu, so the audit's stream, event and scratch are its own.
 struct audit_run {
@@ -4947,14 +5030,10 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
   const size_t n = has_key_tables(c) ? c->n_keys : 0;
   if (n_slots != n) return fail_args(c, entry, ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
   if (expect_pks && n && !c->explicit_committee) return fail_args(c, entry, "key-cache tables are audited with expect_pks == NULL");
-  if (!A.stream) {
-    int lo = 0, hi = 0;
-    HS_CUDA(c, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    HS_CUDA(c, create(A.stream, lo));
-    HS_CUDA(c, create(A.done));
-  }
-  std::vector<uint8_t> live(n, 1);
-  if (c->explicit_committee) std::copy(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin());
+  HS_TRY(audit_stream(c));
+  std::vector<uint8_t> live(n, 1);  // a staged slot is not in service
+  if (c->explicit_committee)
+    std::transform(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin(), [](uint8_t v) { return v == SLOT_STAGED ? 0 : v; });
   const size_t res_bytes = 8 + 4 * (2 + n);
   h2d_stage in;
   const size_t s_res = in.add(nullptr, res_bytes), s_pks = in.add(expect_pks, expect_pks ? n * 32 : 0),
@@ -4972,9 +5051,9 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
         expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
-    HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
+    HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
   }
-  HS_TRY(launch_table_audit(c, A.stream, c->d_btable, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
+  HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
   HS_CUDA(c, cudaEventRecord(A.done, A.stream));
   r.gen = c->key_gen;
   r.n_slots = n;
@@ -5009,6 +5088,52 @@ extern "C" int hs_table_audit(hs_ctx *c, const uint8_t *expect_pks, const uint32
   return failed ? fail(c, HS_ERR_SELFTEST, audit_message(r.first(), n_slots, r.bits()).c_str()) : HS_OK;
 }
 
+// ---- building and proving a list of key slots off the verify path (hs_table_repair, hs_committee_stage)
+// The comb tables of `slots` (their key bytes already in keys.pks), built on the audit's stream by one k_build_comb launch, with the
+// flag bytes into the audit's scratch, then proved by one k_table_audit launch against those key bytes; a key that does not decompress
+// has no table to prove.  Enqueued under c->mu by slot_build_enqueue, waited for and read back without it by slot_build_collect.  The
+// caller holds audit_mu, so the audit's stream, event and scratch are its own.
+struct slot_build {
+  size_t n = 0;
+  const uint8_t *d_out = nullptr;  // flag bytes (n), then at res_off an audit_out: first (8 bytes), bits[2 + n]
+  size_t res_off = 0;
+  std::vector<uint8_t> h;          // d_out read back
+  uint8_t flag(size_t k) const { return h[k]; }
+  bool proved(size_t k) const {    // the table of list position k passed, or the key has none
+    uint32_t bits;
+    memcpy(&bits, h.data() + res_off + 8 + 4 * (2 + k), 4);
+    return !(h[k] & 1u) || !bits;
+  }
+};
+static int slot_build_enqueue(hs_ctx *c, const std::vector<uint32_t> &slots, slot_build &B) {
+  audit_state &A = c->audit;
+  const size_t n = slots.size();
+  HS_TRY(audit_stream(c));
+  h2d_stage st;
+  const size_t s_slots = st.add(slots.data(), 4 * n), s_flags = st.add(nullptr, n), s_res = st.add(nullptr, 8 + 4 * (2 + n));
+  HS_TRY(st.upload(c, A.scratch, A.stream));
+  uint8_t *out = st.ptr(s_flags), *res = st.ptr(s_res);
+  HS_CUDA(c, cudaMemsetAsync(out, 0, st.total - st.sec[s_flags].off, A.stream));
+  HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
+  const uint32_t *d_slots = reinterpret_cast<const uint32_t *>(st.ptr(s_slots));
+  HS_TRY(launch_build(c, c->keys.pks, d_slots, n, 1, c->cp.wa, c->cp.na, c->keys.atables, out, A.stream));
+  HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, d_slots, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, out,
+                            audit_out{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)}));
+  HS_CUDA(c, cudaEventRecord(A.done, A.stream));  // the key-cache paths, registration and updates wait for it before they rewrite
+  B.n = n;
+  B.d_out = out;
+  B.res_off = (size_t)(res - out);
+  B.h.resize(st.total - st.sec[s_flags].off);
+  return HS_OK;
+}
+static cudaError_t slot_build_collect(hs_ctx *c, slot_build &B) {
+  audit_state &A = c->audit;
+  cudaError_t e = cudaEventSynchronize(A.done);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(B.h.data(), B.d_out, B.h.size(), cudaMemcpyDeviceToHost, A.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(A.stream);
+  return e;
+}
+
 // ---- repair of what the audit finds (hs_table_repair)
 // Empties the signature cache and the certificate cache of every verify queue of the context (under c->mu, the device drained): a
 // record accepted against a wrong table must not be answered from a cache.  Requests in flight complete as they would.
@@ -5037,18 +5162,20 @@ static int repair_locked(hs_ctx *c, std::unique_lock<std::mutex> &g, const audit
   const bool committee = c->explicit_committee;
   const uint32_t *bits = first.bits();
   if (bits[0]) {
-    HS_TRY(launch_build(c, nullptr, 1, 0, c->cp.wb, c->cp.nb, c->d_btable, nullptr, c->stream));
+    HS_TRY(launch_build(c, nullptr, nullptr, 1, 0, c->cp.wb, c->cp.nb, c->d_btable, nullptr, c->stream));
     HS_CUDA(c, cudaStreamSynchronize(c->stream));
   }
   std::vector<uint32_t> R;
   for (size_t s = 0; s < first.n_slots; s++) {
     if (!(bits[2 + s] & (HS_AUDIT_KEY | HS_AUDIT_FLAG | HS_AUDIT_TABLE))) continue;
-    const bool live = !committee || (expect_live ? (expect_live[s >> 5] >> (s & 31)) & 1u : (expect_pks || c->h_key_live[s]));
+    // A staged slot stays staged with flag 0: its commit writes its proved flag byte.
+    const bool staged = committee && c->h_key_live[s] == SLOT_STAGED;
+    const bool live = !staged && (!committee || (expect_live ? (expect_live[s >> 5] >> (s & 31)) & 1u : (expect_pks || c->h_key_live[s])));
     if (live) {
       R.push_back((uint32_t)s);
       if (expect_pks) memcpy(c->h_pks.data() + 32 * s, expect_pks + 32 * s, 32);
     }
-    if (committee) c->h_key_live[s] = live ? SLOT_REPAIR : 0;
+    if (committee && !staged) c->h_key_live[s] = live ? SLOT_REPAIR : 0;
     HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + s, 0, 1, c->stream));
   }
   if (first.n_slots) HS_TRY(publish_hash(c));  // also the whole repair of a LOOKUP finding
@@ -5056,28 +5183,12 @@ static int repair_locked(hs_ctx *c, std::unique_lock<std::mutex> &g, const audit
   HS_TRY(flush_queue_caches(c));
   const uint64_t gen = ++c->key_gen;
   if (R.empty()) return HS_OK;
-  // Rebuild R on the audit's stream: key bytes, table, flag byte into staging; then k_table_audit over each table on its own.
-  const size_t per = 24;  // an audit_out of one table (8 + 4 * 3 bytes, 8-aligned): bits[2] is the slot's
-  h2d_stage st;
-  const size_t s_flags = st.add(nullptr, R.size()), s_res = st.add(nullptr, per * R.size());
-  HS_TRY(st.upload(c, A.scratch, A.stream));
-  HS_CUDA(c, cudaMemsetAsync(st.ptr(s_flags), 0, st.total - st.sec[s_flags].off, A.stream));
-  for (size_t k = 0; k < R.size(); k++) {
-    const size_t s = R[k];
-    ge_niels *table = c->keys.atables + s * c->a_table_entries;
-    uint8_t *res = st.ptr(s_res) + per * k;
-    HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * s, c->h_pks.data() + 32 * s, 32, cudaMemcpyHostToDevice, A.stream));
-    HS_TRY(launch_build(c, c->keys.pks + 32 * s, 1, 1, c->cp.wa, c->cp.na, table, st.ptr(s_flags) + k, A.stream));
-    HS_TRY(launch_table_audit(c, A.stream, table, 1, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks + 32 * s, st.ptr(s_flags) + k,
-                              audit_out{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)}));
-  }
-  HS_CUDA(c, cudaEventRecord(A.done, A.stream));  // the key-cache paths, registration and updates wait for it before they rewrite
-  std::vector<uint8_t> h(per * R.size() + R.size());
+  // Rebuild R on the audit's stream: key bytes, then every table in one build launch and one proof launch.
+  for (uint32_t s : R) HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)s, c->h_pks.data() + 32 * (size_t)s, 32, cudaMemcpyHostToDevice, A.stream));
+  slot_build B;
+  HS_TRY(slot_build_enqueue(c, R, B));
   if (committee) g.unlock();
-  cudaError_t e = cudaEventSynchronize(A.done);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), st.ptr(s_flags), R.size(), cudaMemcpyDeviceToHost, A.stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h.data() + R.size(), st.ptr(s_res), per * R.size(), cudaMemcpyDeviceToHost, A.stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(A.stream);
+  const cudaError_t e = slot_build_collect(c, B);
   if (committee) g.lock();
   if (e != cudaSuccess) return fail(c, HS_ERR_CUDA, "hs_table_repair: rebuild", e);  // R stays out of service
   // Back into service: each slot of R an update or a registration did not take over meanwhile, whose table passed (a key that does
@@ -5085,10 +5196,8 @@ static int repair_locked(hs_ctx *c, std::unique_lock<std::mutex> &g, const audit
   for (size_t k = 0; k < R.size(); k++) {
     const size_t s = R[k];
     if (committee && (!c->explicit_committee || s >= c->n_keys || c->h_key_live[s] != SLOT_REPAIR)) continue;
-    uint32_t slot_bits;
-    memcpy(&slot_bits, h.data() + R.size() + per * k + 8 + 8, 4);
-    if ((h[k] & 1u) && slot_bits) continue;
-    HS_CUDA(c, cudaMemcpyAsync(c->keys.key_flags + s, h.data() + k, 1, cudaMemcpyHostToDevice, c->stream));
+    if (!B.proved(k)) continue;
+    HS_CUDA(c, cudaMemcpyAsync(c->keys.key_flags + s, B.h.data() + k, 1, cudaMemcpyHostToDevice, c->stream));
     if (committee) c->h_key_live[s] = SLOT_LIVE;
   }
   if (committee && c->explicit_committee) HS_TRY(publish_hash(c));
@@ -5123,6 +5232,102 @@ extern "C" int hs_table_repair(hs_ctx *c, const uint8_t *expect_pks, const uint3
   *out_found = found;
   *out_failed = failed;
   return failed ? fail(c, HS_ERR_SELFTEST, audit_message(last.first(), n_slots, last.bits()).c_str()) : HS_OK;
+}
+
+// ---- staged committee change (hs_committee_stage / hs_committee_commit / hs_committee_discard)
+// stage(A, R) + commit leaves the context as hs_committee_update(A, none) + hs_committee_update(none, R) would.  The stage picks the
+// slots as update does and marks them SLOT_STAGED (out of service: not in the hash table, flag 0), then builds and proves their tables
+// off the verify path as a repair does.  The commit writes the proved flags, takes R out of service and publishes the hash table.
+extern "C" int hs_committee_stage(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const uint32_t *remove_idx, size_t n_remove,
+                                  uint32_t *out_add_idx) {
+  const char *entry = "hs_committee_stage";
+  if (!c || (n_add && (!add_pks || !out_add_idx)) || (n_remove && !remove_idx)) return fail_args(c, entry, "bad argument");
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  slot_plan P;
+  slot_build B;
+  uint64_t gen = 0;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    if (!committee_registered(c)) return fail_args(c, entry, "no committee registered");
+    if (c->stage.busy) return fail_args(c, entry, "a stage is already pending (commit or discard it)");
+    plan_adds(c, add_pks, n_add, SLOT_STAGED, P);
+    if (P.full) return fail(c, HS_ERR_NOMEM, "hs_committee_stage: too few free and spare slots (use hs_committee_update)");
+    for (size_t i = 0; i < n_remove; i++)  // against the slots in use once the additions are in, as the second update would check
+      if (remove_idx[i] >= P.live.size()) return fail_args(c, entry, "remove index out of range");
+    HS_CUDA(c, cudaSetDevice(c->device));
+    committee_stage &S = c->stage;
+    S.busy = true;
+    S.fresh = P.fresh;
+    S.remove.assign(remove_idx, remove_idx + n_remove);
+    for (uint32_t s : P.fresh) S.keys.insert(S.keys.end(), P.pks.begin() + 32 * (size_t)s, P.pks.begin() + 32 * (size_t)s + 32);
+    c->h_key_live = P.live;
+    gen = c->key_gen;
+    // Key bytes of slots out of service: no launch resolves a key to them, and a committee-indexed record naming one rejects on its flag.
+    const auto enqueue = [&]() -> int {
+      if (P.fresh.empty()) return HS_OK;
+      HS_TRY(audit_stream(c));
+      for (size_t k = 0; k < P.fresh.size(); k++)
+        HS_CUDA(c, cudaMemcpyAsync(c->keys.pks + 32 * (size_t)P.fresh[k], S.keys.data() + 32 * k, 32, cudaMemcpyHostToDevice, c->audit.stream));
+      return slot_build_enqueue(c, P.fresh, B);
+    };
+    if (const int rc = enqueue()) {
+      stage_drop(c);
+      return rc;
+    }
+  }
+  const cudaError_t e = P.fresh.empty() ? cudaSuccess : slot_build_collect(c, B);
+  std::lock_guard<std::mutex> g(c->mu);
+  if (c->key_gen != gen) return fail_args(c, entry, "a registration or update ran during the stage; stage again");  // it dropped the stage
+  if (e != cudaSuccess) {
+    stage_drop(c);
+    return fail(c, HS_ERR_CUDA, "hs_committee_stage: build", e);
+  }
+  for (size_t k = 0; k < P.fresh.size(); k++)
+    if (!B.proved(k)) {
+      stage_drop(c);
+      return fail(c, HS_ERR_SELFTEST, ("hs_committee_stage: slot " + std::to_string(P.fresh[k]) + ": the staged comb table failed its proof (TABLE)").c_str());
+    }
+  c->stage.flags.assign(B.h.begin(), B.h.begin() + P.fresh.size());
+  c->stage.ready = true;
+  std::copy(P.idx.begin(), P.idx.end(), out_add_idx);
+  return HS_OK;
+}
+
+extern "C" int hs_committee_commit(hs_ctx *c) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> ga(c->audit_mu);  // before mu: the commit never waits for an audit while it holds the mutex
+  std::lock_guard<std::mutex> g(c->mu);
+  committee_stage &S = c->stage;
+  if (!S.ready || !committee_registered(c))
+    return fail_args(c, "hs_committee_commit", "no stage pending (none was made, or a registration or update discarded it)");
+  HS_CUDA(c, cudaSetDevice(c->device));
+  // A launch in flight that resolved a key to a removed slot must not see its flag cleared.  Adding slots disturbs no launch in flight.
+  if (!S.remove.empty()) HS_CUDA(c, cudaDeviceSynchronize());
+  c->key_gen++;
+  for (size_t k = 0; k < S.fresh.size(); k++) {
+    const uint32_t s = S.fresh[k];
+    if (s >= c->n_keys) {  // a spare: the spares a stage takes follow n_keys without a gap
+      c->n_keys = (size_t)s + 1;
+      c->h_pks.resize(c->n_keys * 32);
+    }
+    memcpy(c->h_pks.data() + 32 * (size_t)s, S.keys.data() + 32 * k, 32);
+    c->h_key_live[s] = SLOT_LIVE;
+    HS_CUDA(c, cudaMemcpyAsync(c->keys.key_flags + s, S.flags.data() + k, 1, cudaMemcpyHostToDevice, c->stream));
+  }
+  for (uint32_t s : S.remove) {
+    c->h_key_live[s] = 0;
+    HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + s, 0, 1, c->stream));
+  }
+  stage_drop(c);
+  return publish_hash(c);  // behind the flag bytes on the same stream; the key bytes were in place when the stage returned
+}
+
+extern "C" int hs_committee_discard(hs_ctx *c) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  std::lock_guard<std::mutex> g(c->mu);
+  stage_drop(c);
+  return HS_OK;
 }
 
 // ---- explanation of a verdict (hs_explain_rec128): k_explain over the staged records, on the context's stream.  No context table is

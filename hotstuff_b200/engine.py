@@ -275,6 +275,19 @@ class Engine:
         """Incremental epoch change (hs_committee_update): returns the indices assigned to the added keys."""
         return _committee_update(self, self.lib.hs_committee_update, "hs_committee_update", add, remove)
 
+    def committee_stage(self, add=None, remove=None):
+        """Prepares a committee change off the verify path (hs_committee_stage): returns the indices the added keys will have.  Nothing
+        changes for verification until committee_commit; stage + commit leaves the engine as update(add) then update(remove=remove)."""
+        return _committee_update(self, self.lib.hs_committee_stage, "hs_committee_stage", add, remove)
+
+    def committee_commit(self):
+        """Switches the staged change in (hs_committee_commit): builds no table."""
+        self._check(self.lib.hs_committee_commit(self.h), "hs_committee_commit")
+
+    def committee_discard(self):
+        """Frees the staged slots (hs_committee_discard); a no-op when nothing is staged."""
+        self._check(self.lib.hs_committee_discard(self.h), "hs_committee_discard")
+
     def set_table_budget(self, nbytes):
         self._check(self.lib.hs_set_table_budget(self.h, int(nbytes)), "hs_set_table_budget")
 
@@ -477,6 +490,41 @@ class MultiEngine:
     def update_committee(self, add=None, remove=None):
         """hs_multi_committee_update: returns the indices assigned to the added keys (the same on every member)."""
         return _committee_update(self, self.lib.hs_multi_committee_update, "hs_multi_committee_update", add, remove)
+
+    def stage_committee(self, add=None, remove=None):
+        """The staged committee change on every member, member by member through hs_committee_stage (as a repair is): stages on every
+        member at once, one thread each, and returns the indices, the same on every member.  If any member fails, or the members
+        return different indices, the stage is discarded on every member and EngineError raised: nothing stays staged."""
+        res = [None] * len(self._members)
+
+        def stage(i):
+            try:
+                res[i] = self._members[i].committee_stage(add, remove)
+            except EngineError as e:
+                res[i] = e
+
+        threads = [threading.Thread(target=stage, args=(i,)) for i in range(len(self._members))]
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+        err = next((r for r in res if isinstance(r, EngineError)), None)
+        if err is None and any(not np.array_equal(r, res[0]) for r in res[1:]):
+            err = EngineError("stage_committee: the members gave different indices")
+        if err is not None:
+            self.discard_committee()
+            raise err
+        return res[0]
+
+    def commit_committee(self):
+        """hs_committee_commit on every member.  After a failure the members may differ: re-register."""
+        for e in self._members:
+            e.committee_commit()
+
+    def discard_committee(self):
+        """hs_committee_discard on every member."""
+        for e in self._members:
+            e.committee_discard()
 
     def verify_rec128(self, recs, mode=MODE_STRICT):
         return _verify_rec128(self, self.lib.hs_multi_verify_rec128, "hs_multi_verify_rec128", recs, mode)

@@ -165,11 +165,37 @@ int hs_ingest_consensus_frames(const uint8_t *frames, const uint64_t *off /* n +
  * decompresses.  Replaces the per-call PublicKey::from_bytes of crypto/src/lib.rs:202,216. */
 int hs_committee_register(hs_ctx *ctx, const uint8_t *pks /* N x 32 */, size_t N, uint32_t *out_valid_bitmap);
 /* Incremental epoch change: validators remove_idx[] stop verifying (their indices become free), keys add_pks[] take a free
- * or spare slot (registration reserves N/16, at least 16, spare slots) and only their tables are built; out_add_idx[i]
+ * or spare slot (registration reserves N/16, at least 16, spare slots) and only their tables are built, in one launch; out_add_idx[i]
  * receives the index of add_pks[i] (an already-registered key returns its existing index).  Everyone else keeps index and
- * table.  HS_ERR_NOMEM when no slot is free: re-register.  Requires a registered committee. */
+ * table.  HS_ERR_NOMEM when no slot is free: re-register.  Requires a registered committee.  Holds the context's mutex and drains the
+ * device for the whole call, so verification waits for it; it discards a pending hs_committee_stage. */
 int hs_committee_update(hs_ctx *ctx, const uint8_t *add_pks /* n_add x 32 */, size_t n_add, const uint32_t *remove_idx, size_t n_remove,
                         uint32_t *out_add_idx);
+/* Staged committee change: prepare the next committee while the current one verifies, then switch it in with a short commit.
+ *   - Rule: hs_committee_stage(A, R) followed by hs_committee_commit leaves the context exactly as hs_committee_update(A, none) followed
+ *     by hs_committee_update(none, R): the same out_add_idx, hs_key_slots, key bytes, flag bytes, hash table, comb tables and verdicts.
+ *     So added keys take free slots, lowest first, then spares; a registered key keeps its index; a key repeated in A takes one slot; a
+ *     key of A whose slot is in R ends up removed; R's slots are not reused by the stage; a remove index may name any slot in use once
+ *     A is in, spares included.
+ *   - hs_committee_stage needs a registered committee.  Under the context's mutex it checks the arguments, picks the slots and writes
+ *     the added keys' bytes; then it builds every added key's comb table in one launch and proves them all in one audit launch (the checks
+ *     of hs_table_audit), on the audit's private lowest-priority stream and without the mutex, so verify queues keep launching.  It is
+ *     serialised with audits and repairs, and returns once the tables are built and proved.
+ *   - Until the commit, verification is exactly as before the stage: added keys are not in the committee (key-bytes calls take the
+ *     generic path with the same verdicts), a committee-indexed record naming a staged index rejects, removed validators keep verifying,
+ *     hs_key_slots does not change and an audit with the map from before the stage finds nothing.  A repair leaves a stage pending.
+ *   - Errors: HS_ERR_NOMEM when too few free and spare slots are left (nothing is staged: use hs_committee_update); HS_ERR_ARG for a
+ *     stage already pending, no registered committee, a remove index out of range, or a registration or update that ran during the
+ *     stage; HS_ERR_SELFTEST when a staged table fails its proof (nothing stays staged).  Every error writes nothing.
+ *   - hs_committee_commit applies the pending stage: the proved flag bytes of the added slots, the removed slots' flags cleared, then the
+ *     hash table.  It builds no table.  A stage that removes slots drains the device first, as hs_committee_update does; one that only
+ *     adds does not, since adding slots disturbs no launch in flight.  HS_ERR_ARG and no change when no stage is pending: none was made,
+ *     or a registration or update since it discarded it.
+ *   - hs_committee_discard frees the staged slots; a no-op when nothing is staged. */
+int hs_committee_stage(hs_ctx *ctx, const uint8_t *add_pks /* n_add x 32 */, size_t n_add, const uint32_t *remove_idx, size_t n_remove,
+                       uint32_t *out_add_idx);
+int hs_committee_commit(hs_ctx *ctx);
+int hs_committee_discard(hs_ctx *ctx);
 /* Memory budget (bytes) for the per-key tables of the NEXT registration / key-cache allocation (0 = default, ~62 % of the
  * device; also env HS_TABLE_BUDGET_MB at context creation).  The engine picks the widest window that fits: e.g. 4,096 keys in
  * 18 GB -> 12-bit windows.  Lets the engine sit beside another tenant on the same GPU. */
@@ -604,8 +630,12 @@ int hs_peer_timed_out(hs_ctx *ctx);
  *     with its hs_last_error; the outputs are then undefined and the caller rejects every signature of the call.
  *   - Committee: hs_multi_committee_register registers on every member at once.  If any member fails, or the members' out_valid_bitmap
  *     differ (HS_ERR_CUDA), every member ends with NO committee.  hs_multi_committee_update must give every member the same out_add_idx;
- *     a mismatch is HS_ERR_CUDA, and after any failure of it the members may differ: re-register.  The committee-indexed forms need every
- *     member registered through these two calls: never change a member's committee directly.
+ *     a mismatch is HS_ERR_CUDA, and after any failure of it the members may differ: re-register.  A staged change
+ *     (hs_committee_stage / _commit / _discard) is made member by member through hs_multi_member with the same arguments, as a repair is:
+ *     stage on every member (at once, from one thread per member); if any stage fails or the members return different indices, discard
+ *     on every member; otherwise commit on every member.  After a failed commit the members may differ: re-register.  The bindings do
+ *     exactly this (MultiEngine.stage_committee / commit_committee / discard_committee, hs::MultiEngine, multi::Multi).  Apart from that,
+ *     the committee-indexed forms need every member's committee changed through the two calls above: never change one member alone.
  *   - Pinned memory from hs_host_alloc (cudaMallocHost) is portable under UVA: every member DMAs from the caller's pinned buffers directly.
  *   - hs_multi_destroy joins the workers and destroys the members (and the verify queues created on them); it must not race with calls.
  *     A failed hs_multi_create (n_devices == 0, a bad ordinal, no memory) leaves no thread and no member behind. */

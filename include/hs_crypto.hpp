@@ -95,6 +95,17 @@ class Engine {
     check(hs_explain_rec128(ctx_, recs, n, why.data()), "hs_explain_rec128");
     return why;
   }
+  // Staged committee change (hs_committee_stage): the added keys' tables are built and proved off the verify path and nothing changes
+  // for verification until committee_commit.  Returns the indices the added keys will have: stage + commit leaves the engine as
+  // hs_committee_update(add) then hs_committee_update(remove) would.  Throws EngineError on any failure (HS_ERR_NOMEM: too few free and
+  // spare slots, use hs_committee_update).
+  std::vector<uint32_t> committee_stage(const uint8_t *add_pks, size_t n_add, const uint32_t *remove_idx, size_t n_remove) const {
+    std::vector<uint32_t> idx(n_add);
+    check(hs_committee_stage(ctx_, add_pks, n_add, remove_idx, n_remove, idx.data()), "hs_committee_stage");
+    return idx;
+  }
+  void committee_commit() const { check(hs_committee_commit(ctx_), "hs_committee_commit"); }
+  void committee_discard() const { check(hs_committee_discard(ctx_), "hs_committee_discard"); }
   std::string error() const { return hs_last_error(ctx_); }
 
  private:
@@ -137,6 +148,39 @@ class MultiEngine {
     std::vector<uint32_t> idx(n_add);
     check(hs_multi_committee_update(m_, add_pks, n_add, remove_idx, n_remove, idx.data()), "hs_multi_committee_update");
     return idx;
+  }
+  // The staged committee change on every member, member by member through the single-context calls (as a repair is): stages on every
+  // member at once, one thread each, and returns the indices, the same on every member.  If any member fails, or the members return
+  // different indices, the stage is discarded on every member and EngineError thrown: nothing stays staged.
+  std::vector<uint32_t> stage_committee(const uint8_t *add_pks, size_t n_add, const uint32_t *remove_idx, size_t n_remove) {
+    std::vector<std::future<std::vector<uint32_t>>> parts;
+    for (auto &e : members_)
+      parts.push_back(std::async(std::launch::async, [&e, add_pks, n_add, remove_idx, n_remove] {
+        return e->committee_stage(add_pks, n_add, remove_idx, n_remove);
+      }));
+    std::vector<std::vector<uint32_t>> idx;
+    std::string err;
+    for (auto &p : parts) {
+      try {
+        idx.push_back(p.get());
+      } catch (const EngineError &x) {
+        if (err.empty()) err = x.what();
+      }
+    }
+    for (size_t i = 1; err.empty() && i < idx.size(); i++)
+      if (idx[i] != idx[0]) err = "stage_committee: member " + std::to_string(i) + " gave other indices than member 0";
+    if (!err.empty()) {
+      for (auto &e : members_) hs_committee_discard(e->raw());
+      throw EngineError(err);
+    }
+    return idx.at(0);
+  }
+  // hs_committee_commit on every member.  After a failure the members may differ: re-register.
+  void commit_committee() {
+    for (auto &e : members_) e->committee_commit();
+  }
+  void discard_committee() {
+    for (auto &e : members_) e->committee_discard();
   }
   std::vector<uint32_t> verify_rec128(const hs_rec128 *recs, size_t n, uint32_t mode = HS_MODE_STRICT) {
     std::vector<uint32_t> bm((n + 31) / 32);

@@ -39,6 +39,11 @@ impl Drop for Multi {
     fn drop(&mut self) { unsafe { hs_multi_destroy(self.0) } }   // joins the workers, destroys the members and their queues
 }
 
+/// A member context handed to a staging thread (each call is serialised on the member's own mutex).
+struct Member(*mut HsCtx);
+unsafe impl Send for Member {}
+unsafe impl Sync for Member {}
+
 fn bits(bm: &[u32], n: usize) -> Vec<bool> { (0..n).map(|i| bm[i / 32] >> (i % 32) & 1 == 1).collect() }
 
 impl Multi {
@@ -70,6 +75,42 @@ impl Multi {
         if rc != HS_OK { return Err(self.err()); }
         out.truncate(add.len());
         Ok(out)
+    }
+    /// The staged committee change on every member, member by member through the single-context calls (as a repair is): stages on
+    /// every member at once, one thread each, and returns the added validators' indices.  If any member fails, or the members return
+    /// different indices, the stage is discarded on every member and Err returned: nothing stays staged.
+    pub fn stage_committee(&self, add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {
+        let members: Vec<Member> = (0..self.members()).map(|i| Member(self.member(i))).collect();
+        let res: Vec<Result<Vec<u32>, GpuError>> = std::thread::scope(|s| {
+            let hs: Vec<_> = members.iter().map(|m| s.spawn(move || { let m: &Member = m; super::stage_on(m.0, add, remove_idx) })).collect();
+            hs.into_iter().map(|h| h.join().unwrap_or(Err(GpuError::Unavailable))).collect()
+        });
+        let (mut idx, mut fail): (Option<Vec<u32>>, Option<GpuError>) = (None, None);
+        for r in res {
+            match r {
+                Err(e) => { if fail.is_none() { fail = Some(e); } }
+                Ok(v) => match &idx {
+                    None => idx = Some(v),
+                    Some(x) if *x == v => {}
+                    Some(_) => { if fail.is_none() { fail = Some(GpuError::Engine("stage_committee: the members gave different indices".into())); } }
+                },
+            }
+        }
+        match fail {
+            None => Ok(idx.unwrap_or_default()),
+            Some(e) => {
+                for m in &members { let _ = super::discard_on(m.0); }
+                Err(e)
+            }
+        }
+    }
+    /// Commits the staged change on every member.  Err: the members may differ, re-register.
+    pub fn commit_committee(&self) -> Result<(), GpuError> {
+        (0..self.members()).try_for_each(|i| super::commit_on(self.member(i)))
+    }
+    /// Discards the staged change on every member.
+    pub fn discard_committee(&self) -> Result<(), GpuError> {
+        (0..self.members()).try_for_each(|i| super::discard_on(self.member(i)))
     }
     /// hs_verify_rec128 across the members.  An engine failure rejects everything.
     pub fn verify_rec128(&self, recs: &[HsRec128], mode: u32) -> Vec<bool> {

@@ -94,6 +94,9 @@ extern "C" {
     fn hs_last_error(ctx: *const HsCtx) -> *const std::os::raw::c_char;
     fn hs_committee_register(ctx: *mut HsCtx, pks: *const u8, n: usize, out_valid_bitmap: *mut u32) -> c_int;
     fn hs_committee_update(ctx: *mut HsCtx, add_pks: *const u8, n_add: usize, remove_idx: *const u32, n_remove: usize, out_add_idx: *mut u32) -> c_int;
+    fn hs_committee_stage(ctx: *mut HsCtx, add_pks: *const u8, n_add: usize, remove_idx: *const u32, n_remove: usize, out_add_idx: *mut u32) -> c_int;
+    fn hs_committee_commit(ctx: *mut HsCtx) -> c_int;
+    fn hs_committee_discard(ctx: *mut HsCtx) -> c_int;
     fn hs_verify_strict_batch(ctx: *mut HsCtx, recs: *const HsRec128, n: usize, out_bitmap: *mut u32) -> c_int;
     fn hs_verify_batch_shared_msg(ctx: *mut HsCtx, digest: *const u8, votes: *const HsVote, n: usize,
                                   all_ok: *mut c_int, out_bitmap_or_null: *mut u32) -> c_int;
@@ -122,6 +125,10 @@ static DISABLED: AtomicBool = AtomicBool::new(false);
 /// The node-side index -> key map of the registered committee (None = a freed index): registration order, then every update's
 /// removals and returned indices.  `audit_tables` checks the engine's slots against it after every change.
 static KEYS: Mutex<Vec<Option<[u8; 32]>>> = Mutex::new(Vec::new());
+/// The staged committee change (`stage_committee`) that `commit_committee` applies to KEYS: the added keys, their indices and the removed
+/// indices.  KEYS lists no staged index before the commit: the engine holds staged slots out of service, and the audit would report one.
+struct Staged { add: Vec<[u8; 32]>, idx: Vec<u32>, remove: Vec<u32> }
+static STAGED: Mutex<Option<Staged>> = Mutex::new(None);
 
 /// None when no GPU / the library failed to initialise / the self-test failed: every caller below then stays on the CPU path.
 fn ctx() -> Option<*mut HsCtx> {
@@ -146,6 +153,7 @@ pub fn register_committee(keys: &[[u8; 32]]) -> Result<(), GpuError> {
     let rc = unsafe { hs_committee_register(c, keys.as_ptr() as *const u8, keys.len(), valid.as_mut_ptr()) };
     if rc != HS_OK { KEYS.lock().unwrap().clear(); return Err(GpuError::Engine(last_error(c))); }
     *KEYS.lock().unwrap() = keys.iter().map(|k| Some(*k)).collect();
+    *STAGED.lock().unwrap() = None;  // a registration discards a staged change
     let bad: Vec<usize> = (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect();
     if bad.is_empty() { Ok(()) } else { Err(GpuError::InvalidKeys(bad)) }
 }
@@ -213,6 +221,7 @@ pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>
     let mut keys = KEYS.lock().unwrap();  // held across the update and its audit: the map and the engine change together
     let rc = unsafe { hs_committee_update(c, add.as_ptr() as *const u8, add.len(), remove_idx.as_ptr(), remove_idx.len(), out.as_mut_ptr()) };
     if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    *STAGED.lock().unwrap() = None;  // an update discards a staged change
     out.truncate(add.len());
     for &i in remove_idx { keys[i as usize] = None; }
     for (k, &i) in add.iter().zip(out.iter()) {
@@ -221,6 +230,57 @@ pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>
     }
     audit_tables(&keys)?;
     Ok(out)
+}
+/// hs_committee_stage / hs_committee_commit / hs_committee_discard on one context: the shim's own and, one per member, `multi::Multi`'s.
+fn stage_on(c: *mut HsCtx, add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {
+    let mut out = vec![0u32; add.len().max(1)];
+    let rc = unsafe { hs_committee_stage(c, add.as_ptr() as *const u8, add.len(), remove_idx.as_ptr(), remove_idx.len(), out.as_mut_ptr()) };
+    if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    out.truncate(add.len());
+    Ok(out)
+}
+fn commit_on(c: *mut HsCtx) -> Result<(), GpuError> {
+    let rc = unsafe { hs_committee_commit(c) };
+    if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    Ok(())
+}
+fn discard_on(c: *mut HsCtx) -> Result<(), GpuError> {
+    let rc = unsafe { hs_committee_discard(c) };
+    if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    Ok(())
+}
+/// Prepares the next epoch's committee while this one verifies (hs_committee_stage): the added validators' tables are built and
+/// proved on the GPU's lowest-priority stream, and nothing changes for verification until `commit_committee`.  Returns the indices the
+/// added validators will have.  Blocks for the build (about 0.1 ms per key): call it from `spawn_blocking` during the last rounds of
+/// the epoch.  An Err naming too few free and spare slots (HS_ERR_NOMEM) means: call `update_committee` at the boundary instead.
+pub fn stage_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>, GpuError> {
+    let c = ctx().ok_or(GpuError::Unavailable)?;
+    let mut staged = STAGED.lock().unwrap();
+    let idx = stage_on(c, add, remove_idx)?;
+    *staged = Some(Staged { add: add.to_vec(), idx: idx.clone(), remove: remove_idx.to_vec() });
+    Ok(idx)
+}
+/// Switches the staged committee in at the epoch boundary (hs_committee_commit: no table is built), applies the change to the node's
+/// map as `update_committee` would (additions, then removals) and audits the tables against it.
+pub fn commit_committee() -> Result<(), GpuError> {
+    let c = ctx().ok_or(GpuError::Unavailable)?;
+    let mut keys = KEYS.lock().unwrap();  // held across the commit and its audit: the map and the engine change together
+    let st = STAGED.lock().unwrap().take().ok_or_else(|| GpuError::Engine("commit_committee: nothing staged".into()))?;
+    commit_on(c)?;
+    for (k, &i) in st.add.iter().zip(st.idx.iter()) {
+        if i as usize >= keys.len() { keys.resize(i as usize + 1, None); }
+        keys[i as usize] = Some(*k);
+    }
+    for &i in &st.remove { keys[i as usize] = None; }
+    audit_tables(&keys)
+}
+/// Drops a staged committee change (hs_committee_discard).
+pub fn discard_committee() -> Result<(), GpuError> {
+    let c = ctx().ok_or(GpuError::Unavailable)?;
+    let mut staged = STAGED.lock().unwrap();
+    discard_on(c)?;
+    *staged = None;
+    Ok(())
 }
 
 /// Signature::verify for n triples.  None = "use the CPU path" (no GPU, or too few signatures to pay for a launch);

@@ -2262,24 +2262,70 @@ struct sig_counters {
   dev_mem<uint32_t> ctr;
   mapped<uint32_t> hctr;
 };
-// The batch lane's arena, scratch, streams and events (hs_queue_batch builds them whole, or not at all).
-struct batch_lane {
-  mapped<uint8_t> arena;    // request regions (inputs, then result words and the tail)
-  dev_mem<uint8_t> mirror;  // the inputs of the region in flight, at the same offsets
-  dev_mem<uint32_t> dig;    // the request's Digests, 32 bytes per preimage
+// ---- side lanes of the verify queue: the batch lane (hs_queue_batch) and the explain lane (hs_queue_explain)
+// A side lane's requests never enter the ring.  Each takes a region of the lane's mapped arena under q->mu and is filled outside it:
+// inputs, then result words, then a 16-byte tail whose word [1] is the completion word.  One launch is in flight per lane, on the lane's
+// own streams; it takes the ready requests at the front of the lane's list, and each request completes when its completion word
+// carries the launch's number.  The functions below serve both lanes; what differs is the lane_kind.
+struct side_lane;
+struct lane_kind {
+  const char *name;                          // in the lane's error texts
+  const char *configure;                     // the entry point that turns it on
+  size_t per_launch;                         // requests one launch takes at most
+  const char *launch_err, *incomplete;       // texts of a failed stream and of a completion word missing on drained streams
+  int (*enqueue)(hs_queue *q, side_lane &L);  // enqueues the launch of L.launch on the lane's streams (under c->mu)
+  void (*count)(side_lane &L);               // counts a launch whose every request completed HS_OK
+};
+static int batch_enqueue(hs_queue *q, side_lane &L);
+static void batch_count(side_lane &L);
+static int explain_enqueue(hs_queue *q, side_lane &L);
+static void explain_count(side_lane &L);
+static const lane_kind batch_kind{"batch", "hs_queue_batch", 1, "verify queue batch pass", "verify queue: k_batch_done did not complete",
+                                  batch_enqueue, batch_count};
+static const lane_kind explain_kind{"explain", "hs_queue_explain", SIZE_MAX, "verify queue explain launch",
+                                    "verify queue: k_queue_explain did not complete", explain_enqueue, explain_count};
+struct lane_req {
+  ticket_sink sink;
+  uint32_t n_bits;                // the ticket's verdict bits
+  uint32_t n, m, n_groups;        // the launch's shape: records (items), messages (preimages), groups,
+  uint64_t pre_bytes;             //   preimage bytes
+  uint64_t o_res, o_tail, size;   // its result words, its tail and its size, from the lane's region layout
+  uint64_t a_off = 0, a_pos = 0, a_end = 0;  // region offset in the arena; arena positions of its start and past its end
+  uint32_t seq = 0;               // the completion word (set at launch)
+  bool ready = false, done = false;
+};
+// A side lane's arena, its device mirror and its streams (lane_configure builds them whole, or not at all).
+struct lane_bufs {
+  mapped<uint8_t> arena;    // request regions
+  dev_mem<uint8_t> mirror;  // the inputs of the regions in flight, at the same offsets
+  stream_h stream, side;    // the lane's stream (the device's lowest priority) and, for the batch lane, its miss pass's stream
+};
+// Off while max_recs is 0.  Requests wait in reqs in submit order.  launch is the requests of the launch in flight (dispatcher thread;
+// changed under q->mu).  The buffers change only while the lane is off and reqs is empty.
+struct side_lane {
+  explicit side_lane(const lane_kind &k) : kind(k) {}
+  const lane_kind &kind;
+  size_t max_recs = 0, max_bytes = 0;  // limits of one request
+  byte_ring ring;                      // positions in buf.arena
+  lane_bufs buf;
+  std::deque<lane_req> reqs;
+  std::vector<lane_req *> launch;
+  uint32_t seq = 0;
+  uint64_t stats[HS_QUEUE_BATCH_STATS] = {};  // hs_queue_batch_stats / hs_queue_explain_stats
+  std::mutex cfg_mu;                          // serialises the lane's configure calls
+};
+static_assert(HS_QUEUE_EXPLAIN_STATS <= HS_QUEUE_BATCH_STATS, "a lane's stats array holds either lane's counters");
+// The batch lane's own scratch: the pass's Digests, hs_verify_groups' per-item buffers and the miss pass's events.
+struct batch_scratch {
+  dev_mem<uint32_t> dig;  // the request's Digests, 32 bytes per preimage
   dev_mem<fe> xyz;
   dev_mem<uint8_t> meta;
   dev_mem<uint32_t> vidx, miss, miss_count, items, grej, counter;
-  stream_h stream, side;  // the lane's stream (the bulk stream's priority) and its miss pass's stream
   event_h ev[2];
 };
-// The explain lane's arena, its device mirror, the launch's request list and its stream (hs_queue_explain builds them whole, or not at
-// all).
-struct explain_lane {
-  mapped<uint8_t> arena;    // request regions (records and preimages, then why bytes and the tail)
-  dev_mem<uint8_t> mirror;  // the regions of the launch in flight, at the same offsets (k_queue_explain reads them and counts in them)
-  mapped<xq_desc> list;     // the launch's requests
-  stream_h stream;          // the device's lowest priority
+// The explain lane's own scratch: the launch's request list.
+struct explain_scratch {
+  mapped<xq_desc> list;
 };
 struct hs_queue {
   hs_ctx *c = nullptr;
@@ -2336,48 +2382,9 @@ struct hs_queue {
   std::deque<uint64_t> gpend;
   generic_lists gen_bufs;
   uint64_t gstats[HS_QUEUE_GENERIC_STATS] = {};      // hs_queue_generic_stats
-  // batch lane (hs_queue_batch): off while b_max_items is 0.  Requests wait in bq in submit order, each with a region of the mapped
-  // arena lane.arena (b_arena); a region is filled outside q->mu and the request is dispatched once `ready`.  One pass is in flight at
-  // a time (b_cur, dispatcher thread), and regions are released in request order when their requests complete.  The lane's buffers
-  // and streams change only while the lane is off and bq is empty.
-  struct breq {
-    ticket_sink sink;
-    uint32_t n, n_groups, n_msgs;
-    uint64_t pre_bytes;
-    uint64_t a_off, a_end;  // region offset in the arena; arena position past it
-    uint64_t o_pre, o_sig, o_pk, o_mi, o_gi, o_mo, o_res, o_tail;  // sections, relative to the region (batch_layout)
-    uint32_t seq;           // the completion word k_batch_done writes
-    bool ready;
-  };
-  size_t b_max_items = 0, b_max_bytes = 0;
-  byte_ring b_arena;
-  batch_lane lane;
-  std::deque<breq> bq;
-  breq *b_cur = nullptr;  // the request in flight (dispatcher thread; set and cleared under q->mu)
-  uint32_t b_seq = 0;
-  uint64_t bstats[HS_QUEUE_BATCH_STATS] = {};  // hs_queue_batch_stats
-  std::mutex b_cfg_mu;                          // serialises hs_queue_batch calls
-  // explain lane (hs_queue_explain): off while x_max_records is 0.  Requests wait in xq in submit order, each with a region of the
-  // mapped arena xlane.arena (x_arena), filled outside q->mu and launchable once `ready`.  One k_queue_explain launch is in flight at a
-  // time: the first x_launched requests of xq (dispatcher thread; set and cleared under q->mu).  Each completes as soon as its
-  // completion word is up; the launch's regions are released, and its requests leave xq, when all of them have.  The lane's buffers and
-  // stream change only while the lane is off and xq is empty.
-  struct xreq {
-    ticket_sink sink;
-    uint32_t n, m, pre_bytes;
-    uint64_t a_off, a_pos, a_end;  // region offset in the arena; arena positions of its start and past its end
-    uint32_t seq;                  // the completion word k_queue_explain writes (set at launch)
-    bool ready, done;
-  };
-  size_t x_max_records = 0, x_max_bytes = 0;
-  byte_ring x_arena;
-  explain_lane xlane;
-  std::deque<xreq> xq;
-  size_t x_launched = 0;    // requests of the launch in flight (0: none)
-  uint64_t x_launch_recs = 0;
-  uint32_t x_seq = 0;
-  uint64_t xstats[HS_QUEUE_EXPLAIN_STATS] = {};  // hs_queue_explain_stats
-  std::mutex x_cfg_mu;                           // serialises hs_queue_explain calls
+  side_lane batch{batch_kind}, explain{explain_kind};  // the side lanes (dispatched in this order, ahead of ring work)
+  batch_scratch batch_scr;
+  explain_scratch explain_scr;
   uint64_t head = 0, launched = 0, tail = 0;
   size_t next_ticket = 1;
   uint32_t seq = 0;
@@ -2743,14 +2750,13 @@ static void queue_dispatch(hs_queue *q, uint64_t lo, uint64_t hi) {
 // its verdicts (the flags -> bits mapping of run_small).  A launch is retired once every request in its range — riders
 // included — has its word.  Every 4,096 passes both streams are queried: a CUDA error, or a drained stream with a word still
 // missing in a launch it ran, finishes the open requests with HS_ERR_CUDA (never an accept) and retires the launch.
-static void batch_watch(hs_queue *q, bool query);
-static void explain_watch(hs_queue *q, bool query);
+static std::array<side_lane *, 2> queue_lanes(hs_queue *q);
+static void lane_watch(hs_queue *q, side_lane &L, bool query);
 static void queue_watch(hs_queue *q) {
   std::vector<queue_completion> fire;
   cudaError_t qes[2] = {cudaErrorNotReady, cudaErrorNotReady};  // [0] stream, [1] bulk_stream: a launch is judged by its own
   const bool query = (++q->spins & 0xfff) == 0;
-  batch_watch(q, query);
-  explain_watch(q, query);
+  for (side_lane *L : queue_lanes(q)) lane_watch(q, *L, query);
   if (query) {  // queried BEFORE the words are read
     qes[0] = cudaStreamQuery(q->stream);
     qes[1] = cudaStreamQuery(q->bulk_stream);
@@ -2801,7 +2807,141 @@ static void queue_watch(hs_queue *q) {
   queue_fire(fire);
 }
 
-// ---- batch lane (hs_queue_submit_batch): one hs_verify_groups pass per request, on the lane's stream and scratch
+// ---- side lanes (see lane_kind): what both lanes share
+static std::array<side_lane *, 2> queue_lanes(hs_queue *q) { return {&q->batch, &q->explain}; }
+// The first lane, in dispatch order, with no launch in flight and a ready request at the front of its list (null: none).
+static side_lane *lane_ready_locked(hs_queue *q) {
+  for (side_lane *L : queue_lanes(q))
+    if (L->launch.empty() && !L->reqs.empty() && L->reqs.front().ready) return L;
+  return nullptr;
+}
+// Waits for L's last launch: its buffers may be released after this.
+static cudaError_t lane_drain(const side_lane &L) {
+  const cudaError_t e = L.buf.stream ? cudaStreamSynchronize(L.buf.stream) : cudaSuccess;
+  const cudaError_t f = L.buf.side ? cudaStreamSynchronize(L.buf.side) : cudaSuccess;
+  return e != cudaSuccess ? e : f;
+}
+
+// Completes each open request of L's launch whose completion word carries the launch's number.  qe is what the lane's streams report:
+// cudaErrorNotReady leaves the others open; drained streams (cudaSuccess) or an error (a failed enqueue passes cudaErrorLaunchFailure)
+// complete them with HS_ERR_CUDA (never a result).  Once none is open, the launch is counted when every request of it completed HS_OK
+// and its regions are released; its requests leave L's list only after their callbacks ran, so a resize returns after them.
+static void lane_complete(hs_queue *q, side_lane &L, cudaError_t qe) {
+  std::vector<queue_completion> fire;
+  bool open = false, ok = true;
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    for (lane_req *r : L.launch) {
+      if (r->done) continue;
+      const uint8_t *a = L.buf.arena.h + r->a_off;
+      if (reinterpret_cast<const volatile uint32_t *>(a + r->o_tail)[1] == r->seq) {
+        std::atomic_thread_fence(std::memory_order_acquire);
+        ticket_close_locked(q, r->sink, HS_OK, r->n_bits, reinterpret_cast<const uint32_t *>(a + r->o_res), fire);
+      } else if (qe == cudaErrorNotReady) {
+        open = true;
+        continue;
+      } else {
+        if (qe == cudaSuccess) fail(q->c, HS_ERR_CUDA, L.kind.incomplete);
+        ticket_close_locked(q, r->sink, HS_ERR_CUDA, r->n_bits, nullptr, fire);
+        ok = false;
+      }
+      r->done = true;
+    }
+    if (!open) {
+      if (ok) L.kind.count(L);
+      L.ring.release_to(L.launch.back()->a_end);
+    }
+  }
+  queue_fire(fire);
+  if (open) return;
+  std::lock_guard<std::mutex> g(q->mu);
+  L.reqs.erase(L.reqs.begin(), L.reqs.begin() + (long)L.launch.size());
+  L.launch.clear();
+  q->cv_done.notify_all();  // for callback tickets too: a resize waits for the lane's list to empty
+}
+
+// One launch takes the ready requests at the front of L's list, at most L.kind.per_launch of them, and enqueues its work under c->mu
+// only while it enqueues.  A failed enqueue completes every request of the launch with HS_ERR_CUDA.
+static void lane_dispatch(hs_queue *q, side_lane &L) {
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    const uint32_t seq = ++L.seq ? L.seq : ++L.seq;  // never 0: the regions' tails were zeroed at submit
+    for (size_t k = 0; k < L.reqs.size() && k < L.kind.per_launch && L.reqs[k].ready; k++) {
+      L.reqs[k].seq = seq;
+      L.launch.push_back(&L.reqs[k]);
+    }
+  }
+  int rc;
+  {
+    std::lock_guard<std::mutex> g(q->c->mu);
+    rc = L.kind.enqueue(q, L);
+  }
+  if (rc != HS_OK) lane_complete(q, L, cudaErrorLaunchFailure);
+}
+
+// Polls L's launch in flight.  When `query`, the lane's streams are queried first, before the words are read: a CUDA error fails the
+// open requests, and drained streams with a word still missing mean the launch did not complete.
+static void lane_watch(hs_queue *q, side_lane &L, bool query) {
+  if (L.launch.empty()) return;  // (set and cleared on this thread)
+  cudaError_t qe = cudaErrorNotReady;
+  if (query) {
+    const cudaError_t s[2] = {cudaStreamQuery(L.buf.stream), L.buf.side ? cudaStreamQuery(L.buf.side) : cudaSuccess};
+    if (s[0] == cudaSuccess && s[1] == cudaSuccess) qe = cudaSuccess;
+    for (cudaError_t x : s)
+      if (x != cudaSuccess && x != cudaErrorNotReady) {
+        fail(q->c, HS_ERR_CUDA, L.kind.launch_err, x);
+        qe = x;
+      }
+  }
+  lane_complete(q, L, qe);
+}
+
+// Resizes lane L to max_recs records and max_bytes bytes per request, or turns it off (0, 0).  It refuses new requests, waits for the
+// submitted ones to complete and for the lane's streams to drain (a failed drain is HS_ERR_CUDA and leaves the lane off), and releases
+// the lane's buffers and its own scratch before it allocates new ones: an arena where two of the largest regions fit (one can be
+// filled while the other's launch runs), its mirror, a stream at the device's lowest priority, and what own(scratch, buffers, arena
+// bytes, the device's highest stream priority) allocates.
+template <class Scratch, class Own>
+static int lane_configure(hs_queue *q, side_lane &L, size_t max_recs, size_t max_bytes, Scratch &scr, Own own) {
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> cfg(L.cfg_mu);
+  {
+    std::unique_lock<std::mutex> lk(q->mu);
+    if (max_recs == L.max_recs && max_bytes == L.max_bytes) return HS_OK;
+    L.max_recs = L.max_bytes = 0;  // refuses new requests while the lane changes
+    q->cv_done.wait(lk, [&] { return L.reqs.empty(); });
+  }
+  HS_CUDA(c, cudaSetDevice(c->device));
+  HS_CUDA(c, lane_drain(L));
+  L.buf = {};  // released before the new lane is allocated
+  scr = {};
+  L.ring = byte_ring{};
+  if (!max_recs) return HS_OK;
+  uint64_t acap = 4096;
+  while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
+  lane_bufs B;
+  Scratch S;
+  int lo = 0, hi = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+  if (e == cudaSuccess) e = create(B.stream, lo);
+  if (e == cudaSuccess) e = alloc(B.arena, acap);
+  if (e == cudaSuccess) e = alloc(B.mirror, acap);
+  if (e == cudaSuccess) e = own(S, B, acap, hi);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(c, HS_ERR_NOMEM, (std::string(L.kind.configure) + ": no pinned host or device memory for the " + L.kind.name + " lane").c_str(), e);
+  }
+  memset(B.arena.h, 0, acap);
+  L.buf = std::move(B);
+  scr = std::move(S);
+  std::lock_guard<std::mutex> g(q->mu);
+  L.ring = byte_ring{acap, 0, 0};
+  L.max_recs = max_recs;
+  L.max_bytes = max_bytes;
+  return HS_OK;
+}
+
+// ---- batch lane (hs_queue_submit_batch): one hs_verify_groups pass per request, on the lane's streams and scratch
 // A request's region: pre_off (u64, n_msgs + 1) | preimages | sig (64 B each) | pk (32 B each) | msg_idx (u32) | group_idx (u32) |
 // modes (u8) | result words (group words, then item words) | tail: [0] items outside the committee, [1] completion word.  Every
 // section starts 16-byte aligned.  The inputs (everything before the result words) cross the bus in one copy into the mirror.
@@ -2825,186 +2965,72 @@ static batch_layout batch_layout_of(uint64_t n_msgs, uint64_t pre_bytes, uint64_
 // A batch ticket's verdict bits: whole words, the group words then the item words.
 static uint32_t batch_bits(uint64_t n_groups, uint64_t n) { return (uint32_t)(32 * ((n_groups + 31) / 32 + (n + 31) / 32)); }
 
-// Completes the request in flight (dispatcher thread): its result words go to its callback or ticket, then its region is released.
-static void batch_complete(hs_queue *q, int status) {
-  std::vector<queue_completion> fire;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    const hs_queue::breq &r = *q->b_cur;
-    if (status == HS_OK) {
-      q->bstats[0]++;
-      q->bstats[1] += r.n;
-      q->bstats[2] += r.n_groups;
-      q->bstats[3] += r.pre_bytes;
-      q->bstats[4] += reinterpret_cast<const volatile uint32_t *>(q->lane.arena.h + r.a_off + r.o_tail)[0];
-    }
-    ticket_close_locked(q, r.sink, status, batch_bits(r.n_groups, r.n), reinterpret_cast<const uint32_t *>(q->lane.arena.h + r.a_off + r.o_res), fire);
-    q->b_arena.release_to(r.a_end);
-    q->b_cur = nullptr;
-    q->bq.pop_front();
-    q->cv_done.notify_all();  // for callback tickets too: hs_queue_batch waits for bq to drain
-  }
-  queue_fire(fire);
-}
-
-// Enqueues the pass of request r on the lane's streams, under c->mu only while it enqueues.  Touches no scratch, stream, event or
-// per-call state of the context, so synchronous calls, `_dev` calls and the queue's other launches can be in flight meanwhile.
-static int batch_launch(hs_queue *q, const hs_queue::breq &r) {
+// Enqueues the pass of the launch's one request.  Touches no scratch, stream, event or per-call state of the context, so synchronous
+// calls, `_dev` calls and the queue's other launches can be in flight meanwhile.
+static int batch_enqueue(hs_queue *q, side_lane &L) {
   hs_ctx *c = q->c;
-  std::lock_guard<std::mutex> g(c->mu);
-  cudaStream_t s = q->lane.stream;
-  const uint8_t *m = q->lane.mirror + r.a_off;
-  HS_CUDA(c, cudaMemcpyAsync(q->lane.mirror + r.a_off, q->lane.arena.h + r.a_off, r.o_res, cudaMemcpyHostToDevice, s));
-  k_digest32<<<blocks_for(r.n_msgs), HS_THREADS, 0, s>>>(m + r.o_pre, reinterpret_cast<const uint64_t *>(m), 0, r.n_msgs, q->lane.dig);
+  const lane_req &r = *L.launch.front();
+  const batch_layout B = batch_layout_of(r.m, r.pre_bytes, r.n, r.n_groups);
+  const batch_scratch &S = q->batch_scr;
+  cudaStream_t s = L.buf.stream;
+  const uint8_t *m = L.buf.mirror + r.a_off;
+  HS_CUDA(c, cudaMemcpyAsync(L.buf.mirror + r.a_off, L.buf.arena.h + r.a_off, B.o_res, cudaMemcpyHostToDevice, s));
+  k_digest32<<<blocks_for(r.m), HS_THREADS, 0, s>>>(m + B.o_pre, reinterpret_cast<const uint64_t *>(m), 0, r.m, S.dig);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
-  in_layout L{m + r.o_sig, 64, m + r.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(q->lane.dig.get()), 32, reinterpret_cast<const uint32_t *>(m + r.o_mi),
+  in_layout I{m + B.o_sig, 64, m + B.o_pk, 32, nullptr, reinterpret_cast<const uint8_t *>(S.dig.get()), 32, reinterpret_cast<const uint32_t *>(m + B.o_mi),
               nullptr, 32, 0};
   // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
   const bool committee = committee_registered(c);
-  const pass_scratch S{q->lane.xyz, q->lane.meta, q->lane.vidx, q->lane.miss, q->lane.miss_count, q->lane.side, {q->lane.ev[0], q->lane.ev[1]}, nullptr};
-  HS_TRY(launch_main(c, L, r.n, committee, false, ctx_tables(c), S, s, [](bool) { return HS_OK; }));
+  const pass_scratch P{S.xyz, S.meta, S.vidx, S.miss, S.miss_count, L.buf.side, {S.ev[0], S.ev[1]}, nullptr};
+  HS_TRY(launch_main(c, I, r.n, committee, false, ctx_tables(c), P, s, [](bool) { return HS_OK; }));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
-  HS_TRY(launch_finish(c, L, r.n, q->lane.xyz, q->lane.meta, HS_MODE_STRICT, m + r.o_mo, q->lane.items, peer_route{}, fin_group, s));
-  HS_CUDA(c, cudaMemsetAsync(q->lane.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
-  uint8_t *res = q->lane.arena.d + r.a_off;
-  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(q->lane.items, reinterpret_cast<const uint32_t *>(m + r.o_gi), r.n, r.n_groups, q->lane.grej,
-                                                    reinterpret_cast<uint32_t *>(res + r.o_res), committee ? q->lane.miss_count.get() : nullptr,
-                                                    reinterpret_cast<uint32_t *>(res + r.o_tail), r.seq, q->lane.counter);
+  HS_TRY(launch_finish(c, I, r.n, S.xyz, S.meta, HS_MODE_STRICT, m + B.o_mo, S.items, peer_route{}, fin_group, s));
+  HS_CUDA(c, cudaMemsetAsync(S.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
+  uint8_t *res = L.buf.arena.d + r.a_off;
+  k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(S.items, reinterpret_cast<const uint32_t *>(m + B.o_gi), r.n, r.n_groups, S.grej,
+                                                    reinterpret_cast<uint32_t *>(res + B.o_res), committee ? S.miss_count.get() : nullptr,
+                                                    reinterpret_cast<uint32_t *>(res + B.o_tail), r.seq, S.counter);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
 }
-static void batch_dispatch(hs_queue *q) {
-  hs_queue::breq *r;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    r = q->b_cur = &q->bq.front();
-    r->seq = ++q->b_seq ? q->b_seq : ++q->b_seq;  // never 0: the region's tail was zeroed at submit
+static void batch_count(side_lane &L) {
+  for (const lane_req *r : L.launch) {
+    L.stats[0]++;
+    L.stats[1] += r->n;
+    L.stats[2] += r->n_groups;
+    L.stats[3] += r->pre_bytes;
+    L.stats[4] += reinterpret_cast<const volatile uint32_t *>(L.buf.arena.h + r->a_off + r->o_tail)[0];
   }
-  if (batch_launch(q, *r) != HS_OK) batch_complete(q, HS_ERR_CUDA);
-}
-// The request in flight is done when its completion word carries its number.  When `query`, the lane's streams are queried first: a
-// CUDA error, or both streams drained without the word, completes it with HS_ERR_CUDA (never an accept).
-static void batch_watch(hs_queue *q, bool query) {
-  if (!q->b_cur) return;
-  const hs_queue::breq &r = *q->b_cur;
-  cudaError_t qe[2] = {cudaErrorNotReady, cudaErrorNotReady};
-  if (query) {
-    qe[0] = cudaStreamQuery(q->lane.stream);
-    qe[1] = cudaStreamQuery(q->lane.side);
-  }
-  int status = -1;
-  for (cudaError_t x : qe)
-    if (x != cudaSuccess && x != cudaErrorNotReady) status = fail(q->c, HS_ERR_CUDA, "verify queue batch pass", x);
-  if (status < 0 && reinterpret_cast<const volatile uint32_t *>(q->lane.arena.h + r.a_off + r.o_tail)[1] == r.seq) {
-    std::atomic_thread_fence(std::memory_order_acquire);
-    status = HS_OK;
-  } else if (status < 0 && qe[0] == cudaSuccess && qe[1] == cudaSuccess) {
-    status = fail(q->c, HS_ERR_CUDA, "verify queue: k_batch_done did not complete");
-  }
-  if (status >= 0) batch_complete(q, status);
-}
-static bool batch_ready_locked(const hs_queue *q) { return !q->b_cur && !q->bq.empty() && q->bq.front().ready; }
-// Waits for the lane's last pass (the lane is off and bq is empty): its buffers may be released after this.
-static void batch_drain(hs_queue *q) {
-  if (q->lane.stream) cudaStreamSynchronize(q->lane.stream);
-  if (q->lane.side) cudaStreamSynchronize(q->lane.side);
 }
 
 // ---- explain lane (hs_queue_submit_explain, hs_queue_submit_explain_msgs): k_queue_explain over every ready request, on the lane's stream
 // An explain ticket's bits: the why bytes packed four to a word, little-endian.
 static uint32_t explain_bits(uint64_t n) { return (uint32_t)(32 * ((n + 3) / 4)); }
-static bool explain_ready_locked(const hs_queue *q) { return !q->x_launched && !q->xq.empty() && q->xq.front().ready; }
-// Retires the launch in flight once every request of it has completed and their callbacks have run (under q->mu): counts it when it ran
-// (ok), releases its regions and drops its requests.  hs_queue_explain waits for xq to empty, so a resize returns after the callbacks.
-static void explain_retire_locked(hs_queue *q, bool ok) {
-  if (ok) {
-    q->xstats[0]++;
-    q->xstats[1] += q->x_launch_recs;
-    q->xstats[2] += q->x_launched;
-  }
-  q->x_arena.release_to(q->xq[q->x_launched - 1].a_end);
-  q->xq.erase(q->xq.begin(), q->xq.begin() + (long)q->x_launched);
-  q->x_launched = 0;
-  q->cv_done.notify_all();  // for callback tickets too: hs_queue_explain waits for xq to drain
-}
-// One launch takes every ready request at the front of xq.  Their regions are one span of arena positions, which crosses the bus in at
-// most two copies (the span may wrap once) into the mirror; the context's mutex is held only while the copies and the launch are
-// enqueued, and the launch reads no context table, so nothing else of the context waits for it.
-static void explain_dispatch(hs_queue *q) {
+// The launch's regions are one span of arena positions, which crosses the bus in at most two copies (the span may wrap once) into the
+// mirror, tails included: k_queue_explain counts in the mirror's tails.  The launch reads no context table, so nothing else of the
+// context waits for it.
+static int explain_enqueue(hs_queue *q, side_lane &L) {
   hs_ctx *c = q->c;
-  uint32_t k = 0;
-  uint64_t recs = 0, p0 = 0, p1 = 0;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    const uint32_t seq = ++q->x_seq ? q->x_seq : ++q->x_seq;  // never 0: the regions' tails were zeroed at submit
-    for (; k < q->xq.size() && q->xq[k].ready; k++) {
-      hs_queue::xreq &r = q->xq[k];
-      r.seq = seq;
-      q->xlane.list.h[k] = xq_desc{r.a_off, r.n, (uint32_t)recs, r.m, r.pre_bytes, seq, 0};
-      recs += r.n;
-    }
-    q->x_launched = k;
-    q->x_launch_recs = recs;
-    p0 = q->xq.front().a_pos;
-    p1 = q->xq[k - 1].a_end;
+  uint32_t recs = 0;
+  for (size_t k = 0; k < L.launch.size(); k++) {
+    const lane_req &r = *L.launch[k];
+    q->explain_scr.list.h[k] = xq_desc{r.a_off, r.n, recs, r.m, (uint32_t)r.pre_bytes, r.seq, 0};
+    recs += r.n;
   }
-  cudaError_t e;
-  {
-    std::lock_guard<std::mutex> g(c->mu);
-    cudaStream_t s = q->xlane.stream;
-    const uint64_t o0 = q->x_arena.off(p0), first = std::min(p1 - p0, q->x_arena.cap - o0);
-    e = cudaMemcpyAsync(q->xlane.mirror + o0, q->xlane.arena.h + o0, first, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess && p1 - p0 > first) e = cudaMemcpyAsync(q->xlane.mirror.get(), q->xlane.arena.h, p1 - p0 - first, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_queue_explain(c, q->xlane.list.d, k, (uint32_t)recs, q->xlane.mirror, q->xlane.arena.d, s);
-    if (e != cudaSuccess) fail(c, HS_ERR_CUDA, "verify queue explain launch", e);
-  }
-  if (e == cudaSuccess) return;
-  std::vector<queue_completion> fire;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    for (uint32_t i = 0; i < k; i++) ticket_close_locked(q, q->xq[i].sink, HS_ERR_CUDA, explain_bits(q->xq[i].n), nullptr, fire);
-  }
-  queue_fire(fire);
-  std::lock_guard<std::mutex> g(q->mu);
-  explain_retire_locked(q, false);
+  cudaStream_t s = L.buf.stream;
+  const uint64_t p0 = L.launch.front()->a_pos, p1 = L.launch.back()->a_end;
+  const uint64_t o0 = L.ring.off(p0), first = std::min(p1 - p0, L.ring.cap - o0);
+  cudaError_t e = cudaMemcpyAsync(L.buf.mirror + o0, L.buf.arena.h + o0, first, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess && p1 - p0 > first) e = cudaMemcpyAsync(L.buf.mirror.get(), L.buf.arena.h, p1 - p0 - first, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = launch_queue_explain(c, q->explain_scr.list.d, (uint32_t)L.launch.size(), recs, L.buf.mirror, L.buf.arena.d, s);
+  return e == cudaSuccess ? HS_OK : fail(c, HS_ERR_CUDA, "verify queue explain launch", e);
 }
-// Completes each request of the launch in flight whose completion word carries the launch's number.  When `query`, the lane's stream is
-// queried first: a CUDA error, or a drained stream with a word still missing, completes the open requests with HS_ERR_CUDA (never an
-// explanation).
-static void explain_watch(hs_queue *q, bool query) {
-  if (!q->x_launched) return;  // (set and cleared on this thread)
-  cudaError_t qe = query ? cudaStreamQuery(q->xlane.stream) : cudaErrorNotReady;
-  if (qe != cudaSuccess && qe != cudaErrorNotReady) fail(q->c, HS_ERR_CUDA, "verify queue explain launch", qe);
-  std::vector<queue_completion> fire;
-  bool open = false, ok = true;
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    for (size_t k = 0; k < q->x_launched; k++) {
-      hs_queue::xreq &r = q->xq[k];
-      if (r.done) continue;
-      const xq_layout L = xq_layout_of(r.n, r.m, r.pre_bytes);
-      const uint8_t *a = q->xlane.arena.h + r.a_off;
-      if (reinterpret_cast<const volatile uint32_t *>(a + L.o_tail)[1] == r.seq) {
-        std::atomic_thread_fence(std::memory_order_acquire);
-        ticket_close_locked(q, r.sink, HS_OK, explain_bits(r.n), reinterpret_cast<const uint32_t *>(a + L.o_why), fire);
-        r.done = true;
-      } else if (qe == cudaErrorNotReady) {
-        open = true;
-      } else {
-        if (qe == cudaSuccess) fail(q->c, HS_ERR_CUDA, "verify queue: k_queue_explain did not complete");
-        ticket_close_locked(q, r.sink, HS_ERR_CUDA, explain_bits(r.n), nullptr, fire);
-        r.done = true;
-        ok = false;
-      }
-    }
-  }
-  queue_fire(fire);
-  if (!open) {
-    std::lock_guard<std::mutex> g(q->mu);
-    explain_retire_locked(q, ok);
-  }
+static void explain_count(side_lane &L) {
+  L.stats[0]++;
+  for (const lane_req *r : L.launch) L.stats[1] += r->n;
+  L.stats[2] += L.launch.size();
 }
 
 static size_t queue_small_inflight_locked(const hs_queue *q) {
@@ -3023,6 +3049,7 @@ static bool queue_generic_ready_locked(const hs_queue *q) {
 
 static void queue_main(hs_queue *q) {
   cudaSetDevice(q->c->device);
+  const std::array<side_lane *, 2> lanes = queue_lanes(q);
   std::unique_lock<std::mutex> lk(q->mu);
   for (;;) {
     if (!q->cc_ready.empty()) {  // requests the certificate cache answered at submit
@@ -3033,13 +3060,9 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_fire(fire);
       lk.lock();
-    } else if (batch_ready_locked(q)) {  // first: one short enqueue, and a vote burst would otherwise keep postponing it
+    } else if (side_lane *L = lane_ready_locked(q)) {  // first: one short enqueue, and a vote burst would otherwise keep postponing it
       lk.unlock();
-      batch_dispatch(q);
-      lk.lock();
-    } else if (explain_ready_locked(q)) {  // the same for the explain lane
-      lk.unlock();
-      explain_dispatch(q);
+      lane_dispatch(q, *L);
       lk.lock();
     } else if ((q->launched < q->tail && queue_small_inflight_locked(q) < HS_QUEUE_MAX_INFLIGHT) || queue_generic_ready_locked(q)) {
       // everything pending; only the waiting generic requests while the small launches are at their limit
@@ -3048,11 +3071,12 @@ static void queue_main(hs_queue *q) {
       lk.unlock();
       queue_dispatch(q, lo, hi);
       lk.lock();
-    } else if (!q->inflight.empty() || q->b_cur || q->x_launched) {
+    } else if (!q->inflight.empty() || std::any_of(lanes.begin(), lanes.end(), [](side_lane *L) { return !L->launch.empty(); })) {
       lk.unlock();
       queue_watch(q);
       lk.lock();
-    } else if (q->stop && q->bq.empty() && q->xq.empty()) {  // (a batch or explain request still being copied in is announced on cv_work)
+    } else if (q->stop && std::all_of(lanes.begin(), lanes.end(), [](side_lane *L) { return L->reqs.empty(); })) {
+      // (a lane request still being copied in is announced on cv_work)
       break;
     } else {
       q->cv_work.wait(lk);
@@ -3071,8 +3095,7 @@ static void queue_free(hs_queue *q) {
   // the last launches' blocks have exited before the ring goes
   if (q->ev_last) cudaEventSynchronize(q->ev_last);
   if (q->ev_bulk_last) cudaEventSynchronize(q->ev_bulk_last);
-  batch_drain(q);
-  if (q->xlane.stream) cudaStreamSynchronize(q->xlane.stream);
+  for (side_lane *L : queue_lanes(q)) lane_drain(*L);
   delete q;  // the owners release the rest
 }
 
@@ -4154,6 +4177,45 @@ static int queue_read_stats(hs_queue *q, const char *what, uint64_t *out, uint64
   memcpy(out, q->*arr, sizeof(q->*arr));
   return HS_OK;
 }
+// The same for the first n counters of a side lane's.
+static int queue_read_stats(hs_queue *q, const char *what, uint64_t *out, side_lane hs_queue::*lane, size_t n) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, (std::string(what) + ": bad argument").c_str());
+  std::lock_guard<std::mutex> g(q->mu);
+  memcpy(out, (q->*lane).stats, 8 * n);
+  return HS_OK;
+}
+
+// Submits request r to lane L: under q->mu it checks that the lane is on and that r fits the lane's limits, takes r's region of the
+// arena and joins the lane's list; then fill(region) writes its inputs without the lock, its result words and tail are zeroed, and it
+// becomes ready.  The region is the request's alone until it completes.
+template <class Fill>
+static int lane_submit(hs_queue *q, side_lane &L, const char *what, lane_req r, size_t *out_ticket, Fill fill) {
+  lane_req *p = nullptr;
+  const int rc = queue_submit(q, what, r.sink, r.n_bits, out_ticket, [&](const ticket_sink &s) {
+    if (!L.max_recs) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": the " + L.kind.name + " lane is off (" + L.kind.configure + ")").c_str());
+    if (r.n > L.max_recs || r.size > L.max_bytes)
+      return fail(q->c, HS_ERR_ARG, (std::string(what) + ": larger than the " + L.kind.name + " lane's limits").c_str());
+    const std::optional<uint64_t> start = L.ring.take(r.size);
+    if (!start) return HS_ERR_NOMEM;
+    r.sink = s;
+    r.a_off = L.ring.off(*start);
+    r.a_pos = *start;
+    r.a_end = L.ring.tail = *start + r.size;
+    L.reqs.push_back(r);
+    p = &L.reqs.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
+    return HS_OK;
+  });
+  if (rc != HS_OK) return rc;
+  uint8_t *a = L.buf.arena.h + p->a_off;
+  fill(a);
+  memset(a + p->o_res, 0, p->size - p->o_res);  // result words and the tail
+  {
+    std::lock_guard<std::mutex> g(q->mu);
+    p->ready = true;
+  }
+  q->cv_work.notify_one();
+  return HS_OK;
+}
 }  // extern "C++"
 
 int hs_queue_submit(hs_queue *q, const hs_rec128 *recs, size_t n, uint32_t mode, hs_queue_cb *cb, void *user, size_t *out_ticket) {
@@ -4340,51 +4402,22 @@ int hs_queue_generic_stats(hs_queue *q, uint64_t out[HS_QUEUE_GENERIC_STATS]) {
 int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
   if (!q || (max_items == 0) != (max_bytes == 0) || max_items > HS_QUEUE_BATCH_MAX_ITEMS || max_bytes > HS_QUEUE_BATCH_MAX_BYTES)
     return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_batch: bad argument");
-  hs_ctx *c = q->c;
-  std::lock_guard<std::mutex> cfg(q->b_cfg_mu);
-  {
-    std::unique_lock<std::mutex> lk(q->mu);
-    if (max_items == q->b_max_items && max_bytes == q->b_max_bytes) return HS_OK;
-    q->b_max_items = q->b_max_bytes = 0;  // refuses new batch requests while the lane changes
-    q->cv_done.wait(lk, [q] { return q->bq.empty(); });
-  }
-  HS_CUDA(c, cudaSetDevice(c->device));
-  batch_drain(q);
-  q->lane = {};  // released before the new lane is allocated
-  q->b_arena = byte_ring{};
-  if (!max_items) return HS_OK;
-  uint64_t acap = 4096;  // two of the largest regions fit: one can be filled while the other's pass runs
-  while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
-  batch_lane B;
-  int lo = 0, hi = 0;
-  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = create(B.stream, lo);
-  if (e == cudaSuccess) e = create(B.side, hi);
-  for (event_h &ev : B.ev)
-    if (e == cudaSuccess) e = create(ev);
-  if (e == cudaSuccess) e = alloc(B.arena, acap);
-  if (e == cudaSuccess) e = alloc(B.mirror, acap);
-  if (e == cudaSuccess) e = alloc(B.dig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
-  if (e == cudaSuccess) e = alloc(B.xyz, max_items * 3 * sizeof(fe));
-  if (e == cudaSuccess) e = alloc(B.meta, max_items);
-  if (e == cudaSuccess) e = alloc(B.vidx, max_items * 4);
-  if (e == cudaSuccess) e = alloc(B.miss, max_items * 4);
-  if (e == cudaSuccess) e = alloc(B.miss_count, 4);
-  if (e == cudaSuccess) e = alloc(B.items, (max_items + 31) / 32 * 4);
-  if (e == cudaSuccess) e = alloc(B.grej, max_bytes + 16);  // group words of a region fit in max_bytes
-  if (e == cudaSuccess) e = alloc(B.counter, 4);
-  if (e == cudaSuccess) e = cudaMemset(B.counter, 0, 4);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(c, HS_ERR_NOMEM, "hs_queue_batch: no pinned host or device memory for the batch lane", e);
-  }
-  memset(B.arena.h, 0, acap);
-  q->lane = std::move(B);
-  std::lock_guard<std::mutex> g(q->mu);
-  q->b_arena = byte_ring{acap, 0, 0};
-  q->b_max_items = max_items;
-  q->b_max_bytes = max_bytes;
-  return HS_OK;
+  return lane_configure(q, q->batch, max_items, max_bytes, q->batch_scr, [&](batch_scratch &B, lane_bufs &L, uint64_t, int hi) {
+    cudaError_t e = create(L.side, hi);
+    for (event_h &ev : B.ev)
+      if (e == cudaSuccess) e = create(ev);
+    if (e == cudaSuccess) e = alloc(B.dig, (max_bytes / 8 + 1) * 32);  // a preimage costs at least its 8-byte offset
+    if (e == cudaSuccess) e = alloc(B.xyz, max_items * 3 * sizeof(fe));
+    if (e == cudaSuccess) e = alloc(B.meta, max_items);
+    if (e == cudaSuccess) e = alloc(B.vidx, max_items * 4);
+    if (e == cudaSuccess) e = alloc(B.miss, max_items * 4);
+    if (e == cudaSuccess) e = alloc(B.miss_count, 4);
+    if (e == cudaSuccess) e = alloc(B.items, (max_items + 31) / 32 * 4);
+    if (e == cudaSuccess) e = alloc(B.grej, max_bytes + 16);  // group words of a region fit in max_bytes
+    if (e == cudaSuccess) e = alloc(B.counter, 4);
+    if (e == cudaSuccess) e = cudaMemset(B.counter, 0, 4);
+    return e;
+  });
 }
 
 int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
@@ -4399,40 +4432,21 @@ int hs_queue_submit_batch(hs_queue *q, const uint8_t *preimages, const uint64_t 
       return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: index or mode out of range");
   const uint64_t pre_bytes = pre_off[n_msgs];
   const batch_layout B = batch_layout_of(n_msgs, pre_bytes, n_items, n_groups);
-  hs_queue::breq *r = nullptr;
-  const int rc = queue_submit(q, "hs_queue_submit_batch", ticket_sink{0, cb, user}, batch_bits(n_groups, n_items), out_ticket, [&](const ticket_sink &s) {
-    if (!q->b_max_items) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: the batch lane is off (hs_queue_batch)");
-    if (n_items > q->b_max_items || B.size > q->b_max_bytes) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_batch: larger than the batch lane's limits");
-    const std::optional<uint64_t> start = q->b_arena.take(B.size);
-    if (!start) return HS_ERR_NOMEM;
-    q->b_arena.tail = *start + B.size;
-    q->bq.push_back(hs_queue::breq{s, (uint32_t)n_items, (uint32_t)n_groups, (uint32_t)n_msgs, pre_bytes, q->b_arena.off(*start), q->b_arena.tail,
-                                   B.o_pre, B.o_sig, B.o_pk, B.o_mi, B.o_gi, B.o_mo, B.o_res, B.o_tail, 0, false});
-    r = &q->bq.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
-    return HS_OK;
+  const lane_req r{{0, cb, user}, batch_bits(n_groups, n_items), (uint32_t)n_items, (uint32_t)n_msgs, (uint32_t)n_groups, pre_bytes, B.o_res, B.o_tail, B.size};
+  return lane_submit(q, q->batch, "hs_queue_submit_batch", r, out_ticket, [&](uint8_t *a) {
+    memcpy(a, pre_off, 8 * (n_msgs + 1));
+    if (pre_bytes) memcpy(a + B.o_pre, preimages, pre_bytes);
+    memcpy(a + B.o_sig, sig, 64 * n_items);
+    memcpy(a + B.o_pk, pk, 32 * n_items);
+    memcpy(a + B.o_mi, msg_idx, 4 * n_items);
+    memcpy(a + B.o_gi, group_idx, 4 * n_items);
+    if (modes) memcpy(a + B.o_mo, modes, n_items);
+    else memset(a + B.o_mo, HS_MODE_STRICT, n_items);
   });
-  if (rc != HS_OK) return rc;
-  // the region is this request's alone until it completes: fill it without holding q->mu
-  uint8_t *a = q->lane.arena.h + r->a_off;
-  memcpy(a, pre_off, 8 * (n_msgs + 1));
-  if (pre_bytes) memcpy(a + B.o_pre, preimages, pre_bytes);
-  memcpy(a + B.o_sig, sig, 64 * n_items);
-  memcpy(a + B.o_pk, pk, 32 * n_items);
-  memcpy(a + B.o_mi, msg_idx, 4 * n_items);
-  memcpy(a + B.o_gi, group_idx, 4 * n_items);
-  if (modes) memcpy(a + B.o_mo, modes, n_items);
-  else memset(a + B.o_mo, HS_MODE_STRICT, n_items);
-  memset(a + B.o_res, 0, B.size - B.o_res);  // result words and the completion word
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    r->ready = true;
-  }
-  q->cv_work.notify_one();
-  return HS_OK;
 }
 
 int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]) {
-  return queue_read_stats(q, "hs_queue_batch_stats", out, &hs_queue::bstats);
+  return queue_read_stats(q, "hs_queue_batch_stats", out, &hs_queue::batch, HS_QUEUE_BATCH_STATS);
 }
 
 #define HS_QUEUE_EXPLAIN_MAX_RECORDS (1u << 24)
@@ -4440,77 +4454,17 @@ int hs_queue_batch_stats(hs_queue *q, uint64_t out[HS_QUEUE_BATCH_STATS]) {
 int hs_queue_explain(hs_queue *q, size_t max_records, size_t max_bytes) {
   if (!q || (max_records == 0) != (max_bytes == 0) || max_records > HS_QUEUE_EXPLAIN_MAX_RECORDS || max_bytes > HS_QUEUE_EXPLAIN_MAX_BYTES)
     return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_explain: bad argument");
-  hs_ctx *c = q->c;
-  std::lock_guard<std::mutex> cfg(q->x_cfg_mu);
-  {
-    std::unique_lock<std::mutex> lk(q->mu);
-    if (max_records == q->x_max_records && max_bytes == q->x_max_bytes) return HS_OK;
-    q->x_max_records = q->x_max_bytes = 0;  // refuses new explain requests while the lane changes
-    q->cv_done.wait(lk, [q] { return q->xq.empty(); });
-  }
-  HS_CUDA(c, cudaSetDevice(c->device));
-  if (q->xlane.stream) HS_CUDA(c, cudaStreamSynchronize(q->xlane.stream));
-  q->xlane = {};  // released before the new lane is allocated
-  q->x_arena = byte_ring{};
-  if (!max_records) return HS_OK;
-  uint64_t acap = 4096;  // two of the largest regions fit: one can be filled while the other's launch runs
-  while (acap < 2 * (uint64_t)max_bytes) acap <<= 1;
-  const uint64_t max_reqs = acap / xq_layout_of(1, 0, 0).size + 1;  // regions the arena holds at once
-  explain_lane X;
-  int lo = 0, hi = 0;
-  cudaError_t e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = create(X.stream, lo);
-  if (e == cudaSuccess) e = alloc(X.arena, acap);
-  if (e == cudaSuccess) e = alloc(X.mirror, acap);
-  if (e == cudaSuccess) e = alloc(X.list, max_reqs * sizeof(xq_desc));
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(c, HS_ERR_NOMEM, "hs_queue_explain: no pinned host or device memory for the explain lane", e);
-  }
-  memset(X.arena.h, 0, acap);
-  q->xlane = std::move(X);
-  std::lock_guard<std::mutex> g(q->mu);
-  q->x_arena = byte_ring{acap, 0, 0};
-  q->x_max_records = max_records;
-  q->x_max_bytes = max_bytes;
-  return HS_OK;
-}
-
-// Submits one explain request of n records whose region is laid out by L: under q->mu the request takes its region, then fill(region)
-// writes its records (and preimages) without the lock, and the request becomes ready.
-extern "C++" {
-template <class Fill>
-static int explain_submit(hs_queue *q, const char *what, size_t n, uint64_t m, uint64_t pre_bytes, ticket_sink sink, size_t *out_ticket, Fill fill) {
-  const xq_layout L = xq_layout_of(n, m, pre_bytes);
-  hs_queue::xreq *r = nullptr;
-  const int rc = queue_submit(q, what, sink, explain_bits(n), out_ticket, [&](const ticket_sink &s) {
-    if (!q->x_max_records) return fail(q->c, HS_ERR_ARG, (std::string(what) + ": the explain lane is off (hs_queue_explain)").c_str());
-    if (n > q->x_max_records || L.size > q->x_max_bytes)
-      return fail(q->c, HS_ERR_ARG, (std::string(what) + ": larger than the explain lane's limits").c_str());
-    const std::optional<uint64_t> start = q->x_arena.take(L.size);
-    if (!start) return HS_ERR_NOMEM;
-    q->x_arena.tail = *start + L.size;
-    q->xq.push_back(hs_queue::xreq{s, (uint32_t)n, (uint32_t)m, (uint32_t)pre_bytes, q->x_arena.off(*start), *start, q->x_arena.tail, 0, false, false});
-    r = &q->xq.back();  // stays valid: only the dispatcher pops, and never a request that is not ready
-    return HS_OK;
+  return lane_configure(q, q->explain, max_records, max_bytes, q->explain_scr, [](explain_scratch &X, lane_bufs &, uint64_t acap, int) {
+    const uint64_t max_reqs = acap / xq_layout_of(1, 0, 0).size + 1;  // regions the arena holds at once
+    return alloc(X.list, max_reqs * sizeof(xq_desc));
   });
-  if (rc != HS_OK) return rc;
-  uint8_t *a = q->xlane.arena.h + r->a_off;
-  fill(a, L);
-  memset(a + L.o_why, 0, L.size - L.o_why);  // why bytes (the last word's unused bytes stay 0), the count and the completion word
-  {
-    std::lock_guard<std::mutex> g(q->mu);
-    r->ready = true;
-  }
-  q->cv_work.notify_one();
-  return HS_OK;
 }
-}  // extern "C++"
 
 int hs_queue_submit_explain(hs_queue *q, const hs_rec128 *recs, size_t n, hs_queue_cb *cb, void *user, size_t *out_ticket) {
   if (!q || !recs || n == 0 || n > HS_QUEUE_EXPLAIN_MAX_RECORDS) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_submit_explain: bad argument");
-  return explain_submit(q, "hs_queue_submit_explain", n, 0, 0, ticket_sink{0, cb, user}, out_ticket,
-                        [&](uint8_t *a, const xq_layout &) { memcpy(a, recs, n * sizeof(hs_rec128)); });
+  const xq_layout L = xq_layout_of(n, 0, 0);
+  const lane_req r{{0, cb, user}, explain_bits(n), (uint32_t)n, 0, 0, 0, L.o_why, L.o_tail, L.size};
+  return lane_submit(q, q->explain, "hs_queue_submit_explain", r, out_ticket, [&](uint8_t *a) { memcpy(a, recs, n * sizeof(hs_rec128)); });
 }
 
 int hs_queue_submit_explain_msgs(hs_queue *q, const uint8_t *preimages, const uint64_t *pre_off, size_t n_msgs, const uint8_t *sig, const uint8_t *pk,
@@ -4522,21 +4476,22 @@ int hs_queue_submit_explain_msgs(hs_queue *q, const uint8_t *preimages, const ui
   for (size_t i = 0; i < n; i++)
     if (msg_idx[i] >= n_msgs) return fail(q->c, HS_ERR_ARG, "hs_queue_submit_explain_msgs: message index out of range");
   const uint64_t pre_bytes = pre_off[n_msgs];
-  return explain_submit(q, "hs_queue_submit_explain_msgs", n, n_msgs, pre_bytes, ticket_sink{0, cb, user}, out_ticket,
-                        [&](uint8_t *a, const xq_layout &L) {
-                          for (size_t i = 0; i < n; i++) {
-                            memcpy(a + 128 * i, sig + 64 * i, 64);
-                            memcpy(a + 128 * i + 64, pk + 32 * i, 32);
-                            memset(a + 128 * i + 96, 0, 32);
-                          }
-                          memcpy(a + L.o_off, pre_off, 8 * (n_msgs + 1));
-                          memcpy(a + L.o_mi, msg_idx, 4 * n);
-                          if (pre_bytes) memcpy(a + L.o_pre, preimages, pre_bytes);
-                        });
+  const xq_layout L = xq_layout_of(n, n_msgs, pre_bytes);
+  const lane_req r{{0, cb, user}, explain_bits(n), (uint32_t)n, (uint32_t)n_msgs, 0, pre_bytes, L.o_why, L.o_tail, L.size};
+  return lane_submit(q, q->explain, "hs_queue_submit_explain_msgs", r, out_ticket, [&](uint8_t *a) {
+    for (size_t i = 0; i < n; i++) {
+      memcpy(a + 128 * i, sig + 64 * i, 64);
+      memcpy(a + 128 * i + 64, pk + 32 * i, 32);
+      memset(a + 128 * i + 96, 0, 32);
+    }
+    memcpy(a + L.o_off, pre_off, 8 * (n_msgs + 1));
+    memcpy(a + L.o_mi, msg_idx, 4 * n);
+    if (pre_bytes) memcpy(a + L.o_pre, preimages, pre_bytes);
+  });
 }
 
 int hs_queue_explain_stats(hs_queue *q, uint64_t out[HS_QUEUE_EXPLAIN_STATS]) {
-  return queue_read_stats(q, "hs_queue_explain_stats", out, &hs_queue::xstats);
+  return queue_read_stats(q, "hs_queue_explain_stats", out, &hs_queue::explain, HS_QUEUE_EXPLAIN_STATS);
 }
 
 void hs_queue_destroy(hs_queue *q) {

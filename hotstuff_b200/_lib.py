@@ -87,6 +87,10 @@ SIGNATURES = {
     "hs_key_slots": (c_size_t, [c_void_p]),
     "hs_table_audit": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32)]),
     "hs_table_repair": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32), ctypes.POINTER(c_u32)]),
+    "hs_scrub_start": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_u32, c_u32, c_u32, c_void_p, c_void_p]),
+    "hs_scrub_set_map": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t]),
+    "hs_scrub_stop": (c_int, [c_void_p]),
+    "hs_scrub_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_explain_rec128": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "hs_multi_create": (c_int, [ctypes.POINTER(c_void_p), c_void_p, c_size_t, c_u32]),
     "hs_multi_destroy": (None, [c_void_p]),
@@ -103,6 +107,8 @@ SIGNATURES = {
 
 # hs_queue_cb: void (void *user, size_t ticket, int status, const uint32_t *bitmap)
 QUEUE_CB = ctypes.CFUNCTYPE(None, c_void_p, c_size_t, c_int, ctypes.POINTER(c_u32))
+# hs_scrub_cb: void (void *user, uint32_t found, uint32_t failed, size_t first_slot)
+SCRUB_CB = ctypes.CFUNCTYPE(None, c_void_p, c_u32, c_u32, c_size_t)
 
 _lib = None
 

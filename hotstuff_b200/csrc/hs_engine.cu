@@ -21,9 +21,11 @@
 //   (one warp per long message, schedules expanded across lanes).
 // Front ends: QC / TC / Timeout / Block groups with on-GPU digests and per-certificate AND; load-generation keygen / signer.
 #include <cuda_runtime.h>
+#include <pthread.h>
 #include <algorithm>
 #include <array>
 #include <atomic>
+#include <chrono>
 #include <condition_variable>
 #include <cstdint>
 #include <cstdio>
@@ -40,6 +42,7 @@
 #include <random>
 #include <string>
 #include <string_view>
+#include <system_error>
 #include <thread>
 #include <unordered_map>
 #include <vector>
@@ -1146,6 +1149,48 @@ __global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_ni
   }
   if (!ok) audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
 }
+// The range form (hs_scrub_start): entries [first, first + count) of the base-point table, entry e being entry e % (2^(W-1) + 1) of
+// window e / (2^(W-1) + 1), the table's storage order.  Warp g takes the g-th run of 32 entries of one window from the run holding
+// `first`, with the checks above; a lane outside the range only feeds the shuffles.  An entry's checks read its own window and, for
+// entry 1, entry 2^(W-1) of the window before, so slices that together cover the table find exactly what the full audit finds, and
+// report it with the same key.  An overload of the unlisted form, so the two forms above keep their code.
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, uint64_t first, uint64_t count,
+                                                                       int W, int n_windows, audit_out O) {
+  static_assert(!LISTED, "the range form covers the base-point table");
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t H = (uint64_t)1 << (W - 1), stride = H + 1, runs = (H + 1 + 31) / 32;
+  const uint64_t r = (first / stride) * runs + (first % stride) / 32 + (uint64_t)blockIdx.x * HS_AUDIT_WARPS + (threadIdx.x >> 5);
+  const uint64_t win = r / runs;
+  if (win >= (uint64_t)n_windows) return;  // whole warps leave together
+  const uint32_t m = (uint32_t)((r % runs) * 32 + lane);
+  const uint64_t idx = win * stride + m;
+  const bool in_window = m <= H, in = in_window && idx >= first && idx - first < count;
+  if (!__any_sync(0xffffffffu, in)) return;
+  const ge_niels *wt = tables + win * stride;
+  ge_niels e, prev, one;
+  niels_load_stream(e, wt + (in_window ? m : H));
+  niels_load(one, wt + 1);
+  {
+    uint32_t *pe = reinterpret_cast<uint32_t *>(&e), *pp = reinterpret_cast<uint32_t *>(&prev);
+#pragma unroll
+    for (int j = 0; j < 24; j++) pp[j] = __shfl_up_sync(0xffffffffu, pe[j], 1);
+  }
+  if (lane == 0 && m > 0) niels_load(prev, wt + m - 1);
+  uint32_t ok = in ? audit_entry_local(e, prev, one, m) : 1u;
+  if (in && m == 1) {
+    if (win == 0) {
+      ge_ext P;
+      audit_anchor_point(P, nullptr);
+      ok &= audit_anchor(e, P);
+    } else {
+      ge_niels last;
+      niels_load(last, wt - stride + H);
+      ok &= audit_link(e, last);
+    }
+  }
+  if (!ok) audit_report(O, 0, HS_AUDIT_BASE, audit_key(0, (uint32_t)win + 1, m));
+}
 
 // ------------------------------------------------------------------------------------------------ explanation of a verdict
 // hs_explain_rec128: a thread per packed hs_rec128 record, grid-stride, one HS_WHY_* byte out per record.  It reads the records and
@@ -1606,6 +1651,28 @@ struct committee_stage {
   std::vector<uint8_t> flags;   // their proved flag bytes
   std::vector<uint32_t> remove; // the slots the commit takes out of service
 };
+// The engine-owned scrub (hs_scrub_start): its thread, the map it audits against and where its pass stands.  `m` guards all but `th`
+// (hs_scrub_start / hs_scrub_stop, under hs_ctx::scrub_life) and the counters (read at any time).  Lock order: m, audit_mu, mu.
+enum { SCRUB_PASSES, SCRUB_SLOTS, SCRUB_BASE, SCRUB_TICKS, SCRUB_FINDINGS, SCRUB_REPAIRED, SCRUB_FAILED, SCRUB_PAUSED, SCRUB_NSTATS };
+struct scrub_state {
+  std::thread th;
+  std::mutex m;
+  std::condition_variable cv;
+  bool stop = false;
+  int rc = 0;                       // the error that ended the thread early (returned by hs_scrub_stop)
+  // the map: the caller's (has_pks / has_live) or the engine's own, for the slot map of generation map_gen
+  std::vector<uint8_t> pks;
+  std::vector<uint32_t> live;
+  bool has_pks = false, has_live = false;
+  size_t n_slots = 0;
+  uint64_t map_gen = 0;
+  uint32_t period_us = 0, slots_per_tick = 0, base_per_tick = 0;
+  hs_scrub_cb *cb = nullptr;
+  void *user = nullptr;
+  size_t next_slot = 0;             // the pass: the slots before next_slot and the base entries before next_base are audited
+  uint64_t next_base = 0;
+  std::atomic<uint64_t> stats[SCRUB_NSTATS] = {};
+};
 struct hs_ctx {
   int device = 0;
   unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
@@ -1641,8 +1708,13 @@ struct hs_ctx {
   // key-table generation: bumped (under mu) by every path that frees or rewrites the per-key tables, key bytes, flags or hash table, so
   // an audit that ran across such a change reports nothing.  Those paths first wait for audit.done (or synchronise the device).
   uint64_t key_gen = 0;
+  // slot-map generation: bumped with key_gen by registration, hs_committee_update, hs_committee_commit and the key cache's changes,
+  // i.e. whenever hs_key_slots or a slot's key or liveness changes; a repair restores the map and leaves it alone.
+  uint64_t map_gen = 0;
   std::mutex audit_mu;               // one hs_table_audit at a time: it owns `audit` for the whole call, `mu` only briefly
   audit_state audit;
+  std::mutex scrub_life;             // hs_scrub_start / hs_scrub_stop: starting and joining the scrub's thread
+  scrub_state scrub;
   // multi-GPU peer routing
   peer_route peers{};
   int peer_rank = 0;
@@ -1793,11 +1865,13 @@ static void set_window(comb_params &cp, bool a, int w) {
 // Before a key-cache path rewrites tables, key bytes or the hash table on `stream`: an audit's kernels in flight finish first.
 static int audit_fence(hs_ctx *c, cudaStream_t stream) {
   c->key_gen++;
+  c->map_gen++;
   if (c->audit.done) HS_CUDA(c, cudaStreamWaitEvent(stream, c->audit.done, 0));
   return HS_OK;
 }
 static void cache_release(hs_ctx *c) {  // callers have synchronised the device
   c->key_gen++;
+  c->map_gen++;
   c->keys = {};
   c->n_keys = 0;
   c->h_pks.clear();
@@ -1826,6 +1900,7 @@ static int cache_allocate(hs_ctx *c, cudaStream_t stream) {
   c->a_table_entries = comb_table_entries(wa);
   HS_CUDA(c, make_key_store(c->keys, c->cache_cap, key_index::capacity_for(c->cache_cap), wa, stream));
   c->key_gen++;  // nothing to wait for: the store had no tables, so no audit reads it
+  c->map_gen++;
   c->h_index.reset(c->cache_cap);
   c->h_pks.clear();
   return HS_OK;
@@ -3211,6 +3286,7 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
 
 void hs_ctx_destroy(hs_ctx *c) {
   if (!c) return;
+  hs_scrub_stop(c);  // joins the scrub's thread before anything it uses goes
   std::vector<hs_queue *> qs;
   {
     std::lock_guard<std::mutex> g(c->queues_mu);
@@ -3424,6 +3500,7 @@ int hs_committee_update(hs_ctx *c, const uint8_t *add_pks, size_t n_add, const u
     if (remove_idx[i] >= c->n_keys) return fail(c, HS_ERR_ARG, "hs_committee_update: remove index out of range");
   stage_drop(c);
   c->key_gen++;
+  c->map_gen++;
   for (size_t i = 0; i < n_remove; i++) {
     c->h_key_live[remove_idx[i]] = 0;
     HS_CUDA(c, cudaMemsetAsync(c->keys.key_flags + remove_idx[i], 0, 1, c->stream));
@@ -4931,17 +5008,25 @@ static std::string audit_message(uint64_t first, size_t n_slots, const uint32_t 
   return m;
 }
 
+// Entries [first, first + count) of the base-point table, count > 0 (the range form of k_table_audit).
+struct base_range {
+  uint64_t first, count;
+};
 // k_table_audit over n_tables tables on `stream`: tables 0 .. n_tables - 1, or with d_slots the listed slots' (auditable and findings by
-// list position).  auditable: nullable for the base-point table.
+// list position), or with `range` that range of the base-point table.  auditable: nullable for the base-point table.
 static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *tables, const uint32_t *d_slots, size_t n_tables, size_t entries,
-                              int W, int n_windows, const uint8_t *pks, const uint8_t *auditable, const audit_out &O) {
-  const uint64_t warps = (uint64_t)n_tables * n_windows * ((((uint64_t)1 << (W - 1)) + 1 + 31) / 32);
-  const auto launch = [&](auto listed) {
-    k_table_audit<decltype(listed)::value><<<(unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS), 32 * HS_AUDIT_WARPS, 0, stream>>>(
-        tables, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
+                              int W, int n_windows, const uint8_t *pks, const uint8_t *auditable, const audit_out &O,
+                              const base_range *range = nullptr) {
+  const uint64_t stride = comb_window_stride(W), runs = (stride + 31) / 32;
+  const auto run_of = [&](uint64_t e) { return e / stride * runs + e % stride / 32; };
+  const uint64_t warps = range ? run_of(range->first + range->count - 1) - run_of(range->first) + 1 : (uint64_t)n_tables * n_windows * runs;
+  const unsigned blocks = (unsigned)((warps + HS_AUDIT_WARPS - 1) / HS_AUDIT_WARPS);
+  const auto launch = [&](auto listed, auto... args) {
+    k_table_audit<decltype(listed)::value><<<blocks, 32 * HS_AUDIT_WARPS, 0, stream>>>(tables, args...);
   };
-  if (d_slots) launch(std::true_type{});
-  else launch(std::false_type{});
+  if (range) launch(std::false_type{}, range->first, range->count, W, n_windows, O);
+  else if (d_slots) launch(std::true_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
+  else launch(std::false_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
@@ -4977,9 +5062,17 @@ struct audit_run {
     return f;
   }
 };
-// Checks the arguments, snapshots the slots and their liveness, uploads and enqueues.  Nothing here waits for a kernel.
+// Part of an audit (a scrub tick): the KEY / FLAG / LOOKUP checks of every slot and hash entry as the complete audit runs them (a
+// thread each), the comb tables of the slots in `tables` only, and entries [base_first, base_first + base_count) of the base-point table.
+// Findings land at the slots' own bits; the first-finding key names a slot relative to its run and is not read.
+struct audit_slice {
+  std::vector<std::pair<size_t, size_t>> tables;  // [begin, end) runs of slots
+  uint64_t base_first = 0, base_count = 0;
+};
+// Checks the arguments, snapshots the slots and their liveness, uploads and enqueues: the complete audit, or with `slice` that part.
+// Nothing here waits for a kernel.
 static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots,
-                                audit_run &r) {
+                                audit_run &r, const audit_slice *slice = nullptr) {
   audit_state &A = c->audit;
   HS_CUDA(c, cudaSetDevice(c->device));
   const size_t n = has_key_tables(c) ? c->n_keys : 0;
@@ -5006,9 +5099,19 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
         expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
-    HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
+    if (!slice)
+      HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
+    for (const auto &[b, e] : slice ? slice->tables : std::vector<std::pair<size_t, size_t>>{})  // a run: the same form on that window of the arrays
+      if (b < e && e <= n)
+        HS_TRY(launch_table_audit(c, A.stream, c->keys.atables + b * c->a_table_entries, nullptr, e - b, c->a_table_entries, c->cp.wa, c->cp.na,
+                                  c->keys.pks + 32 * b, in.ptr(s_ok) + b, audit_out{O.first, O.bits + b}));
   }
-  HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
+  if (!slice) {
+    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
+  } else if (slice->base_count) {
+    const base_range R{slice->base_first, slice->base_count};
+    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O, &R));
+  }
   HS_CUDA(c, cudaEventRecord(A.done, A.stream));
   r.gen = c->key_gen;
   r.n_slots = n;
@@ -5259,6 +5362,7 @@ extern "C" int hs_committee_commit(hs_ctx *c) {
   // A launch in flight that resolved a key to a removed slot must not see its flag cleared.  Adding slots disturbs no launch in flight.
   if (!S.remove.empty()) HS_CUDA(c, cudaDeviceSynchronize());
   c->key_gen++;
+  c->map_gen++;
   for (size_t k = 0; k < S.fresh.size(); k++) {
     const uint32_t s = S.fresh[k];
     if (s >= c->n_keys) {  // a spare: the spares a stage takes follow n_keys without a gap
@@ -5282,6 +5386,199 @@ extern "C" int hs_committee_discard(hs_ctx *c) {
   std::lock_guard<std::mutex> ga(c->audit_mu);
   std::lock_guard<std::mutex> g(c->mu);
   stage_drop(c);
+  return HS_OK;
+}
+
+// ---- the engine-owned scrub of the live key tables (hs_scrub_start / hs_scrub_set_map / hs_scrub_stop / hs_scrub_stats)
+// Takes the caller's map (or the engine's own) for the current slot map, under S.m: the rules of hs_table_audit.  A new map starts a
+// new pass.
+static int scrub_map_locked(hs_ctx *c, scrub_state &S, const char *entry, const uint8_t *pks, const uint32_t *live, size_t n_slots) {
+  std::lock_guard<std::mutex> g(c->mu);
+  const size_t n = has_key_tables(c) ? c->n_keys : 0;
+  if (n_slots != n) return fail_args(c, entry, ("n_slots is " + std::to_string(n_slots) + ", hs_key_slots is " + std::to_string(n)).c_str());
+  if (pks && n && !c->explicit_committee) return fail_args(c, entry, "key-cache tables are scrubbed with expect_pks == NULL");
+  S.has_pks = pks && n;
+  S.has_live = live && n;
+  S.pks.assign(S.has_pks ? pks : nullptr, S.has_pks ? pks + 32 * n : nullptr);
+  S.live.assign(S.has_live ? live : nullptr, S.has_live ? live + (n + 31) / 32 : nullptr);
+  S.n_slots = n;
+  S.map_gen = c->map_gen;
+  S.next_slot = 0;
+  S.next_base = 0;
+  return HS_OK;
+}
+// What one tick found, for the callback: the classes found, those its proof still finds, the lowest slot with a finding.
+struct scrub_report {
+  uint32_t found = 0, failed = 0;
+  size_t first_slot = SIZE_MAX;
+};
+// The runs of slots with a finding in `r` whose tables `sl` does not cover.
+static std::vector<std::pair<size_t, size_t>> scrub_flagged_outside(const audit_run &r, const audit_slice &sl) {
+  std::vector<std::pair<size_t, size_t>> out;
+  for (size_t s = 0; s < r.n_slots; s++) {
+    if (!r.bits()[2 + s] || std::any_of(sl.tables.begin(), sl.tables.end(), [s](const auto &t) { return t.first <= s && s < t.second; })) continue;
+    if (!out.empty() && out.back().second == s) out.back().second = s + 1;
+    else out.push_back({s, s + 1});
+  }
+  return out;
+}
+static uint64_t scrub_items(const audit_run &r) {  // the slots, the base-point table and the stray hash entries with a finding
+  uint64_t k = (r.bits()[0] ? 1 : 0) + (r.bits()[1] ? 1 : 0);
+  for (size_t s = 0; s < r.n_slots; s++) k += r.bits()[2 + s] ? 1 : 0;
+  return k;
+}
+// One tick, under S.m: audit the next slice against the map; on a finding, audit the flagged slots' tables too, repair exactly what
+// was found (repair_locked, as hs_table_repair does) and prove it by auditing the slice again.  A slot map newer than the scrub's map
+// pauses the tick.  Errors other than a map change end the scrub.
+static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
+  const char *entry = "hs_scrub", *changed = "key tables changed during a scrub tick";
+  const uint8_t *pks = S.has_pks ? S.pks.data() : nullptr;
+  const uint32_t *live = S.has_live ? S.live.data() : nullptr;
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  audit_run r;
+  audit_slice sl;
+  uint64_t live_slots = 0;
+  size_t s = S.next_slot;
+  const uint64_t E = comb_table_entries(c->cp.wb);
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    if (c->map_gen != S.map_gen) {
+      S.stats[SCRUB_PAUSED]++;
+      return HS_OK;
+    }
+    // the next slots_per_tick slots in service, with the slots out of service up to the next one in service (they have no table)
+    const auto in_service = [c](size_t k) { return !c->explicit_committee || (c->h_key_live[k] && c->h_key_live[k] != SLOT_STAGED); };
+    while (s < S.n_slots && (live_slots < S.slots_per_tick || !in_service(s))) live_slots += in_service(s++) ? 1 : 0;
+    sl.tables.push_back({S.next_slot, s});
+    sl.base_first = S.next_base;
+    sl.base_count = std::min<uint64_t>(S.base_per_tick, E - S.next_base);
+    HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, r, &sl));
+  }
+  int rc = audit_collect(c, entry, changed, r);
+  if (rc == HS_ERR_ARG) {  // the slot map changed under the tick: nothing it found counts, and the next tick pauses
+    S.stats[SCRUB_PAUSED]++;
+    return HS_OK;
+  }
+  HS_TRY(rc);
+  S.stats[SCRUB_TICKS]++;
+  S.stats[SCRUB_SLOTS] += live_slots;
+  S.stats[SCRUB_BASE] += sl.base_count;
+  S.next_slot = s;
+  S.next_base += sl.base_count;
+  if (S.next_slot >= S.n_slots && S.next_base >= E) {
+    S.stats[SCRUB_PASSES]++;
+    S.next_slot = 0;
+    S.next_base = 0;
+  }
+  if (!r.failed()) return HS_OK;
+  // A slot the slot checks flagged outside the slice: its table decides what the repair rebuilds (key bytes that changed without a
+  // map to compare them with show as LOOKUP here, and as TABLE through the anchor).
+  const auto outside = scrub_flagged_outside(r, sl);
+  if (!outside.empty()) {
+    audit_run t;
+    audit_slice st;
+    st.tables = outside;
+    {
+      std::lock_guard<std::mutex> g(c->mu);
+      HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, t, &st));
+    }
+    rc = audit_collect(c, entry, changed, t);
+    if (rc == HS_ERR_ARG) {
+      S.stats[SCRUB_PAUSED]++;
+      return HS_OK;
+    }
+    HS_TRY(rc);
+    uint32_t *bits = reinterpret_cast<uint32_t *>(r.res.data() + 8);
+    for (size_t k = 0; k < 2 + r.n_slots; k++) bits[k] |= t.bits()[k];
+    sl.tables.insert(sl.tables.end(), outside.begin(), outside.end());
+  }
+  rep.found = r.failed();
+  for (size_t k = 0; k < r.n_slots && rep.first_slot == SIZE_MAX; k++)
+    if (r.bits()[2 + k]) rep.first_slot = k;
+  audit_run last;
+  {
+    std::unique_lock<std::mutex> g(c->mu);
+    rc = repair_locked(c, g, r, pks, live, changed);
+    if (rc == HS_OK) rc = audit_enqueue_locked(c, entry, pks, live, S.n_slots, last, &sl);
+  }
+  if (rc == HS_OK) rc = audit_collect(c, entry, changed, last);
+  if (rc != HS_OK && rc != HS_ERR_ARG) return rc;
+  // A repair the slot map changed under is not proved: its findings count as failed.
+  const audit_run &after = rc == HS_OK ? last : r;
+  rep.failed = after.failed();
+  S.stats[SCRUB_FINDINGS] += scrub_items(r);
+  S.stats[SCRUB_FAILED] += scrub_items(after);
+  for (size_t k = 0; k < r.n_slots; k++) S.stats[SCRUB_REPAIRED] += (r.bits()[2 + k] && !after.bits()[2 + k]) ? 1 : 0;
+  return HS_OK;
+}
+static void scrub_loop(hs_ctx *c) {
+  scrub_state &S = c->scrub;
+  pthread_setname_np(pthread_self(), "hs_scrub");  // names it in ps / top and /proc/<pid>/task/*/comm
+  cudaSetDevice(c->device);
+  std::unique_lock<std::mutex> l(S.m);
+  while (!S.cv.wait_for(l, std::chrono::microseconds(S.period_us), [&S] { return S.stop; })) {
+    scrub_report rep;
+    if ((S.rc = scrub_tick(c, S, rep)) != HS_OK) return;
+    if (rep.found && S.cb) {  // without S.m: the callback may call hs_scrub_set_map
+      l.unlock();
+      S.cb(S.user, rep.found, rep.failed, rep.first_slot);
+      l.lock();
+    }
+  }
+}
+
+extern "C" int hs_scrub_start(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots, uint32_t period_us,
+                              uint32_t slots_per_tick, uint32_t base_entries_per_tick, hs_scrub_cb *cb, void *user) {
+  if (!c || !period_us || !slots_per_tick || !base_entries_per_tick) return fail_args(c, "hs_scrub_start", "bad argument");
+  std::lock_guard<std::mutex> gl(c->scrub_life);
+  scrub_state &S = c->scrub;
+  if (S.th.joinable()) return fail_args(c, "hs_scrub_start", "a scrub is already running on this context (hs_scrub_stop it first)");
+  {
+    std::lock_guard<std::mutex> l(S.m);
+    HS_TRY(scrub_map_locked(c, S, "hs_scrub_start", expect_pks, expect_live, n_slots));
+    S.period_us = period_us;
+    S.slots_per_tick = slots_per_tick;
+    S.base_per_tick = base_entries_per_tick;
+    S.cb = cb;
+    S.user = user;
+    S.stop = false;
+    S.rc = HS_OK;
+    for (auto &v : S.stats) v = 0;
+  }
+  try {
+    S.th = std::thread(scrub_loop, c);
+  } catch (const std::system_error &) {
+    return fail(c, HS_ERR_NOMEM, "hs_scrub_start: no thread");
+  }
+  return HS_OK;
+}
+
+extern "C" int hs_scrub_set_map(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> l(c->scrub.m);
+  return scrub_map_locked(c, c->scrub, "hs_scrub_set_map", expect_pks, expect_live, n_slots);
+}
+
+extern "C" int hs_scrub_stop(hs_ctx *c) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> gl(c->scrub_life);
+  scrub_state &S = c->scrub;
+  if (!S.th.joinable()) return HS_OK;
+  if (S.th.get_id() == std::this_thread::get_id()) return fail_args(c, "hs_scrub_stop", "called from the scrub's callback");
+  {
+    std::lock_guard<std::mutex> l(S.m);
+    S.stop = true;
+  }
+  S.cv.notify_all();
+  S.th.join();
+  const int rc = S.rc;
+  S.rc = HS_OK;
+  return rc;
+}
+
+extern "C" int hs_scrub_stats(hs_ctx *c, uint64_t out[HS_SCRUB_STATS]) {
+  if (!c || !out) return HS_ERR_ARG;
+  for (int k = 0; k < SCRUB_NSTATS; k++) out[k] = c->scrub.stats[k].load();
   return HS_OK;
 }
 

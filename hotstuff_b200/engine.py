@@ -161,6 +161,48 @@ class Engine:
             self._check(rc, "hs_table_repair")
         return int(found.value), int(failed.value), bits[:n]
 
+    SCRUB_STATS = ("passes", "slots_audited", "base_entries_audited", "ticks", "findings", "slots_repaired", "failed_repairs",
+                   "ticks_paused")
+
+    def _scrub_map(self, expect, live, what):
+        n = self.key_slots if expect is None else _u8(expect, 32).reshape(-1, 32).shape[0]
+        exp = None if expect is None else _u8(expect, 32).reshape(-1, 32)
+        lv = None if live is None else np.ascontiguousarray(live, dtype=np.uint32)
+        if lv is not None and lv.size < (n + 31) // 32:
+            raise ValueError("%s: %d live words for %d slots" % (what, lv.size, n))
+        return n, exp, lv, (_ptr(exp) if n and exp is not None else None), (_ptr(lv) if lv is not None and lv.size else None)
+
+    def scrub_start(self, expect=None, live=None, period_us=15625, slots_per_tick=128, base_entries_per_tick=2883585, callback=None):
+        """Starts the engine-owned scrub of the live key tables (hs_scrub_start): every period_us a thread audits the next slots_per_tick
+        key slots in service and base_entries_per_tick entries of the base-point table against expect / live (as for table_audit; None:
+        the engine's host mirror), repairs what it finds and calls callback(found, failed, first_slot) once per tick that found anything,
+        on the scrub's thread.  After a committee change it pauses until scrub_set_map.  The defaults make a pass of a 4,096-key
+        committee and the 24-bit base-point table 32 ticks, about half a second (DESIGN.md §5j).  Raises EngineError when a scrub
+        already runs or the map breaks the audit's rules."""
+        n, exp, lv, p_exp, p_lv = self._scrub_map(expect, live, "scrub_start")
+        cb = None
+        if callback is not None:
+            cb = _lib.SCRUB_CB(lambda user, found, failed, first_slot: callback(int(found), int(failed), int(first_slot)))
+        rc = self.lib.hs_scrub_start(self.h, p_exp, p_lv, n, int(period_us), int(slots_per_tick), int(base_entries_per_tick),
+                                     ctypes.cast(cb, ctypes.c_void_p) if cb is not None else None, None)
+        self._check(rc, "hs_scrub_start")
+        self._scrub_keep = (cb, exp, lv)  # the trampoline lives as long as the thread that calls it
+
+    def scrub_set_map(self, expect=None, live=None):
+        """The map of the slots after a committee change (hs_scrub_set_map): the paused scrub resumes with a new pass."""
+        n, exp, lv, p_exp, p_lv = self._scrub_map(expect, live, "scrub_set_map")
+        self._check(self.lib.hs_scrub_set_map(self.h, p_exp, p_lv, n), "hs_scrub_set_map")
+
+    def scrub_stop(self):
+        """Stops the scrub and joins its thread (hs_scrub_stop); a no-op when none runs."""
+        self._check(self.lib.hs_scrub_stop(self.h), "hs_scrub_stop")
+
+    def scrub_stats(self):
+        """The scrub's counters (hs_scrub_stats) as a dict keyed by SCRUB_STATS."""
+        out = (ctypes.c_uint64 * len(self.SCRUB_STATS))()
+        self._check(self.lib.hs_scrub_stats(self.h, out), "hs_scrub_stats")
+        return dict(zip(self.SCRUB_STATS, (int(v) for v in out)))
+
     def explain(self, recs):
         """Table-free re-check of (n,128) uint8 records (hs_explain_rec128) -> uint8[n] of WHY_* bits, one per failed check.  The strict
         verdict is 1 iff the byte is 0; the batch-eq verdict is 1 iff it has no bit outside WHY_A_SMALL | WHY_R_SMALL."""

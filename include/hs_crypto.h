@@ -502,6 +502,45 @@ int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 3
 int hs_table_repair(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
                     size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_found, uint32_t *out_failed);
 
+/* ---- scrub of the live key tables: the audit and repair above, a bounded slice at a time, on an engine-owned thread -------------
+ * hs_scrub_start starts one thread per context that wakes every period_us microseconds.  Each tick takes the audit's turn (it is
+ * serialised with hs_table_audit, hs_table_repair, hs_committee_stage and hs_committee_commit) and audits one slice:
+ *   - the next slots_per_tick key slots in service, in slot order and wrapping at the end (the slots out of service between them have
+ *     no table and come free): their comb tables, with hs_table_audit's checks;
+ *   - the next base_entries_per_tick entries of the base-point table (entry e is entry e % (2^(w-1) + 1) of window e / (2^(w-1) + 1));
+ *   - the KEY, FLAG and LOOKUP checks of every slot and every hash entry: a thread each, so every tick runs them all.
+ *   A pass is complete when every slot in service and every base entry has been audited since it began; a pass takes
+ *   max(ceil(slots in service / slots_per_tick), ceil(base entries / base_entries_per_tick)) ticks, and the next one starts from slot 0
+ *   and entry 0.  The kernels run on the audit's private lowest-priority stream; the context's mutex is held only to snapshot and enqueue,
+ *   as in hs_table_audit.
+ *   - Authority: the map given (expect_pks / expect_live, nullable, n_slots == hs_key_slots) or, with NULL, the engine's host mirror,
+ *     with hs_table_audit's rules.  A registration, hs_committee_update, hs_committee_commit or a key-cache change makes it stale: from
+ *     then on every tick pauses (and counts the pause) until hs_scrub_set_map gives the map of the new slots.  No tick audits against a
+ *     stale map, and a committee change is never reported as a finding.  A pending stage is not a change.  A new map starts a new pass.
+ *   - Repair: a tick that finds anything also audits the tables of the slots its slot checks flagged, repairs exactly what it found from
+ *     the same authority as hs_table_repair does (failing slots rebuilt and proved off the verify path, the hash table rebuilt, the
+ *     base-point table rebuilt with the device drained; every verify queue's signature and certificate caches emptied), then audits its
+ *     slice and those slots again.  A slot whose repair fails stays out of service.  Then cb (nullable) runs once, on the scrub's thread:
+ *     found = the HS_AUDIT_* classes found, failed = those the second audit still finds (0: all repaired), first_slot = the lowest slot
+ *     with a finding ((size_t)-1: only the base-point table or a stray hash entry).  cb may call hs_scrub_set_map and any entry point
+ *     but hs_scrub_stop and hs_ctx_destroy.
+ *   - HS_ERR_ARG: a scrub already runs on ctx, period_us, slots_per_tick or base_entries_per_tick is 0, or the map breaks the audit's
+ *     rules.  A CUDA error in a tick ends the thread; hs_scrub_stop returns it.
+ *   - hs_scrub_stop joins the thread (waiting for a tick in progress); a no-op returning HS_OK when none runs.  hs_ctx_destroy calls it.
+ *   - hs_scrub_stats: the counters of the current or last scrub, readable at any time.
+ *   Without hs_scrub_start nothing of this runs.  A multi-device context is scrubbed member by member (hs_multi_member). */
+typedef void(hs_scrub_cb)(void *user, uint32_t found, uint32_t failed, size_t first_slot); /* HS_AUDIT_* bits */
+int hs_scrub_start(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
+                   size_t n_slots, uint32_t period_us, uint32_t slots_per_tick, uint32_t base_entries_per_tick, hs_scrub_cb *cb_or_null,
+                   void *user);
+int hs_scrub_set_map(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
+                     size_t n_slots);
+int hs_scrub_stop(hs_ctx *ctx);
+/* passes completed, slots audited, base entries audited, ticks, findings (slots, the base-point table and stray hash entries with a
+ * finding), slots repaired, failed repairs (findings the second audit still finds), ticks paused on a stale map */
+#define HS_SCRUB_STATS 8
+int hs_scrub_stats(hs_ctx *ctx, uint64_t out[HS_SCRUB_STATS]);
+
 /* ---- explanation of a verdict: a table-free re-check that names every check a record fails ------------------------------------
  * A verify call answers 0 for malformed bytes, a small-order key or R, a signature over another message and a false reject by the
  * engine alike.  This call re-checks records by a separate method and reports each check of the decision procedure as its own bit

@@ -88,6 +88,33 @@ class Engine {
     if (slot_bits) *slot_bits = std::move(bits);
     return failed;
   }
+  // The engine-owned scrub (hs_scrub_start): every period_us a thread audits the next slots_per_tick slots in service and
+  // base_entries_per_tick base-point entries against `expect` / `live` (as for table_audit; the engine copies them), repairs what it
+  // finds and calls cb (nullable) once per tick that found anything, on its thread.  After a committee change it pauses until
+  // scrub_set_map.  Throws EngineError when a scrub already runs or the map breaks the audit's rules.
+  void scrub_start(const std::vector<std::array<uint8_t, 32>> *expect, const std::vector<uint32_t> *live, uint32_t period_us,
+                   uint32_t slots_per_tick, uint32_t base_entries_per_tick, hs_scrub_cb *cb = nullptr, void *user = nullptr) const {
+    const size_t n = expect ? expect->size() : key_slots();
+    if (live && live->size() < (n + 31) / 32) throw EngineError("scrub_start: live bitmap shorter than the slots");
+    check(hs_scrub_start(ctx_, expect && n ? expect->front().data() : nullptr, live && !live->empty() ? live->data() : nullptr, n, period_us,
+                         slots_per_tick, base_entries_per_tick, cb, user),
+          "hs_scrub_start");
+  }
+  // The map of the slots after a committee change (hs_scrub_set_map): the paused scrub resumes with a new pass.
+  void scrub_set_map(const std::vector<std::array<uint8_t, 32>> *expect = nullptr, const std::vector<uint32_t> *live = nullptr) const {
+    const size_t n = expect ? expect->size() : key_slots();
+    if (live && live->size() < (n + 31) / 32) throw EngineError("scrub_set_map: live bitmap shorter than the slots");
+    check(hs_scrub_set_map(ctx_, expect && n ? expect->front().data() : nullptr, live && !live->empty() ? live->data() : nullptr, n),
+          "hs_scrub_set_map");
+  }
+  // Stops the scrub and joins its thread (hs_scrub_stop); a no-op when none runs.  Not from the scrub's callback.
+  void scrub_stop() const { check(hs_scrub_stop(ctx_), "hs_scrub_stop"); }
+  // passes, slots audited, base entries audited, ticks, findings, slots repaired, failed repairs, ticks paused (hs_scrub_stats).
+  std::array<uint64_t, HS_SCRUB_STATS> scrub_stats() const {
+    std::array<uint64_t, HS_SCRUB_STATS> s{};
+    check(hs_scrub_stats(ctx_, s.data()), "hs_scrub_stats");
+    return s;
+  }
   // Table-free re-check of n records (hs_explain_rec128): one byte of HS_WHY_* bits per record, one bit per failed check.  Strict
   // verdict 1 <=> 0; batch-eq verdict 1 <=> no bit outside HS_WHY_A_SMALL | HS_WHY_R_SMALL.  Throws EngineError on a CUDA error.
   std::vector<uint8_t> explain(const hs_rec128 *recs, size_t n) const {

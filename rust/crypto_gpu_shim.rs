@@ -54,6 +54,10 @@ pub mod groups_dev;
 /// (`multi::Multi`).
 #[path = "crypto_gpu_multi.rs"]
 pub mod multi;
+/// The engine-owned scrub of the live key tables (hs_scrub_*): a bounded slice audited and repaired per tick against the node's map,
+/// started once after `self_test` (`scrub::start`) and given the new map after every committee change.
+#[path = "crypto_gpu_scrub.rs"]
+pub mod scrub;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)
@@ -152,7 +156,9 @@ pub fn register_committee(keys: &[[u8; 32]]) -> Result<(), GpuError> {
     let mut valid = vec![0u32; (keys.len() + 31) / 32];
     let rc = unsafe { hs_committee_register(c, keys.as_ptr() as *const u8, keys.len(), valid.as_mut_ptr()) };
     if rc != HS_OK { KEYS.lock().unwrap().clear(); return Err(GpuError::Engine(last_error(c))); }
-    *KEYS.lock().unwrap() = keys.iter().map(|k| Some(*k)).collect();
+    let mut map = KEYS.lock().unwrap();
+    *map = keys.iter().map(|k| Some(*k)).collect();
+    scrub::set_map(c, &map)?;
     *STAGED.lock().unwrap() = None;  // a registration discards a staged change
     let bad: Vec<usize> = (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect();
     if bad.is_empty() { Ok(()) } else { Err(GpuError::InvalidKeys(bad)) }
@@ -169,8 +175,8 @@ pub fn self_test() -> Result<(), GpuError> {
     Err(GpuError::Engine(format!("self-test failed (status {}, paths {:#x}): {}", rc, failed, last_error(c))))
 }
 /// Audit of the live key tables (hs_table_audit): every comb-table entry, key slot and lookup entry of the engine against `expected`,
-/// the node's index -> key map (None = a freed index).  `self_test` and `update_committee` call it; a live node may also call it
-/// periodically from a blocking task.  A finding is repaired once from the same map (hs_table_repair: only the failing slots, lookup
+/// the node's index -> key map (None = a freed index).  `self_test` and `update_committee` call it; between those, `scrub::start`
+/// keeps auditing on the engine's own thread.  A finding is repaired once from the same map (hs_table_repair: only the failing slots, lookup
 /// entries or base-point table are rebuilt, and the caches of verified records are emptied); the GPU stays on when the repair's own
 /// final audit is clean, and is switched off for the life of the process, as after a failed self-test, only when the repair fails.
 /// Tables that changed while it ran (a committee change from another task) are audited again.
@@ -229,6 +235,7 @@ pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>
         keys[i as usize] = Some(*k);
     }
     audit_tables(&keys)?;
+    scrub::set_map(c, &keys)?;
     Ok(out)
 }
 /// hs_committee_stage / hs_committee_commit / hs_committee_discard on one context: the shim's own and, one per member, `multi::Multi`'s.
@@ -272,7 +279,8 @@ pub fn commit_committee() -> Result<(), GpuError> {
         keys[i as usize] = Some(*k);
     }
     for &i in &st.remove { keys[i as usize] = None; }
-    audit_tables(&keys)
+    audit_tables(&keys)?;
+    scrub::set_map(c, &keys)
 }
 /// Drops a staged committee change (hs_committee_discard).
 pub fn discard_committee() -> Result<(), GpuError> {

@@ -71,6 +71,8 @@ SIGNATURES = {
     "hs_queue_cert_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_sig_cache": (c_int, [c_void_p, c_size_t]),
     "hs_queue_sig_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_queue_sig_share": (c_int, [c_void_p, c_int]),
+    "hs_queue_sig_share_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_generic": (c_int, [c_void_p, c_int]),
     "hs_queue_generic_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_batch": (c_int, [c_void_p, c_size_t, c_size_t]),

@@ -924,9 +924,14 @@ __device__ __forceinline__ void fe_load_global(fe &r, const fe *p) {
 __host__ __device__ inline uint32_t mode_flag(uint32_t mode) { return mode == HS_MODE_BATCH_EQ ? HS_F_EQ : HS_F_STRICT; }
 // verdict(i, fl) turns record i's flags into its bit: one mode for the pass (k_verify_finish) or record i's own mode byte
 // (k_verify_finish_modes).
-template <class Verdict>
+// CACHED (a pass that shares a queue's signature cache, hs_queue_sig_share): a record k_sig_probe decided carries HS_META_CACHED and
+// its stored flags in meta and Z = 1 in xyz, so it takes its flags from meta; every record's flag byte goes to fl_out for k_sig_fill.
+// The CACHED = false instantiations are the kernels without it, instruction for instruction.
+#define HS_META_CACHED 0x40u  // meta: decided from the signature cache; the low bits are the stored flags
+template <bool CACHED, class Verdict>
 __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
-                                                   Verdict verdict, uint32_t *__restrict__ bitmap, const peer_route &P, const int group) {
+                                                   Verdict verdict, uint32_t *__restrict__ bitmap, const peer_route &P, const int group,
+                                                   uint8_t *__restrict__ fl_out = nullptr) {
   __shared__ fe tot[HS_THREADS];
   const size_t t = (size_t)blockIdx.x * HS_THREADS + threadIdx.x;
   const size_t first = t * (size_t)group;
@@ -965,7 +970,13 @@ __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n,
       load32(R, L.sig + i * L.sig_stride);
       uint32_t m = meta[i];
       if (zero_z) m &= ~HS_META_PARSE_OK;
-      const uint32_t fl = verify_flags_from(X, Y, zinv, R, m);
+      uint32_t fl;
+      if constexpr (CACHED) {
+        fl = (m & HS_META_CACHED) ? (m & 0x1fu) : verify_flags_from(X, Y, zinv, R, m);
+        fl_out[i] = (uint8_t)fl;
+      } else {
+        fl = verify_flags_from(X, Y, zinv, R, m);
+      }
       const uint32_t ok = verdict(i, fl);
       if (ok) bits |= 1u << c;
     }
@@ -1000,14 +1011,105 @@ __device__ __forceinline__ void verify_finish_body(const in_layout &L, size_t n,
 }
 __global__ void __launch_bounds__(HS_THREADS) k_verify_finish(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
                                                                uint32_t mode, uint32_t *__restrict__ bitmap, const peer_route P, const int group) {
-  verify_finish_body(L, n, xyz, meta, [&](size_t, uint32_t fl) { return fl & mode_flag(mode); }, bitmap, P, group);
+  verify_finish_body<false>(L, n, xyz, meta, [&](size_t, uint32_t fl) { return fl & mode_flag(mode); }, bitmap, P, group);
 }
 // Per-record verdict modes (hs_verify_groups_dev, hs_verify_groups, the queue's batch lane): every word written locally or stored into
 // the peers' buffers is a final item verdict.
 __global__ void __launch_bounds__(HS_THREADS) k_verify_finish_modes(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
                                                                      const uint8_t *__restrict__ item_mode, uint32_t *__restrict__ bitmap, const peer_route P,
                                                                      const int group) {
-  verify_finish_body(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & mode_flag(item_mode[i]); }, bitmap, P, group);
+  verify_finish_body<false>(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & mode_flag(item_mode[i]); }, bitmap, P, group);
+}
+// The same two kernels for a pass that shares a signature cache (CACHED above).
+__global__ void __launch_bounds__(HS_THREADS) k_verify_finish_cached(in_layout L, size_t n, const fe *__restrict__ xyz, const uint8_t *__restrict__ meta,
+                                                                      uint32_t mode, uint32_t *__restrict__ bitmap, const peer_route P, const int group,
+                                                                      uint8_t *__restrict__ fl_out) {
+  verify_finish_body<true>(L, n, xyz, meta, [&](size_t, uint32_t fl) { return fl & mode_flag(mode); }, bitmap, P, group, fl_out);
+}
+__global__ void __launch_bounds__(HS_THREADS) k_verify_finish_modes_cached(in_layout L, size_t n, const fe *__restrict__ xyz,
+                                                                            const uint8_t *__restrict__ meta, const uint8_t *__restrict__ item_mode,
+                                                                            uint32_t *__restrict__ bitmap, const peer_route P, const int group,
+                                                                            uint8_t *__restrict__ fl_out) {
+  verify_finish_body<true>(L, n, xyz, meta, [&](size_t i, uint32_t fl) { return fl & mode_flag(item_mode[i]); }, bitmap, P, group, fl_out);
+}
+
+// ------------------------------------------------------------------------------------------------ shared signature cache (hs_queue_sig_share)
+// A synchronous verify pass or a batch-lane pass that shares a queue's signature cache runs k_sig_probe after the key lookup,
+// k_verify_main<committee> over the records it left, the cached finish kernel, then k_sig_fill.  Counts go to sc.ctr: [0] records
+// probed, [1] hits (k_sig_probe), [2] inserts, [3] inserts that evicted a live entry (k_sig_fill).  Only records with a registered key
+// and a 32-byte message (every pass that shares has one) take part; the words of record i are sig | registered key bytes | Digest.
+struct sig_rec_words {
+  uint32_t R[8], S[8], A[8], M[8];
+  __device__ __forceinline__ uint32_t operator()(int j) const { return j < 8 ? R[j] : j < 16 ? S[j - 8] : j < 24 ? A[j - 16] : M[j - 24]; }
+};
+__device__ __forceinline__ void sig_load_words(sig_rec_words &w, const in_layout &L, const committee_tables &C, size_t i, uint32_t v) {
+  load32(w.R, L.sig + i * L.sig_stride);
+  load32(w.S, L.sig + i * L.sig_stride + 32);
+  load32(w.A, C.pks + (size_t)v * 32);
+  load32(w.M, L.msg + (size_t)(L.midx ? __ldg(L.midx + i) : i) * L.msg_stride);
+}
+// The block's counts into two of sc.ctr's words: per warp with one reduction each, then one atomic per warp.
+__device__ __forceinline__ void sig_count_pair(const sig_cache_dev &sc, int k, uint32_t a, uint32_t b) {
+  const uint32_t sa = __reduce_add_sync(0xffffffffu, a), sb = __reduce_add_sync(0xffffffffu, b);
+  if ((threadIdx.x & 31) == 0) {
+    if (sa) atomicAdd(sc.ctr + k, sa);
+    if (sb) atomicAdd(sc.ctr + k + 1, sb);
+  }
+}
+// One thread per record.  A hit writes the stored flags | HS_META_CACHED to meta and (0 : 1 : 1) to xyz, so the finish kernel's inversion
+// stays well-defined; every other record the committee pass owns is appended to list (count in *list_n), warp by warp in record order.
+// With side_pass, records whose key missed the lookup belong to the generic pass and are left alone.  Only a slot in service (flag bit 0,
+// which k_verify_main<true> requires for acceptance) is probed: hs_committee_update's removal and hs_table_repair's rebuild clear only a
+// slot's flags, so its old key bytes stay in C.pks and would still match a record cached before; such a record goes to the list instead
+// and is rejected there, as without the cache.
+__global__ void __launch_bounds__(256) k_sig_probe(in_layout L, size_t n, committee_tables C, sig_cache_dev sc, int side_pass, fe *__restrict__ xyz,
+                                                   uint8_t *__restrict__ meta, uint32_t *__restrict__ list, uint32_t *__restrict__ list_n) {
+  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+  const bool active = i < n;
+  const uint32_t v = active ? __ldg(L.vidx + i) : HS_NO_KEY;
+  const bool have_key = v < C.n_keys;
+  const bool in_service = have_key && (__ldg(C.key_flags + v) & 1u);
+  uint32_t hit = 0;
+  if (in_service) {
+    sig_rec_words w;
+    sig_load_words(w, L, C, i, v);
+    uint32_t bucket;
+    hit = sig_probe_thread(sc, w, bucket);
+  }
+  if (hit) {
+    meta[i] = (uint8_t)((hit & 0x1fu) | HS_META_CACHED);
+    uint4 *dst = reinterpret_cast<uint4 *>(xyz + i * 3);
+    dst[0] = dst[1] = dst[3] = dst[5] = make_uint4(0, 0, 0, 0);
+    dst[2] = dst[4] = make_uint4(1, 0, 0, 0);
+  }
+  const bool append = active && !hit && (have_key || !side_pass);
+  const uint32_t mask = __ballot_sync(0xffffffffu, append);
+  const int lane = threadIdx.x & 31;
+  uint32_t base = 0;
+  if (mask && lane == 0) base = atomicAdd(list_n, (uint32_t)__popc(mask));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (append) list[base + __popc(mask & ((1u << lane) - 1u))] = (uint32_t)i;
+  sig_count_pair(sc, 0, in_service ? 1u : 0u, hit ? 1u : 0u);
+}
+// One thread per record: a record the pass verified (not decided from the cache) with a registered key, judged strict (by its mode
+// byte, else the pass's mode) and with HS_F_EQ in its flags fl[i] is inserted with its whole flag byte.
+__global__ void __launch_bounds__(256) k_sig_fill(in_layout L, size_t n, committee_tables C, sig_cache_dev sc, const uint8_t *__restrict__ meta,
+                                                  const uint8_t *__restrict__ fl, uint32_t mode, const uint8_t *__restrict__ item_mode) {
+  const size_t i = (size_t)blockIdx.x * 256 + threadIdx.x;
+  uint32_t ins = 0;
+  if (i < n) {
+    const uint32_t v = __ldg(L.vidx + i), f = fl[i];
+    const bool strict = mode_flag(item_mode ? item_mode[i] : mode) == HS_F_STRICT;
+    if (v < C.n_keys && !(meta[i] & HS_META_CACHED) && strict && (f & HS_F_EQ)) {
+      sig_rec_words w;
+      sig_load_words(w, L, C, i, v);
+      uint64_t h = 0;
+#pragma unroll
+      for (int j = 0; j < 32; j++) h += sig_mix(w(j), __ldg(sc.key + j));
+      ins = sig_insert(sc, sig_bucket_of(sc, h), w, f);
+    }
+  }
+  sig_count_pair(sc, 2, ins != 0, ins == 2);
 }
 
 // ------------------------------------------------------------------------------------------------ table construction
@@ -1742,6 +1844,14 @@ struct hs_ctx {
   std::string err = "ok";
   std::mutex queues_mu;               // guards queues only (hs_ctx_destroy tears them down without holding `mu`)
   std::vector<hs_queue *> queues;     // verify queues attached to this context
+  // hs_queue_sig_share (under mu): the queue whose signature cache the host-pointer verify calls share; the table of the call in
+  // progress (b == nullptr: it does not share) and its shared passes; their scratch, device counters and mapped copy of the counts
+  hs_queue *share_q = nullptr;
+  sig_cache_dev share_sc{};
+  uint32_t share_passes = 0;
+  dev_buf share_list, share_fl;
+  dev_mem<uint32_t> share_ctr;  // HS_SIG_CTRS counts, then the miss list's count
+  mapped<uint32_t> share_h;     // HS_SIG_CTRS
 };
 // The context holds per-key tables: a registered committee's or learned keys'.  Registration, hs_committee_update and learn_process
 // raise n_keys only once `keys` is in place, and cache_release clears both, so n_keys > 0 alone implies the second term.
@@ -2008,6 +2118,14 @@ static pass_tables store_tables(const key_store &S, const key_index &index, size
   return pass_tables{{S.pks, S.key_flags, (uint32_t)n_keys, S.atables, entries}, {S.slots, index.mask, S.pks, (uint32_t)n_keys}, cp};
 }
 static pass_tables ctx_tables(const hs_ctx *c) { return store_tables(c->keys, c->h_index, c->n_keys, c->a_table_entries, c->cp); }
+// A pass that shares a queue's signature cache (hs_queue_sig_share): the table, the pass's device counters (sc.ctr, HS_SIG_CTRS words,
+// then the miss list's count), the miss list, every record's flag byte, and the mapped words its counts are copied to at the end.
+struct share_pass {
+  sig_cache_dev sc;
+  uint32_t *list;
+  uint8_t *fl;
+  uint32_t *h_ctr;
+};
 // A pass on `stream` reads the key cache's tables only after their latest build, which learn_process may have enqueued on another stream.
 static int wait_key_cache_build(hs_ctx *c, cudaStream_t stream) {
   if (c->learn.ev_tables && !c->explicit_committee) HS_CUDA(c, cudaStreamWaitEvent(stream, c->learn.ev_tables, 0));
@@ -2015,10 +2133,11 @@ static int wait_key_cache_build(hs_ctx *c, cudaStream_t stream) {
 }
 // The main phase on `stream`: with committee tables, [k_key_lookup, then k_verify_main<false> over the misses on S.side] beside
 // k_verify_main<true>; without, k_verify_main<false> over every record.  after_lookup(have_lookup) runs where run_verify collects
-// keys for the key cache.  L.vidx is set to the lookup's indices when it runs.
+// keys for the key cache.  L.vidx is set to the lookup's indices when it runs.  sh (nullable, committee passes only): k_sig_probe
+// decides the records the cache holds and k_verify_main<true> runs over the list of the others.
 template <class AfterLookup>
 static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool indexed, const pass_tables &K, const pass_scratch &S,
-                       cudaStream_t stream, AfterLookup after_lookup) {
+                       cudaStream_t stream, AfterLookup after_lookup, const share_pass *sh = nullptr) {
   main_out O{S.xyz, S.meta, 0};
   const committee_tables &C = K.C;
   if (committee) {
@@ -2042,8 +2161,18 @@ static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool i
       HS_CUDA(c, cudaGetLastError());
       HS_CUDA(c, cudaEventRecord(S.ev_side[1], S.side));
     }
+    const uint32_t *n_ptr = nullptr, *list = nullptr;
+    if (sh) {
+      uint32_t *list_n = sh->sc.ctr + HS_SIG_CTRS;
+      HS_CUDA(c, cudaMemsetAsync(sh->sc.ctr, 0, 4 * (HS_SIG_CTRS + 1), stream));
+      k_sig_probe<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, C, sh->sc, indexed ? 0 : 1, S.xyz, S.meta, sh->list, list_n);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+      n_ptr = list_n;
+      list = sh->list;
+    }
     if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[0], stream));
-    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, nullptr, nullptr, c->d_btable, C, O, K.cp);
+    k_verify_main<true><<<blocks_for(n), HS_THREADS, 0, stream>>>(L, n, n_ptr, list, c->d_btable, C, O, K.cp);
     if (S.prof) HS_CUDA(c, cudaEventRecord(S.prof[1], stream));
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
@@ -2057,16 +2186,30 @@ static int launch_main(hs_ctx *c, in_layout &L, size_t n, bool committee, bool i
   return HS_OK;
 }
 // Threads of k_verify_finish own `fin_group` records each; launched on `stream`.  d_item_mode (device, nullable): record i is judged
-// by its own mode byte (k_verify_finish_modes) instead of `mode`.
+// by its own mode byte (k_verify_finish_modes) instead of `mode`.  sh (nullable): the pass shares a signature cache, so the cached
+// kernels run and write every record's flag byte to sh->fl.
 static int launch_finish(hs_ctx *c, const in_layout &L, size_t n, const fe *xyz, const uint8_t *meta, uint32_t mode, const uint8_t *d_item_mode,
-                         uint32_t *d_bitmap, const peer_route &P, int fin_group, cudaStream_t stream) {
+                         uint32_t *d_bitmap, const peer_route &P, int fin_group, cudaStream_t stream, const share_pass *sh = nullptr) {
   const size_t fin_threads = (n + fin_group - 1) / fin_group;
-  if (d_item_mode)
+  if (sh && d_item_mode)
+    k_verify_finish_modes_cached<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, d_item_mode, d_bitmap, P, fin_group, sh->fl);
+  else if (sh)
+    k_verify_finish_cached<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, P, fin_group, sh->fl);
+  else if (d_item_mode)
     k_verify_finish_modes<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, d_item_mode, d_bitmap, P, fin_group);
   else
     k_verify_finish<<<blocks_for(fin_threads), HS_THREADS, 0, stream>>>(L, n, xyz, meta, mode, d_bitmap, P, fin_group);
   c->launches++;
   HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+// The end of a shared pass, after its finish kernel on `stream`: k_sig_fill, then the pass's counts to sh.h_ctr.
+static int launch_sig_fill(hs_ctx *c, const in_layout &L, size_t n, const committee_tables &C, const share_pass &sh, const uint8_t *meta,
+                           uint32_t mode, const uint8_t *d_item_mode, cudaStream_t stream) {
+  k_sig_fill<<<blocks_for(n, 256), 256, 0, stream>>>(L, n, C, sh.sc, meta, sh.fl, mode, d_item_mode);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  HS_CUDA(c, cudaMemcpyAsync(sh.h_ctr, sh.sc.ctr, 4 * HS_SIG_CTRS, cudaMemcpyDeviceToHost, stream));
   return HS_OK;
 }
 
@@ -2104,8 +2247,16 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
   }
   const pass_scratch S{(fe *)XYZ.p.get(), (uint8_t *)META.p.get(), (uint32_t *)c->vidx.p.get(), (uint32_t *)c->miss.p.get(), c->d_miss_count, c->stream_side,
                        {c->ev_side[0], c->ev_side[1]}, c->profile_main ? c->ev_prof : nullptr};
+  // a host-pointer call that shares a signature cache (share_call), over 32-byte messages (so on the context's stream, never deferred)
+  const bool share = c->share_sc.b && committee && stream == c->stream && !L.off && L.fixed_len == 32;
+  share_pass SP{};
+  if (share) {
+    HS_TRY(ensure(c, c->share_list, n * 4));
+    HS_TRY(ensure(c, c->share_fl, n));
+    SP = share_pass{c->share_sc, (uint32_t *)c->share_list.p.get(), (uint8_t *)c->share_fl.p.get(), c->share_h.h};
+  }
   HS_TRY(launch_main(c, L, n, committee, indexed, ctx_tables(c), S, stream,
-                     [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }));
+                     [&](bool have_lookup) { return learn_collect(c, L, n, have_lookup, stream); }, share ? &SP : nullptr));
   // small batches: small groups, so that enough blocks exist to hide each block's serial inversion; when the tail overlaps the next pass
   // (deferred mode) latency is hidden anyway and the 16-record group costs the fewest inversions
   const int fin_group = (defer || n >= (1u << 19)) ? 16 : (n >= (1u << 18) ? 8 : 4);
@@ -2120,7 +2271,12 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     HS_CUDA(c, cudaStreamWaitEvent(c->stream_tail, c->ev_main_done, 0));
     fin_stream = c->stream_tail;
   }
-  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_item_mode, d_bitmap, P, fin_group, fin_stream));
+  HS_TRY(launch_finish(c, L, n, (const fe *)XYZ.p.get(), (const uint8_t *)META.p.get(), mode, d_item_mode, d_bitmap, P, fin_group, fin_stream,
+                       share ? &SP : nullptr));
+  if (share) {
+    HS_TRY(launch_sig_fill(c, L, n, ctx_tables(c).C, SP, (const uint8_t *)META.p.get(), mode, d_item_mode, stream));
+    c->share_passes++;
+  }
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
   return HS_OK;
 }
@@ -2349,12 +2505,12 @@ struct lane_kind {
   size_t per_launch;                         // requests one launch takes at most
   const char *launch_err, *incomplete;       // texts of a failed stream and of a completion word missing on drained streams
   int (*enqueue)(hs_queue *q, side_lane &L);  // enqueues the launch of L.launch on the lane's streams (under c->mu)
-  void (*count)(side_lane &L);               // counts a launch whose every request completed HS_OK
+  void (*count)(hs_queue *q, side_lane &L);  // counts a launch whose every request completed HS_OK (under q->mu)
 };
 static int batch_enqueue(hs_queue *q, side_lane &L);
-static void batch_count(side_lane &L);
+static void batch_count(hs_queue *q, side_lane &L);
 static int explain_enqueue(hs_queue *q, side_lane &L);
-static void explain_count(side_lane &L);
+static void explain_count(hs_queue *q, side_lane &L);
 static const lane_kind batch_kind{"batch", "hs_queue_batch", 1, "verify queue batch pass", "verify queue: k_batch_done did not complete",
                                   batch_enqueue, batch_count};
 static const lane_kind explain_kind{"explain", "hs_queue_explain", SIZE_MAX, "verify queue explain launch",
@@ -2367,6 +2523,7 @@ struct lane_req {
   uint64_t o_res, o_tail, size;   // its result words, its tail and its size, from the lane's region layout
   uint64_t a_off = 0, a_pos = 0, a_end = 0;  // region offset in the arena; arena positions of its start and past its end
   uint32_t seq = 0;               // the completion word (set at launch)
+  uint32_t share_gen = 0;         // batch lane: the signature-cache table its pass shared (0: none; set at launch)
   bool ready = false, done = false;
 };
 // A side lane's arena, its device mirror and its streams (lane_configure builds them whole, or not at all).
@@ -2397,6 +2554,11 @@ struct batch_scratch {
   dev_mem<uint8_t> meta;
   dev_mem<uint32_t> vidx, miss, miss_count, items, grej, counter;
   event_h ev[2];
+  // a pass that shares the queue's signature cache (hs_queue_sig_share): its miss list, flag bytes, device counters (HS_SIG_CTRS, then
+  // the list's count) and the mapped copy of the counts
+  dev_mem<uint32_t> share_list, share_ctr;
+  dev_mem<uint8_t> share_fl;
+  mapped<uint32_t> share_h;
 };
 // The explain lane's own scratch: the launch's request list.
 struct explain_scratch {
@@ -2479,9 +2641,41 @@ struct hs_queue {
   uint32_t sig_bmask = 0, sig_gen = 0;
   sig_counters sigc;
   uint64_t sstats[HS_QUEUE_SIG_STATS] = {};  // hs_queue_sig_stats ([4]: inserts - evictions into the current table)
+  // hs_queue_sig_share: ev_share is recorded after every batch-lane pass that shares the table (under c->mu), so a resize can wait for it
+  event_h ev_share;
+  uint64_t shstats[HS_QUEUE_SIG_SHARE_STATS] = {};  // hs_queue_sig_share_stats
   std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
   std::condition_variable cv_work, cv_done;
   std::thread th;
+};
+
+// ---- hs_queue_sig_share: the host-pointer verify calls and the batch lane share one queue's signature cache
+// The counts of one shared pass (h: its mapped HS_SIG_CTRS words, complete) into q's counters, under q->mu; gen: the table it shared.
+static void sig_share_count(hs_queue *q, const uint32_t *h, uint32_t gen) {
+  const volatile uint32_t *v = h;
+  for (int k = 0; k < HS_SIG_CTRS; k++) q->shstats[k] += v[k];
+  q->shstats[4]++;
+  if (gen == q->sig_gen) q->sstats[4] += v[2] - v[3];
+}
+// Set on every verify queue's dispatcher thread: the synchronous calls it makes for slow-path requests neither probe nor insert.
+static thread_local bool t_queue_dispatcher = false;
+// Held, under c->mu, by each host-pointer call that takes part (hs_verify_rec128, hs_verify_batch_shared_msg, hs_verify_qcs,
+// hs_verify_tcs, hs_verify_groups): while it lives, run_verify's committee pass over 32-byte messages on the context's stream shares the
+// table of c->share_q.  Each of these calls runs at most one such pass; once its results are back its counts go to the queue.
+struct share_call {
+  hs_ctx *c;
+  explicit share_call(hs_ctx *ctx) : c(ctx) {
+    hs_queue *q = c->share_q;
+    c->share_passes = 0;
+    c->share_sc = (q && !t_queue_dispatcher) ? sig_cache_dev{q->d_sig, q->sigc.key, q->sig_bmask, c->share_ctr, nullptr} : sig_cache_dev{};
+  }
+  ~share_call() {
+    if (c->share_passes && cudaStreamSynchronize(c->stream) == cudaSuccess) {
+      std::lock_guard<std::mutex> g(c->share_q->mu);
+      sig_share_count(c->share_q, c->share_h.h, c->share_q->sig_gen);
+    }
+    c->share_sc = sig_cache_dev{};
+  }
 };
 
 struct queue_completion {
@@ -2923,7 +3117,7 @@ static void lane_complete(hs_queue *q, side_lane &L, cudaError_t qe) {
       r->done = true;
     }
     if (!open) {
-      if (ok) L.kind.count(L);
+      if (ok) L.kind.count(q, L);
       L.ring.release_to(L.launch.back()->a_end);
     }
   }
@@ -3044,9 +3238,9 @@ static uint32_t batch_bits(uint64_t n_groups, uint64_t n) { return (uint32_t)(32
 // calls, `_dev` calls and the queue's other launches can be in flight meanwhile.
 static int batch_enqueue(hs_queue *q, side_lane &L) {
   hs_ctx *c = q->c;
-  const lane_req &r = *L.launch.front();
+  lane_req &r = *L.launch.front();
   const batch_layout B = batch_layout_of(r.m, r.pre_bytes, r.n, r.n_groups);
-  const batch_scratch &S = q->batch_scr;
+  batch_scratch &S = q->batch_scr;
   cudaStream_t s = L.buf.stream;
   const uint8_t *m = L.buf.mirror + r.a_off;
   HS_CUDA(c, cudaMemcpyAsync(L.buf.mirror + r.a_off, L.buf.arena.h + r.a_off, B.o_res, cudaMemcpyHostToDevice, s));
@@ -3058,9 +3252,17 @@ static int batch_enqueue(hs_queue *q, side_lane &L) {
   // only an explicitly registered committee: learned key-cache tables may be rebuilt by a synchronous call, and the lane never learns
   const bool committee = committee_registered(c);
   const pass_scratch P{S.xyz, S.meta, S.vidx, S.miss, S.miss_count, L.buf.side, {S.ev[0], S.ev[1]}, nullptr};
-  HS_TRY(launch_main(c, I, r.n, committee, false, ctx_tables(c), P, s, [](bool) { return HS_OK; }));
+  // the queue shares its signature cache (hs_queue_sig_share): the pass probes and fills it
+  const bool share = committee && c->share_q == q && q->d_sig;
+  const share_pass SH{sig_cache_dev{q->d_sig, q->sigc.key, q->sig_bmask, S.share_ctr, nullptr}, S.share_list, S.share_fl, S.share_h.h};
+  r.share_gen = share ? q->sig_gen : 0;
+  HS_TRY(launch_main(c, I, r.n, committee, false, ctx_tables(c), P, s, [](bool) { return HS_OK; }, share ? &SH : nullptr));
   const int fin_group = r.n >= (1u << 19) ? 16 : (r.n >= (1u << 18) ? 8 : 4);
-  HS_TRY(launch_finish(c, I, r.n, S.xyz, S.meta, HS_MODE_STRICT, m + B.o_mo, S.items, peer_route{}, fin_group, s));
+  HS_TRY(launch_finish(c, I, r.n, S.xyz, S.meta, HS_MODE_STRICT, m + B.o_mo, S.items, peer_route{}, fin_group, s, share ? &SH : nullptr));
+  if (share) {
+    HS_TRY(launch_sig_fill(c, I, r.n, ctx_tables(c).C, SH, S.meta, HS_MODE_STRICT, m + B.o_mo, s));
+    HS_CUDA(c, cudaEventRecord(q->ev_share, s));
+  }
   HS_CUDA(c, cudaMemsetAsync(S.grej, 0, 4 * ((r.n_groups + 31) / 32), s));
   uint8_t *res = L.buf.arena.d + r.a_off;
   k_batch_done<<<blocks_for(r.n, 256), 256, 0, s>>>(S.items, reinterpret_cast<const uint32_t *>(m + B.o_gi), r.n, r.n_groups, S.grej,
@@ -3070,8 +3272,9 @@ static int batch_enqueue(hs_queue *q, side_lane &L) {
   HS_CUDA(c, cudaGetLastError());
   return HS_OK;
 }
-static void batch_count(side_lane &L) {
+static void batch_count(hs_queue *q, side_lane &L) {
   for (const lane_req *r : L.launch) {
+    if (r->share_gen) sig_share_count(q, q->batch_scr.share_h.h, r->share_gen);
     L.stats[0]++;
     L.stats[1] += r->n;
     L.stats[2] += r->n_groups;
@@ -3102,7 +3305,7 @@ static int explain_enqueue(hs_queue *q, side_lane &L) {
   if (e == cudaSuccess) e = launch_queue_explain(c, q->explain_scr.list.d, (uint32_t)L.launch.size(), recs, L.buf.mirror, L.buf.arena.d, s);
   return e == cudaSuccess ? HS_OK : fail(c, HS_ERR_CUDA, "verify queue explain launch", e);
 }
-static void explain_count(side_lane &L) {
+static void explain_count(hs_queue *, side_lane &L) {
   L.stats[0]++;
   for (const lane_req *r : L.launch) L.stats[1] += r->n;
   L.stats[2] += L.launch.size();
@@ -3124,6 +3327,7 @@ static bool queue_generic_ready_locked(const hs_queue *q) {
 
 static void queue_main(hs_queue *q) {
   cudaSetDevice(q->c->device);
+  t_queue_dispatcher = true;
   const std::array<side_lane *, 2> lanes = queue_lanes(q);
   std::unique_lock<std::mutex> lk(q->mu);
   for (;;) {
@@ -3603,6 +3807,7 @@ int hs_verify_qcs(hs_ctx *c, const uint8_t *preimages, size_t n_qc, const uint8_
     return HS_OK;
   }
   std::lock_guard<std::mutex> g(c->mu);
+  share_call sh(c);
   HS_CUDA(c, cudaSetDevice(c->device));
   h2d_stage S;
   const size_t s_pre = S.add(preimages, n_qc * 40), s_dig = S.add(nullptr, n_qc * 32), s_sig = S.add(sig, n_votes * 64),
@@ -3683,6 +3888,7 @@ int hs_verify_tcs(hs_ctx *c, const uint64_t *tc_rounds, size_t n_tc, const uint8
     return HS_OK;
   }
   std::lock_guard<std::mutex> g(c->mu);
+  share_call sh(c);
   HS_CUDA(c, cudaSetDevice(c->device));
   h2d_stage S;
   const size_t s_r = S.add(tc_rounds, n_tc * 8), s_hq = S.add(high_qc_rounds, n_votes * 8), s_dig = S.add(nullptr, n_votes * 32),
@@ -3720,6 +3926,7 @@ int hs_verify_groups(hs_ctx *c, const uint8_t *preimages, const uint64_t *pre_of
     return HS_OK;
   }
   std::lock_guard<std::mutex> g(c->mu);
+  share_call sh(c);
   HS_CUDA(c, cudaSetDevice(c->device));
   h2d_stage S;
   const size_t s_off = S.add(pre_off, (n_msgs + 1) * 8), s_pre = S.add(preimages, pre_off[n_msgs], 8), s_sig = S.add(sig, n_items * 64),
@@ -3860,6 +4067,7 @@ int hs_verify_rec128(hs_ctx *c, const hs_rec128 *recs, size_t n, uint32_t mode, 
   if (const char *why = hs_args::rec128(recs, n, mode, out_bitmap)) return fail_args(c, "hs_verify_rec128", why);
   if (n == 0) return HS_OK;
   std::lock_guard<std::mutex> g(c->mu);
+  share_call sh(c);
   HS_CUDA(c, cudaSetDevice(c->device));
   // latency path: every key must already have a table (registered or learned)
   if (small_eligible(c, n) && small_stage(c, n, [&](size_t i) { return small_src{recs[i].sig, recs[i].msg, host_key_lookup(c, recs[i].pk)}; }))
@@ -3899,6 +4107,7 @@ int hs_verify_batch_shared_msg(hs_ctx *c, const uint8_t digest[32], const hs_vot
     return HS_OK;
   }
   std::lock_guard<std::mutex> g(c->mu);
+  share_call sh(c);
   HS_CUDA(c, cudaSetDevice(c->device));
   const size_t words = (n + 31) / 32;
   std::vector<uint32_t> tmp;
@@ -4412,9 +4621,12 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries) {
 static int sig_cache_set_locked(hs_queue *q, uint32_t buckets) {
   hs_ctx *c = q->c;
   HS_CUDA(c, cudaSetDevice(c->device));
-  // Drains the queue's streams: no launch that probes the old table survives these lines.
+  // Drains the queue's streams: no launch that probes the old table survives these lines.  Nor does a batch-lane pass that shares it
+  // (hs_queue_sig_share; enqueued under c->mu), and the synchronous calls that share it hold c->mu until their results are back.
   HS_CUDA(c, cudaStreamSynchronize(q->stream));
   HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));
+  if (q->ev_share) HS_CUDA(c, cudaEventSynchronize(q->ev_share));
+  if (!buckets && c->share_q == q) c->share_q = nullptr;  // turning the cache off ends the sharing; a resize keeps it
   q->d_sig.reset();
   {
     std::lock_guard<std::mutex> gq(q->mu);
@@ -4449,6 +4661,35 @@ static int sig_cache_set_locked(hs_queue *q, uint32_t buckets) {
 
 int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]) {
   return queue_read_stats(q, "hs_queue_sig_stats", out, &hs_queue::sstats);
+}
+
+int hs_queue_sig_share(hs_queue *q, int on) {
+  if (!q) return fail(nullptr, HS_ERR_ARG, "hs_queue_sig_share: bad argument");
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> g(c->mu);  // the synchronous calls and the batch lane read c->share_q only while they hold c->mu
+  if (!on) {
+    if (c->share_q == q) c->share_q = nullptr;
+    return HS_OK;
+  }
+  if (!q->d_sig) return fail(c, HS_ERR_ARG, "hs_queue_sig_share: the queue's signature cache is off");
+  if (c->share_q && c->share_q != q) return fail(c, HS_ERR_ARG, "hs_queue_sig_share: another queue of the context shares its cache");
+  HS_CUDA(c, cudaSetDevice(c->device));
+  if (!q->ev_share) HS_CUDA(c, create(q->ev_share));
+  if (!c->share_ctr) {  // first use on the context: the synchronous calls' counters, whole or not at all
+    dev_mem<uint32_t> d;
+    mapped<uint32_t> h;
+    cudaError_t e = alloc(d, 4 * (HS_SIG_CTRS + 1));
+    if (e == cudaSuccess) e = alloc(h, 4 * HS_SIG_CTRS);
+    if (e != cudaSuccess) return fail(c, HS_ERR_NOMEM, "hs_queue_sig_share", e);
+    c->share_ctr = std::move(d);
+    c->share_h = std::move(h);
+  }
+  c->share_q = q;
+  return HS_OK;
+}
+
+int hs_queue_sig_share_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_SHARE_STATS]) {
+  return queue_read_stats(q, "hs_queue_sig_share_stats", out, &hs_queue::shstats);
 }
 
 int hs_queue_generic(hs_queue *q, int on) {
@@ -4493,6 +4734,10 @@ int hs_queue_batch(hs_queue *q, size_t max_items, size_t max_bytes) {
     if (e == cudaSuccess) e = alloc(B.grej, max_bytes + 16);  // group words of a region fit in max_bytes
     if (e == cudaSuccess) e = alloc(B.counter, 4);
     if (e == cudaSuccess) e = cudaMemset(B.counter, 0, 4);
+    if (e == cudaSuccess) e = alloc(B.share_list, max_items * 4);
+    if (e == cudaSuccess) e = alloc(B.share_fl, max_items);
+    if (e == cudaSuccess) e = alloc(B.share_ctr, 4 * (HS_SIG_CTRS + 1));
+    if (e == cudaSuccess) e = alloc(B.share_h, 4 * HS_SIG_CTRS);
     return e;
   });
 }
@@ -4573,6 +4818,10 @@ int hs_queue_explain_stats(hs_queue *q, uint64_t out[HS_QUEUE_EXPLAIN_STATS]) {
 
 void hs_queue_destroy(hs_queue *q) {
   if (!q) return;
+  {
+    std::lock_guard<std::mutex> g(q->c->mu);  // ends the sharing (hs_queue_sig_share): later synchronous calls run without the table
+    if (q->c->share_q == q) q->c->share_q = nullptr;
+  }
   {
     std::lock_guard<std::mutex> g(q->c->queues_mu);
     auto &v = q->c->queues;

@@ -839,6 +839,22 @@ class VerifyQueue:
         self.engine._check(self.lib.hs_queue_sig_stats(self.h, out), "hs_queue_sig_stats")
         return dict(zip(self.SIG_STATS, (int(x) for x in out)))
 
+    def sig_share(self, on):
+        """Shares the signature cache (hs_queue_sig_share) with the synchronous verify calls on the engine and with the batch lane:
+        their committee passes answer records the table holds and insert the strict records they accept, so a TC or Block verified
+        synchronously after its Timeouts came through the queue costs probes.  Needs the cache on; one queue per engine.  Verdicts do
+        not change.  False turns it off (the default)."""
+        self.engine._check(self.lib.hs_queue_sig_share(self.h, 1 if on else 0), "hs_queue_sig_share")
+
+    SIG_SHARE_STATS = ("probed", "hits", "inserts", "evictions", "passes")
+
+    def sig_share_stats(self):
+        """Counters of the shared passes (hs_queue_sig_share_stats): records probed, hits, inserts, inserts that evicted a live
+        entry, and the shared passes."""
+        out = (ctypes.c_uint64 * len(self.SIG_SHARE_STATS))()
+        self.engine._check(self.lib.hs_queue_sig_share_stats(self.h, out), "hs_queue_sig_share_stats")
+        return dict(zip(self.SIG_SHARE_STATS, (int(x) for x in out)))
+
     def generic(self, on):
         """Turns the generic-key device path on or off (hs_queue_generic): with it on, a request with a key outside the registered
         committee (every request, when none is registered) is verified by a queue kernel on the GPU instead of synchronously on the

@@ -313,6 +313,34 @@ int hs_queue_sig_cache(hs_queue *q, size_t entries);
 /* Counters of completed launches: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live entry,
  * [4] entries held now */
 int hs_queue_sig_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_STATS]);
+/* Sharing of q's signature cache with the synchronous verify calls on q's context and with q's batch lane.  A TC's votes are the
+ * Timeouts' author signatures; when the Timeouts came through the queue, a TC or Block above GROUP_MAX_SIGS verified synchronously,
+ * or a collected burst on the batch lane, then answers those records from the same table instead of verifying them again.
+ *   - on = 0 is the default: every call launches exactly the kernels it launches without this call.
+ *   - Taking part once on = 1, they probe q's table and fill it: the host-pointer calls hs_verify_strict_batch, hs_verify_rec128,
+ *     hs_verify_batch_shared_msg, hs_verify_qcs, hs_verify_tcs and hs_verify_groups on q's context, when their pass runs the committee
+ *     kernel (k_verify_main<committee>); and q's batch-lane passes.
+ *   - Not taking part: the latency path of 64 records or fewer; every `_dev` entry point (deferred mode, the peer all-gather);
+ *     hs_verify_msgs, hs_verify_var and hs_verify_committee; hs_self_test, the table audit and the repair; and the calls q's own
+ *     dispatcher makes for slow-path requests (slow-path requests and riders neither probe nor insert, as above).
+ *   - Probe: the table's rule, all 128 bytes equal (sig, the registered key's bytes, the Digest); a committee-indexed record uses its
+ *     slot's key bytes.  Records whose key is not registered take the generic side pass and neither probe nor insert; a record whose
+ *     committee slot is out of service (removed by hs_committee_update, or being rebuilt by hs_table_repair) is verified, and so
+ *     rejected, exactly as with sharing off.
+ *   - Insert: only a record judged in STRICT mode whose flags have HS_F_EQ, with its whole flag byte, so a hit answers both modes.
+ *     Strict records are the ones a node meets again (a Timeout author's signature returns in the TC and in the Block carrying it);
+ *     a Block's QC votes (batch-eq) do not, and inserting them would evict those every round.
+ *   - Verdicts are bit for bit those of the same call with sharing off.
+ *   - HS_ERR_ARG when q's signature cache is off or another queue of the context already shares.  hs_queue_sig_cache(q, 0) and
+ *     hs_queue_destroy(q) end the sharing; a resize keeps it, with the new table, after the lane passes in flight and under the
+ *     context's lock, which the synchronous calls hold until their results are back.  A table repair empties the shared table.
+ *   - hs_queue_sig_stats keeps counting the queue's ring kernels only, except [4] (entries held), which includes shared inserts.
+ *   - hs_multi_* calls run member entry points: a member whose queue shares takes part. */
+int hs_queue_sig_share(hs_queue *q, int on);
+#define HS_QUEUE_SIG_SHARE_STATS 5
+/* Counters of the shared passes whose results are back: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live
+ * entry, [4] shared passes */
+int hs_queue_sig_share_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_SHARE_STATS]);
 /* Generic-key device path of the queue.  0 = off (the default: the queue launches exactly the kernels it launches without this
  * call, and a request the committee path cannot serve runs synchronously on the queue's thread).  On: such a request (no committee
  * registered, or any key of the request outside it) is verified on the GPU instead, by k_queue_generic on the queue's

@@ -331,6 +331,15 @@ class VerifyQueue {
     e_.check(hs_queue_sig_stats(q_, s.data()), "hs_queue_sig_stats");
     return s;
   }
+  // hs_queue_sig_share: the synchronous verify calls on the context and the batch lane probe and fill this queue's signature cache
+  // (off by default; needs the cache on, one queue per context).  Verdicts do not change.
+  void sig_share(bool on) { e_.check(hs_queue_sig_share(q_, on ? 1 : 0), "hs_queue_sig_share"); }
+  // hs_queue_sig_share_stats: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live entry, [4] shared passes.
+  std::array<uint64_t, HS_QUEUE_SIG_SHARE_STATS> sig_share_stats() const {
+    std::array<uint64_t, HS_QUEUE_SIG_SHARE_STATS> s{};
+    e_.check(hs_queue_sig_share_stats(q_, s.data()), "hs_queue_sig_share_stats");
+    return s;
+  }
   // hs_queue_generic: verify requests with keys outside the committee on the GPU, not on the dispatcher thread (off by default;
   // off drains the generic launches in flight).  Verdicts do not change.
   void generic(bool on) { e_.check(hs_queue_generic(q_, on ? 1 : 0), "hs_queue_generic"); }

@@ -34,6 +34,10 @@ pub mod cert_cache;
 /// it.  Turned on with the certificate cache (`cert_cache::enable`).
 #[path = "crypto_gpu_sig_cache.rs"]
 pub mod sig_cache;
+/// Sharing of that cache (hs_queue_sig_share) with the synchronous fallbacks for TCs and Blocks above GROUP_MAX_SIGS and with the
+/// batch lane: the votes the queue verified in the Timeouts are hits there too.  Turned on with the cache (`sig_cache::enable`).
+#[path = "crypto_gpu_sig_share.rs"]
+pub mod sig_share;
 /// The queue's generic-key device path (hs_queue_generic): a request with a key outside the registered committee is verified by a
 /// queue kernel instead of holding up the queue's thread.  Turned on when the node-wide queue is created (`queue::queue`).
 #[path = "crypto_gpu_generic_queue.rs"]

@@ -25,10 +25,14 @@ extern "C" {
 
 static ENABLE: Once = Once::new();
 
-/// Turns the cache on for the node-wide queue, once.  A failure leaves it off: every record is then verified, with the same
-/// verdicts.
+/// Turns the cache on for the node-wide queue, once, and then shares it with the synchronous calls and the batch lane
+/// (`sig_share::enable`).  A failure leaves it off: every record is then verified, with the same verdicts.
 pub(crate) fn enable(q: *mut HsQueue) {
-    ENABLE.call_once(|| { let _ = unsafe { hs_queue_sig_cache(q, SIG_CACHE_ENTRIES) }; });
+    ENABLE.call_once(|| {
+        if unsafe { hs_queue_sig_cache(q, SIG_CACHE_ENTRIES) } == HS_OK {
+            super::sig_share::enable(q);
+        }
+    });
 }
 
 /// The cache's counters for the node's metrics: records probed, hits, inserts, inserts that evicted a live entry, entries held.

@@ -1780,6 +1780,9 @@ struct hs_ctx {
   unsigned n_sms = 0;                // multiprocessors of `device` (sizes the grid of the side pass)
   stream_h stream, stream2, stream_side;
   event_h ev[2], ev_done[2], ev_side[2];
+  // recorded after the last enqueue of every `_dev` verify pass on a caller's stream: the host-pointer calls reuse the same scratch on
+  // `stream`, which waits for it before its first enqueue (h2d_stage::upload on `stream`, hs_verify_msgs)
+  event_h ev_dev_pass;
   dev_mem<ge_niels> d_btable;
   comb_params cp{};
   size_t a_table_entries = 0;
@@ -1912,6 +1915,10 @@ struct h2d_stage {
     return n++;
   }
   int upload(hs_ctx *c, dev_buf &buf, cudaStream_t stream) {
+    // The host-pointer entry points stage on the context's stream and then run passes over the verify scratch, which a `_dev` pass on
+    // the caller's stream may still read: they wait for it.  The self-test, the audit, the scrub and slot builds stage on streams of
+    // their own for work over scratch of their own, and do not.
+    if (stream == c->stream) HS_CUDA(c, cudaStreamWaitEvent(stream, c->ev_dev_pass, 0));
     HS_TRY(ensure(c, buf, total));
     base = (uint8_t *)buf.p.get();
     for (size_t k = 0; k < n; k++)
@@ -2278,6 +2285,9 @@ static int run_verify(hs_ctx *c, in_layout L, size_t n, uint32_t mode, uint32_t 
     c->share_passes++;
   }
   if (defer) HS_CUDA(c, cudaEventRecord(c->ev_tail[set], c->stream_tail));
+  // a pass on a caller's stream: the next host-pointer call waits for it before it reuses this scratch (and group_digests, whose
+  // Digest kernel hs_verify_groups_dev enqueued before this pass on the same stream)
+  if (fin_stream != c->stream) HS_CUDA(c, cudaEventRecord(c->ev_dev_pass, fin_stream));
   return HS_OK;
 }
 
@@ -3462,6 +3472,7 @@ int hs_ctx_create(hs_ctx **out, int device, uint32_t flags) {
     if (e == cudaSuccess) e = create(c->ev_done[i]);
     if (e == cudaSuccess) e = create(c->ev_side[i]);
   }
+  if (e == cudaSuccess) e = create(c->ev_dev_pass);
   if (e == cudaSuccess) e = alloc(c->d_miss_count, 4);
   if (e == cudaSuccess) e = create(c->stream_tail);
   if (e == cudaSuccess) e = create(c->ev_main_done);
@@ -4209,6 +4220,8 @@ int hs_verify_msgs(hs_ctx *c, const uint8_t *sig, const uint8_t *pk, const uint3
   }
   // (A short "ramp" first chunk was tried and measured slower — 7.1e7 vs 7.6e7 verifies/s: every extra chunk costs one more
   // generic-pass latency when the batch contains unknown keys.)
+  // The chunks' passes reuse the verify scratch on `stream`, after any `_dev` pass that may still read it (staging on stream2 does not)
+  HS_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_dev_pass, 0));
   size_t lo = 0;
   for (size_t j = 0; lo < n; j++) {
     const int b = (int)(j & 1);

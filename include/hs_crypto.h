@@ -14,7 +14,13 @@
  *   - Malformed inputs (S >= l, non-decompressible A or R, ...) are verdict 0, never an error.
  *   - Host-pointer entry points copy inputs to the device, run, and copy results back before returning; nothing is
  *     retained.  `_dev` entry points take device pointers and a cudaStream_t (as void*) and return after enqueueing.
- *   - A context is bound to one CUDA device and is thread-safe (calls are serialised on an internal mutex).
+ *   - A context is bound to one CUDA device.  Its host-pointer calls are thread-safe (serialised on an internal mutex).  `_dev` calls
+ *     take no mutex, so they are not serialised with calls on other threads: issue them from one thread, on one stream at a time.
+ *   - A host-pointer call runs after the non-deferred `_dev` verify passes enqueued earlier on the same thread on the stream last
+ *     used for one (the context remembers only the latest pass, which with one stream at a time orders it after all of them): both
+ *     use the context's verify scratch, so the host call's stream waits for that pass first.  The latency path (64 records or fewer
+ *     whose keys all have tables, registered or learned), the self-test, the audit, repairs, staged committee changes and the scrub
+ *     have scratch of their own and do not wait.
  *   - Bitmaps: bit (i & 31) of word (i >> 5) is the verdict of item i; unused high bits of the last word are 0.
  */
 #ifndef HS_CRYPTO_H
@@ -599,7 +605,12 @@ int hs_scrub_stats(hs_ctx *ctx, uint64_t out[HS_SCRUB_STATS]);
 #define HS_WHY_EQUATION 32u
 int hs_explain_rec128(hs_ctx *ctx, const hs_rec128 *recs, size_t n, uint8_t *out_why /* n */);
 
-/* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) ------------------- */
+/* ---- device-resident entry points (inputs already in HBM; enqueue on `stream`, a cudaStream_t) -------------------
+ * Every kernel and copy of a call is ordered after the caller's earlier work on `stream`; misses of the committee lookup run on an
+ * internal stream and join back into `stream` before the finish kernel.  The calls take no mutex (see Conventions): one thread and one
+ * stream at a time per context.  A host-pointer call made after a verify pass (rec128, var, committee, msgs, qc_votes, groups) waits
+ * on the device for the latest such pass before it reuses the shared scratch; with deferred mode on, host-pointer calls must still not
+ * be mixed with deferred passes in flight (hs_set_deferred). */
 int hs_verify_rec128_dev(hs_ctx *ctx, const void *d_recs, size_t n, uint32_t mode, void *d_bitmap, void *stream);
 int hs_verify_var_dev(hs_ctx *ctx, const void *d_sig, const void *d_pk, const void *d_msgs, const void *d_off, size_t n,
                       uint32_t mode, void *d_bitmap, void *stream);

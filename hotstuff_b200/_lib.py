@@ -73,6 +73,8 @@ SIGNATURES = {
     "hs_queue_sig_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_sig_share": (c_int, [c_void_p, c_int]),
     "hs_queue_sig_share_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_queue_sig_audit": (c_int, [c_void_p, c_size_t, c_size_t, ctypes.POINTER(c_u64)]),
+    "hs_queue_sig_audit_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_generic": (c_int, [c_void_p, c_int]),
     "hs_queue_generic_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
     "hs_queue_batch": (c_int, [c_void_p, c_size_t, c_size_t]),
@@ -93,6 +95,7 @@ SIGNATURES = {
     "hs_scrub_set_map": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t]),
     "hs_scrub_stop": (c_int, [c_void_p]),
     "hs_scrub_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_scrub_sig_cache": (c_int, [c_void_p, c_void_p, c_u32]),
     "hs_explain_rec128": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "hs_multi_create": (c_int, [ctypes.POINTER(c_void_p), c_void_p, c_size_t, c_u32]),
     "hs_multi_destroy": (None, [c_void_p]),

@@ -1111,6 +1111,64 @@ __global__ void __launch_bounds__(256) k_sig_fill(in_layout L, size_t n, committ
   }
   sig_count_pair(sc, 2, ins != 0, ins == 2);
 }
+// The audit of a signature-cache table (hs_queue_sig_audit): a thread per entry of buckets [first, first + count), grid-stride.  An entry
+// read as one version by the probes' rule (seq acquired, the words and flags relaxed, a fence, seq again) is re-checked from its 128 bytes
+// alone with explain_record, which reads no table; flags_from_why of the result is the byte any verify path writes for that record.  An
+// entry whose byte differs gets that byte through sig_insert's writer protocol (claim seq, store, fence, release s0 + 2), so a hit
+// answers exactly what a verify would, reject included.  seq never goes back to 0 and the words are never cleared: 128 zero bytes are
+// a record too.  An entry being written, torn between the reads, or claimed by a writer before the correction is skipped.
+// out: [0] held, [1] corrected, [2] skipped, [3] the first correction as position (bucket * HS_SIG_WAYS + way) << 24 | stored byte << 16 |
+// derived byte << 8 | why, kept by atomicMin (position < 2^26).
+__global__ void __launch_bounds__(HS_THREADS) k_sig_audit(sig_bucket *b, uint32_t first, uint32_t count, unsigned long long *out) {
+  uint32_t held = 0, corrected = 0, skipped = 0;
+  for (uint32_t j = blockIdx.x * HS_THREADS + threadIdx.x; j < count * HS_SIG_WAYS; j += gridDim.x * HS_THREADS) {
+    const uint32_t bucket = first + j / HS_SIG_WAYS, way = j % HS_SIG_WAYS;
+    sig_entry *x = b[bucket].e + way;
+    const uint32_t s0 = ld_acquire_gpu(&x->seq);
+    if (!s0) continue;
+    uint32_t R[8], S[8], A[8], M[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+      R[k] = ld_relaxed_gpu(x->w + k);
+      S[k] = ld_relaxed_gpu(x->w + 8 + k);
+      A[k] = ld_relaxed_gpu(x->w + 16 + k);
+      M[k] = ld_relaxed_gpu(x->w + 24 + k);
+    }
+    const uint32_t fl = ld_relaxed_gpu(&x->flags);
+    __threadfence();
+    if ((s0 & 1u) || ld_relaxed_gpu(&x->seq) != s0) {
+      skipped++;
+      continue;
+    }
+    uint32_t h[16];
+    sha512_ram32(h, R, A, M);
+    ge_cached tab[9];
+    const uint32_t why = explain_record(R, S, A, h, tab), want = flags_from_why(why);
+    if ((fl & 0x1fu) == want) {
+      held++;
+      continue;
+    }
+    if (atomicCAS(&x->seq, s0, s0 + 1) != s0) {  // a writer put a newer record here
+      skipped++;
+      continue;
+    }
+    __threadfence();
+    st_relaxed_gpu(&x->flags, want);
+    __threadfence();
+    st_relaxed_gpu(&x->seq, s0 + 2);
+    held++;
+    corrected++;
+    atomicMin(out + 3, ((unsigned long long)(bucket * HS_SIG_WAYS + way) << 24) | ((fl & 0xffu) << 16) | (want << 8) | why);
+  }
+  held = __reduce_add_sync(0xffffffffu, held);
+  corrected = __reduce_add_sync(0xffffffffu, corrected);
+  skipped = __reduce_add_sync(0xffffffffu, skipped);
+  if ((threadIdx.x & 31) == 0) {
+    if (held) atomicAdd(out, (unsigned long long)held);
+    if (corrected) atomicAdd(out + 1, (unsigned long long)corrected);
+    if (skipped) atomicAdd(out + 2, (unsigned long long)skipped);
+  }
+}
 
 // ------------------------------------------------------------------------------------------------ table construction
 // thread = (point p, window w, block b of HS_BUILD_BLOCK entries).  slots (nullable): point p is slot slots[p], its key at encs + 32
@@ -1773,6 +1831,11 @@ struct scrub_state {
   void *user = nullptr;
   size_t next_slot = 0;             // the pass: the slots before next_slot and the base entries before next_base are audited
   uint64_t next_base = 0;
+  // hs_scrub_sig_cache: the queue whose signature cache each tick also audits, sig_per_tick buckets from sig_next on, in the table of
+  // generation sig_gen (a new table starts at bucket 0)
+  hs_queue *sig_q = nullptr;
+  uint32_t sig_per_tick = 0, sig_gen = 0;
+  size_t sig_next = 0;
   std::atomic<uint64_t> stats[SCRUB_NSTATS] = {};
 };
 struct hs_ctx {
@@ -2338,6 +2401,14 @@ static cudaError_t launch_queue_explain(hs_ctx *c, const xq_desc *list, uint32_t
   c->launches++;
   return cudaGetLastError();
 }
+// k_sig_audit over buckets [first, first + n) of table b, results into out (4 words).  Its threads run explain_record's re-check as the
+// explain lane's do, so it takes the same share of the SMs.
+static cudaError_t launch_sig_audit(hs_ctx *c, sig_bucket *b, uint32_t first, uint32_t n, unsigned long long *out, cudaStream_t s) {
+  const unsigned grid = (unsigned)std::min<size_t>(blocks_for((size_t)n * HS_SIG_WAYS), std::max<size_t>(1, c->n_sms / HS_QUEUE_EXPLAIN_SM_DIV));
+  k_sig_audit<<<grid, HS_THREADS, 0, s>>>(b, first, n, out);
+  c->launches++;
+  return cudaGetLastError();
+}
 
 // ---- latency path (host side)
 // key bytes -> table index through the host mirror of the device hash table (registered committee or learned cache)
@@ -2654,6 +2725,11 @@ struct hs_queue {
   // hs_queue_sig_share: ev_share is recorded after every batch-lane pass that shares the table (under c->mu), so a resize can wait for it
   event_h ev_share;
   uint64_t shstats[HS_QUEUE_SIG_SHARE_STATS] = {};  // hs_queue_sig_share_stats
+  // hs_queue_sig_audit: ev_audit is recorded after every audit launch on the table (under c->mu), so a resize can wait for it; d_audit
+  // holds a launch's four result words (audits run one at a time under c->audit_mu)
+  event_h ev_audit;
+  dev_mem<unsigned long long> d_audit;
+  uint64_t astats[HS_QUEUE_SIG_AUDIT_STATS] = {};  // hs_queue_sig_audit_stats
   std::mutex mu;  // everything above that submit / poll / wait touch: tail, reqs of pending slots, results, head, stop
   std::condition_variable cv_work, cv_done;
   std::thread th;
@@ -3384,6 +3460,7 @@ static void queue_free(hs_queue *q) {
   // the last launches' blocks have exited before the ring goes
   if (q->ev_last) cudaEventSynchronize(q->ev_last);
   if (q->ev_bulk_last) cudaEventSynchronize(q->ev_bulk_last);
+  if (q->ev_audit) cudaEventSynchronize(q->ev_audit);
   for (side_lane *L : queue_lanes(q)) lane_drain(*L);
   delete q;  // the owners release the rest
 }
@@ -4639,6 +4716,7 @@ static int sig_cache_set_locked(hs_queue *q, uint32_t buckets) {
   HS_CUDA(c, cudaStreamSynchronize(q->stream));
   HS_CUDA(c, cudaStreamSynchronize(q->bulk_stream));
   if (q->ev_share) HS_CUDA(c, cudaEventSynchronize(q->ev_share));
+  if (q->ev_audit) HS_CUDA(c, cudaEventSynchronize(q->ev_audit));  // an audit of the old table (hs_queue_sig_audit, enqueued under c->mu)
   if (!buckets && c->share_q == q) c->share_q = nullptr;  // turning the cache off ends the sharing; a resize keeps it
   q->d_sig.reset();
   {
@@ -4834,6 +4912,10 @@ void hs_queue_destroy(hs_queue *q) {
   {
     std::lock_guard<std::mutex> g(q->c->mu);  // ends the sharing (hs_queue_sig_share): later synchronous calls run without the table
     if (q->c->share_q == q) q->c->share_q = nullptr;
+  }
+  {
+    std::lock_guard<std::mutex> l(q->c->scrub.m);  // a scrub tick auditing q's cache (hs_scrub_sig_cache) holds it until it is done
+    if (q->c->scrub.sig_q == q) q->c->scrub.sig_q = nullptr;
   }
   {
     std::lock_guard<std::mutex> g(q->c->queues_mu);
@@ -5651,6 +5733,75 @@ extern "C" int hs_committee_discard(hs_ctx *c) {
   return HS_OK;
 }
 
+// ---- audit of a verify queue's signature cache (hs_queue_sig_audit, and the scrub's slices of it)
+// The range an audit takes: buckets [first, first + n) (n = 0: none), and whether that is the whole table (a pass).
+struct sig_audit_range {
+  size_t first = 0, n = 0;
+  bool pass = false;
+};
+// One k_sig_audit launch on the audit's stream: pick(buckets, sig_gen, range) chooses the range under c->mu from the table's size (0:
+// the cache is off) and generation; false is HS_ERR_ARG.  Enqueued under c->mu, waited for and read back without it.  The caller holds
+// audit_mu.  out: hs_queue_sig_audit's words; q's counters take the run.
+template <class Pick>
+static int sig_audit_run(hs_queue *q, const char *entry, Pick pick, uint64_t out[HS_QUEUE_SIG_AUDIT_OUT]) {
+  hs_ctx *c = q->c;
+  sig_audit_range r;
+  {
+    std::lock_guard<std::mutex> g(c->mu);  // the dispatcher and hs_queue_sig_cache change the table only under it
+    if (!pick(q->d_sig ? q->sig_bmask + 1 : 0u, q->sig_gen, r))
+      return fail_args(c, entry, "the signature cache is off, or the bucket range leaves its table");
+    if (r.n) {
+      HS_CUDA(c, cudaSetDevice(c->device));
+      HS_TRY(audit_stream(c));
+      if (!q->ev_audit) HS_CUDA(c, create(q->ev_audit));
+      if (!q->d_audit) HS_CUDA(c, alloc(q->d_audit, 4 * sizeof(unsigned long long)));
+      const cudaStream_t s = c->audit.stream;
+      HS_CUDA(c, cudaMemsetAsync(q->d_audit, 0, 3 * sizeof(unsigned long long), s));
+      HS_CUDA(c, cudaMemsetAsync(q->d_audit + 3, 0xff, sizeof(unsigned long long), s));
+      HS_CUDA(c, launch_sig_audit(c, q->d_sig, (uint32_t)r.first, (uint32_t)r.n, q->d_audit, s));
+      HS_CUDA(c, cudaEventRecord(q->ev_audit, s));  // sig_cache_set_locked waits for it before the table goes
+    }
+  }
+  unsigned long long res[4] = {0, 0, 0, ~0ull};
+  if (r.n) {
+    HS_CUDA(c, cudaEventSynchronize(q->ev_audit));
+    HS_CUDA(c, cudaMemcpyAsync(res, q->d_audit, sizeof(res), cudaMemcpyDeviceToHost, c->audit.stream));
+    HS_CUDA(c, cudaStreamSynchronize(c->audit.stream));
+  }
+  const bool any = res[3] != ~0ull;
+  const uint64_t v[HS_QUEUE_SIG_AUDIT_OUT] = {res[0], res[1], res[2], any ? res[3] >> 24 : UINT64_MAX, any ? (res[3] >> 16) & 0xff : 0,
+                                              any ? (res[3] >> 8) & 0xff : 0, any ? res[3] & 0xff : 0};
+  memcpy(out, v, sizeof(v));
+  std::lock_guard<std::mutex> gq(q->mu);
+  if (r.n) {
+    q->astats[0]++;
+    q->astats[1] += res[0];
+    q->astats[2] += res[1];
+    q->astats[3] += res[2];
+  }
+  if (r.pass) q->astats[4]++;
+  return HS_OK;
+}
+
+extern "C" int hs_queue_sig_audit(hs_queue *q, size_t first_bucket, size_t n_buckets, uint64_t out[HS_QUEUE_SIG_AUDIT_OUT]) {
+  if (!q || !out) return fail(q ? q->c : nullptr, HS_ERR_ARG, "hs_queue_sig_audit: bad argument");
+  std::lock_guard<std::mutex> ga(q->c->audit_mu);
+  return sig_audit_run(
+      q, "hs_queue_sig_audit",
+      [&](uint32_t buckets, uint32_t, sig_audit_range &r) {
+        if (!buckets || first_bucket >= buckets || n_buckets > buckets - first_bucket) return false;
+        r.first = first_bucket;
+        r.n = n_buckets ? n_buckets : buckets - first_bucket;
+        r.pass = r.first == 0 && r.n == buckets;
+        return true;
+      },
+      out);
+}
+
+extern "C" int hs_queue_sig_audit_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_AUDIT_STATS]) {
+  return queue_read_stats(q, "hs_queue_sig_audit_stats", out, &hs_queue::astats);
+}
+
 // ---- the engine-owned scrub of the live key tables (hs_scrub_start / hs_scrub_set_map / hs_scrub_stop / hs_scrub_stats)
 // Takes the caller's map (or the engine's own) for the current slot map, under S.m: the rules of hs_table_audit.  A new map starts a
 // new pass.
@@ -5773,6 +5924,34 @@ static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
   for (size_t k = 0; k < r.n_slots; k++) S.stats[SCRUB_REPAIRED] += (r.bits()[2 + k] && !after.bits()[2 + k]) ? 1 : 0;
   return HS_OK;
 }
+// The signature-cache slice of a tick, under S.m and whether or not the slot map is paused: the next sig_per_tick buckets of the attached
+// queue's table (hs_scrub_sig_cache), wrapping at its end; a new table starts at bucket 0, and a cache that is off is skipped.  A
+// correction is reported as HS_AUDIT_SIGCACHE in found, never in failed: the entry holds the re-checked byte once it is corrected.
+static int scrub_sig_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
+  if (!S.sig_q) return HS_OK;
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  uint64_t out[HS_QUEUE_SIG_AUDIT_OUT];
+  HS_TRY(sig_audit_run(
+      S.sig_q, "hs_scrub",
+      [&S](uint32_t buckets, uint32_t gen, sig_audit_range &r) {
+        if (gen != S.sig_gen) {
+          S.sig_gen = gen;
+          S.sig_next = 0;
+        }
+        if (!buckets) return true;
+        r.first = S.sig_next;
+        r.n = std::min<size_t>(S.sig_per_tick, buckets - r.first);
+        S.sig_next = r.first + r.n;
+        if (S.sig_next >= buckets) {
+          r.pass = true;
+          S.sig_next = 0;
+        }
+        return true;
+      },
+      out));
+  if (out[1]) rep.found |= HS_AUDIT_SIGCACHE;
+  return HS_OK;
+}
 static void scrub_loop(hs_ctx *c) {
   scrub_state &S = c->scrub;
   pthread_setname_np(pthread_self(), "hs_scrub");  // names it in ps / top and /proc/<pid>/task/*/comm
@@ -5781,6 +5960,7 @@ static void scrub_loop(hs_ctx *c) {
   while (!S.cv.wait_for(l, std::chrono::microseconds(S.period_us), [&S] { return S.stop; })) {
     scrub_report rep;
     if ((S.rc = scrub_tick(c, S, rep)) != HS_OK) return;
+    if ((S.rc = scrub_sig_tick(c, S, rep)) != HS_OK) return;
     if (rep.found && S.cb) {  // without S.m: the callback may call hs_scrub_set_map
       l.unlock();
       S.cb(S.user, rep.found, rep.failed, rep.first_slot);
@@ -5838,6 +6018,17 @@ extern "C" int hs_scrub_stop(hs_ctx *c) {
   return rc;
 }
 
+extern "C" int hs_scrub_sig_cache(hs_ctx *c, hs_queue *q, uint32_t buckets_per_tick) {
+  if (!c || (q && (q->c != c || !buckets_per_tick))) return fail_args(c, "hs_scrub_sig_cache", "bad argument");
+  scrub_state &S = c->scrub;
+  std::lock_guard<std::mutex> l(S.m);
+  S.sig_q = q;
+  S.sig_per_tick = buckets_per_tick;
+  S.sig_gen = 0;
+  S.sig_next = 0;
+  return HS_OK;
+}
+
 extern "C" int hs_scrub_stats(hs_ctx *c, uint64_t out[HS_SCRUB_STATS]) {
   if (!c || !out) return HS_ERR_ARG;
   for (int k = 0; k < SCRUB_NSTATS; k++) out[k] = c->scrub.stats[k].load();
@@ -5889,5 +6080,29 @@ extern "C" int hs_test_poke(hs_ctx *c, int region, size_t index, size_t byte_off
   v ^= xor_mask;
   HS_CUDA(c, cudaMemcpy(p, &v, 1, cudaMemcpyHostToDevice));
   return HS_OK;
+}
+// XORs one byte of the signature-cache entry of q that holds rec (sig | key bytes | Digest) on an idle queue: byte_offset < 128 into its
+// words, 128 its flag byte.  HS_ERR_ARG when the cache is off, no entry holds rec or the offset is past the flag byte.  It changes the
+// bytes a hit answers from, never seq or the round-robin counter.
+extern "C" int hs_test_poke_sig(hs_queue *q, const uint8_t rec[128], size_t byte_offset, uint8_t xor_mask) {
+  if (!q || !rec || byte_offset > 128) return HS_ERR_ARG;
+  hs_ctx *c = q->c;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!q->d_sig) return fail_args(c, "hs_test_poke_sig", "the signature cache is off");
+  HS_CUDA(c, cudaSetDevice(c->device));
+  HS_CUDA(c, cudaDeviceSynchronize());
+  std::vector<sig_bucket> t((size_t)q->sig_bmask + 1);
+  HS_CUDA(c, cudaMemcpy(t.data(), q->d_sig, t.size() * sizeof(sig_bucket), cudaMemcpyDeviceToHost));
+  for (size_t b = 0; b < t.size(); b++)
+    for (int e = 0; e < HS_SIG_WAYS; e++) {
+      const sig_entry &x = t[b].e[e];
+      if (!x.seq || (x.seq & 1u) || memcmp(x.w, rec, 128)) continue;
+      const size_t off = b * sizeof(sig_bucket) + e * sizeof(sig_entry) + (byte_offset < 128 ? byte_offset : offsetof(sig_entry, flags));
+      uint8_t *p = reinterpret_cast<uint8_t *>(q->d_sig.get()) + off;
+      const uint8_t v = reinterpret_cast<const uint8_t *>(t.data())[off] ^ xor_mask;
+      HS_CUDA(c, cudaMemcpy(p, &v, 1, cudaMemcpyHostToDevice));
+      return HS_OK;
+    }
+  return fail_args(c, "hs_test_poke_sig", "no entry holds the record");
 }
 #endif

@@ -506,6 +506,16 @@ HS_HD uint32_t explain_record(const uint32_t (&R)[8], const uint32_t (&S)[8], co
   if (!ge_proj_equals_affine(Rp.X, Rp.Y, Rp.Z, Rpt.X, Rpt.Y)) why |= HS_WHY_EQUATION;
   return why;
 }
+// The flag byte verify_flags_from writes for the same record, from its explain_record mask: the signature cache's audit
+// (hs_queue_sig_audit) re-derives a stored entry's flags with it, table-free.
+HS_HD uint32_t flags_from_why(uint32_t why) {
+  uint32_t fl = 0;
+  if (!(why & (HS_WHY_S_NONCANONICAL | HS_WHY_A_INVALID))) fl |= HS_F_PARSE_OK;
+  if (!(why & ~(HS_WHY_A_SMALL | HS_WHY_R_SMALL))) fl |= HS_F_EQ;
+  if (why & (HS_WHY_A_SMALL | HS_WHY_R_SMALL)) fl |= HS_F_SMALL;
+  if (!why) fl |= HS_F_STRICT;
+  return fl;
+}
 
 // ---- signing (load generation only: SURVEY §8f.4 — the reference node signs on the CPU, one signature per request,
 // crypto/src/lib.rs:185-191; this exists to synthesise 2^20-scale benchmark / test inputs in milliseconds).  RFC 8032 §5.1.6:

@@ -20,6 +20,7 @@ WHY_R_INVALID = 4       # R does not decompress
 WHY_A_SMALL = 8         # [8]A is the identity
 WHY_R_SMALL = 16        # [8]R is the identity
 WHY_EQUATION = 32       # S, A, R parse and [S]B + [k](-A) != R
+AUDIT_SIGCACHE = 32  # a scrub callback's found: the tick corrected a signature-cache entry (hs_scrub_sig_cache)
 
 
 class EngineError(RuntimeError):
@@ -202,6 +203,12 @@ class Engine:
         out = (ctypes.c_uint64 * len(self.SCRUB_STATS))()
         self._check(self.lib.hs_scrub_stats(self.h, out), "hs_scrub_stats")
         return dict(zip(self.SCRUB_STATS, (int(v) for v in out)))
+
+    def scrub_sig_cache(self, queue, buckets_per_tick=512):
+        """Attaches a VerifyQueue of this engine to the scrub (hs_scrub_sig_cache): every tick then also audits the next
+        buckets_per_tick buckets of its signature cache (VerifyQueue.sig_audit), wrapping around, and a tick that corrected an entry
+        calls back with AUDIT_SIGCACHE in found.  None detaches."""
+        self._check(self.lib.hs_scrub_sig_cache(self.h, queue.h if queue is not None else None, int(buckets_per_tick)), "hs_scrub_sig_cache")
 
     def explain(self, recs):
         """Table-free re-check of (n,128) uint8 records (hs_explain_rec128) -> uint8[n] of WHY_* bits, one per failed check.  The strict
@@ -854,6 +861,30 @@ class VerifyQueue:
         out = (ctypes.c_uint64 * len(self.SIG_SHARE_STATS))()
         self.engine._check(self.lib.hs_queue_sig_share_stats(self.h, out), "hs_queue_sig_share_stats")
         return dict(zip(self.SIG_SHARE_STATS, (int(x) for x in out)))
+
+    SIG_AUDIT_OUT = ("held", "corrected", "skipped", "first_position", "first_stored", "first_derived", "first_why")
+
+    def sig_audit(self, first_bucket=0, n_buckets=0):
+        """Audits the signature cache (hs_queue_sig_audit): every held entry of buckets [first_bucket, first_bucket + n_buckets) (0: to
+        the end of the table) is re-checked from its 128 bytes with the table-free re-check of Engine.explain, and a flag byte that
+        disagrees is corrected.  Returns a dict keyed by SIG_AUDIT_OUT: entries held, corrected and skipped (being written), and the
+        first correction's position (bucket * 4 + way; None: no correction), stored and derived flag bytes and WHY_* mask.  Raises
+        EngineError when the cache is off or the range leaves the table."""
+        out = (ctypes.c_uint64 * len(self.SIG_AUDIT_OUT))()
+        self.engine._check(self.lib.hs_queue_sig_audit(self.h, int(first_bucket), int(n_buckets), out), "hs_queue_sig_audit")
+        r = dict(zip(self.SIG_AUDIT_OUT, (int(x) for x in out)))
+        if r["first_position"] == 2**64 - 1:
+            r["first_position"] = None
+        return r
+
+    SIG_AUDIT_STATS = ("audits", "checked", "corrected", "skipped", "passes")
+
+    def sig_audit_stats(self):
+        """Counters over sig_audit calls and scrub slices (hs_queue_sig_audit_stats): audits, entries re-checked, corrected, skipped,
+        and full passes of the table."""
+        out = (ctypes.c_uint64 * len(self.SIG_AUDIT_STATS))()
+        self.engine._check(self.lib.hs_queue_sig_audit_stats(self.h, out), "hs_queue_sig_audit_stats")
+        return dict(zip(self.SIG_AUDIT_STATS, (int(x) for x in out)))
 
     def generic(self, on):
         """Turns the generic-key device path on or off (hs_queue_generic): with it on, a request with a key outside the registered

@@ -347,6 +347,30 @@ int hs_queue_sig_share(hs_queue *q, int on);
 /* Counters of the shared passes whose results are back: [0] records probed, [1] hits, [2] inserts, [3] inserts that evicted a live
  * entry, [4] shared passes */
 int hs_queue_sig_share_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_SHARE_STATS]);
+/* Audit of q's signature cache: every held entry of buckets [first_bucket, first_bucket + n_buckets) re-checked from its 128 stored
+ * bytes, and the flag bytes that disagree corrected.  A hit answers from the stored flag byte with no check at all, so a flipped bit
+ * there is a false accept (a batch-eq-only record answered strict) or a false reject that lasts until the entry is evicted.
+ *   - Check: a thread per entry reads it as one version by the probes' rule (an entry being written, or changed between the reads, is
+ *     skipped), computes k = SHA-512(R || A || Digest) and hs_explain_rec128's mask with no table of any kind (no comb table, key slot
+ *     or base-point table), and derives from the mask the flag byte every verify path writes for that record.
+ *   - Correction: an entry whose flag byte differs gets the derived byte under the writers' protocol; one a writer claimed meanwhile
+ *     holds a newer record and is skipped.  A corrected entry's hits then answer exactly what a verify answers, reject included.
+ *     Entries are never emptied or evicted by the audit, and the probe and insert paths are unchanged.
+ *   - n_buckets = 0: from first_bucket to the end of the table (the whole table with first_bucket 0).  HS_ERR_ARG writes nothing: q or
+ *     out NULL, the cache off, or a range that leaves the table.
+ *   - out: [0] entries held (re-checked), [1] corrected, [2] skipped, [3] the first corrected position (bucket * 4 + way; UINT64_MAX:
+ *     none), [4] its stored flag byte, [5] its derived flag byte, [6] its HS_WHY_* mask ([4..6] are 0 with no correction).
+ *   - Synchronous.  The kernel runs on the table audit's private stream of the lowest priority, on at most a quarter of the SMs, and
+ *     takes hs_table_audit's turn (audits, repairs, stages, commits and scrub ticks of the context run one at a time); the context's
+ *     mutex is held only to read the table and enqueue, so the queue keeps launching beside it.  hs_queue_sig_cache (a resize, off,
+ *     or the flush of hs_table_repair) waits for an audit in flight before its table goes.
+ *   - hs_scrub_sig_cache runs it a slice per scrub tick. */
+#define HS_QUEUE_SIG_AUDIT_OUT 7
+int hs_queue_sig_audit(hs_queue *q, size_t first_bucket, size_t n_buckets, uint64_t out[HS_QUEUE_SIG_AUDIT_OUT]);
+#define HS_QUEUE_SIG_AUDIT_STATS 5
+/* Counters over hs_queue_sig_audit calls and scrub slices: [0] audits, [1] entries re-checked (held), [2] corrected, [3] skipped,
+ * [4] full passes of the table */
+int hs_queue_sig_audit_stats(hs_queue *q, uint64_t out[HS_QUEUE_SIG_AUDIT_STATS]);
 /* Generic-key device path of the queue.  0 = off (the default: the queue launches exactly the kernels it launches without this
  * call, and a request the committee path cannot serve runs synchronously on the queue's thread).  On: such a request (no committee
  * registered, or any key of the request outside it) is verified on the GPU instead, by k_queue_generic on the queue's
@@ -509,6 +533,7 @@ size_t hs_key_slots(const hs_ctx *ctx);
                                      bytes), or a hash entry names this slot although it is not live */
 #define HS_AUDIT_TABLE  (1u << 3) /* an entry of the slot's comb table is not the multiple of -A it must hold */
 #define HS_AUDIT_BASE   (1u << 4) /* out_failed only: an entry of the base-point table is not the multiple of B it must hold */
+#define HS_AUDIT_SIGCACHE (1u << 5) /* a scrub callback's found only: the tick corrected a signature-cache entry (hs_scrub_sig_cache) */
 int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
                    size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_failed);
 
@@ -574,6 +599,15 @@ int hs_scrub_stop(hs_ctx *ctx);
  * finding), slots repaired, failed repairs (findings the second audit still finds), ticks paused on a stale map */
 #define HS_SCRUB_STATS 8
 int hs_scrub_stats(hs_ctx *ctx, uint64_t out[HS_SCRUB_STATS]);
+/* Attaches q (a queue of ctx) to ctx's scrub: from then on every tick also audits the next buckets_per_tick buckets of q's signature
+ * cache with hs_queue_sig_audit, wrapping at the end of the table, whether or not the slot map is paused.  A new table (a resize, or
+ * the cache turned off and on) starts again at bucket 0; while the cache is off the slice audits nothing.  q_or_null = NULL detaches.
+ *   - A tick that corrected an entry calls cb with HS_AUDIT_SIGCACHE in found (first_slot is (size_t)-1 unless a slot had a finding);
+ *     failed never carries it.  hs_queue_sig_audit_stats counts the slices and the passes they complete.
+ *   - The attachment outlives hs_scrub_stop / hs_scrub_start; hs_queue_destroy(q) detaches q, after a tick in progress.  Without this
+ *     call a scrub launches nothing for any queue.
+ *   - HS_ERR_ARG: ctx NULL, q of another context, or buckets_per_tick 0 with q given. */
+int hs_scrub_sig_cache(hs_ctx *ctx, hs_queue *q_or_null, uint32_t buckets_per_tick);
 
 /* ---- explanation of a verdict: a table-free re-check that names every check a record fails ------------------------------------
  * A verify call answers 0 for malformed bytes, a small-order key or R, a signature over another message and a false reject by the

@@ -28,6 +28,8 @@ struct EngineError : std::runtime_error {
   using std::runtime_error::runtime_error;
 };
 
+class VerifyQueue;
+
 class Engine {
  public:
   explicit Engine(int device = 0, uint32_t flags = 0) {
@@ -115,6 +117,9 @@ class Engine {
     check(hs_scrub_stats(ctx_, s.data()), "hs_scrub_stats");
     return s;
   }
+  // Attaches q (a queue of this engine) to the scrub (hs_scrub_sig_cache): every tick also audits the next buckets_per_tick buckets of
+  // its signature cache, and a tick that corrected an entry calls back with HS_AUDIT_SIGCACHE in found.  nullptr detaches.
+  inline void scrub_sig_cache(const VerifyQueue *q, uint32_t buckets_per_tick = 512) const;
   // Table-free re-check of n records (hs_explain_rec128): one byte of HS_WHY_* bits per record, one bit per failed check.  Strict
   // verdict 1 <=> 0; batch-eq verdict 1 <=> no bit outside HS_WHY_A_SMALL | HS_WHY_R_SMALL.  Throws EngineError on a CUDA error.
   std::vector<uint8_t> explain(const hs_rec128 *recs, size_t n) const {
@@ -340,6 +345,21 @@ class VerifyQueue {
     e_.check(hs_queue_sig_share_stats(q_, s.data()), "hs_queue_sig_share_stats");
     return s;
   }
+  // hs_queue_sig_audit: re-checks every held entry of buckets [first_bucket, first_bucket + n_buckets) (0: to the end) from its bytes and
+  // corrects the flag bytes that disagree.  [0] held, [1] corrected, [2] skipped, [3] first corrected position (UINT64_MAX: none),
+  // [4] its stored flags, [5] its derived flags, [6] its HS_WHY_* mask.  Throws EngineError when the cache is off or the range leaves it.
+  std::array<uint64_t, HS_QUEUE_SIG_AUDIT_OUT> sig_audit(size_t first_bucket = 0, size_t n_buckets = 0) {
+    std::array<uint64_t, HS_QUEUE_SIG_AUDIT_OUT> s{};
+    e_.check(hs_queue_sig_audit(q_, first_bucket, n_buckets, s.data()), "hs_queue_sig_audit");
+    return s;
+  }
+  // hs_queue_sig_audit_stats: [0] audits, [1] entries re-checked, [2] corrected, [3] skipped, [4] full passes of the table.
+  std::array<uint64_t, HS_QUEUE_SIG_AUDIT_STATS> sig_audit_stats() const {
+    std::array<uint64_t, HS_QUEUE_SIG_AUDIT_STATS> s{};
+    e_.check(hs_queue_sig_audit_stats(q_, s.data()), "hs_queue_sig_audit_stats");
+    return s;
+  }
+  hs_queue *raw() const { return q_; }
   // hs_queue_generic: verify requests with keys outside the committee on the GPU, not on the dispatcher thread (off by default;
   // off drains the generic launches in flight).  Verdicts do not change.
   void generic(bool on) { e_.check(hs_queue_generic(q_, on ? 1 : 0), "hs_queue_generic"); }
@@ -465,6 +485,10 @@ class VerifyQueue {
   const Engine &e_;
   hs_queue *q_ = nullptr;
 };
+
+inline void Engine::scrub_sig_cache(const VerifyQueue *q, uint32_t buckets_per_tick) const {
+  check(hs_scrub_sig_cache(ctx_, q ? q->raw() : nullptr, buckets_per_tick), "hs_scrub_sig_cache");
+}
 
 struct Digest {  // crypto/src/lib.rs:22
   std::array<uint8_t, 32> bytes{};

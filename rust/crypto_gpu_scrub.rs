@@ -39,18 +39,22 @@ fn map_of(expected: &[Option<[u8; 32]>]) -> (Vec<u8>, Vec<u32>) {
 }
 
 unsafe extern "C" fn on_finding(_user: *mut c_void, _found: u32, failed: u32, _first_slot: usize) {
-    // found alone: the engine repaired and re-proved what it found, and the caches of verified records were emptied
+    // found alone: the engine repaired and re-proved what it found, and the caches of verified records were emptied; a corrected
+    // signature-cache entry (HS_AUDIT_SIGCACHE) holds its re-checked flag byte and is never in failed
     if failed != 0 { DISABLED.store(true, Ordering::Release); }
 }
 
-/// Starts the scrub against the shim's map.  Call it once at start-up, after `register_committee` and `self_test`.
+/// Starts the scrub against the shim's map.  Call it once at start-up, after `register_committee` and `self_test`.  When the
+/// node-wide queue's signature cache is on, each tick also re-checks a slice of it (`sig_audit::attach`).
 pub fn start() -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let keys = KEYS.lock().unwrap();
     let (pks, live) = map_of(&keys);
     let rc = unsafe { hs_scrub_start(c, if keys.is_empty() { std::ptr::null() } else { pks.as_ptr() }, live.as_ptr(), keys.len(), SCRUB_PERIOD_US,
                                      SCRUB_SLOTS_PER_TICK, SCRUB_BASE_ENTRIES_PER_TICK, Some(on_finding), std::ptr::null_mut()) };
-    if rc == HS_OK { Ok(()) } else { Err(GpuError::Engine(last_error(c))) }
+    if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
+    super::sig_audit::attach();
+    Ok(())
 }
 
 /// Gives the scrub the map after a committee change (the shim calls it with KEYS held); until then the scrub pauses.

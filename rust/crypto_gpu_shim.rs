@@ -38,6 +38,10 @@ pub mod sig_cache;
 /// batch lane: the votes the queue verified in the Timeouts are hits there too.  Turned on with the cache (`sig_cache::enable`).
 #[path = "crypto_gpu_sig_share.rs"]
 pub mod sig_share;
+/// The audit of that cache (hs_queue_sig_audit): every held entry re-checked from its bytes and a wrong flag byte corrected, a slice
+/// per scrub tick (`sig_audit::attach`) and the whole table on an `engine_fault` (`sig_audit::audit_cache`).
+#[path = "crypto_gpu_sig_audit.rs"]
+pub mod sig_audit;
 /// The queue's generic-key device path (hs_queue_generic): a request with a key outside the registered committee is verified by a
 /// queue kernel instead of holding up the queue's thread.  Turned on when the node-wide queue is created (`queue::queue`).
 #[path = "crypto_gpu_generic_queue.rs"]
@@ -213,7 +217,7 @@ pub struct Explained { pub index: usize, pub why: u8, pub engine_fault: bool }
 /// Explains a rejected message: `recs` are its records, `modes` their verdict modes (HS_MODE_*) and `verdicts` the bits the engine
 /// returned for them.  Only the first rejected record is re-checked (hs_explain_rec128, a table-free re-check on the GPU), so a flood of
 /// junk signatures costs one extra record per rejected message, not one per signature.  On `engine_fault` the caller audits and repairs
-/// the tables (`audit_tables`) and answers that message on the dalek path.  None = no record was rejected, no GPU, or the re-check
+/// the tables (`audit_tables`), re-checks the signature cache (`sig_audit::audit_cache`) and answers that message on the dalek path.  None = no record was rejected, no GPU, or the re-check
 /// failed (keep the rejection).
 pub fn explain_rejected(recs: &[HsRec128], modes: &[u8], verdicts: &[bool]) -> Option<Explained> {
     let index = verdicts.iter().position(|ok| !ok)?;

@@ -8,6 +8,7 @@
 // cache on, the queue's kernels keep every record they accepted (signature, key bytes and Digest), so those votes are probes that
 // hit instead of verifies.  Verdicts are those of the queue without it.
 use std::os::raw::c_int;
+use std::sync::atomic::{AtomicBool, Ordering};
 use std::sync::Once;
 
 use super::queue::HsQueue;
@@ -24,16 +25,23 @@ extern "C" {
 }
 
 static ENABLE: Once = Once::new();
+static ON: AtomicBool = AtomicBool::new(false);
 
 /// Turns the cache on for the node-wide queue, once, and then shares it with the synchronous calls and the batch lane
-/// (`sig_share::enable`).  A failure leaves it off: every record is then verified, with the same verdicts.
+/// (`sig_share::enable`) and attaches it to the scrub (`sig_audit::attach`).  A failure leaves it off: every record is then verified,
+/// with the same verdicts.
 pub(crate) fn enable(q: *mut HsQueue) {
     ENABLE.call_once(|| {
         if unsafe { hs_queue_sig_cache(q, SIG_CACHE_ENTRIES) } == HS_OK {
             super::sig_share::enable(q);
+            ON.store(true, Ordering::Release);
+            super::sig_audit::attach();
         }
     });
 }
+
+/// Whether `enable` turned the cache on.
+pub(crate) fn is_on() -> bool { ON.load(Ordering::Acquire) }
 
 /// The cache's counters for the node's metrics: records probed, hits, inserts, inserts that evicted a live entry, entries held.
 /// None when there is no GPU queue.

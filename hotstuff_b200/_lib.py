@@ -91,6 +91,9 @@ SIGNATURES = {
     "hs_key_slots": (c_size_t, [c_void_p]),
     "hs_table_audit": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32)]),
     "hs_table_repair": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32), ctypes.POINTER(c_u32)]),
+    "hs_table_mend": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_u32), ctypes.POINTER(c_u32)]),
+    "hs_table_mend_stats": (c_int, [c_void_p, ctypes.POINTER(c_u64)]),
+    "hs_scrub_mend": (c_int, [c_void_p, c_int]),
     "hs_scrub_start": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_u32, c_u32, c_u32, c_void_p, c_void_p]),
     "hs_scrub_set_map": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t]),
     "hs_scrub_stop": (c_int, [c_void_p]),

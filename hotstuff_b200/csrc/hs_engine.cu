@@ -1271,11 +1271,24 @@ __global__ void __launch_bounds__(256) k_slot_audit(key_table T, const uint8_t *
 // audit keeps the code it had before the list).  Short blocks: the lowest-priority stream's blocks give way to verify launches at every
 // block boundary.
 #define HS_AUDIT_WARPS 4
-template <bool LISTED>
-__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, const uint32_t *__restrict__ slots,
-                                                                       size_t n_tables, size_t table_entries, int W, int n_windows,
-                                                                       const uint8_t *__restrict__ pks, const uint8_t *__restrict__ auditable,
-                                                                       audit_out O) {
+// The window findings of the mend's audits (hs_table_mend), by audit_mend_flags: bit base + t (n_windows + 1) + i for window i of table
+// t (its list position, slot or 0 for the base-point table), and bit base + t (n_windows + 1) + n_windows when its anchor failed.
+struct audit_wins {
+  uint32_t *bits;
+  uint64_t base;
+};
+__device__ __forceinline__ void audit_report_windows(const audit_wins &Wo, uint64_t t, uint32_t win, int n_windows, uint32_t f) {
+  const uint64_t row = Wo.base + t * (uint64_t)(n_windows + 1);
+  const auto set = [&](uint64_t b) { atomicOr(Wo.bits + (b >> 5), 1u << (b & 31)); };
+  if (f & 1u) set(row + win);
+  if (f & 2u) set(row + win - 1);
+  if (f & 4u) set(row + n_windows);
+}
+// The body of both table forms; WINDOWS also reports the windows to mend (the kernels without it keep the code they had before).
+template <bool LISTED, bool WINDOWS>
+__device__ __forceinline__ void table_audit_run(const ge_niels *__restrict__ tables, const uint32_t *__restrict__ slots, size_t n_tables,
+                                                size_t table_entries, int W, int n_windows, const uint8_t *__restrict__ pks,
+                                                const uint8_t *__restrict__ auditable, const audit_out &O, const audit_wins &Wo) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t H = (uint64_t)1 << (W - 1), runs = (H + 1 + 31) / 32;
   const uint64_t g = (uint64_t)blockIdx.x * HS_AUDIT_WARPS + (threadIdx.x >> 5);
@@ -1296,28 +1309,50 @@ __global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_ni
   }
   if (lane == 0 && m > 0) niels_load(prev, wt + m - 1);
   uint32_t ok = in ? audit_entry_local(e, prev, one, m) : 1u;
+  uint32_t edge = 1u;  // the anchor or link check, apart from ok in the WINDOWS form
   if (m == 1) {
     if (win == 0) {
       ge_ext P;
       audit_anchor_point(P, pks ? reinterpret_cast<const uint32_t *>(pks + s * 32) : nullptr);
-      ok &= audit_anchor(e, P);
+      if constexpr (WINDOWS) edge = audit_anchor(e, P);
+      else ok &= audit_anchor(e, P);
     } else {
       ge_niels last;
       niels_load(last, wt - comb_window_stride(W) + H);
-      ok &= audit_link(e, last);
+      if constexpr (WINDOWS) edge = audit_link(e, last);
+      else ok &= audit_link(e, last);
     }
   }
-  if (!ok) audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
+  if constexpr (WINDOWS) {
+    if (!(ok & edge)) audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
+    audit_report_windows(Wo, t, win, n_windows, audit_mend_flags(win, m, ok, edge));
+  } else if (!ok) {
+    audit_report(O, pks ? 2 + t : 0, pks ? HS_AUDIT_TABLE : HS_AUDIT_BASE, audit_key(pks ? t + 1 : 0, win + 1, m));
+  }
+}
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, const uint32_t *__restrict__ slots,
+                                                                       size_t n_tables, size_t table_entries, int W, int n_windows,
+                                                                       const uint8_t *__restrict__ pks, const uint8_t *__restrict__ auditable,
+                                                                       audit_out O) {
+  table_audit_run<LISTED, false>(tables, slots, n_tables, table_entries, W, n_windows, pks, auditable, O, audit_wins{});
+}
+// The same with the window findings (hs_table_mend's audits).
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, const uint32_t *__restrict__ slots,
+                                                                       size_t n_tables, size_t table_entries, int W, int n_windows,
+                                                                       const uint8_t *__restrict__ pks, const uint8_t *__restrict__ auditable,
+                                                                       audit_out O, audit_wins Wo) {
+  table_audit_run<LISTED, true>(tables, slots, n_tables, table_entries, W, n_windows, pks, auditable, O, Wo);
 }
 // The range form (hs_scrub_start): entries [first, first + count) of the base-point table, entry e being entry e % (2^(W-1) + 1) of
 // window e / (2^(W-1) + 1), the table's storage order.  Warp g takes the g-th run of 32 entries of one window from the run holding
 // `first`, with the checks above; a lane outside the range only feeds the shuffles.  An entry's checks read its own window and, for
 // entry 1, entry 2^(W-1) of the window before, so slices that together cover the table find exactly what the full audit finds, and
 // report it with the same key.  An overload of the unlisted form, so the two forms above keep their code.
-template <bool LISTED>
-__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, uint64_t first, uint64_t count,
-                                                                       int W, int n_windows, audit_out O) {
-  static_assert(!LISTED, "the range form covers the base-point table");
+template <bool WINDOWS>
+__device__ __forceinline__ void table_audit_range_run(const ge_niels *__restrict__ tables, uint64_t first, uint64_t count, int W, int n_windows,
+                                                      const audit_out &O, const audit_wins &Wo) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t H = (uint64_t)1 << (W - 1), stride = H + 1, runs = (H + 1 + 31) / 32;
   const uint64_t r = (first / stride) * runs + (first % stride) / 32 + (uint64_t)blockIdx.x * HS_AUDIT_WARPS + (threadIdx.x >> 5);
@@ -1338,18 +1373,70 @@ __global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_ni
   }
   if (lane == 0 && m > 0) niels_load(prev, wt + m - 1);
   uint32_t ok = in ? audit_entry_local(e, prev, one, m) : 1u;
+  uint32_t edge = 1u;  // the anchor or link check, apart from ok in the WINDOWS form
   if (in && m == 1) {
     if (win == 0) {
       ge_ext P;
       audit_anchor_point(P, nullptr);
-      ok &= audit_anchor(e, P);
+      if constexpr (WINDOWS) edge = audit_anchor(e, P);
+      else ok &= audit_anchor(e, P);
     } else {
       ge_niels last;
       niels_load(last, wt - stride + H);
-      ok &= audit_link(e, last);
+      if constexpr (WINDOWS) edge = audit_link(e, last);
+      else ok &= audit_link(e, last);
     }
   }
-  if (!ok) audit_report(O, 0, HS_AUDIT_BASE, audit_key(0, (uint32_t)win + 1, m));
+  if constexpr (WINDOWS) {
+    if (!(ok & edge)) audit_report(O, 0, HS_AUDIT_BASE, audit_key(0, (uint32_t)win + 1, m));
+    audit_report_windows(Wo, 0, (uint32_t)win, n_windows, audit_mend_flags((uint32_t)win, m, ok, edge));
+  } else if (!ok) {
+    audit_report(O, 0, HS_AUDIT_BASE, audit_key(0, (uint32_t)win + 1, m));
+  }
+}
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, uint64_t first, uint64_t count,
+                                                                       int W, int n_windows, audit_out O) {
+  static_assert(!LISTED, "the range form covers the base-point table");
+  table_audit_range_run<false>(tables, first, count, W, n_windows, O, audit_wins{});
+}
+template <bool LISTED>
+__global__ void __launch_bounds__(32 * HS_AUDIT_WARPS) k_table_audit(const ge_niels *__restrict__ tables, uint64_t first, uint64_t count,
+                                                                       int W, int n_windows, audit_out O, audit_wins Wo) {
+  static_assert(!LISTED, "the range form covers the base-point table");
+  table_audit_range_run<true>(tables, first, count, W, n_windows, O, Wo);
+}
+
+// ------------------------------------------------------------------------------------------------ mend (hs_table_mend)
+// A work item: window `win` of the base-point table (slot == HS_MEND_BASE) or of slot `slot`'s comb table.
+#define HS_MEND_BASE 0xffffffffu
+struct mend_item {
+  uint32_t slot, win;
+};
+// thread = (item, block b of HS_BUILD_BLOCK entries of its window), blocks [first_block, first_block + n_blocks) of the launch's items
+// in (item, b) order.  Each thread builds its block into its own HS_BUILD_BLOCK + 1 entries of `stage` (comb_mend_block: the arithmetic
+// of k_build_comb, P = -A from the slot's stored key bytes or B) and stores the entries that differ from the live table.  rewritten:
+// the entries stored, reduced per warp.  A key that does not decompress has no table to mend (the audit does not check it either).
+__global__ void __launch_bounds__(HS_THREADS) k_mend_windows(const mend_item *__restrict__ items, uint64_t first_block, uint64_t n_blocks, int W,
+                                                             ge_niels *tables, size_t table_entries, const uint8_t *__restrict__ pks,
+                                                             ge_niels *stage, unsigned long long *rewritten) {
+  const uint64_t t = (uint64_t)blockIdx.x * HS_THREADS + threadIdx.x;
+  const uint64_t blocks_per_window = ((uint64_t)1 << (W - 1)) / HS_BUILD_BLOCK;
+  uint32_t stored = 0;
+  if (t < n_blocks) {
+    const uint64_t g = first_block + t;
+    const mend_item it = items[g / blocks_per_window];
+    const int b = (int)(g % blocks_per_window);
+    const bool base = it.slot == HS_MEND_BASE;
+    ge_ext P;
+    if (audit_anchor_point(P, base ? nullptr : reinterpret_cast<const uint32_t *>(pks + 32 * (size_t)it.slot))) {
+      ge_niels *window = tables + (base ? 0 : it.slot * table_entries) + (size_t)it.win * comb_window_stride(W);
+      fe prod[HS_BUILD_BLOCK];
+      stored = comb_mend_block(window, stage + t * (HS_BUILD_BLOCK + 1), P, W, (int)it.win, b * HS_BUILD_BLOCK, HS_BUILD_BLOCK, prod);
+    }
+  }
+  stored = __reduce_add_sync(0xffffffffu, stored);
+  if ((threadIdx.x & 31) == 0 && stored) atomicAdd(rewritten, (unsigned long long)stored);
 }
 
 // ------------------------------------------------------------------------------------------------ explanation of a verdict
@@ -1775,6 +1862,7 @@ struct audit_state {
   stream_h stream;
   event_h done;
   dev_buf scratch;
+  dev_buf stage;  // hs_table_mend's staging: HS_BUILD_BLOCK + 1 entries per thread of one k_mend_windows launch
 };
 // A ring of slots that k_verify_small, k_verify_bulk, k_queue_generic and k_queue_digests work over (slot = position & mask): the
 // latency path's (one request in slot 0), a verify queue's and the self-test's.
@@ -1813,6 +1901,8 @@ struct committee_stage {
 };
 // The engine-owned scrub (hs_scrub_start): its thread, the map it audits against and where its pass stands.  `m` guards all but `th`
 // (hs_scrub_start / hs_scrub_stop, under hs_ctx::scrub_life) and the counters (read at any time).  Lock order: m, audit_mu, mu.
+// hs_table_mend_stats: calls, windows recomputed, entries rewritten, windows left, slots left to repair, cache flushes
+enum { MEND_CALLS, MEND_WINDOWS, MEND_REWRITTEN, MEND_WINDOWS_LEFT, MEND_SLOTS_LEFT, MEND_FLUSHES, MEND_NSTATS };
 enum { SCRUB_PASSES, SCRUB_SLOTS, SCRUB_BASE, SCRUB_TICKS, SCRUB_FINDINGS, SCRUB_REPAIRED, SCRUB_FAILED, SCRUB_PAUSED, SCRUB_NSTATS };
 struct scrub_state {
   std::thread th;
@@ -1827,6 +1917,7 @@ struct scrub_state {
   size_t n_slots = 0;
   uint64_t map_gen = 0;
   uint32_t period_us = 0, slots_per_tick = 0, base_per_tick = 0;
+  bool mend = false;                // hs_scrub_mend: a tick whose findings can all be mended mends them instead of repairing
   hs_scrub_cb *cb = nullptr;
   void *user = nullptr;
   size_t next_slot = 0;             // the pass: the slots before next_slot and the base entries before next_base are audited
@@ -1881,6 +1972,7 @@ struct hs_ctx {
   uint64_t map_gen = 0;
   std::mutex audit_mu;               // one hs_table_audit at a time: it owns `audit` for the whole call, `mu` only briefly
   audit_state audit;
+  std::atomic<uint64_t> mend_stats[MEND_NSTATS] = {};  // hs_table_mend_stats (the scrub's mends included)
   std::mutex scrub_life;             // hs_scrub_start / hs_scrub_stop: starting and joining the scrub's thread
   scrub_state scrub;
   // multi-GPU peer routing
@@ -5360,7 +5452,7 @@ struct base_range {
 // list position), or with `range` that range of the base-point table.  auditable: nullable for the base-point table.
 static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *tables, const uint32_t *d_slots, size_t n_tables, size_t entries,
                               int W, int n_windows, const uint8_t *pks, const uint8_t *auditable, const audit_out &O,
-                              const base_range *range = nullptr) {
+                              const base_range *range = nullptr, const audit_wins *wins = nullptr) {
   const uint64_t stride = comb_window_stride(W), runs = (stride + 31) / 32;
   const auto run_of = [&](uint64_t e) { return e / stride * runs + e % stride / 32; };
   const uint64_t warps = range ? run_of(range->first + range->count - 1) - run_of(range->first) + 1 : (uint64_t)n_tables * n_windows * runs;
@@ -5368,7 +5460,11 @@ static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *ta
   const auto launch = [&](auto listed, auto... args) {
     k_table_audit<decltype(listed)::value><<<blocks, 32 * HS_AUDIT_WARPS, 0, stream>>>(tables, args...);
   };
-  if (range) launch(std::false_type{}, range->first, range->count, W, n_windows, O);
+  if (wins) {  // the same forms with the window findings (hs_table_mend)
+    if (range) launch(std::false_type{}, range->first, range->count, W, n_windows, O, *wins);
+    else if (d_slots) launch(std::true_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O, *wins);
+    else launch(std::false_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O, *wins);
+  } else if (range) launch(std::false_type{}, range->first, range->count, W, n_windows, O);
   else if (d_slots) launch(std::true_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
   else launch(std::false_type{}, d_slots, n_tables, entries, W, n_windows, pks, auditable, O);
   c->launches++;
@@ -5393,7 +5489,11 @@ struct audit_run {
   uint64_t gen = 0;              // key_gen when the kernels were enqueued
   size_t n_slots = 0;
   const uint8_t *d_res = nullptr;
-  std::vector<uint8_t> res;      // the first finding's audit_key() (8 bytes), then bits[2 + n_slots]
+  std::vector<uint8_t> res;      // the first finding's audit_key() (8 bytes), then bits[2 + n_slots], then the window findings
+  // With the window findings (hs_table_mend's audits): the audit_wins bits of the key tables from bit 0 (table t's row at t (na + 1)),
+  // those of the base-point table from word base_word (row 0, nb + 1 bits).  win_words == 0: none.
+  int na = 0, nb = 0;
+  size_t base_word = 0, win_words = 0;
   uint64_t first() const {
     uint64_t f;
     memcpy(&f, res.data(), 8);
@@ -5405,6 +5505,18 @@ struct audit_run {
     for (size_t s = 0; s < n_slots; s++) f |= bits()[2 + s];
     return f;
   }
+  uint32_t *wins() { return reinterpret_cast<uint32_t *>(res.data() + 8) + 2 + n_slots; }
+  const uint32_t *wins() const { return bits() + 2 + n_slots; }
+  bool win_bit(uint64_t b) const { return (wins()[b >> 5] >> (b & 31)) & 1u; }
+  bool key_win(size_t t, int i) const { return win_bit((uint64_t)t * (na + 1) + i); }  // i == na: the anchor failed
+  bool base_win(int i) const { return win_bit(32 * (uint64_t)base_word + i); }
+  // Sizes the window findings for n_keys key tables and the base-point table at c's geometry.
+  void size_windows(const comb_params &cp, size_t n_keys) {
+    na = cp.na;
+    nb = cp.nb;
+    base_word = (n_keys * (size_t)(na + 1) + 31) / 32;
+    win_words = base_word + (nb + 1 + 31) / 32;
+  }
 };
 // Part of an audit (a scrub tick): the KEY / FLAG / LOOKUP checks of every slot and hash entry as the complete audit runs them (a
 // thread each), the comb tables of the slots in `tables` only, and entries [base_first, base_first + base_count) of the base-point table.
@@ -5415,8 +5527,9 @@ struct audit_slice {
 };
 // Checks the arguments, snapshots the slots and their liveness, uploads and enqueues: the complete audit, or with `slice` that part.
 // Nothing here waits for a kernel.
+// windows: the WINDOWS forms, with the window findings in r (hs_table_mend and a scrub that mends).
 static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots,
-                                audit_run &r, const audit_slice *slice = nullptr) {
+                                audit_run &r, const audit_slice *slice = nullptr, bool windows = false) {
   audit_state &A = c->audit;
   HS_CUDA(c, cudaSetDevice(c->device));
   const size_t n = has_key_tables(c) ? c->n_keys : 0;
@@ -5426,7 +5539,10 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
   std::vector<uint8_t> live(n, 1);  // a staged slot is not in service
   if (c->explicit_committee)
     std::transform(c->h_key_live.begin(), c->h_key_live.begin() + n, live.begin(), [](uint8_t v) { return v == SLOT_STAGED ? 0 : v; });
-  const size_t res_bytes = 8 + 4 * (2 + n);
+  r = audit_run{};
+  r.n_slots = n;
+  if (windows) r.size_windows(c->cp, n);
+  const size_t res_bytes = 8 + 4 * (2 + n + r.win_words);
   h2d_stage in;
   const size_t s_res = in.add(nullptr, res_bytes), s_pks = in.add(expect_pks, expect_pks ? n * 32 : 0),
                s_live = in.add(expect_live, expect_live ? 4 * ((n + 31) / 32) : 0), s_mirror = in.add(live.data(), n),
@@ -5436,6 +5552,9 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
   HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
   HS_CUDA(c, cudaMemsetAsync(res + 8, 0, res_bytes - 8, A.stream));
   const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
+  uint32_t *const wbits = reinterpret_cast<uint32_t *>(res + 8) + 2 + n;
+  const audit_wins key_wins{wbits, 0}, base_wins{wbits + r.base_word, 0};
+  const auto kw = [&](size_t b) { return audit_wins{wbits, b * (size_t)(c->cp.na + 1)}; };
   if (n) {
     const key_table T = ctx_tables(c).T;
     k_slot_audit<<<blocks_for(n + (size_t)T.mask + 1, 256), 256, 0, A.stream>>>(
@@ -5444,21 +5563,25 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
     c->launches++;
     HS_CUDA(c, cudaGetLastError());
     if (!slice)
-      HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O));
+      HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O,
+                                nullptr, windows ? &key_wins : nullptr));
     for (const auto &[b, e] : slice ? slice->tables : std::vector<std::pair<size_t, size_t>>{})  // a run: the same form on that window of the arrays
-      if (b < e && e <= n)
+      if (b < e && e <= n) {
+        const audit_wins w = kw(b);
         HS_TRY(launch_table_audit(c, A.stream, c->keys.atables + b * c->a_table_entries, nullptr, e - b, c->a_table_entries, c->cp.wa, c->cp.na,
-                                  c->keys.pks + 32 * b, in.ptr(s_ok) + b, audit_out{O.first, O.bits + b}));
+                                  c->keys.pks + 32 * b, in.ptr(s_ok) + b, audit_out{O.first, O.bits + b}, nullptr, windows ? &w : nullptr));
+      }
   }
   if (!slice) {
-    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O));
+    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O,
+                              nullptr, windows ? &base_wins : nullptr));
   } else if (slice->base_count) {
     const base_range R{slice->base_first, slice->base_count};
-    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O, &R));
+    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, comb_table_entries(c->cp.wb), c->cp.wb, c->cp.nb, nullptr, nullptr, O, &R,
+                              windows ? &base_wins : nullptr));
   }
   HS_CUDA(c, cudaEventRecord(A.done, A.stream));
   r.gen = c->key_gen;
-  r.n_slots = n;
   r.d_res = res;
   r.res.resize(res_bytes);
   return HS_OK;
@@ -5634,6 +5757,193 @@ extern "C" int hs_table_repair(hs_ctx *c, const uint8_t *expect_pks, const uint3
   *out_found = found;
   *out_failed = failed;
   return failed ? fail(c, HS_ERR_SELFTEST, audit_message(last.first(), n_slots, last.bits()).c_str()) : HS_OK;
+}
+
+// ---- mend of what the audit finds, in place and with no drain (hs_table_mend, and the scrub with hs_scrub_mend)
+// What the mend takes of audit r (run with its window findings): every flagged window of the base-point table, whose anchor B is a
+// constant; and the flagged windows of each slot whose only finding is TABLE, unless its anchor failed with no map (have_map) to
+// confirm its key bytes: bytes that changed but still decompress look exactly like a bad anchor, and a table rebuilt from them would
+// hold the wrong key's multiples.  Everything else is left to hs_table_repair.
+struct mend_plan {
+  std::vector<mend_item> base, keys;  // the windows to recompute
+  std::vector<uint32_t> slots;        // the slots of `keys`, in slot order
+  uint32_t left = 0;                  // the HS_AUDIT_* classes left
+  uint64_t windows_left = 0, slots_left = 0;
+};
+static mend_plan mend_plan_of(const audit_run &r, bool have_map) {
+  mend_plan P;
+  const uint32_t *bits = r.bits();
+  if (bits[0]) {
+    for (int i = 0; i < r.nb; i++)
+      if (r.base_win(i)) P.base.push_back({HS_MEND_BASE, (uint32_t)i});
+    if (P.base.empty()) P.left |= HS_AUDIT_BASE;
+  }
+  P.left |= bits[1];
+  for (size_t s = 0; s < r.n_slots; s++) {
+    if (!bits[2 + s]) continue;
+    const size_t before = P.keys.size();
+    if (bits[2 + s] == HS_AUDIT_TABLE && (have_map || !r.key_win(s, r.na)))
+      for (int i = 0; i < r.na; i++)
+        if (r.key_win(s, i)) P.keys.push_back({(uint32_t)s, (uint32_t)i});
+    if (P.keys.size() > before) {
+      P.slots.push_back((uint32_t)s);
+      continue;
+    }
+    P.left |= bits[2 + s];
+    P.slots_left++;
+    for (int i = 0; i < r.na; i++) P.windows_left += r.key_win(s, i) ? 1 : 0;
+  }
+  return P;
+}
+// Threads of one k_mend_windows launch: a wave of the device at 256 threads per SM, so its staging (6,240 bytes a thread: 211 MB on
+// 132 SMs) stays bounded whatever the window; a 24-bit base window (2^23 entries, 131,072 threads) takes four launches.
+static size_t mend_chunk(const hs_ctx *c) { return (size_t)c->n_sms * 256; }
+// One mend of plan P: enqueued under c->mu by mend_enqueue_locked, waited for and read back without it by mend_collect.  The proof
+// audits each mended window again: the base-point table's by the range form over the window and the next (whose entry 1 links to
+// it), the slots' by the listed form over their whole tables.  The caller holds audit_mu.
+struct mend_run {
+  const uint8_t *d_out = nullptr;  // entries rewritten (8 bytes), then the proof's results
+  std::vector<uint8_t> h;
+  audit_run proof;                 // its slot t is P.slots[t]
+  uint64_t rewritten() const {
+    uint64_t v;
+    memcpy(&v, h.data(), 8);
+    return v;
+  }
+};
+static int mend_enqueue_locked(hs_ctx *c, const char *entry, const char *changed, const audit_run &first, const mend_plan &P, mend_run &M) {
+  audit_state &A = c->audit;
+  // The last check before the stores: a registration, update, commit or key-cache change since the audit leaves nothing stored.  Any
+  // later one waits for A.done (audit_fence, or a drained device) before it writes, so it lands after these stores.
+  if (c->key_gen != first.gen) return fail_args(c, entry, changed);
+  HS_CUDA(c, cudaSetDevice(c->device));
+  const size_t k = P.slots.size();
+  M.proof.n_slots = k;
+  M.proof.size_windows(c->cp, k);
+  const size_t proof_bytes = 8 + 4 * (2 + k + M.proof.win_words);
+  std::vector<mend_item> items(P.base);
+  items.insert(items.end(), P.keys.begin(), P.keys.end());
+  const std::vector<uint8_t> ones(k, 1);
+  h2d_stage st;
+  const size_t s_items = st.add(items.data(), items.size() * sizeof(mend_item)), s_slots = st.add(P.slots.data(), 4 * k),
+               s_ok = st.add(ones.data(), k), s_out = st.add(nullptr, 8 + proof_bytes);
+  HS_TRY(st.upload(c, A.scratch, A.stream));
+  uint8_t *out = st.ptr(s_out), *res = out + 8;
+  HS_CUDA(c, cudaMemsetAsync(out, 0, 8 + proof_bytes, A.stream));
+  HS_CUDA(c, cudaMemsetAsync(res, 0xff, 8, A.stream));
+  unsigned long long *rewritten = reinterpret_cast<unsigned long long *>(out);
+  const mend_item *d_items = reinterpret_cast<const mend_item *>(st.ptr(s_items));
+  const size_t chunk = mend_chunk(c);
+  const auto mend = [&](const mend_item *its, size_t n_items, int W, ge_niels *tables, size_t table_entries, const uint8_t *pks) -> int {
+    const uint64_t total = (uint64_t)n_items * (((uint64_t)1 << (W - 1)) / HS_BUILD_BLOCK);
+    for (uint64_t b = 0; b < total; b += chunk) {
+      const uint64_t nb = std::min<uint64_t>(chunk, total - b);
+      k_mend_windows<<<blocks_for(nb), HS_THREADS, 0, A.stream>>>(its, b, nb, W, tables, table_entries, pks,
+                                                                  static_cast<ge_niels *>(A.stage.p.get()), rewritten);
+      c->launches++;
+      HS_CUDA(c, cudaGetLastError());
+    }
+    return HS_OK;
+  };
+  if (!P.base.empty()) HS_TRY(mend(d_items, P.base.size(), c->cp.wb, c->d_btable, 0, nullptr));
+  if (k) HS_TRY(mend(d_items + P.base.size(), P.keys.size(), c->cp.wa, c->keys.atables, c->a_table_entries, c->keys.pks));
+  const audit_out O{reinterpret_cast<unsigned long long *>(res), reinterpret_cast<uint32_t *>(res + 8)};
+  uint32_t *const wbits = reinterpret_cast<uint32_t *>(res + 8) + 2 + k;
+  const uint64_t E = comb_table_entries(c->cp.wb), stride = comb_window_stride(c->cp.wb);
+  const audit_wins base_wins{wbits + M.proof.base_word, 0}, key_wins{wbits, 0};
+  for (size_t j = 0; j < P.base.size();) {  // runs of consecutive windows, each with the window after it
+    size_t e = j + 1;
+    while (e < P.base.size() && P.base[e].win == P.base[e - 1].win + 1) e++;
+    const uint64_t from = P.base[j].win * stride;
+    const base_range R{from, std::min<uint64_t>(E, (P.base[e - 1].win + 2) * stride) - from};
+    HS_TRY(launch_table_audit(c, A.stream, c->d_btable, nullptr, 1, E, c->cp.wb, c->cp.nb, nullptr, nullptr, O, &R, &base_wins));
+    j = e;
+  }
+  if (k)
+    HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, reinterpret_cast<const uint32_t *>(st.ptr(s_slots)), k, c->a_table_entries, c->cp.wa,
+                              c->cp.na, c->keys.pks, st.ptr(s_ok), O, nullptr, &key_wins));
+  HS_CUDA(c, cudaEventRecord(A.done, A.stream));  // registration, updates and the key-cache paths wait for it before they rewrite
+  M.d_out = out;
+  M.h.resize(8 + proof_bytes);
+  return HS_OK;
+}
+static int mend_collect(hs_ctx *c, mend_run &M) {
+  audit_state &A = c->audit;
+  HS_CUDA(c, cudaEventSynchronize(A.done));
+  HS_CUDA(c, cudaMemcpyAsync(M.h.data(), M.d_out, M.h.size(), cudaMemcpyDeviceToHost, A.stream));
+  HS_CUDA(c, cudaStreamSynchronize(A.stream));
+  M.proof.res.assign(M.h.begin() + 8, M.h.end());
+  return HS_OK;
+}
+// Mends what audit `first` found (run with its window findings) and proves it; *left: the classes left (not mendable, or still failing
+// the proof).  Never drains the device and never changes a slot's service state: the context's mutex is held to enqueue and, when an
+// entry was rewritten, to empty every verify queue's caches as a repair does (a record may have been decided against the wrong entry).
+// The caller holds audit_mu.
+static int mend_found(hs_ctx *c, const char *entry, const char *changed, const audit_run &first, bool have_map, uint32_t &left) {
+  c->mend_stats[MEND_CALLS]++;
+  const mend_plan P = mend_plan_of(first, have_map);
+  left = P.left;
+  uint64_t windows_left = P.windows_left, slots_left = P.slots_left;
+  const size_t windows = P.base.size() + P.keys.size();
+  if (windows) {
+    const uint64_t threads = std::max<uint64_t>(P.base.empty() ? 0 : ((uint64_t)1 << (c->cp.wb - 1)) / HS_BUILD_BLOCK,
+                                                P.keys.empty() ? 0 : ((uint64_t)1 << (c->cp.wa - 1)) / HS_BUILD_BLOCK);
+    HS_TRY(ensure(c, c->audit.stage, std::min<uint64_t>(mend_chunk(c), threads * windows) * (HS_BUILD_BLOCK + 1) * sizeof(ge_niels)));
+    mend_run M;
+    {
+      std::lock_guard<std::mutex> g(c->mu);
+      HS_TRY(mend_enqueue_locked(c, entry, changed, first, P, M));
+    }
+    HS_TRY(mend_collect(c, M));
+    const audit_run &pr = M.proof;
+    if (pr.bits()[0]) {
+      left |= HS_AUDIT_BASE;
+      for (int i = 0; i < pr.nb; i++) windows_left += pr.base_win(i) ? 1 : 0;
+    }
+    for (size_t t = 0; t < pr.n_slots; t++) {
+      if (!pr.bits()[2 + t]) continue;
+      left |= pr.bits()[2 + t];
+      slots_left++;
+      for (int i = 0; i < pr.na; i++) windows_left += pr.key_win(t, i) ? 1 : 0;
+    }
+    const uint64_t rewritten = M.rewritten();
+    c->mend_stats[MEND_WINDOWS] += windows;
+    c->mend_stats[MEND_REWRITTEN] += rewritten;
+    if (rewritten) {
+      std::lock_guard<std::mutex> g(c->mu);
+      HS_TRY(flush_queue_caches(c));
+      c->mend_stats[MEND_FLUSHES]++;
+    }
+  }
+  c->mend_stats[MEND_WINDOWS_LEFT] += windows_left;
+  c->mend_stats[MEND_SLOTS_LEFT] += slots_left;
+  return HS_OK;
+}
+
+extern "C" int hs_table_mend(hs_ctx *c, const uint8_t *expect_pks, const uint32_t *expect_live, size_t n_slots, uint8_t *out_slot_bits,
+                             uint32_t *out_found, uint32_t *out_left) {
+  if (!c || !out_found || !out_left) return fail(c, HS_ERR_ARG, "hs_table_mend: bad argument");
+  const char *entry = "hs_table_mend", *changed = "key tables changed during the mend; run it again";
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  audit_run first;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    HS_TRY(audit_enqueue_locked(c, entry, expect_pks, expect_live, n_slots, first, nullptr, true));
+  }
+  HS_TRY(audit_collect(c, entry, changed, first));
+  uint32_t left = 0;
+  HS_TRY(mend_found(c, entry, changed, first, expect_pks != nullptr, left));
+  for (size_t s = 0; s < n_slots && out_slot_bits; s++) out_slot_bits[s] = (uint8_t)first.bits()[2 + s];
+  *out_found = first.failed();
+  *out_left = left;
+  if (!left) return HS_OK;
+  return fail(c, HS_ERR_SELFTEST, ("hs_table_mend: findings of HS_AUDIT_* classes " + std::to_string(left) + " left to hs_table_repair").c_str());
+}
+
+extern "C" int hs_table_mend_stats(hs_ctx *c, uint64_t out[HS_MEND_STATS]) {
+  if (!c || !out) return HS_ERR_ARG;
+  for (int k = 0; k < MEND_NSTATS; k++) out[k] = c->mend_stats[k].load();
+  return HS_OK;
 }
 
 // ---- staged committee change (hs_committee_stage / hs_committee_commit / hs_committee_discard)
@@ -5865,7 +6175,7 @@ static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
     sl.tables.push_back({S.next_slot, s});
     sl.base_first = S.next_base;
     sl.base_count = std::min<uint64_t>(S.base_per_tick, E - S.next_base);
-    HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, r, &sl));
+    HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, r, &sl, S.mend));
   }
   int rc = audit_collect(c, entry, changed, r);
   if (rc == HS_ERR_ARG) {  // the slot map changed under the tick: nothing it found counts, and the next tick pauses
@@ -5893,7 +6203,7 @@ static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
     st.tables = outside;
     {
       std::lock_guard<std::mutex> g(c->mu);
-      HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, t, &st));
+      HS_TRY(audit_enqueue_locked(c, entry, pks, live, S.n_slots, t, &st, S.mend));
     }
     rc = audit_collect(c, entry, changed, t);
     if (rc == HS_ERR_ARG) {
@@ -5903,15 +6213,20 @@ static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
     HS_TRY(rc);
     uint32_t *bits = reinterpret_cast<uint32_t *>(r.res.data() + 8);
     for (size_t k = 0; k < 2 + r.n_slots; k++) bits[k] |= t.bits()[k];
+    for (size_t k = 0; k < r.win_words; k++) r.wins()[k] |= t.wins()[k];
     sl.tables.insert(sl.tables.end(), outside.begin(), outside.end());
   }
   rep.found = r.failed();
   for (size_t k = 0; k < r.n_slots && rep.first_slot == SIZE_MAX; k++)
     if (r.bits()[2 + k]) rep.first_slot = k;
+  // With hs_scrub_mend, findings that can all be mended are mended (no drain, no slot out of service); anything else is repaired.
+  const bool mend = S.mend && !mend_plan_of(r, pks != nullptr).left;
+  uint32_t left = 0;
+  if (mend) rc = mend_found(c, entry, changed, r, pks != nullptr, left);
   audit_run last;
   {
     std::unique_lock<std::mutex> g(c->mu);
-    rc = repair_locked(c, g, r, pks, live, changed);
+    if (!mend) rc = repair_locked(c, g, r, pks, live, changed);
     if (rc == HS_OK) rc = audit_enqueue_locked(c, entry, pks, live, S.n_slots, last, &sl);
   }
   if (rc == HS_OK) rc = audit_collect(c, entry, changed, last);
@@ -5921,7 +6236,7 @@ static int scrub_tick(hs_ctx *c, scrub_state &S, scrub_report &rep) {
   rep.failed = after.failed();
   S.stats[SCRUB_FINDINGS] += scrub_items(r);
   S.stats[SCRUB_FAILED] += scrub_items(after);
-  for (size_t k = 0; k < r.n_slots; k++) S.stats[SCRUB_REPAIRED] += (r.bits()[2 + k] && !after.bits()[2 + k]) ? 1 : 0;
+  for (size_t k = 0; k < r.n_slots && !mend; k++) S.stats[SCRUB_REPAIRED] += (r.bits()[2 + k] && !after.bits()[2 + k]) ? 1 : 0;
   return HS_OK;
 }
 // The signature-cache slice of a tick, under S.m and whether or not the slot map is paused: the next sig_per_tick buckets of the attached
@@ -6026,6 +6341,13 @@ extern "C" int hs_scrub_sig_cache(hs_ctx *c, hs_queue *q, uint32_t buckets_per_t
   S.sig_per_tick = buckets_per_tick;
   S.sig_gen = 0;
   S.sig_next = 0;
+  return HS_OK;
+}
+
+extern "C" int hs_scrub_mend(hs_ctx *c, int on) {
+  if (!c) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> l(c->scrub.m);  // between ticks
+  c->scrub.mend = on != 0;
   return HS_OK;
 }
 

@@ -387,6 +387,45 @@ HS_HD void comb_build_block(ge_niels *table, const ge_ext &P, int W, int win, in
   }
 }
 
+// ---- mend (hs_table_mend): the entries comb_build_block writes for (win, first, count), built into `stage` (count + 1 entries of
+// scratch; stage[0] stands for entry `first`) and never into the table, then compared with the live entries of `window` (entry 0 of
+// that window of the table): only an entry whose 96 bytes differ is stored, once, with its final affine bytes.  A correct entry is
+// never written, so a gather that runs beside the mend reads a changed value only where the table was already wrong.  Returns the
+// entries stored.
+HS_HD uint32_t niels_store_if_differs(ge_niels *dst, const ge_niels &v) {
+#if defined(__CUDA_ARCH__)
+  uint4 *d = reinterpret_cast<uint4 *>(dst);
+  const uint4 w[6] = {make_uint4(v.ypx.v[0], v.ypx.v[1], v.ypx.v[2], v.ypx.v[3]),     make_uint4(v.ypx.v[4], v.ypx.v[5], v.ypx.v[6], v.ypx.v[7]),
+                      make_uint4(v.ymx.v[0], v.ymx.v[1], v.ymx.v[2], v.ymx.v[3]),     make_uint4(v.ymx.v[4], v.ymx.v[5], v.ymx.v[6], v.ymx.v[7]),
+                      make_uint4(v.xy2d.v[0], v.xy2d.v[1], v.xy2d.v[2], v.xy2d.v[3]), make_uint4(v.xy2d.v[4], v.xy2d.v[5], v.xy2d.v[6], v.xy2d.v[7])};
+  uint32_t diff = 0;
+#pragma unroll
+  for (int j = 0; j < 6; j++) {
+    const uint4 a = __ldcg(d + j);  // L2: the current bytes, never a stale L1 line
+    diff |= (a.x ^ w[j].x) | (a.y ^ w[j].y) | (a.z ^ w[j].z) | (a.w ^ w[j].w);
+  }
+  if (!diff) return 0;
+#pragma unroll
+  for (int j = 0; j < 6; j++) d[j] = w[j];
+  return 1;
+#else
+  if (!memcmp(dst, &v, sizeof(ge_niels))) return 0;
+  memcpy(dst, &v, sizeof(ge_niels));
+  return 1;
+#endif
+}
+HS_HD uint32_t comb_mend_block(ge_niels *window, ge_niels *stage, const ge_ext &P, int W, int win, int first, int count, fe *prod) {
+  // comb_build_block addresses the block from a table's start: given the stage's address less the block's offset in a table, it writes
+  // entries first .. first + count to stage[0 ..], and k_build_comb keeps its code.
+  comb_build_block(stage - (size_t)win * comb_window_stride(W) - first, P, W, win, first, count, prod);
+  uint32_t stored = 0;
+#if defined(__CUDA_ARCH__)
+#pragma unroll 1
+#endif
+  for (int c = first ? 1 : 0; c <= count; c++) stored += niels_store_if_differs(window + first + c, stage[c]);
+  return stored;
+}
+
 // ---- table audit (hs_table_audit): every entry of a built comb table checked against the layout above with the curve arithmetic the
 // verify paths use, never with comb_build_block.  An entry passes when it is canonical, its third coordinate is 2dxy of the first two,
 // and it is the previous entry of its window plus entry 1; entry 0 must be the identity, entry 1 of window 0 the table's point, and entry
@@ -470,6 +509,16 @@ HS_HD uint32_t audit_anchor(const ge_niels &one, const ge_ext &P) { return audit
 // The first finding of an audit, as one 64-bit key whose minimum is the first in (slot, window, entry) order: code 0 = the base table,
 // s + 1 = key slot s; window field 0 = a finding about the slot itself (key bytes, flag, lookup), i + 1 = window i of its table.
 HS_HD uint64_t audit_key(uint64_t code, uint32_t wfield, uint32_t entry) { return (code << 32) | ((uint64_t)wfield << 26) | entry; }
+// The windows a finding at entry m of window win puts up for the mend (hs_table_mend), from its local checks (audit_entry_local) and
+// its edge check (the anchor for window 0, the link otherwise; 1 for m != 1).  Bit 0: its own window, which holds every entry whose
+// local check can fail.  Bit 1: the window before, as well, for a failed link: its entry 2^(w-1) may be the wrong one.  Bit 2: the
+// anchor failed (window 0 is flagged too): the slot's key bytes may have changed instead, so only a map that confirms them lets it be
+// mended.  A flagged window that is correct costs its recomputation and nothing else: the mend writes no correct entry.
+HS_HD uint32_t audit_mend_flags(uint32_t win, uint32_t m, uint32_t local_ok, uint32_t edge_ok) {
+  uint32_t f = (local_ok && edge_ok) ? 0u : 1u;
+  if (m == 1 && !edge_ok) f |= win ? 2u : 4u;
+  return f;
+}
 
 // ---- explanation of a verdict (hs_explain_rec128): every check of the decision procedure above as its own HS_WHY_* bit, evaluated
 // independently (no "first failure"), with no table of any kind and without the fast paths' shortcuts: [S]B and [k](-A) both by the

@@ -162,6 +162,36 @@ class Engine:
             self._check(rc, "hs_table_repair")
         return int(found.value), int(failed.value), bits[:n]
 
+    def table_mend(self, expect=None, live=None):
+        """Mend of corrupt comb-table entries in place (hs_table_mend): recomputes the windows the audit flags off the table and stores
+        only the entries that differ, with no drain and no slot out of service.  expect / live as for table_audit.  Returns (found, left,
+        slot_bits): the HS_AUDIT_* classes the audit found, those left for table_repair (0 = everything mended; KEY, FLAG and LOOKUP
+        findings are always left) and the audit's uint8 of HS_AUDIT_* bits per slot.  Raises EngineError as table_audit does."""
+        n = self.key_slots if expect is None else _u8(expect, 32).reshape(-1, 32).shape[0]
+        exp = None if expect is None else _u8(expect, 32).reshape(-1, 32)
+        lv = None if live is None else np.ascontiguousarray(live, dtype=np.uint32)
+        if lv is not None and lv.size < (n + 31) // 32:
+            raise ValueError("table_mend: %d live words for %d slots" % (lv.size, n))
+        bits = np.zeros(max(1, n), dtype=np.uint8)
+        found, left = ctypes.c_uint32(0), ctypes.c_uint32(0)
+        rc = self.lib.hs_table_mend(self.h, _ptr(exp) if n and exp is not None else None, _ptr(lv) if lv is not None and lv.size else None, n,
+                                    _ptr(bits), ctypes.byref(found), ctypes.byref(left))
+        if rc != HS_ERR_SELFTEST:
+            self._check(rc, "hs_table_mend")
+        return int(found.value), int(left.value), bits[:n]
+
+    MEND_STATS = ("calls", "windows_recomputed", "entries_rewritten", "windows_left", "slots_left", "cache_flushes")
+
+    def mend_stats(self):
+        """The mend's counters (hs_table_mend_stats), the scrub's mends included, as a dict keyed by MEND_STATS."""
+        out = (ctypes.c_uint64 * len(self.MEND_STATS))()
+        self._check(self.lib.hs_table_mend_stats(self.h, out), "hs_table_mend_stats")
+        return dict(zip(self.MEND_STATS, (int(v) for v in out)))
+
+    def scrub_mend(self, on=True):
+        """With on, a scrub tick whose findings can all be mended mends them (table_mend) instead of repairing them (hs_scrub_mend)."""
+        self._check(self.lib.hs_scrub_mend(self.h, 1 if on else 0), "hs_scrub_mend")
+
     SCRUB_STATS = ("passes", "slots_audited", "base_entries_audited", "ticks", "findings", "slots_repaired", "failed_repairs",
                    "ticks_paused")
 

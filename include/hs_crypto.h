@@ -36,7 +36,7 @@ extern "C" {
 #define HS_ERR_CUDA 1
 #define HS_ERR_ARG 2
 #define HS_ERR_NOMEM 3
-#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer; hs_table_audit / hs_table_repair: a table, slot or lookup entry is wrong */
+#define HS_ERR_SELFTEST 4 /* hs_self_test: a path gave a wrong answer; hs_table_audit / hs_table_repair / hs_table_mend: a table, slot or lookup entry is wrong */
 
 /* verdict selector for the verify entry points */
 #define HS_MODE_STRICT 0u /* Signature::verify semantics  = dalek verify_strict          (crypto/src/lib.rs:200-204) */
@@ -561,6 +561,36 @@ int hs_table_audit(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 3
 int hs_table_repair(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
                     size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_found, uint32_t *out_failed);
 
+/* ---- mend of corrupt comb-table entries in place: no drain, no slot out of service -------------------------------------------
+ * Runs hs_table_audit, also noting the windows that hold its TABLE and BASE findings, recomputes those windows into a bounded scratch
+ * buffer with the build's arithmetic, and stores only the entries whose bytes differ from the fresh build's.  A correct entry is never
+ * written; a wrong one is overwritten once with the right bytes.  A verify that gathers an entry while it is stored reads the old value,
+ * the new one or a mix of the two, and each is wrong only where the table already was, so verification goes on throughout and the
+ * slot stays in service.  Then the mended windows are audited again (the base-point table's windows with the window after each, the
+ * mended slots' whole tables), and, if any entry was rewritten, every verify queue's signature and certificate caches are emptied as
+ * hs_table_repair empties them.  The arguments are hs_table_audit's, with its rules.
+ *   - What is mended: BASE findings (the anchor B is a constant), and the TABLE findings of a slot whose only class is TABLE.  A slot whose
+ *     anchor (entry 1 of window 0) fails is mended only with expect_pks given: without a map, key bytes that changed but still
+ *     decompress look exactly like a bad anchor, and a table rebuilt from them would hold another key's multiples.  KEY, FLAG and LOOKUP
+ *     findings, and the slots that carry them, are left untouched.
+ *   - *out_found: the classes the locating audit found; out_slot_bits (nullable): its per-slot bits; *out_left: the classes left, i.e.
+ *     not mendable or still failing the second audit.  HS_OK iff *out_left == 0; otherwise HS_ERR_SELFTEST, and hs_table_repair then
+ *     finds only what is left.  On a clean context it is one audit and writes nothing.
+ *   - Isolation: it takes the audit's turn (serialised with hs_table_audit, hs_table_repair, the committee stage and commit and the scrub's
+ *     ticks) and holds the context's mutex only to snapshot, to enqueue and to empty the caches; its kernels run on the audit's
+ *     lowest-priority stream.  It never drains the device and never changes a slot's service state.  Its staging (65 entries of 96
+ *     bytes per thread of one launch, 211 MB on a 132-SM device) is allocated on first use and kept with the context.
+ *   - HS_ERR_ARG writes nothing: the audit's argument errors, or key tables that changed between the audit and the stores (a
+ *     registration, update, commit or key-cache change: nothing was stored; call it again).  A change after the stores were enqueued
+ *     waits for them before it writes.  `_dev` verify passes must not overlap a mend, as for an audit.
+ *   - A multi-device context is mended member by member (hs_multi_member) with the same map, as it is repaired. */
+int hs_table_mend(hs_ctx *ctx, const uint8_t *expect_pks_or_null /* n_slots x 32 */, const uint32_t *expect_live_or_null /* bitmap */,
+                  size_t n_slots, uint8_t *out_slot_bits_or_null /* n_slots */, uint32_t *out_found, uint32_t *out_left);
+/* calls (the scrub's mends included), windows recomputed, entries rewritten, windows left (flagged but not mended, or failing the
+ * second audit), slots left to hs_table_repair, cache flushes */
+#define HS_MEND_STATS 6
+int hs_table_mend_stats(hs_ctx *ctx, uint64_t out[HS_MEND_STATS]);
+
 /* ---- scrub of the live key tables: the audit and repair above, a bounded slice at a time, on an engine-owned thread -------------
  * hs_scrub_start starts one thread per context that wakes every period_us microseconds.  Each tick takes the audit's turn (it is
  * serialised with hs_table_audit, hs_table_repair, hs_committee_stage and hs_committee_commit) and audits one slice:
@@ -599,6 +629,11 @@ int hs_scrub_stop(hs_ctx *ctx);
  * finding), slots repaired, failed repairs (findings the second audit still finds), ticks paused on a stale map */
 #define HS_SCRUB_STATS 8
 int hs_scrub_stats(hs_ctx *ctx, uint64_t out[HS_SCRUB_STATS]);
+/* on != 0: a tick whose findings can all be mended (hs_table_mend's rules, with the scrub's map) mends them instead of repairing them;
+ * a tick with any other finding repairs, as without it.  The callback's found / failed keep their meaning, and the mend's work counts
+ * in hs_table_mend_stats, not in the scrub's repaired slots.  Off on a new context; the setting outlives hs_scrub_stop / hs_scrub_start
+ * and takes effect from the next tick.  HS_ERR_ARG: ctx NULL. */
+int hs_scrub_mend(hs_ctx *ctx, int on);
 /* Attaches q (a queue of ctx) to ctx's scrub: from then on every tick also audits the next buckets_per_tick buckets of q's signature
  * cache with hs_queue_sig_audit, wrapping at the end of the table, whether or not the slot map is paused.  A new table (a resize, or
  * the cache turned off and on) starts again at bucket 0; while the cache is off the slice audits nothing.  q_or_null = NULL detaches.

@@ -90,6 +90,30 @@ class Engine {
     if (slot_bits) *slot_bits = std::move(bits);
     return failed;
   }
+  // Mend of corrupt comb-table entries in place (hs_table_mend): no drain, no slot out of service.  Arguments as for table_repair.
+  // Returns the classes left for table_repair (0: everything mended, or nothing was wrong; KEY, FLAG and LOOKUP are always left); found
+  // receives the classes the audit found, slot_bits (nullable) its per-slot bits.  Throws EngineError as table_audit does.
+  uint32_t table_mend(const std::vector<std::array<uint8_t, 32>> *expect = nullptr, const std::vector<uint32_t> *live = nullptr,
+                      uint32_t *found = nullptr, std::vector<uint8_t> *slot_bits = nullptr) const {
+    const size_t n = expect ? expect->size() : key_slots();
+    if (live && live->size() < (n + 31) / 32) throw EngineError("table_mend: live bitmap shorter than the slots");
+    std::vector<uint8_t> bits(n);
+    uint32_t f = 0, left = 0;
+    const int rc = hs_table_mend(ctx_, expect && n ? expect->front().data() : nullptr, live && !live->empty() ? live->data() : nullptr, n,
+                                 bits.data(), &f, &left);
+    if (rc != HS_ERR_SELFTEST) check(rc, "hs_table_mend");
+    if (found) *found = f;
+    if (slot_bits) *slot_bits = std::move(bits);
+    return left;
+  }
+  // calls, windows recomputed, entries rewritten, windows left, slots left to repair, cache flushes (hs_table_mend_stats).
+  std::array<uint64_t, HS_MEND_STATS> mend_stats() const {
+    std::array<uint64_t, HS_MEND_STATS> s{};
+    check(hs_table_mend_stats(ctx_, s.data()), "hs_table_mend_stats");
+    return s;
+  }
+  // on: a scrub tick whose findings can all be mended mends them instead of repairing them (hs_scrub_mend).
+  void scrub_mend(bool on) const { check(hs_scrub_mend(ctx_, on ? 1 : 0), "hs_scrub_mend"); }
   // The engine-owned scrub (hs_scrub_start): every period_us a thread audits the next slots_per_tick slots in service and
   // base_entries_per_tick base-point entries against `expect` / `live` (as for table_audit; the engine copies them), repairs what it
   // finds and calls cb (nullable) once per tick that found anything, on its thread.  After a committee change it pauses until

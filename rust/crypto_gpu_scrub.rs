@@ -31,7 +31,7 @@ extern "C" {
 }
 
 /// The node's index -> key map as the engine takes it: key bytes (zeros for a freed index) and the bitmap of live indices.
-fn map_of(expected: &[Option<[u8; 32]>]) -> (Vec<u8>, Vec<u32>) {
+pub(crate) fn map_of(expected: &[Option<[u8; 32]>]) -> (Vec<u8>, Vec<u32>) {
     let pks: Vec<u8> = expected.iter().flat_map(|k| k.unwrap_or([0u8; 32])).collect();
     let mut live = vec![0u32; (expected.len() + 31) / 32];
     for (i, k) in expected.iter().enumerate() { if k.is_some() { live[i / 32] |= 1 << (i % 32); } }

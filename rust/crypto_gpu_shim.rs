@@ -66,6 +66,10 @@ pub mod multi;
 /// started once after `self_test` (`scrub::start`) and given the new map after every committee change.
 #[path = "crypto_gpu_scrub.rs"]
 pub mod scrub;
+/// The mend of corrupt comb-table entries in place (hs_table_mend*, hs_scrub_mend): what the audit finds fixed with no drain and no
+/// validator out of service, with `audit_tables` (the repair) for what it leaves (`mend::mend_tables`, `mend::attach_scrub`).
+#[path = "crypto_gpu_mend.rs"]
+pub mod mend;
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)

@@ -31,6 +31,8 @@ SIGNATURES = {
     "hs_qc_and_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p]),
     "hs_verify_groups_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
                                      c_void_p]),
+    "hs_explain_groups_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t,
+                                      c_void_p, c_void_p, c_void_p]),
     "hs_ingest_consensus_frames": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "hs_committee_register": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p]),
     "hs_committee_update": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),

@@ -52,6 +52,7 @@
 #include "hs_selftest_vectors.h"
 #include "key_index.h"
 #include "verify_core.cuh"
+#include "explain_select.cuh"
 
 #define HS_THREADS 128
 #define HS_FINISH_GROUP 16  // signatures whose Z's share one inversion
@@ -1528,6 +1529,109 @@ __global__ void __launch_bounds__(HS_THREADS) k_queue_explain(const xq_desc *__r
   }
 }
 
+// hs_explain_groups_dev: the ordered selection of the items whose bit is 0, then a re-check per selected item.  The selection keeps its
+// count on the device: k_sel_count sums the zero bits of each block of HS_SEL_WORDS bitmap words, k_sel_top turns the block sums into
+// exclusive offsets (one block, carry across chunks) and writes the counts to out, and k_sel_scatter ranks each word within its block
+// again and writes the lowest `cap` indices (explain_select.cuh).  k_explain_items reads its count from out[1].
+#define HS_SEL_TOP 1024
+// Exclusive prefix sum of v over the block, and the block's total in *total (blockDim.x = HS_SEL_WORDS or HS_SEL_TOP).
+__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *warp_sums, uint32_t *total) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+  uint32_t x = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t y = __shfl_up_sync(0xffffffffu, x, d);
+    if (lane >= (uint32_t)d) x += y;
+  }
+  if (lane == 31) warp_sums[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    uint32_t s = lane < n_warps ? warp_sums[lane] : 0, t = s;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xffffffffu, t, d);
+      if (lane >= (uint32_t)d) t += y;
+    }
+    if (lane < n_warps) warp_sums[lane] = t - s;  // exclusive offset of each warp
+    if (lane == 31) *total = t;
+  }
+  __syncthreads();
+  const uint32_t r = warp_sums[warp] + x - v;
+  __syncthreads();  // warp_sums and *total may be reused by the caller's next scan
+  return r;
+}
+__global__ void __launch_bounds__(HS_SEL_WORDS) k_sel_count(const uint32_t *__restrict__ bm, uint64_t n, uint32_t *__restrict__ bsum) {
+  __shared__ uint32_t ws[HS_SEL_WORDS / 32], total;
+  const uint64_t w = (uint64_t)blockIdx.x * HS_SEL_WORDS + threadIdx.x;
+  const uint32_t c = w < (n + 31) / 32 ? __popc(bitmap_zero_bits(bm[w], n, w)) : 0;
+  block_excl_scan(c, ws, &total);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = total;
+}
+// bsum[0 .. n_blocks) in place -> exclusive offsets.  out: [0] zero bits, [1] selected = min(zero bits, cap), [2] 0 faults, [3] no fault
+// yet.
+__global__ void __launch_bounds__(HS_SEL_TOP) k_sel_top(uint32_t *bsum, uint32_t n_blocks, uint64_t cap, uint32_t *out) {
+  __shared__ uint32_t ws[HS_SEL_TOP / 32], total;
+  uint32_t carry = 0;
+  for (uint32_t base = 0; base < n_blocks; base += HS_SEL_TOP) {
+    const uint32_t b = base + threadIdx.x, v = b < n_blocks ? bsum[b] : 0;
+    const uint32_t r = block_excl_scan(v, ws, &total);
+    if (b < n_blocks) bsum[b] = carry + r;
+    carry += total;
+  }
+  if (threadIdx.x == 0) {
+    out[0] = carry;
+    out[1] = cap < carry ? (uint32_t)cap : carry;
+    out[2] = 0;
+    out[3] = 0xffffffffu;
+  }
+}
+__global__ void __launch_bounds__(HS_SEL_WORDS) k_sel_scatter(const uint32_t *__restrict__ bm, uint64_t n, const uint32_t *__restrict__ boff,
+                                                              const uint32_t *__restrict__ out, uint32_t *__restrict__ list) {
+  __shared__ uint32_t ws[HS_SEL_WORDS / 32], total;
+  const uint64_t w = (uint64_t)blockIdx.x * HS_SEL_WORDS + threadIdx.x;
+  const uint32_t zeros = w < (n + 31) / 32 ? bitmap_zero_bits(bm[w], n, w) : 0;
+  const uint32_t r = block_excl_scan(__popc(zeros), ws, &total);
+  select_scatter(zeros, (uint64_t)boff[blockIdx.x] + r, w, out[1], list);
+}
+// A thread per selected item, grid-stride over out[1] of them (the grid is a fixed share of the SMs: see launch_explain_items).  Item i
+// = list[j] is re-checked exactly as k_queue_explain re-checks a preimage record: sig[i], pk[i] and Digest = SHA-512(preimage of
+// msg_idx[i])[..32], hashed by sha512_prefix_msg; then sha512_ram32 and explain_record.  Its why byte goes to why[i]; an item the mask
+// finds valid in its mode (why_valid_in_mode) is an engine fault, counted per warp into out[2] with the lowest index in out[3].  It reads
+// the caller's arrays and nothing else: no context table, key slot, flag or hash table, and no base-point table.
+__global__ void __launch_bounds__(HS_THREADS) k_explain_items(const uint32_t *__restrict__ list, const uint8_t *__restrict__ pre,
+                                                              const uint64_t *__restrict__ pre_off, const uint8_t *__restrict__ sig,
+                                                              const uint8_t *__restrict__ pk, const uint32_t *__restrict__ msg_idx,
+                                                              const uint8_t *__restrict__ mode, uint8_t *__restrict__ why, uint32_t *out) {
+  const uint32_t n = out[1];
+  uint32_t faults = 0, first = 0xffffffffu;
+  for (uint32_t j = blockIdx.x * HS_THREADS + threadIdx.x; j < n; j += gridDim.x * HS_THREADS) {
+    const uint32_t i = list[j];
+    uint32_t R[8], S[8], A[8], M[8], h[16];
+    load32(R, sig + 64 * (size_t)i);
+    load32(S, sig + 64 * (size_t)i + 32);
+    load32(A, pk + 32 * (size_t)i);
+    const uint32_t k = msg_idx[i];
+    const uint64_t none[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    sha512_prefix_msg(h, none, 0, pre + pre_off[k], pre_off[k + 1] - pre_off[k]);
+#pragma unroll
+    for (int w = 0; w < 8; w++) M[w] = h[w];
+    sha512_ram32(h, R, A, M);
+    ge_cached tab[9];
+    const uint32_t y = explain_record(R, S, A, h, tab);
+    why[i] = (uint8_t)y;
+    if (why_valid_in_mode(y, mode ? mode[i] : HS_MODE_STRICT)) {
+      faults++;
+      first = min(first, i);
+    }
+  }
+  faults = __reduce_add_sync(0xffffffffu, faults);
+  first = __reduce_min_sync(0xffffffffu, first);
+  if ((threadIdx.x & 31) == 0 && faults) {
+    atomicAdd(out + 2, faults);
+    atomicMin(out + 3, first);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ Digest kernels
 __global__ void __launch_bounds__(HS_THREADS) k_digest32(const uint8_t *__restrict__ data, const uint64_t *__restrict__ off, uint64_t fixed_len,
                                                           size_t n, uint32_t *__restrict__ out) {
@@ -1947,6 +2051,7 @@ struct hs_ctx {
   // grow-only device scratch
   dev_buf in[2], digest[2], xyz, meta, vidx, miss, out;
   dev_buf group_digests;  // hs_verify_groups_dev: Digests of the pass's preimages (read by the main kernels only, so one set serves deferred mode)
+  dev_buf explain_sel;    // hs_explain_groups_dev: block offsets, then the selected item list (not the verify scratch: host calls never wait for it)
   dev_mem<uint32_t> d_miss_count;
   // key cache: tables for keys that were never registered but keep showing up (learned between calls)
   bool explicit_committee = false;   // hs_committee_register was called with keys: the set is fixed, nothing is learned
@@ -4048,6 +4153,36 @@ int hs_verify_groups_dev(hs_ctx *c, const void *d_pre, const void *d_off, size_t
   HS_TRY(hs_digest32_dev(c, d_pre, d_off, n_msgs, dig, stream));
   in_layout L{(const uint8_t *)d_sig, 64, (const uint8_t *)d_pk, 32, (const uint32_t *)d_vidx, dig, 32, (const uint32_t *)d_msg_idx, nullptr, 32, 0};
   return run_verify(c, L, n_items, HS_MODE_STRICT, (uint32_t *)d_item_bitmap, (cudaStream_t)stream, d_pk == nullptr, (const uint8_t *)d_mode);
+}
+
+// ---- explanation of a device-resident pass's rejected items (hs_explain_groups_dev): the selection kernels, then k_explain_items on at
+// most a quarter of the SMs (the explain lane's share, HS_QUEUE_EXPLAIN_SM_DIV), all on `stream` over scratch of its own.  It records no
+// ev_dev_pass: the host-pointer calls do not share its scratch, so they never wait for it.
+int hs_explain_groups_dev(hs_ctx *c, const void *d_pre, const void *d_off, size_t n_msgs, const void *d_sig, const void *d_pk, const void *d_msg_idx,
+                          const void *d_mode, const void *d_item_bitmap, size_t n_items, size_t max_explain, void *d_why, void *d_out, void *stream) {
+  if (!c || (n_items && (!d_pre || !d_off || !d_sig || !d_pk || !d_msg_idx || !d_item_bitmap || !d_why || !d_out)))
+    return fail(c, HS_ERR_ARG, "hs_explain_groups_dev: bad argument");
+  if (n_items && n_msgs == 0) return fail(c, HS_ERR_ARG, "hs_explain_groups_dev: items without preimages");
+  if (n_items > 0xffffffffu) return fail(c, HS_ERR_ARG, "hs_explain_groups_dev: more than 2^32 - 1 items");
+  if (n_items == 0) return HS_OK;
+  HS_CUDA(c, cudaSetDevice(c->device));
+  const cudaStream_t s = (cudaStream_t)stream;
+  const size_t n_words = (n_items + 31) / 32, n_blocks = (n_words + HS_SEL_WORDS - 1) / HS_SEL_WORDS;
+  const size_t cap = max_explain && max_explain < n_items ? max_explain : n_items;
+  HS_TRY(ensure(c, c->explain_sel, (n_blocks + cap) * 4));
+  uint32_t *boff = (uint32_t *)c->explain_sel.p.get(), *list = boff + n_blocks, *out = (uint32_t *)d_out;
+  const uint32_t *bm = (const uint32_t *)d_item_bitmap;
+  if (c->deferred) HS_TRY(hs_results_wait(c, stream));  // the item words of deferred passes are written on the tail stream
+  HS_CUDA(c, cudaMemsetAsync(d_why, HS_WHY_NOT_EXAMINED, n_items, s));
+  k_sel_count<<<(unsigned)n_blocks, HS_SEL_WORDS, 0, s>>>(bm, n_items, boff);
+  k_sel_top<<<1, HS_SEL_TOP, 0, s>>>(boff, (uint32_t)n_blocks, cap, out);
+  k_sel_scatter<<<(unsigned)n_blocks, HS_SEL_WORDS, 0, s>>>(bm, n_items, boff, out, list);
+  const unsigned grid = (unsigned)std::min<size_t>(blocks_for(cap), std::max<size_t>(1, c->n_sms / HS_QUEUE_EXPLAIN_SM_DIV));
+  k_explain_items<<<grid, HS_THREADS, 0, s>>>(list, (const uint8_t *)d_pre, (const uint64_t *)d_off, (const uint8_t *)d_sig, (const uint8_t *)d_pk,
+                                              (const uint32_t *)d_msg_idx, (const uint8_t *)d_mode, (uint8_t *)d_why, out);
+  c->launches += 4;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
 }
 
 // ---- TC::verify / Timeout::verify for many certificates (consensus/src/messages.rs:250-265,290-315)

@@ -20,6 +20,8 @@ WHY_R_INVALID = 4       # R does not decompress
 WHY_A_SMALL = 8         # [8]A is the identity
 WHY_R_SMALL = 16        # [8]R is the identity
 WHY_EQUATION = 32       # S, A, R parse and [S]B + [k](-A) != R
+WHY_NOT_EXAMINED = 0x80  # hs_explain_groups_dev only: the item was accepted, or is past max_explain
+EXPLAIN_DEV_OUT = 4      # hs_explain_groups_dev's out words
 AUDIT_SIGCACHE = 32  # a scrub callback's found: the tick corrected a signature-cache entry (hs_scrub_sig_cache)
 
 
@@ -432,6 +434,18 @@ class Engine:
         ptr = lambda t: None if t is None else t.data_ptr()
         self._check(self.lib.hs_verify_groups_dev(self.h, ptr(d_pre), ptr(d_off), n_msgs, ptr(d_sig), ptr(d_pk), ptr(d_vidx), ptr(d_msg_idx),
                                                   ptr(d_mode), n_items, ptr(d_item_bitmap), self._stream()), "hs_verify_groups_dev")
+
+    def explain_groups_dev(self, d_pre, d_off, n_msgs, d_sig, d_pk, d_msg_idx, d_item_bitmap, n_items, d_why, d_out, d_mode=None,
+                           max_explain=0):
+        """hs_explain_groups_dev: the table-free re-check of Engine.explain for the items of a verify_groups_dev pass whose bit in
+        d_item_bitmap is 0 (the lowest-index max_explain of them; 0 = all), enqueued on torch's current stream.  d_pk holds key bytes
+        (for a committee-indexed pass, the caller's map gathered by validator index).  d_why (uint8, n_items) receives each examined
+        item's WHY_* mask and WHY_NOT_EXAMINED elsewhere; d_out (int32 / uint32, EXPLAIN_DEV_OUT) receives the items whose bit is 0, the
+        items examined, the engine faults among them (rejected, yet valid in their mode) and the lowest faulting index (0xffffffff: none)."""
+        ptr = lambda t: None if t is None else t.data_ptr()
+        self._check(self.lib.hs_explain_groups_dev(self.h, ptr(d_pre), ptr(d_off), n_msgs, ptr(d_sig), ptr(d_pk), ptr(d_msg_idx), ptr(d_mode),
+                                                   ptr(d_item_bitmap), n_items, max_explain, ptr(d_why), ptr(d_out), self._stream()),
+                    "hs_explain_groups_dev")
 
     def keygen_batch_dev(self, d_seeds, d_pks, n):
         self._check(self.lib.hs_keygen_batch_dev(self.h, d_seeds.data_ptr(), n, d_pks.data_ptr(), self._stream()), "hs_keygen_batch_dev")

@@ -719,6 +719,34 @@ int hs_qc_and_dev(hs_ctx *ctx, const void *d_vote_bitmap, const void *d_qc_idx, 
 int hs_verify_groups_dev(hs_ctx *ctx, const void *d_preimages, const void *d_pre_off /* n_msgs + 1 */, size_t n_msgs, const void *d_sig,
                          const void *d_pk_or_null, const void *d_validator_idx_or_null, const void *d_msg_idx, const void *d_mode_or_null,
                          size_t n_items, void *d_item_bitmap, void *stream);
+/* Explanation of the rejected items of a device-resident pass, on the GPU, with nothing copied to the host: the table-free re-check of
+ * hs_explain_rec128 for every item whose bit is 0, and a count of engine faults (items rejected that the re-check finds valid in their mode).
+ *   - Inputs: the arrays of an hs_verify_groups_dev pass (preimages, pre_off, sig, msg_idx, mode) with KEY BYTES in pk, and d_item_bitmap,
+ *     that pass's item bitmap or any bitmap the caller builds.  Item i is examined when its bit is 0: the lowest-index max_explain such
+ *     items, or all of them with max_explain = 0.  Selection is by item index, so the result is deterministic.
+ *   - d_why[i] (n_items bytes): for an examined item, byte for byte what hs_explain_rec128 returns for the record (sig[i], pk[i],
+ *     SHA-512(preimage of msg_idx[i])[..32]); every other byte is HS_WHY_NOT_EXAMINED.
+ *   - d_out (HS_EXPLAIN_DEV_OUT uint32 words): [0] items whose bit is 0, [1] items examined, [2] engine faults among them, [3] the lowest
+ *     index of an engine fault (0xffffffff: none).  An examined item is an engine fault when its mask is 0 under a strict mode byte (any
+ *     byte but 1, or a NULL mode array: hs_verify_groups_dev treats every byte other than 1 as strict), or has no bit other than
+ *     HS_WHY_A_SMALL | HS_WHY_R_SMALL under mode byte 1.  A node that sees out[2] > 0 audits and repairs its tables and answers those
+ *     messages on another verifier.
+ *   - Keys are always key bytes, and the call reads no context table (no comb table, key slot, flag, hash table or base-point table), as
+ *     hs_explain_rec128.  For a committee-indexed pass, pass the caller's own index -> key map gathered by validator index (map[vidx]), so
+ *     the check does not depend on the tables it is meant to doubt.
+ *   - Ordering: enqueued on `stream`, after the caller's earlier work there; the bitmap is read in stream order.  In deferred mode the
+ *     stream first waits on the device for the pass tails already enqueued (as hs_results_wait); there is no host wait.
+ *   - Scratch: its own, not the verify scratch, so host-pointer calls do not wait for it.  Growing it (the first call, or a larger one)
+ *     may synchronise the device, as other `_dev` scratch growth does.  The re-check runs on at most a quarter of the SMs (the explain
+ *     lane's share), grid-stride beyond that, so a flood of junk leaves the other SMs to verify work on other streams.
+ *   - Isolation: it does not teach the key cache and touches no verify queue, cache or counter; its launches count in hs_kernel_launches.
+ *   - n_items == 0 returns HS_OK, writes nothing and launches nothing.  HS_ERR_ARG writes nothing: NULL required pointers (all but
+ *     mode) or n_msgs == 0 with n_items > 0, or n_items above 2^32 - 1.  Device arrays are trusted, as in hs_verify_groups_dev. */
+#define HS_WHY_NOT_EXAMINED 0x80u /* this call only: the item was accepted, or is past max_explain */
+#define HS_EXPLAIN_DEV_OUT 4
+int hs_explain_groups_dev(hs_ctx *ctx, const void *d_preimages, const void *d_pre_off /* n_msgs + 1 */, size_t n_msgs, const void *d_sig,
+                          const void *d_pk, const void *d_msg_idx, const void *d_mode_or_null, const void *d_item_bitmap, size_t n_items,
+                          size_t max_explain, void *d_why /* n_items bytes */, void *d_out /* HS_EXPLAIN_DEV_OUT x uint32 */, void *stream);
 
 /* ---- load generation: RFC 8032 key generation and signing of 32-byte digests ON THE GPU ---------------------------------------
  * generate_keypair / Signature::new (crypto/src/lib.rs:167-175,185-191) for input synthesis only: the node itself signs one

@@ -151,6 +151,17 @@ class Engine {
     check(hs_explain_rec128(ctx_, recs, n, why.data()), "hs_explain_rec128");
     return why;
   }
+  // The same re-check for the rejected items of a device-resident pass (hs_explain_groups_dev), enqueued on `stream` (a cudaStream_t)
+  // with every array in device memory: the pass's arrays with key bytes in d_pk, its item bitmap, and max_explain (0 = every rejected
+  // item).  d_why receives n_items bytes (HS_WHY_NOT_EXAMINED for an item not examined), d_out HS_EXPLAIN_DEV_OUT words: items whose
+  // bit is 0, items examined, engine faults, the lowest faulting index (0xffffffff: none).  Throws EngineError when nothing was enqueued.
+  void explain_groups_dev(const void *d_preimages, const void *d_pre_off, size_t n_msgs, const void *d_sig, const void *d_pk, const void *d_msg_idx,
+                          const void *d_mode_or_null, const void *d_item_bitmap, size_t n_items, size_t max_explain, void *d_why, void *d_out,
+                          void *stream) const {
+    check(hs_explain_groups_dev(ctx_, d_preimages, d_pre_off, n_msgs, d_sig, d_pk, d_msg_idx, d_mode_or_null, d_item_bitmap, n_items, max_explain,
+                                d_why, d_out, stream),
+          "hs_explain_groups_dev");
+  }
   // Staged committee change (hs_committee_stage): the added keys' tables are built and proved off the verify path and nothing changes
   // for verification until committee_commit.  Returns the indices the added keys will have: stage + commit leaves the engine as
   // hs_committee_update(add) then hs_committee_update(remove) would.  Throws EngineError on any failure (HS_ERR_NOMEM: too few free and

@@ -58,6 +58,10 @@ pub mod explain_queue;
 /// the caller's stream (`groups_dev::verify_groups_dev`).
 #[path = "crypto_gpu_groups_dev.rs"]
 pub mod groups_dev;
+/// The explanation of such a pass's rejected items on the GPU (hs_explain_groups_dev): a why byte per rejected item and a count of
+/// engine faults, with nothing copied to the host (`explain_dev::explain_rejected_dev`).
+#[path = "crypto_gpu_explain_dev.rs"]
+pub mod explain_dev;
 /// Several GPUs from this one process (hs_multi_*): large verifies sharded across them, small ones spread round-robin
 /// (`multi::Multi`).
 #[path = "crypto_gpu_multi.rs"]

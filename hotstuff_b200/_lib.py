@@ -39,6 +39,7 @@ SIGNATURES = {
     "hs_committee_stage": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
     "hs_committee_commit": (c_int, [c_void_p]),
     "hs_committee_discard": (c_int, [c_void_p]),
+    "hs_committee_stage_register": (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_void_p, c_void_p]),
     "hs_set_table_budget": (c_int, [c_void_p, c_size_t]),
     "hs_verify_committee": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_u32, c_void_p]),
     "hs_digest32_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),

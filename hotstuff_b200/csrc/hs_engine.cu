@@ -2002,6 +2002,13 @@ struct committee_stage {
   std::vector<uint8_t> keys;    // their key bytes (32 each)
   std::vector<uint8_t> flags;   // their proved flag bytes
   std::vector<uint32_t> remove; // the slots the commit takes out of service
+  // A staged registration (hs_committee_stage_register): `whole`, with no slot above.  keys and flags hold its N keys and their proved
+  // flag bytes; `store` is the new key store beside the live one (moved in here only once proved), with its index, slots and window.
+  bool whole = false;
+  key_store store;
+  key_index index;
+  size_t capacity = 0;
+  int wa = 0;
 };
 // The engine-owned scrub (hs_scrub_start): its thread, the map it audits against and where its pass stands.  `m` guards all but `th`
 // (hs_scrub_start / hs_scrub_stop, under hs_ctx::scrub_life) and the counters (read at any time).  Lock order: m, audit_mu, mu.
@@ -3845,17 +3852,26 @@ void hs_host_free(void *p) {
 }
 
 // ---- committee registration
-// Table slots (capk: N plus spares) and per-key window (wa) that registering N keys picks now.
-static int committee_geometry(hs_ctx *c, size_t N, size_t &capk, int &wa) {
-  // widest per-key window whose tables fit in the budget: ~62 % of the device by default (80 GB H100: 16 bits up to
-  // ~1 k keys, 15 up to ~1.8 k, 14 up to ~3.3 k, 13 up to ~6.3 k, 12 up to ~11 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device
+// Bytes the per-key tables of a registration may take now: ~62 % of the device by default (80 GB H100: 16 bits up to ~1 k keys, 15
+// up to ~1.8 k, 14 up to ~3.3 k, 13 up to ~6.3 k, 12 up to ~11 k), or HS_TABLE_BUDGET_MB / hs_set_table_budget for a shared device,
+// and never more than 7/8 of the free memory.
+static int committee_budget(hs_ctx *c, size_t &budget) {
   size_t free_b = 0, total_b = 0;
   HS_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
-  size_t budget = total_b / 100 * 62;
+  budget = total_b / 100 * 62;
   if (c->table_budget) budget = c->table_budget;
   if (budget > free_b - free_b / 8) budget = free_b - free_b / 8;
-  // spare slots (1/16 of the set, at least 16) let hs_committee_update add validators without rebuilding anything
-  capk = N + (N / 16 > 16 ? N / 16 : 16);
+  return HS_OK;
+}
+// Table slots of a committee of N keys: spare slots (1/16 of the set, at least 16) let hs_committee_update add validators without
+// rebuilding anything.
+static size_t committee_capacity(size_t N) { return N + (N / 16 > 16 ? N / 16 : 16); }
+// Table slots (capk: N plus spares) and per-key window (wa) that registering N keys picks now: the widest window whose tables fit in
+// the budget.
+static int committee_geometry(hs_ctx *c, size_t N, size_t &capk, int &wa) {
+  size_t budget = 0;
+  HS_TRY(committee_budget(c, budget));
+  capk = committee_capacity(N);
   wa = 8;
   for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8}) {  // 17 bits: 15 windows (94 MB per key: committees up to ~500 keys on 80 GB); 18 would still need 15
     if (c->wa_forced && w != c->wa_forced) continue;
@@ -5607,6 +5623,17 @@ static int launch_table_audit(hs_ctx *c, cudaStream_t stream, const ge_niels *ta
   return HS_OK;
 }
 
+// k_slot_audit over the slots and hash entries of T on `stream`: the KEY / FLAG / LOOKUP checks against the liveness mirror `live` and
+// the caller's map (expect_pks / expect_live, nullable), writing `auditable` for k_table_audit.
+static int launch_slot_audit(hs_ctx *c, cudaStream_t stream, const key_table &T, const uint8_t *key_flags, const uint8_t *live,
+                             const uint8_t *expect_pks, const uint32_t *expect_live, uint8_t *auditable, const audit_out &O) {
+  k_slot_audit<<<blocks_for((size_t)T.n_keys + (size_t)T.mask + 1, 256), 256, 0, stream>>>(T, key_flags, live, expect_pks, expect_live,
+                                                                                          (expect_pks || expect_live) ? 1 : 0, auditable, O);
+  c->launches++;
+  HS_CUDA(c, cudaGetLastError());
+  return HS_OK;
+}
+
 // The audit's private stream of the lowest priority and its event, created on first use.
 static int audit_stream(hs_ctx *c) {
   audit_state &A = c->audit;
@@ -5691,12 +5718,8 @@ static int audit_enqueue_locked(hs_ctx *c, const char *entry, const uint8_t *exp
   const audit_wins key_wins{wbits, 0}, base_wins{wbits + r.base_word, 0};
   const auto kw = [&](size_t b) { return audit_wins{wbits, b * (size_t)(c->cp.na + 1)}; };
   if (n) {
-    const key_table T = ctx_tables(c).T;
-    k_slot_audit<<<blocks_for(n + (size_t)T.mask + 1, 256), 256, 0, A.stream>>>(
-        T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
-        expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, (expect_pks || expect_live) ? 1 : 0, in.ptr(s_ok), O);
-    c->launches++;
-    HS_CUDA(c, cudaGetLastError());
+    HS_TRY(launch_slot_audit(c, A.stream, ctx_tables(c).T, c->keys.key_flags, in.ptr(s_mirror), expect_pks ? in.ptr(s_pks) : nullptr,
+                             expect_live ? reinterpret_cast<const uint32_t *>(in.ptr(s_live)) : nullptr, in.ptr(s_ok), O));
     if (!slice)
       HS_TRY(launch_table_audit(c, A.stream, c->keys.atables, nullptr, n, c->a_table_entries, c->cp.wa, c->cp.na, c->keys.pks, in.ptr(s_ok), O,
                                 nullptr, windows ? &key_wins : nullptr));
@@ -6140,11 +6163,37 @@ extern "C" int hs_committee_stage(hs_ctx *c, const uint8_t *add_pks, size_t n_ad
   return HS_OK;
 }
 
+// The commit of a staged registration, under both mutexes: drains the device as registration does, releases the key cache's state and
+// moves the proved store in.  The replaced store goes to `old`, which the caller frees once it has released the mutexes.
+static int register_commit_locked(hs_ctx *c, key_store &old) {
+  HS_CUDA(c, cudaSetDevice(c->device));
+  // A queue enqueues a launch only while it holds c->mu, so nothing launched against the old indices survives this line.
+  HS_CUDA(c, cudaDeviceSynchronize());
+  committee_stage S = std::move(c->stage);
+  old = std::move(c->keys);
+  cache_release(c);  // bumps key_gen and map_gen: the scrub pauses, and an audit against the old map is refused
+  c->learn_pending = false;
+  c->cache_full = false;
+  c->cache_enabled = c->cache_wanted;
+  c->keys = std::move(S.store);
+  set_window(c->cp, true, S.wa);
+  c->a_table_entries = comb_table_entries(S.wa);
+  c->n_keys = S.keys.size() / 32;
+  c->key_capacity = S.capacity;
+  c->explicit_committee = true;
+  c->h_pks = std::move(S.keys);
+  c->h_index = std::move(S.index);
+  c->h_key_live.assign(c->n_keys, SLOT_LIVE);
+  return HS_OK;
+}
+
 extern "C" int hs_committee_commit(hs_ctx *c) {
   if (!c) return HS_ERR_ARG;
+  key_store old;  // declared before the locks: freed after both are released (cudaFree of the old tables waits for the device)
   std::lock_guard<std::mutex> ga(c->audit_mu);  // before mu: the commit never waits for an audit while it holds the mutex
   std::lock_guard<std::mutex> g(c->mu);
   committee_stage &S = c->stage;
+  if (S.ready && S.whole) return register_commit_locked(c, old);
   if (!S.ready || !committee_registered(c))
     return fail_args(c, "hs_committee_commit", "no stage pending (none was made, or a registration or update discarded it)");
   HS_CUDA(c, cudaSetDevice(c->device));
@@ -6172,9 +6221,112 @@ extern "C" int hs_committee_commit(hs_ctx *c) {
 
 extern "C" int hs_committee_discard(hs_ctx *c) {
   if (!c) return HS_ERR_ARG;
+  key_store staged;  // a staged registration's store, freed after both locks are released
   std::lock_guard<std::mutex> ga(c->audit_mu);
   std::lock_guard<std::mutex> g(c->mu);
+  staged = std::move(c->stage.store);
   stage_drop(c);
+  return HS_OK;
+}
+
+// ---- staged registration (hs_committee_stage_register; hs_committee_commit and hs_committee_discard apply or drop it)
+// Test builds XOR one armed byte of the staged store before its proof (hs_test_poke_staged); the product build does nothing.
+static int staged_poke_apply(hs_ctx *c, key_store &K, size_t N, size_t entries, cudaStream_t stream);
+// stage_register(P, w) + commit leaves the context as hs_committee_register(P) leaves one whose window came out as w.  Under c->mu the
+// stage checks the arguments, picks the geometry and marks itself pending; then, holding only audit_mu, it builds a whole new key store
+// beside the live one on the audit's stream and proves it with the audit's checks.  Nothing live is read or written until the commit.
+extern "C" int hs_committee_stage_register(hs_ctx *c, const uint8_t *pks, size_t N, int key_bits, uint32_t *out_valid_bitmap,
+                                           int *out_key_bits) {
+  const char *entry = "hs_committee_stage_register";
+  if (!c || !pks || N == 0 || N >= HS_NO_KEY || (key_bits && (key_bits < 8 || key_bits > 17))) return fail_args(c, entry, "bad argument");
+  std::lock_guard<std::mutex> ga(c->audit_mu);
+  const size_t capk = committee_capacity(N);
+  int wa = 0;
+  comb_params cp{};
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    if (c->stage.busy) return fail_args(c, entry, "a stage is already pending (commit or discard it)");
+    if (key_bits && c->wa_forced && key_bits != c->wa_forced) return fail_args(c, entry, "key_bits differs from the context's forced window");
+    HS_CUDA(c, cudaSetDevice(c->device));
+    size_t budget = 0;  // with the live store still allocated
+    HS_TRY(committee_budget(c, budget));
+    const int want = key_bits ? key_bits : c->wa_forced;
+    for (int w : {17, 16, 15, 14, 13, 12, 11, 10, 9, 8})
+      if ((!want || w == want) && capk * comb_table_entries(w) * sizeof(ge_niels) <= budget) {
+        wa = w;
+        break;
+      }
+    if (!wa) return fail(c, HS_ERR_NOMEM, "hs_committee_stage_register: the tables do not fit in the table budget beside the live store");
+    if (sc_ndigits_rt(wa) + c->cp.nb > HS_MAX_DIGITS) return fail_args(c, entry, "window combination exceeds HS_MAX_DIGITS");
+    cp = c->cp;
+    set_window(cp, true, wa);
+    c->stage.busy = true;
+    c->stage.whole = true;
+  }
+  key_index index;
+  index.reset(capk);
+  index.build(pks, N, [](size_t) { return true; });
+  const size_t entries = comb_table_entries(wa);
+  key_store K;
+  std::vector<uint8_t> fl(N), res(8 + 4 * (2 + N));
+  audit_state &A = c->audit;
+  const int rc = [&]() -> int {
+    HS_TRY(audit_stream(c));
+    const cudaError_t e = make_key_store(K, capk, index.slots.size(), wa, A.stream);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      return fail(c, HS_ERR_NOMEM, "hs_committee_stage_register: the staged tables do not fit in device memory", e);
+    }
+    HS_CUDA(c, cudaMemcpyAsync(K.pks, pks, N * 32, cudaMemcpyHostToDevice, A.stream));
+    HS_CUDA(c, cudaMemcpyAsync(K.slots, index.slots.data(), index.slots.size() * 4, cudaMemcpyHostToDevice, A.stream));
+    HS_TRY(launch_build(c, K.pks, nullptr, N, 1, wa, cp.na, K.atables, K.key_flags, A.stream));
+    HS_TRY(staged_poke_apply(c, K, N, entries, A.stream));  // test builds: hs_test_poke_staged; a no-op otherwise
+    // The proof: every slot in service, its key bytes against the caller's, its flag byte and lookup, every hash entry, every table.
+    const std::vector<uint8_t> live(N, SLOT_LIVE);
+    h2d_stage in;
+    const size_t s_res = in.add(nullptr, res.size()), s_pks = in.add(pks, N * 32), s_live = in.add(live.data(), N), s_ok = in.add(nullptr, N);
+    HS_TRY(in.upload(c, A.scratch, A.stream));
+    uint8_t *d_res = in.ptr(s_res);
+    HS_CUDA(c, cudaMemsetAsync(d_res, 0xff, 8, A.stream));
+    HS_CUDA(c, cudaMemsetAsync(d_res + 8, 0, res.size() - 8, A.stream));
+    const audit_out O{reinterpret_cast<unsigned long long *>(d_res), reinterpret_cast<uint32_t *>(d_res + 8)};
+    HS_TRY(launch_slot_audit(c, A.stream, store_tables(K, index, N, entries, cp).T, K.key_flags, in.ptr(s_live), in.ptr(s_pks), nullptr,
+                             in.ptr(s_ok), O));
+    HS_TRY(launch_table_audit(c, A.stream, K.atables, nullptr, N, entries, wa, cp.na, K.pks, in.ptr(s_ok), O));
+    // No event: A.done orders the key-cache paths behind the audits, and learning need not wait for this build.
+    HS_CUDA(c, cudaMemcpyAsync(res.data(), d_res, res.size(), cudaMemcpyDeviceToHost, A.stream));
+    HS_CUDA(c, cudaMemcpyAsync(fl.data(), K.key_flags, N, cudaMemcpyDeviceToHost, A.stream));
+    HS_CUDA(c, cudaStreamSynchronize(A.stream));
+    const uint32_t *bits = reinterpret_cast<const uint32_t *>(res.data() + 8);
+    uint32_t failed = bits[1];
+    for (size_t s = 0; s < N; s++) failed |= bits[2 + s];
+    if (failed) {
+      uint64_t first;
+      memcpy(&first, res.data(), 8);
+      return fail(c, HS_ERR_SELFTEST, ("hs_committee_stage_register: the staged store failed its proof: " + audit_message(first, N, bits)).c_str());
+    }
+    return HS_OK;
+  }();
+  std::lock_guard<std::mutex> g(c->mu);
+  committee_stage &S = c->stage;
+  if (!S.busy || !S.whole) return fail_args(c, entry, "a registration or update ran during the stage; stage again");  // it dropped the stage
+  if (rc != HS_OK) {
+    S = {};
+    return rc;
+  }
+  S.store = std::move(K);
+  S.index = std::move(index);
+  S.capacity = capk;
+  S.wa = wa;
+  S.keys.assign(pks, pks + N * 32);
+  S.flags = fl;
+  S.ready = true;
+  if (out_valid_bitmap) {
+    for (size_t w = 0; w < (N + 31) / 32; w++) out_valid_bitmap[w] = 0;
+    for (size_t i = 0; i < N; i++)
+      if (fl[i] & 1) out_valid_bitmap[i >> 5] |= 1u << (i & 31);
+  }
+  if (out_key_bits) *out_key_bits = wa;
   return HS_OK;
 }
 
@@ -6538,6 +6690,43 @@ extern "C" int hs_test_poke(hs_ctx *c, int region, size_t index, size_t byte_off
   HS_CUDA(c, cudaMemcpy(p, &v, 1, cudaMemcpyHostToDevice));
   return HS_OK;
 }
+// Arms one byte (hs_test_poke's POKE_TABLE, POKE_KEY or POKE_FLAG addressing) that c's next hs_committee_stage_register XORs in its
+// staged store between the build and the proof; an index or offset past that store leaves it untouched.  One armed byte per process.
+static struct {
+  hs_ctx *c = nullptr;
+  int region = 0;
+  size_t index = 0, byte_offset = 0;
+  uint8_t xor_mask = 0;
+} staged_poke;
+static std::mutex staged_poke_mu;
+extern "C" int hs_test_poke_staged(hs_ctx *c, int region, size_t index, size_t byte_offset, uint8_t xor_mask) {
+  if (!c || (region != POKE_TABLE && region != POKE_KEY && region != POKE_FLAG)) return HS_ERR_ARG;
+  std::lock_guard<std::mutex> g(staged_poke_mu);
+  staged_poke.c = c;
+  staged_poke.region = region;
+  staged_poke.index = index;
+  staged_poke.byte_offset = byte_offset;
+  staged_poke.xor_mask = xor_mask;
+  return HS_OK;
+}
+// Applies and disarms the armed byte when it is c's, on the staged store K of N slots, on `stream` behind its build.
+static int staged_poke_apply(hs_ctx *c, key_store &K, size_t N, size_t entries, cudaStream_t stream) {
+  std::lock_guard<std::mutex> g(staged_poke_mu);
+  if (staged_poke.c != c) return HS_OK;
+  staged_poke.c = nullptr;
+  const size_t i = staged_poke.index, off = staged_poke.byte_offset;
+  uint8_t *p = nullptr;
+  if (staged_poke.region == POKE_TABLE && i < N && off < entries * sizeof(ge_niels)) p = reinterpret_cast<uint8_t *>(K.atables + i * entries) + off;
+  else if (staged_poke.region == POKE_KEY && i < N && off < 32) p = K.pks + 32 * i + off;
+  else if (staged_poke.region == POKE_FLAG && i < N && off == 0) p = K.key_flags + i;
+  if (!p) return HS_OK;
+  uint8_t v = 0;
+  HS_CUDA(c, cudaMemcpyAsync(&v, p, 1, cudaMemcpyDeviceToHost, stream));
+  HS_CUDA(c, cudaStreamSynchronize(stream));
+  v ^= staged_poke.xor_mask;
+  HS_CUDA(c, cudaMemcpyAsync(p, &v, 1, cudaMemcpyHostToDevice, stream));
+  return HS_OK;
+}
 // XORs one byte of the signature-cache entry of q that holds rec (sig | key bytes | Digest) on an idle queue: byte_offset < 128 into its
 // words, 128 its flag byte.  HS_ERR_ARG when the cache is off, no entry holds rec or the offset is past the flag byte.  It changes the
 // bytes a hit answers from, never seq or the round-robin counter.
@@ -6562,4 +6751,6 @@ extern "C" int hs_test_poke_sig(hs_queue *q, const uint8_t rec[128], size_t byte
     }
   return fail_args(c, "hs_test_poke_sig", "no entry holds the record");
 }
+#else
+static int staged_poke_apply(hs_ctx *, key_store &, size_t, size_t, cudaStream_t) { return HS_OK; }
 #endif

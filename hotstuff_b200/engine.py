@@ -361,13 +361,29 @@ class Engine:
         changes for verification until committee_commit; stage + commit leaves the engine as update(add) then update(remove=remove)."""
         return _committee_update(self, self.lib.hs_committee_stage, "hs_committee_stage", add, remove)
 
+    def committee_stage_register(self, pks, key_bits=0):
+        """Builds and proves a whole new key store for pks beside the live one (hs_committee_stage_register): returns the keys' validity
+        (bool[N]) and the window.  Nothing changes for verification until committee_commit; stage + commit leaves the engine as
+        committee_register(pks) at that window.  key_bits 0: the widest window that fits beside the live store; 8..17: that window."""
+        pks = _u8(pks, 32).reshape(-1, 32)
+        n = pks.shape[0]
+        bm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
+        bits = ctypes.c_int(0)
+        self._check(self.lib.hs_committee_stage_register(self.h, _ptr(pks) if n else None, n, int(key_bits), _ptr(bm), ctypes.byref(bits)),
+                    "hs_committee_stage_register")
+        self._staged_keys = n
+        return bitmap_to_bools(bm, n), bits.value
+
     def committee_commit(self):
-        """Switches the staged change in (hs_committee_commit): builds no table."""
+        """Switches the staged change in (hs_committee_commit): builds no table.  A staged registration replaces the committee."""
         self._check(self.lib.hs_committee_commit(self.h), "hs_committee_commit")
+        if getattr(self, "_staged_keys", None) is not None:
+            self.n_keys, self._staged_keys = self._staged_keys, None
 
     def committee_discard(self):
-        """Frees the staged slots (hs_committee_discard); a no-op when nothing is staged."""
+        """Frees the staged slots or the staged store (hs_committee_discard); a no-op when nothing is staged."""
         self._check(self.lib.hs_committee_discard(self.h), "hs_committee_discard")
+        self._staged_keys = None
 
     def set_table_budget(self, nbytes):
         self._check(self.lib.hs_set_table_budget(self.h, int(nbytes)), "hs_set_table_budget")
@@ -515,6 +531,7 @@ def _committee_register(owner, fn, name, pks):
     bm = np.zeros(max(1, (n + 31) // 32), dtype=np.uint32)
     owner._check(fn(owner.h, _ptr(pks) if n else None, n, _ptr(bm)), name)
     owner.n_keys = n
+    owner._staged_keys = None  # a registration discards a staged one
     return bitmap_to_bools(bm, n)
 
 
@@ -523,6 +540,7 @@ def _committee_update(owner, fn, name, add, remove):
     rem = np.zeros(0, np.uint32) if remove is None else np.ascontiguousarray(remove, dtype=np.uint32)
     out = np.zeros(max(1, add.shape[0]), dtype=np.uint32)
     owner._check(fn(owner.h, _ptr(add) if add.shape[0] else None, add.shape[0], _ptr(rem) if rem.shape[0] else None, rem.shape[0], _ptr(out)), name)
+    owner._staged_keys = None  # an update discards a staged registration; an incremental stage succeeds only with none pending
     return out[: add.shape[0]]
 
 
@@ -607,17 +625,48 @@ class MultiEngine:
         if err is not None:
             self.discard_committee()
             raise err
+        self._staged_keys = None
+        return res[0]
+
+    def stage_register_committee(self, pks, key_bits=0):
+        """The staged registration on every member, member by member through hs_committee_stage_register: stages on every member at
+        once, one thread each, and returns the keys' validity (bool[N]) and the window, the same on every member.  If any member fails,
+        or the members differ in either, the stage is discarded on every member and EngineError raised: every member keeps its committee.
+        commit_committee switches it in."""
+        res = [None] * len(self._members)
+
+        def stage(i):
+            try:
+                res[i] = self._members[i].committee_stage_register(pks, key_bits)
+            except EngineError as e:
+                res[i] = e
+
+        threads = [threading.Thread(target=stage, args=(i,)) for i in range(len(self._members))]
+        for t in threads:
+            t.start()
+        for t in threads:
+            t.join()
+        err = next((r for r in res if isinstance(r, EngineError)), None)
+        if err is None and any(not np.array_equal(r[0], res[0][0]) or r[1] != res[0][1] for r in res[1:]):
+            err = EngineError("stage_register_committee: the members gave different validity or windows")
+        if err is not None:
+            self.discard_committee()
+            raise err
+        self._staged_keys = len(res[0][0])
         return res[0]
 
     def commit_committee(self):
         """hs_committee_commit on every member.  After a failure the members may differ: re-register."""
         for e in self._members:
             e.committee_commit()
+        if getattr(self, "_staged_keys", None) is not None:
+            self.n_keys, self._staged_keys = self._staged_keys, None
 
     def discard_committee(self):
         """hs_committee_discard on every member."""
         for e in self._members:
             e.committee_discard()
+        self._staged_keys = None
 
     def verify_rec128(self, recs, mode=MODE_STRICT):
         return _verify_rec128(self, self.lib.hs_multi_verify_rec128, "hs_multi_verify_rec128", recs, mode)

@@ -202,6 +202,35 @@ int hs_committee_stage(hs_ctx *ctx, const uint8_t *add_pks /* n_add x 32 */, siz
                        uint32_t *out_add_idx);
 int hs_committee_commit(hs_ctx *ctx);
 int hs_committee_discard(hs_ctx *ctx);
+/* Staged registration: build and prove a whole new key store beside the live one, then switch it in with hs_committee_commit.  Use it
+ * where hs_committee_stage returns HS_ERR_NOMEM, or where the per-key window should change.
+ *   - Rule: hs_committee_stage_register(P, w) followed by hs_committee_commit leaves the context exactly as hs_committee_register(P) leaves
+ *     a context whose window came out as w: the same out_valid_bitmap, hs_key_slots, slot capacity (N plus N/16 spares, at least 16), key
+ *     bytes, flag bytes, hash table, comb tables, hs_window_bits and verdicts on every path; the key cache is released; later
+ *     hs_committee_update / hs_committee_stage calls behave as after that registration.
+ *   - key_bits: 0 picks the widest window whose NEW tables alone fit in the table budget (hs_set_table_budget) and in 7/8 of the free
+ *     memory with the live store still allocated, so it may be narrower than what a registration would pick after releasing the old
+ *     store: discard and stage again with an explicit width to choose.  8..17: that window exactly, under the same test.  The budget
+ *     bounds each store, not their sum: both stores stay resident from the stage until the commit frees the old one, so the per-key
+ *     tables may use up to about twice the budget meanwhile.  A tenant sharing the device must leave room for that, or register instead.  A context created with a forced key window
+ *     stages at that window.  *out_key_bits (nullable) receives the window; out_valid_bitmap (nullable): bit i = key i decompresses.
+ *   - Under the context's mutex it checks the arguments and picks the geometry; then, serialised with audits, repairs, mends, scrub ticks
+ *     and hs_committee_stage but without the mutex, it builds all N tables in one launch on the audit's private lowest-priority stream and
+ *     proves the staged store with hs_table_audit's checks (KEY against pks, FLAG, LOOKUP, every hash entry, every comb-table entry).
+ *   - Until the commit, verification is exactly as before the stage: the live tables, hs_key_slots, hs_window_bits and audits against the
+ *     current map are untouched.  A context with no registered committee may stage a registration; the commit replaces its key cache.
+ *   - Errors, none of which touch the live committee: HS_ERR_NOMEM when the staged store does not fit (nothing stays allocated; a budget
+ *     too small for any window gives it too, where hs_committee_register would still try 8-bit windows); HS_ERR_SELFTEST when the proof
+ *     fails (nothing stays staged); HS_ERR_ARG for N == 0, N >= HS_NO_KEY, key_bits outside 0 and 8..17 or unlike a forced window, a
+ *     stage of either kind already pending, or a registration or update that ran during the stage.  Every error writes nothing.
+ *   - hs_committee_commit applies a staged registration: it drains the device as hs_committee_register does, moves the staged store in,
+ *     releases the key cache's state and starts a new slot map (the scrub pauses until hs_scrub_set_map; an audit with the old map
+ *     returns HS_ERR_ARG).  It frees the old store after releasing the context's mutex.  The signature and certificate caches are kept, as
+ *     for hs_committee_stage.  A registration or update since the stage discarded it: HS_ERR_ARG and no change.  hs_committee_discard
+ *     frees the staged store.  A repair, mend or audit leaves a staged registration pending.
+ *   - As for hs_committee_register, no `_dev` verify pass may be in flight across the commit. */
+int hs_committee_stage_register(hs_ctx *ctx, const uint8_t *pks /* N x 32 */, size_t N, int key_bits, uint32_t *out_valid_bitmap,
+                                int *out_key_bits);
 /* Memory budget (bytes) for the per-key tables of the NEXT registration / key-cache allocation (0 = default, ~62 % of the
  * device; also env HS_TABLE_BUDGET_MB at context creation).  The engine picks the widest window that fits: e.g. 4,096 keys in
  * 18 GB -> 12-bit windows.  Lets the engine sit beside another tenant on the same GPU. */
@@ -809,7 +838,10 @@ int hs_peer_timed_out(hs_ctx *ctx);
  *     (hs_committee_stage / _commit / _discard) is made member by member through hs_multi_member with the same arguments, as a repair is:
  *     stage on every member (at once, from one thread per member); if any stage fails or the members return different indices, discard
  *     on every member; otherwise commit on every member.  After a failed commit the members may differ: re-register.  The bindings do
- *     exactly this (MultiEngine.stage_committee / commit_committee / discard_committee, hs::MultiEngine, multi::Multi).  Apart from that,
+ *     exactly this (MultiEngine.stage_committee / commit_committee / discard_committee, hs::MultiEngine, multi::Multi).  A staged
+ *     registration (hs_committee_stage_register) is made the same way, and is committed only when every member staged with the same
+ *     out_valid_bitmap and window: a failed or mismatched stage is discarded on every member, which all keep their committee
+ *     (MultiEngine.stage_register_committee, hs::MultiEngine::stage_register_committee, multi::Multi::stage_register_committee).  Apart from that,
  *     the committee-indexed forms need every member's committee changed through the two calls above: never change one member alone.
  *   - Pinned memory from hs_host_alloc (cudaMallocHost) is portable under UVA: every member DMAs from the caller's pinned buffers directly.
  *   - hs_multi_destroy joins the workers and destroys the members (and the verify queues created on them); it must not race with calls.

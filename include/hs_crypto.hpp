@@ -173,6 +173,16 @@ class Engine {
   }
   void committee_commit() const { check(hs_committee_commit(ctx_), "hs_committee_commit"); }
   void committee_discard() const { check(hs_committee_discard(ctx_), "hs_committee_discard"); }
+  // A whole new key store for pks built and proved beside the live one (hs_committee_stage_register), switched in by committee_commit:
+  // stage + commit leaves the engine as hs_committee_register(pks) at the returned window.  key_bits 0: the widest window that fits beside
+  // the live store; 8..17: that window.  Returns ceil(N / 32) words of key validity and the window.  Throws EngineError on any failure
+  // (the live committee is untouched).
+  std::pair<std::vector<uint32_t>, int> committee_stage_register(const uint8_t *pks, size_t N, int key_bits = 0) const {
+    std::vector<uint32_t> valid((N + 31) / 32);
+    int bits = 0;
+    check(hs_committee_stage_register(ctx_, pks, N, key_bits, valid.data(), &bits), "hs_committee_stage_register");
+    return {valid, bits};
+  }
   std::string error() const { return hs_last_error(ctx_); }
 
  private:
@@ -241,6 +251,31 @@ class MultiEngine {
       throw EngineError(err);
     }
     return idx.at(0);
+  }
+  // The staged registration on every member, member by member through the single-context call: stages on every member at once, one
+  // thread each, and returns the validity words and the window, the same on every member.  If any member fails, or the members differ
+  // in either, the stage is discarded on every member and EngineError thrown: every member keeps its committee.  commit_committee
+  // switches it in.
+  std::pair<std::vector<uint32_t>, int> stage_register_committee(const uint8_t *pks, size_t N, int key_bits = 0) {
+    std::vector<std::future<std::pair<std::vector<uint32_t>, int>>> parts;
+    for (auto &e : members_)
+      parts.push_back(std::async(std::launch::async, [&e, pks, N, key_bits] { return e->committee_stage_register(pks, N, key_bits); }));
+    std::vector<std::pair<std::vector<uint32_t>, int>> res;
+    std::string err;
+    for (auto &p : parts) {
+      try {
+        res.push_back(p.get());
+      } catch (const EngineError &x) {
+        if (err.empty()) err = x.what();
+      }
+    }
+    for (size_t i = 1; err.empty() && i < res.size(); i++)
+      if (res[i] != res[0]) err = "stage_register_committee: member " + std::to_string(i) + " gave other validity or window than member 0";
+    if (!err.empty()) {
+      for (auto &e : members_) hs_committee_discard(e->raw());
+      throw EngineError(err);
+    }
+    return res.at(0);
   }
   // hs_committee_commit on every member.  After a failure the members may differ: re-register.
   void commit_committee() {

@@ -104,6 +104,36 @@ impl Multi {
             }
         }
     }
+    /// The staged registration on every member, member by member through the single-context call: stages on every member at once,
+    /// one thread each, and returns the window and the indices of keys that do not decompress.  If any member fails, or the members
+    /// differ in validity or window, the stage is discarded on every member and Err returned: every member keeps its committee.
+    /// `commit_committee` switches it in.
+    pub fn stage_register_committee(&self, keys: &[[u8; 32]], key_bits: i32) -> Result<(i32, Vec<usize>), GpuError> {
+        let members: Vec<Member> = (0..self.members()).map(|i| Member(self.member(i))).collect();
+        let res: Vec<Result<(Vec<u32>, i32), GpuError>> = std::thread::scope(|s| {
+            let hs: Vec<_> = members.iter()
+                .map(|m| s.spawn(move || { let m: &Member = m; super::stage_register::stage_register_on(m.0, keys, key_bits) })).collect();
+            hs.into_iter().map(|h| h.join().unwrap_or(Err(GpuError::Unavailable))).collect()
+        });
+        let (mut got, mut fail): (Option<(Vec<u32>, i32)>, Option<GpuError>) = (None, None);
+        for r in res {
+            match r {
+                Err(e) => { if fail.is_none() { fail = Some(e); } }
+                Ok(v) => match &got {
+                    None => got = Some(v),
+                    Some(x) if *x == v => {}
+                    Some(_) => { if fail.is_none() { fail = Some(GpuError::Engine("stage_register_committee: the members gave different validity or windows".into())); } }
+                },
+            }
+        }
+        match (fail, got) {
+            (None, Some((valid, bits))) => Ok((bits, (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect())),
+            (fail, _) => {
+                for m in &members { let _ = super::discard_on(m.0); }
+                Err(fail.unwrap_or(GpuError::Unavailable))
+            }
+        }
+    }
     /// Commits the staged change on every member.  Err: the members may differ, re-register.
     pub fn commit_committee(&self) -> Result<(), GpuError> {
         (0..self.members()).try_for_each(|i| super::commit_on(self.member(i)))

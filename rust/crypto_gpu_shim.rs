@@ -74,6 +74,12 @@ pub mod scrub;
 /// validator out of service, with `audit_tables` (the repair) for what it leaves (`mend::mend_tables`, `mend::attach_scrub`).
 #[path = "crypto_gpu_mend.rs"]
 pub mod mend;
+/// The staged registration (hs_committee_stage_register): the next committee's whole key store built and proved beside the live one,
+/// switched in at the boundary with one drain, for a change the spare slots cannot hold or a new window (`stage_register_committee`,
+/// `commit_registration`).
+#[path = "crypto_gpu_stage_register.rs"]
+pub mod stage_register;
+pub use stage_register::{commit_registration, discard_registration, stage_register_committee};
 
 #[repr(C)] pub struct HsCtx { _private: [u8; 0] }
 #[repr(C)] #[derive(Clone, Copy)] pub struct HsRec128 { pub sig: [u8; 64], pub pk: [u8; 32], pub msg: [u8; 32] } // (Signature, PublicKey, Digest)
@@ -145,9 +151,15 @@ static DISABLED: AtomicBool = AtomicBool::new(false);
 /// The node-side index -> key map of the registered committee (None = a freed index): registration order, then every update's
 /// removals and returned indices.  `audit_tables` checks the engine's slots against it after every change.
 static KEYS: Mutex<Vec<Option<[u8; 32]>>> = Mutex::new(Vec::new());
-/// The staged committee change (`stage_committee`) that `commit_committee` applies to KEYS: the added keys, their indices and the removed
-/// indices.  KEYS lists no staged index before the commit: the engine holds staged slots out of service, and the audit would report one.
-struct Staged { add: Vec<[u8; 32]>, idx: Vec<u32>, remove: Vec<u32> }
+/// What the engine holds staged, mirrored here: it has one stage, of either kind, and hs_committee_commit / hs_committee_discard apply
+/// to whichever is pending.  A change (`stage_committee`) is applied to KEYS by `commit_committee`: the added keys, their indices and the
+/// removed indices (KEYS lists no staged index before the commit: the engine holds staged slots out of service, and the audit would
+/// report one).  A registration (`stage_register::stage_register_committee`) replaces KEYS at `stage_register::commit_registration`.
+/// Each commit and discard checks the kind before it calls the engine; a registration or update clears it, as the engine does.
+enum Staged {
+    Change { add: Vec<[u8; 32]>, idx: Vec<u32>, remove: Vec<u32> },
+    Registration(Vec<[u8; 32]>),
+}
 static STAGED: Mutex<Option<Staged>> = Mutex::new(None);
 
 /// None when no GPU / the library failed to initialise / the self-test failed: every caller below then stays on the CPU path.
@@ -171,11 +183,15 @@ pub fn register_committee(keys: &[[u8; 32]]) -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut valid = vec![0u32; (keys.len() + 31) / 32];
     let rc = unsafe { hs_committee_register(c, keys.as_ptr() as *const u8, keys.len(), valid.as_mut_ptr()) };
-    if rc != HS_OK { KEYS.lock().unwrap().clear(); return Err(GpuError::Engine(last_error(c))); }
+    if rc != HS_OK {
+        KEYS.lock().unwrap().clear();
+        *STAGED.lock().unwrap() = None;  // past its argument checks, a registration discards the engine's stage even when it fails
+        return Err(GpuError::Engine(last_error(c)));
+    }
     let mut map = KEYS.lock().unwrap();
     *map = keys.iter().map(|k| Some(*k)).collect();
     scrub::set_map(c, &map)?;
-    *STAGED.lock().unwrap() = None;  // a registration discards a staged change
+    *STAGED.lock().unwrap() = None;  // a registration discards a staged change or registration
     let bad: Vec<usize> = (0..keys.len()).filter(|i| valid[i / 32] >> (i % 32) & 1 == 0).collect();
     if bad.is_empty() { Ok(()) } else { Err(GpuError::InvalidKeys(bad)) }
 }
@@ -243,7 +259,7 @@ pub fn update_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>
     let mut keys = KEYS.lock().unwrap();  // held across the update and its audit: the map and the engine change together
     let rc = unsafe { hs_committee_update(c, add.as_ptr() as *const u8, add.len(), remove_idx.as_ptr(), remove_idx.len(), out.as_mut_ptr()) };
     if rc != HS_OK { return Err(GpuError::Engine(last_error(c))); }
-    *STAGED.lock().unwrap() = None;  // an update discards a staged change
+    *STAGED.lock().unwrap() = None;  // an update discards a staged change or registration
     out.truncate(add.len());
     for &i in remove_idx { keys[i as usize] = None; }
     for (k, &i) in add.iter().zip(out.iter()) {
@@ -280,28 +296,38 @@ pub fn stage_committee(add: &[[u8; 32]], remove_idx: &[u32]) -> Result<Vec<u32>,
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut staged = STAGED.lock().unwrap();
     let idx = stage_on(c, add, remove_idx)?;
-    *staged = Some(Staged { add: add.to_vec(), idx: idx.clone(), remove: remove_idx.to_vec() });
+    *staged = Some(Staged::Change { add: add.to_vec(), idx: idx.clone(), remove: remove_idx.to_vec() });
     Ok(idx)
 }
 /// Switches the staged committee in at the epoch boundary (hs_committee_commit: no table is built), applies the change to the node's
-/// map as `update_committee` would (additions, then removals) and audits the tables against it.
+/// map as `update_committee` would (additions, then removals) and audits the tables against it.  A staged registration is committed by
+/// `stage_register::commit_registration` instead.  If the engine's commit fails, the stage stays recorded: discard it.
 pub fn commit_committee() -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut keys = KEYS.lock().unwrap();  // held across the commit and its audit: the map and the engine change together
-    let st = STAGED.lock().unwrap().take().ok_or_else(|| GpuError::Engine("commit_committee: nothing staged".into()))?;
+    let mut staged = STAGED.lock().unwrap();
+    let (add, idx, remove) = match staged.as_ref() {
+        Some(Staged::Change { add, idx, remove }) => (add.clone(), idx.clone(), remove.clone()),
+        Some(Staged::Registration(_)) => return Err(GpuError::Engine("commit_committee: a registration is staged (commit_registration)".into())),
+        None => return Err(GpuError::Engine("commit_committee: nothing staged".into())),
+    };
     commit_on(c)?;
-    for (k, &i) in st.add.iter().zip(st.idx.iter()) {
+    *staged = None;
+    for (k, &i) in add.iter().zip(idx.iter()) {
         if i as usize >= keys.len() { keys.resize(i as usize + 1, None); }
         keys[i as usize] = Some(*k);
     }
-    for &i in &st.remove { keys[i as usize] = None; }
+    for &i in &remove { keys[i as usize] = None; }
     audit_tables(&keys)?;
     scrub::set_map(c, &keys)
 }
-/// Drops a staged committee change (hs_committee_discard).
+/// Drops a staged committee change (hs_committee_discard).  A staged registration is dropped by `stage_register::discard_registration`.
 pub fn discard_committee() -> Result<(), GpuError> {
     let c = ctx().ok_or(GpuError::Unavailable)?;
     let mut staged = STAGED.lock().unwrap();
+    if let Some(Staged::Registration(_)) = *staged {
+        return Err(GpuError::Engine("discard_committee: a registration is staged (discard_registration)".into()));
+    }
     discard_on(c)?;
     *staged = None;
     Ok(())
